@@ -32,6 +32,15 @@ extern "C" {
 #define UALM_ESTATE (-3)    /* call order (no map / no params / nothing uploaded) */
 #define UALM_ELIMIT (-4)    /* problem exceeds compiled limits (N, M, int_K) */
 
+/* ret_code of a problem whose solve was stopped early (no such exit exists in the reference; it is modelled on its earlyExit).
+ * stop = (max_evals > 0 && n_evals >= max_evals) || the lane's cancel request, tested after every accepted line search (where
+ * earlyExit tests k > 1000): L-BFGS then returns CANCELED, the ALM loop updates the duals and judges convergence as after any
+ * cancel, and ends with UALM_RET_STOPPED even when that test passes (res_h / res_g tell whether epsilon_con was met).  The ALM
+ * loop tests `stop` once more after judgeConvergence, so no inner solve starts after it holds.  A running line search is not
+ * interrupted: a problem stopped by the budget has max_evals <= n_evals <= max_evals + 64.  The outputs are those of the last
+ * evaluation, as for every exit.  A record with another ret_code never had a stop act on it: it is the unbudgeted result. */
+#define UALM_RET_STOPPED 3
+
 /* ---- parameters: the 21 alm_traj_opt/ * values (alm_traj_opt.cpp:7-27) + uneven_map/gravity ---- */
 typedef struct {
     double rho_T, rho_ter, max_vel, max_acc_lon, max_acc_lat, max_kap, min_cxi, max_sig;
@@ -60,9 +69,10 @@ void ualm_map_geometry(double map_size_x, double map_size_y, double xy_resolutio
 /* ---- per-problem result record (what the reference prints / returns: alm_traj_opt.cpp:176,252,267,272-273;
  *      alm_traj_opt.h:142) ---- */
 typedef struct {
-    int32_t ret_code;        /* 0 converged / 1 L-BFGS hard error / 2 ALM max_iter (the reference's codes); UALM_ELIMIT (-4): this
-                                problem exceeds the compiled limits (N <= 64, M <= 128) and was not solved -- the rest of its
-                                batch is unaffected */
+    int32_t ret_code;        /* 0 converged / 1 L-BFGS hard error / 2 ALM max_iter (the reference's codes); UALM_RET_STOPPED (3):
+                                the evaluation budget (ualm_set_budget) or a deadline (ualm_wait_batch_for) stopped it, see below;
+                                UALM_ELIMIT (-4): this problem exceeds the compiled limits (N <= 64, M <= 128) and was not solved --
+                                the rest of its batch is unaffected */
     int32_t outer_iters;
     int32_t n_evals;         /* cost+gradient evaluations */
     int32_t n_lbfgs_iters;   /* accepted line searches */
@@ -135,6 +145,14 @@ int ualm_select_lane(ualm_ctx_t *ctx, int lane);
 int ualm_submit_batch(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
                       const double *inner_xy, const double *inner_yaw, int depth, int *ticket);
 int ualm_wait_batch(ualm_ctx_t *ctx, int ticket, ualm_result_t *results, double *c_xy, double *c_yaw);
+/* ualm_wait_batch with a deadline: if the batch is not complete timeout_ms after the call, the lane's cancel request is set (the
+ * problems still running stop at their next stop test with UALM_RET_STOPPED), the batch drains and complete records come back.
+ * The request ends with the batch: the next batch on the lane starts without one. */
+int ualm_wait_batch_for(ualm_ctx_t *ctx, int ticket, double timeout_ms, ualm_result_t *results, double *c_xy, double *c_yaw);
+/* Evaluation budget per problem for the solves launched afterwards by every solving entry point (ualm_solve_batch,
+ * ualm_solve_resident, ualm_submit_batch, ualm_solve_batch_multi through each context): max_evals = 0 (the default) is none,
+ * negative values are UALM_EINVAL.  Refused (UALM_ESTATE) while a submitted batch is in flight. */
+int ualm_set_budget(ualm_ctx_t *ctx, int32_t max_evals);
 int ualm_mark_begin(ualm_ctx_t *ctx);
 int ualm_mark_end(ualm_ctx_t *ctx, float *ms);
 

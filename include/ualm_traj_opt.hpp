@@ -149,6 +149,8 @@ public:
 
     // ALMTrajOpt::init(nh): the caller fills `params` from its rosparam server, then calls init()
     void init() { check(ualm_set_params(ctx_, &params), "ualm_set_params"); }
+    // evaluation budget per problem of the following solves (0 = none); a stopped problem returns UALM_RET_STOPPED (ualm.h)
+    void setBudget(int max_evals) { check(ualm_set_budget(ctx_, max_evals), "ualm_set_budget"); }
 
     // ALMTrajOpt::setEnvironment(UnevenMap::Ptr): the map grid (UnevenMap::map_buffer is private in the reference,
     // uneven_map.h:91, so the maintainer-side binding passes geometry + a float4 view of the cells; INTEGRATION.md)
@@ -204,6 +206,11 @@ public:
         return ticket;
     }
     void waitBatch(int ticket, ualm_result_t *results, double *c_xy, double *c_yaw) { check(ualm_wait_batch(ctx_, ticket, results, c_xy, c_yaw), "ualm_wait_batch"); }
+    // the same with a deadline: after timeout_ms the problems still running are stopped (UALM_RET_STOPPED) and the batch drains
+    void waitBatchFor(int ticket, double timeout_ms, ualm_result_t *results, double *c_xy, double *c_yaw)
+    {
+        check(ualm_wait_batch_for(ctx_, ticket, timeout_ms, results, c_xy, c_yaw), "ualm_wait_batch_for");
+    }
 
     // What the MPC receives and tracks, for the batch solved last on the selected lane (ualm_mpc_export_batch): the SE2Traj message
     // arrays of PlanManager (plan_manager.cpp:151-185), the MPC side's own MINCO over them (traj_anal.hpp:125-181) and the largest

@@ -11,6 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libualm.so")
 
 UALM_OK, UALM_ENOCUDA, UALM_EINVAL, UALM_ESTATE, UALM_ELIMIT = 0, -1, -2, -3, -4
+UALM_RET_STOPPED = 3   # ret_code of a problem stopped by the evaluation budget or a deadline (include/ualm.h)
 
 
 class Params(C.Structure):
@@ -116,11 +117,14 @@ def lib():
         L.ualm_select_lane.argtypes = [vp, C.c_int]
         L.ualm_submit_batch.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, dp, C.c_int, C.POINTER(C.c_int)]
         L.ualm_wait_batch.argtypes = [vp, C.c_int, C.POINTER(Result), dp, dp]
+        L.ualm_wait_batch_for.argtypes = [vp, C.c_int, C.c_double, C.POINTER(Result), dp, dp]
+        L.ualm_set_budget.argtypes = [vp, C.c_int32]
         L.ualm_mark_begin.argtypes = [vp]
         L.ualm_mark_end.argtypes = [vp, C.POINTER(C.c_float)]
         L.ualm_solve_batch_multi.argtypes = [C.POINTER(vp), C.c_int, C.c_int, ip, ip, dp, dp, dp, dp, C.POINTER(Result), dp, dp]
         L.ualm_pack_records_device_async.argtypes = [vp, vp, C.c_int]
         for name in ("ualm_reset_stream", "ualm_set_map_f64", "ualm_max_lanes", "ualm_select_lane", "ualm_submit_batch", "ualm_wait_batch",
+                     "ualm_wait_batch_for", "ualm_set_budget",
                      "ualm_mark_begin", "ualm_mark_end", "ualm_solve_batch_multi", "ualm_pack_records_device_async"):
             getattr(L, name).restype = C.c_int
         for name in ("ualm_create", "ualm_destroy", "ualm_set_params", "ualm_set_map", "ualm_solve_batch",

@@ -58,6 +58,12 @@ class BatchALMTrajOpt:
         _check(self.L.ualm_set_params(self.h, C.byref(self.params)))
         return self
 
+    def set_budget(self, max_evals):
+        """ualm_set_budget: evaluation budget per problem of the solves launched afterwards (0 = none).  A problem it stops ends
+        with ret_code UALM_RET_STOPPED (3) after max_evals..max_evals + 64 evaluations."""
+        _check(self.L.ualm_set_budget(self.h, int(max_evals)))
+        return self
+
     def set_stream(self, cuda_stream_ptr):
         _check(self.L.ualm_set_stream(self.h, C.c_void_p(cuda_stream_ptr)))
         return self
@@ -106,13 +112,18 @@ class BatchALMTrajOpt:
         self._tickets[t.value] = (pb, host)
         return t.value
 
-    def wait(self, ticket, out=None):
-        """ualm_wait_batch: (results, c_xy, c_yaw) of the ticket's batch; `out` = optional preallocated (res, cxy, cyaw)."""
+    def wait(self, ticket, out=None, timeout_ms=None):
+        """ualm_wait_batch: (results, c_xy, c_yaw) of the ticket's batch; `out` = optional preallocated (res, cxy, cyaw).
+        timeout_ms (ualm_wait_batch_for): if the batch is not complete by then, its running problems are stopped (ret_code
+        UALM_RET_STOPPED) and the complete records of the drained batch come back."""
         pb, _ = self._tickets.pop(ticket)
         if out is None:
             out = ((Result * pb.B)(), np.zeros(int(12 * pb.N.astype(np.int64).sum())), np.zeros(int(6 * pb.M.astype(np.int64).sum())))
         res, cxy, cyaw = out
-        _check(self.L.ualm_wait_batch(self.h, int(ticket), res, _p(cxy), _p(cyaw)))
+        if timeout_ms is None:
+            _check(self.L.ualm_wait_batch(self.h, int(ticket), res, _p(cxy), _p(cyaw)))
+        else:
+            _check(self.L.ualm_wait_batch_for(self.h, int(ticket), float(timeout_ms), res, _p(cxy), _p(cyaw)))
         return res, cxy, cyaw
 
     # ---- three-step path -------------------------------------------------------------

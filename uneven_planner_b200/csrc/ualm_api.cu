@@ -7,12 +7,14 @@
 #include "ualm_tp_host.h"
 
 #include <algorithm>
+#include <chrono>
 #include <cstdio>
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
 #include <numeric>
 #include <string>
+#include <thread>
 #include <vector>
 
 using namespace ualm;
@@ -77,8 +79,14 @@ struct Lane {
     int last_launches = 0;
     SmemLayout L;
     size_t smem_bytes = 0;
+    // cancel word of the lane's solves (ualm_wait_batch_for), in device memory: the host raises it by a copy on the context's
+    // cancel stream while the kernels run.  (A word in mapped pinned host memory, read over PCIe at every stop test, made the bench
+    // step 5 % slower on an H100 80GB HBM3 at a 400 W power limit.)
+    int *d_cancel = nullptr;
     void release()
     {
+        if (d_cancel) cudaFree(d_cancel);
+        d_cancel = nullptr;
         d_desc.release(); d_order.release(); d_wdesc.release();
         DevBuf<double> *bufs[] = {&d_x0, &d_x, &d_lambda, &d_mu, &d_scale_cx, &d_hx, &d_gx, &d_lm_s, &d_lm_y, &d_lm_aux, &d_fac,
                                   &d_scr, &d_ws, &d_cxy, &d_cyaw, &d_f, &d_grad, &d_sfx};
@@ -111,6 +119,10 @@ struct ualm_ctx {
     // pipeline timing (ualm_mark_begin / ualm_mark_end): events on the lanes' own streams, joined on `join`
     cudaStream_t join = nullptr;
     cudaEvent_t evA = nullptr, evB = nullptr;
+    // deadline (ualm_wait_batch_for): {0, 1} in pinned memory, copied into a lane's cancel word on the lane's stream before a launch
+    // (clear) or on `cancel` while it runs (raise); copies go through the copy engines, so they do not wait for free SMs
+    int *h_flags = nullptr;
+    cudaStream_t cancel = nullptr;
 };
 
 static int lane_make(ualm_ctx *c, Lane &l)
@@ -123,6 +135,8 @@ static int lane_make(ualm_ctx *c, Lane &l)
     for (int q = 0; q < Lane::NAUX + 1; q++) CK(cudaEventCreateWithFlags(&l.evs[q], cudaEventDisableTiming));
     CK(cudaEventCreate(&l.ev0));
     CK(cudaEventCreate(&l.ev1));
+    CK(cudaMalloc(&l.d_cancel, sizeof(int)));
+    CK(cudaMemset(l.d_cancel, 0, sizeof(int)));
     (void)c;
     return UALM_OK;
 }
@@ -164,6 +178,9 @@ extern "C" int ualm_create(ualm_ctx_t **out, int device, int precision)
     int rc = lane_make(c, c->lanes[0]);
     if (rc == UALM_OK) {
         cudaError_t e1 = cudaStreamCreateWithFlags(&c->join, cudaStreamNonBlocking);
+        if (e1 == cudaSuccess) e1 = cudaStreamCreateWithFlags(&c->cancel, cudaStreamNonBlocking);
+        if (e1 == cudaSuccess) e1 = cudaHostAlloc(&c->h_flags, 2 * sizeof(int), cudaHostAllocDefault);
+        if (e1 == cudaSuccess) { c->h_flags[0] = 0; c->h_flags[1] = 1; }
         if (e1 == cudaSuccess) e1 = cudaEventCreate(&c->evA);
         if (e1 == cudaSuccess) e1 = cudaEventCreate(&c->evB);
         if (e1 != cudaSuccess) rc = fail(UALM_ENOCUDA, std::string("context streams/events: ") + cudaGetErrorString(e1));
@@ -182,6 +199,8 @@ extern "C" int ualm_destroy(ualm_ctx_t *c)
     c->cells.release(); c->cells64.release();
     for (auto &l : c->lanes) l.release();
     if (c->join) cudaStreamDestroy(c->join);
+    if (c->cancel) cudaStreamDestroy(c->cancel);
+    if (c->h_flags) cudaFreeHost(c->h_flags);
     if (c->evA) cudaEventDestroy(c->evA);
     if (c->evB) cudaEventDestroy(c->evB);
     delete c;
@@ -536,6 +555,9 @@ extern "C" int ualm_solve_resident(ualm_ctx_t *c)
     if (!c->have_map || !c->have_params || !l->have_batch) return fail(UALM_ESTATE, "set_params, set_map and upload must precede solve");
     CK(cudaSetDevice(c->device));
     l->last_launches = 0;
+    CK(cudaMemcpyAsync(l->d_cancel, &c->h_flags[0], sizeof(int), cudaMemcpyHostToDevice, l->stream));   // no request carries over
+    DevParams dp = c->dp;
+    dp.cancel = l->d_cancel;
     CK(cudaEventRecord(l->ev0, l->stream));
     if (l->n_active > 0) {
         // the classes run concurrently: class 0 on the lane stream, the others on auxiliary streams
@@ -550,7 +572,7 @@ extern "C" int ualm_solve_resident(ualm_ctx_t *c)
             BatchPtrs bp = batch_ptrs(c);
             bp.wdesc = l->d_wdesc.p + cl.wd_off;
             bp.n_leader_slots = 4 / cl.G;
-            solve_kernel<<<cl.n_ctas, UALM_THREADS * UALM_WPB, cl.smem, st>>>(bp, c->dp, c->dm, cl.L);
+            solve_kernel<<<cl.n_ctas, UALM_THREADS * UALM_WPB, cl.smem, st>>>(bp, dp, c->dm, cl.L);
             CK(cudaGetLastError());
             l->last_launches++;
             if (ci > 0) { CK(cudaEventRecord(l->evs[ai], st)); CK(cudaStreamWaitEvent(l->stream, l->evs[ai], 0)); }
@@ -676,6 +698,46 @@ extern "C" int ualm_wait_batch(ualm_ctx_t *c, int ticket, ualm_result_t *results
     c->lanes[ticket].in_flight = false;
     c->cur = keep; c->b = &c->lanes[keep];
     return rc;
+}
+
+// deadline-bounded wait: poll the lane's completion until the timeout, then raise its cancel word and wait for the batch to drain
+// (every problem still running stops at its next stop test, include/ualm.h UALM_RET_STOPPED)
+extern "C" int ualm_wait_batch_for(ualm_ctx_t *c, int ticket, double timeout_ms, ualm_result_t *results, double *c_xy, double *c_yaw)
+{
+    if (!c || ticket < 0 || ticket >= UALM_MAX_LANES) return fail(UALM_EINVAL, "bad ticket");
+    if (!(timeout_ms >= 0.0)) return fail(UALM_EINVAL, "timeout_ms must be >= 0");
+    if (c->tp) {
+        if (!ualm_tp::tp_lane_in_flight(c->tp, ticket)) return fail(UALM_ESTATE, "ticket is not in flight");
+        std::string em;
+        const int rc = ualm_tp::tp_collect(c->tp, ticket, &em, timeout_ms);
+        if (rc) return fail(rc, em);
+        TP_CALL(ualm_tp::tp_download(c->tp, ticket, results, c_xy, c_yaw, err));
+    }
+    Lane &l = c->lanes[ticket];
+    if (!l.in_flight) return fail(UALM_ESTATE, "ticket is not in flight");
+    CK(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    while (true) {
+        const cudaError_t q = cudaEventQuery(l.ev1);
+        if (q == cudaSuccess) break;
+        if (q != cudaErrorNotReady) CK(q);
+        if (std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() >= timeout_ms) {
+            CK(cudaMemcpyAsync(l.d_cancel, &c->h_flags[1], sizeof(int), cudaMemcpyHostToDevice, c->cancel));
+            break;
+        }
+        std::this_thread::yield();
+    }
+    return ualm_wait_batch(c, ticket, results, c_xy, c_yaw);
+}
+
+extern "C" int ualm_set_budget(ualm_ctx_t *c, int32_t max_evals)
+{
+    if (!c) return fail(UALM_EINVAL, "null ctx");
+    if (max_evals < 0) return fail(UALM_EINVAL, "max_evals must be >= 0 (0 = no budget)");
+    if (c->tp) TP_CALL(ualm_tp::tp_set_budget(c->tp, max_evals, err));
+    if (int rc = lanes_idle(c, "ualm_set_budget")) return rc;
+    c->dp.max_evals = max_evals;
+    return UALM_OK;
 }
 
 // ---- one host process, several GPUs: contexts on different devices (same params and map set on each), the batch dealt over

@@ -66,6 +66,10 @@ struct DevParams {
     int inner_max_iter;
     int mem_size, past, int_K;
     R gravity;
+    // stop predicate of the solve (ualm_set_budget / ualm_wait_batch_for): evaluation budget (0 = none) and the lane's cancel
+    // word in device memory (null = none), set per launch
+    int max_evals;
+    const volatile int *cancel;
 };
 
 struct DevMap {
@@ -166,7 +170,8 @@ __host__ __device__ inline SmemLayout make_layout(int Nmax, int Mmax, int nmax, 
 // scalar slots in sm[L.sc + ...]
 enum {
     SC_TX1 = 0, SC_TX2, SC_TX3, SC_TX4, SC_TX5, SC_TY1, SC_TY2, SC_TY3, SC_TY4, SC_TY5,
-    SC_SCALE_FX, SC_RHO, SC_F, SC_JERK, SC_CONSTR, SC_TAUCOST, SC_JERKRAW, SC_RTY, SC_CMD
+    SC_SCALE_FX, SC_RHO, SC_F, SC_JERK, SC_CONSTR, SC_TAUCOST, SC_JERKRAW, SC_RTY, SC_CMD,
+    SC_STOPPED   // != 0: the stop predicate fired inside the inner solve that just ended
 };
 
 // Handles to shared memory: a 32-bit address in the shared state space.  Accesses through them are explicit ld.shared /
@@ -1544,6 +1549,16 @@ __device__ UALM_NOINLINE R lane_absmax(SPtr a, int n, int lane)
 
 struct LbfgsOut { int ret; R f; int iters; int max_bound; int sum_bound; };
 
+// stop = (max_evals > 0 && n_evals >= max_evals) || cancel requested, evaluated where earlyExit is (and by the ALM loop after
+// judgeConvergence).  Lane 0 alone reads the cancel word; the broadcast keeps the decision warp-uniform.
+__device__ __forceinline__ bool stop_requested(const Traj &t, const DevParams &p, int lane)
+{
+    int c = 0;
+    if (p.cancel && lane == 0) c = *p.cancel;
+    c = __shfl_sync(0xffffffffu, c, 0);
+    return (p.max_evals > 0 && t.n_evals >= p.max_evals) || c != 0;
+}
+
 // lbfgs_optimize + line_search_lewisoverton (lbfgs.hpp:276-389, 439-722).  All 32 lanes follow the same control flow:
 // every scalar the decisions depend on is the result of a warp-uniform reduction or a shared-memory scalar.
 __device__ UALM_NOINLINE LbfgsOut lbfgs_optimize(Traj &t, const DevMap &map, const DevParams &p, int lane)
@@ -1618,7 +1633,11 @@ __device__ UALM_NOINLINE LbfgsOut lbfgs_optimize(Traj &t, const DevMap &map, con
             break;
         }
         out.iters++;
-        if (k > 1000) { ret = LBFGS_CANCELED; break; } // earlyExit alm_traj_opt.cpp:1016 (k > 1e3)
+        {
+            const bool stop = stop_requested(t, p, lane);
+            if (stop && lane == 0) t.sc[SC_STOPPED] = 1.0;
+            if (k > 1000 || stop) { ret = LBFGS_CANCELED; break; } // earlyExit alm_traj_opt.cpp:1016 (k > 1e3)
+        }
         {
             const R gn = lane_absmax(t.g, n, lane), xn = lane_absmax(t.x, n, lane);
             if (gn / fmax(1.0, xn) < p.g_epsilon) { ret = LBFGS_CONVERGENCE; break; }
@@ -2024,6 +2043,17 @@ __device__ UALM_NOINLINE void traj_setup(Traj &t, const BatchPtrs &bp, const Dev
     if (ln == 0) { *t.plast = clock64(); s_prof[PF_TOTAL] = -clock64(); }
 }
 
+// exit of the ALM loop after judgeConvergence (include/ualm.h, UALM_RET_STOPPED): a stop that fired inside the inner solve that
+// just ended, else convergence, else a stop that holds now; -1 = go on (to the max_iter test).  Not inlined: inside solve_kernel
+// (255 registers) the test costs a spill
+__device__ UALM_NOINLINE int alm_exit(Traj &t, const DevParams &p, int lane, bool converged)
+{
+    if ((R)t.sc[SC_STOPPED] != 0.0) return UALM_RET_STOPPED;
+    if (converged) return 0;
+    if (stop_requested(t, p, lane)) return UALM_RET_STOPPED;
+    return -1;
+}
+
 // =============================================================================================
 // kernels (CTA = 4 warp slots; solve_kernel: warp groups per trajectory, the test kernels: one warp per trajectory)
 // =============================================================================================
@@ -2087,7 +2117,7 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) solve_kernel(const __
     for (int q = lane; q < 6 * S; q += 32) { t.mu[q] = 0.0; t.gx[q] = 0.0; }
     for (int q = lane; q < 7 * S; q += 32) t.scale_cx[q] = 1.0;
     for (int q = lane; q < n; q += 32) t.x[q] = bp.x0[t.pd->off_x + q];
-    if (lane == 0) { t.sc[SC_SCALE_FX] = 1.0; t.sc[SC_RHO] = p.rho; }
+    if (lane == 0) { t.sc[SC_SCALE_FX] = 1.0; t.sc[SC_RHO] = p.rho; t.sc[SC_STOPPED] = 0.0; }
     UALM_SYNC();
     if (p.use_scaling) init_scaling(t, map, p, lane);
     prof_mark(t, lane, PF_SCALING);
@@ -2129,7 +2159,10 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) solve_kernel(const __
         if (lane == 0) t.sc[SC_RHO] = rho_new;
         UALM_SYNC();
         prof_mark(t, lane, PF_DUAL);
-        if (fmax(rh, rg) < p.epsilon_con) break;
+        {
+            const int e = alm_exit(t, p, lane, fmax(rh, rg) < p.epsilon_con);
+            if (e >= 0) { ret_code = e; break; }
+        }
         if ((R)(++iter) > p.max_iter) { ret_code = 2; break; }
     }
     int join = 0;

@@ -5,6 +5,7 @@
 #include "ualm_tp_host.h"
 
 #include <algorithm>
+#include <chrono>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -86,7 +87,7 @@ struct TpEngine {
     int sg = 1;                           // subgroups per batch in use (UALM_TP_SUBGROUPS, <= TP_SUBGROUPS); 1 measured best: the batches in flight already are the groups
     int Nmax_live = 1, Mmax_live = 1;
     Buf<TpState> st;
-    Buf<int> active, n_active, remaining;
+    Buf<int> active, n_active, remaining, cancel;
     Buf<double> vec, cd, gw, kb_cost, lm_ys, lm_alpha, wf, wt;
     Buf<unsigned char> cr, gdc, gdt, dual, hs, hy, wway;
     Buf<long long> wf_off, wway_off, kprof;
@@ -169,8 +170,12 @@ int tp_create(TpEngine **out, int device, int precision, std::string *err)
             if (err) *err = "group stream creation failed";
             return failed(UALM_ENOCUDA);
         }
-    if (e->remaining.ensure(TP_MAX_TICKETS) != cudaSuccess || e->n_active.ensure(TP_NGROUPS) != cudaSuccess) { if (err) *err = "allocation failed"; return failed(UALM_ENOCUDA); }
+    if (e->remaining.ensure(TP_MAX_TICKETS) != cudaSuccess || e->n_active.ensure(TP_NGROUPS) != cudaSuccess || e->cancel.ensure(TP_LANES) != cudaSuccess) {
+        if (err) *err = "allocation failed";
+        return failed(UALM_ENOCUDA);
+    }
     cudaMemsetAsync(e->remaining.p, 0, sizeof(int) * TP_MAX_TICKETS, e->stream);
+    cudaMemsetAsync(e->cancel.p, 0, sizeof(int) * TP_LANES, e->stream);
     cudaMemsetAsync(e->n_active.p, 0, sizeof(int) * TP_NGROUPS, e->stream);
     int rc = build_tables(e, err);
     if (rc) return failed(rc);
@@ -209,7 +214,7 @@ void tp_destroy(TpEngine *e)
         if (l.ev0) cudaEventDestroy(l.ev0);
         if (l.ev1) cudaEventDestroy(l.ev1);
     }
-    e->cells.release(); e->st.release(); e->active.release(); e->n_active.release(); e->remaining.release(); e->vec.release(); e->cd.release(); e->gw.release();
+    e->cells.release(); e->st.release(); e->active.release(); e->n_active.release(); e->remaining.release(); e->cancel.release(); e->vec.release(); e->cd.release(); e->gw.release();
     e->kb_cost.release(); e->lm_ys.release(); e->lm_alpha.release(); e->cr.release(); e->gdc.release(); e->gdt.release(); e->dual.release();
     e->hs.release(); e->hy.release(); e->wway.release(); e->wf.release(); e->wt.release(); e->wf_off.release(); e->wway_off.release();
     if (e->h_remaining) cudaFreeHost(e->h_remaining);
@@ -243,6 +248,13 @@ int tp_set_params(TpEngine *e, const ualm_params_t *p, std::string *err)
     e->capacity = 0; e->free_slots.clear(); e->live = 0;
     for (int g = 0; g < TP_NGROUPS; g++) { e->glive[g] = 0; e->gscale[g] = 0; e->gcompact[g] = false; }
     for (auto &l : e->lanes) { l.collected = false; }
+    return UALM_OK;
+}
+
+int tp_set_budget(TpEngine *e, int max_evals, std::string *err)
+{
+    if (any_in_flight(e)) { if (err) *err = "ualm_set_budget while a batch is in flight"; return UALM_ESTATE; }
+    e->p.max_evals = max_evals;
     return UALM_OK;
 }
 
@@ -296,7 +308,7 @@ static int pool_alloc(TpEngine *e, int cap, std::string *err)
     TCK(cudaStreamSynchronize(e->stream));
     TpPool &E = e->E;
     E.capacity = cap; E.m = m; E.K = K; E.Smax = (int)Smax; E.use_tma = e->use_tma;
-    E.st = e->st.p; E.active = e->active.p; E.n_active = e->n_active.p; E.remaining = e->remaining.p;
+    E.st = e->st.p; E.active = e->active.p; E.n_active = e->n_active.p; E.remaining = e->remaining.p; E.cancel = e->cancel.p;
     E.vec = e->vec.p; E.cd = e->cd.p; E.gw = e->gw.p; E.cr = e->f32() ? (void *)e->cr.p : (void *)e->cd.p; E.gdc = e->gdc.p; E.gdt = e->gdt.p;
     E.kb_cost = e->kb_cost.p; E.dual = e->dual.p; E.hs = e->hs.p; E.hy = e->hy.p; E.lm_ys = e->lm_ys.p; E.lm_alpha = e->lm_alpha.p;
     E.wf = e->wf.p; E.wf_off = e->wf_off.p; E.wt = e->wt.p; E.wway = e->wway.p; E.wway_off = e->wway_off.p;
@@ -420,6 +432,7 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, std::s
     TCK(cudaEventRecord(l.ev0, e->stream));
     l.launches = 0;
     TCK(cudaMemcpyAsync(l.d_res.p, res0.data(), sizeof(ualm_result_t) * l.B, cudaMemcpyHostToDevice, e->stream));
+    TCK(cudaMemsetAsync(e->cancel.p + lane, 0, sizeof(int), e->stream));      // a cancel request of the lane's previous batch does not carry over
     if (BA < l.B) {
         TCK(cudaMemsetAsync(l.d_cxy.p, 0, sizeof(double) * l.tot_cxy, e->stream));
         TCK(cudaMemsetAsync(l.d_cyaw.p, 0, sizeof(double) * l.tot_cyaw, e->stream));
@@ -537,13 +550,15 @@ static int run_rounds(TpEngine *e, int nr, std::string *err)
     return UALM_OK;
 }
 
-int tp_collect(TpEngine *e, int lane, std::string *err)
+int tp_collect(TpEngine *e, int lane, std::string *err, double timeout_ms)
 {
     if (lane < 0 || lane >= TP_LANES) { if (err) *err = "lane out of range"; return UALM_EINVAL; }
     TpLane &l = e->lanes[lane];
     if (l.collected) return UALM_OK;
     if (!l.in_flight) { if (err) *err = "nothing in flight on this lane"; return UALM_ESTATE; }
     TCK(cudaSetDevice(e->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    bool cancelled = false;
     long long guard = 0;
     while (true) {
         // the lane's own groups are the pace setters: wait for what was queued for them, then look at the lane's counter
@@ -551,6 +566,12 @@ int tp_collect(TpEngine *e, int lane, std::string *err)
         TCK(cudaMemcpyAsync(e->h_remaining, e->remaining.p, sizeof(int) * TP_LANES, cudaMemcpyDeviceToHost, e->stream));
         TCK(cudaStreamSynchronize(e->stream));
         if (e->h_remaining[lane] <= 0) break;
+        if (timeout_ms >= 0.0 && !cancelled && std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() >= timeout_ms) {
+            const int one = 1;      // read by ka_kernel at the stop tests of the rounds queued from now on
+            TCK(cudaMemcpyAsync(e->cancel.p + lane, &one, sizeof(int), cudaMemcpyHostToDevice, e->stream));
+            TCK(cudaStreamSynchronize(e->stream));
+            cancelled = true;
+        }
         int rc = run_rounds(e, e->chunk, err);        // every live group advances, not only this lane's
         if (rc) return rc;
         if ((guard += e->chunk) > 400000) { if (err) *err = "throughput engine: a trajectory did not terminate"; return UALM_ENOCUDA; }

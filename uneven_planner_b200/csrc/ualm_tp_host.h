@@ -20,7 +20,10 @@ int tp_set_map(TpEngine *e, const ualm_map_geom_t *g, const float *cells, std::s
 int tp_upload(TpEngine *e, int lane, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time, const double *inner_xy,
               const double *inner_yaw, std::string *err);
 int tp_admit(TpEngine *e, int lane, std::string *err);                       // asynchronous
-int tp_collect(TpEngine *e, int lane, std::string *err);                     // blocks: rounds until the lane's batch is done
+// blocks: rounds until the lane's batch is done.  timeout_ms >= 0: once that much time has passed since the call, the lane's
+// cancel word is raised before the next rounds (its trajectories stop at their next stop test)
+int tp_collect(TpEngine *e, int lane, std::string *err, double timeout_ms = -1.0);
+int tp_set_budget(TpEngine *e, int max_evals, std::string *err);              // evaluation budget of the solves admitted afterwards
 int tp_download(TpEngine *e, int lane, ualm_result_t *results, double *c_xy, double *c_yaw, std::string *err);
 int tp_pack_records(TpEngine *e, int lane, double *d_records, int stride, std::string *err);
 bool tp_lane_in_flight(TpEngine *e, int lane);

@@ -78,6 +78,7 @@ struct TpParams {
     double rho, beta, gamma, epsilon_con, max_iter, g_epsilon, min_step, delta;
     int inner_max_iter, mem_size, past, int_K;
     double gravity;
+    int max_evals;          // evaluation budget per problem (ualm_set_budget), 0 = none
 };
 
 struct TpMap {
@@ -105,6 +106,7 @@ struct TpPool {
     int *active;            // [TP_NGROUPS][capacity] active slot list per group
     int *n_active;          // [TP_NGROUPS]
     int *remaining;         // per ticket: trajectories not yet done
+    const int *cancel;      // per ticket: cancel request (ualm_wait_batch_for), raised by the host between rounds
     double *vec;            // [cap][5][TP_NVAR]  x | g | xp | gp | d
     double *cd;             // [cap][TP_CSTRIDE]  coefficients of the last forward solve (double)
     double *gw;             // [cap][TP_CSTRIDE]  z = dc/dT(piece) of the last forward solve (same layout as cd)
@@ -544,6 +546,32 @@ __device__ int ls_begin(const SlotView &v, int lane)
     return 0;
 }
 
+// the stop predicate of include/ualm.h (UALM_RET_STOPPED), tested where earlyExit is and by the ALM loop after judgeConvergence
+__device__ __forceinline__ bool stop_requested(const TpPool &E, const TpParams &p, const TpState *st)
+{
+    return (p.max_evals > 0 && st->n_evals >= p.max_evals) || E.cancel[st->ticket] != 0;
+}
+
+// the stop test at the earlyExit point; a stop that fires is marked in ret_code for the ALM loop (alm_ends)
+__device__ __forceinline__ bool stop_fires(const TpPool &E, const TpParams &p, TpState *st, int lane)
+{
+    const bool s = stop_requested(E, p, st);
+    if (s && lane == 0) st->ret_code = UALM_RET_STOPPED;
+    return s;
+}
+
+// the ALM loop's exits after judgeConvergence failed (alm_traj_opt.cpp:262-267): the stop fired inside the inner solve that just
+// ended or holds now (UALM_RET_STOPPED), else ++iter > max_iter (2).  Not inlined: inside ka_kernel (128 registers) the stop test
+// costs a spill
+__device__ __noinline__ bool alm_ends(const TpPool &E, const TpParams &p, TpState *st, int lane)
+{
+    if (st->ret_code == UALM_RET_STOPPED || stop_requested(E, p, st)) { if (lane == 0) st->ret_code = UALM_RET_STOPPED; return true; }
+    const int iter = st->outer_iter + 1;
+    if (lane == 0) st->outer_iter = iter;
+    if ((double)iter > p.max_iter) { if (lane == 0) st->ret_code = 2; return true; }
+    return false;
+}
+
 // one ka step for a trajectory whose evaluation at v.x has just been finished: runs the optimizer's control flow up to the next
 // evaluation request (returns the new phase) or to the end of the solve (PH_DONE).  alm_traj_opt.cpp:234-271, lbfgs.hpp:439-722
 template <class R>
@@ -613,7 +641,7 @@ __device__ int advance(const TpPool &E, const TpParams &p, const SlotView &v, in
         } else {
             int k = st->k;
             if (lane == 0) st->iters_total++;
-            if (k > 1000) { lret = LB_CANCELED; ended = true; }        // earlyExit, alm_traj_opt.cpp:1016
+            if (stop_fires(E, p, st, lane) || k > 1000) { lret = LB_CANCELED; ended = true; }        // earlyExit, alm_traj_opt.cpp:1016
             if (!ended) {
                 const double gn = vabsmax(v.g, n, lane), xn = vabsmax(v.x, n, lane);
                 if (gn / fmax(1.0, xn) < p.g_epsilon) { lret = LB_CONVERGENCE; ended = true; }
@@ -760,12 +788,9 @@ __device__ int advance(const TpPool &E, const TpParams &p, const SlotView &v, in
             mg = fmax(mg, fabs(fmax(gq, -mq / rho_new)));
         }
         mh = warp_max(mh); mg = warp_max(mg);
-        int iter = st->outer_iter;
         if (lane == 0) { st->rho = rho_new; st->res_h = mh; st->res_g = mg; }
-        if (fmax(mh, mg) < p.epsilon_con) return PH_DONE;
-        ++iter;
-        if (lane == 0) st->outer_iter = iter;
-        if ((double)iter > p.max_iter) { if (lane == 0) st->ret_code = 2; return PH_DONE; }
+        if (fmax(mh, mg) < p.epsilon_con) return PH_DONE;         // a stop that fired in this inner solve keeps its mark in ret_code
+        if (alm_ends(E, p, st, lane)) return PH_DONE;
     }
     __syncwarp();
     return PH_REQ_FIRST;           // next lbfgs_optimize starts with an evaluation at the current x
