@@ -99,11 +99,21 @@ const char *ualm_last_error(void);
  * ualm_sync (or a stream-ordered consumer on the SAME stream) before touching its outputs. */
 int ualm_set_stream(ualm_ctx_t *ctx, void *cuda_stream);
 int ualm_reset_stream(ualm_ctx_t *ctx);
-/* ALMTrajOpt::init.  int_K, mem_size and past are baked into uploaded batches: a parameter change invalidates every resident
- * batch (upload again before the next solve / eval); it is refused while a submitted batch is in flight. */
+/* ---- environments ----
+ * An environment is one parameter set (ualm_set_params) plus one map grid (ualm_set_map / ualm_set_map_f64).  A context holds up
+ * to UALM_MAX_ENVS of them, and every problem of a batch names its own (the *_env entry points below; the entry points without
+ * the suffix put every problem in environment 0).  A problem's result is exactly what it is in a batch of its environment alone.
+ *   ualm_select_env(ctx, e): ualm_set_params / ualm_set_map / ualm_set_map_f64 bind environment e from now on (0 <= e <
+ *                            UALM_MAX_ENVS; environment 0 is selected at creation).  Each environment owns its grid. */
+#define UALM_MAX_ENVS 4
+int ualm_select_env(ualm_ctx_t *ctx, int env);
+/* ALMTrajOpt::init, for the selected environment.  int_K, mem_size and past are baked into uploaded batches: a parameter change
+ * (of any environment) invalidates every resident batch (upload again before the next solve / eval); it is refused while a
+ * submitted batch is in flight. */
 int ualm_set_params(ualm_ctx_t *ctx, const ualm_params_t *p);
-/* cells: host, [X][Y][Yaw][4] float {z, sigma, zbx, zby}, address x*Y*Yaw + y*Yaw + yaw (uneven_map.h:427-435).
- * One-time upload (replaces setEnvironment; the reference's map_buffer is private, uneven_map.h:91). */
+/* cells: host, [X][Y][Yaw][4] float {z, sigma, zbx, zby}, address x*Y*Yaw + y*Yaw + yaw (uneven_map.h:427-435), for the selected
+ * environment.  One-time upload (replaces setEnvironment; the reference's map_buffer is private, uneven_map.h:91).  Refused while
+ * a submitted batch is in flight. */
 int ualm_set_map(ualm_ctx_t *ctx, const ualm_map_geom_t *g, const float *cells);
 /* The reference's own grid: UnevenMap::map_buffer is RXS2 {double z, sigma; Vector2d zb} (uneven_map.h:36-64), i.e. 4 doubles
  * per cell in the same address order.  repack_to_float = 0 keeps the doubles on the device (82 MB for 200x200x64: bit parity
@@ -123,6 +133,17 @@ int ualm_solve_batch(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M,
  *   upload (H2D) -> solve_resident (kernels only, asynchronous on the context stream) -> download (D2H). */
 int ualm_upload(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *bnd,
                 const double *total_time, const double *inner_xy, const double *inner_yaw);
+/* The *_env forms take the arguments of their counterparts plus env[B], the environment of every problem (NULL = all 0; the
+ * counterparts are these with env = NULL).  An index outside [0, UALM_MAX_ENVS) is UALM_EINVAL, an environment without both
+ * parameters and a grid bound is UALM_ESTATE; nothing is touched on either error.  The budget (ualm_set_budget) and the deadline
+ * (ualm_wait_batch_for) act on every problem of a batch alike.  ualm_eval_batch, ualm_init_scaling_batch,
+ * ualm_feasibility_batch and ualm_mpc_export_batch use each problem's environment; ualm_time_penalty_kernel refuses a batch
+ * that mixes environments (UALM_EINVAL). */
+int ualm_upload_env(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
+                    const double *inner_xy, const double *inner_yaw, const int32_t *env);
+int ualm_solve_batch_env(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
+                         const double *inner_xy, const double *inner_yaw, const int32_t *env, ualm_result_t *results, double *c_xy,
+                         double *c_yaw);
 int ualm_solve_resident(ualm_ctx_t *ctx);
 int ualm_sync(ualm_ctx_t *ctx);
 int ualm_download(ualm_ctx_t *ctx, ualm_result_t *results, double *c_xy, double *c_yaw);
@@ -144,6 +165,8 @@ int ualm_max_lanes(void);
 int ualm_select_lane(ualm_ctx_t *ctx, int lane);
 int ualm_submit_batch(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
                       const double *inner_xy, const double *inner_yaw, int depth, int *ticket);
+int ualm_submit_batch_env(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
+                          const double *inner_xy, const double *inner_yaw, const int32_t *env, int depth, int *ticket);
 int ualm_wait_batch(ualm_ctx_t *ctx, int ticket, ualm_result_t *results, double *c_xy, double *c_yaw);
 /* ualm_wait_batch with a deadline: if the batch is not complete timeout_ms after the call, the lane's cancel request is set (the
  * problems still running stop at their next stop test with UALM_RET_STOPPED), the batch drains and complete records come back.
@@ -157,13 +180,16 @@ int ualm_mark_begin(ualm_ctx_t *ctx);
 int ualm_mark_end(ualm_ctx_t *ctx, float *ms);
 
 /* ---- several GPUs from one host process (SURVEY 8b item 4) ----
- * ctxs[r] lives on its own device with the same parameters and map bound.  The batch is dealt over the contexts (cost-sorted
+ * ctxs[r] lives on its own device with the same parameters and map bound (in every environment the batch uses).  The batch is dealt over the contexts (cost-sorted
  * snake), every device solves its shard concurrently, and the results come back in problem order.  There is no collective: the
  * problems never interact and one host gathers by D2H copies.  (One process per GPU: ualm_pack_records_device + an NCCL
  * all-gather of the records on the caller's communicator, uneven_planner_b200/distributed.py.) */
 int ualm_solve_batch_multi(ualm_ctx_t **ctxs, int nctx, int B, const int32_t *N, const int32_t *M, const double *bnd,
                            const double *total_time, const double *inner_xy, const double *inner_yaw, ualm_result_t *results,
                            double *c_xy, double *c_yaw);
+int ualm_solve_batch_multi_env(ualm_ctx_t **ctxs, int nctx, int B, const int32_t *N, const int32_t *M, const double *bnd,
+                               const double *total_time, const double *inner_xy, const double *inner_yaw, const int32_t *env,
+                               ualm_result_t *results, double *c_xy, double *c_yaw);
 
 /* Fixed-stride result records for the multi-GPU all-gather: writes B records of `stride` doubles into
  * a DEVICE buffer (e.g. a torch tensor): [ret, outer, evals, iters, cost, jerk, T, res_h, res_g, N, M, pad,
@@ -174,7 +200,8 @@ int ualm_pack_records_device_async(ualm_ctx_t *ctx, double *d_records, int strid
 /* ---- phase entry points (kernel-level parity; SURVEY 8b item 3) ----
  * One innerCallback evaluation (alm_traj_opt.cpp:280-347) per problem of the uploaded batch at the given
  * decision vectors x (packed, n_b = 1+2(N_b-1)+(M_b-1)) with duals lambda[S_b], mu[6 S_b], scale_cx[7 S_b]
- * in the reference's index layout (alm_traj_opt.cpp:705-707, 832-946), S_b = N_b (int_K+1).
+ * in the reference's index layout (alm_traj_opt.cpp:705-707, 832-946), S_b = N_b (int_K+1) with the int_K of problem b's
+ * environment.
  * Outputs (host): f[B], grad (packed n_b), hx (packed S_b), gx (packed 6 S_b). Any input dual may be
  * NULL (zeros / ones).  scale_fx[B], rho scalar. */
 int ualm_eval_batch(ualm_ctx_t *ctx, const double *x, const double *lambda, const double *mu,

@@ -161,6 +161,17 @@ public:
         check(ualm_set_map_f64(ctx_, &geom, rxs2_cells, repack_to_float ? 1 : 0), "ualm_set_map_f64");
     }
 
+    // Environment `env` (0 <= env < UALM_MAX_ENVS): a parameter set and a map grid of its own, for batches that mix terrains or
+    // vehicle classes (optimizeBatch / submitBatch with env[]).  init() and setEnvironment() above bind environment 0.
+    void setEnvironment(int env, const ualm_params_t &p, const ualm_map_geom_t &geom, const float *cells_xyzw)
+    {
+        bindEnv(env, p, [&] { return ualm_set_map(ctx_, &geom, cells_xyzw); }, "ualm_set_map");
+    }
+    void setEnvironment(int env, const ualm_params_t &p, const ualm_map_geom_t &geom, const double *rxs2_cells, bool repack_to_float = false)
+    {
+        bindEnv(env, p, [&] { return ualm_set_map_f64(ctx_, &geom, rxs2_cells, repack_to_float ? 1 : 0); }, "ualm_set_map_f64");
+    }
+
     // ---- single problem, the reference's call (alm_traj_opt.h:92-98), plain pointers ----
     // initStateXY/endStateXY: 2x3 column-major; innerPtsXY: 2 x (N-1) column-major; initYaw/endYaw: 3; innerPtsYaw: M-1
     int optimizeSE2Traj(const double *initStateXY, const double *endStateXY, const double *innerPtsXY, int n_inner_xy,
@@ -196,6 +207,12 @@ public:
     {
         check(ualm_solve_batch(ctx_, B, N, M, bnd, total_time, inner_xy, inner_yaw, results, c_xy, c_yaw), "ualm_solve_batch");
     }
+    // the same with the environment of every problem (env[B], nullptr = all 0)
+    void optimizeBatch(int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time, const double *inner_xy,
+                       const double *inner_yaw, const int32_t *env, ualm_result_t *results, double *c_xy, double *c_yaw)
+    {
+        check(ualm_solve_batch_env(ctx_, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, results, c_xy, c_yaw), "ualm_solve_batch_env");
+    }
 
     // pipelined form: submit returns once the batch is uploaded and queued (up to `depth` batches in flight), wait collects it
     int submitBatch(int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time, const double *inner_xy,
@@ -203,6 +220,13 @@ public:
     {
         int ticket = -1;
         check(ualm_submit_batch(ctx_, B, N, M, bnd, total_time, inner_xy, inner_yaw, depth, &ticket), "ualm_submit_batch");
+        return ticket;
+    }
+    int submitBatch(int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time, const double *inner_xy,
+                    const double *inner_yaw, const int32_t *env, int depth)
+    {
+        int ticket = -1;
+        check(ualm_submit_batch_env(ctx_, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, depth, &ticket), "ualm_submit_batch_env");
         return ticket;
     }
     void waitBatch(int ticket, ualm_result_t *results, double *c_xy, double *c_yaw) { check(ualm_wait_batch(ctx_, ticket, results, c_xy, c_yaw), "ualm_wait_batch"); }
@@ -247,6 +271,18 @@ private:
     static void check(int rc, const char *what)
     {
         if (rc != UALM_OK) throw std::runtime_error(std::string(what) + ": " + ualm_last_error());
+    }
+    // select `env`, bind its parameters and grid, select environment 0 again (also when a call throws)
+    template <class F>
+    void bindEnv(int env, const ualm_params_t &p, F set_map, const char *what)
+    {
+        check(ualm_select_env(ctx_, env), "ualm_select_env");
+        int rc = ualm_set_params(ctx_, &p);
+        const std::string msg = rc != UALM_OK ? std::string("ualm_set_params: ") + ualm_last_error() : std::string();
+        if (rc == UALM_OK) rc = set_map();
+        const std::string msg2 = msg.empty() && rc != UALM_OK ? std::string(what) + ": " + ualm_last_error() : msg;
+        ualm_select_env(ctx_, 0);
+        if (rc != UALM_OK) throw std::runtime_error(msg2);
     }
     ualm_ctx_t *ctx_ = nullptr;
     ualm_result_t last_{};

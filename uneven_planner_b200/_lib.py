@@ -12,6 +12,7 @@ LIB_PATH = os.path.join(HERE, "libualm.so")
 
 UALM_OK, UALM_ENOCUDA, UALM_EINVAL, UALM_ESTATE, UALM_ELIMIT = 0, -1, -2, -3, -4
 UALM_RET_STOPPED = 3   # ret_code of a problem stopped by the evaluation budget or a deadline (include/ualm.h)
+UALM_MAX_ENVS = 4      # environments (parameter set + map grid) per context (include/ualm.h, ualm_select_env)
 
 
 class Params(C.Structure):
@@ -123,9 +124,15 @@ def lib():
         L.ualm_mark_end.argtypes = [vp, C.POINTER(C.c_float)]
         L.ualm_solve_batch_multi.argtypes = [C.POINTER(vp), C.c_int, C.c_int, ip, ip, dp, dp, dp, dp, C.POINTER(Result), dp, dp]
         L.ualm_pack_records_device_async.argtypes = [vp, vp, C.c_int]
+        L.ualm_select_env.argtypes = [vp, C.c_int]
+        L.ualm_upload_env.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, dp, ip]
+        L.ualm_solve_batch_env.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, dp, ip, C.POINTER(Result), dp, dp]
+        L.ualm_submit_batch_env.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, dp, ip, C.c_int, C.POINTER(C.c_int)]
+        L.ualm_solve_batch_multi_env.argtypes = [C.POINTER(vp), C.c_int, C.c_int, ip, ip, dp, dp, dp, dp, ip, C.POINTER(Result), dp, dp]
         for name in ("ualm_reset_stream", "ualm_set_map_f64", "ualm_max_lanes", "ualm_select_lane", "ualm_submit_batch", "ualm_wait_batch",
                      "ualm_wait_batch_for", "ualm_set_budget",
-                     "ualm_mark_begin", "ualm_mark_end", "ualm_solve_batch_multi", "ualm_pack_records_device_async"):
+                     "ualm_mark_begin", "ualm_mark_end", "ualm_solve_batch_multi", "ualm_pack_records_device_async", "ualm_select_env",
+                     "ualm_upload_env", "ualm_solve_batch_env", "ualm_submit_batch_env", "ualm_solve_batch_multi_env"):
             getattr(L, name).restype = C.c_int
         for name in ("ualm_create", "ualm_destroy", "ualm_set_params", "ualm_set_map", "ualm_solve_batch",
                      "ualm_upload", "ualm_solve_resident", "ualm_sync", "ualm_download", "ualm_last_solve_ms",

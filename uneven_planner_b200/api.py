@@ -4,6 +4,8 @@
     init(params)            <- ALMTrajOpt::init(nh)                 (alm_traj_opt.cpp:5-45)
     set_environment(map)    <- ALMTrajOpt::setEnvironment(map)      (alm_traj_opt.h:127-130)
     optimize(problems)      <- B x ALMTrajOpt::optimizeSE2Traj(...) (alm_traj_opt.h:92-98), then getTraj()
+A context holds up to UALM_MAX_ENVS environments (parameter set + map grid): init(params, env=k) / set_environment(map, env=k)
+bind environment k, and a batch whose `env` array is set solves every problem in its own environment (ProblemBatch.env).
 All compute happens inside libualm.so on the GPU; this file only marshals numpy arrays.
 """
 import ctypes as C
@@ -19,6 +21,11 @@ ip = C.POINTER(C.c_int32)
 
 def _p(a, t=dp):
     return None if a is None else a.ctypes.data_as(t)
+
+
+def _env(pb):
+    """int32 environment index per problem, or None (= all environment 0)"""
+    return None if getattr(pb, "env", None) is None else np.ascontiguousarray(pb.env, np.int32)
 
 
 class UalmError(RuntimeError):
@@ -40,6 +47,8 @@ class BatchALMTrajOpt:
         self.h = C.c_void_p()
         _check(L.ualm_create(C.byref(self.h), device, precision))
         self.params = None
+        self.env_params = {}
+        self.env = 0            # the selected environment (ualm_select_env)
         self.pb = None
 
     def close(self):
@@ -53,9 +62,22 @@ class BatchALMTrajOpt:
         except Exception:
             pass
 
-    def init(self, params=None):
-        self.params = params or _lib.default_params()
-        _check(self.L.ualm_set_params(self.h, C.byref(self.params)))
+    def select_env(self, env):
+        """ualm_select_env: init / set_environment without an `env` argument bind environment `env` from now on."""
+        _check(self.L.ualm_select_env(self.h, int(env)))
+        self.env = int(env)
+        return self
+
+    def init(self, params=None, env=None):
+        """ualm_set_params for environment `env` (None: the selected one, environment 0 unless select_env chose another; a given
+        `env` stays selected).  self.params keeps environment 0's."""
+        params = params or _lib.default_params()
+        if env is not None:
+            self.select_env(env)
+        _check(self.L.ualm_set_params(self.h, C.byref(params)))
+        self.env_params[self.env] = params
+        if self.env == 0:
+            self.params = params
         return self
 
     def set_budget(self, max_evals):
@@ -68,10 +90,13 @@ class BatchALMTrajOpt:
         _check(self.L.ualm_set_stream(self.h, C.c_void_p(cuda_stream_ptr)))
         return self
 
-    def set_environment(self, mapdata, repack_to_float=False):
-        """Binds the map grid.  A map that carries the reference's own double grid (`cells64`, RXS2 = 4 doubles per cell) goes
-        through ualm_set_map_f64; repack_to_float rounds it to the float4 grid on the way."""
-        self.map = mapdata
+    def set_environment(self, mapdata, repack_to_float=False, env=None):
+        """Binds the map grid of environment `env` (None: the selected one, as for init).  A map that carries the reference's own double
+        grid (`cells64`, RXS2 = 4 doubles per cell) goes through ualm_set_map_f64; repack_to_float rounds it to the float4 grid on the way."""
+        if env is not None:
+            self.select_env(env)
+        if self.env == 0:
+            self.map = mapdata
         c64 = getattr(mapdata, "cells64", None)
         if c64 is not None:
             _check(self.L.ualm_set_map_f64(self.h, C.byref(mapdata.geom), c64.ctypes.data_as(dp), 1 if repack_to_float else 0))
@@ -106,10 +131,12 @@ class BatchALMTrajOpt:
                                                         pb.inner_yaw.astype(np.float64))]
         N, M, bnd, T, ixy, iyaw = host
         t = C.c_int(-1)
-        _check(self.L.ualm_submit_batch(self.h, pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), int(depth), C.byref(t)))
+        env = _env(pb)
+        _check(self.L.ualm_submit_batch_env(self.h, pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), _p(env, ip), int(depth),
+                                            C.byref(t)))
         if not hasattr(self, "_tickets"):
             self._tickets = {}
-        self._tickets[t.value] = (pb, host)
+        self._tickets[t.value] = (pb, (host, env))
         return t.value
 
     def wait(self, ticket, out=None, timeout_ms=None):
@@ -135,8 +162,9 @@ class BatchALMTrajOpt:
         self._keep = [np.ascontiguousarray(a) for a in (pb.N.astype(np.int32), pb.M.astype(np.int32), pb.bnd.astype(np.float64),
                                                         pb.total_time.astype(np.float64), pb.inner_xy.astype(np.float64),
                                                         pb.inner_yaw.astype(np.float64))]
-        N, M, bnd, T, ixy, iyaw = self._keep
-        _check(self.L.ualm_upload(self.h, pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw)))
+        self._keep.append(_env(pb))
+        N, M, bnd, T, ixy, iyaw, env = self._keep
+        _check(self.L.ualm_upload_env(self.h, pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), _p(env, ip)))
 
     def solve_resident(self):
         _check(self.L.ualm_solve_resident(self.h))
@@ -166,7 +194,9 @@ class BatchALMTrajOpt:
         res = (Result * pb.B)()
         cxy = np.zeros(int(12 * N.astype(np.int64).sum()))
         cyaw = np.zeros(int(6 * M.astype(np.int64).sum()))
-        _check(self.L.ualm_solve_batch(self.h, pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), res, _p(cxy), _p(cyaw)))
+        env = _env(pb)
+        _check(self.L.ualm_solve_batch_env(self.h, pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), _p(env, ip), res, _p(cxy),
+                                           _p(cyaw)))
         return res, cxy, cyaw
 
     def pack_records(self, dev_ptr, stride, wait=True):
@@ -174,20 +204,33 @@ class BatchALMTrajOpt:
         _check(f(self.h, C.c_void_p(dev_ptr), stride))
 
     # ---- phase entry points ----------------------------------------------------------
+    def _samples(self, pb):
+        """samples per problem: N (int_K + 1) with the int_K of the problem's environment"""
+        K = np.array([self.env_params[e].int_K if e in self.env_params else 0 for e in range(_lib.UALM_MAX_ENVS)], np.int64)
+        env = np.zeros(pb.B, np.int64) if getattr(pb, "env", None) is None else np.asarray(pb.env, np.int64)
+        return pb.N.astype(np.int64) * (K[env] + 1)
+
     def eval_batch(self, x=None, lam=None, mu=None, scale_cx=None, scale_fx=None, rho=None):
+        """ualm_eval_batch at one penalty weight `rho` for every problem.  rho=None: the `rho` parameter of the batch's environments,
+        which must then agree (pass rho explicitly for a batch whose environments differ in it)."""
         pb = self.pb
-        K = self.params.int_K
-        nx = int(pb.nvar().sum()); S = int(pb.nsamples(K).sum())
+        if rho is None:
+            envs = [0] if getattr(pb, "env", None) is None else sorted({int(e) for e in pb.env})
+            rhos = {self.env_params[e].rho for e in envs if e in self.env_params}
+            if len(rhos) != 1:
+                raise ValueError("eval_batch: the batch's environments differ in rho (or have no parameters bound): pass rho")
+            rho = rhos.pop()
+        nx = int(pb.nvar().sum()); S = int(self._samples(pb).sum())
         f = np.zeros(pb.B); grad = np.zeros(nx); hx = np.zeros(S); gx = np.zeros(6 * S)
         cxy = np.zeros(int(12 * pb.N.astype(np.int64).sum())); cyaw = np.zeros(int(6 * pb.M.astype(np.int64).sum()))
         arrs = [None if a is None else np.ascontiguousarray(a, np.float64) for a in (x, lam, mu, scale_cx, scale_fx)]
         _check(self.L.ualm_eval_batch(self.h, _p(arrs[0]), _p(arrs[1]), _p(arrs[2]), _p(arrs[3]), _p(arrs[4]),
-                                      float(self.params.rho if rho is None else rho), _p(f), _p(grad), _p(hx), _p(gx), _p(cxy), _p(cyaw)))
+                                      float(rho), _p(f), _p(grad), _p(hx), _p(gx), _p(cxy), _p(cyaw)))
         return dict(f=f, grad=grad, hx=hx, gx=gx, c_xy=cxy, c_yaw=cyaw)
 
     def init_scaling_batch(self):
         pb = self.pb
-        S = int(pb.nsamples(self.params.int_K).sum())
+        S = int(self._samples(pb).sum())
         sfx = np.zeros(pb.B); scx = np.zeros(7 * S)
         _check(self.L.ualm_init_scaling_batch(self.h, _p(sfx), _p(scx)))
         return sfx, scx
@@ -241,7 +284,7 @@ class BatchALMTrajOpt:
 
 
 def solve_batch_multi(opts, pb):
-    """ualm_solve_batch_multi: one host process, one BatchALMTrajOpt per device (same params and map bound on each)."""
+    """ualm_solve_batch_multi_env: one host process, one BatchALMTrajOpt per device (same params and maps bound on each)."""
     L = opts[0].L
     hs = (C.c_void_p * len(opts))(*[o.h for o in opts])
     N = np.ascontiguousarray(pb.N, np.int32); M = np.ascontiguousarray(pb.M, np.int32)
@@ -249,5 +292,7 @@ def solve_batch_multi(opts, pb):
     ixy = np.ascontiguousarray(pb.inner_xy, np.float64); iyaw = np.ascontiguousarray(pb.inner_yaw, np.float64)
     res = (Result * pb.B)()
     cxy = np.zeros(int(12 * N.astype(np.int64).sum())); cyaw = np.zeros(int(6 * M.astype(np.int64).sum()))
-    _check(L.ualm_solve_batch_multi(hs, len(opts), pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), res, _p(cxy), _p(cyaw)))
+    env = _env(pb)
+    _check(L.ualm_solve_batch_multi_env(hs, len(opts), pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), _p(env, ip), res, _p(cxy),
+                                        _p(cyaw)))
     return res, cxy, cyaw

@@ -60,13 +60,20 @@ struct Lane {
     std::vector<ProbDesc> desc;
     std::vector<int> order;              // launch order over the ACTIVE problems (largest first)
     std::vector<unsigned char> skip;     // problems over the compiled limits: not solved, ret_code = UALM_ELIMIT in their record
+    // environments: env[b] of every problem; eidx = all problems grouped by environment (ascending within one), environment e at
+    // [eoff[e], eoff[e + 1]).  The one-warp-per-problem kernels run once per environment present, over its slice of d_eidx
+    std::vector<int> env, eidx;
+    int eoff[UALM_MAX_ENVS + 1] = {};
+    DevBuf<int> d_eidx;
+    SmemLayout eL[UALM_MAX_ENVS];        // their layouts (maxima over the environment's problems)
+    size_t esmem[UALM_MAX_ENVS] = {};
     long long tot_x = 0, tot_s = 0, tot_cxy = 0, tot_cyaw = 0, tot_hist = 0, tot_scr = 0, tot_fac = 0, tot_ws = 0;
     DevBuf<ProbDesc> d_desc;
     DevBuf<int> d_order;
     DevBuf<int4> d_wdesc;
     std::vector<int4> wdesc;
     std::vector<int> group;      // warps per problem (1, 2 or 4)
-    struct GClass { int G = 1, n_ctas = 0, r0 = 0, r1 = 0, occ = 1; size_t wd_off = 0, smem = 0; SmemLayout L; };
+    struct GClass { int G = 1, n_ctas = 0, r0 = 0, r1 = 0, occ = 1, env = 0; size_t wd_off = 0, smem = 0; SmemLayout L; };
     std::vector<GClass> cls;
     enum { NAUX = 7 };
     cudaStream_t aux[NAUX] = {};
@@ -77,8 +84,6 @@ struct Lane {
     DevBuf<double> d_pieceT, d_feas;
     float last_ms = 0.f;
     int last_launches = 0;
-    SmemLayout L;
-    size_t smem_bytes = 0;
     // cancel word of the lane's solves (ualm_wait_batch_for), in device memory: the host raises it by a copy on the context's
     // cancel stream while the kernels run.  (A word in mapped pinned host memory, read over PCIe at every stop test, made the bench
     // step 5 % slower on an H100 80GB HBM3 at a 400 W power limit.)
@@ -87,7 +92,7 @@ struct Lane {
     {
         if (d_cancel) cudaFree(d_cancel);
         d_cancel = nullptr;
-        d_desc.release(); d_order.release(); d_wdesc.release();
+        d_desc.release(); d_order.release(); d_wdesc.release(); d_eidx.release();
         DevBuf<double> *bufs[] = {&d_x0, &d_x, &d_lambda, &d_mu, &d_scale_cx, &d_hx, &d_gx, &d_lm_s, &d_lm_y, &d_lm_aux, &d_fac,
                                   &d_scr, &d_ws, &d_cxy, &d_cyaw, &d_f, &d_grad, &d_sfx};
         for (auto *b : bufs) b->release();
@@ -102,15 +107,22 @@ struct Lane {
     }
 };
 
-struct ualm_ctx {
-    int device = 0, precision = 64;
-    ualm_tp::TpEngine *tp = nullptr;     // precision 32 / 65: the throughput engine (ualm_tp.cu) behind the same entry points
+// One environment: a parameter set and a map grid (ualm_select_env).  The kernels take both as per-launch grid constants.
+struct Env {
     bool have_params = false, have_map = false;
     ualm_params_t hp;
     DevParams dp;
     DevMap dm;
     DevBuf<float4> cells;
     DevBuf<double> cells64;
+};
+
+struct ualm_ctx {
+    int device = 0, precision = 64;
+    ualm_tp::TpEngine *tp = nullptr;     // precision 32 / 65: the throughput engine (ualm_tp.cu) behind the same entry points
+    Env envs[UALM_MAX_ENVS];
+    int sel_env = 0;                     // the environment ualm_set_params / ualm_set_map bind (ualm_select_env)
+    int max_evals = 0;                   // ualm_set_budget
     Lane lanes[UALM_MAX_LANES];
     Lane *b = nullptr;            // the selected lane (ualm_select_lane; lane 0 by default)
     int cur = 0, next_submit = 0;
@@ -196,7 +208,7 @@ extern "C" int ualm_destroy(ualm_ctx_t *c)
     cudaSetDevice(c->device);
     cudaDeviceSynchronize();
     if (c->tp) { ualm_tp::tp_destroy(c->tp); c->tp = nullptr; }
-    c->cells.release(); c->cells64.release();
+    for (auto &v : c->envs) { v.cells.release(); v.cells64.release(); }
     for (auto &l : c->lanes) l.release();
     if (c->join) cudaStreamDestroy(c->join);
     if (c->cancel) cudaStreamDestroy(c->cancel);
@@ -244,42 +256,58 @@ extern "C" int ualm_reset_stream(ualm_ctx_t *c)
     return UALM_OK;
 }
 
+// binding is refused while a batch is in flight, on the parity lanes and on the throughput engine's
+static int lanes_idle(ualm_ctx *c, const char *what)
+{
+    for (int q = 0; q < UALM_MAX_LANES; q++)
+        if (c->tp ? ualm_tp::tp_lane_in_flight(c->tp, q) : c->lanes[q].in_flight)
+            return fail(UALM_ESTATE, std::string(what) + " while a submitted batch is in flight (ualm_wait_batch first)");
+    return UALM_OK;
+}
+
 extern "C" int ualm_set_params(ualm_ctx_t *c, const ualm_params_t *p)
 {
     if (!c || !p) return fail(UALM_EINVAL, "null argument");
     if (p->int_K < 1 || p->int_K > 128) return fail(UALM_ELIMIT, "int_K out of range [1,128]");
     if (p->mem_size < 1 || p->mem_size > 1024) return fail(UALM_ELIMIT, "mem_size out of range [1,1024]");
     if (p->past < 0 || p->past > 16) return fail(UALM_ELIMIT, "past out of range [0,16]");
-    for (auto &l : c->lanes)
-        if (l.in_flight) return fail(UALM_ESTATE, "ualm_set_params while a submitted batch is in flight (ualm_wait_batch first)");
+    if (int rc = lanes_idle(c, "ualm_set_params")) return rc;
+    // the throughput engine has its own limits (int_K <= 127): the context's copy and its flag change only once it has accepted them,
+    // so a refused binding leaves the environment as it was
+    if (c->tp) {
+        std::string em;
+        if (int rc = ualm_tp::tp_set_params(c->tp, c->sel_env, p, &em)) return fail(rc, em);
+    }
     // int_K, mem_size and past are baked into the resident batches' descriptors, buffer sizes and shared-memory layouts: a
     // parameter change invalidates every uploaded batch (it must be uploaded again before the next solve / eval call)
     for (auto &l : c->lanes) { l.have_batch = false; l.solved = false; }
-    c->hp = *p;
-    DevParams &d = c->dp;
+    Env &v = c->envs[c->sel_env];
+    v.hp = *p;
+    DevParams &d = v.dp;
     d.rho_T = p->rho_T; d.rho_ter = p->rho_ter; d.max_vel = p->max_vel; d.max_acc_lon = p->max_acc_lon; d.max_acc_lat = p->max_acc_lat;
     d.max_kap = p->max_kap; d.min_cxi = p->min_cxi; d.max_sig = p->max_sig; d.use_scaling = p->use_scaling; d.rho = p->rho;
     d.beta = p->beta; d.gamma = p->gamma; d.epsilon_con = p->epsilon_con; d.max_iter = p->max_iter; d.g_epsilon = p->g_epsilon;
     d.min_step = p->min_step; d.delta = p->delta; d.inner_max_iter = (int)p->inner_max_iter; d.mem_size = p->mem_size; d.past = p->past;
     d.int_K = p->int_K; d.gravity = p->gravity;
-    c->have_params = true;
-    if (c->tp) TP_CALL(ualm_tp::tp_set_params(c->tp, p, err));
+    v.have_params = true;
     return UALM_OK;
 }
 
-static int map_geometry_set(ualm_ctx *c, const ualm_map_geom_t *g)
+extern "C" int ualm_select_env(ualm_ctx_t *c, int env)
 {
-    DevMap &m = c->dm;
+    if (!c) return fail(UALM_EINVAL, "null ctx");
+    if (env < 0 || env >= UALM_MAX_ENVS) return fail(UALM_EINVAL, "env out of range [0, UALM_MAX_ENVS)");
+    c->sel_env = env;
+    return UALM_OK;
+}
+
+static int map_geometry_set(Env &v, const ualm_map_geom_t *g)
+{
+    DevMap &m = v.dm;
     for (int k = 0; k < 3; k++) { m.vn[k] = g->voxel_num[k]; m.origin[k] = g->origin[k]; m.maxb[k] = g->max_boundary[k]; }
     m.xy_res = g->xy_resolution; m.yaw_res = g->yaw_resolution;
     m.xy_inv = 1.0 / g->xy_resolution; m.yaw_inv = 1.0 / g->yaw_resolution; // uneven_map.cpp:104-105
-    c->have_map = true;
-    return UALM_OK;
-}
-static int lanes_idle(ualm_ctx *c, const char *what)
-{
-    for (auto &l : c->lanes)
-        if (l.in_flight) return fail(UALM_ESTATE, std::string(what) + " while a submitted batch is in flight (ualm_wait_batch first)");
+    v.have_map = true;
     return UALM_OK;
 }
 
@@ -288,15 +316,20 @@ extern "C" int ualm_set_map(ualm_ctx_t *c, const ualm_map_geom_t *g, const float
     if (!c || !g || !cells) return fail(UALM_EINVAL, "null argument");
     if (int rc = lanes_idle(c, "ualm_set_map")) return rc;
     CK(cudaSetDevice(c->device));
+    // the engine's grid first: the context's copy (which serves the post-solve scan) and its flag change only once it is bound
+    if (c->tp) {
+        std::string em;
+        if (int rc = ualm_tp::tp_set_map(c->tp, c->sel_env, g, cells, &em)) return fail(rc, em);
+    }
     CK(cudaDeviceSynchronize());
     const size_t ncell = (size_t)g->voxel_num[0] * g->voxel_num[1] * g->voxel_num[2];
-    CK(c->cells.ensure(ncell));
-    CK(cudaMemcpy(c->cells.p, cells, ncell * sizeof(float4), cudaMemcpyHostToDevice));
-    c->cells64.release();
-    c->dm.cells = c->cells.p; c->dm.cells64 = nullptr;
-    map_geometry_set(c, g);
-    if (c->tp) TP_CALL(ualm_tp::tp_set_map(c->tp, g, cells, err));      // (the context's own copy serves the post-solve scan)
-    return UALM_OK;
+    Env &v = c->envs[c->sel_env];
+    v.have_map = false;         // until the copy below is complete (a failed copy leaves the environment unbound, not half bound)
+    CK(v.cells.ensure(ncell));
+    CK(cudaMemcpy(v.cells.p, cells, ncell * sizeof(float4), cudaMemcpyHostToDevice));
+    v.cells64.release();
+    v.dm.cells = v.cells.p; v.dm.cells64 = nullptr;
+    return map_geometry_set(v, g);
 }
 
 // the reference's own grid: UnevenMap::map_buffer is RXS2 {double z, sigma; Vector2d zb} = 4 doubles per cell (uneven_map.h:36-64)
@@ -312,27 +345,52 @@ extern "C" int ualm_set_map_f64(ualm_ctx_t *c, const ualm_map_geom_t *g, const d
         for (size_t q = 0; q < 4 * ncell; q++) f[q] = (float)cells[q];
         return ualm_set_map(c, g, f.data());
     }
-    CK(c->cells64.ensure(4 * ncell));
-    CK(cudaMemcpy(c->cells64.p, cells, 4 * ncell * sizeof(double), cudaMemcpyHostToDevice));
-    c->cells.release();
-    c->dm.cells = nullptr; c->dm.cells64 = c->cells64.p;
-    return map_geometry_set(c, g);
+    Env &v = c->envs[c->sel_env];
+    v.have_map = false;         // until the copy below is complete
+    CK(v.cells64.ensure(4 * ncell));
+    CK(cudaMemcpy(v.cells64.p, cells, 4 * ncell * sizeof(double), cudaMemcpyHostToDevice));
+    v.cells.release();
+    v.dm.cells = nullptr; v.dm.cells64 = v.cells64.p;
+    return map_geometry_set(v, g);
 }
 
+// the one-warp-per-problem layout of every environment present in the lane's batch (sized by that environment's maxima)
 static int prepare_launch(ualm_ctx *c)
 {
     Lane *b = c->b;
-    b->L = make_layout(b->Nmax, b->Mmax, b->nmax, c->dp.mem_size, c->dp.past, c->dp.int_K, b->Smax);
-    b->smem_bytes = (size_t)b->L.total_doubles * sizeof(double) * UALM_WPB;
-    if (b->smem_bytes > 227 * 1024) return fail(UALM_ELIMIT, "problem too large for shared memory (N/M/int_K too big)");
-    // the attribute is per function, not per lane: only ever raise it (another lane's kernels may be in flight with a larger size)
-    static size_t smem_max = 0;
-    if (b->smem_bytes > smem_max) {
-        smem_max = b->smem_bytes;
-        CK(cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
-        CK(cudaFuncSetAttribute(eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
-        CK(cudaFuncSetAttribute(scaling_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
-        CK(cudaFuncSetAttribute(penalty_only_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
+    for (int e = 0; e < UALM_MAX_ENVS; e++) {
+        if (b->eoff[e + 1] == b->eoff[e]) continue;
+        int Nm = 1, Mm = 1, nm = 1, Sm = 1;
+        for (int q = b->eoff[e]; q < b->eoff[e + 1]; q++) {
+            const ProbDesc &d = b->desc[b->eidx[q]];
+            if (b->skip[b->eidx[q]]) continue;
+            Nm = std::max(Nm, d.N); Mm = std::max(Mm, d.M); nm = std::max(nm, d.n); Sm = std::max(Sm, d.S);
+        }
+        const DevParams &dp = c->envs[e].dp;
+        b->eL[e] = make_layout(Nm, Mm, nm, dp.mem_size, dp.past, dp.int_K, Sm);
+        b->esmem[e] = (size_t)b->eL[e].total_doubles * sizeof(double) * UALM_WPB;
+        if (b->esmem[e] > 227 * 1024) return fail(UALM_ELIMIT, "problem too large for shared memory (N/M/int_K too big)");
+        // the attribute is per function, not per lane: only ever raise it (another lane's kernels may be in flight with a larger size)
+        static size_t smem_max = 0;
+        if (b->esmem[e] > smem_max) {
+            smem_max = b->esmem[e];
+            CK(cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
+            CK(cudaFuncSetAttribute(eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
+            CK(cudaFuncSetAttribute(scaling_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
+            CK(cudaFuncSetAttribute(penalty_only_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
+        }
+    }
+    return UALM_OK;
+}
+
+// env[B] (NULL = all 0): every index in range and every environment used fully bound, checked before anything is touched
+static int check_envs(ualm_ctx *c, int B, const int32_t *env)
+{
+    for (int b = 0; b < (env ? B : 1); b++) {
+        const int e = env ? env[b] : 0;
+        if (e < 0 || e >= UALM_MAX_ENVS) return fail(UALM_EINVAL, "env index out of range [0, UALM_MAX_ENVS)");
+        if (!c->envs[e].have_params || !c->envs[e].have_map)
+            return fail(UALM_ESTATE, "environment " + std::to_string(e) + " has no parameters or no map grid bound (ualm_select_env + ualm_set_params / ualm_set_map)");
     }
     return UALM_OK;
 }
@@ -355,12 +413,36 @@ static BatchPtrs batch_ptrs(ualm_ctx *c)
     return b;
 }
 
+// launch(e, bp, count) once per environment present in the selected lane's batch, with bp.order / bp.n_active set to that
+// environment's problems (eval_kernel, scaling_kernel and penalty_only_kernel map their warps to problems through them)
+template <class F>
+static int per_env(ualm_ctx *c, F launch)
+{
+    Lane *l = c->b;
+    for (int e = 0; e < UALM_MAX_ENVS; e++) {
+        const int cnt = l->eoff[e + 1] - l->eoff[e];
+        if (cnt == 0) continue;
+        BatchPtrs bp = batch_ptrs(c);
+        bp.order = l->d_eidx.p + l->eoff[e];
+        bp.n_active = cnt;
+        launch(e, bp, cnt);
+        CK(cudaGetLastError());
+    }
+    return UALM_OK;
+}
+
 extern "C" int ualm_upload(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
                            const double *inner_xy, const double *inner_yaw)
 {
+    return ualm_upload_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, nullptr);
+}
+
+extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
+                               const double *inner_xy, const double *inner_yaw, const int32_t *env)
+{
     if (!c || B < 0 || (B > 0 && (!N || !M || !bnd || !total_time))) return fail(UALM_EINVAL, "bad argument");
-    if (c->tp) TP_CALL(ualm_tp::tp_upload(c->tp, c->cur, B, N, M, bnd, total_time, inner_xy, inner_yaw, err));
-    if (!c->have_params) return fail(UALM_ESTATE, "ualm_set_params must be called before ualm_upload");
+    if (int rc = check_envs(c, B, env)) return rc;
+    if (c->tp) TP_CALL(ualm_tp::tp_upload(c->tp, c->cur, B, N, M, env, bnd, total_time, inner_xy, inner_yaw, err));
     Lane *l = c->b;
     if (l->in_flight) return fail(UALM_ESTATE, "ualm_upload into a lane whose submitted batch is still in flight");
     // validate everything before touching the lane; the lane holds no batch until this call has fully succeeded
@@ -373,8 +455,9 @@ extern "C" int ualm_upload(ualm_ctx_t *c, int B, const int32_t *N, const int32_t
     if ((need_xy > 0 && !inner_xy) || (need_yaw > 0 && !inner_yaw)) return fail(UALM_EINVAL, "inner waypoint arrays are NULL but N > 1 or M > 1");
     l->have_batch = false; l->solved = false;
     CK(cudaSetDevice(c->device));
-    const int K = c->dp.int_K, m = c->dp.mem_size;
     l->B = B; l->desc.assign(B, ProbDesc()); l->order.clear(); l->group.assign(B, 1); l->skip.assign(B, 0);
+    l->env.assign(B, 0);
+    if (env) l->env.assign(env, env + B);
     l->Nmax = l->Mmax = l->nmax = l->Smax = 1;
     for (int b = 0; b < B; b++) {
         ProbDesc &d = l->desc[b];
@@ -382,10 +465,16 @@ extern "C" int ualm_upload(ualm_ctx_t *c, int B, const int32_t *N, const int32_t
         // compiled limits (n <= 256: the L-BFGS register tile, UALM_NREG in ualm_kernels.cuh): such a problem is not solved, its
         // record says UALM_ELIMIT, and the rest of the batch runs
         if (N[b] > UALM_NMAX || M[b] > UALM_MMAX) { l->skip[b] = 1; d.n = 0; d.S = 0; continue; }
-        d.n = 1 + 2 * (N[b] - 1) + (M[b] - 1); d.S = N[b] * (K + 1);
+        d.n = 1 + 2 * (N[b] - 1) + (M[b] - 1); d.S = N[b] * (c->envs[l->env[b]].dp.int_K + 1);
         l->Nmax = std::max(l->Nmax, d.N); l->Mmax = std::max(l->Mmax, d.M); l->nmax = std::max(l->nmax, d.n); l->Smax = std::max(l->Smax, d.S);
         l->order.push_back(b);
     }
+    l->eidx.clear();
+    for (int e = 0; e < UALM_MAX_ENVS; e++) {
+        l->eoff[e] = (int)l->eidx.size();
+        for (int b = 0; b < B; b++) if (l->env[b] == e) l->eidx.push_back(b);
+    }
+    l->eoff[UALM_MAX_ENVS] = B;
     l->n_active = (int)l->order.size();
     const int BA = l->n_active;
     // launch order: most samples first (longest-processing-time-first keeps the tail short)
@@ -410,6 +499,7 @@ extern "C" int ualm_upload(ualm_ctx_t *c, int B, const int32_t *N, const int32_t
         }
         const long long W = 4LL * occ0 * dev_sms;   // warp slots on the device
         std::vector<Lane::GClass> best;
+        std::vector<int> best_ord;
         for (int attempt = 0; attempt < 32; attempt++) {
             // Policy: helpers shorten the latency of a trajectory without adding to the L2-resident working set, while more
             // resident trajectories thrash the L2.  So: everything that fits gets 4 warps; beyond that 2 warps per trajectory,
@@ -427,42 +517,51 @@ extern "C" int ualm_upload(ualm_ctx_t *c, int B, const int32_t *N, const int32_t
                 K4 = (long long)(BA * (getenv("UALM_F4") ? atof(getenv("UALM_F4")) : 0.0));
                 K2 = std::min<long long>(BA - K4, (long long)(BA * (getenv("UALM_F2") ? atof(getenv("UALM_F2")) : 0.0))) & ~1LL;
             }
-            // rank ranges per group size, each split into size buckets (the order is by descending size)
+            // rank ranges per group size; within one, the problems of each environment (a class holds one: its parameters and grid
+            // are the launch's), each split into size buckets (the order is by descending size)
             std::vector<Lane::GClass> cls;
+            std::vector<int> ord = l->order;
             const long long lim[4] = {0, K4, K4 + K2, BA};
             for (int gi = 0; gi < 3; gi++) {
                 const int G = gi == 0 ? 4 : gi == 1 ? 2 : 1;
-                const long long a = lim[gi], b2 = lim[gi + 1];
-                if (b2 <= a) continue;
-                const int nsplit = (b2 - a) >= 96 ? (gi == 2 ? 3 : 2) : 1;
-                for (int sp = 0; sp < nsplit; sp++) {
-                    Lane::GClass cl;
-                    cl.G = G;
-                    long long s0 = a + (b2 - a) * sp / nsplit, s1 = a + (b2 - a) * (sp + 1) / nsplit;
-                    const int per = 4 / G;                         // problems per CTA
-                    if (sp > 0) s0 = a + ((s0 - a + per - 1) / per) * per;
-                    if (sp + 1 < nsplit) s1 = a + ((s1 - a + per - 1) / per) * per;
-                    if (s1 <= s0) continue;
-                    cl.r0 = (int)s0; cl.r1 = (int)s1;
-                    int Nm = 1, Mm = 1, nm = 1, Sm = 1;
-                    for (long long r = s0; r < s1; r++) {
-                        const ProbDesc &d = l->desc[l->order[r]];
-                        Nm = std::max(Nm, d.N); Mm = std::max(Mm, d.M); nm = std::max(nm, d.n); Sm = std::max(Sm, d.S);
+                if (lim[gi + 1] <= lim[gi]) continue;
+                std::stable_sort(ord.begin() + lim[gi], ord.begin() + lim[gi + 1], [&](int x, int y) { return l->env[x] < l->env[y]; });
+                for (long long a = lim[gi], b2; a < lim[gi + 1]; a = b2) {
+                    const int ce = l->env[ord[a]];
+                    for (b2 = a; b2 < lim[gi + 1] && l->env[ord[b2]] == ce; b2++) {}
+                    const DevParams &ep = c->envs[ce].dp;
+                    const int nsplit = (b2 - a) >= 96 ? (gi == 2 ? 3 : 2) : 1;
+                    for (int sp = 0; sp < nsplit; sp++) {
+                        Lane::GClass cl;
+                        cl.G = G; cl.env = ce;
+                        long long s0 = a + (b2 - a) * sp / nsplit, s1 = a + (b2 - a) * (sp + 1) / nsplit;
+                        const int per = 4 / G;                         // problems per CTA
+                        if (sp > 0) s0 = a + ((s0 - a + per - 1) / per) * per;
+                        if (sp + 1 < nsplit) s1 = a + ((s1 - a + per - 1) / per) * per;
+                        if (s1 <= s0) continue;
+                        cl.r0 = (int)s0; cl.r1 = (int)s1;
+                        int Nm = 1, Mm = 1, nm = 1, Sm = 1;
+                        for (long long r = s0; r < s1; r++) {
+                            const ProbDesc &d = l->desc[ord[r]];
+                            Nm = std::max(Nm, d.N); Mm = std::max(Mm, d.M); nm = std::max(nm, d.n); Sm = std::max(Sm, d.S);
+                        }
+                        cl.L = make_layout(Nm, Mm, nm, ep.mem_size, ep.past, ep.int_K, Sm);
+                        cl.smem = ((size_t)per * cl.L.total_doubles + (size_t)(4 - per) * RINGD) * sizeof(double);
+                        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cl.occ, solve_kernel, UALM_THREADS * UALM_WPB, cl.smem));
+                        cl.n_ctas = (int)((s1 - s0 + per - 1) / per);
+                        cls.push_back(cl);
                     }
-                    cl.L = make_layout(Nm, Mm, nm, c->dp.mem_size, c->dp.past, c->dp.int_K, Sm);
-                    cl.smem = ((size_t)per * cl.L.total_doubles + (size_t)(4 - per) * RINGD) * sizeof(double);
-                    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cl.occ, solve_kernel, UALM_THREADS * UALM_WPB, cl.smem));
-                    cl.n_ctas = (int)((s1 - s0 + per - 1) / per);
-                    cls.push_back(cl);
                 }
             }
             double sm_need = 0.0;
             for (auto &cl : cls) sm_need += (double)cl.n_ctas / std::max(cl.occ, 1);
             best = cls;
+            best_ord = ord;
             // multi-wave batches need not fit at once; batches meant to be fully resident must
             if (forced || 2LL * BA > W || sm_need <= 0.98 * dev_sms || attempt >= 12) break;
         }
         l->cls = best;
+        l->order = best_ord;
         l->wdesc.clear();
         for (auto &cl : l->cls) {
             cl.wd_off = l->wdesc.size();
@@ -497,12 +596,14 @@ extern "C" int ualm_upload(ualm_ctx_t *c, int B, const int32_t *N, const int32_t
                 fprintf(stderr, "[ualm] class G=%d: problems [%d,%d) %d CTAs, smem %zu B, %d CTAs/SM\n", cl.G, cl.r0, cl.r1, cl.n_ctas, cl.smem, cl.occ);
         }
     }
-    long long ox = 0, os = 0, ocx = 0, ocy = 0, oh = 0, oscr = 0, oixy = 0, oiyaw = 0, ofac = 0, ows = 0;
+    long long ox = 0, os = 0, ocx = 0, ocy = 0, oh = 0, oscr = 0, oixy = 0, oiyaw = 0, ofac = 0, ows = 0, oaux = 0;
     std::vector<double> x0;
     std::vector<ualm_result_t> res0(B);
     for (int b = 0; b < B; b++) {
         ProbDesc &d = l->desc[b];
+        const int m = c->envs[l->env[b]].dp.mem_size;
         d.off_x = ox; d.off_s = os; d.off_cxy = ocx; d.off_cyaw = ocy; d.off_hist = oh; d.off_scr = oscr; d.off_fac = ofac; d.off_ws = ows;
+        d.off_aux = oaux; oaux += 3LL * m;
         for (int k = 0; k < 18; k++) d.bnd[k] = bnd[(size_t)b * 18 + k];
         d.total_time = total_time[b];
         memset(&res0[b], 0, sizeof(ualm_result_t));
@@ -523,7 +624,8 @@ extern "C" int ualm_upload(ualm_ctx_t *c, int B, const int32_t *N, const int32_t
     CK(l->d_desc.ensure(B)); CK(l->d_order.ensure(BA)); CK(l->d_wdesc.ensure(l->wdesc.size())); CK(l->d_x0.ensure(ox)); CK(l->d_x.ensure(ox)); CK(l->d_grad.ensure(ox));
     CK(l->d_lambda.ensure(os)); CK(l->d_hx.ensure(os)); CK(l->d_mu.ensure(6 * os)); CK(l->d_gx.ensure(6 * os)); CK(l->d_scale_cx.ensure(7 * os));
     CK(l->d_lm_s.ensure(oh)); CK(l->d_lm_y.ensure(oh)); CK(l->d_scr.ensure(oscr));
-    CK(l->d_ws.ensure(ows)); CK(l->d_fac.ensure(ofac)); CK(l->d_lm_aux.ensure((size_t)std::max(B, 1) * 3 * m));
+    CK(l->d_ws.ensure(ows)); CK(l->d_fac.ensure(ofac)); CK(l->d_lm_aux.ensure((size_t)std::max(oaux, 1LL)));
+    CK(l->d_eidx.ensure(B));
     // factor arrays: entries outside the band-in-matrix positions (and the pad rows) are never written and must read 0
     if (ofac > 0) CK(cudaMemsetAsync(l->d_fac.p, 0, sizeof(double) * ofac, l->stream));
     CK(l->d_prof.ensure((size_t)std::max(B, 1) * UALM_NPROF));
@@ -532,6 +634,7 @@ extern "C" int ualm_upload(ualm_ctx_t *c, int B, const int32_t *N, const int32_t
     if (B > 0) {
         CK(cudaMemcpyAsync(l->d_desc.p, l->desc.data(), sizeof(ProbDesc) * B, cudaMemcpyHostToDevice, l->stream));
         if (BA > 0) CK(cudaMemcpyAsync(l->d_order.p, l->order.data(), sizeof(int) * BA, cudaMemcpyHostToDevice, l->stream));
+        CK(cudaMemcpyAsync(l->d_eidx.p, l->eidx.data(), sizeof(int) * B, cudaMemcpyHostToDevice, l->stream));
         if (!l->wdesc.empty()) CK(cudaMemcpyAsync(l->d_wdesc.p, l->wdesc.data(), sizeof(int4) * l->wdesc.size(), cudaMemcpyHostToDevice, l->stream));
         if (ox > 0) CK(cudaMemcpyAsync(l->d_x0.p, x0.data(), sizeof(double) * ox, cudaMemcpyHostToDevice, l->stream));
         // records of skipped problems (the kernels overwrite the others), zero coefficients and durations for them
@@ -552,12 +655,11 @@ extern "C" int ualm_solve_resident(ualm_ctx_t *c)
     if (!c) return fail(UALM_EINVAL, "null ctx");
     if (c->tp) TP_CALL(ualm_tp::tp_admit(c->tp, c->cur, err));      // joins the pool of running trajectories; ualm_sync / download drive the rounds
     Lane *l = c->b;
-    if (!c->have_map || !c->have_params || !l->have_batch) return fail(UALM_ESTATE, "set_params, set_map and upload must precede solve");
+    // (the upload checked that every environment of the batch is bound, and nothing unbinds one)
+    if (!l->have_batch) return fail(UALM_ESTATE, "set_params, set_map and upload must precede solve");
     CK(cudaSetDevice(c->device));
     l->last_launches = 0;
     CK(cudaMemcpyAsync(l->d_cancel, &c->h_flags[0], sizeof(int), cudaMemcpyHostToDevice, l->stream));   // no request carries over
-    DevParams dp = c->dp;
-    dp.cancel = l->d_cancel;
     CK(cudaEventRecord(l->ev0, l->stream));
     if (l->n_active > 0) {
         // the classes run concurrently: class 0 on the lane stream, the others on auxiliary streams
@@ -572,7 +674,11 @@ extern "C" int ualm_solve_resident(ualm_ctx_t *c)
             BatchPtrs bp = batch_ptrs(c);
             bp.wdesc = l->d_wdesc.p + cl.wd_off;
             bp.n_leader_slots = 4 / cl.G;
-            solve_kernel<<<cl.n_ctas, UALM_THREADS * UALM_WPB, cl.smem, st>>>(bp, dp, c->dm, cl.L);
+            // the class's environment: its parameters and grid are the launch's grid constants, the solve reads them as before
+            DevParams dp = c->envs[cl.env].dp;
+            dp.cancel = l->d_cancel;
+            dp.max_evals = c->max_evals;
+            solve_kernel<<<cl.n_ctas, UALM_THREADS * UALM_WPB, cl.smem, st>>>(bp, dp, c->envs[cl.env].dm, cl.L);
             CK(cudaGetLastError());
             l->last_launches++;
             if (ci > 0) { CK(cudaEventRecord(l->evs[ai], st)); CK(cudaStreamWaitEvent(l->stream, l->evs[ai], 0)); }
@@ -651,7 +757,13 @@ extern "C" int ualm_download(ualm_ctx_t *c, ualm_result_t *results, double *c_xy
 extern "C" int ualm_solve_batch(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
                                 const double *inner_xy, const double *inner_yaw, ualm_result_t *results, double *c_xy, double *c_yaw)
 {
-    int rc = ualm_upload(c, B, N, M, bnd, total_time, inner_xy, inner_yaw);
+    return ualm_solve_batch_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, nullptr, results, c_xy, c_yaw);
+}
+extern "C" int ualm_solve_batch_env(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
+                                    const double *inner_xy, const double *inner_yaw, const int32_t *env, ualm_result_t *results, double *c_xy,
+                                    double *c_yaw)
+{
+    int rc = ualm_upload_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env);
     if (rc) return rc;
     rc = ualm_solve_resident(c);
     if (rc) return rc;
@@ -663,13 +775,20 @@ extern "C" int ualm_solve_batch(ualm_ctx_t *c, int B, const int32_t *N, const in
 extern "C" int ualm_submit_batch(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
                                  const double *inner_xy, const double *inner_yaw, int depth, int *ticket)
 {
+    return ualm_submit_batch_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, nullptr, depth, ticket);
+}
+extern "C" int ualm_submit_batch_env(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
+                                     const double *inner_xy, const double *inner_yaw, const int32_t *env, int depth, int *ticket)
+{
     if (!c || !ticket) return fail(UALM_EINVAL, "null argument");
     if (depth < 1 || depth > UALM_MAX_LANES) return fail(UALM_EINVAL, "depth out of range [1, UALM_MAX_LANES]");
     const int lane = c->next_submit % depth;
     if (c->tp) {
         if (ualm_tp::tp_lane_in_flight(c->tp, lane)) return fail(UALM_ESTATE, "all lanes of this depth are in flight: ualm_wait_batch the oldest ticket first");
+        if (B < 0 || (B > 0 && (!N || !M || !bnd || !total_time))) return fail(UALM_EINVAL, "bad argument");
+        if (int rc = check_envs(c, B, env)) return rc;
         std::string em;
-        int rc = ualm_tp::tp_upload(c->tp, lane, B, N, M, bnd, total_time, inner_xy, inner_yaw, &em);
+        int rc = ualm_tp::tp_upload(c->tp, lane, B, N, M, env, bnd, total_time, inner_xy, inner_yaw, &em);
         if (!rc) rc = ualm_tp::tp_admit(c->tp, lane, &em);
         if (rc) return fail(rc, em);
         *ticket = lane; c->next_submit = (lane + 1) % depth;
@@ -678,7 +797,7 @@ extern "C" int ualm_submit_batch(ualm_ctx_t *c, int B, const int32_t *N, const i
     if (c->lanes[lane].in_flight) return fail(UALM_ESTATE, "all lanes of this depth are in flight: ualm_wait_batch the oldest ticket first");
     const int keep = c->cur;
     int rc = ualm_select_lane(c, lane);
-    if (!rc) rc = ualm_upload(c, B, N, M, bnd, total_time, inner_xy, inner_yaw);
+    if (!rc) rc = ualm_upload_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env);
     if (!rc) rc = ualm_solve_resident(c);
     if (!rc) { c->lanes[lane].in_flight = true; *ticket = lane; c->next_submit = (lane + 1) % depth; }
     c->cur = keep; c->b = &c->lanes[keep];
@@ -736,7 +855,7 @@ extern "C" int ualm_set_budget(ualm_ctx_t *c, int32_t max_evals)
     if (max_evals < 0) return fail(UALM_EINVAL, "max_evals must be >= 0 (0 = no budget)");
     if (c->tp) TP_CALL(ualm_tp::tp_set_budget(c->tp, max_evals, err));
     if (int rc = lanes_idle(c, "ualm_set_budget")) return rc;
-    c->dp.max_evals = max_evals;
+    c->max_evals = max_evals;
     return UALM_OK;
 }
 
@@ -748,10 +867,17 @@ extern "C" int ualm_solve_batch_multi(ualm_ctx_t **ctxs, int nctx, int B, const 
                                       const double *total_time, const double *inner_xy, const double *inner_yaw, ualm_result_t *results,
                                       double *c_xy, double *c_yaw)
 {
+    return ualm_solve_batch_multi_env(ctxs, nctx, B, N, M, bnd, total_time, inner_xy, inner_yaw, nullptr, results, c_xy, c_yaw);
+}
+extern "C" int ualm_solve_batch_multi_env(ualm_ctx_t **ctxs, int nctx, int B, const int32_t *N, const int32_t *M, const double *bnd,
+                                          const double *total_time, const double *inner_xy, const double *inner_yaw, const int32_t *env,
+                                          ualm_result_t *results, double *c_xy, double *c_yaw)
+{
     if (!ctxs || nctx < 1 || B < 0) return fail(UALM_EINVAL, "bad argument");
     for (int r = 0; r < nctx; r++) if (!ctxs[r]) return fail(UALM_EINVAL, "null ctx in list");
     if (B == 0) return UALM_OK;
     if (!N || !M || !bnd || !total_time) return fail(UALM_EINVAL, "null argument");
+    for (int r = 0; r < nctx; r++) if (int rc = check_envs(ctxs[r], B, env)) return rc;
     std::vector<long long> oxy(B + 1, 0), oyw(B + 1, 0), ocx(B + 1, 0), ocy(B + 1, 0);
     for (int b = 0; b < B; b++) {
         if (N[b] < 1 || M[b] < 1) return fail(UALM_EINVAL, "piece counts must be >= 1");
@@ -767,12 +893,12 @@ extern "C" int ualm_solve_batch_multi(ualm_ctx_t **ctxs, int nctx, int B, const 
         shard[(rnd % 2 == 0) ? k : nctx - 1 - k].push_back(ord[pos]);
     }
     for (auto &s : shard) std::sort(s.begin(), s.end());
-    struct Sub { std::vector<int32_t> N, M; std::vector<double> bnd, T, ixy, iyw, cxy, cyw; std::vector<ualm_result_t> res; };
+    struct Sub { std::vector<int32_t> N, M, E; std::vector<double> bnd, T, ixy, iyw, cxy, cyw; std::vector<ualm_result_t> res; };
     std::vector<Sub> sub(nctx);
     for (int r = 0; r < nctx; r++) {
         Sub &s = sub[r];
         for (int b : shard[r]) {
-            s.N.push_back(N[b]); s.M.push_back(M[b]); s.T.push_back(total_time[b]);
+            s.N.push_back(N[b]); s.M.push_back(M[b]); s.T.push_back(total_time[b]); s.E.push_back(env ? env[b] : 0);
             s.bnd.insert(s.bnd.end(), bnd + 18 * (size_t)b, bnd + 18 * (size_t)b + 18);
             if (oxy[b + 1] > oxy[b]) s.ixy.insert(s.ixy.end(), inner_xy + oxy[b], inner_xy + oxy[b + 1]);
             if (oyw[b + 1] > oyw[b]) s.iyw.insert(s.iyw.end(), inner_yaw + oyw[b], inner_yaw + oyw[b + 1]);
@@ -786,7 +912,8 @@ extern "C" int ualm_solve_batch_multi(ualm_ctx_t **ctxs, int nctx, int B, const 
     // upload + launch everywhere first (asynchronous per device), then collect
     for (int r = 0; r < nctx; r++) {
         if (shard[r].empty()) continue;
-        int rc = ualm_upload(ctxs[r], (int)shard[r].size(), sub[r].N.data(), sub[r].M.data(), sub[r].bnd.data(), sub[r].T.data(), sub[r].ixy.data(), sub[r].iyw.data());
+        int rc = ualm_upload_env(ctxs[r], (int)shard[r].size(), sub[r].N.data(), sub[r].M.data(), sub[r].bnd.data(), sub[r].T.data(), sub[r].ixy.data(),
+                                 sub[r].iyw.data(), sub[r].E.data());
         if (!rc) rc = ualm_solve_resident(ctxs[r]);
         if (rc) return rc;
     }
@@ -856,7 +983,7 @@ extern "C" int ualm_eval_batch(ualm_ctx_t *c, const double *x, const double *lam
                                double *c_yaw)
 {
     if (c && c->tp) TP_CALL(ualm_tp::tp_eval(c->tp, c->cur, x, lambda, mu, scale_cx, scale_fx, rho, f, grad, hx, gx, c_xy, c_yaw, err));
-    if (!c || !c->b->have_batch || !c->have_map) return fail(UALM_ESTATE, "upload and set_map first");
+    if (!c || !c->b->have_batch) return fail(UALM_ESTATE, "upload and set_map first");
     Lane *l = c->b;
     if (l->n_active != l->B) return fail(UALM_ELIMIT, "ualm_eval_batch: the uploaded batch holds problems over the compiled limits");
     CK(cudaSetDevice(c->device));
@@ -867,8 +994,10 @@ extern "C" int ualm_eval_batch(ualm_ctx_t *c, const double *x, const double *lam
     if ((rc = put(c, l->d_scale_cx.p, scale_cx, 7 * l->tot_s, 1.0))) return rc;
     if ((rc = put(c, l->d_sfx.p, scale_fx, l->B, 1.0))) return rc;
     if (l->B > 0) {
-        eval_kernel<<<(l->B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->smem_bytes, l->stream>>>(batch_ptrs(c), c->dp, c->dm, l->L, rho);
-        CK(cudaGetLastError());
+        if ((rc = per_env(c, [&](int e, const BatchPtrs &bp, int cnt) {
+                 eval_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].dm, l->eL[e], rho);
+             })))
+            return rc;
         if (f) CK(cudaMemcpyAsync(f, l->d_f.p, sizeof(double) * l->B, cudaMemcpyDeviceToHost, l->stream));
         if (grad) CK(cudaMemcpyAsync(grad, l->d_grad.p, sizeof(double) * l->tot_x, cudaMemcpyDeviceToHost, l->stream));
         if (hx) CK(cudaMemcpyAsync(hx, l->d_hx.p, sizeof(double) * l->tot_s, cudaMemcpyDeviceToHost, l->stream));
@@ -883,13 +1012,15 @@ extern "C" int ualm_eval_batch(ualm_ctx_t *c, const double *x, const double *lam
 extern "C" int ualm_init_scaling_batch(ualm_ctx_t *c, double *scale_fx, double *scale_cx)
 {
     if (c && c->tp) TP_CALL(ualm_tp::tp_init_scaling(c->tp, c->cur, scale_fx, scale_cx, err));
-    if (!c || !c->b->have_batch || !c->have_map) return fail(UALM_ESTATE, "upload and set_map first");
+    if (!c || !c->b->have_batch) return fail(UALM_ESTATE, "upload and set_map first");
     Lane *l = c->b;
     if (l->n_active != l->B) return fail(UALM_ELIMIT, "ualm_init_scaling_batch: the uploaded batch holds problems over the compiled limits");
     CK(cudaSetDevice(c->device));
     if (l->B > 0) {
-        scaling_kernel<<<(l->B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->smem_bytes, l->stream>>>(batch_ptrs(c), c->dp, c->dm, l->L);
-        CK(cudaGetLastError());
+        if (int rc = per_env(c, [&](int e, const BatchPtrs &bp, int cnt) {
+                scaling_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].dm, l->eL[e]);
+            }))
+            return rc;
         if (scale_fx) CK(cudaMemcpyAsync(scale_fx, l->d_sfx.p, sizeof(double) * l->B, cudaMemcpyDeviceToHost, l->stream));
         if (scale_cx) CK(cudaMemcpyAsync(scale_cx, l->d_scale_cx.p, sizeof(double) * 7 * l->tot_s, cudaMemcpyDeviceToHost, l->stream));
     }
@@ -901,9 +1032,11 @@ extern "C" int ualm_time_penalty_kernel(ualm_ctx_t *c, int reps, float *ms_per_l
 {
     if (reps < 1) return fail(UALM_EINVAL, "reps < 1");
     if (c && c->tp) TP_CALL(ualm_tp::tp_time_penalty(c->tp, c->cur, reps, (getenv("UALM_TP_TMA") && atoi(getenv("UALM_TP_TMA"))) ? 1 : 0, ms_per_launch, algorithmic_bytes, err));
-    if (!c || !c->b->have_batch || !c->have_map) return fail(UALM_ESTATE, "upload and set_map first");
+    if (!c || !c->b->have_batch) return fail(UALM_ESTATE, "upload and set_map first");
     Lane *l = c->b;
     if (l->n_active != l->B) return fail(UALM_ELIMIT, "ualm_time_penalty_kernel: the uploaded batch holds problems over the compiled limits");
+    for (int b = 1; b < l->B; b++)
+        if (l->env[b] != l->env[0]) return fail(UALM_EINVAL, "ualm_time_penalty_kernel: the uploaded batch mixes environments");
     if (ms_per_launch) *ms_per_launch = 0.f;
     if (algorithmic_bytes) *algorithmic_bytes = 0.0;
     if (l->B == 0) return UALM_OK;
@@ -912,9 +1045,11 @@ extern "C" int ualm_time_penalty_kernel(ualm_ctx_t *c, int reps, float *ms_per_l
     if ((rc = put(c, l->d_lambda.p, nullptr, l->tot_s, 0.0))) return rc;
     if ((rc = put(c, l->d_mu.p, nullptr, 6 * l->tot_s, 0.0))) return rc;
     if ((rc = put(c, l->d_scale_cx.p, nullptr, 7 * l->tot_s, 1.0))) return rc;
-    penalty_only_kernel<<<(l->B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->smem_bytes, l->stream>>>(batch_ptrs(c), c->dp, c->dm, l->L, 1); // warm-up
+    const int e = l->env[0];
+    const BatchPtrs bp = batch_ptrs(c);
+    penalty_only_kernel<<<(l->B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].dm, l->eL[e], 1); // warm-up
     CK(cudaEventRecord(l->ev0, l->stream));
-    penalty_only_kernel<<<(l->B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->smem_bytes, l->stream>>>(batch_ptrs(c), c->dp, c->dm, l->L, reps);
+    penalty_only_kernel<<<(l->B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].dm, l->eL[e], reps);
     CK(cudaEventRecord(l->ev1, l->stream));
     CK(cudaGetLastError());
     CK(cudaEventSynchronize(l->ev1));
@@ -961,9 +1096,41 @@ __global__ void piece_T_from_results(const ualm_result_t *res, int B, double *pi
 }
 } // namespace ualm
 
+// feasibility_kernel over a batch whose problem b is in environment env[b]: one launch with that environment's parameters and grid
+// when there is only one, else one launch per environment over its problem indices
+static int feasibility_launch(ualm_ctx *c, const BatchPtrs &bp, int B, const int32_t *env, double dt, double *d_out, cudaStream_t st)
+{
+    bool mixed = false;
+    for (int b = 1; b < B; b++) mixed = mixed || env[b] != env[0];
+    if (!mixed) {
+        const Env &v = c->envs[B > 0 ? env[0] : 0];
+        feasibility_kernel<<<(B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(bp, v.dp, v.dm, dt, d_out, nullptr, B);
+        CK(cudaGetLastError());
+        return UALM_OK;
+    }
+    struct Tmp { DevBuf<int> idx; ~Tmp() { idx.release(); } } t;
+    std::vector<int> idx;
+    int off[UALM_MAX_ENVS + 1];
+    for (int e = 0; e < UALM_MAX_ENVS; e++) {
+        off[e] = (int)idx.size();
+        for (int b = 0; b < B; b++) if (env[b] == e) idx.push_back(b);
+    }
+    off[UALM_MAX_ENVS] = (int)idx.size();
+    CK(t.idx.ensure(idx.size()));
+    CK(cudaMemcpyAsync(t.idx.p, idx.data(), sizeof(int) * idx.size(), cudaMemcpyHostToDevice, st));
+    for (int e = 0; e < UALM_MAX_ENVS; e++) {
+        const int cnt = off[e + 1] - off[e];
+        if (cnt == 0) continue;
+        feasibility_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(bp, c->envs[e].dp, c->envs[e].dm, dt, d_out, t.idx.p + off[e], cnt);
+        CK(cudaGetLastError());
+    }
+    CK(cudaStreamSynchronize(st));       // idx and its device copy are local
+    return UALM_OK;
+}
+
 // the scan over coefficients that already sit on the device (B problems, ragged offsets from N / M, piece durations from the records)
-static int feasibility_from_device(ualm_ctx *c, int B, const int32_t *N, const int32_t *M, const ualm_result_t *d_res, const double *d_cxy, const double *d_cyaw,
-                                   double dt, double *out10)
+static int feasibility_from_device(ualm_ctx *c, int B, const int32_t *N, const int32_t *M, const int32_t *env, const ualm_result_t *d_res, const double *d_cxy,
+                                   const double *d_cyaw, double dt, double *out10)
 {
     struct Tmp { DevBuf<ProbDesc> desc; DevBuf<double> pt, feas; ~Tmp() { desc.release(); pt.release(); feas.release(); } } t;
     std::vector<ProbDesc> desc(B);
@@ -980,8 +1147,7 @@ static int feasibility_from_device(ualm_ctx *c, int B, const int32_t *N, const i
     BatchPtrs bp;
     memset(&bp, 0, sizeof(bp));
     bp.B = B; bp.desc = t.desc.p; bp.c_xy = const_cast<double *>(d_cxy); bp.c_yaw = const_cast<double *>(d_cyaw); bp.piece_T = t.pt.p;
-    feasibility_kernel<<<(B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB>>>(bp, c->dp, c->dm, dt, t.feas.p);
-    CK(cudaGetLastError());
+    if (int rc = feasibility_launch(c, bp, B, env, dt, t.feas.p, 0)) return rc;
     CK(cudaMemcpy(out10, t.feas.p, sizeof(double) * 10 * B, cudaMemcpyDeviceToHost));
     return UALM_OK;
 }
@@ -991,20 +1157,18 @@ extern "C" int ualm_feasibility_batch(ualm_ctx_t *c, double dt, double *out10)
     if (!c || !out10 || !(dt > 0.0)) return fail(UALM_EINVAL, "null argument or dt <= 0");
     if (c->tp) {
         const ualm_result_t *d_res; const double *d_cxy, *d_cyaw;
-        int B = 0; const int32_t *N = nullptr, *M = nullptr;
-        if (ualm_tp::tp_lane_outputs(c->tp, c->cur, &d_res, &d_cxy, &d_cyaw, &B, &N, &M) != UALM_OK)
+        int B = 0; const int32_t *N = nullptr, *M = nullptr, *E = nullptr;
+        if (ualm_tp::tp_lane_outputs(c->tp, c->cur, &d_res, &d_cxy, &d_cyaw, &B, &N, &M, &E) != UALM_OK)
             return fail(UALM_ESTATE, "ualm_feasibility_batch needs a solved, collected batch (ualm_sync / ualm_download first)");
         CK(cudaSetDevice(c->device));
         if (B == 0) return UALM_OK;
-        return feasibility_from_device(c, B, N, M, d_res, d_cxy, d_cyaw, dt, out10);
+        return feasibility_from_device(c, B, N, M, E, d_res, d_cxy, d_cyaw, dt, out10);
     }
     Lane *l = c->b;
-    if (!c->have_map || !c->have_params || !l->have_batch || !l->solved) return fail(UALM_ESTATE, "ualm_feasibility_batch needs a solved resident batch");
+    if (!l->have_batch || !l->solved) return fail(UALM_ESTATE, "ualm_feasibility_batch needs a solved resident batch");
     CK(cudaSetDevice(c->device));
     if (l->B == 0) return UALM_OK;
-    const BatchPtrs bp = batch_ptrs(c);
-    feasibility_kernel<<<(l->B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, l->stream>>>(bp, c->dp, c->dm, dt, l->d_feas.p);
-    CK(cudaGetLastError());
+    if (int rc = feasibility_launch(c, batch_ptrs(c), l->B, l->env.data(), dt, l->d_feas.p, l->stream)) return rc;
     CK(cudaMemcpyAsync(out10, l->d_feas.p, sizeof(double) * 10 * l->B, cudaMemcpyDeviceToHost, l->stream));
     CK(cudaStreamSynchronize(l->stream));
     return UALM_OK;
@@ -1042,8 +1206,8 @@ extern "C" int ualm_mpc_export_batch(ualm_ctx_t *c, double dt, const double *ini
     if (!c || !(dt > 0.0)) return fail(UALM_EINVAL, "null ctx or dt <= 0");
     if (c->tp) {
         const ualm_result_t *d_res; const double *d_cxy, *d_cyaw;
-        int B = 0; const int32_t *N = nullptr, *M = nullptr;
-        if (ualm_tp::tp_lane_outputs(c->tp, c->cur, &d_res, &d_cxy, &d_cyaw, &B, &N, &M) != UALM_OK)
+        int B = 0; const int32_t *N = nullptr, *M = nullptr, *E = nullptr;     // (the hand-over reads no parameter and no grid)
+        if (ualm_tp::tp_lane_outputs(c->tp, c->cur, &d_res, &d_cxy, &d_cyaw, &B, &N, &M, &E) != UALM_OK)
             return fail(UALM_ESTATE, "ualm_mpc_export_batch needs a solved, collected batch (ualm_sync / ualm_download first)");
         CK(cudaSetDevice(c->device));
         if (B == 0) return UALM_OK;

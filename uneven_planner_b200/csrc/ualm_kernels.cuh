@@ -90,6 +90,7 @@ struct ProbDesc {
     long long off_scr;    // UALM_NFIELD * S per-sample scratch
     long long off_fac;    // factor arrays: Fxy ((6N + 2 pad) rows), Fyaw ((6M + 2 pad) rows), UALM_FW doubles per row
     long long off_ws;     // initScaling adjoint workspace (12 N + 6 M) * 32
+    long long off_aux;    // 3 * mem_size of the problem's environment (lm_aux)
     R bnd[18];
     R total_time;
 };
@@ -106,7 +107,7 @@ struct BatchPtrs {
     R *x;                    // packed final decision vectors
     R *lambda, *mu, *scale_cx, *hx, *gx;
     R *lm_s, *lm_y;
-    R *lm_aux;               // per problem 3 * mem_size: lm_alpha | lm_ys | RN(1 / lm_ys)
+    R *lm_aux;               // per problem 3 * mem_size at off_aux: lm_alpha | lm_ys | RN(1 / lm_ys)
     R *scratch;
     R *fac;                  // LU factors
     R *ws_scaling;           // initScaling adjoint workspace
@@ -2020,7 +2021,7 @@ __device__ UALM_NOINLINE void traj_setup(Traj &t, const BatchPtrs &bp, const Dev
     t.mu = bp.mu + 6 * pd->off_s; t.gx = bp.gx + 6 * pd->off_s;
     t.scale_cx = bp.scale_cx + 7 * pd->off_s;
     t.lm_s = bp.lm_s + pd->off_hist; t.lm_y = bp.lm_y + pd->off_hist;
-    t.lm_alpha = bp.lm_aux + (size_t)prob * 3 * p.mem_size; t.lm_ys = t.lm_alpha + p.mem_size; t.lm_rys = t.lm_ys + p.mem_size;
+    t.lm_alpha = bp.lm_aux + pd->off_aux; t.lm_ys = t.lm_alpha + p.mem_size; t.lm_rys = t.lm_ys + p.mem_size;
     t.scr = bp.scratch + pd->off_scr;
     {
         const long long rx = 6 * pd->N + 2 * UALM_FPAD, ry = 6 * pd->M + 2 * UALM_FPAD;
@@ -2308,11 +2309,13 @@ struct AbsMax {   // "if (fabs(best) < fabs(v)) best = v" over samples in time o
         }
     }
 };
+// idx: the n problems to scan (those of one environment, whose parameters and grid this launch carries), or null for 0 .. n - 1
 __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) feasibility_kernel(const __grid_constant__ BatchPtrs bp, const __grid_constant__ DevParams p,
-        const __grid_constant__ DevMap map, R dt, R *out)
+        const __grid_constant__ DevMap map, R dt, R *out, const int *idx, int n)
 {
-    const int lane = threadIdx.x & 31, prob = blockIdx.x * UALM_WPB + (threadIdx.x >> 5);
-    if (prob >= bp.B) return;   // whole warp exits
+    const int lane = threadIdx.x & 31, w = blockIdx.x * UALM_WPB + (threadIdx.x >> 5);
+    if (w >= n) return;         // whole warp exits
+    const int prob = idx ? idx[w] : w;
     const ProbDesc *pd = bp.desc + prob;
     if (pd->S == 0) {            // over the compiled limits: not solved (ret_code = UALM_ELIMIT)
         if (lane < 10) out[10 * (size_t)prob + lane] = 0.0;

@@ -38,10 +38,13 @@ struct Buf {
     void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 };
 
+static_assert(TP_SUBGROUPS >= UALM_MAX_ENVS, "a lane runs the problems of environment k in its group k: one group per environment");
+
 struct TpLane {
     bool have_batch = false, in_flight = false, collected = false;
     int B = 0, Nmax = 1, Mmax = 1, mode = 0;
-    std::vector<int32_t> N, M;
+    std::vector<int32_t> N, M, env;
+    bool mixed = false;               // the batch holds problems of more than one environment
     std::vector<int> slots;
     std::vector<AdmitDesc> ad;
     std::vector<GatherDesc> gd;
@@ -63,13 +66,16 @@ struct TpEngine {
     size_t esz() const { return precision == 32 ? 4 : 8; }
     cudaStream_t stream = nullptr;
     cudaEvent_t evA = nullptr, evB = nullptr;
-    bool have_params = false, have_map = false;
-    TpParams p;
-    TpMap map;
-    CUtensorMap tmap;
-    bool have_tmap = false;
+    // environments (ualm_select_env): parameters, grid and its TMA descriptor of each; group g runs with those of genv[g]
+    bool have_params[UALM_MAX_ENVS] = {}, have_map[UALM_MAX_ENVS] = {};
+    TpParams p[UALM_MAX_ENVS];
+    TpMap map[UALM_MAX_ENVS];
+    CUtensorMap tmap[UALM_MAX_ENVS];
+    bool have_tmap[UALM_MAX_ENVS] = {};
+    int genv[TP_NGROUPS] = {};
+    int max_evals = 0;
     int use_tma = 0;              // map corners of kb_kernel: 0 = direct gather through L1 (default: measured faster), 1 = TMA-staged tiles (UALM_TP_TMA=1)
-    Buf<float4> cells;
+    Buf<float4> cells[UALM_MAX_ENVS];
     // pool
     TpPool E;
     int capacity = 0;
@@ -214,7 +220,8 @@ void tp_destroy(TpEngine *e)
         if (l.ev0) cudaEventDestroy(l.ev0);
         if (l.ev1) cudaEventDestroy(l.ev1);
     }
-    e->cells.release(); e->st.release(); e->active.release(); e->n_active.release(); e->remaining.release(); e->cancel.release(); e->vec.release(); e->cd.release(); e->gw.release();
+    for (auto &b : e->cells) b.release();
+    e->st.release(); e->active.release(); e->n_active.release(); e->remaining.release(); e->cancel.release(); e->vec.release(); e->cd.release(); e->gw.release();
     e->kb_cost.release(); e->lm_ys.release(); e->lm_alpha.release(); e->cr.release(); e->gdc.release(); e->gdt.release(); e->dual.release();
     e->hs.release(); e->hy.release(); e->wway.release(); e->wf.release(); e->wt.release(); e->wf_off.release(); e->wway_off.release();
     if (e->h_remaining) cudaFreeHost(e->h_remaining);
@@ -230,49 +237,65 @@ static bool any_in_flight(TpEngine *e)
     return false;
 }
 
-int tp_set_params(TpEngine *e, const ualm_params_t *p, std::string *err)
+// the pool strides are sized by the largest int_K and mem_size over the bound environments
+static int max_K(const TpEngine *e)
+{
+    int K = 1;
+    for (int v = 0; v < UALM_MAX_ENVS; v++) if (e->have_params[v]) K = std::max(K, e->p[v].int_K);
+    return K;
+}
+static int max_m(const TpEngine *e)
+{
+    int m = 1;
+    for (int v = 0; v < UALM_MAX_ENVS; v++) if (e->have_params[v]) m = std::max(m, e->p[v].mem_size);
+    return m;
+}
+
+int tp_set_params(TpEngine *e, int env, const ualm_params_t *p, std::string *err)
 {
     if (p->int_K < 1 || p->int_K > TP_KB_THREADS - 1) { if (err) *err = "int_K out of range [1,127] on the throughput path"; return UALM_ELIMIT; }
     if (p->mem_size < 1 || p->mem_size > 1024) { if (err) *err = "mem_size out of range [1,1024]"; return UALM_ELIMIT; }
     if (p->past < 0 || p->past > 16) { if (err) *err = "past out of range [0,16]"; return UALM_ELIMIT; }
     if (any_in_flight(e)) { if (err) *err = "ualm_set_params while a batch is in flight"; return UALM_ESTATE; }
-    TpParams &d = e->p;
+    TpParams &d = e->p[env];
     d.rho_T = p->rho_T; d.rho_ter = p->rho_ter; d.max_vel = p->max_vel; d.max_acc_lon = p->max_acc_lon; d.max_acc_lat = p->max_acc_lat;
     d.max_kap = p->max_kap; d.min_cxi = p->min_cxi; d.max_sig = p->max_sig; d.use_scaling = p->use_scaling; d.rho = p->rho;
     d.beta = p->beta; d.gamma = p->gamma; d.epsilon_con = p->epsilon_con; d.max_iter = p->max_iter; d.g_epsilon = p->g_epsilon;
     d.min_step = p->min_step; d.delta = p->delta; d.inner_max_iter = (int)p->inner_max_iter; d.mem_size = p->mem_size; d.past = p->past;
-    d.int_K = p->int_K; d.gravity = p->gravity;
-    e->have_params = true;
-    // the pool strides depend on int_K and mem_size: it is rebuilt at the next admission; uploaded batches stay valid (they hold
-    // problem data only), but nothing may be resident in the pool
+    d.int_K = p->int_K; d.gravity = p->gravity; d.max_evals = e->max_evals;
+    e->have_params[env] = true;
+    // the pool strides depend on the largest int_K and mem_size: it is rebuilt at the next admission.  The uploaded batches' sample
+    // offsets depend on int_K: they are invalidated, as on the parity path (upload again)
     e->capacity = 0; e->free_slots.clear(); e->live = 0;
     for (int g = 0; g < TP_NGROUPS; g++) { e->glive[g] = 0; e->gscale[g] = 0; e->gcompact[g] = false; }
-    for (auto &l : e->lanes) { l.collected = false; }
+    for (auto &l : e->lanes) { l.collected = false; l.have_batch = false; }
     return UALM_OK;
 }
 
 int tp_set_budget(TpEngine *e, int max_evals, std::string *err)
 {
     if (any_in_flight(e)) { if (err) *err = "ualm_set_budget while a batch is in flight"; return UALM_ESTATE; }
-    e->p.max_evals = max_evals;
+    e->max_evals = max_evals;
+    for (auto &p : e->p) p.max_evals = max_evals;
     return UALM_OK;
 }
 
-int tp_set_map(TpEngine *e, const ualm_map_geom_t *g, const float *cells, std::string *err)
+int tp_set_map(TpEngine *e, int env, const ualm_map_geom_t *g, const float *cells, std::string *err)
 {
     if (any_in_flight(e)) { if (err) *err = "ualm_set_map while a batch is in flight"; return UALM_ESTATE; }
+    e->have_map[env] = false;     // until the grid below is complete
     TCK(cudaSetDevice(e->device));
     TCK(cudaStreamSynchronize(e->stream));
     const size_t ncell = (size_t)g->voxel_num[0] * g->voxel_num[1] * g->voxel_num[2];
-    TCK(e->cells.ensure(ncell));
-    TCK(cudaMemcpy(e->cells.p, cells, ncell * sizeof(float4), cudaMemcpyHostToDevice));
-    TpMap &m = e->map;
-    m.cells = e->cells.p;
+    TCK(e->cells[env].ensure(ncell));
+    TCK(cudaMemcpy(e->cells[env].p, cells, ncell * sizeof(float4), cudaMemcpyHostToDevice));
+    TpMap &m = e->map[env];
+    m.cells = e->cells[env].p;
     for (int k = 0; k < 3; k++) { m.vn[k] = g->voxel_num[k]; m.origin[k] = g->origin[k]; m.maxb[k] = g->max_boundary[k]; }
     m.xy_res = g->xy_resolution; m.yaw_res = g->yaw_resolution; m.xy_inv = 1.0 / g->xy_resolution; m.yaw_inv = 1.0 / g->yaw_resolution;
     // TMA descriptor of the grid: a 3-D float tensor {4 * Yaw, Y, X} (innermost first), box = 8 yaw layers x 8 x 8 cells
-    e->have_tmap = false;
-    memset(&e->tmap, 0, sizeof(e->tmap));
+    e->have_tmap[env] = false;
+    memset(&e->tmap[env], 0, sizeof(e->tmap[env]));
     typedef CUresult (*EncodeFn)(CUtensorMap *, CUtensorMapDataType, cuuint32_t, void *, const cuuint64_t *, const cuuint64_t *, const cuuint32_t *, const cuuint32_t *,
                                  CUtensorMapInterleave, CUtensorMapSwizzle, CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
     void *fn = nullptr;
@@ -282,19 +305,21 @@ int tp_set_map(TpEngine *e, const ualm_map_geom_t *g, const float *cells, std::s
         const cuuint64_t strides[2] = {(cuuint64_t)16 * g->voxel_num[2], (cuuint64_t)16 * g->voxel_num[2] * g->voxel_num[1]};
         const cuuint32_t box[3] = {4 * TP_TILE, TP_TILE, TP_TILE};
         const cuuint32_t estr[3] = {1, 1, 1};
-        const CUresult r = ((EncodeFn)fn)(&e->tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void *)e->cells.p, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                                          CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-        e->have_tmap = (r == CUDA_SUCCESS) && g->voxel_num[2] >= TP_TILE && g->voxel_num[1] >= TP_TILE && g->voxel_num[0] >= TP_TILE;
+        const CUresult r = ((EncodeFn)fn)(&e->tmap[env], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void *)e->cells[env].p, dims, strides, box, estr,
+                                          CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                                          CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+        e->have_tmap[env] = (r == CUDA_SUCCESS) && g->voxel_num[2] >= TP_TILE && g->voxel_num[1] >= TP_TILE && g->voxel_num[0] >= TP_TILE;
     }
-    if (getenv("UALM_DEBUG")) fprintf(stderr, "[ualm-tp] tensor map %s, TMA staging %s\n", e->have_tmap ? "encoded" : "unavailable", (e->have_tmap && e->use_tma) ? "on" : "off");
-    e->have_map = true;
+    if (getenv("UALM_DEBUG"))
+        fprintf(stderr, "[ualm-tp] env %d: tensor map %s, TMA staging %s\n", env, e->have_tmap[env] ? "encoded" : "unavailable", (e->have_tmap[env] && e->use_tma) ? "on" : "off");
+    e->have_map[env] = true;
     return UALM_OK;
 }
 
 // (re)allocate the pool for `cap` slots with the current parameters; only when nothing is resident
 static int pool_alloc(TpEngine *e, int cap, std::string *err)
 {
-    const int K = e->p.int_K, m = e->p.mem_size;
+    const int K = max_K(e), m = max_m(e);
     const size_t Smax = (size_t)TP_NMAX * (K + 1), es = e->esz();
     TCK(e->st.ensure(cap)); TCK(e->active.ensure((size_t)cap * TP_NGROUPS));
     TCK(e->vec.ensure((size_t)cap * 5 * TP_NVAR)); TCK(e->cd.ensure((size_t)cap * TP_CSTRIDE)); TCK(e->gw.ensure((size_t)cap * TP_CSTRIDE));
@@ -324,13 +349,17 @@ static int pool_alloc(TpEngine *e, int cap, std::string *err)
     return UALM_OK;
 }
 
-int tp_upload(TpEngine *e, int lane, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time, const double *inner_xy,
-              const double *inner_yaw, std::string *err)
+int tp_upload(TpEngine *e, int lane, int B, const int32_t *N, const int32_t *M, const int32_t *env, const double *bnd, const double *total_time,
+              const double *inner_xy, const double *inner_yaw, std::string *err)
 {
     if (lane < 0 || lane >= TP_LANES) { if (err) *err = "lane out of range"; return UALM_EINVAL; }
-    if (!e->have_params) { if (err) *err = "ualm_set_params must be called before ualm_upload"; return UALM_ESTATE; }
     TpLane &l = e->lanes[lane];
     if (l.in_flight) { if (err) *err = "ualm_upload into a lane whose batch is still in flight"; return UALM_ESTATE; }
+    for (int b = 0; b < (env ? B : 1); b++) {       // the engine's own state: every environment used has parameters and a grid
+        const int v = env ? env[b] : 0;
+        if (v < 0 || v >= UALM_MAX_ENVS) { if (err) *err = "env index out of range [0, UALM_MAX_ENVS)"; return UALM_EINVAL; }
+        if (!e->have_params[v] || !e->have_map[v]) { if (err) *err = "environment " + std::to_string(v) + " has no parameters or no map grid bound"; return UALM_ESTATE; }
+    }
     long long need_xy = 0, need_yaw = 0;
     for (int b = 0; b < B; b++) {
         if (N[b] < 1 || M[b] < 1) { if (err) *err = "piece counts must be >= 1"; return UALM_EINVAL; }
@@ -339,9 +368,12 @@ int tp_upload(TpEngine *e, int lane, int B, const int32_t *N, const int32_t *M, 
     }
     if ((need_xy > 0 && !inner_xy) || (need_yaw > 0 && !inner_yaw)) { if (err) *err = "inner waypoint arrays are NULL but N > 1 or M > 1"; return UALM_EINVAL; }
     TCK(cudaSetDevice(e->device));
-    const int K = e->p.int_K;
     l.have_batch = false; l.collected = false;
     l.B = B; l.N.assign(N, N + B); l.M.assign(M, M + B); l.ad.assign(B, AdmitDesc()); l.gd.assign(B, GatherDesc());
+    l.env.assign(B, 0);
+    if (env) l.env.assign(env, env + B);
+    l.mixed = false;
+    for (int b = 1; b < B; b++) l.mixed = l.mixed || l.env[b] != l.env[0];
     l.Nmax = l.Mmax = 1;
     std::vector<double> x0;
     std::vector<long long> offs(B + 1, 0);
@@ -361,7 +393,7 @@ int tp_upload(TpEngine *e, int lane, int B, const int32_t *N, const int32_t *M, 
             x0.push_back(T > 1.0 ? (std::sqrt(2.0 * T - 1.0) - 1.0) : (1.0 - std::sqrt(2.0 / T - 1.0)));   // logC2, alm_traj_opt.h:238-241
             for (long long q = 0; q < nxy; q++) x0.push_back(inner_xy[oixy + q]);
             for (long long q = 0; q < nyw; q++) x0.push_back(inner_yaw[oiyw + q]);
-            ox += 1 + nxy + nyw; os += (long long)N[b] * (K + 1);
+            ox += 1 + nxy + nyw; os += (long long)N[b] * (e->p[l.env[b]].int_K + 1);
             l.Nmax = std::max(l.Nmax, (int)N[b]); l.Mmax = std::max(l.Mmax, (int)M[b]);
         }
         oixy += nxy; oiyw += nyw;
@@ -382,7 +414,9 @@ int tp_upload(TpEngine *e, int lane, int B, const int32_t *N, const int32_t *M, 
 static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, std::string *err)
 {
     TpLane &l = e->lanes[lane];
-    if (!e->have_params || !e->have_map || !l.have_batch) { if (err) *err = "set_params, set_map and upload must precede the solve"; return UALM_ESTATE; }
+    if (!l.have_batch) { if (err) *err = "set_params, set_map and upload must precede the solve"; return UALM_ESTATE; }
+    for (int b = 0; b < l.B; b++)
+        if (!e->have_map[l.env[b]]) { if (err) *err = "environment " + std::to_string(l.env[b]) + " has no map grid bound"; return UALM_ESTATE; }
     if (l.in_flight) { if (err) *err = "lane already in flight"; return UALM_ESTATE; }
     TCK(cudaSetDevice(e->device));
     int need = 0;
@@ -393,7 +427,7 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, std::s
     {
         size_t free_b = 0, total_b = 0;
         TCK(cudaMemGetInfo(&free_b, &total_b));
-        const double per_slot = 5.0 * TP_NVAR * 8 + 3.0 * TP_CSTRIDE * 8 + (double)TP_NDUAL * TP_NMAX * (e->p.int_K + 1) * e->esz() + 2.0 * e->p.mem_size * TP_NVAR * e->esz();
+        const double per_slot = 5.0 * TP_NVAR * 8 + 3.0 * TP_CSTRIDE * 8 + (double)TP_NDUAL * TP_NMAX * (max_K(e) + 1) * e->esz() + 2.0 * max_m(e) * TP_NVAR * e->esz();
         while (mult > 1 && per_slot * mult * need > 0.75 * free_b) mult /= 2;
     }
     if (e->live == 0 && e->capacity < mult * need) {
@@ -414,19 +448,29 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, std::s
         const int s = e->free_slots.back();
         e->free_slots.pop_back();
         l.slots.push_back(s);
-        const int g = lane * TP_SUBGROUPS + (single_group ? 0 : k % e->sg);
+        // a batch of one environment is dealt over the lane's e->sg groups; in a mixed batch group k runs environment k
+        const int g = lane * TP_SUBGROUPS + (l.mixed ? l.env[b] : single_group ? 0 : k % e->sg);
         l.ad[b].slot = s; l.ad[b].mode = mode; l.ad[b].group = g; l.gd[b].slot = s;
         e->glive[g]++;
+        e->genv[g] = l.env[b];
         k++;
     }
     e->live += (int)l.slots.size();
     e->Nmax_live = std::max(e->Nmax_live, l.Nmax); e->Mmax_live = std::max(e->Mmax_live, l.Mmax);
-    // compact descriptors of the admitted problems only (skipped ones keep their UALM_ELIMIT record)
+    // compact descriptors of the admitted problems only (skipped ones keep their UALM_ELIMIT record), grouped by environment: one
+    // admit_kernel launch per environment, with its own use_scaling and int_K.  offs: sample offsets in the caller's dual arrays
     std::vector<AdmitDesc> ad;
     std::vector<long long> offs;
+    int eoff[UALM_MAX_ENVS + 1];
     {
+        std::vector<long long> os_of(l.B, 0);
         long long os = 0;
-        for (int b = 0; b < l.B; b++) if (l.ad[b].slot >= 0) { ad.push_back(l.ad[b]); offs.push_back(os); os += (long long)l.N[b] * (e->p.int_K + 1); }
+        for (int b = 0; b < l.B; b++) if (l.ad[b].slot >= 0) { os_of[b] = os; os += (long long)l.N[b] * (e->p[l.env[b]].int_K + 1); }
+        for (int v = 0; v < UALM_MAX_ENVS; v++) {
+            eoff[v] = (int)ad.size();
+            for (int b = 0; b < l.B; b++) if (l.ad[b].slot >= 0 && l.env[b] == v) { ad.push_back(l.ad[b]); offs.push_back(os_of[b]); }
+        }
+        eoff[UALM_MAX_ENVS] = (int)ad.size();
     }
     const int BA = (int)ad.size();
     TCK(cudaEventRecord(l.ev0, e->stream));
@@ -445,15 +489,20 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, std::s
         TCK(cudaMemcpyAsync(e->remaining.p + lane, e->h_remaining + lane, sizeof(int), cudaMemcpyHostToDevice, e->stream));
         const double *lam = l.has_lam ? l.d_lam.p : nullptr, *mu = l.has_mu ? l.d_mu.p : nullptr, *scx = l.has_scx ? l.d_scin.p : nullptr,
                      *sfx = l.has_sfx ? l.d_sfin.p : nullptr;
-        if (e->f32()) admit_kernel<float><<<BA, 128, 0, e->stream>>>(e->E, l.d_ad.p, l.d_x0.p, BA, e->p.use_scaling, e->p.int_K, lam, mu, scx, sfx, l.rho_eval, l.d_offs.p);
-        else admit_kernel<double><<<BA, 128, 0, e->stream>>>(e->E, l.d_ad.p, l.d_x0.p, BA, e->p.use_scaling, e->p.int_K, lam, mu, scx, sfx, l.rho_eval, l.d_offs.p);
-        TCK(cudaGetLastError());
+        for (int v = 0; v < UALM_MAX_ENVS; v++) {
+            const int n = eoff[v + 1] - eoff[v];
+            if (n == 0) continue;
+            const TpParams &p = e->p[v];
+            if (e->f32()) admit_kernel<float><<<n, 128, 0, e->stream>>>(e->E, l.d_ad.p + eoff[v], l.d_x0.p, n, p.use_scaling, p.int_K, lam, mu, scx, sfx, l.rho_eval, l.d_offs.p + eoff[v]);
+            else admit_kernel<double><<<n, 128, 0, e->stream>>>(e->E, l.d_ad.p + eoff[v], l.d_x0.p, n, p.use_scaling, p.int_K, lam, mu, scx, sfx, l.rho_eval, l.d_offs.p + eoff[v]);
+            TCK(cudaGetLastError());
+            l.launches++;
+        }
         // host-synchronised: ad / offs / res0 are stack-local staging vectors, and the lane's group streams start after the admission
         TCK(cudaStreamSynchronize(e->stream));
-        l.launches++;
         for (int q = 0; q < TP_SUBGROUPS; q++) {
             const int g = lane * TP_SUBGROUPS + q;
-            if (e->glive[g] > 0) { e->gcompact[g] = true; if ((mode == 0 && e->p.use_scaling) || mode == 2) e->gscale[g] = std::max(e->gscale[g], 1); }
+            if (e->glive[g] > 0) { e->gcompact[g] = true; if ((mode == 0 && e->p[e->genv[g]].use_scaling) || mode == 2) e->gscale[g] = std::max(e->gscale[g], 1); }
         }
     } else {
         e->h_remaining[lane] = 0;
@@ -491,21 +540,21 @@ static void ka_layout(TpEngine *e)
     const int hstride = (int)(((size_t)nmax * e->esz() + 15) / 16 * 16 / e->esz());
     const size_t col = ((size_t)12 * e->Nmax_live + 6 * e->Mmax_live) * 8, hist = (((size_t)TP_HRING * 2 * hstride * e->esz()) + 15) & ~(size_t)15;
     e->E.ka_hist_bytes = (int)hist;                                             // behind the ring: 1 / ys and alpha of the two-loop (2 m doubles)
-    e->E.ka_col_bytes = (int)((std::max(col, hist + 2 * (size_t)e->p.mem_size * 8) + 15) & ~(size_t)15);
+    e->E.ka_col_bytes = (int)((std::max(col, hist + 2 * (size_t)max_m(e) * 8) + 15) & ~(size_t)15);
     e->E.ka_hist_stride = hstride;
 }
 static size_t ka_smem_bytes(TpEngine *e) { return (size_t)e->ka_warps * e->E.ka_col_bytes; }
 
-// one round of group g on its stream: ka -> [ks] -> kb
+// one round of group g on its stream: ka -> [ks] -> kb, with the parameters, grid and TMA descriptor of the group's environment
 template <class R>
 static int launch_round(TpEngine *e, int g, bool with_ks, bool tma, std::string *err)
 {
-    const int upper = e->glive[g];
+    const int upper = e->glive[g], v = e->genv[g];
     cudaStream_t st = e->gstream[g];
-    ka_kernel<R><<<(upper + e->ka_warps - 1) / e->ka_warps, 32 * e->ka_warps, ka_smem_bytes(e), st>>>(e->E, e->p, g);
-    if (with_ks) ks_kernel<R><<<upper, TP_KB_THREADS, ks_smem_bytes(e), st>>>(e->E, e->p, e->map, g);
-    if (tma) kb_kernel<R, true><<<upper, TP_KB_THREADS, kb_smem_bytes(e, true), st>>>(e->E, e->p, e->map, e->tmap, g);
-    else kb_kernel<R, false><<<upper, TP_KB_THREADS, kb_smem_bytes(e, false), st>>>(e->E, e->p, e->map, e->tmap, g);
+    ka_kernel<R><<<(upper + e->ka_warps - 1) / e->ka_warps, 32 * e->ka_warps, ka_smem_bytes(e), st>>>(e->E, e->p[v], g);
+    if (with_ks) ks_kernel<R><<<upper, TP_KB_THREADS, ks_smem_bytes(e), st>>>(e->E, e->p[v], e->map[v], g);
+    if (tma && e->have_tmap[v]) kb_kernel<R, true><<<upper, TP_KB_THREADS, kb_smem_bytes(e, true), st>>>(e->E, e->p[v], e->map[v], e->tmap[v], g);
+    else kb_kernel<R, false><<<upper, TP_KB_THREADS, kb_smem_bytes(e, false), st>>>(e->E, e->p[v], e->map[v], e->tmap[v], g);
     TCK(cudaGetLastError());
     return UALM_OK;
 }
@@ -531,7 +580,7 @@ static int run_rounds(TpEngine *e, int nr, std::string *err)
     if (e->live <= 0) return UALM_OK;
     int rc = e->f32() ? set_attrs<float>(e, err) : set_attrs<double>(e, err);
     if (rc) return rc;
-    const bool tma = e->have_tmap && e->use_tma;
+    const bool tma = e->use_tma;          // (for the environments whose grid has a tensor map)
     for (int r = 0; r < nr; r++) {
         for (int g = 0; g < TP_NGROUPS; g++) {
             if (e->glive[g] <= 0) continue;
@@ -696,7 +745,7 @@ int tp_eval(TpEngine *e, int lane, const double *x, const double *lambda, const 
             double *f, double *grad, double *hx, double *gx, double *c_xy, double *c_yaw, std::string *err)
 {
     TpLane &l = e->lanes[lane];
-    if (!l.have_batch || !e->have_map) { if (err) *err = "upload and set_map first"; return UALM_ESTATE; }
+    if (!l.have_batch) { if (err) *err = "upload and set_map first"; return UALM_ESTATE; }
     for (int b = 0; b < l.B; b++) if (l.N[b] > TP_NMAX || l.M[b] > TP_MMAX) { if (err) *err = "batch holds problems over the compiled limits"; return UALM_ELIMIT; }
     TCK(cudaSetDevice(e->device));
     if (x && l.tot_x > 0) TCK(cudaMemcpyAsync(l.d_x0.p, x, sizeof(double) * l.tot_x, cudaMemcpyHostToDevice, e->stream));
@@ -726,7 +775,7 @@ int tp_eval(TpEngine *e, int lane, const double *x, const double *lambda, const 
 int tp_init_scaling(TpEngine *e, int lane, double *scale_fx, double *scale_cx, std::string *err)
 {
     TpLane &l = e->lanes[lane];
-    if (!l.have_batch || !e->have_map) { if (err) *err = "upload and set_map first"; return UALM_ESTATE; }
+    if (!l.have_batch) { if (err) *err = "upload and set_map first"; return UALM_ESTATE; }
     for (int b = 0; b < l.B; b++) if (l.N[b] > TP_NMAX || l.M[b] > TP_MMAX) { if (err) *err = "batch holds problems over the compiled limits"; return UALM_ELIMIT; }
     TCK(cudaSetDevice(e->device));
     int rc = admit_impl(e, lane, 2, false, err);
@@ -744,14 +793,16 @@ int tp_init_scaling(TpEngine *e, int lane, double *scale_fx, double *scale_cx, s
 int tp_time_penalty(TpEngine *e, int lane, int reps, int use_tma, float *ms_per_launch, double *algorithmic_bytes, std::string *err)
 {
     TpLane &l = e->lanes[lane];
-    if (!l.have_batch || !e->have_map) { if (err) *err = "upload and set_map first"; return UALM_ESTATE; }
+    if (!l.have_batch) { if (err) *err = "upload and set_map first"; return UALM_ESTATE; }
+    if (l.mixed) { if (err) *err = "ualm_time_penalty_kernel: the uploaded batch mixes environments"; return UALM_EINVAL; }
     if (l.in_flight || e->live > 0) { if (err) *err = "ualm_time_penalty_kernel needs an idle pool"; return UALM_ESTATE; }
     if (ms_per_launch) *ms_per_launch = 0.f;
     if (algorithmic_bytes) *algorithmic_bytes = 0.0;
     if (l.B == 0) return UALM_OK;
     TCK(cudaSetDevice(e->device));
+    const int v = l.env[0];
     // admit as single evaluations (initial guess, zero duals, unit scales), run the forward half of a round, then time kb alone
-    l.has_lam = l.has_mu = l.has_scx = l.has_sfx = false; l.rho_eval = e->p.rho;
+    l.has_lam = l.has_mu = l.has_scx = l.has_sfx = false; l.rho_eval = e->p[v].rho;
     int rc = admit_impl(e, lane, 1, true, err);
     if (rc) return rc;
     rc = e->f32() ? set_attrs<float>(e, err) : set_attrs<double>(e, err);
@@ -761,16 +812,16 @@ int tp_time_penalty(TpEngine *e, int lane, int reps, int use_tma, float *ms_per_
     compact_kernel<<<1, 1024, 0, st>>>(e->E, e->capacity, g);
     e->gcompact[g] = false;
     const int upper = e->glive[g];
-    const bool tma = e->have_tmap && use_tma;
-    if (e->f32()) ka_kernel<float><<<(upper + e->ka_warps - 1) / e->ka_warps, 32 * e->ka_warps, ka_smem_bytes(e), st>>>(e->E, e->p, g);
-    else ka_kernel<double><<<(upper + e->ka_warps - 1) / e->ka_warps, 32 * e->ka_warps, ka_smem_bytes(e), st>>>(e->E, e->p, g);
+    const bool tma = e->have_tmap[v] && use_tma;
+    if (e->f32()) ka_kernel<float><<<(upper + e->ka_warps - 1) / e->ka_warps, 32 * e->ka_warps, ka_smem_bytes(e), st>>>(e->E, e->p[v], g);
+    else ka_kernel<double><<<(upper + e->ka_warps - 1) / e->ka_warps, 32 * e->ka_warps, ka_smem_bytes(e), st>>>(e->E, e->p[v], g);
     auto kb = [&]() {
         if (e->f32()) {
-            if (tma) kb_kernel<float, true><<<upper, TP_KB_THREADS, kb_smem_bytes(e, true), st>>>(e->E, e->p, e->map, e->tmap, g);
-            else kb_kernel<float, false><<<upper, TP_KB_THREADS, kb_smem_bytes(e, false), st>>>(e->E, e->p, e->map, e->tmap, g);
+            if (tma) kb_kernel<float, true><<<upper, TP_KB_THREADS, kb_smem_bytes(e, true), st>>>(e->E, e->p[v], e->map[v], e->tmap[v], g);
+            else kb_kernel<float, false><<<upper, TP_KB_THREADS, kb_smem_bytes(e, false), st>>>(e->E, e->p[v], e->map[v], e->tmap[v], g);
         } else {
-            if (tma) kb_kernel<double, true><<<upper, TP_KB_THREADS, kb_smem_bytes(e, true), st>>>(e->E, e->p, e->map, e->tmap, g);
-            else kb_kernel<double, false><<<upper, TP_KB_THREADS, kb_smem_bytes(e, false), st>>>(e->E, e->p, e->map, e->tmap, g);
+            if (tma) kb_kernel<double, true><<<upper, TP_KB_THREADS, kb_smem_bytes(e, true), st>>>(e->E, e->p[v], e->map[v], e->tmap[v], g);
+            else kb_kernel<double, false><<<upper, TP_KB_THREADS, kb_smem_bytes(e, false), st>>>(e->E, e->p[v], e->map[v], e->tmap[v], g);
         }
     };
     kb();    // warm-up
@@ -786,7 +837,7 @@ int tp_time_penalty(TpEngine *e, int lane, int reps, int use_tma, float *ms_per_
         // SURVEY 8d: per trajectory per evaluation S * 45 e + (25 N + 13 M) e, e = element size of the sample data
         double bytes = 0;
         const double es = (double)e->esz();
-        for (int b = 0; b < l.B; b++) bytes += (double)l.N[b] * (e->p.int_K + 1) * 45 * es + (25.0 * l.N[b] + 13.0 * l.M[b]) * es;
+        for (int b = 0; b < l.B; b++) bytes += (double)l.N[b] * (e->p[v].int_K + 1) * 45 * es + (25.0 * l.N[b] + 13.0 * l.M[b]) * es;
         *algorithmic_bytes = bytes;
     }
     // finish the evaluations and release the slots
@@ -796,11 +847,11 @@ int tp_time_penalty(TpEngine *e, int lane, int reps, int use_tma, float *ms_per_
 }
 
 int tp_lane_outputs(TpEngine *e, int lane, const ualm_result_t **d_res, const double **d_cxy, const double **d_cyaw, int *B, const int32_t **N,
-                    const int32_t **M)
+                    const int32_t **M, const int32_t **env)
 {
     TpLane &l = e->lanes[lane];
     if (!l.collected) return UALM_ESTATE;
-    *d_res = l.d_res.p; *d_cxy = l.d_cxy.p; *d_cyaw = l.d_cyaw.p; *B = l.B; *N = l.N.data(); *M = l.M.data();
+    *d_res = l.d_res.p; *d_cxy = l.d_cxy.p; *d_cyaw = l.d_cyaw.p; *B = l.B; *N = l.N.data(); *M = l.M.data(); *env = l.env.data();
     return UALM_OK;
 }
 

@@ -13,12 +13,14 @@ struct TpEngine;
 // every function returns UALM_OK or a negative UALM_E* code; *err receives the message
 int tp_create(TpEngine **e, int device, int precision, std::string *err);
 void tp_destroy(TpEngine *e);
-int tp_set_params(TpEngine *e, const ualm_params_t *p, std::string *err);
-int tp_set_map(TpEngine *e, const ualm_map_geom_t *g, const float *cells, std::string *err);
+// parameters / grid of environment `env` (0 <= env < UALM_MAX_ENVS)
+int tp_set_params(TpEngine *e, int env, const ualm_params_t *p, std::string *err);
+int tp_set_map(TpEngine *e, int env, const ualm_map_geom_t *g, const float *cells, std::string *err);
 // lanes = tickets: a lane holds one uploaded batch; admit puts it into the pool of running trajectories, collect drives the
-// evaluation rounds until that lane's batch is finished and gathers its results on the device
-int tp_upload(TpEngine *e, int lane, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time, const double *inner_xy,
-              const double *inner_yaw, std::string *err);
+// evaluation rounds until that lane's batch is finished and gathers its results on the device.  env[B]: environment of every
+// problem (NULL = all 0), in range and bound (the caller checks)
+int tp_upload(TpEngine *e, int lane, int B, const int32_t *N, const int32_t *M, const int32_t *env, const double *bnd, const double *total_time,
+              const double *inner_xy, const double *inner_yaw, std::string *err);
 int tp_admit(TpEngine *e, int lane, std::string *err);                       // asynchronous
 // blocks: rounds until the lane's batch is done.  timeout_ms >= 0: once that much time has passed since the call, the lane's
 // cancel word is raised before the next rounds (its trajectories stop at their next stop test)
@@ -36,10 +38,11 @@ int tp_mark_end(TpEngine *e, float *ms, std::string *err);
 int tp_eval(TpEngine *e, int lane, const double *x, const double *lambda, const double *mu, const double *scale_cx, const double *scale_fx, double rho,
             double *f, double *grad, double *hx, double *gx, double *c_xy, double *c_yaw, std::string *err);
 int tp_init_scaling(TpEngine *e, int lane, double *scale_fx, double *scale_cx, std::string *err);
-// time `reps` launches of kb_kernel alone over the lane's batch (the trajectories sit at their initial guess)
+// time `reps` launches of kb_kernel alone over the lane's batch (the trajectories sit at their initial guess); UALM_EINVAL when the
+// batch mixes environments
 int tp_time_penalty(TpEngine *e, int lane, int reps, int use_tma, float *ms_per_launch, double *algorithmic_bytes, std::string *err);
 // device pointers of the lane's gathered outputs (for the post-solve scan)
 int tp_lane_outputs(TpEngine *e, int lane, const ualm_result_t **d_res, const double **d_cxy, const double **d_cyaw, int *B, const int32_t **N,
-                    const int32_t **M);
+                    const int32_t **M, const int32_t **env);
 
 } // namespace ualm_tp

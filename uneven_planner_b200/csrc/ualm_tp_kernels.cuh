@@ -860,7 +860,8 @@ __global__ void compact_kernel(const __grid_constant__ TpPool E, int hi, int gro
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// admission: problem b of a submitted batch -> slot
+// admission: problem b of a submitted batch -> slot.  One launch covers problems of one environment (use_scaling, K are its own);
+// off_s[b]: sample offset of ad[b] in the caller's dual arrays, sfx is indexed by the problem's index in its batch
 // ---------------------------------------------------------------------------------------------------------------------
 struct AdmitDesc { int slot, N, M, ticket, index, mode, group, pad1; long long off_x; double total_time; double bnd[18]; };
 
@@ -893,7 +894,7 @@ __global__ void admit_kernel(const __grid_constant__ TpPool E, const AdmitDesc *
         st->mode = a.mode; st->group = a.group;
         st->need_scale = ((a.mode == 0 && use_scaling) || a.mode == 2) ? 1 : 0;
         st->phase = PH_NEW;
-        if (a.mode == 1) { st->rho = rho_eval; st->scale_fx = sfx ? sfx[b] : 1.0; }
+        if (a.mode == 1) { st->rho = rho_eval; st->scale_fx = sfx ? sfx[a.index] : 1.0; }
     }
 }
 

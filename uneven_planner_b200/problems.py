@@ -45,6 +45,7 @@ class ProblemBatch:
     inner_yaw: np.ndarray    # float64 packed sum (M-1)
     starts: np.ndarray = None
     goals: np.ndarray = None
+    env: np.ndarray = None   # int32 [B]: environment of every problem (include/ualm.h, ualm_select_env); None = all environment 0
 
     @property
     def B(self):
@@ -70,7 +71,8 @@ class ProblemBatch:
                             np.concatenate([self.inner_xy[oxy[i]:oxy[i + 1]] for i in idx]) if len(idx) else np.zeros(0),
                             np.concatenate([self.inner_yaw[oyaw[i]:oyaw[i + 1]] for i in idx]) if len(idx) else np.zeros(0),
                             None if self.starts is None else self.starts[idx].copy(),
-                            None if self.goals is None else self.goals[idx].copy())
+                            None if self.goals is None else self.goals[idx].copy(),
+                            None if self.env is None else self.env[idx].copy())
 
     def x0(self, i):
         """Initial decision vector [tau | Pxy | Pyaw] of problem i (alm_traj_opt.cpp:205-216)."""
@@ -78,6 +80,18 @@ class ProblemBatch:
         T = self.total_time[i]
         tau = (np.sqrt(2.0 * T - 1.0) - 1.0) if T > 1.0 else (1.0 - np.sqrt(2.0 / T - 1.0))
         return np.concatenate([[tau], self.inner_xy[oxy[i]:oxy[i + 1]], self.inner_yaw[oyaw[i]:oyaw[i + 1]]])
+
+
+def concat(batches, envs):
+    """One batch of the problems of `batches` back to back, batch k's in environment envs[k] (a mixed batch; select() reorders it)."""
+    if len(batches) != len(envs):
+        raise ValueError("one environment per batch")
+    cat = lambda f, empty: np.concatenate([getattr(b, f) for b in batches]) if batches else empty
+    have = lambda f: all(getattr(b, f) is not None for b in batches)
+    return ProblemBatch(cat("N", np.zeros(0, np.int32)).astype(np.int32), cat("M", np.zeros(0, np.int32)).astype(np.int32),
+                        cat("bnd", np.zeros((0, 18))), cat("total_time", np.zeros(0)), cat("inner_xy", np.zeros(0)), cat("inner_yaw", np.zeros(0)),
+                        cat("starts", None) if batches and have("starts") else None, cat("goals", None) if batches and have("goals") else None,
+                        np.concatenate([np.full(b.B, int(e), np.int32) for b, e in zip(batches, envs)]) if batches else np.zeros(0, np.int32))
 
 
 def dubins(start, goal, radius=0.6, ds=0.06, max_pts=4096):
