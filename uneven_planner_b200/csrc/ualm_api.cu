@@ -70,11 +70,11 @@ struct Lane {
     long long tot_x = 0, tot_s = 0, tot_cxy = 0, tot_cyaw = 0, tot_hist = 0, tot_scr = 0, tot_fac = 0, tot_ws = 0;
     DevBuf<ProbDesc> d_desc;
     DevBuf<int> d_order;
-    DevBuf<int4> d_wdesc;
-    std::vector<int4> wdesc;
     std::vector<int> group;      // warps per problem (1, 2 or 4)
-    struct GClass { int G = 1, n_ctas = 0, r0 = 0, r1 = 0, occ = 1, env = 0; size_t wd_off = 0, smem = 0; SmemLayout L; };
+    // one solve launch: the problems order[r0, r1) of one group size and one environment, taken from a work queue by grid CTAs
+    struct GClass { int G = 1, n_ctas = 0, grid = 0, r0 = 0, r1 = 0, occ = 1, env = 0; size_t smem = 0; SmemLayout L; };
     std::vector<GClass> cls;
+    DevBuf<int> d_queue;         // one work counter per launch, zeroed before the launches
     enum { NAUX = 7 };
     cudaStream_t aux[NAUX] = {};
     cudaEvent_t evs[NAUX + 1] = {};
@@ -92,7 +92,7 @@ struct Lane {
     {
         if (d_cancel) cudaFree(d_cancel);
         d_cancel = nullptr;
-        d_desc.release(); d_order.release(); d_wdesc.release(); d_eidx.release();
+        d_desc.release(); d_order.release(); d_queue.release(); d_eidx.release();
         DevBuf<double> *bufs[] = {&d_x0, &d_x, &d_lambda, &d_mu, &d_scale_cx, &d_hx, &d_gx, &d_lm_s, &d_lm_y, &d_lm_aux, &d_fac,
                                   &d_scr, &d_ws, &d_cxy, &d_cyaw, &d_f, &d_grad, &d_sfx};
         for (auto *b : bufs) b->release();
@@ -401,7 +401,7 @@ static BatchPtrs batch_ptrs(ualm_ctx *c)
     BatchPtrs b;
     b.B = l->B;
     b.n_active = l->n_active;
-    b.wdesc = l->d_wdesc.p;
+    b.queue = nullptr;
     b.n_leader_slots = 4;
     b.adopt = getenv("UALM_NOADOPT") ? 0 : 1;
     b.desc = l->d_desc.p; b.order = l->d_order.p; b.x0 = l->d_x0.p; b.x = l->d_x.p;
@@ -481,10 +481,12 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
     std::stable_sort(l->order.begin(), l->order.end(), [&](int a, int b2) { return l->desc[a].S > l->desc[b2].S; });
     int rc0 = prepare_launch(c);
     if (rc0) return rc0;
-    // Warp groups and size classes.  Problems are sorted by size; the largest get 4 or 2 warps (helpers for the parallel
-    // phases) as far as the whole batch still fits on the device at once.  Every (group size, size bucket) class is its own
-    // launch with its own shared-memory layout sized by the class maxima: a G=4 CTA holds one trajectory slot + 3 helper
-    // rings, a G=2 CTA two slots + 2 rings, a G=1 CTA four slots.  The classes run concurrently on separate streams.
+    // Warp groups and launches.  Problems are sorted by size; the largest get 4 or 2 warps (helpers for the parallel phases) as
+    // far as the whole batch still fits on the device at once.  Every (group size, environment) range of the order is one launch
+    // with its own shared-memory layout sized by the range's maxima: a G=4 CTA holds one trajectory slot + 3 helper rings, a G=2
+    // CTA two slots + 2 rings, a G=1 CTA four slots.  The slots of a launch take its problems largest first from one work queue
+    // (solve_kernel), so a slot whose trajectory ends early starts the next one; the grid is what the device holds at once, or
+    // fewer CTAs when the range is smaller.  The launches run concurrently on separate streams.
     {
         int dev_sms = 0;
         CK(cudaDeviceGetAttribute(&dev_sms, cudaDevAttrMultiProcessorCount, c->device));
@@ -517,8 +519,8 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
                 K4 = (long long)(BA * (getenv("UALM_F4") ? atof(getenv("UALM_F4")) : 0.0));
                 K2 = std::min<long long>(BA - K4, (long long)(BA * (getenv("UALM_F2") ? atof(getenv("UALM_F2")) : 0.0))) & ~1LL;
             }
-            // rank ranges per group size; within one, the problems of each environment (a class holds one: its parameters and grid
-            // are the launch's), each split into size buckets (the order is by descending size)
+            // rank ranges per group size; within one, the problems of each environment (a launch holds one: its parameters and grid
+            // are the launch's grid constants)
             std::vector<Lane::GClass> cls;
             std::vector<int> ord = l->order;
             const long long lim[4] = {0, K4, K4 + K2, BA};
@@ -530,27 +532,20 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
                     const int ce = l->env[ord[a]];
                     for (b2 = a; b2 < lim[gi + 1] && l->env[ord[b2]] == ce; b2++) {}
                     const DevParams &ep = c->envs[ce].dp;
-                    const int nsplit = (b2 - a) >= 96 ? (gi == 2 ? 3 : 2) : 1;
-                    for (int sp = 0; sp < nsplit; sp++) {
-                        Lane::GClass cl;
-                        cl.G = G; cl.env = ce;
-                        long long s0 = a + (b2 - a) * sp / nsplit, s1 = a + (b2 - a) * (sp + 1) / nsplit;
-                        const int per = 4 / G;                         // problems per CTA
-                        if (sp > 0) s0 = a + ((s0 - a + per - 1) / per) * per;
-                        if (sp + 1 < nsplit) s1 = a + ((s1 - a + per - 1) / per) * per;
-                        if (s1 <= s0) continue;
-                        cl.r0 = (int)s0; cl.r1 = (int)s1;
-                        int Nm = 1, Mm = 1, nm = 1, Sm = 1;
-                        for (long long r = s0; r < s1; r++) {
-                            const ProbDesc &d = l->desc[ord[r]];
-                            Nm = std::max(Nm, d.N); Mm = std::max(Mm, d.M); nm = std::max(nm, d.n); Sm = std::max(Sm, d.S);
-                        }
-                        cl.L = make_layout(Nm, Mm, nm, ep.mem_size, ep.past, ep.int_K, Sm);
-                        cl.smem = ((size_t)per * cl.L.total_doubles + (size_t)(4 - per) * RINGD) * sizeof(double);
-                        CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cl.occ, solve_kernel, UALM_THREADS * UALM_WPB, cl.smem));
-                        cl.n_ctas = (int)((s1 - s0 + per - 1) / per);
-                        cls.push_back(cl);
+                    Lane::GClass cl;
+                    cl.G = G; cl.env = ce; cl.r0 = (int)a; cl.r1 = (int)b2;
+                    int Nm = 1, Mm = 1, nm = 1, Sm = 1;
+                    for (long long r = a; r < b2; r++) {
+                        const ProbDesc &d = l->desc[ord[r]];
+                        Nm = std::max(Nm, d.N); Mm = std::max(Mm, d.M); nm = std::max(nm, d.n); Sm = std::max(Sm, d.S);
                     }
+                    cl.L = make_layout(Nm, Mm, nm, ep.mem_size, ep.past, ep.int_K, Sm);
+                    const int per = 4 / G;                         // trajectory slots per CTA
+                    cl.smem = ((size_t)per * cl.L.total_doubles + (size_t)(4 - per) * RINGD) * sizeof(double);
+                    CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cl.occ, solve_kernel, UALM_THREADS * UALM_WPB, cl.smem));
+                    cl.n_ctas = (int)((b2 - a + per - 1) / per);
+                    cl.grid = (int)std::min<long long>(cl.n_ctas, (long long)std::max(cl.occ, 1) * dev_sms);
+                    cls.push_back(cl);
                 }
             }
             double sm_need = 0.0;
@@ -562,38 +557,11 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
         }
         l->cls = best;
         l->order = best_ord;
-        l->wdesc.clear();
         for (auto &cl : l->cls) {
-            cl.wd_off = l->wdesc.size();
             for (int r = cl.r0; r < cl.r1; r++) l->group[l->order[r]] = cl.G;
-            int q = cl.r0;
-            while (q < cl.r1) {
-                if (cl.G == 4) {
-                    for (int w = 0; w < 4; w++) l->wdesc.push_back(make_int4(l->order[q], 0, 4, w | ((w ? w - 1 : 0) << 8)));
-                    q += 1;
-                } else if (cl.G == 2) {
-                    // CTA j of the class pairs its j-th largest with its j-th smallest problem: the small one ends early and its
-                    // two warps then help the large one (adoption, ualm_kernels.cuh)
-                    const int j = (q - cl.r0) / 2;
-                    const int pa = cl.r0 + j, pb = cl.r1 - 1 - j;
-                    const int pr[2] = {l->order[pa], pb > pa ? l->order[pb] : -1};
-                    for (int h = 0; h < 2; h++) {
-                        if (pr[h] >= 0) {
-                            l->wdesc.push_back(make_int4(pr[h], h, 2, 0));
-                            l->wdesc.push_back(make_int4(pr[h], h, 2, 1 | (h << 8)));
-                        } else { l->wdesc.push_back(make_int4(-1, 0, 1, 0)); l->wdesc.push_back(make_int4(-1, 0, 1, 0)); }
-                    }
-                    q += 2;
-                } else {
-                    for (int w = 0; w < 4; w++) {
-                        if (q < cl.r1) { l->wdesc.push_back(make_int4(l->order[q], w, 1, 0)); q += 1; }
-                        else l->wdesc.push_back(make_int4(-1, 0, 1, 0));
-                    }
-                }
-            }
-            if ((int)((l->wdesc.size() - cl.wd_off) / 4) != cl.n_ctas) return fail(UALM_EINVAL, "internal: class CTA count mismatch");
             if (getenv("UALM_DEBUG"))
-                fprintf(stderr, "[ualm] class G=%d: problems [%d,%d) %d CTAs, smem %zu B, %d CTAs/SM\n", cl.G, cl.r0, cl.r1, cl.n_ctas, cl.smem, cl.occ);
+                fprintf(stderr, "[ualm] launch G=%d env %d: problems [%d,%d), %d CTAs, smem %zu B, %d CTAs/SM\n", cl.G, cl.env, cl.r0, cl.r1, cl.grid,
+                        cl.smem, cl.occ);
         }
     }
     long long ox = 0, os = 0, ocx = 0, ocy = 0, oh = 0, oscr = 0, oixy = 0, oiyaw = 0, ofac = 0, ows = 0, oaux = 0;
@@ -621,7 +589,7 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
         ows += (long long)(12 * d.N + 6 * d.M) * 32 * l->group[b];
     }
     l->tot_x = ox; l->tot_s = os; l->tot_cxy = ocx; l->tot_cyaw = ocy; l->tot_hist = oh; l->tot_scr = oscr; l->tot_fac = ofac; l->tot_ws = ows;
-    CK(l->d_desc.ensure(B)); CK(l->d_order.ensure(BA)); CK(l->d_wdesc.ensure(l->wdesc.size())); CK(l->d_x0.ensure(ox)); CK(l->d_x.ensure(ox)); CK(l->d_grad.ensure(ox));
+    CK(l->d_desc.ensure(B)); CK(l->d_order.ensure(BA)); CK(l->d_queue.ensure(std::max<size_t>(l->cls.size(), 1))); CK(l->d_x0.ensure(ox)); CK(l->d_x.ensure(ox)); CK(l->d_grad.ensure(ox));
     CK(l->d_lambda.ensure(os)); CK(l->d_hx.ensure(os)); CK(l->d_mu.ensure(6 * os)); CK(l->d_gx.ensure(6 * os)); CK(l->d_scale_cx.ensure(7 * os));
     CK(l->d_lm_s.ensure(oh)); CK(l->d_lm_y.ensure(oh)); CK(l->d_scr.ensure(oscr));
     CK(l->d_ws.ensure(ows)); CK(l->d_fac.ensure(ofac)); CK(l->d_lm_aux.ensure((size_t)std::max(oaux, 1LL)));
@@ -635,7 +603,6 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
         CK(cudaMemcpyAsync(l->d_desc.p, l->desc.data(), sizeof(ProbDesc) * B, cudaMemcpyHostToDevice, l->stream));
         if (BA > 0) CK(cudaMemcpyAsync(l->d_order.p, l->order.data(), sizeof(int) * BA, cudaMemcpyHostToDevice, l->stream));
         CK(cudaMemcpyAsync(l->d_eidx.p, l->eidx.data(), sizeof(int) * B, cudaMemcpyHostToDevice, l->stream));
-        if (!l->wdesc.empty()) CK(cudaMemcpyAsync(l->d_wdesc.p, l->wdesc.data(), sizeof(int4) * l->wdesc.size(), cudaMemcpyHostToDevice, l->stream));
         if (ox > 0) CK(cudaMemcpyAsync(l->d_x0.p, x0.data(), sizeof(double) * ox, cudaMemcpyHostToDevice, l->stream));
         // records of skipped problems (the kernels overwrite the others), zero coefficients and durations for them
         CK(cudaMemcpyAsync(l->d_res.p, res0.data(), sizeof(ualm_result_t) * B, cudaMemcpyHostToDevice, l->stream));
@@ -660,25 +627,28 @@ extern "C" int ualm_solve_resident(ualm_ctx_t *c)
     CK(cudaSetDevice(c->device));
     l->last_launches = 0;
     CK(cudaMemcpyAsync(l->d_cancel, &c->h_flags[0], sizeof(int), cudaMemcpyHostToDevice, l->stream));   // no request carries over
+    if (!l->cls.empty()) CK(cudaMemsetAsync(l->d_queue.p, 0, sizeof(int) * l->cls.size(), l->stream));   // every launch's queue full
     CK(cudaEventRecord(l->ev0, l->stream));
     if (l->n_active > 0) {
-        // the classes run concurrently: class 0 on the lane stream, the others on auxiliary streams
+        // the launches run concurrently: launch 0 on the lane stream, the others on auxiliary streams
         const int last = Lane::NAUX;
         CK(cudaEventRecord(l->evs[last], l->stream));
         for (size_t ci = 0; ci < l->cls.size(); ci++) {
             auto &cl = l->cls[ci];
-            if (cl.n_ctas == 0) continue;
+            if (cl.grid == 0) continue;
             const int ai = (int)((ci - 1) % Lane::NAUX);
             cudaStream_t st = ci == 0 ? l->stream : l->aux[ai];
             if (ci > 0) CK(cudaStreamWaitEvent(st, l->evs[last], 0));
             BatchPtrs bp = batch_ptrs(c);
-            bp.wdesc = l->d_wdesc.p + cl.wd_off;
+            bp.queue = l->d_queue.p + ci;
+            bp.order = l->d_order.p + cl.r0;
+            bp.n_active = cl.r1 - cl.r0;
             bp.n_leader_slots = 4 / cl.G;
-            // the class's environment: its parameters and grid are the launch's grid constants, the solve reads them as before
+            // the launch's environment: its parameters and grid are the launch's grid constants, the solve reads them as before
             DevParams dp = c->envs[cl.env].dp;
             dp.cancel = l->d_cancel;
             dp.max_evals = c->max_evals;
-            solve_kernel<<<cl.n_ctas, UALM_THREADS * UALM_WPB, cl.smem, st>>>(bp, dp, c->envs[cl.env].dm, cl.L);
+            solve_kernel<<<cl.grid, UALM_THREADS * UALM_WPB, cl.smem, st>>>(bp, dp, c->envs[cl.env].dm, cl.L);
             CK(cudaGetLastError());
             l->last_launches++;
             if (ci > 0) { CK(cudaEventRecord(l->evs[ai], st)); CK(cudaStreamWaitEvent(l->stream, l->evs[ai], 0)); }

@@ -98,11 +98,11 @@ struct ProbDesc {
 struct BatchPtrs {
     int B;
     int n_active;            // problems within the compiled limits = entries of `order`
-    const int4 *wdesc;       // solve_kernel: per warp slot {problem (-1 = idle), leader slot in CTA, group size, warp in group | helper ring << 8}
+    int *queue;              // solve_kernel: the launch's work counter (zero at launch); slots take order[atomicAdd(queue, 1)]
     int n_leader_slots;      // solve_kernel: full per-trajectory slots per CTA (4 / G); helper rings follow them
     int adopt;               // solve_kernel: warps of a finished trajectory join the other trajectory of a two-slot CTA
     const ProbDesc *desc;
-    const int *order;        // launch order (largest first); blockIdx.x -> problem index
+    const int *order;        // launch order (largest first) -> problem index
     const R *x0;             // packed initial decision vectors
     R *x;                    // packed final decision vectors
     R *lambda, *mu, *scale_cx, *hx, *gx;
@@ -172,7 +172,8 @@ __host__ __device__ inline SmemLayout make_layout(int Nmax, int Mmax, int nmax, 
 enum {
     SC_TX1 = 0, SC_TX2, SC_TX3, SC_TX4, SC_TX5, SC_TY1, SC_TY2, SC_TY3, SC_TY4, SC_TY5,
     SC_SCALE_FX, SC_RHO, SC_F, SC_JERK, SC_CONSTR, SC_TAUCOST, SC_JERKRAW, SC_RTY, SC_CMD,
-    SC_STOPPED   // != 0: the stop predicate fired inside the inner solve that just ended
+    SC_STOPPED,  // != 0: the stop predicate fired inside the inner solve that just ended
+    SC_PROB      // the problem a CMD_NEXT hands to the helpers
 };
 
 // Handles to shared memory: a 32-bit address in the shared state space.  Accesses through them are explicit ld.shared /
@@ -262,10 +263,11 @@ __device__ __forceinline__ void prof_mark(const Traj &t, int tid, int phase)
 }
 
 // ---- leader / helper protocol inside a warp group (named barrier 1 + leader warp index, 32*G participants) ----
-enum { CMD_SAMPLES = 1, CMD_ACCUM = 2, CMD_SCALE = 3, CMD_EXIT = 4, CMD_REGROUP = 5, CMD_JOIN = 6 };
-// Adoption (CTAs that hold two trajectories with two warps each): when one trajectory finishes, its two warps join the other
-// trajectory's group as helpers 2 and 3, so the slower of the pair runs its parallel phases on the whole CTA.  Per leader slot
-// one state word: RUNNING -> (mate asks) JOINREQ -> (leader switches its group to the 128-thread barrier) JOINED; -> DONE.
+enum { CMD_SAMPLES = 1, CMD_ACCUM = 2, CMD_SCALE = 3, CMD_EXIT = 4, CMD_REGROUP = 5, CMD_JOIN = 6, CMD_NEXT = 7 };
+// Adoption (CTAs that hold two trajectories with two warps each): when a slot finds the launch's queue empty, its two warps join
+// the other trajectory's group as helpers 2 and 3, so the slower of the pair runs its parallel phases on the whole CTA.  Per
+// leader slot one state word: DONE (no problem) -> RUNNING (problem published) -> (mate asks) JOINREQ -> (leader switches its
+// group to the 128-thread barrier) JOINED; -> DONE.  A slot that has been joined takes no further problem.
 // The partition of the parallel phases over warps never changes a result bit (every output entry has one owner and a fixed
 // summation order), so the solve stays batch-invariant.
 enum { AD_RUNNING = 0, AD_JOINREQ = 1, AD_JOINED = 2, AD_DONE = 3 };
@@ -2015,8 +2017,7 @@ __device__ UALM_NOINLINE void traj_setup(Traj &t, const BatchPtrs &bp, const Dev
     t.x = S8(L.x); t.g = S8(L.g); t.xp = S8(L.xp); t.gp = S8(L.gp); t.d = S8(L.d); t.pf = S8(L.pf); t.s1tab = S8(L.s1tab);
     t.base = S8(L.base); t.sc = S8(L.sc); t.win = S8(L.win); t.tmpl = S8(L.tmpl); t.ring = S8(L.ring);
     t.yawidx = SPtrU16{sm + 8u * (unsigned)L.yawidx};
-    t.lutab = sm + 8u * (unsigned)L.lutab;
-    if (wig == 0) lu_build_consts(t.lutab, threadIdx.x & 31);
+    t.lutab = sm + 8u * (unsigned)L.lutab;     // filled once per leader slot (lu_build_consts): it does not depend on the problem
     t.lambda = bp.lambda + pd->off_s; t.hx = bp.hx + pd->off_s;
     t.mu = bp.mu + 6 * pd->off_s; t.gx = bp.gx + 6 * pd->off_s;
     t.scale_cx = bp.scale_cx + 7 * pd->off_s;
@@ -2059,15 +2060,21 @@ __device__ UALM_NOINLINE int alm_exit(Traj &t, const DevParams &p, int lane, boo
 // kernels (CTA = 4 warp slots; solve_kernel: warp groups per trajectory, the test kernels: one warp per trajectory)
 // =============================================================================================
 
-// helper warps of a group: execute the parallel phases the leader posts, nothing else
+// helper warps of a group: execute the parallel phases the leader posts, nothing else.  Returns the group's next problem
+// (CMD_NEXT), -1 (CMD_EXIT) or -2 (CMD_JOIN: the warps join the mate's trajectory)
 __device__ UALM_NOINLINE int helper_loop(Traj &t, const DevMap &map, const DevParams &p, int lane)
 {
     while (true) {
         group_bar(t);
         const int cmd = (int)(R)t.sc[SC_CMD];
-        if (cmd == CMD_EXIT) return 0;
-        if (cmd == CMD_JOIN) return 1;
+        if (cmd == CMD_EXIT) return -1;
+        if (cmd == CMD_JOIN) return -2;
         if (cmd == CMD_REGROUP) { group_bar(t); t.G = 4; t.barid = UALM_BAR_BIG; continue; }
+        if (cmd == CMD_NEXT) {
+            const int prob = (int)(R)t.sc[SC_PROB];
+            group_bar(t);                       // the leader may overwrite the command word after this barrier
+            return prob;
+        }
         if (cmd == CMD_SAMPLES) penalty_samples(t, map, p, 32 * t.wig + lane, 32 * t.G);
         else if (cmd == CMD_ACCUM) accumulate_tasks(t, 32 * (t.wig - 1) + lane, 32 * (t.G - 1));
         else if (cmd == CMD_SCALE) scaling_rounds(t, map, p, 32 * t.wig + lane, 32 * t.G, lane);
@@ -2075,43 +2082,65 @@ __device__ UALM_NOINLINE int helper_loop(Traj &t, const DevMap &map, const DevPa
     }
 }
 
-// warps of a finished two-warp group: serve the other trajectory of the CTA as helpers 2 and 3 until it ends
+// warps of a two-warp group that found the queue empty: serve the mate slot's trajectory `prob` as helpers 2 and 3 until it ends
 __device__ UALM_NOINLINE void join_mate(Traj &t, const BatchPtrs &bp, const DevParams &p, const DevMap &map, const SmemLayout &L, unsigned sbase, int mate,
-                                        int wig, int lane)
+                                        int prob, int wig, int lane)
 {
-    const int4 wm = bp.wdesc[blockIdx.x * UALM_WPB + 2 * mate];
     const unsigned smm = sbase + 8u * (unsigned)(mate * L.total_doubles);
-    traj_setup(t, bp, p, L, smm, smm, wm.x, 4, wig, mate);
+    traj_setup(t, bp, p, L, smm, smm, prob, 4, wig, mate);
     t.barid = UALM_BAR_BIG;
     helper_loop(t, map, p, lane);
 }
 
-// full solve: optimizeSE2Traj (alm_traj_opt.cpp:168-278)
-__global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) solve_kernel(const __grid_constant__ BatchPtrs bp, const __grid_constant__ DevParams p, const __grid_constant__ DevMap map,
-        const __grid_constant__ SmemLayout L)
+// leader of a slot between two problems: take the next problem of the launch's queue (largest first) and hand it to the helpers.
+// Returns the problem; -1 when the slot is done; -2 when the queue is empty and the group's warps join the mate's trajectory
+// (`adopt` = the CTA's two adoption state words, null without adoption; `probs` = the problems the slots published).  A slot
+// that has been joined takes no further problem.
+__device__ UALM_NOINLINE int slot_next(Traj &t, const BatchPtrs &bp, int *adopt, int *probs, int slot, int lane)
 {
-    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5, wslot = blockIdx.x * UALM_WPB + w;
-    const int4 wd = bp.wdesc[wslot];
-    __shared__ int s_adopt[2];
-    const bool adoptable = (bp.n_leader_slots == 2 && bp.adopt);
-    if (adoptable) {
-        if (threadIdx.x < 2) s_adopt[threadIdx.x] = bp.wdesc[blockIdx.x * UALM_WPB + 2 * threadIdx.x].x < 0 ? AD_DONE : AD_RUNNING;
-        __syncthreads();
+    bool joined = false;
+    if (t.adopt) {                              // end of the slot's last problem
+        int old = 0;
+        if (lane == 0) old = atomicExch(t.adopt, AD_DONE);
+        old = __shfl_sync(0xffffffffu, old, 0);
+        if (old == AD_JOINREQ) regroup_now(t, lane);     // the mate's warps already wait on the CTA-wide barrier: release them below
+        joined = t.G == 4;
     }
-    if (wd.x < 0) return;   // idle warp slot
-    const unsigned sbase = (unsigned)__cvta_generic_to_shared(ualm_smem);
-    const int wig = wd.w & 0xff, hring = wd.w >> 8;
-    const unsigned sm = sbase + 8u * (unsigned)(wd.y * L.total_doubles);
-    // a helper's own shared memory is just a factor ring behind the leader slots; traj_setup adds L.ring to sm_own
-    const unsigned sm_own = wig == 0 ? sm
-                                     : sbase + 8u * (unsigned)(bp.n_leader_slots * L.total_doubles + hring * (2 * UALM_RINGB * 6 * UALM_FW)) - 8u * (unsigned)L.ring;
-    const int prob = wd.x;
-    Traj t;
-    traj_setup(t, bp, p, L, sm, sm_own, prob, wd.z, wig, wd.y);
-    if (wig > 0) {
-        if (helper_loop(t, map, p, lane)) join_mate(t, bp, p, map, L, sbase, 1 - wd.y, 3, lane);
-        return;
+    int next = -1;
+    if (!joined) {
+        if (lane == 0) {
+            const int q = atomicAdd(bp.queue, 1);
+            next = q < bp.n_active ? bp.order[q] : -1;
+        }
+        next = __shfl_sync(0xffffffffu, next, 0);
     }
+    if (next >= 0) {
+        if (lane == 0) t.sc[SC_PROB] = (R)next;
+        group_post(t, lane, CMD_NEXT);
+        group_bar(t);                           // the helpers have read the problem
+        if (adopt && lane == 0) {               // publish it: from here on the mate may ask to join
+            probs[slot] = next;
+            __threadfence_block();
+            atomicExch(&adopt[slot], AD_RUNNING);
+        }
+        return next;
+    }
+    int join = 0;
+    if (adopt && !joined && lane == 0) {        // offer this group's warps to the mate's trajectory, if it has one running
+        join = atomicCAS(&adopt[1 - slot], AD_RUNNING, AD_JOINREQ) == AD_RUNNING;
+        __threadfence_block();                  // probs[1 - slot] is read after this (the mate published it before RUNNING)
+    }
+    join = __shfl_sync(0xffffffffu, join, 0);
+    group_post(t, lane, join ? CMD_JOIN : CMD_EXIT);
+    return join ? -2 : -1;
+}
+
+// one problem on a leader slot, from its setup to its result record (`adopt` = the slot's adoption state word, or null).  Not
+// inlined: the loop over the queue around it would otherwise add spill to the solve
+__device__ UALM_NOINLINE void solve_problem(Traj &t, const BatchPtrs &bp, const DevParams &p, const DevMap &map, const SmemLayout &L, unsigned sm, int slot,
+                                            int *adopt, int prob, int lane)
+{
+    traj_setup(t, bp, p, L, sm, sm, prob, 4 / bp.n_leader_slots, 0, slot);
     const int N = t.N, M = t.M, n = t.n, S = t.S;
     // duals and scales (alm_traj_opt.cpp:193-203)
     for (int q = lane; q < S; q += 32) { t.lambda[q] = 0.0; t.hx[q] = 0.0; }
@@ -2122,7 +2151,7 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) solve_kernel(const __
     UALM_SYNC();
     if (p.use_scaling) init_scaling(t, map, p, lane);
     prof_mark(t, lane, PF_SCALING);
-    if (adoptable && wd.z == 2) t.adopt = &s_adopt[wd.y];   // joiners only take part in the evaluation phases
+    t.adopt = adopt;                      // joiners only take part in the evaluation phases
 
     int ret_code = 0, iter = 0, last = 0, iters_total = 0, max_bound = 0, sum_bound = 0;
     R inner_cost = 0.0, rh = 0.0, rg = 0.0;
@@ -2166,18 +2195,6 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) solve_kernel(const __
         }
         if ((R)(++iter) > p.max_iter) { ret_code = 2; break; }
     }
-    int join = 0;
-    if (t.adopt) {
-        int old = 0;
-        if (lane == 0) old = atomicExch(t.adopt, AD_DONE);
-        old = __shfl_sync(0xffffffffu, old, 0);
-        if (old == AD_JOINREQ) regroup_now(t, lane);         // the mate's warps already wait on the CTA-wide barrier: release them below
-        if (t.G == 2) {                                      // nobody joined this group: offer its warps to the mate
-            if (lane == 0) join = atomicCAS(&s_adopt[1 - wd.y], AD_RUNNING, AD_JOINREQ) == AD_RUNNING;
-            join = __shfl_sync(0xffffffffu, join, 0);
-        }
-    }
-    group_post(t, lane, join ? CMD_JOIN : CMD_EXIT);
     // outputs: coefficients / decision vector of the LAST evaluation's MINCO state (Q1), result record
     const int nx = 6 * N, ny = 6 * M;
     for (int q = lane; q < 2 * nx; q += 32) bp.c_xy[t.pd->off_cxy + q] = t.cxy[q];
@@ -2198,10 +2215,43 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) solve_kernel(const __
             for (int q = 0; q < UALM_NPROF; q++) bp.prof[(size_t)prob * UALM_NPROF + q] = t.prof[q];
         }
     }
-    if (join) {
-        UALM_SYNC();
-        join_mate(t, bp, p, map, L, sbase, 1 - wd.y, 2, lane);
+    UALM_SYNC();
+}
+
+// full solve: optimizeSE2Traj (alm_traj_opt.cpp:168-278).  Each leader slot of a CTA solves problems from the launch's queue until
+// it is empty, so a slot whose trajectory ends early takes the next one instead of idling until its CTA's slowest trajectory ends.
+// Every buffer a problem reads or writes is its own (ProbDesc offsets) and the slot's shared memory is set up again per problem,
+// so which slot solves which problem, and when, changes no result bit.
+__global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) solve_kernel(const __grid_constant__ BatchPtrs bp, const __grid_constant__ DevParams p, const __grid_constant__ DevMap map,
+        const __grid_constant__ SmemLayout L)
+{
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int G = UALM_WPB / bp.n_leader_slots, slot = w / G, wig = w - slot * G;   // group size, leader slot, warp in group
+    __shared__ int s_adopt[2], s_prob[2];
+    const bool adoptable = (bp.n_leader_slots == 2 && bp.adopt);
+    if (adoptable) {
+        if (threadIdx.x < 2) s_adopt[threadIdx.x] = AD_DONE;
+        __syncthreads();
     }
+    const unsigned sbase = (unsigned)__cvta_generic_to_shared(ualm_smem);
+    const unsigned sm = sbase + 8u * (unsigned)(slot * L.total_doubles);
+    Traj t;
+    t.G = G; t.barid = 1 + slot; t.sc = SPtr{sm + 8u * (unsigned)L.sc}; t.adopt = nullptr;   // the group before its first problem
+    if (wig > 0) {
+        // a helper's own shared memory is just a factor ring behind the leader slots (ring wig - 1 in a four-warp group, the slot's
+        // in a two-warp group); traj_setup adds L.ring to sm_own
+        const int hring = G == 4 ? wig - 1 : slot;
+        const unsigned sm_own = sbase + 8u * (unsigned)(bp.n_leader_slots * L.total_doubles + hring * (2 * UALM_RINGB * 6 * UALM_FW)) - 8u * (unsigned)L.ring;
+        int prob;
+        while ((prob = helper_loop(t, map, p, lane)) >= 0) traj_setup(t, bp, p, L, sm, sm_own, prob, G, wig, slot);
+        if (prob == -2) join_mate(t, bp, p, map, L, sbase, 1 - slot, ((volatile int *)s_prob)[1 - slot], 3, lane);
+        return;
+    }
+    lu_build_consts(sm + 8u * (unsigned)L.lutab, lane);
+    int *const adopt = adoptable ? s_adopt : nullptr;
+    int prob;
+    while ((prob = slot_next(t, bp, adopt, s_prob, slot, lane)) >= 0) solve_problem(t, bp, p, map, L, sm, slot, adopt ? adopt + slot : nullptr, prob, lane);
+    if (prob == -2) join_mate(t, bp, p, map, L, sbase, 1 - slot, ((volatile int *)s_prob)[1 - slot], 2, lane);
 }
 
 // one innerCallback evaluation per problem at caller-provided x / duals (kernel-level parity)
@@ -2213,6 +2263,7 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) eval_kernel(const __g
     const unsigned sm = (unsigned)__cvta_generic_to_shared(ualm_smem) + 8u * (unsigned)((threadIdx.x >> 5) * L.total_doubles);
     const int prob = bp.order[wslot];
     Traj t;
+    lu_build_consts(sm + 8u * (unsigned)L.lutab, lane);
     traj_setup(t, bp, p, L, sm, sm, prob, 1, 0, threadIdx.x >> 5);
     for (int q = lane; q < t.n; q += 32) t.x[q] = bp.x0[t.pd->off_x + q];
     if (lane == 0) { t.sc[SC_SCALE_FX] = bp.scale_fx_io[prob]; t.sc[SC_RHO] = rho; }
@@ -2234,6 +2285,7 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) scaling_kernel(const 
     const unsigned sm = (unsigned)__cvta_generic_to_shared(ualm_smem) + 8u * (unsigned)((threadIdx.x >> 5) * L.total_doubles);
     const int prob = bp.order[wslot];
     Traj t;
+    lu_build_consts(sm + 8u * (unsigned)L.lutab, lane);
     traj_setup(t, bp, p, L, sm, sm, prob, 1, 0, threadIdx.x >> 5);
     for (int q = lane; q < t.n; q += 32) t.x[q] = bp.x0[t.pd->off_x + q];
     if (lane == 0) { t.sc[SC_SCALE_FX] = 1.0; t.sc[SC_RHO] = p.rho; }
@@ -2252,6 +2304,7 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) penalty_only_kernel(c
     const unsigned sm = (unsigned)__cvta_generic_to_shared(ualm_smem) + 8u * (unsigned)((threadIdx.x >> 5) * L.total_doubles);
     const int prob = bp.order[wslot];
     Traj t;
+    lu_build_consts(sm + 8u * (unsigned)L.lutab, lane);
     traj_setup(t, bp, p, L, sm, sm, prob, 1, 0, threadIdx.x >> 5);
     for (int q = lane; q < t.n; q += 32) t.x[q] = bp.x0[t.pd->off_x + q];
     if (lane == 0) { t.sc[SC_SCALE_FX] = 1.0; t.sc[SC_RHO] = p.rho; }
