@@ -188,6 +188,11 @@ __device__ __forceinline__ double lds64(unsigned a)
     return v;
 }
 __device__ __forceinline__ void sts64(unsigned a, double v) { asm volatile("st.shared.f64 [%0], %1;" ::"r"(a), "d"(v) : "memory"); }
+// a store under a predicate: keeps the compiler from turning a guarded store into a divergent branch
+__device__ __forceinline__ void sts64_if(bool p, unsigned a, double v)
+{
+    asm volatile("{\n .reg .pred q;\n setp.ne.u32 q, %0, 0;\n @q st.shared.f64 [%1], %2;\n}" ::"r"((unsigned)p), "r"(a), "d"(v) : "memory");
+}
 struct SRef {   // proxy "reference" to one shared double
     unsigned a;
     __device__ __forceinline__ operator double() const { return lds64(a); }
@@ -477,7 +482,8 @@ __device__ __forceinline__ int tmpl_index(int r, int n6)
 //   .x the multiplier entry this lane divides (the pivot itself for the reciprocal lane and for idle lanes),
 //   .y the entry this lane updates, .z the pivot-row entry of that update,
 //   .w control: bits 0-1 lane holding the update's multiplier, 2 multiplier/reciprocal lane, 3 reciprocal lane, 4 update
-//      enabled, 5 factor store enabled, bits 8.. offset of this lane's factor entry in row k of F.
+//      enabled, 5 factor store enabled, bits 8-14 offset of this lane's factor entry in row k of F, bits 16-18 row offset o of
+//      this lane's multiplier L(k+o, k) (0: no multiplier), which also names the right-hand-side row it eliminates.
 // Built once per trajectory slot (3.3 KB of shared memory).
 #define UALM_WROW 16
 __device__ __forceinline__ void sts128(unsigned a, uint4 v)
@@ -513,7 +519,8 @@ __device__ __forceinline__ void lu_build_consts(unsigned tab, int lane)
             c.x = 8u * (unsigned)((tt + o) * UALM_WROW + 6 - o);
             c.y = 8u * (unsigned)((tt + uo) * UALM_WROW + 6 + uc - uo);
             c.z = 8u * (unsigned)(tt * UALM_WROW + 6 + uc);
-            c.w = (unsigned)ul | (act ? 4u : 0u) | (isr ? 8u : 0u) | (upd ? 16u : 0u) | ((act || ulane) ? 32u : 0u) | ((unsigned)so << 8);
+            c.w = (unsigned)ul | (act ? 4u : 0u) | (isr ? 8u : 0u) | (upd ? 16u : 0u) | ((act || ulane) ? 32u : 0u) | ((unsigned)so << 8) |
+                  ((unsigned)o << 16);
         }
         sts128(tab + 16u * (unsigned)e, c);
     }
@@ -523,6 +530,12 @@ __device__ __forceinline__ void lu_build_consts(unsigned tab, int lane)
 // lockstep.  Element-wise the update sequence is the reference's; within one pivot step the <=4 multipliers, the reciprocal of
 // the pivot and the <=12 updates run on different lanes.  Final factors stream to global memory: F[row][q] = LU(row, row-6+q),
 // F[row][13] = RN(1 / LU(row,row)) for the division-free sweeps.
+//
+// The forward sweep L y = b (banded_system.hpp:96-103) runs inside the factorization, on the right-hand sides in t.cxy (x and
+// y columns) and t.cyaw: the lane that forms L(k+o, k) also applies b(k+o) -= L(k+o, k) * b(k), skipped where L(k+o, k) == 0
+// as in the reference.  L(k+o, k) is final when pivot step k forms it and b(k) is final after step k-1 (its last update comes
+// from row k-1), so every element of b receives the reference's subtractions with the same operands in the same (ascending)
+// order.
 //
 // Six pivots (one period of the structure) form a super-step on a 12-row shared-memory window: rows 0..5 are the pivot rows,
 // rows 6..11 the rows below them; after the six steps rows 6..11 move up and fresh template rows enter.  Because the window
@@ -536,6 +549,8 @@ __device__ UALM_NOINLINE void lu_dual(Traj &t, int lane)
     const unsigned Wb = (t.win + sys * (12 * UALM_WROW)).a;
     const SPtr TM = t.tmpl + sys * (12 * UALM_FW);
     R *F = sys ? t.Fyaw : t.Fxy;
+    // right-hand-side columns of this system; the yaw half-warp names its one column twice, so its second store repeats the first
+    const unsigned B0 = (sys ? t.cyaw : t.cxy).a, B1 = sys ? 0u : 8u * (unsigned)n6;
     {
         const R T1 = t.sc[sys ? SC_TY1 : SC_TX1], T2 = t.sc[sys ? SC_TY2 : SC_TX2], T3 = t.sc[sys ? SC_TY3 : SC_TX3],
                 T4 = t.sc[sys ? SC_TY4 : SC_TX4], T5 = t.sc[sys ? SC_TY5 : SC_TX5];
@@ -580,6 +595,8 @@ __device__ UALM_NOINLINE void lu_dual(Traj &t, int lane)
         // pivot types of this super-step: the last six pivots have their own patterns; a finished system idles on type 12
         const int ty0 = (j >= P) ? 12 : (j == P - 1 ? 6 : 0);
         unsigned ctab = tab + 256u * (unsigned)ty0, apiv = Wb + 8u * 6u, aurow = Wb + 8u * (unsigned)(6 + uq);
+        // b(k) of pivot k = 6j + tt; a finished system stays on its last block (no lane eliminates there)
+        unsigned abk = B0 + 48u * (unsigned)(j < P ? j : P - 1);
         uint4 cn = lds128(ctab);
 #pragma unroll 1
         for (int tt = 0; tt < 6; tt++) {
@@ -587,11 +604,13 @@ __device__ UALM_NOINLINE void lu_dual(Traj &t, int lane)
             if (ty0 != 12) ctab += 256u;
             cn = lds128(ctab);                                   // constants of the next step (tt = 5 reads one entry ahead: unused)
             const bool act = (c.w & 4u) != 0, isr = (c.w & 8u) != 0;
+            const unsigned abi = abk + 8u * ((c.w >> 16) & 7u);  // b(k+o)
             const R piv = lds64(apiv);
             const R av = lds64(Wb + c.x);
             const R urow = lds64(aurow);
             const R u = lds64(Wb + c.z);
             const R w = lds64(Wb + c.y);
+            const R bk0 = lds64(abk), bk1 = lds64(abk + B1), bi0 = lds64(abi), bi1 = lds64(abi + B1);
             const R a = isr ? 1.0 : av;
             const bool nz = act && (a != 0.0);
             // exact zeros are skipped by the reference (banded_system.hpp:74) and would push the division onto its slow path
@@ -609,8 +628,13 @@ __device__ UALM_NOINLINE void lu_dual(Traj &t, int lane)
             const bool unz = ((unsigned long long)__double_as_longlong(u) << 1) != 0ull;
             const bool mnz = ((unsigned long long)__double_as_longlong(mr) << 1) != 0ull;
             if ((c.w & 16u) && unz && mnz) sts64(Wb + c.y, w - mr * u);
+            // forward elimination, after the window update so that it does not delay the next pivot (predicated, not a branch)
+            const bool fwd = abi != abk && (((unsigned long long)__double_as_longlong(m) << 1) != 0ull);
+            sts64_if(fwd, abi, bi0 - m * bk0);
+            sts64_if(fwd, abi + B1, bi1 - m * bk1);
             UALM_SYNC();
             Fk += UALM_FW;
+            if (ty0 != 12) abk += 8u;
             apiv += 8u * UALM_WROW; aurow += 8u * UALM_WROW;
         }
         // rows 6..11 move up; the next six rows of A enter (each lane moves its own band column: no hazard between lanes)
@@ -639,15 +663,14 @@ __device__ UALM_NOINLINE void lu_dual(Traj &t, int lane)
 }
 
 // ---------------------------------------------------------------------------------------------
-// Triangular sweeps (banded_system.hpp:96-145), one block of six rows at a time with the static patterns above and the
+// Triangular sweeps (banded_system.hpp:104-145), one block of six rows at a time with the static patterns above and the
 // reference's per-element update order (ascending j for the forward sweeps, descending j for the backward ones, then the
-// division).
-//   KIND 0: L y = b      blocks ascending,  entries F[i][6-d]
+// division).  L y = b (banded_system.hpp:96-103) runs inside lu_dual.
 //   KIND 1: U x = y      blocks descending, entries F[i][6+d],  then / F[i][6]
 //   KIND 2: U^T y = b    blocks ascending,  entries U(i-d,i) = F[i-d][6+d] (the neighbour block's rows), then / F[i][6]
 //   KIND 3: L^T x = y    blocks descending, entries L(i+d,i) = F[i+d][6-d]
 // Bit d-1 of the mask of row type t (= row mod 6) says whether term d can be non-zero; the last block of a system (tail
-// rows) uses the full mask for the L-based kinds.  Factor blocks arrive through a UALM_RINGB-block cp.async ring per system
+// rows) uses the full mask for KIND 3.  Factor blocks arrive through a UALM_RINGB-block cp.async ring per system
 // (prefetch distance UALM_RINGB - 2 blocks); the previous block's six results stay in registers, so no window shifting is needed.
 // ---------------------------------------------------------------------------------------------
 // six 6-bit masks packed per kind (row type t at bits 6t..6t+5)
@@ -658,8 +681,7 @@ __host__ __device__ constexpr unsigned long long pack6(int a, int b, int c, int 
 }
 __host__ __device__ constexpr int sweep_mask(int kind, int t)
 {
-    return (int)(((kind == 0 ? pack6(0x3f, 0x3e, 0x3c, 0x00, 0x00, 0x1f)      // L rows
-                 : kind == 1 ? pack6(0x0c, 0x06, 0x03, 0x23, 0x21, 0x18)      // U rows
+    return (int)(((kind == 1 ? pack6(0x0c, 0x06, 0x03, 0x23, 0x21, 0x18)      // U rows
                  : kind == 2 ? pack6(0x00, 0x00, 0x00, 0x2f, 0x3f, 0x03)      // U columns
                              : pack6(0x30, 0x38, 0x3c, 0x1e, 0x0f, 0x07))     // L columns
                   >> (6 * t)) & 0x3f);
@@ -669,7 +691,7 @@ template <int KIND, int NCOL, bool FULL, bool EXACT, class BP>
 __device__ __forceinline__ bool sweep_rows(SPtr blk, SPtr nb, bool hasnb, BP b0, BP b1, int bst, int row0, const R (&rhs0)[6], const R (&rhs1)[6],
                                            const R (&prev0)[6], const R (&prev1)[6], R (&cur0)[6], R (&cur1)[6])
 {
-    constexpr bool ASC = (KIND == 0 || KIND == 2);
+    constexpr bool ASC = (KIND == 2);
     constexpr bool DIV = (KIND == 1 || KIND == 2);
     constexpr bool TR = (KIND == 2 || KIND == 3);   // transposed access: the factor entry lives in the neighbour's row
     bool bad = false;
@@ -686,9 +708,8 @@ __device__ __forceinline__ bool sweep_rows(SPtr blk, SPtr nb, bool hasnb, BP b0,
                 const int tn = ASC ? t - d : t + d;
                 const bool incur = ASC ? (tn >= 0) : (tn <= 5);
                 const int tq = incur ? tn : (ASC ? tn + 6 : tn - 6);
-                // factor entry: KIND 0: L(i,i-d) = F[i][6-d]; KIND 1: U(i,i+d) = F[i][6+d];
-                //               KIND 2: U(i-d,i) = F[i-d][6+d]; KIND 3: L(i+d,i) = F[i+d][6-d]
-                if (!TR) fv[t][d] = f[ASC ? 6 - d : 6 + d];
+                // factor entry: KIND 1: U(i,i+d) = F[i][6+d]; KIND 2: U(i-d,i) = F[i-d][6+d]; KIND 3: L(i+d,i) = F[i+d][6-d]
+                if (!TR) fv[t][d] = f[6 + d];
                 else if (incur) fv[t][d] = blk[tq * UALM_FW + (ASC ? 6 + d : 6 - d)];
                 else fv[t][d] = hasnb ? (R)nb[tq * UALM_FW + (ASC ? 6 + d : 6 - d)] : 0.0;
             }
@@ -760,8 +781,8 @@ template <int KIND, int NCOL, bool DUAL, class BP>
 __device__ UALM_NOINLINE void sweep(const R *facA, int PA, const R *facB, int PB, SPtr ringA, SPtr ringB, BP b0, BP b1, int bst, int sel,
                                     bool active, int lane, int cstart = 0)
 {
-    constexpr bool ASC = (KIND == 0 || KIND == 2);
-    constexpr bool LKIND = (KIND == 0 || KIND == 3);   // kinds whose tail block needs the full pattern
+    constexpr bool ASC = (KIND == 2);
+    constexpr bool LKIND = (KIND == 3);                // the kind whose tail block needs the full pattern
     constexpr int BLK = 6 * UALM_FW;                    // doubles per block (42 x 16 B)
     const int nb = DUAL ? (PA > PB ? PA : PB) : PA;
     auto issue = [&](int c) {
@@ -837,12 +858,11 @@ __device__ UALM_NOINLINE void minco_generate(Traj &t, int lane)
     for (int i = lane; i < M - 1; i += 32) t.cyaw[6 * i + 5] = Pyaw[i];
     UALM_SYNC();
     prof_mark(t, lane, PF_FILL);
-    lu_dual(t, lane);
+    lu_dual(t, lane);   // also L y = b on the right-hand sides
     prof_mark(t, lane, PF_LU);
-    // lanes 0/1: x / y columns against the xy factors; lane 2: the yaw column, all in lockstep
+    // U x = y: lanes 0/1: x / y columns against the xy factors; lane 2: the yaw column, all in lockstep
     {
         const SPtr col = lane < 2 ? t.cxy + lane * nx : t.cyaw;
-        sweep<0, 1, true, SPtr>(t.Fxy, N, t.Fyaw, M, t.ring, t.ring + UALM_RINGB * 6 * UALM_FW, col, col, 1, lane == 2, lane < 3, lane);
         sweep<1, 1, true, SPtr>(t.Fxy, N, t.Fyaw, M, t.ring, t.ring + UALM_RINGB * 6 * UALM_FW, col, col, 1, lane == 2, lane < 3, lane);
     }
     UALM_SYNC();
