@@ -203,7 +203,8 @@ int ualm_pack_records_device_async(ualm_ctx_t *ctx, double *d_records, int strid
  * in the reference's index layout (alm_traj_opt.cpp:705-707, 832-946), S_b = N_b (int_K+1) with the int_K of problem b's
  * environment.
  * Outputs (host): f[B], grad (packed n_b), hx (packed S_b), gx (packed 6 S_b). Any input dual may be
- * NULL (zeros / ones).  scale_fx[B], rho scalar. */
+ * NULL (zeros / ones).  scale_fx[B], rho scalar.  x NULL evaluates at the uploaded initial guesses; a given x does not
+ * replace them. */
 int ualm_eval_batch(ualm_ctx_t *ctx, const double *x, const double *lambda, const double *mu,
                     const double *scale_cx, const double *scale_fx, double rho,
                     double *f, double *grad, double *hx, double *gx, double *c_xy, double *c_yaw);

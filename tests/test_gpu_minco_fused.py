@@ -17,19 +17,21 @@ def gpu(built):
     return api
 
 
-def _arc_problem(N, M, zero_ends=False, radius=2.5, arc=1.5 * np.pi, speed=0.5):
-    """One problem whose waypoints lie on a circular arc around the map centre: N xy pieces, M yaw pieces.  zero_ends: zero
-    boundary velocity and acceleration, so that those right-hand-side rows are exact zeros."""
+def _arc_problem(N, M, zero_ends=False, radius=2.5, arc=1.5 * np.pi, speed=0.5, centre=(0.0, 0.0), start=0.0):
+    """One problem whose waypoints lie on a circular arc around `centre` (the map centre by default), from polar angle `start`
+    counter-clockwise over `arc`: N xy pieces, M yaw pieces.  zero_ends: zero boundary velocity and acceleration, so that those
+    right-hand-side rows are exact zeros."""
     from uneven_planner_b200 import problems
     length = radius * arc
     T = 1.2 * length / speed
-    a = arc * np.linspace(0.0, 1.0, N + 1)
-    pts = radius * np.stack([np.cos(a), np.sin(a)], axis=1)
-    yaw = arc * np.linspace(0.0, 1.0, M + 1) + 0.5 * np.pi
+    a = start + arc * np.linspace(0.0, 1.0, N + 1)
+    rel = radius * np.stack([np.cos(a), np.sin(a)], axis=1)
+    pts = rel + np.asarray(centre, np.float64)
+    yaw = start + arc * np.linspace(0.0, 1.0, M + 1) + 0.5 * np.pi
     tan0, tan1 = np.array([-np.sin(a[0]), np.cos(a[0])]), np.array([-np.sin(a[-1]), np.cos(a[-1])])
     v = 0.0 if zero_ends else speed
-    acc0 = np.zeros(2) if zero_ends else -speed ** 2 / radius * pts[0] / radius
-    acc1 = np.zeros(2) if zero_ends else -speed ** 2 / radius * pts[-1] / radius
+    acc0 = np.zeros(2) if zero_ends else -speed ** 2 / radius * rel[0] / radius
+    acc1 = np.zeros(2) if zero_ends else -speed ** 2 / radius * rel[-1] / radius
     dyaw = 0.0 if zero_ends else speed / radius
     bnd = np.concatenate([pts[0], v * tan0, acc0, pts[-1], v * tan1, acc1, [yaw[0], dyaw, 0.0, yaw[-1], dyaw, 0.0]])
     return problems.ProblemBatch(np.array([N], np.int32), np.array([M], np.int32), bnd.reshape(1, 18), np.array([T]),
@@ -37,6 +39,8 @@ def _arc_problem(N, M, zero_ends=False, radius=2.5, arc=1.5 * np.pi, speed=0.5):
 
 
 CASES = {
+    "one_piece": dict(N=1, M=1, arc=0.5 * np.pi),
+    "one_xy_piece_most_yaw_pieces": dict(N=1, M=128, arc=0.5 * np.pi),
     "smallest": dict(N=2, M=1),
     "compiled_limits": dict(N=64, M=128),
     "xy_longer_than_yaw": dict(N=40, M=3),

@@ -212,15 +212,16 @@ def test_full_solve_without_scaling_volcano_parameters(gpu, bumps_map):
 
 
 def test_edge_cases(gpu, bumps_map):
-    """ragged / extreme shapes: the shortest path the resampler can emit, a long one, a start outside the map
-    (zero terrain, uneven_map.h:260-265), and an empty batch."""
+    """ragged / extreme shapes: a path shorter than one piece (one xy and one yaw piece, T < 1 s), a short one, a long one,
+    a start outside the map (zero terrain, uneven_map.h:260-265), and an empty batch."""
     from uneven_planner_b200 import _lib, problems
-    paths = [problems.dubins([0, 0, 0.0], [0.45, 0.02, 0.0]),              # N=2, M=4
+    paths = [problems.dubins([0, 0, 0.0], [0.1, 0.0, 0.0]),                # N=1, M=1, T=0.24 s
+             problems.dubins([0, 0, 0.0], [0.45, 0.02, 0.0]),              # N=2, M=4
              problems.dubins([-4.5, -4.5, 0.7], [4.5, 4.5, 0.7]),           # long diagonal
              problems.dubins([4.2, 0.0, 0.0], [5.6, 0.3, 0.2]),             # leaves the map
              problems.dubins([1.0, 1.0, 3.0], [1.0, -1.2, -0.2])]
     pb = problems.from_paths(paths)
-    assert pb.N.min() == 2
+    assert (pb.N[0], pb.M[0]) == (1, 1) and pb.total_time[0] < 1.0 and pb.N[1] == 2
     p = _lib.default_params()
     res, cxy, cyaw, ores = _solve_both(gpu, bumps_map, pb, p)
     _assert_solve_parity(pb, res, cxy, cyaw, ores)

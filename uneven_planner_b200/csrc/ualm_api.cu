@@ -78,7 +78,7 @@ struct Lane {
     enum { NAUX = 7 };
     cudaStream_t aux[NAUX] = {};
     cudaEvent_t evs[NAUX + 1] = {};
-    DevBuf<double> d_x0, d_x, d_lambda, d_mu, d_scale_cx, d_hx, d_gx, d_lm_s, d_lm_y, d_lm_aux, d_fac, d_scr, d_ws, d_cxy, d_cyaw, d_f, d_grad, d_sfx;
+    DevBuf<double> d_x0, d_x, d_xev, d_lambda, d_mu, d_scale_cx, d_hx, d_gx, d_lm_s, d_lm_y, d_lm_aux, d_fac, d_scr, d_ws, d_cxy, d_cyaw, d_f, d_grad, d_sfx;
     DevBuf<ualm_result_t> d_res;
     DevBuf<long long> d_prof;
     DevBuf<double> d_pieceT, d_feas;
@@ -93,7 +93,7 @@ struct Lane {
         if (d_cancel) cudaFree(d_cancel);
         d_cancel = nullptr;
         d_desc.release(); d_order.release(); d_queue.release(); d_eidx.release();
-        DevBuf<double> *bufs[] = {&d_x0, &d_x, &d_lambda, &d_mu, &d_scale_cx, &d_hx, &d_gx, &d_lm_s, &d_lm_y, &d_lm_aux, &d_fac,
+        DevBuf<double> *bufs[] = {&d_x0, &d_x, &d_xev, &d_lambda, &d_mu, &d_scale_cx, &d_hx, &d_gx, &d_lm_s, &d_lm_y, &d_lm_aux, &d_fac,
                                   &d_scr, &d_ws, &d_cxy, &d_cyaw, &d_f, &d_grad, &d_sfx};
         for (auto *b : bufs) b->release();
         d_res.release(); d_prof.release(); d_pieceT.release(); d_feas.release();
@@ -958,14 +958,21 @@ extern "C" int ualm_eval_batch(ualm_ctx_t *c, const double *x, const double *lam
     if (l->n_active != l->B) return fail(UALM_ELIMIT, "ualm_eval_batch: the uploaded batch holds problems over the compiled limits");
     CK(cudaSetDevice(c->device));
     int rc;
-    if (x) { if ((rc = put(c, l->d_x0.p, x, l->tot_x, 0.0))) return rc; }
+    // the evaluation point goes to its own buffer: d_x0 keeps the uploaded initial guesses, which ualm_init_scaling_batch and a
+    // later solve of the resident batch start from
+    if (x) {
+        CK(l->d_xev.ensure(l->tot_x));
+        if ((rc = put(c, l->d_xev.p, x, l->tot_x, 0.0))) return rc;
+    }
     if ((rc = put(c, l->d_lambda.p, lambda, l->tot_s, 0.0))) return rc;
     if ((rc = put(c, l->d_mu.p, mu, 6 * l->tot_s, 0.0))) return rc;
     if ((rc = put(c, l->d_scale_cx.p, scale_cx, 7 * l->tot_s, 1.0))) return rc;
     if ((rc = put(c, l->d_sfx.p, scale_fx, l->B, 1.0))) return rc;
     if (l->B > 0) {
         if ((rc = per_env(c, [&](int e, const BatchPtrs &bp, int cnt) {
-                 eval_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].dm, l->eL[e], rho);
+                 BatchPtrs be = bp;
+                 if (x) be.x0 = l->d_xev.p;
+                 eval_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(be, c->envs[e].dp, c->envs[e].dm, l->eL[e], rho);
              })))
             return rc;
         if (f) CK(cudaMemcpyAsync(f, l->d_f.p, sizeof(double) * l->B, cudaMemcpyDeviceToHost, l->stream));

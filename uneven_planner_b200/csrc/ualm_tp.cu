@@ -51,13 +51,13 @@ struct TpLane {
     long long tot_x = 0, tot_s = 0, tot_cxy = 0, tot_cyaw = 0;
     Buf<AdmitDesc> d_ad;
     Buf<GatherDesc> d_gd;
-    Buf<double> d_x0, d_cxy, d_cyaw, d_xout, d_f, d_grad, d_hx, d_gx, d_sfx, d_scx, d_lam, d_mu, d_scin, d_sfin;
+    Buf<double> d_x0, d_xev, d_cxy, d_cyaw, d_xout, d_f, d_grad, d_hx, d_gx, d_sfx, d_scx, d_lam, d_mu, d_scin, d_sfin;
     Buf<long long> d_offs;
     Buf<ualm_result_t> d_res;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     int launches = 0;
     double rho_eval = 1.0;
-    bool has_lam = false, has_mu = false, has_scx = false, has_sfx = false;
+    bool has_lam = false, has_mu = false, has_scx = false, has_sfx = false, has_xev = false;   // has_xev: admit from d_xev, not d_x0
 };
 
 struct TpEngine {
@@ -214,7 +214,7 @@ void tp_destroy(TpEngine *e)
     }
     for (int g = 0; g < TP_NGROUPS; g++) { if (e->gstream[g]) cudaStreamDestroy(e->gstream[g]); if (e->gev[g]) cudaEventDestroy(e->gev[g]); }
     for (auto &l : e->lanes) {
-        l.d_ad.release(); l.d_gd.release(); l.d_x0.release(); l.d_cxy.release(); l.d_cyaw.release(); l.d_xout.release(); l.d_f.release(); l.d_grad.release();
+        l.d_ad.release(); l.d_gd.release(); l.d_x0.release(); l.d_xev.release(); l.d_cxy.release(); l.d_cyaw.release(); l.d_xout.release(); l.d_f.release(); l.d_grad.release();
         l.d_hx.release(); l.d_gx.release(); l.d_sfx.release(); l.d_scx.release(); l.d_lam.release(); l.d_mu.release(); l.d_scin.release(); l.d_sfin.release();
         l.d_offs.release(); l.d_res.release();
         if (l.ev0) cudaEventDestroy(l.ev0);
@@ -487,14 +487,15 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, std::s
         TCK(cudaMemcpyAsync(l.d_gd.p, l.gd.data(), sizeof(GatherDesc) * l.B, cudaMemcpyHostToDevice, e->stream));
         e->h_remaining[lane] = BA;
         TCK(cudaMemcpyAsync(e->remaining.p + lane, e->h_remaining + lane, sizeof(int), cudaMemcpyHostToDevice, e->stream));
+        const double *x0 = l.has_xev ? l.d_xev.p : l.d_x0.p;
         const double *lam = l.has_lam ? l.d_lam.p : nullptr, *mu = l.has_mu ? l.d_mu.p : nullptr, *scx = l.has_scx ? l.d_scin.p : nullptr,
                      *sfx = l.has_sfx ? l.d_sfin.p : nullptr;
         for (int v = 0; v < UALM_MAX_ENVS; v++) {
             const int n = eoff[v + 1] - eoff[v];
             if (n == 0) continue;
             const TpParams &p = e->p[v];
-            if (e->f32()) admit_kernel<float><<<n, 128, 0, e->stream>>>(e->E, l.d_ad.p + eoff[v], l.d_x0.p, n, p.use_scaling, p.int_K, lam, mu, scx, sfx, l.rho_eval, l.d_offs.p + eoff[v]);
-            else admit_kernel<double><<<n, 128, 0, e->stream>>>(e->E, l.d_ad.p + eoff[v], l.d_x0.p, n, p.use_scaling, p.int_K, lam, mu, scx, sfx, l.rho_eval, l.d_offs.p + eoff[v]);
+            if (e->f32()) admit_kernel<float><<<n, 128, 0, e->stream>>>(e->E, l.d_ad.p + eoff[v], x0, n, p.use_scaling, p.int_K, lam, mu, scx, sfx, l.rho_eval, l.d_offs.p + eoff[v]);
+            else admit_kernel<double><<<n, 128, 0, e->stream>>>(e->E, l.d_ad.p + eoff[v], x0, n, p.use_scaling, p.int_K, lam, mu, scx, sfx, l.rho_eval, l.d_offs.p + eoff[v]);
             TCK(cudaGetLastError());
             l.launches++;
         }
@@ -748,15 +749,22 @@ int tp_eval(TpEngine *e, int lane, const double *x, const double *lambda, const 
     if (!l.have_batch) { if (err) *err = "upload and set_map first"; return UALM_ESTATE; }
     for (int b = 0; b < l.B; b++) if (l.N[b] > TP_NMAX || l.M[b] > TP_MMAX) { if (err) *err = "batch holds problems over the compiled limits"; return UALM_ELIMIT; }
     TCK(cudaSetDevice(e->device));
-    if (x && l.tot_x > 0) TCK(cudaMemcpyAsync(l.d_x0.p, x, sizeof(double) * l.tot_x, cudaMemcpyHostToDevice, e->stream));
+    // the evaluation point goes to its own buffer: d_x0 keeps the uploaded initial guesses, which ualm_init_scaling_batch and a
+    // later solve of the resident batch start from
+    const bool xev = x && l.tot_x > 0;
+    if (xev) {
+        TCK(l.d_xev.ensure(l.tot_x));
+        TCK(cudaMemcpyAsync(l.d_xev.p, x, sizeof(double) * l.tot_x, cudaMemcpyHostToDevice, e->stream));
+    }
     int rc;
     if ((rc = put(e, l.d_lam, lambda, l.tot_s, l.has_lam, err))) return rc;
     if ((rc = put(e, l.d_mu, mu, 6 * l.tot_s, l.has_mu, err))) return rc;
     if ((rc = put(e, l.d_scin, scale_cx, 7 * l.tot_s, l.has_scx, err))) return rc;
     if ((rc = put(e, l.d_sfin, scale_fx, l.B, l.has_sfx, err))) return rc;
     l.rho_eval = rho;
+    l.has_xev = xev;
     rc = admit_impl(e, lane, 1, false, err);
-    l.has_lam = l.has_mu = l.has_scx = l.has_sfx = false;
+    l.has_lam = l.has_mu = l.has_scx = l.has_sfx = l.has_xev = false;
     if (rc) return rc;
     if ((rc = tp_collect(e, lane, err))) return rc;
     if (l.B > 0) {
