@@ -172,6 +172,20 @@ int ualm_wait_batch(ualm_ctx_t *ctx, int ticket, ualm_result_t *results, double 
  * problems still running stop at their next stop test with UALM_RET_STOPPED), the batch drains and complete records come back.
  * The request ends with the batch: the next batch on the lane starts without one. */
 int ualm_wait_batch_for(ualm_ctx_t *ctx, int ticket, double timeout_ms, ualm_result_t *results, double *c_xy, double *c_yaw);
+/* Problems of a submitted batch that have finished since the last poll of this ticket, without waiting for the rest.
+ * wait_ms = 0: return at once; > 0: block until at least one new problem is final or wait_ms has passed; < 0: UALM_EINVAL.
+ * idx[0 .. *n_new) = their problem indices (capacity B of the ticket); each problem is returned exactly once per ticket.
+ * Their records and coefficients are written at their problem-order positions of results / c_xy / c_yaw, the buffers and
+ * layout ualm_wait_batch takes (c_xy / c_yaw may be NULL); other entries are not touched.  *n_pending = problems not yet
+ * returned.  Every record and coefficient returned is bit for bit what ualm_wait_batch returns for that problem.
+ * ualm_wait_batch / ualm_wait_batch_for after any number of polls behave exactly as today and return all B records.
+ * A problem over the compiled limits (UALM_ELIMIT) is returned by the first poll; one the budget or a deadline stops is returned
+ * when it stops (UALM_RET_STOPPED).  A null ctx, a bad ticket, wait_ms < 0 or a null idx / n_new / n_pending is UALM_EINVAL; a
+ * ticket not in flight (also one already waited) is UALM_ESTATE.  Only tickets of ualm_submit_batch* can be polled.  The parity
+ * path publishes each problem from the solve itself; the throughput path advances only inside host calls, so each poll also
+ * runs the engine: it waits for the ticket's queued rounds, publishes what they finished and queues the next rounds. */
+int ualm_poll_batch(ualm_ctx_t *ctx, int ticket, double wait_ms, int32_t *idx, int *n_new, int *n_pending,
+                    ualm_result_t *results, double *c_xy, double *c_yaw);
 /* Evaluation budget per problem for the solves launched afterwards by every solving entry point (ualm_solve_batch,
  * ualm_solve_resident, ualm_submit_batch, ualm_solve_batch_multi through each context): max_evals = 0 (the default) is none,
  * negative values are UALM_EINVAL.  Refused (UALM_ESTATE) while a submitted batch is in flight. */

@@ -235,6 +235,16 @@ public:
     {
         check(ualm_wait_batch_for(ctx_, ticket, timeout_ms, results, c_xy, c_yaw), "ualm_wait_batch_for");
     }
+    // the problems of a submitted batch that finished since the last poll (ualm_poll_batch): their indices into idx (capacity B),
+    // their records and coefficients at their problem-order places of results / c_xy / c_yaw (the buffers waitBatch takes; c_xy /
+    // c_yaw may be null).  Returns how many; *pending = problems not returned yet.  wait_ms > 0 blocks until one is new or wait_ms
+    // has passed.  waitBatch afterwards returns the whole batch as before
+    int pollBatch(int ticket, double wait_ms, int32_t *idx, int *pending, ualm_result_t *results, double *c_xy, double *c_yaw)
+    {
+        int n_new = 0;
+        check(ualm_poll_batch(ctx_, ticket, wait_ms, idx, &n_new, pending, results, c_xy, c_yaw), "ualm_poll_batch");
+        return n_new;
+    }
 
     // What the MPC receives and tracks, for the batch solved last on the selected lane (ualm_mpc_export_batch): the SE2Traj message
     // arrays of PlanManager (plan_manager.cpp:151-185), the MPC side's own MINCO over them (traj_anal.hpp:125-181) and the largest

@@ -119,6 +119,7 @@ def lib():
         L.ualm_submit_batch.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, dp, C.c_int, C.POINTER(C.c_int)]
         L.ualm_wait_batch.argtypes = [vp, C.c_int, C.POINTER(Result), dp, dp]
         L.ualm_wait_batch_for.argtypes = [vp, C.c_int, C.c_double, C.POINTER(Result), dp, dp]
+        L.ualm_poll_batch.argtypes = [vp, C.c_int, C.c_double, ip, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(Result), dp, dp]
         L.ualm_set_budget.argtypes = [vp, C.c_int32]
         L.ualm_mark_begin.argtypes = [vp]
         L.ualm_mark_end.argtypes = [vp, C.POINTER(C.c_float)]
@@ -130,7 +131,7 @@ def lib():
         L.ualm_submit_batch_env.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, dp, ip, C.c_int, C.POINTER(C.c_int)]
         L.ualm_solve_batch_multi_env.argtypes = [C.POINTER(vp), C.c_int, C.c_int, ip, ip, dp, dp, dp, dp, ip, C.POINTER(Result), dp, dp]
         for name in ("ualm_reset_stream", "ualm_set_map_f64", "ualm_max_lanes", "ualm_select_lane", "ualm_submit_batch", "ualm_wait_batch",
-                     "ualm_wait_batch_for", "ualm_set_budget",
+                     "ualm_wait_batch_for", "ualm_poll_batch", "ualm_set_budget",
                      "ualm_mark_begin", "ualm_mark_end", "ualm_solve_batch_multi", "ualm_pack_records_device_async", "ualm_select_env",
                      "ualm_upload_env", "ualm_solve_batch_env", "ualm_submit_batch_env", "ualm_solve_batch_multi_env"):
             getattr(L, name).restype = C.c_int

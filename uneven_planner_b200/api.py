@@ -145,13 +145,41 @@ class BatchALMTrajOpt:
         UALM_RET_STOPPED) and the complete records of the drained batch come back."""
         pb, _ = self._tickets.pop(ticket)
         if out is None:
-            out = ((Result * pb.B)(), np.zeros(int(12 * pb.N.astype(np.int64).sum())), np.zeros(int(6 * pb.M.astype(np.int64).sum())))
+            out = self.outputs(pb)
         res, cxy, cyaw = out
         if timeout_ms is None:
             _check(self.L.ualm_wait_batch(self.h, int(ticket), res, _p(cxy), _p(cyaw)))
         else:
             _check(self.L.ualm_wait_batch_for(self.h, int(ticket), float(timeout_ms), res, _p(cxy), _p(cyaw)))
         return res, cxy, cyaw
+
+    @staticmethod
+    def outputs(pb):
+        """Empty (results, c_xy, c_yaw) for batch `pb`, the buffers wait(out=) and poll(out) fill."""
+        return (Result * pb.B)(), np.zeros(int(12 * pb.N.astype(np.int64).sum())), np.zeros(int(6 * pb.M.astype(np.int64).sum()))
+
+    def poll(self, ticket, out, wait_ms=0.0):
+        """ualm_poll_batch: the problems of the ticket's batch that finished since the last poll, without waiting for the rest.
+        Their records and coefficients go to their problem-order places in `out` = (results, c_xy, c_yaw), as wait(out=) fills them
+        (c_xy / c_yaw may be None); nothing else in `out` is touched.  wait_ms > 0 blocks until at least one problem is new or
+        wait_ms has passed.  Returns (new problem indices as an int32 array, number of problems not yet returned).  wait(ticket)
+        afterwards returns the whole batch as before."""
+        if ticket not in getattr(self, "_tickets", {}):
+            raise ValueError("poll: %r is not a ticket in flight on this context" % (ticket,))
+        wait_ms = float(wait_ms)
+        if not wait_ms >= 0.0:
+            raise ValueError("poll: wait_ms must be >= 0")
+        pb = self._tickets[ticket][0]
+        res, cxy, cyaw = out
+        if not isinstance(res, C.Array) or res._type_ is not Result or len(res) != pb.B:
+            raise ValueError("poll: out[0] must be a ctypes array of %d Result records" % pb.B)
+        for a, n, name in ((cxy, 12 * int(pb.N.astype(np.int64).sum()), "c_xy"), (cyaw, 6 * int(pb.M.astype(np.int64).sum()), "c_yaw")):
+            if a is not None and (not isinstance(a, np.ndarray) or a.dtype != np.float64 or not a.flags.c_contiguous or a.size != n):
+                raise ValueError("poll: out %s must be None or a contiguous float64 array of %d entries" % (name, n))
+        idx = np.zeros(max(pb.B, 1), np.int32)
+        n_new, n_pending = C.c_int(), C.c_int()
+        _check(self.L.ualm_poll_batch(self.h, int(ticket), wait_ms, _p(idx, ip), C.byref(n_new), C.byref(n_pending), res, _p(cxy), _p(cyaw)))
+        return idx[:n_new.value].copy(), n_pending.value
 
     # ---- three-step path -------------------------------------------------------------
     def upload(self, pb):

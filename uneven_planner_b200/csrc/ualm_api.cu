@@ -88,10 +88,12 @@ struct Lane {
     // cancel stream while the kernels run.  (A word in mapped pinned host memory, read over PCIe at every stop test, made the bench
     // step 5 % slower on an H100 80GB HBM3 at a 400 W power limit.)
     int *d_cancel = nullptr;
+    ualm_mbox::Mailbox mbox;             // results of a submitted batch as its problems finish (ualm_poll_batch)
     void release()
     {
         if (d_cancel) cudaFree(d_cancel);
         d_cancel = nullptr;
+        mbox.release();
         d_desc.release(); d_order.release(); d_queue.release(); d_eidx.release();
         DevBuf<double> *bufs[] = {&d_x0, &d_x, &d_xev, &d_lambda, &d_mu, &d_scale_cx, &d_hx, &d_gx, &d_lm_s, &d_lm_y, &d_lm_aux, &d_fac,
                                   &d_scr, &d_ws, &d_cxy, &d_cyaw, &d_f, &d_grad, &d_sfx};
@@ -410,6 +412,7 @@ static BatchPtrs batch_ptrs(ualm_ctx *c)
     b.c_xy = l->d_cxy.p; b.c_yaw = l->d_cyaw.p; b.results = l->d_res.p; b.piece_T = l->d_pieceT.p; b.f_out = l->d_f.p; b.grad_out = l->d_grad.p;
     b.scale_fx_io = l->d_sfx.p;
     b.prof = c->profile ? l->d_prof.p : nullptr;
+    b.mbox = ualm_mbox::Ptrs{};
     return b;
 }
 
@@ -617,10 +620,9 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
     return UALM_OK;
 }
 
-extern "C" int ualm_solve_resident(ualm_ctx_t *c)
+// the solve launches of the selected lane's batch; `publish`: every problem also goes to the lane's mailbox as it ends (submit only)
+static int solve_launch(ualm_ctx *c, bool publish)
 {
-    if (!c) return fail(UALM_EINVAL, "null ctx");
-    if (c->tp) TP_CALL(ualm_tp::tp_admit(c->tp, c->cur, err));      // joins the pool of running trajectories; ualm_sync / download drive the rounds
     Lane *l = c->b;
     // (the upload checked that every environment of the batch is bound, and nothing unbinds one)
     if (!l->have_batch) return fail(UALM_ESTATE, "set_params, set_map and upload must precede solve");
@@ -644,6 +646,7 @@ extern "C" int ualm_solve_resident(ualm_ctx_t *c)
             bp.order = l->d_order.p + cl.r0;
             bp.n_active = cl.r1 - cl.r0;
             bp.n_leader_slots = 4 / cl.G;
+            if (publish) bp.mbox = l->mbox.device();
             // the launch's environment: its parameters and grid are the launch's grid constants, the solve reads them as before
             DevParams dp = c->envs[cl.env].dp;
             dp.cancel = l->d_cancel;
@@ -657,6 +660,13 @@ extern "C" int ualm_solve_resident(ualm_ctx_t *c)
     CK(cudaEventRecord(l->ev1, l->stream));
     l->solved = true;
     return UALM_OK;
+}
+
+extern "C" int ualm_solve_resident(ualm_ctx_t *c)
+{
+    if (!c) return fail(UALM_EINVAL, "null ctx");
+    if (c->tp) TP_CALL(ualm_tp::tp_admit(c->tp, c->cur, err));      // joins the pool of running trajectories; ualm_sync / download drive the rounds
+    return solve_launch(c, false);
 }
 
 extern "C" int ualm_sync(ualm_ctx_t *c)
@@ -759,7 +769,7 @@ extern "C" int ualm_submit_batch_env(ualm_ctx_t *c, int B, const int32_t *N, con
         if (int rc = check_envs(c, B, env)) return rc;
         std::string em;
         int rc = ualm_tp::tp_upload(c->tp, lane, B, N, M, env, bnd, total_time, inner_xy, inner_yaw, &em);
-        if (!rc) rc = ualm_tp::tp_admit(c->tp, lane, &em);
+        if (!rc) rc = ualm_tp::tp_admit(c->tp, lane, &em, true);
         if (rc) return fail(rc, em);
         *ticket = lane; c->next_submit = (lane + 1) % depth;
         return UALM_OK;
@@ -768,7 +778,12 @@ extern "C" int ualm_submit_batch_env(ualm_ctx_t *c, int B, const int32_t *N, con
     const int keep = c->cur;
     int rc = ualm_select_lane(c, lane);
     if (!rc) rc = ualm_upload_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env);
-    if (!rc) rc = ualm_solve_resident(c);
+    if (!rc) {
+        Lane &l = c->lanes[lane];
+        const cudaError_t e = l.mbox.begin(B, N, M, l.skip.data());
+        if (e != cudaSuccess) rc = fail(UALM_ENOCUDA, std::string("result mailbox: ") + cudaGetErrorString(e));
+    }
+    if (!rc) rc = solve_launch(c, true);
     if (!rc) { c->lanes[lane].in_flight = true; *ticket = lane; c->next_submit = (lane + 1) % depth; }
     c->cur = keep; c->b = &c->lanes[keep];
     return rc;
@@ -817,6 +832,33 @@ extern "C" int ualm_wait_batch_for(ualm_ctx_t *c, int ticket, double timeout_ms,
         std::this_thread::yield();
     }
     return ualm_wait_batch(c, ticket, results, c_xy, c_yaw);
+}
+
+// the problems of a submitted batch that have finished since the last poll of the ticket: read from the lane's mailbox, which the
+// solve fills as each problem ends (ualm_mailbox.h).  wait_ms > 0: yield-poll the flags until one is new or the time is up
+extern "C" int ualm_poll_batch(ualm_ctx_t *c, int ticket, double wait_ms, int32_t *idx, int *n_new, int *n_pending, ualm_result_t *results,
+                               double *c_xy, double *c_yaw)
+{
+    if (!c || ticket < 0 || ticket >= UALM_MAX_LANES) return fail(UALM_EINVAL, "bad ticket");
+    if (!(wait_ms >= 0.0)) return fail(UALM_EINVAL, "wait_ms must be >= 0");
+    if (!idx || !n_new || !n_pending) return fail(UALM_EINVAL, "null argument");
+    if (c->tp) TP_CALL(ualm_tp::tp_poll(c->tp, ticket, wait_ms, idx, n_new, n_pending, results, c_xy, c_yaw, err));
+    Lane &l = c->lanes[ticket];
+    if (!l.in_flight) return fail(UALM_ESTATE, "ticket is not in flight");
+    CK(cudaSetDevice(c->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    int n = 0;
+    while (true) {
+        n = l.mbox.collect(idx, results, c_xy, c_yaw);
+        if (n > 0 || l.mbox.pending() == 0 || wait_ms == 0.0) break;
+        const cudaError_t q = cudaEventQuery(l.ev1);     // a failed launch is reported, not waited out
+        if (q != cudaSuccess && q != cudaErrorNotReady) CK(q);
+        if (std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() >= wait_ms) break;
+        std::this_thread::yield();
+    }
+    *n_new = n;
+    *n_pending = l.mbox.pending();
+    return UALM_OK;
 }
 
 extern "C" int ualm_set_budget(ualm_ctx_t *c, int32_t max_evals)

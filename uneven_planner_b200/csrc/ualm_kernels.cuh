@@ -23,6 +23,7 @@
 
 #include "ualm.h"
 #include "ualm_detmath.h"
+#include "ualm_mailbox.h"
 
 #define UALM_THREADS 32         // threads per warp slot
 #define UALM_WPB 4              // warp slots per CTA (4 / 2 / 1 trajectories with 1 / 2 / 4 warps each)
@@ -117,6 +118,7 @@ struct BatchPtrs {
     // eval entry
     R *f_out, *grad_out, *scale_fx_io;
     long long *prof;         // optional [grid][UALM_NPROF] phase cycle counters (lane 0 of each warp)
+    ualm_mbox::Ptrs mbox;    // solve_kernel: the lane's result mailbox (ualm_poll_batch), flag null = publish nothing
 };
 
 // per-sample scratch fields (SoA: scratch[field * S + s])
@@ -2155,6 +2157,26 @@ __device__ UALM_NOINLINE int slot_next(Traj &t, const BatchPtrs &bp, int *adopt,
     return join ? -2 : -1;
 }
 
+// ualm_poll_batch: copy the coefficients and the record of problem `prob`, which this warp has just written to the lane's outputs,
+// into the lane's mailbox and raise the problem's flag (ualm_mailbox.h).  Each lane copies the coefficient entries it wrote itself;
+// the record was written by lane 0 before the warp barrier that precedes the call.  Nothing without a mailbox (every launch not
+// made by ualm_submit_batch*).  Not inlined, like alm_exit, and the test is in here: with it at the call site solve_kernel spilled
+// 4 bytes more
+__device__ UALM_NOINLINE void publish_problem(const BatchPtrs &bp, int prob, int lane)
+{
+    if (!bp.mbox.flag) return;
+    const ProbDesc *pd = bp.desc + prob;
+    const ualm_mbox::Ptrs &mb = bp.mbox;
+    const long long ox = pd->off_cxy, oy = pd->off_cyaw;
+    const int nxy = 12 * pd->N, nyaw = 6 * pd->M;
+    for (int q = lane; q < nxy; q += 32) mb.c_xy[ox + q] = bp.c_xy[ox + q];
+    for (int q = lane; q < nyaw; q += 32) mb.c_yaw[oy + q] = bp.c_yaw[oy + q];
+    static_assert(sizeof(ualm_result_t) % 8 == 0 && sizeof(ualm_result_t) / 8 <= 32, "the record is copied as one 8-byte word per lane");
+    if (lane < (int)(sizeof(ualm_result_t) / 8))
+        ((long long *)(mb.res + prob))[lane] = ((const long long *)(bp.results + prob))[lane];
+    ualm_mbox::raise_flag_warp(mb, prob, lane);
+}
+
 // one problem on a leader slot, from its setup to its result record (`adopt` = the slot's adoption state word, or null).  Not
 // inlined: the loop over the queue around it would otherwise add spill to the solve
 __device__ UALM_NOINLINE void solve_problem(Traj &t, const BatchPtrs &bp, const DevParams &p, const DevMap &map, const SmemLayout &L, unsigned sm, int slot,
@@ -2236,6 +2258,7 @@ __device__ UALM_NOINLINE void solve_problem(Traj &t, const BatchPtrs &bp, const 
         }
     }
     UALM_SYNC();
+    publish_problem(bp, prob, lane);
 }
 
 // full solve: optimizeSE2Traj (alm_traj_opt.cpp:168-278).  Each leader slot of a CTA solves problems from the launch's queue until

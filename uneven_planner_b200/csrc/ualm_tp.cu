@@ -10,6 +10,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <thread>
 #include <vector>
 
 namespace ualm_tp {
@@ -58,6 +59,10 @@ struct TpLane {
     int launches = 0;
     double rho_eval = 1.0;
     bool has_lam = false, has_mu = false, has_scx = false, has_sfx = false, has_xev = false;   // has_xev: admit from d_xev, not d_x0
+    // a submitted batch (ualm_submit_batch): its problems go to the mailbox as they finish (tp_poll); d_pub = published already
+    bool publish = false;
+    ualm_mbox::Mailbox mbox;
+    Buf<int> d_pub;
 };
 
 struct TpEngine {
@@ -216,7 +221,7 @@ void tp_destroy(TpEngine *e)
     for (auto &l : e->lanes) {
         l.d_ad.release(); l.d_gd.release(); l.d_x0.release(); l.d_xev.release(); l.d_cxy.release(); l.d_cyaw.release(); l.d_xout.release(); l.d_f.release(); l.d_grad.release();
         l.d_hx.release(); l.d_gx.release(); l.d_sfx.release(); l.d_scx.release(); l.d_lam.release(); l.d_mu.release(); l.d_scin.release(); l.d_sfin.release();
-        l.d_offs.release(); l.d_res.release();
+        l.d_offs.release(); l.d_res.release(); l.d_pub.release(); l.mbox.release();
         if (l.ev0) cudaEventDestroy(l.ev0);
         if (l.ev1) cudaEventDestroy(l.ev1);
     }
@@ -513,10 +518,21 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, std::s
     return UALM_OK;
 }
 
-int tp_admit(TpEngine *e, int lane, std::string *err)
+int tp_admit(TpEngine *e, int lane, std::string *err, bool publish)
 {
     if (lane < 0 || lane >= TP_LANES) { if (err) *err = "lane out of range"; return UALM_EINVAL; }
-    return admit_impl(e, lane, 0, false, err);
+    TpLane &l = e->lanes[lane];
+    if (publish && l.have_batch && !l.in_flight) {      // (admit_impl refuses the other cases)
+        std::vector<unsigned char> skip(l.B);
+        for (int b = 0; b < l.B; b++) skip[b] = l.N[b] > TP_NMAX || l.M[b] > TP_MMAX;
+        TCK(cudaSetDevice(e->device));
+        TCK(l.mbox.begin(l.B, l.N.data(), l.M.data(), skip.data()));
+        TCK(l.d_pub.ensure(l.B));
+        if (l.B > 0) TCK(cudaMemsetAsync(l.d_pub.p, 0, sizeof(int) * l.B, e->stream));   // ordered before admission's synchronise
+    }
+    const int rc = admit_impl(e, lane, 0, false, err);
+    if (rc == UALM_OK) l.publish = publish;
+    return rc;
 }
 
 static size_t kb_smem_bytes(TpEngine *e, bool tma)
@@ -651,7 +667,36 @@ int tp_collect(TpEngine *e, int lane, std::string *err, double timeout_ms)
     e->live -= (int)l.slots.size();
     l.slots.clear();
     for (int q = 0; q < TP_SUBGROUPS; q++) { const int g = lane * TP_SUBGROUPS + q; e->glive[g] = 0; e->gscale[g] = 0; e->gcompact[g] = false; }
-    l.in_flight = false; l.collected = true;
+    l.in_flight = false; l.collected = true; l.publish = false;
+    return UALM_OK;
+}
+
+int tp_poll(TpEngine *e, int lane, double wait_ms, int32_t *idx, int *n_new, int *n_pending, ualm_result_t *results, double *c_xy, double *c_yaw,
+            std::string *err)
+{
+    TpLane &l = e->lanes[lane];
+    if (!l.in_flight || !l.publish) { if (err) *err = "ticket is not in flight"; return UALM_ESTATE; }
+    TCK(cudaSetDevice(e->device));
+    const auto t0 = std::chrono::steady_clock::now();
+    int n = l.mbox.collect(idx, results, c_xy, c_yaw);      // the problems over the compiled limits, published at submit
+    // the engine advances only inside host calls: each try is one iteration of tp_collect's loop with the publication in place of
+    // the counter read
+    while (n == 0 && l.mbox.pending() > 0) {
+        for (int q = 0; q < TP_SUBGROUPS; q++) TCK(cudaStreamSynchronize(e->gstream[lane * TP_SUBGROUPS + q]));
+        if (e->f32()) publish_kernel<float><<<l.B, 128, 0, e->stream>>>(e->E, l.d_gd.p, l.B, l.d_pub.p, l.mbox.device());
+        else publish_kernel<double><<<l.B, 128, 0, e->stream>>>(e->E, l.d_gd.p, l.B, l.d_pub.p, l.mbox.device());
+        TCK(cudaGetLastError());
+        TCK(cudaStreamSynchronize(e->stream));         // before the next rounds are queued: the slots it reads stay as they are
+        n = l.mbox.collect(idx, results, c_xy, c_yaw);
+        if (l.mbox.pending() > 0) {
+            const int rc = run_rounds(e, e->chunk, err);
+            if (rc) return rc;
+        }
+        if (std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() >= wait_ms) break;
+        std::this_thread::yield();
+    }
+    *n_new = n;
+    *n_pending = l.mbox.pending();
     return UALM_OK;
 }
 

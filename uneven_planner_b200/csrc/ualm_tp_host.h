@@ -21,7 +21,12 @@ int tp_set_map(TpEngine *e, int env, const ualm_map_geom_t *g, const float *cell
 // problem (NULL = all 0), in range and bound (the caller checks)
 int tp_upload(TpEngine *e, int lane, int B, const int32_t *N, const int32_t *M, const int32_t *env, const double *bnd, const double *total_time,
               const double *inner_xy, const double *inner_yaw, std::string *err);
-int tp_admit(TpEngine *e, int lane, std::string *err);                       // asynchronous
+// asynchronous.  publish: the batch's problems go to the lane's result mailbox as they finish (ualm_submit_batch, for tp_poll)
+int tp_admit(TpEngine *e, int lane, std::string *err, bool publish = false);
+// ualm_poll_batch on a lane admitted with publish: one step of the engine per try (wait for the lane's queued rounds, publish its
+// finished problems, queue the next rounds of every live group), repeated until a problem is new or wait_ms has passed
+int tp_poll(TpEngine *e, int lane, double wait_ms, int32_t *idx, int *n_new, int *n_pending, ualm_result_t *results, double *c_xy, double *c_yaw,
+            std::string *err);
 // blocks: rounds until the lane's batch is done.  timeout_ms >= 0: once that much time has passed since the call, the lane's
 // cancel word is raised before the next rounds (its trajectories stop at their next stop test)
 int tp_collect(TpEngine *e, int lane, std::string *err, double timeout_ms = -1.0);

@@ -4,6 +4,7 @@
 #pragma once
 
 #include "ualm_tp_kernels.cuh"
+#include "ualm_mailbox.h"
 
 namespace ualm_tp {
 
@@ -743,14 +744,11 @@ __global__ void __launch_bounds__(TP_KB_THREADS) ks_kernel(const __grid_constant
 // ---------------------------------------------------------------------------------------------------------------------
 struct GatherDesc { int slot, N, M, pad; long long off_cxy, off_cyaw, off_x, off_s; };
 
+// problem b (admitted, in slot g.slot) -> the outputs given (null = not wanted), by one CTA
 template <class R>
-__global__ void gather_kernel(const __grid_constant__ TpPool E, const GatherDesc *gd, int B, ualm_result_t *res, double *c_xy, double *c_yaw, double *x_out,
-                              double *f_out, double *grad_out, double *hx_out, double *gx_out, double *sfx_out, double *scx_out)
+__device__ void gather_one(const TpPool &E, const GatherDesc &g, int b, ualm_result_t *res, double *c_xy, double *c_yaw, double *x_out, double *f_out,
+                           double *grad_out, double *hx_out, double *gx_out, double *sfx_out, double *scx_out)
 {
-    const int b = blockIdx.x;
-    if (b >= B) return;
-    const GatherDesc g = gd[b];
-    if (g.slot < 0) return;        // over the compiled limits: its record (UALM_ELIMIT) and zero outputs were written at admission
     const TpState *st = E.st + g.slot;
     const int N = g.N, M = g.M, n = st->n, S = st->S;
     const double *cd = E.cd + (size_t)g.slot * TP_CSTRIDE;
@@ -776,6 +774,38 @@ __global__ void gather_kernel(const __grid_constant__ TpPool E, const GatherDesc
         }
         if (f_out) f_out[b] = st->f_last;
         if (sfx_out) sfx_out[b] = st->scale_fx;
+    }
+}
+
+template <class R>
+__global__ void gather_kernel(const __grid_constant__ TpPool E, const GatherDesc *gd, int B, ualm_result_t *res, double *c_xy, double *c_yaw, double *x_out,
+                              double *f_out, double *grad_out, double *hx_out, double *gx_out, double *sfx_out, double *scx_out)
+{
+    const int b = blockIdx.x;
+    if (b >= B) return;
+    const GatherDesc g = gd[b];
+    if (g.slot < 0) return;        // over the compiled limits: its record (UALM_ELIMIT) and zero outputs were written at admission
+    gather_one<R>(E, g, b, res, c_xy, c_yaw, x_out, f_out, grad_out, hx_out, gx_out, sfx_out, scx_out);
+}
+
+// finished problems of a batch in flight -> the lane's result mailbox (ualm_poll_batch, ualm_mailbox.h), one CTA per problem.  A slot
+// is freed only when its batch is collected, so a slot in PH_DONE holds the final state gather_kernel will read: the mailbox gets
+// the bits ualm_wait_batch returns.  pub[b] marks problem b published (device memory: the device never reads the mailbox).  Runs
+// while none of the lane's rounds does
+template <class R>
+__global__ void publish_kernel(const __grid_constant__ TpPool E, const GatherDesc *gd, int B, int *pub, const __grid_constant__ ualm_mbox::Ptrs mb)
+{
+    const int b = blockIdx.x;
+    if (b >= B) return;
+    const GatherDesc g = gd[b];
+    if (g.slot < 0 || pub[b] || E.st[g.slot].phase != PH_DONE) return;     // the same for every thread of the CTA
+    gather_one<R>(E, g, b, mb.res, mb.c_xy, mb.c_yaw, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, nullptr);
+    __threadfence_system();
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        __threadfence_system();
+        *(volatile int32_t *)(mb.flag + b) = 1;
+        pub[b] = 1;
     }
 }
 
