@@ -33,7 +33,9 @@ extern "C" {
 #define UALM_ELIMIT (-4)    /* problem exceeds compiled limits (N, M, int_K) */
 
 /* ret_code of a problem whose solve was stopped early (no such exit exists in the reference; it is modelled on its earlyExit).
- * stop = (max_evals > 0 && n_evals >= max_evals) || the lane's cancel request, tested after every accepted line search (where
+ * Three causes stop a problem: its evaluation budget (ualm_set_budget), a deadline (ualm_wait_batch_for, which cancels every
+ * problem of its batch) and a cancel of the problem itself (ualm_cancel_problems).
+ * stop = (max_evals > 0 && n_evals >= max_evals) || the problem's stop word is raised, tested after every accepted line search (where
  * earlyExit tests k > 1000): L-BFGS then returns CANCELED, the ALM loop updates the duals and judges convergence as after any
  * cancel, and ends with UALM_RET_STOPPED even when that test passes (res_h / res_g tell whether epsilon_con was met).  The ALM
  * loop tests `stop` once more after judgeConvergence, so no inner solve starts after it holds.  A running line search is not
@@ -70,7 +72,8 @@ void ualm_map_geometry(double map_size_x, double map_size_y, double xy_resolutio
  *      alm_traj_opt.h:142) ---- */
 typedef struct {
     int32_t ret_code;        /* 0 converged / 1 L-BFGS hard error / 2 ALM max_iter (the reference's codes); UALM_RET_STOPPED (3):
-                                the evaluation budget (ualm_set_budget) or a deadline (ualm_wait_batch_for) stopped it, see below;
+                                the evaluation budget (ualm_set_budget), a deadline (ualm_wait_batch_for) or a cancel
+                                (ualm_cancel_problems) stopped it, see above;
                                 UALM_ELIMIT (-4): this problem exceeds the compiled limits (N <= 64, M <= 128) and was not solved --
                                 the rest of its batch is unaffected */
     int32_t outer_iters;
@@ -168,9 +171,9 @@ int ualm_submit_batch(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M
 int ualm_submit_batch_env(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
                           const double *inner_xy, const double *inner_yaw, const int32_t *env, int depth, int *ticket);
 int ualm_wait_batch(ualm_ctx_t *ctx, int ticket, ualm_result_t *results, double *c_xy, double *c_yaw);
-/* ualm_wait_batch with a deadline: if the batch is not complete timeout_ms after the call, the lane's cancel request is set (the
- * problems still running stop at their next stop test with UALM_RET_STOPPED), the batch drains and complete records come back.
- * The request ends with the batch: the next batch on the lane starts without one. */
+/* ualm_wait_batch with a deadline: if the batch is not complete timeout_ms after the call, every problem of the batch is cancelled
+ * as by ualm_cancel_problems (the problems still running stop at their next stop test with UALM_RET_STOPPED), the batch drains
+ * and complete records come back.  The request ends with the batch: the next batch on the lane starts without one. */
 int ualm_wait_batch_for(ualm_ctx_t *ctx, int ticket, double timeout_ms, ualm_result_t *results, double *c_xy, double *c_yaw);
 /* Problems of a submitted batch that have finished since the last poll of this ticket, without waiting for the rest.
  * wait_ms = 0: return at once; > 0: block until at least one new problem is final or wait_ms has passed; < 0: UALM_EINVAL.
@@ -186,6 +189,16 @@ int ualm_wait_batch_for(ualm_ctx_t *ctx, int ticket, double timeout_ms, ualm_res
  * runs the engine: it waits for the ticket's queued rounds, publishes what they finished and queues the next rounds. */
 int ualm_poll_batch(ualm_ctx_t *ctx, int ticket, double wait_ms, int32_t *idx, int *n_new, int *n_pending,
                     ualm_result_t *results, double *c_xy, double *c_yaw);
+/* Stop the listed problems of a submitted batch.  Each one stops at its next stop test, exactly as a deadline stops it
+ * (UALM_RET_STOPPED, the trajectory of its last evaluation).  Problems that are already final keep their records bit for bit.
+ * A problem not yet started runs to its first stop test.  Every other problem of the batch, and every other ticket, is
+ * unaffected bit for bit.  Cancelled problems come back through ualm_poll_batch / ualm_wait_batch like any other.
+ * A null ctx, a bad ticket, n < 0, a null idx with n > 0 or an index outside [0, B) is UALM_EINVAL; a ticket not in flight (also
+ * one already waited) is UALM_ESTATE; a refused call raises nothing.  n = 0 does nothing; duplicate indices and repeated calls are
+ * harmless.  Only tickets of ualm_submit_batch* can be cancelled, from the thread that polls.  The parity path raises the stop
+ * words by a copy that runs while the kernels hold the SMs; on the throughput path, which advances only inside host calls, the
+ * cancel takes effect at the rounds that the next ualm_poll_batch / ualm_wait_batch* queues. */
+int ualm_cancel_problems(ualm_ctx_t *ctx, int ticket, int n, const int32_t *idx);
 /* Evaluation budget per problem for the solves launched afterwards by every solving entry point (ualm_solve_batch,
  * ualm_solve_resident, ualm_submit_batch, ualm_solve_batch_multi through each context): max_evals = 0 (the default) is none,
  * negative values are UALM_EINVAL.  Refused (UALM_ESTATE) while a submitted batch is in flight. */

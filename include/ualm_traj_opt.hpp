@@ -245,6 +245,9 @@ public:
         check(ualm_poll_batch(ctx_, ticket, wait_ms, idx, &n_new, pending, results, c_xy, c_yaw), "ualm_poll_batch");
         return n_new;
     }
+    // stop the problems idx[0, n) of a submitted batch at their next stop test (ualm_cancel_problems): they come back through
+    // pollBatch / waitBatch with UALM_RET_STOPPED, or with their own result if they were final first; the rest is unaffected
+    void cancelProblems(int ticket, int n, const int32_t *idx) { check(ualm_cancel_problems(ctx_, ticket, n, idx), "ualm_cancel_problems"); }
 
     // What the MPC receives and tracks, for the batch solved last on the selected lane (ualm_mpc_export_batch): the SE2Traj message
     // arrays of PlanManager (plan_manager.cpp:151-185), the MPC side's own MINCO over them (traj_anal.hpp:125-181) and the largest

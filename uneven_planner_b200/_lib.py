@@ -11,7 +11,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libualm.so")
 
 UALM_OK, UALM_ENOCUDA, UALM_EINVAL, UALM_ESTATE, UALM_ELIMIT = 0, -1, -2, -3, -4
-UALM_RET_STOPPED = 3   # ret_code of a problem stopped by the evaluation budget or a deadline (include/ualm.h)
+UALM_RET_STOPPED = 3   # ret_code of a problem stopped by the evaluation budget, a deadline or a cancel (include/ualm.h)
 UALM_MAX_ENVS = 4      # environments (parameter set + map grid) per context (include/ualm.h, ualm_select_env)
 
 
@@ -120,6 +120,7 @@ def lib():
         L.ualm_wait_batch.argtypes = [vp, C.c_int, C.POINTER(Result), dp, dp]
         L.ualm_wait_batch_for.argtypes = [vp, C.c_int, C.c_double, C.POINTER(Result), dp, dp]
         L.ualm_poll_batch.argtypes = [vp, C.c_int, C.c_double, ip, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(Result), dp, dp]
+        L.ualm_cancel_problems.argtypes = [vp, C.c_int, C.c_int, ip]
         L.ualm_set_budget.argtypes = [vp, C.c_int32]
         L.ualm_mark_begin.argtypes = [vp]
         L.ualm_mark_end.argtypes = [vp, C.POINTER(C.c_float)]
@@ -131,7 +132,7 @@ def lib():
         L.ualm_submit_batch_env.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, dp, ip, C.c_int, C.POINTER(C.c_int)]
         L.ualm_solve_batch_multi_env.argtypes = [C.POINTER(vp), C.c_int, C.c_int, ip, ip, dp, dp, dp, dp, ip, C.POINTER(Result), dp, dp]
         for name in ("ualm_reset_stream", "ualm_set_map_f64", "ualm_max_lanes", "ualm_select_lane", "ualm_submit_batch", "ualm_wait_batch",
-                     "ualm_wait_batch_for", "ualm_poll_batch", "ualm_set_budget",
+                     "ualm_wait_batch_for", "ualm_poll_batch", "ualm_cancel_problems", "ualm_set_budget",
                      "ualm_mark_begin", "ualm_mark_end", "ualm_solve_batch_multi", "ualm_pack_records_device_async", "ualm_select_env",
                      "ualm_upload_env", "ualm_solve_batch_env", "ualm_submit_batch_env", "ualm_solve_batch_multi_env"):
             getattr(L, name).restype = C.c_int

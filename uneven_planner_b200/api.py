@@ -181,6 +181,22 @@ class BatchALMTrajOpt:
         _check(self.L.ualm_poll_batch(self.h, int(ticket), wait_ms, _p(idx, ip), C.byref(n_new), C.byref(n_pending), res, _p(cxy), _p(cyaw)))
         return idx[:n_new.value].copy(), n_pending.value
 
+    def cancel(self, ticket, idx):
+        """ualm_cancel_problems: stop the problems `idx` (integer indices into the ticket's batch) at their next stop test.  Each comes
+        back through poll / wait, with ret_code UALM_RET_STOPPED or, if it was final first, its own result; every other problem and
+        ticket is unaffected.  Duplicates and repeated calls are harmless.  Nothing is cancelled when an argument is refused."""
+        if ticket not in getattr(self, "_tickets", {}):
+            raise ValueError("cancel: %r is not a ticket in flight on this context" % (ticket,))
+        a = np.asarray(idx)
+        if a.ndim > 1 or (a.size and not np.issubdtype(a.dtype, np.integer)):
+            raise ValueError("cancel: idx must be a 1-D sequence of problem indices")
+        a = np.ascontiguousarray(a.reshape(-1), np.int64)
+        B = self._tickets[ticket][0].B
+        if a.size and (a.min() < 0 or a.max() >= B):
+            raise ValueError("cancel: problem index out of range [0, %d)" % B)
+        a = a.astype(np.int32)
+        _check(self.L.ualm_cancel_problems(self.h, int(ticket), int(a.size), _p(a, ip)))
+
     # ---- three-step path -------------------------------------------------------------
     def upload(self, pb):
         self.pb = pb

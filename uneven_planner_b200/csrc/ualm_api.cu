@@ -84,15 +84,22 @@ struct Lane {
     DevBuf<double> d_pieceT, d_feas;
     float last_ms = 0.f;
     int last_launches = 0;
-    // cancel word of the lane's solves (ualm_wait_batch_for), in device memory: the host raises it by a copy on the context's
-    // cancel stream while the kernels run.  (A word in mapped pinned host memory, read over PCIe at every stop test, made the bench
-    // step 5 % slower on an H100 80GB HBM3 at a 400 W power limit.)
-    int *d_cancel = nullptr;
+    // stop words of the lane's solves, one per problem (ualm_cancel_problems, ualm_wait_batch_for), in device memory: cleared on the
+    // lane stream before every solve launch (ev_clear marks that), raised while the kernels run by copying the whole pinned mirror
+    // h_stop (grows only, like the mailbox) on the context's cancel stream after ev_clear.  Words only go from 0 to 1 during a batch
+    // and only the host writes them, so a copy of the whole mirror never lowers a word.  (A word in mapped pinned host memory, read
+    // over PCIe at every stop test, made the bench step 5 % slower on an H100 80GB HBM3 at a 400 W power limit.)
+    DevBuf<int> d_stop;
+    int *h_stop = nullptr;
+    size_t h_stop_cap = 0;
+    bool raised = false;                 // a raise copy of the batch in flight may still be queued on the cancel stream
+    cudaEvent_t ev_clear = nullptr;
     ualm_mbox::Mailbox mbox;             // results of a submitted batch as its problems finish (ualm_poll_batch)
     void release()
     {
-        if (d_cancel) cudaFree(d_cancel);
-        d_cancel = nullptr;
+        d_stop.release();
+        if (h_stop) cudaFreeHost(h_stop);
+        h_stop = nullptr; h_stop_cap = 0;
         mbox.release();
         d_desc.release(); d_order.release(); d_queue.release(); d_eidx.release();
         DevBuf<double> *bufs[] = {&d_x0, &d_x, &d_xev, &d_lambda, &d_mu, &d_scale_cx, &d_hx, &d_gx, &d_lm_s, &d_lm_y, &d_lm_aux, &d_fac,
@@ -104,6 +111,7 @@ struct Lane {
         for (int q = 0; q < NAUX + 1; q++) if (evs[q]) cudaEventDestroy(evs[q]);
         if (ev0) cudaEventDestroy(ev0);
         if (ev1) cudaEventDestroy(ev1);
+        if (ev_clear) cudaEventDestroy(ev_clear);
         if (own_stream) cudaStreamDestroy(own_stream);
         made = false;
     }
@@ -133,9 +141,8 @@ struct ualm_ctx {
     // pipeline timing (ualm_mark_begin / ualm_mark_end): events on the lanes' own streams, joined on `join`
     cudaStream_t join = nullptr;
     cudaEvent_t evA = nullptr, evB = nullptr;
-    // deadline (ualm_wait_batch_for): {0, 1} in pinned memory, copied into a lane's cancel word on the lane's stream before a launch
-    // (clear) or on `cancel` while it runs (raise); copies go through the copy engines, so they do not wait for free SMs
-    int *h_flags = nullptr;
+    // raises of the lanes' stop words (ualm_cancel_problems, ualm_wait_batch_for): copies go through the copy engines, so they do
+    // not wait for free SMs
     cudaStream_t cancel = nullptr;
 };
 
@@ -149,8 +156,7 @@ static int lane_make(ualm_ctx *c, Lane &l)
     for (int q = 0; q < Lane::NAUX + 1; q++) CK(cudaEventCreateWithFlags(&l.evs[q], cudaEventDisableTiming));
     CK(cudaEventCreate(&l.ev0));
     CK(cudaEventCreate(&l.ev1));
-    CK(cudaMalloc(&l.d_cancel, sizeof(int)));
-    CK(cudaMemset(l.d_cancel, 0, sizeof(int)));
+    CK(cudaEventCreateWithFlags(&l.ev_clear, cudaEventDisableTiming));
     (void)c;
     return UALM_OK;
 }
@@ -193,8 +199,6 @@ extern "C" int ualm_create(ualm_ctx_t **out, int device, int precision)
     if (rc == UALM_OK) {
         cudaError_t e1 = cudaStreamCreateWithFlags(&c->join, cudaStreamNonBlocking);
         if (e1 == cudaSuccess) e1 = cudaStreamCreateWithFlags(&c->cancel, cudaStreamNonBlocking);
-        if (e1 == cudaSuccess) e1 = cudaHostAlloc(&c->h_flags, 2 * sizeof(int), cudaHostAllocDefault);
-        if (e1 == cudaSuccess) { c->h_flags[0] = 0; c->h_flags[1] = 1; }
         if (e1 == cudaSuccess) e1 = cudaEventCreate(&c->evA);
         if (e1 == cudaSuccess) e1 = cudaEventCreate(&c->evB);
         if (e1 != cudaSuccess) rc = fail(UALM_ENOCUDA, std::string("context streams/events: ") + cudaGetErrorString(e1));
@@ -214,7 +218,6 @@ extern "C" int ualm_destroy(ualm_ctx_t *c)
     for (auto &l : c->lanes) l.release();
     if (c->join) cudaStreamDestroy(c->join);
     if (c->cancel) cudaStreamDestroy(c->cancel);
-    if (c->h_flags) cudaFreeHost(c->h_flags);
     if (c->evA) cudaEventDestroy(c->evA);
     if (c->evB) cudaEventDestroy(c->evB);
     delete c;
@@ -597,6 +600,7 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
     CK(l->d_lm_s.ensure(oh)); CK(l->d_lm_y.ensure(oh)); CK(l->d_scr.ensure(oscr));
     CK(l->d_ws.ensure(ows)); CK(l->d_fac.ensure(ofac)); CK(l->d_lm_aux.ensure((size_t)std::max(oaux, 1LL)));
     CK(l->d_eidx.ensure(B));
+    CK(l->d_stop.ensure((size_t)std::max(B, 1)));
     // factor arrays: entries outside the band-in-matrix positions (and the pad rows) are never written and must read 0
     if (ofac > 0) CK(cudaMemsetAsync(l->d_fac.p, 0, sizeof(double) * ofac, l->stream));
     CK(l->d_prof.ensure((size_t)std::max(B, 1) * UALM_NPROF));
@@ -628,7 +632,10 @@ static int solve_launch(ualm_ctx *c, bool publish)
     if (!l->have_batch) return fail(UALM_ESTATE, "set_params, set_map and upload must precede solve");
     CK(cudaSetDevice(c->device));
     l->last_launches = 0;
-    CK(cudaMemcpyAsync(l->d_cancel, &c->h_flags[0], sizeof(int), cudaMemcpyHostToDevice, l->stream));   // no request carries over
+    // no stop request carries over: the words are cleared before the solve, and raises are queued after ev_clear
+    if (l->h_stop) memset(l->h_stop, 0, sizeof(int) * l->h_stop_cap);
+    CK(cudaMemsetAsync(l->d_stop.p, 0, sizeof(int) * std::max(l->B, 1), l->stream));
+    CK(cudaEventRecord(l->ev_clear, l->stream));
     if (!l->cls.empty()) CK(cudaMemsetAsync(l->d_queue.p, 0, sizeof(int) * l->cls.size(), l->stream));   // every launch's queue full
     CK(cudaEventRecord(l->ev0, l->stream));
     if (l->n_active > 0) {
@@ -649,7 +656,7 @@ static int solve_launch(ualm_ctx *c, bool publish)
             if (publish) bp.mbox = l->mbox.device();
             // the launch's environment: its parameters and grid are the launch's grid constants, the solve reads them as before
             DevParams dp = c->envs[cl.env].dp;
-            dp.cancel = l->d_cancel;
+            dp.cancel = l->d_stop.p;
             dp.max_evals = c->max_evals;
             solve_kernel<<<cl.grid, UALM_THREADS * UALM_WPB, cl.smem, st>>>(bp, dp, c->envs[cl.env].dm, cl.L);
             CK(cudaGetLastError());
@@ -780,8 +787,15 @@ extern "C" int ualm_submit_batch_env(ualm_ctx_t *c, int B, const int32_t *N, con
     if (!rc) rc = ualm_upload_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env);
     if (!rc) {
         Lane &l = c->lanes[lane];
-        const cudaError_t e = l.mbox.begin(B, N, M, l.skip.data());
+        cudaError_t e = l.mbox.begin(B, N, M, l.skip.data());
         if (e != cudaSuccess) rc = fail(UALM_ENOCUDA, std::string("result mailbox: ") + cudaGetErrorString(e));
+        if (!rc && l.h_stop_cap < (size_t)std::max(B, 1)) {      // the stop words' host mirror (solve_launch clears it)
+            if (l.h_stop) cudaFreeHost(l.h_stop);
+            l.h_stop = nullptr; l.h_stop_cap = 0;
+            e = cudaHostAlloc(&l.h_stop, sizeof(int) * std::max(B, 1), cudaHostAllocDefault);
+            if (e != cudaSuccess) rc = fail(UALM_ENOCUDA, std::string("stop words: ") + cudaGetErrorString(e));
+            else l.h_stop_cap = (size_t)std::max(B, 1);
+        }
     }
     if (!rc) rc = solve_launch(c, true);
     if (!rc) { c->lanes[lane].in_flight = true; *ticket = lane; c->next_submit = (lane + 1) % depth; }
@@ -798,14 +812,33 @@ extern "C" int ualm_wait_batch(ualm_ctx_t *c, int ticket, ualm_result_t *results
     if (!c->lanes[ticket].in_flight) return fail(UALM_ESTATE, "ticket is not in flight");
     const int keep = c->cur;
     c->cur = ticket; c->b = &c->lanes[ticket];
-    const int rc = ualm_download(c, results, c_xy, c_yaw);
+    int rc = ualm_download(c, results, c_xy, c_yaw);
+    // a raise that the batch outran may still be queued: it lands before the lane's next clear, and the mirror is free again
+    if (c->lanes[ticket].raised) {
+        const cudaError_t e = cudaStreamSynchronize(c->cancel);
+        if (!rc && e != cudaSuccess) rc = fail(UALM_ENOCUDA, std::string("cudaStreamSynchronize(cancel): ") + cudaGetErrorString(e));
+        c->lanes[ticket].raised = false;
+    }
     c->lanes[ticket].in_flight = false;
     c->cur = keep; c->b = &c->lanes[keep];
     return rc;
 }
 
-// deadline-bounded wait: poll the lane's completion until the timeout, then raise its cancel word and wait for the batch to drain
-// (every problem still running stops at its next stop test, include/ualm.h UALM_RET_STOPPED)
+// raise the stop words idx[0, n) of parity lane `l` (idx = null: all B), in the host mirror and then by one H2D copy of the whole
+// mirror on the cancel stream, ordered after the clear of the lane's current batch
+static int raise_stop(ualm_ctx *c, Lane &l, int n, const int32_t *idx)
+{
+    if (idx) for (int k = 0; k < n; k++) l.h_stop[idx[k]] = 1;
+    else for (int b = 0; b < l.B; b++) l.h_stop[b] = 1;
+    if (l.B == 0) return UALM_OK;
+    CK(cudaStreamWaitEvent(c->cancel, l.ev_clear, 0));
+    CK(cudaMemcpyAsync(l.d_stop.p, l.h_stop, sizeof(int) * l.B, cudaMemcpyHostToDevice, c->cancel));
+    l.raised = true;
+    return UALM_OK;
+}
+
+// deadline-bounded wait: poll the lane's completion until the timeout, then raise every stop word of its batch and wait for the
+// batch to drain (every problem still running stops at its next stop test, include/ualm.h UALM_RET_STOPPED)
 extern "C" int ualm_wait_batch_for(ualm_ctx_t *c, int ticket, double timeout_ms, ualm_result_t *results, double *c_xy, double *c_yaw)
 {
     if (!c || ticket < 0 || ticket >= UALM_MAX_LANES) return fail(UALM_EINVAL, "bad ticket");
@@ -826,7 +859,7 @@ extern "C" int ualm_wait_batch_for(ualm_ctx_t *c, int ticket, double timeout_ms,
         if (q == cudaSuccess) break;
         if (q != cudaErrorNotReady) CK(q);
         if (std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() >= timeout_ms) {
-            CK(cudaMemcpyAsync(l.d_cancel, &c->h_flags[1], sizeof(int), cudaMemcpyHostToDevice, c->cancel));
+            if (int rc = raise_stop(c, l, 0, nullptr)) return rc;
             break;
         }
         std::this_thread::yield();
@@ -859,6 +892,24 @@ extern "C" int ualm_poll_batch(ualm_ctx_t *c, int ticket, double wait_ms, int32_
     *n_new = n;
     *n_pending = l.mbox.pending();
     return UALM_OK;
+}
+
+// stop the problems idx[0, n) of a submitted batch at their next stop test: their words in the lane's host mirror, then the mirror to
+// the device on the cancel stream (the parity path; the copy engines serve it while the kernels hold the SMs) or, on the throughput
+// path, on the engine's stream before the rounds the next poll or wait queues.  Everything is checked before a word is raised
+extern "C" int ualm_cancel_problems(ualm_ctx_t *c, int ticket, int n, const int32_t *idx)
+{
+    if (!c || ticket < 0 || ticket >= UALM_MAX_LANES) return fail(UALM_EINVAL, "bad ticket");
+    if (n < 0) return fail(UALM_EINVAL, "n must be >= 0");
+    if (n > 0 && !idx) return fail(UALM_EINVAL, "null idx");
+    if (c->tp) TP_CALL(ualm_tp::tp_cancel(c->tp, ticket, n, idx, err));
+    Lane &l = c->lanes[ticket];
+    if (!l.in_flight) return fail(UALM_ESTATE, "ticket is not in flight");
+    for (int k = 0; k < n; k++)
+        if (idx[k] < 0 || idx[k] >= l.B) return fail(UALM_EINVAL, "problem index out of range [0, B)");
+    if (n == 0) return UALM_OK;
+    CK(cudaSetDevice(c->device));
+    return raise_stop(c, l, n, idx);
 }
 
 extern "C" int ualm_set_budget(ualm_ctx_t *c, int32_t max_evals)

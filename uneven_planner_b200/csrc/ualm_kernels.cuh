@@ -67,8 +67,8 @@ struct DevParams {
     int inner_max_iter;
     int mem_size, past, int_K;
     R gravity;
-    // stop predicate of the solve (ualm_set_budget / ualm_wait_batch_for): evaluation budget (0 = none) and the lane's cancel
-    // word in device memory (null = none), set per launch
+    // stop predicate of the solve (ualm_set_budget / ualm_cancel_problems / ualm_wait_batch_for): evaluation budget (0 = none)
+    // and the lane's stop words in device memory, one per problem of its batch (null = none), set per launch
     int max_evals;
     const volatile int *cancel;
 };
@@ -1575,11 +1575,12 @@ __device__ UALM_NOINLINE R lane_absmax(SPtr a, int n, int lane)
 struct LbfgsOut { int ret; R f; int iters; int max_bound; int sum_bound; };
 
 // stop = (max_evals > 0 && n_evals >= max_evals) || cancel requested, evaluated where earlyExit is (and by the ALM loop after
-// judgeConvergence).  Lane 0 alone reads the cancel word; the broadcast keeps the decision warp-uniform.
+// judgeConvergence).  Lane 0 alone reads the problem's stop word (the slot's SC_PROB, set by slot_next); the broadcast keeps the
+// decision warp-uniform.
 __device__ __forceinline__ bool stop_requested(const Traj &t, const DevParams &p, int lane)
 {
     int c = 0;
-    if (p.cancel && lane == 0) c = *p.cancel;
+    if (p.cancel && lane == 0) c = p.cancel[(int)(R)t.sc[SC_PROB]];
     c = __shfl_sync(0xffffffffu, c, 0);
     return (p.max_evals > 0 && t.n_evals >= p.max_evals) || c != 0;
 }

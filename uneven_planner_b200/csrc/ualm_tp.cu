@@ -63,6 +63,11 @@ struct TpLane {
     bool publish = false;
     ualm_mbox::Mailbox mbox;
     Buf<int> d_pub;
+    // stop words, one per problem (TpPool::stop), and their pinned host mirror (grows only): cleared at admission on the engine's
+    // stream, raised by copying the whole mirror on the same stream (tp_cancel, tp_collect's deadline)
+    Buf<int> d_stop;
+    int *h_stop = nullptr;
+    size_t h_stop_cap = 0;
 };
 
 struct TpEngine {
@@ -98,7 +103,7 @@ struct TpEngine {
     int sg = 1;                           // subgroups per batch in use (UALM_TP_SUBGROUPS, <= TP_SUBGROUPS); 1 measured best: the batches in flight already are the groups
     int Nmax_live = 1, Mmax_live = 1;
     Buf<TpState> st;
-    Buf<int> active, n_active, remaining, cancel;
+    Buf<int> active, n_active, remaining;
     Buf<double> vec, cd, gw, kb_cost, lm_ys, lm_alpha, wf, wt;
     Buf<unsigned char> cr, gdc, gdt, dual, hs, hy, wway;
     Buf<long long> wf_off, wway_off, kprof;
@@ -181,12 +186,11 @@ int tp_create(TpEngine **out, int device, int precision, std::string *err)
             if (err) *err = "group stream creation failed";
             return failed(UALM_ENOCUDA);
         }
-    if (e->remaining.ensure(TP_MAX_TICKETS) != cudaSuccess || e->n_active.ensure(TP_NGROUPS) != cudaSuccess || e->cancel.ensure(TP_LANES) != cudaSuccess) {
+    if (e->remaining.ensure(TP_MAX_TICKETS) != cudaSuccess || e->n_active.ensure(TP_NGROUPS) != cudaSuccess) {
         if (err) *err = "allocation failed";
         return failed(UALM_ENOCUDA);
     }
     cudaMemsetAsync(e->remaining.p, 0, sizeof(int) * TP_MAX_TICKETS, e->stream);
-    cudaMemsetAsync(e->cancel.p, 0, sizeof(int) * TP_LANES, e->stream);
     cudaMemsetAsync(e->n_active.p, 0, sizeof(int) * TP_NGROUPS, e->stream);
     int rc = build_tables(e, err);
     if (rc) return failed(rc);
@@ -221,12 +225,13 @@ void tp_destroy(TpEngine *e)
     for (auto &l : e->lanes) {
         l.d_ad.release(); l.d_gd.release(); l.d_x0.release(); l.d_xev.release(); l.d_cxy.release(); l.d_cyaw.release(); l.d_xout.release(); l.d_f.release(); l.d_grad.release();
         l.d_hx.release(); l.d_gx.release(); l.d_sfx.release(); l.d_scx.release(); l.d_lam.release(); l.d_mu.release(); l.d_scin.release(); l.d_sfin.release();
-        l.d_offs.release(); l.d_res.release(); l.d_pub.release(); l.mbox.release();
+        l.d_offs.release(); l.d_res.release(); l.d_pub.release(); l.mbox.release(); l.d_stop.release();
+        if (l.h_stop) cudaFreeHost(l.h_stop);
         if (l.ev0) cudaEventDestroy(l.ev0);
         if (l.ev1) cudaEventDestroy(l.ev1);
     }
     for (auto &b : e->cells) b.release();
-    e->st.release(); e->active.release(); e->n_active.release(); e->remaining.release(); e->cancel.release(); e->vec.release(); e->cd.release(); e->gw.release();
+    e->st.release(); e->active.release(); e->n_active.release(); e->remaining.release(); e->vec.release(); e->cd.release(); e->gw.release();
     e->kb_cost.release(); e->lm_ys.release(); e->lm_alpha.release(); e->cr.release(); e->gdc.release(); e->gdt.release(); e->dual.release();
     e->hs.release(); e->hy.release(); e->wway.release(); e->wf.release(); e->wt.release(); e->wf_off.release(); e->wway_off.release();
     if (e->h_remaining) cudaFreeHost(e->h_remaining);
@@ -338,7 +343,7 @@ static int pool_alloc(TpEngine *e, int cap, std::string *err)
     TCK(cudaStreamSynchronize(e->stream));
     TpPool &E = e->E;
     E.capacity = cap; E.m = m; E.K = K; E.Smax = (int)Smax; E.use_tma = e->use_tma;
-    E.st = e->st.p; E.active = e->active.p; E.n_active = e->n_active.p; E.remaining = e->remaining.p; E.cancel = e->cancel.p;
+    E.st = e->st.p; E.active = e->active.p; E.n_active = e->n_active.p; E.remaining = e->remaining.p;
     E.vec = e->vec.p; E.cd = e->cd.p; E.gw = e->gw.p; E.cr = e->f32() ? (void *)e->cr.p : (void *)e->cd.p; E.gdc = e->gdc.p; E.gdt = e->gdt.p;
     E.kb_cost = e->kb_cost.p; E.dual = e->dual.p; E.hs = e->hs.p; E.hy = e->hy.p; E.lm_ys = e->lm_ys.p; E.lm_alpha = e->lm_alpha.p;
     E.wf = e->wf.p; E.wf_off = e->wf_off.p; E.wt = e->wt.p; E.wway = e->wway.p; E.wway_off = e->wway_off.p;
@@ -443,6 +448,21 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, std::s
         if (rc) return rc;
     }
     if ((int)e->free_slots.size() < need) { if (err) *err = "throughput pool exhausted: collect a batch in flight first (the pool grows only when idle)"; return UALM_ELIMIT; }
+    // the lane's stop words: no request of its previous batch carries over (nothing raises them while the lane is not in flight, and
+    // the raises of its previous batch were complete when that batch was collected)
+    {
+        const size_t nw = (size_t)std::max(l.B, 1);
+        TCK(l.d_stop.ensure(nw));
+        if (l.h_stop_cap < nw) {
+            if (l.h_stop) cudaFreeHost(l.h_stop);
+            l.h_stop = nullptr; l.h_stop_cap = 0;
+            TCK(cudaMallocHost(&l.h_stop, sizeof(int) * nw));
+            l.h_stop_cap = nw;
+        }
+        memset(l.h_stop, 0, sizeof(int) * l.h_stop_cap);
+        TCK(cudaMemsetAsync(l.d_stop.p, 0, sizeof(int) * nw, e->stream));
+        e->E.stop[lane] = l.d_stop.p;
+    }
     l.slots.clear();
     std::vector<ualm_result_t> res0(l.B);
     int k = 0;
@@ -481,7 +501,6 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, std::s
     TCK(cudaEventRecord(l.ev0, e->stream));
     l.launches = 0;
     TCK(cudaMemcpyAsync(l.d_res.p, res0.data(), sizeof(ualm_result_t) * l.B, cudaMemcpyHostToDevice, e->stream));
-    TCK(cudaMemsetAsync(e->cancel.p + lane, 0, sizeof(int), e->stream));      // a cancel request of the lane's previous batch does not carry over
     if (BA < l.B) {
         TCK(cudaMemsetAsync(l.d_cxy.p, 0, sizeof(double) * l.tot_cxy, e->stream));
         TCK(cudaMemsetAsync(l.d_cyaw.p, 0, sizeof(double) * l.tot_cyaw, e->stream));
@@ -616,6 +635,28 @@ static int run_rounds(TpEngine *e, int nr, std::string *err)
     return UALM_OK;
 }
 
+// raise the stop words idx[0, n) of lane l's batch (idx = null: all B): set them in the mirror, then copy the whole mirror on the
+// engine's stream.  Words only go from 0 to 1 while the batch runs, so the copy never lowers one; the rounds the next poll or
+// wait queues see it (both synchronise the engine's stream first)
+static int raise_stop(TpEngine *e, TpLane &l, int n, const int32_t *idx, std::string *err)
+{
+    if (idx) for (int k = 0; k < n; k++) l.h_stop[idx[k]] = 1;
+    else for (int b = 0; b < l.B; b++) l.h_stop[b] = 1;
+    if (l.B > 0) TCK(cudaMemcpyAsync(l.d_stop.p, l.h_stop, sizeof(int) * l.B, cudaMemcpyHostToDevice, e->stream));
+    return UALM_OK;
+}
+
+int tp_cancel(TpEngine *e, int lane, int n, const int32_t *idx, std::string *err)
+{
+    TpLane &l = e->lanes[lane];
+    if (!l.in_flight || !l.publish) { if (err) *err = "ticket is not in flight"; return UALM_ESTATE; }
+    for (int k = 0; k < n; k++)
+        if (idx[k] < 0 || idx[k] >= l.B) { if (err) *err = "problem index out of range [0, B)"; return UALM_EINVAL; }
+    if (n == 0) return UALM_OK;
+    TCK(cudaSetDevice(e->device));
+    return raise_stop(e, l, n, idx, err);
+}
+
 int tp_collect(TpEngine *e, int lane, std::string *err, double timeout_ms)
 {
     if (lane < 0 || lane >= TP_LANES) { if (err) *err = "lane out of range"; return UALM_EINVAL; }
@@ -633,8 +674,9 @@ int tp_collect(TpEngine *e, int lane, std::string *err, double timeout_ms)
         TCK(cudaStreamSynchronize(e->stream));
         if (e->h_remaining[lane] <= 0) break;
         if (timeout_ms >= 0.0 && !cancelled && std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() >= timeout_ms) {
-            const int one = 1;      // read by ka_kernel at the stop tests of the rounds queued from now on
-            TCK(cudaMemcpyAsync(e->cancel.p + lane, &one, sizeof(int), cudaMemcpyHostToDevice, e->stream));
+            // every stop word of the batch, read by ka_kernel at the stop tests of the rounds queued from now on
+            int rc = raise_stop(e, l, 0, nullptr, err);
+            if (rc) return rc;
             TCK(cudaStreamSynchronize(e->stream));
             cancelled = true;
         }

@@ -27,8 +27,12 @@ int tp_admit(TpEngine *e, int lane, std::string *err, bool publish = false);
 // finished problems, queue the next rounds of every live group), repeated until a problem is new or wait_ms has passed
 int tp_poll(TpEngine *e, int lane, double wait_ms, int32_t *idx, int *n_new, int *n_pending, ualm_result_t *results, double *c_xy, double *c_yaw,
             std::string *err);
-// blocks: rounds until the lane's batch is done.  timeout_ms >= 0: once that much time has passed since the call, the lane's
-// cancel word is raised before the next rounds (its trajectories stop at their next stop test)
+// ualm_cancel_problems on a lane admitted with publish: raises the stop words idx[0, n) (the caller checked n and idx), which the
+// rounds queued by the next tp_poll / tp_collect see.  UALM_ESTATE when the lane is not in flight, UALM_EINVAL for an index
+// outside [0, B); nothing is raised on either
+int tp_cancel(TpEngine *e, int lane, int n, const int32_t *idx, std::string *err);
+// blocks: rounds until the lane's batch is done.  timeout_ms >= 0: once that much time has passed since the call, every stop word
+// of the lane's batch is raised before the next rounds (its trajectories stop at their next stop test)
 int tp_collect(TpEngine *e, int lane, std::string *err, double timeout_ms = -1.0);
 int tp_set_budget(TpEngine *e, int max_evals, std::string *err);              // evaluation budget of the solves admitted afterwards
 int tp_download(TpEngine *e, int lane, ualm_result_t *results, double *c_xy, double *c_yaw, std::string *err);

@@ -106,7 +106,9 @@ struct TpPool {
     int *active;            // [TP_NGROUPS][capacity] active slot list per group
     int *n_active;          // [TP_NGROUPS]
     int *remaining;         // per ticket: trajectories not yet done
-    const int *cancel;      // per ticket: cancel request (ualm_wait_batch_for), raised by the host between rounds
+    // per lane: its stop words, one per problem of its batch (ualm_cancel_problems, ualm_wait_batch_for); the host may raise them
+    // while a round runs
+    const int *stop[TP_MAXLANES];
     double *vec;            // [cap][5][TP_NVAR]  x | g | xp | gp | d
     double *cd;             // [cap][TP_CSTRIDE]  coefficients of the last forward solve (double)
     double *gw;             // [cap][TP_CSTRIDE]  z = dc/dT(piece) of the last forward solve (same layout as cd)
@@ -546,16 +548,21 @@ __device__ int ls_begin(const SlotView &v, int lane)
     return 0;
 }
 
-// the stop predicate of include/ualm.h (UALM_RET_STOPPED), tested where earlyExit is and by the ALM loop after judgeConvergence
-__device__ __forceinline__ bool stop_requested(const TpPool &E, const TpParams &p, const TpState *st)
+// the stop predicate of include/ualm.h (UALM_RET_STOPPED), tested where earlyExit is and by the ALM loop after judgeConvergence.
+// Lane 0 alone reads the trajectory's stop word and broadcasts it: a raise that lands in the middle of a round cannot split the
+// warp's decision
+__device__ __forceinline__ bool stop_requested(const TpPool &E, const TpParams &p, const TpState *st, int lane)
 {
-    return (p.max_evals > 0 && st->n_evals >= p.max_evals) || E.cancel[st->ticket] != 0;
+    int c = 0;
+    if (lane == 0) c = ((const volatile int *)E.stop[st->ticket])[st->index];
+    c = __shfl_sync(0xffffffffu, c, 0);
+    return (p.max_evals > 0 && st->n_evals >= p.max_evals) || c != 0;
 }
 
 // the stop test at the earlyExit point; a stop that fires is marked in ret_code for the ALM loop (alm_ends)
 __device__ __forceinline__ bool stop_fires(const TpPool &E, const TpParams &p, TpState *st, int lane)
 {
-    const bool s = stop_requested(E, p, st);
+    const bool s = stop_requested(E, p, st, lane);
     if (s && lane == 0) st->ret_code = UALM_RET_STOPPED;
     return s;
 }
@@ -565,7 +572,7 @@ __device__ __forceinline__ bool stop_fires(const TpPool &E, const TpParams &p, T
 // costs a spill
 __device__ __noinline__ bool alm_ends(const TpPool &E, const TpParams &p, TpState *st, int lane)
 {
-    if (st->ret_code == UALM_RET_STOPPED || stop_requested(E, p, st)) { if (lane == 0) st->ret_code = UALM_RET_STOPPED; return true; }
+    if (st->ret_code == UALM_RET_STOPPED || stop_requested(E, p, st, lane)) { if (lane == 0) st->ret_code = UALM_RET_STOPPED; return true; }
     const int iter = st->outer_iter + 1;
     if (lane == 0) st->outer_iter = iter;
     if ((double)iter > p.max_iter) { if (lane == 0) st->ret_code = 2; return true; }
