@@ -160,7 +160,8 @@ int ualm_last_solve_ms(ualm_ctx_t *ctx, float *ms, int *launches);
  *   ualm_select_lane(ctx, i): upload / solve_resident / sync / download / pack_records / last_solve_ms / eval / feasibility act
  *                             on lane i (0 <= i < ualm_max_lanes(); lane 0 is selected at creation).
  *   ualm_submit_batch:  upload + launch on the next lane of a `depth`-deep ring, returns a ticket without waiting for the solve
- *                       (host inputs are consumed before it returns).  UALM_ESTATE when that lane is still in flight.
+ *                       (host inputs are consumed before it returns); the batch then runs to completion on the device on both
+ *                       paths.  UALM_ESTATE when that lane is still in flight.
  *   ualm_wait_batch:    blocks until the ticket's batch is complete, D2H of its results (same outputs as ualm_solve_batch).
  *   ualm_mark_begin / ualm_mark_end: CUDA-event time (ms) from the selected lane's stream at mark_begin to the completion of the
  *                       last solve of every lane at mark_end. */
@@ -184,9 +185,10 @@ int ualm_wait_batch_for(ualm_ctx_t *ctx, int ticket, double timeout_ms, ualm_res
  * ualm_wait_batch / ualm_wait_batch_for after any number of polls behave exactly as today and return all B records.
  * A problem over the compiled limits (UALM_ELIMIT) is returned by the first poll; one the budget or a deadline stops is returned
  * when it stops (UALM_RET_STOPPED).  A null ctx, a bad ticket, wait_ms < 0 or a null idx / n_new / n_pending is UALM_EINVAL; a
- * ticket not in flight (also one already waited) is UALM_ESTATE.  Only tickets of ualm_submit_batch* can be polled.  The parity
- * path publishes each problem from the solve itself; the throughput path advances only inside host calls, so each poll also
- * runs the engine: it waits for the ticket's queued rounds, publishes what they finished and queues the next rounds. */
+ * ticket not in flight (also one already waited) is UALM_ESTATE.  Only tickets of ualm_submit_batch* can be polled.  On both
+ * paths a submitted batch runs to completion on the device with no further host call, and each problem is published into the
+ * ticket's mailbox from the device as it finishes; a poll only reads that mailbox, so the caller may sleep or do other work between
+ * polls without holding any batch back. */
 int ualm_poll_batch(ualm_ctx_t *ctx, int ticket, double wait_ms, int32_t *idx, int *n_new, int *n_pending,
                     ualm_result_t *results, double *c_xy, double *c_yaw);
 /* Stop the listed problems of a submitted batch.  Each one stops at its next stop test, exactly as a deadline stops it
@@ -195,9 +197,9 @@ int ualm_poll_batch(ualm_ctx_t *ctx, int ticket, double wait_ms, int32_t *idx, i
  * unaffected bit for bit.  Cancelled problems come back through ualm_poll_batch / ualm_wait_batch like any other.
  * A null ctx, a bad ticket, n < 0, a null idx with n > 0 or an index outside [0, B) is UALM_EINVAL; a ticket not in flight (also
  * one already waited) is UALM_ESTATE; a refused call raises nothing.  n = 0 does nothing; duplicate indices and repeated calls are
- * harmless.  Only tickets of ualm_submit_batch* can be cancelled, from the thread that polls.  The parity path raises the stop
- * words by a copy that runs while the kernels hold the SMs; on the throughput path, which advances only inside host calls, the
- * cancel takes effect at the rounds that the next ualm_poll_batch / ualm_wait_batch* queues. */
+ * harmless.  Only tickets of ualm_submit_batch* can be cancelled, from the thread that polls.  On both paths the stop words are
+ * raised by a copy on a stream of their own that lands while the batch runs, so the cancel reaches problems that are running
+ * without any further host call. */
 int ualm_cancel_problems(ualm_ctx_t *ctx, int ticket, int n, const int32_t *idx);
 /* Evaluation budget per problem for the solves launched afterwards by every solving entry point (ualm_solve_batch,
  * ualm_solve_resident, ualm_submit_batch, ualm_solve_batch_multi through each context): max_evals = 0 (the default) is none,

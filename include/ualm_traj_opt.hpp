@@ -238,7 +238,8 @@ public:
     // the problems of a submitted batch that finished since the last poll (ualm_poll_batch): their indices into idx (capacity B),
     // their records and coefficients at their problem-order places of results / c_xy / c_yaw (the buffers waitBatch takes; c_xy /
     // c_yaw may be null).  Returns how many; *pending = problems not returned yet.  wait_ms > 0 blocks until one is new or wait_ms
-    // has passed.  waitBatch afterwards returns the whole batch as before
+    // has passed.  waitBatch afterwards returns the whole batch as before.  The batch runs on the device whether or not anyone polls
+    // (both paths), so the caller may sleep or do other work between polls
     int pollBatch(int ticket, double wait_ms, int32_t *idx, int *pending, ualm_result_t *results, double *c_xy, double *c_yaw)
     {
         int n_new = 0;
@@ -246,7 +247,8 @@ public:
         return n_new;
     }
     // stop the problems idx[0, n) of a submitted batch at their next stop test (ualm_cancel_problems): they come back through
-    // pollBatch / waitBatch with UALM_RET_STOPPED, or with their own result if they were final first; the rest is unaffected
+    // pollBatch / waitBatch with UALM_RET_STOPPED, or with their own result if they were final first; the rest is unaffected.
+    // The cancel reaches running problems on both paths without a further call
     void cancelProblems(int ticket, int n, const int32_t *idx) { check(ualm_cancel_problems(ctx_, ticket, n, idx), "ualm_cancel_problems"); }
 
     // What the MPC receives and tracks, for the batch solved last on the selected lane (ualm_mpc_export_batch): the SE2Traj message

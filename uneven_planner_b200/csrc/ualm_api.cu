@@ -672,7 +672,7 @@ static int solve_launch(ualm_ctx *c, bool publish)
 extern "C" int ualm_solve_resident(ualm_ctx_t *c)
 {
     if (!c) return fail(UALM_EINVAL, "null ctx");
-    if (c->tp) TP_CALL(ualm_tp::tp_admit(c->tp, c->cur, err));      // joins the pool of running trajectories; ualm_sync / download drive the rounds
+    if (c->tp) TP_CALL(ualm_tp::tp_admit(c->tp, c->cur, err));      // joins the pool of running trajectories; its rounds run on the device, ualm_sync waits
     return solve_launch(c, false);
 }
 
@@ -895,8 +895,8 @@ extern "C" int ualm_poll_batch(ualm_ctx_t *c, int ticket, double wait_ms, int32_
 }
 
 // stop the problems idx[0, n) of a submitted batch at their next stop test: their words in the lane's host mirror, then the mirror to
-// the device on the cancel stream (the parity path; the copy engines serve it while the kernels hold the SMs) or, on the throughput
-// path, on the engine's stream before the rounds the next poll or wait queues.  Everything is checked before a word is raised
+// the device on a stream no solve occupies (the copy engines serve it while the kernels hold the SMs): the context's cancel stream on
+// the parity path, the engine's on the throughput path.  Everything is checked before a word is raised
 extern "C" int ualm_cancel_problems(ualm_ctx_t *c, int ticket, int n, const int32_t *idx)
 {
     if (!c || ticket < 0 || ticket >= UALM_MAX_LANES) return fail(UALM_EINVAL, "bad ticket");

@@ -1,5 +1,6 @@
 // ualm_tp.cu -- host side of the throughput engine (precision 32 / 65 of include/ualm.h): slot pool, admission of batches,
-// the round driver (ka -> [ks] -> kb per round, continuous batching across the batches in flight) and result gathering.
+// the device-side round loop of every group (one CUDA graph per group: ka -> [ks] -> kb per round, continuous batching across the
+// batches in flight) and result gathering.
 // Kernels: ualm_tp_kernels.cuh, ualm_tp_samples.cuh.  Compiled with FMA contraction ON (its own translation unit).
 #include "ualm_tp_samples.cuh"
 #include "ualm_tp_host.h"
@@ -23,6 +24,9 @@ namespace ualm_tp {
         if (e_ != cudaSuccess) { if (err) *err = std::string(#call) + ": " + cudaGetErrorString(e_); return UALM_ENOCUDA; } \
     } while (0)
 
+// device buffer, grown only.  Stream-ordered allocation: cudaFree would wait for the whole device, and so hold the admission of a
+// batch until every other batch in flight had finished its round loop.  A buffer is only grown or released when no queued work
+// uses it (the host synchronised that work), and the allocation is complete before ensure returns
 template <class T>
 struct Buf {
     T *p = nullptr;
@@ -30,13 +34,14 @@ struct Buf {
     cudaError_t ensure(size_t n)
     {
         if (n <= cap) return cudaSuccess;
-        if (p) cudaFree(p);
+        if (p) cudaFreeAsync(p, cudaStreamPerThread);
         p = nullptr; cap = 0;
-        cudaError_t e = cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T));
+        cudaError_t e = cudaMallocAsync((void **)&p, std::max<size_t>(n, 1) * sizeof(T), cudaStreamPerThread);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(cudaStreamPerThread);
         if (e == cudaSuccess) cap = n;
         return e;
     }
-    void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
+    void release() { if (p) cudaFreeAsync(p, cudaStreamPerThread); p = nullptr; cap = 0; }
 };
 
 static_assert(TP_SUBGROUPS >= UALM_MAX_ENVS, "a lane runs the problems of environment k in its group k: one group per environment");
@@ -52,6 +57,7 @@ struct TpLane {
     long long tot_x = 0, tot_s = 0, tot_cxy = 0, tot_cyaw = 0;
     Buf<AdmitDesc> d_ad;
     Buf<GatherDesc> d_gd;
+    Buf<GatherDesc> d_gdg;            // a submitted batch in several groups: d_gd once per group, other groups' problems without slot
     Buf<double> d_x0, d_xev, d_cxy, d_cyaw, d_xout, d_f, d_grad, d_hx, d_gx, d_sfx, d_scx, d_lam, d_mu, d_scin, d_sfin;
     Buf<long long> d_offs;
     Buf<ualm_result_t> d_res;
@@ -64,7 +70,7 @@ struct TpLane {
     ualm_mbox::Mailbox mbox;
     Buf<int> d_pub;
     // stop words, one per problem (TpPool::stop), and their pinned host mirror (grows only): cleared at admission on the engine's
-    // stream, raised by copying the whole mirror on the same stream (tp_cancel, tp_collect's deadline)
+    // stream, raised by copying the whole mirror on the cancel stream while the lane's loops run (tp_cancel, tp_collect's deadline)
     Buf<int> d_stop;
     int *h_stop = nullptr;
     size_t h_stop_cap = 0;
@@ -75,6 +81,7 @@ struct TpEngine {
     bool f32() const { return precision == 32; }
     size_t esz() const { return precision == 32 ? 4 : 8; }
     cudaStream_t stream = nullptr;
+    cudaStream_t cstream = nullptr;       // stop-word raises: no group loop occupies it, so a raise reaches the rounds running
     cudaEvent_t evA = nullptr, evB = nullptr;
     // environments (ualm_select_env): parameters, grid and its TMA descriptor of each; group g runs with those of genv[g]
     bool have_params[UALM_MAX_ENVS] = {}, have_map[UALM_MAX_ENVS] = {};
@@ -92,14 +99,20 @@ struct TpEngine {
     std::vector<int> free_slots;
     int live = 0;                 // slots admitted and not yet freed
     // groups: every batch in flight is split into TP_SUBGROUPS groups (group = lane * TP_SUBGROUPS + k); each group has its own
-    // stream, active list and round sequence, so ka of one group overlaps kb of another and a slow trajectory only holds up
-    // the rounds of its own group
+    // stream, active list and round loop (a CUDA graph launched at admission), so ka of one group overlaps kb of another and a slow
+    // trajectory only holds up the rounds of its own group
     cudaStream_t gstream[TP_NGROUPS] = {};
     cudaEvent_t gev[TP_NGROUPS] = {};
+    // the round loop of each group (launch_loop), one per variant (with / without ks_kernel in the first round, with / without
+    // publish_kernel): its graph keeps its conditional node and handle for the engine's life, and every admission replaces the other
+    // nodes and updates the executable graph in place.  Destroying an executable graph waits for the device, which would hold the
+    // admission until every other batch in flight had finished
+    struct Loop { cudaGraph_t G = nullptr, body = nullptr; cudaGraphNode_t cond = nullptr; cudaGraphConditionalHandle h = 0; cudaGraphExec_t exec = nullptr; };
+    Loop loops[TP_NGROUPS][4];
     int glive[TP_NGROUPS] = {};           // slots admitted and not yet freed, per group
-    int gscale[TP_NGROUPS] = {};          // rounds that still have to run ks_kernel
-    bool gcompact[TP_NGROUPS] = {};
-    long long grounds[TP_NGROUPS] = {};
+    Buf<GroupLoop> gloop;                 // [TP_NGROUPS] rounds / launches / round-cap error of each group's loop since its admission
+    GroupLoop *h_gloop = nullptr;         // pinned, TP_SUBGROUPS entries
+    cudaStream_t capstream = nullptr;     // graph capture only
     int sg = 1;                           // subgroups per batch in use (UALM_TP_SUBGROUPS, <= TP_SUBGROUPS); 1 measured best: the batches in flight already are the groups
     int Nmax_live = 1, Mmax_live = 1;
     Buf<TpState> st;
@@ -109,7 +122,6 @@ struct TpEngine {
     Buf<long long> wf_off, wway_off, kprof;
     int *h_remaining = nullptr;   // pinned
     TpLane lanes[TP_LANES];
-    long long rounds_total = 0;
     int chunk = 8;
     int ka_warps = 1;             // warps (= trajectories) per ka_kernel CTA: 1, 2 or 4 (UALM_TP_KA_WARPS); 1 measured best by ~1 %: no warp waits for a CTA mate
     bool prof = false;            // developer profile (UALM_TP_PROFILE=1): in-kernel phase cycle counters, printed at destroy
@@ -174,24 +186,33 @@ int tp_create(TpEngine **out, int device, int precision, std::string *err)
     if (const char *s = getenv("UALM_TP_SUBGROUPS")) e->sg = std::min(TP_SUBGROUPS, std::max(1, atoi(s)));
     memset(&e->E, 0, sizeof(e->E));
     auto failed = [&](int rc) { tp_destroy(e); return rc; };
-    if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreate(&e->evA) != cudaSuccess ||
-        cudaEventCreate(&e->evB) != cudaSuccess || cudaMallocHost(&e->h_remaining, sizeof(int) * TP_MAX_TICKETS) != cudaSuccess) {
+    // group streams first and group-major, so the first groups of up to eight lanes, whose loops run side by side, are created one
+    // after another: CUDA multiplexes streams onto its hardware queues (CUDA_DEVICE_MAX_CONNECTIONS, 8 by default), and a long loop
+    // must not share a queue with another lane's loop (a precaution; not measured on its own)
+    for (int k = 0; k < TP_SUBGROUPS; k++)
+        for (int lane = 0; lane < TP_LANES; lane++) {
+            const int g = lane * TP_SUBGROUPS + k;
+            if (cudaStreamCreateWithFlags(&e->gstream[g], cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&e->gev[g], cudaEventDisableTiming) != cudaSuccess) {
+                if (err) *err = "group stream creation failed";
+                return failed(UALM_ENOCUDA);
+            }
+        }
+    if (cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking) != cudaSuccess || cudaStreamCreateWithFlags(&e->cstream, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaStreamCreateWithFlags(&e->capstream, cudaStreamNonBlocking) != cudaSuccess || cudaEventCreate(&e->evA) != cudaSuccess ||
+        cudaEventCreate(&e->evB) != cudaSuccess || cudaMallocHost(&e->h_remaining, sizeof(int) * TP_MAX_TICKETS) != cudaSuccess ||
+        cudaMallocHost(&e->h_gloop, sizeof(GroupLoop) * TP_SUBGROUPS) != cudaSuccess) {
         if (err) *err = "throughput engine: stream / event / pinned allocation failed";
         return failed(UALM_ENOCUDA);
     }
     for (auto &l : e->lanes)
         if (cudaEventCreate(&l.ev0) != cudaSuccess || cudaEventCreate(&l.ev1) != cudaSuccess) { if (err) *err = "event creation failed"; return failed(UALM_ENOCUDA); }
-    for (int g = 0; g < TP_NGROUPS; g++)
-        if (cudaStreamCreateWithFlags(&e->gstream[g], cudaStreamNonBlocking) != cudaSuccess || cudaEventCreateWithFlags(&e->gev[g], cudaEventDisableTiming) != cudaSuccess) {
-            if (err) *err = "group stream creation failed";
-            return failed(UALM_ENOCUDA);
-        }
-    if (e->remaining.ensure(TP_MAX_TICKETS) != cudaSuccess || e->n_active.ensure(TP_NGROUPS) != cudaSuccess) {
+    if (e->remaining.ensure(TP_MAX_TICKETS) != cudaSuccess || e->n_active.ensure(TP_NGROUPS) != cudaSuccess || e->gloop.ensure(TP_NGROUPS) != cudaSuccess) {
         if (err) *err = "allocation failed";
         return failed(UALM_ENOCUDA);
     }
     cudaMemsetAsync(e->remaining.p, 0, sizeof(int) * TP_MAX_TICKETS, e->stream);
     cudaMemsetAsync(e->n_active.p, 0, sizeof(int) * TP_NGROUPS, e->stream);
+    cudaMemsetAsync(e->gloop.p, 0, sizeof(GroupLoop) * TP_NGROUPS, e->stream);
     int rc = build_tables(e, err);
     if (rc) return failed(rc);
     *out = e;
@@ -221,9 +242,16 @@ void tp_destroy(TpEngine *e)
         fprintf(stderr, " total %.0f\n", (double)tb / std::max(1ll, h[16 + 7]));
         e->kprof.release();
     }
-    for (int g = 0; g < TP_NGROUPS; g++) { if (e->gstream[g]) cudaStreamDestroy(e->gstream[g]); if (e->gev[g]) cudaEventDestroy(e->gev[g]); }
+    for (int g = 0; g < TP_NGROUPS; g++) {
+        for (auto &L : e->loops[g]) {
+            if (L.exec) cudaGraphExecDestroy(L.exec);
+            if (L.G) cudaGraphDestroy(L.G);
+        }
+        if (e->gstream[g]) cudaStreamDestroy(e->gstream[g]);
+        if (e->gev[g]) cudaEventDestroy(e->gev[g]);
+    }
     for (auto &l : e->lanes) {
-        l.d_ad.release(); l.d_gd.release(); l.d_x0.release(); l.d_xev.release(); l.d_cxy.release(); l.d_cyaw.release(); l.d_xout.release(); l.d_f.release(); l.d_grad.release();
+        l.d_ad.release(); l.d_gd.release(); l.d_gdg.release(); l.d_x0.release(); l.d_xev.release(); l.d_cxy.release(); l.d_cyaw.release(); l.d_xout.release(); l.d_f.release(); l.d_grad.release();
         l.d_hx.release(); l.d_gx.release(); l.d_sfx.release(); l.d_scx.release(); l.d_lam.release(); l.d_mu.release(); l.d_scin.release(); l.d_sfin.release();
         l.d_offs.release(); l.d_res.release(); l.d_pub.release(); l.mbox.release(); l.d_stop.release();
         if (l.h_stop) cudaFreeHost(l.h_stop);
@@ -234,10 +262,15 @@ void tp_destroy(TpEngine *e)
     e->st.release(); e->active.release(); e->n_active.release(); e->remaining.release(); e->vec.release(); e->cd.release(); e->gw.release();
     e->kb_cost.release(); e->lm_ys.release(); e->lm_alpha.release(); e->cr.release(); e->gdc.release(); e->gdt.release(); e->dual.release();
     e->hs.release(); e->hy.release(); e->wway.release(); e->wf.release(); e->wt.release(); e->wf_off.release(); e->wway_off.release();
+    e->gloop.release();
     if (e->h_remaining) cudaFreeHost(e->h_remaining);
+    if (e->h_gloop) cudaFreeHost(e->h_gloop);
     if (e->evA) cudaEventDestroy(e->evA);
     if (e->evB) cudaEventDestroy(e->evB);
     if (e->stream) cudaStreamDestroy(e->stream);
+    if (e->cstream) cudaStreamDestroy(e->cstream);
+    if (e->capstream) cudaStreamDestroy(e->capstream);
+    cudaStreamSynchronize(cudaStreamPerThread);      // the buffers' frees
     delete e;
 }
 
@@ -277,7 +310,7 @@ int tp_set_params(TpEngine *e, int env, const ualm_params_t *p, std::string *err
     // the pool strides depend on the largest int_K and mem_size: it is rebuilt at the next admission.  The uploaded batches' sample
     // offsets depend on int_K: they are invalidated, as on the parity path (upload again)
     e->capacity = 0; e->free_slots.clear(); e->live = 0;
-    for (int g = 0; g < TP_NGROUPS; g++) { e->glive[g] = 0; e->gscale[g] = 0; e->gcompact[g] = false; }
+    for (int g = 0; g < TP_NGROUPS; g++) e->glive[g] = 0;
     for (auto &l : e->lanes) { l.collected = false; l.have_batch = false; }
     return UALM_OK;
 }
@@ -421,7 +454,11 @@ int tp_upload(TpEngine *e, int lane, int B, const int32_t *N, const int32_t *M, 
     return UALM_OK;
 }
 
-static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, std::string *err)
+static int start_loops(TpEngine *e, int lane, bool publish, std::string *err);
+
+// admission of the lane's uploaded batch into the pool; loops: launch its groups' round loops (tp_time_penalty launches them itself
+// after its own rounds)
+static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, bool publish, bool loops, std::string *err)
 {
     TpLane &l = e->lanes[lane];
     if (!l.have_batch) { if (err) *err = "set_params, set_map and upload must precede the solve"; return UALM_ESTATE; }
@@ -453,11 +490,13 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, std::s
     {
         const size_t nw = (size_t)std::max(l.B, 1);
         TCK(l.d_stop.ensure(nw));
-        if (l.h_stop_cap < nw) {
+        if (l.h_stop_cap < nw) {         // (in powers of two: freeing pinned memory waits for the device)
+            size_t c = 1024;
+            while (c < nw) c *= 2;
             if (l.h_stop) cudaFreeHost(l.h_stop);
             l.h_stop = nullptr; l.h_stop_cap = 0;
-            TCK(cudaMallocHost(&l.h_stop, sizeof(int) * nw));
-            l.h_stop_cap = nw;
+            TCK(cudaMallocHost(&l.h_stop, sizeof(int) * c));
+            l.h_stop_cap = c;
         }
         memset(l.h_stop, 0, sizeof(int) * l.h_stop_cap);
         TCK(cudaMemsetAsync(l.d_stop.p, 0, sizeof(int) * nw, e->stream));
@@ -509,6 +548,21 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, std::s
         TCK(cudaMemcpyAsync(l.d_ad.p, ad.data(), sizeof(AdmitDesc) * BA, cudaMemcpyHostToDevice, e->stream));
         TCK(cudaMemcpyAsync(l.d_offs.p, offs.data(), sizeof(long long) * BA, cudaMemcpyHostToDevice, e->stream));
         TCK(cudaMemcpyAsync(l.d_gd.p, l.gd.data(), sizeof(GatherDesc) * l.B, cudaMemcpyHostToDevice, e->stream));
+        std::vector<GatherDesc> gdg;
+        int ngroups = 0;
+        for (int q = 0; q < TP_SUBGROUPS; q++) ngroups += e->glive[lane * TP_SUBGROUPS + q] > 0;
+        if (publish && ngroups > 1) {    // per group: start_loops
+            gdg.resize((size_t)TP_SUBGROUPS * l.B);
+            for (int q = 0; q < TP_SUBGROUPS; q++)
+                for (int b = 0; b < l.B; b++) {
+                    GatherDesc &d = gdg[(size_t)q * l.B + b];
+                    d = l.gd[b];
+                    if (l.ad[b].slot < 0 || l.ad[b].group != lane * TP_SUBGROUPS + q) d.slot = -1;
+                }
+            TCK(l.d_gdg.ensure(gdg.size()));
+            TCK(cudaMemcpyAsync(l.d_gdg.p, gdg.data(), sizeof(GatherDesc) * gdg.size(), cudaMemcpyHostToDevice, e->stream));
+        }
+        TCK(cudaMemsetAsync(e->gloop.p + lane * TP_SUBGROUPS, 0, sizeof(GroupLoop) * TP_SUBGROUPS, e->stream));
         e->h_remaining[lane] = BA;
         TCK(cudaMemcpyAsync(e->remaining.p + lane, e->h_remaining + lane, sizeof(int), cudaMemcpyHostToDevice, e->stream));
         const double *x0 = l.has_xev ? l.d_xev.p : l.d_x0.p;
@@ -523,18 +577,15 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, std::s
             TCK(cudaGetLastError());
             l.launches++;
         }
-        // host-synchronised: ad / offs / res0 are stack-local staging vectors, and the lane's group streams start after the admission
+        // host-synchronised: ad / offs / res0 / gdg are stack-local staging vectors, and the lane's group loops start after the
+        // admission (which also cleared the lane's stop words: a raise on the cancel stream lands after that clear)
         TCK(cudaStreamSynchronize(e->stream));
-        for (int q = 0; q < TP_SUBGROUPS; q++) {
-            const int g = lane * TP_SUBGROUPS + q;
-            if (e->glive[g] > 0) { e->gcompact[g] = true; if ((mode == 0 && e->p[e->genv[g]].use_scaling) || mode == 2) e->gscale[g] = std::max(e->gscale[g], 1); }
-        }
     } else {
         e->h_remaining[lane] = 0;
         TCK(cudaStreamSynchronize(e->stream));
     }
-    l.in_flight = true; l.collected = false; l.mode = mode;
-    return UALM_OK;
+    l.in_flight = true; l.collected = false; l.mode = mode; l.publish = publish;
+    return loops ? start_loops(e, lane, publish, err) : UALM_OK;
 }
 
 int tp_admit(TpEngine *e, int lane, std::string *err, bool publish)
@@ -549,9 +600,7 @@ int tp_admit(TpEngine *e, int lane, std::string *err, bool publish)
         TCK(l.d_pub.ensure(l.B));
         if (l.B > 0) TCK(cudaMemsetAsync(l.d_pub.p, 0, sizeof(int) * l.B, e->stream));   // ordered before admission's synchronise
     }
-    const int rc = admit_impl(e, lane, 0, false, err);
-    if (rc == UALM_OK) l.publish = publish;
-    return rc;
+    return admit_impl(e, lane, 0, false, publish, true, err);
 }
 
 static size_t kb_smem_bytes(TpEngine *e, bool tma)
@@ -581,12 +630,11 @@ static void ka_layout(TpEngine *e)
 }
 static size_t ka_smem_bytes(TpEngine *e) { return (size_t)e->ka_warps * e->E.ka_col_bytes; }
 
-// one round of group g on its stream: ka -> [ks] -> kb, with the parameters, grid and TMA descriptor of the group's environment
+// one round of group g on stream st: ka -> [ks] -> kb, with the parameters, grid and TMA descriptor of the group's environment
 template <class R>
-static int launch_round(TpEngine *e, int g, bool with_ks, bool tma, std::string *err)
+static int launch_round(TpEngine *e, int g, cudaStream_t st, bool with_ks, bool tma, std::string *err)
 {
     const int upper = e->glive[g], v = e->genv[g];
-    cudaStream_t st = e->gstream[g];
     ka_kernel<R><<<(upper + e->ka_warps - 1) / e->ka_warps, 32 * e->ka_warps, ka_smem_bytes(e), st>>>(e->E, e->p[v], g);
     if (with_ks) ks_kernel<R><<<upper, TP_KB_THREADS, ks_smem_bytes(e), st>>>(e->E, e->p[v], e->map[v], g);
     if (tma && e->have_tmap[v]) kb_kernel<R, true><<<upper, TP_KB_THREADS, kb_smem_bytes(e, true), st>>>(e->E, e->p[v], e->map[v], e->tmap[v], g);
@@ -610,39 +658,120 @@ static int set_attrs(TpEngine *e, std::string *err)
     return UALM_OK;
 }
 
-// `nr` rounds of every live group, interleaved over the groups' streams
-static int run_rounds(TpEngine *e, int nr, std::string *err)
+// The round loop of group g as one CUDA graph, launched on the group's stream:
+//     compact -> the first round (with ks_kernel when the problems start with initScaling)
+//     WHILE { chunk rounds -> compact -> [publish_kernel] -> loop_ctrl_kernel }
+// The body runs at least once and repeats until the group has no trajectory left to run.  Rounds are per-trajectory lockstep steps,
+// and compaction and publication only change which slots are listed and when results are copied out, so the loop computes what
+// host-queued rounds compute.  Everything a kernel reads from the engine is fixed at capture: the grids by glive[g], which stays
+// until the lane is collected; the pool's shared-memory layout and sizes by the maxima live now, which cover this batch; parameters,
+// grids and budget cannot change while a batch is in flight.  pub_gd: the descriptors publish_kernel walks (null: no publication)
+template <class R>
+static int launch_loop(TpEngine *e, int g, bool with_ks, const GatherDesc *pub_gd, int *launches, std::string *err)
 {
-    if (e->live <= 0) return UALM_OK;
-    int rc = e->f32() ? set_attrs<float>(e, err) : set_attrs<double>(e, err);
-    if (rc) return rc;
+    TpLane &l = e->lanes[g / TP_SUBGROUPS];
+    TpEngine::Loop &L = e->loops[g][(with_ks ? 2 : 0) + (pub_gd ? 1 : 0)];
+    cudaStream_t cs = e->capstream;
     const bool tma = e->use_tma;          // (for the environments whose grid has a tensor map)
-    for (int r = 0; r < nr; r++) {
-        for (int g = 0; g < TP_NGROUPS; g++) {
-            if (e->glive[g] <= 0) continue;
-            if (e->gcompact[g] || (e->grounds[g] % e->chunk) == 0) {
-                compact_kernel<<<1, 1024, 0, e->gstream[g]>>>(e->E, e->capacity, g);
-                e->gcompact[g] = false;
-            }
-            const bool with_ks = e->gscale[g] > 0;
-            rc = e->f32() ? launch_round<float>(e, g, with_ks, tma, err) : launch_round<double>(e, g, with_ks, tma, err);
-            if (rc) return rc;
-            if (e->gscale[g] > 0) e->gscale[g]--;
-            e->grounds[g]++;
-            e->lanes[g / TP_SUBGROUPS].launches += 2 + (with_ks ? 1 : 0);
+    const int body_launches = 2 * e->chunk + 2 + (pub_gd ? 1 : 0);
+    int rc = UALM_OK;
+    auto check = [&](cudaError_t ce, const char *what) {
+        if (ce != cudaSuccess && rc == UALM_OK) { if (err) *err = std::string(what) + ": " + cudaGetErrorString(ce); rc = UALM_ENOCUDA; }
+        return rc == UALM_OK;
+    };
+    auto clear = [&](cudaGraph_t G, cudaGraphNode_t keep) {         // every node of G but `keep`
+        size_t n = 0;
+        if (!check(cudaGraphGetNodes(G, nullptr, &n), "cudaGraphGetNodes")) return false;
+        std::vector<cudaGraphNode_t> nodes(n);
+        if (n && !check(cudaGraphGetNodes(G, nodes.data(), &n), "cudaGraphGetNodes")) return false;
+        for (cudaGraphNode_t v : nodes)
+            if (v != keep && !check(cudaGraphDestroyNode(v), "cudaGraphDestroyNode")) return false;
+        return true;
+    };
+    if (!L.G) {
+        cudaGraphNodeParams cp = {};
+        cp.type = cudaGraphNodeTypeConditional;
+        cp.conditional.type = cudaGraphCondTypeWhile;
+        cp.conditional.size = 1;
+        if (!check(cudaGraphCreate(&L.G, 0), "cudaGraphCreate") ||
+            !check(cudaGraphConditionalHandleCreate(&L.h, L.G, 1, cudaGraphCondAssignDefault), "cudaGraphConditionalHandleCreate"))
+            return rc;
+        cp.conditional.handle = L.h;
+        if (!check(cudaGraphAddNode(&L.cond, L.G, nullptr, 0, &cp), "cudaGraphAddNode(conditional)")) return rc;
+        L.body = cp.conditional.phGraph_out[0];
+    } else if (!clear(L.G, L.cond) || !clear(L.body, nullptr)) {
+        return rc;
+    }
+    // prologue, then the edge from its last node to the conditional node
+    std::vector<cudaGraphNode_t> tail;
+    if (!check(cudaStreamBeginCaptureToGraph(cs, L.G, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal), "cudaStreamBeginCaptureToGraph")) return rc;
+    compact_kernel<<<1, 1024, 0, cs>>>(e->E, e->capacity, g);
+    rc = launch_round<R>(e, g, cs, with_ks, tma, err);
+    {
+        cudaStreamCaptureStatus cst;
+        const cudaGraphNode_t *deps = nullptr;
+        size_t nd = 0;
+        if (check(cudaStreamGetCaptureInfo(cs, &cst, nullptr, nullptr, &deps, &nd), "cudaStreamGetCaptureInfo")) tail.assign(deps, deps + nd);
+    }
+    cudaGraph_t captured = nullptr;
+    check(cudaStreamEndCapture(cs, &captured), "cudaStreamEndCapture");
+    for (cudaGraphNode_t v : tail)
+        if (!check(cudaGraphAddDependencies(L.G, &v, &L.cond, 1), "cudaGraphAddDependencies")) break;
+    if (rc) return rc;
+    // body
+    if (!check(cudaStreamBeginCaptureToGraph(cs, L.body, nullptr, nullptr, 0, cudaStreamCaptureModeThreadLocal), "cudaStreamBeginCaptureToGraph")) return rc;
+    for (int r = 0; r < e->chunk && rc == UALM_OK; r++) rc = launch_round<R>(e, g, cs, false, tma, err);
+    if (rc == UALM_OK) {
+        compact_kernel<<<1, 1024, 0, cs>>>(e->E, e->capacity, g);
+        if (pub_gd) publish_kernel<R><<<l.B, 128, 0, cs>>>(e->E, pub_gd, l.B, l.d_pub.p, l.mbox.device());
+        loop_ctrl_kernel<<<1, 1, 0, cs>>>(L.h, e->n_active.p, e->gloop.p, g, e->chunk, body_launches);
+        check(cudaGetLastError(), "loop body launch");
+    }
+    check(cudaStreamEndCapture(cs, &captured), "cudaStreamEndCapture");
+    if (rc) return rc;
+    // the same graph with new kernel arguments and grids: updated in place (the previous batch of this group has finished)
+    if (L.exec) {
+        cudaGraphExecUpdateResultInfo info;
+        if (cudaGraphExecUpdate(L.exec, L.G, &info) != cudaSuccess) {
+            cudaGetLastError();
+            cudaGraphExecDestroy(L.exec);
+            L.exec = nullptr;
+            if (getenv("UALM_DEBUG")) fprintf(stderr, "[ualm-tp] group %d: loop graph re-instantiated (update result %d)\n", g, (int)info.result);
         }
     }
-    return UALM_OK;
+    if (!L.exec && !check(cudaGraphInstantiate(&L.exec, L.G, 0), "cudaGraphInstantiate")) return rc;
+    if (check(cudaGraphLaunch(L.exec, e->gstream[g]), "cudaGraphLaunch")) *launches += 3 + (with_ks ? 1 : 0);   // the prologue's; loop_ctrl_kernel counts the body's
+    return rc;
+}
+
+// launch the round loop of every live group of `lane` (after its admission); publish: its problems go to the mailbox as they end
+static int start_loops(TpEngine *e, int lane, bool publish, std::string *err)
+{
+    TpLane &l = e->lanes[lane];
+    int rc = e->f32() ? set_attrs<float>(e, err) : set_attrs<double>(e, err);
+    if (rc) return rc;
+    int ngroups = 0;
+    for (int q = 0; q < TP_SUBGROUPS; q++) ngroups += e->glive[lane * TP_SUBGROUPS + q] > 0;
+    for (int q = 0; q < TP_SUBGROUPS && rc == UALM_OK; q++) {
+        const int g = lane * TP_SUBGROUPS + q;
+        if (e->glive[g] <= 0) continue;
+        // each group publishes only its own problems: a slot of another group may be in the middle of its round
+        const GatherDesc *pub = !publish ? nullptr : ngroups > 1 ? l.d_gdg.p + (size_t)q * l.B : l.d_gd.p;
+        const bool with_ks = (l.mode == 0 && e->p[e->genv[g]].use_scaling) || l.mode == 2;
+        rc = e->f32() ? launch_loop<float>(e, g, with_ks, pub, &l.launches, err) : launch_loop<double>(e, g, with_ks, pub, &l.launches, err);
+    }
+    return rc;
 }
 
 // raise the stop words idx[0, n) of lane l's batch (idx = null: all B): set them in the mirror, then copy the whole mirror on the
-// engine's stream.  Words only go from 0 to 1 while the batch runs, so the copy never lowers one; the rounds the next poll or
-// wait queues see it (both synchronise the engine's stream first)
+// cancel stream, which no group loop occupies, so the copy lands while the lane's rounds run (ka_kernel's stop test takes a raise
+// that lands in the middle of a round).  Admission cleared the words and synchronised before the loops started, so the copy is
+// ordered after the clear; words only go from 0 to 1 while the batch runs, so the copy never lowers one
 static int raise_stop(TpEngine *e, TpLane &l, int n, const int32_t *idx, std::string *err)
 {
     if (idx) for (int k = 0; k < n; k++) l.h_stop[idx[k]] = 1;
     else for (int b = 0; b < l.B; b++) l.h_stop[b] = 1;
-    if (l.B > 0) TCK(cudaMemcpyAsync(l.d_stop.p, l.h_stop, sizeof(int) * l.B, cudaMemcpyHostToDevice, e->stream));
+    if (l.B > 0) TCK(cudaMemcpyAsync(l.d_stop.p, l.h_stop, sizeof(int) * l.B, cudaMemcpyHostToDevice, e->cstream));
     return UALM_OK;
 }
 
@@ -657,6 +786,18 @@ int tp_cancel(TpEngine *e, int lane, int n, const int32_t *idx, std::string *err
     return raise_stop(e, l, n, idx, err);
 }
 
+// whether the round loops of the lane's groups have all ended (a failed launch or loop is reported, not waited out)
+static int loops_done(TpEngine *e, int lane, bool *done, std::string *err)
+{
+    *done = true;
+    for (int q = 0; q < TP_SUBGROUPS; q++) {
+        const cudaError_t s = cudaStreamQuery(e->gstream[lane * TP_SUBGROUPS + q]);
+        if (s == cudaErrorNotReady) *done = false;
+        else TCK(s);
+    }
+    return UALM_OK;
+}
+
 int tp_collect(TpEngine *e, int lane, std::string *err, double timeout_ms)
 {
     if (lane < 0 || lane >= TP_LANES) { if (err) *err = "lane out of range"; return UALM_EINVAL; }
@@ -664,25 +805,29 @@ int tp_collect(TpEngine *e, int lane, std::string *err, double timeout_ms)
     if (l.collected) return UALM_OK;
     if (!l.in_flight) { if (err) *err = "nothing in flight on this lane"; return UALM_ESTATE; }
     TCK(cudaSetDevice(e->device));
-    const auto t0 = std::chrono::steady_clock::now();
-    bool cancelled = false;
-    long long guard = 0;
-    while (true) {
-        // the lane's own groups are the pace setters: wait for what was queued for them, then look at the lane's counter
-        for (int q = 0; q < TP_SUBGROUPS; q++) TCK(cudaStreamSynchronize(e->gstream[lane * TP_SUBGROUPS + q]));
-        TCK(cudaMemcpyAsync(e->h_remaining, e->remaining.p, sizeof(int) * TP_LANES, cudaMemcpyDeviceToHost, e->stream));
-        TCK(cudaStreamSynchronize(e->stream));
-        if (e->h_remaining[lane] <= 0) break;
-        if (timeout_ms >= 0.0 && !cancelled && std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() >= timeout_ms) {
-            // every stop word of the batch, read by ka_kernel at the stop tests of the rounds queued from now on
-            int rc = raise_stop(e, l, 0, nullptr, err);
-            if (rc) return rc;
-            TCK(cudaStreamSynchronize(e->stream));
-            cancelled = true;
+    if (timeout_ms >= 0.0) {
+        // deadline: yield-poll the lane's loops until it has passed, then raise every stop word of the batch and let the loops drain
+        // (every trajectory still running stops at its next stop test)
+        const auto t0 = std::chrono::steady_clock::now();
+        while (true) {
+            bool done = false;
+            if (int rc = loops_done(e, lane, &done, err)) return rc;
+            if (done) break;
+            if (std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() >= timeout_ms) {
+                if (int rc = raise_stop(e, l, 0, nullptr, err)) return rc;
+                break;
+            }
+            std::this_thread::yield();
         }
-        int rc = run_rounds(e, e->chunk, err);        // every live group advances, not only this lane's
-        if (rc) return rc;
-        if ((guard += e->chunk) > 400000) { if (err) *err = "throughput engine: a trajectory did not terminate"; return UALM_ENOCUDA; }
+    }
+    for (int q = 0; q < TP_SUBGROUPS; q++) TCK(cudaStreamSynchronize(e->gstream[lane * TP_SUBGROUPS + q]));
+    // a raise the batch outran may still be queued: it lands before the lane's next clear, and the mirror is free again
+    TCK(cudaStreamSynchronize(e->cstream));
+    TCK(cudaMemcpyAsync(e->h_gloop, e->gloop.p + lane * TP_SUBGROUPS, sizeof(GroupLoop) * TP_SUBGROUPS, cudaMemcpyDeviceToHost, e->stream));
+    TCK(cudaStreamSynchronize(e->stream));
+    for (int q = 0; q < TP_SUBGROUPS; q++) {
+        if (e->h_gloop[q].err) { if (err) *err = "throughput engine: a trajectory did not terminate"; return UALM_ENOCUDA; }
+        l.launches += e->h_gloop[q].launches;
     }
     // gather the batch's results into the lane's packed device outputs, free its slots
     const bool ev = l.mode != 0;
@@ -708,7 +853,7 @@ int tp_collect(TpEngine *e, int lane, std::string *err, double timeout_ms)
     for (int s : l.slots) e->free_slots.push_back(s);
     e->live -= (int)l.slots.size();
     l.slots.clear();
-    for (int q = 0; q < TP_SUBGROUPS; q++) { const int g = lane * TP_SUBGROUPS + q; e->glive[g] = 0; e->gscale[g] = 0; e->gcompact[g] = false; }
+    for (int q = 0; q < TP_SUBGROUPS; q++) e->glive[lane * TP_SUBGROUPS + q] = 0;
     l.in_flight = false; l.collected = true; l.publish = false;
     return UALM_OK;
 }
@@ -720,20 +865,12 @@ int tp_poll(TpEngine *e, int lane, double wait_ms, int32_t *idx, int *n_new, int
     if (!l.in_flight || !l.publish) { if (err) *err = "ticket is not in flight"; return UALM_ESTATE; }
     TCK(cudaSetDevice(e->device));
     const auto t0 = std::chrono::steady_clock::now();
-    int n = l.mbox.collect(idx, results, c_xy, c_yaw);      // the problems over the compiled limits, published at submit
-    // the engine advances only inside host calls: each try is one iteration of tp_collect's loop with the publication in place of
-    // the counter read
-    while (n == 0 && l.mbox.pending() > 0) {
-        for (int q = 0; q < TP_SUBGROUPS; q++) TCK(cudaStreamSynchronize(e->gstream[lane * TP_SUBGROUPS + q]));
-        if (e->f32()) publish_kernel<float><<<l.B, 128, 0, e->stream>>>(e->E, l.d_gd.p, l.B, l.d_pub.p, l.mbox.device());
-        else publish_kernel<double><<<l.B, 128, 0, e->stream>>>(e->E, l.d_gd.p, l.B, l.d_pub.p, l.mbox.device());
-        TCK(cudaGetLastError());
-        TCK(cudaStreamSynchronize(e->stream));         // before the next rounds are queued: the slots it reads stay as they are
-        n = l.mbox.collect(idx, results, c_xy, c_yaw);
-        if (l.mbox.pending() > 0) {
-            const int rc = run_rounds(e, e->chunk, err);
-            if (rc) return rc;
-        }
+    int n = 0;
+    while (true) {
+        n = l.mbox.collect(idx, results, c_xy, c_yaw);       // the group loops publish into the mailbox as problems finish
+        if (n > 0 || l.mbox.pending() == 0 || wait_ms == 0.0) break;
+        bool done = false;
+        if (int rc = loops_done(e, lane, &done, err)) return rc;
         if (std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count() >= wait_ms) break;
         std::this_thread::yield();
     }
@@ -850,7 +987,7 @@ int tp_eval(TpEngine *e, int lane, const double *x, const double *lambda, const 
     if ((rc = put(e, l.d_sfin, scale_fx, l.B, l.has_sfx, err))) return rc;
     l.rho_eval = rho;
     l.has_xev = xev;
-    rc = admit_impl(e, lane, 1, false, err);
+    rc = admit_impl(e, lane, 1, false, false, true, err);
     l.has_lam = l.has_mu = l.has_scx = l.has_sfx = l.has_xev = false;
     if (rc) return rc;
     if ((rc = tp_collect(e, lane, err))) return rc;
@@ -873,7 +1010,7 @@ int tp_init_scaling(TpEngine *e, int lane, double *scale_fx, double *scale_cx, s
     if (!l.have_batch) { if (err) *err = "upload and set_map first"; return UALM_ESTATE; }
     for (int b = 0; b < l.B; b++) if (l.N[b] > TP_NMAX || l.M[b] > TP_MMAX) { if (err) *err = "batch holds problems over the compiled limits"; return UALM_ELIMIT; }
     TCK(cudaSetDevice(e->device));
-    int rc = admit_impl(e, lane, 2, false, err);
+    int rc = admit_impl(e, lane, 2, false, false, true, err);
     if (rc) return rc;
     if ((rc = tp_collect(e, lane, err))) return rc;
     if (l.B > 0) {
@@ -898,14 +1035,13 @@ int tp_time_penalty(TpEngine *e, int lane, int reps, int use_tma, float *ms_per_
     const int v = l.env[0];
     // admit as single evaluations (initial guess, zero duals, unit scales), run the forward half of a round, then time kb alone
     l.has_lam = l.has_mu = l.has_scx = l.has_sfx = false; l.rho_eval = e->p[v].rho;
-    int rc = admit_impl(e, lane, 1, true, err);
+    int rc = admit_impl(e, lane, 1, true, false, false, err);
     if (rc) return rc;
     rc = e->f32() ? set_attrs<float>(e, err) : set_attrs<double>(e, err);
     if (rc) return rc;
     const int g = lane * TP_SUBGROUPS;
     cudaStream_t st = e->gstream[g];
     compact_kernel<<<1, 1024, 0, st>>>(e->E, e->capacity, g);
-    e->gcompact[g] = false;
     const int upper = e->glive[g];
     const bool tma = e->have_tmap[v] && use_tma;
     if (e->f32()) ka_kernel<float><<<(upper + e->ka_warps - 1) / e->ka_warps, 32 * e->ka_warps, ka_smem_bytes(e), st>>>(e->E, e->p[v], g);
@@ -935,8 +1071,9 @@ int tp_time_penalty(TpEngine *e, int lane, int reps, int use_tma, float *ms_per_
         for (int b = 0; b < l.B; b++) bytes += (double)l.N[b] * (e->p[v].int_K + 1) * 45 * es + (25.0 * l.N[b] + 13.0 * l.M[b]) * es;
         *algorithmic_bytes = bytes;
     }
-    // finish the evaluations and release the slots
-    rc = tp_collect(e, lane, err);
+    // finish the evaluations (the group's loop, queued behind the timed launches) and release the slots
+    rc = start_loops(e, lane, false, err);
+    if (rc == UALM_OK) rc = tp_collect(e, lane, err);
     l.collected = false;
     return rc;
 }

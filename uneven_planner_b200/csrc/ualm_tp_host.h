@@ -16,23 +16,24 @@ void tp_destroy(TpEngine *e);
 // parameters / grid of environment `env` (0 <= env < UALM_MAX_ENVS)
 int tp_set_params(TpEngine *e, int env, const ualm_params_t *p, std::string *err);
 int tp_set_map(TpEngine *e, int env, const ualm_map_geom_t *g, const float *cells, std::string *err);
-// lanes = tickets: a lane holds one uploaded batch; admit puts it into the pool of running trajectories, collect drives the
-// evaluation rounds until that lane's batch is finished and gathers its results on the device.  env[B]: environment of every
+// lanes = tickets: a lane holds one uploaded batch; admit puts it into the pool of running trajectories and launches the round loop
+// of each of its groups on the device, collect waits for those loops to end and gathers the batch's results on the device.  env[B]: environment of every
 // problem (NULL = all 0), in range and bound (the caller checks)
 int tp_upload(TpEngine *e, int lane, int B, const int32_t *N, const int32_t *M, const int32_t *env, const double *bnd, const double *total_time,
               const double *inner_xy, const double *inner_yaw, std::string *err);
-// asynchronous.  publish: the batch's problems go to the lane's result mailbox as they finish (ualm_submit_batch, for tp_poll)
+// asynchronous: the batch runs to completion without further calls.  publish: the group loops copy the batch's problems into the
+// lane's result mailbox as they finish (ualm_submit_batch, for tp_poll)
 int tp_admit(TpEngine *e, int lane, std::string *err, bool publish = false);
-// ualm_poll_batch on a lane admitted with publish: one step of the engine per try (wait for the lane's queued rounds, publish its
-// finished problems, queue the next rounds of every live group), repeated until a problem is new or wait_ms has passed
+// ualm_poll_batch on a lane admitted with publish: reads the mailbox only (wait_ms > 0: yield-polls its flags until a problem is
+// new or wait_ms has passed); it neither synchronises nor queues anything
 int tp_poll(TpEngine *e, int lane, double wait_ms, int32_t *idx, int *n_new, int *n_pending, ualm_result_t *results, double *c_xy, double *c_yaw,
             std::string *err);
-// ualm_cancel_problems on a lane admitted with publish: raises the stop words idx[0, n) (the caller checked n and idx), which the
-// rounds queued by the next tp_poll / tp_collect see.  UALM_ESTATE when the lane is not in flight, UALM_EINVAL for an index
+// ualm_cancel_problems on a lane admitted with publish: raises the stop words idx[0, n) (the caller checked n and idx) by a copy on
+// the cancel stream, which reaches the rounds that are running.  UALM_ESTATE when the lane is not in flight, UALM_EINVAL for an index
 // outside [0, B); nothing is raised on either
 int tp_cancel(TpEngine *e, int lane, int n, const int32_t *idx, std::string *err);
-// blocks: rounds until the lane's batch is done.  timeout_ms >= 0: once that much time has passed since the call, every stop word
-// of the lane's batch is raised before the next rounds (its trajectories stop at their next stop test)
+// blocks until the lane's group loops have ended.  timeout_ms >= 0: once that much time has passed since the call, every stop word
+// of the lane's batch is raised (its trajectories stop at their next stop test) and the loops drain
 int tp_collect(TpEngine *e, int lane, std::string *err, double timeout_ms = -1.0);
 int tp_set_budget(TpEngine *e, int max_evals, std::string *err);              // evaluation budget of the solves admitted afterwards
 int tp_download(TpEngine *e, int lane, ualm_result_t *results, double *c_xy, double *c_yaw, std::string *err);

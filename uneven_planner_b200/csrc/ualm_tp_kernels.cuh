@@ -866,6 +866,22 @@ __global__ void compact_kernel(const __grid_constant__ TpPool E, int hi, int gro
     if (threadIdx.x == 0) E.n_active[group] = s_count;
 }
 
+// the device-side round loop of one group (ualm_tp.cu: start_loops): what it has run, and whether it hit the round cap
+struct GroupLoop { long long rounds; int launches, err; };
+#define TP_ROUND_CAP 400000             // rounds of one group's loop; a trajectory still running after them did not terminate
+
+// last node of a group's loop body, after the body's compaction: counts the body's rounds and kernel launches, and runs the body
+// again while the group still has a trajectory that is not PH_DONE (n_active > 0) and the round cap is not reached (err = 1 there)
+__global__ void loop_ctrl_kernel(cudaGraphConditionalHandle h, const int *n_active, GroupLoop *gl, int group, int rounds, int launches)
+{
+    GroupLoop &s = gl[group];
+    s.rounds += rounds;
+    s.launches += launches;
+    const bool capped = s.rounds >= TP_ROUND_CAP;
+    if (capped && n_active[group] > 0) s.err = 1;
+    cudaGraphSetConditional(h, (n_active[group] > 0 && !capped) ? 1u : 0u);
+}
+
 // ---------------------------------------------------------------------------------------------------------------------
 // admission: problem b of a submitted batch -> slot.  One launch covers problems of one environment (use_scaling, K are its own);
 // off_s[b]: sample offset of ad[b] in the caller's dual arrays, sfx is indexed by the problem's index in its batch

@@ -791,7 +791,7 @@ __global__ void gather_kernel(const __grid_constant__ TpPool E, const GatherDesc
 // finished problems of a batch in flight -> the lane's result mailbox (ualm_poll_batch, ualm_mailbox.h), one CTA per problem.  A slot
 // is freed only when its batch is collected, so a slot in PH_DONE holds the final state gather_kernel will read: the mailbox gets
 // the bits ualm_wait_batch returns.  pub[b] marks problem b published (device memory: the device never reads the mailbox).  Runs
-// while none of the lane's rounds does
+// in the round loop of a group between its rounds, over descriptors that list only that group's problems (ualm_tp.cu)
 template <class R>
 __global__ void publish_kernel(const __grid_constant__ TpPool E, const GatherDesc *gd, int B, int *pub, const __grid_constant__ ualm_mbox::Ptrs mb)
 {
