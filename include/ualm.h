@@ -123,6 +123,24 @@ int ualm_set_map(ualm_ctx_t *ctx, const ualm_map_geom_t *g, const float *cells);
  * for maps built in-process by the reference); != 0 rounds them to the float4 grid of ualm_set_map (41 MB, what a map read
  * back from this repo's .umap file or from the reference's 6-digit CSV cache holds anyway). */
 int ualm_set_map_f64(ualm_ctx_t *ctx, const ualm_map_geom_t *g, const double *cells, int repack_to_float);
+/* Replace (or bind) the grid of the selected environment for every launch from now on; allowed while batches are in flight.
+ * Work launched before the call keeps the grid it was launched with, bit for bit: batches in flight, and ualm_feasibility_batch
+ * of a lane solved before the call.  Every later launch reads the new grid: ualm_submit_batch*, ualm_solve_resident,
+ * ualm_solve_batch*, the phase entry points.  On return the new grid is complete on the device; the call never waits for
+ * running batches.  On any error the previous grid stays current.  The geometry may differ from the previous grid's.  A null
+ * ctx / g / cells or a voxel_num <= 0 is UALM_EINVAL.
+ * Memory: the grid an environment had before an update stays allocated while a lane still holds it (a lane holds the grids its
+ * last launch read until its next launch or ualm_destroy), so an environment holds at most one grid per such lane plus the
+ * current one.  The grid is float4 (41 MB for 200x200x64); ualm_set_map_f64 keeps serving the double grid when nothing is in
+ * flight.  ualm_set_map / ualm_set_map_f64 keep writing into the current grid in place. */
+int ualm_update_map(ualm_ctx_t *ctx, const ualm_map_geom_t *g, const float *cells);
+/* The same, with the grid built on the device from a point cloud (ualm_map_build_device's preprocessing and kernel) straight into
+ * the new grid: no host round trip.  cells_out (optional, host) receives the grid, which the host front end needs
+ * (ualm_astar_map_t reads sigma from it).  kernel_ms optional.  A null pts or npts < 0 is UALM_EINVAL as well.  The call queues
+ * nothing behind a batch, but its kernel needs free SMs: on the parity path the solve holds them until its work queue runs dry, so
+ * there the call can last into the tail of the batches in flight (DESIGN.md section 3h). */
+int ualm_update_map_from_cloud(ualm_ctx_t *ctx, const float *pts, int64_t npts, const ualm_map_geom_t *g, double ellipsoid_x,
+                               double ellipsoid_y, double ellipsoid_z, int iter_num, float *cells_out, float *kernel_ms);
 
 /* ---- batch solve = B independent optimizeSE2Traj calls ----
  * Ragged inputs are packed back to back in problem order: inner_xy has sum 2(N_b-1) doubles,

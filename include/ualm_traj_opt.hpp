@@ -172,6 +172,20 @@ public:
         bindEnv(env, p, [&] { return ualm_set_map_f64(ctx_, &geom, rxs2_cells, repack_to_float ? 1 : 0); }, "ualm_set_map_f64");
     }
 
+    // Replace the grid of environment `env` while batches are in flight (ualm_update_map): work launched before keeps its grid, every
+    // later launch reads the new one; the call does not wait for running batches.  The parameters of `env` stay as bound
+    void updateEnvironment(int env, const ualm_map_geom_t &geom, const float *cells_xyzw)
+    {
+        onEnv(env, [&] { return ualm_update_map(ctx_, &geom, cells_xyzw); }, "ualm_update_map");
+    }
+    // the same with the grid built on the device from a point cloud (npts x 3 floats); cells_out (optional) receives the grid
+    void updateEnvironmentFromCloud(int env, const float *pts, int64_t npts, const ualm_map_geom_t &geom, double ellipsoid_x = 0.2, double ellipsoid_y = 0.1,
+                                    double ellipsoid_z = 0.1, int iter_num = 2, float *cells_out = nullptr, float *kernel_ms = nullptr)
+    {
+        onEnv(env, [&] { return ualm_update_map_from_cloud(ctx_, pts, npts, &geom, ellipsoid_x, ellipsoid_y, ellipsoid_z, iter_num, cells_out, kernel_ms); },
+              "ualm_update_map_from_cloud");
+    }
+
     // ---- single problem, the reference's call (alm_traj_opt.h:92-98), plain pointers ----
     // initStateXY/endStateXY: 2x3 column-major; innerPtsXY: 2 x (N-1) column-major; initYaw/endYaw: 3; innerPtsYaw: M-1
     int optimizeSE2Traj(const double *initStateXY, const double *endStateXY, const double *innerPtsXY, int n_inner_xy,
@@ -298,6 +312,16 @@ private:
         const std::string msg2 = msg.empty() && rc != UALM_OK ? std::string(what) + ": " + ualm_last_error() : msg;
         ualm_select_env(ctx_, 0);
         if (rc != UALM_OK) throw std::runtime_error(msg2);
+    }
+    // select `env`, run `call`, select environment 0 again (also when the call fails)
+    template <class F>
+    void onEnv(int env, F call, const char *what)
+    {
+        check(ualm_select_env(ctx_, env), "ualm_select_env");
+        const int rc = call();
+        const std::string msg = rc != UALM_OK ? std::string(what) + ": " + ualm_last_error() : std::string();
+        ualm_select_env(ctx_, 0);
+        if (rc != UALM_OK) throw std::runtime_error(msg);
     }
     ualm_ctx_t *ctx_ = nullptr;
     ualm_result_t last_{};

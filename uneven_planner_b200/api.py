@@ -104,6 +104,37 @@ class BatchALMTrajOpt:
             _check(self.L.ualm_set_map(self.h, C.byref(mapdata.geom), mapdata.cells.ctypes.data_as(C.POINTER(C.c_float))))
         return self
 
+    def update_environment(self, mapdata, env=None):
+        """ualm_update_map: replaces the float grid of environment `env` (None: the selected one, as for set_environment) while batches
+        may be in flight.  Work launched before keeps its grid (batches in flight, feasibility of a lane solved before); every later
+        launch reads the new one.  Returns once the new grid is on the device, without waiting for running batches."""
+        if env is not None:
+            self.select_env(env)
+        if self.env == 0:
+            self.map = mapdata
+        cells = np.ascontiguousarray(mapdata.cells, np.float32)
+        _check(self.L.ualm_update_map(self.h, C.byref(mapdata.geom), cells.ctypes.data_as(C.POINTER(C.c_float))))
+        return self
+
+    def update_environment_from_cloud(self, pts, geom=None, ellipsoid=(0.2, 0.1, 0.1), iter_num=2, env=None, name="map"):
+        """ualm_update_map_from_cloud: update_environment with the grid built on the device from a point cloud (as build_map) straight
+        into the new grid.  Returns (UnevenMapData of the new grid, as the host front end needs it; kernel ms)."""
+        from . import maps
+        geom = geom or _lib.map_geometry()
+        if env is not None:
+            self.select_env(env)
+        X, Y, W = geom.voxel_num
+        cells = np.zeros((X, Y, W, 4), np.float32)
+        pts = np.ascontiguousarray(pts, dtype=np.float32).reshape(-1, 3)
+        ms = C.c_float()
+        fp = C.POINTER(C.c_float)
+        _check(self.L.ualm_update_map_from_cloud(self.h, pts.ctypes.data_as(fp), pts.shape[0], C.byref(geom), ellipsoid[0], ellipsoid[1], ellipsoid[2],
+                                                 iter_num, cells.ctypes.data_as(fp), C.byref(ms)))
+        m = maps.UnevenMapData(geom, cells, name)
+        if self.env == 0:
+            self.map = m
+        return m, ms.value
+
     def reset_stream(self):
         _check(self.L.ualm_reset_stream(self.h))
         return self

@@ -12,6 +12,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <numeric>
 #include <string>
 #include <thread>
@@ -46,6 +47,20 @@ struct DevBuf {
     }
     void release() { if (p) cudaFree(p); p = nullptr; cap = 0; }
 };
+
+// One version of an environment's map grid: its device buffer ([X][Y][Yaw] float4, or 4 doubles per cell from ualm_set_map_f64) and
+// the DevMap that points into it.  The environment holds its current version, and every lane holds the versions its last launch read
+// until its next launch or its release, so ualm_update_map* never changes a grid that queued work or a later scan of that work reads.
+// The buffer is freed on the context's free stream, which waits for the completion of every lane that let go of a version (lane_hold),
+// so the last holder's release frees it without a host or device-wide wait.
+struct MapVer {
+    cudaStream_t fs = nullptr;
+    void *p = nullptr;
+    size_t bytes = 0;
+    DevMap dm = {};
+    ~MapVer() { if (p) cudaFreeAsync(p, fs); }
+};
+typedef std::shared_ptr<MapVer> MapRef;
 
 // One in-flight batch ("lane"): its own device buffers, launch plan, streams and events.  A context owns up to UALM_MAX_LANES of
 // them so that several batches can be resident and running at once (the stragglers of batch k drain while batch k+1 fills the
@@ -95,8 +110,10 @@ struct Lane {
     bool raised = false;                 // a raise copy of the batch in flight may still be queued on the cancel stream
     cudaEvent_t ev_clear = nullptr;
     ualm_mbox::Mailbox mbox;             // results of a submitted batch as its problems finish (ualm_poll_batch)
+    MapRef vref[UALM_MAX_ENVS];          // the grid versions the lane's last launch read, per environment of its batch (lane_hold)
     void release()
     {
+        for (auto &r : vref) r.reset();
         d_stop.release();
         if (h_stop) cudaFreeHost(h_stop);
         h_stop = nullptr; h_stop_cap = 0;
@@ -122,9 +139,7 @@ struct Env {
     bool have_params = false, have_map = false;
     ualm_params_t hp;
     DevParams dp;
-    DevMap dm;
-    DevBuf<float4> cells;
-    DevBuf<double> cells64;
+    MapRef map;                          // the current grid version: what every launch from now on reads
 };
 
 struct ualm_ctx {
@@ -144,6 +159,11 @@ struct ualm_ctx {
     // raises of the lanes' stop words (ualm_cancel_problems, ualm_wait_batch_for): copies go through the copy engines, so they do
     // not wait for free SMs
     cudaStream_t cancel = nullptr;
+    // grid versions: allocated, filled and built on `mstream`, freed on `fstream` (MapVer).  No solve runs on either, so an update
+    // never waits for one, and fstream's waits for lanes never hold up an update.  They come from a memory pool of their own, so a
+    // freed grid shares no pool block with other buffers and goes back to the device at the next synchronisation
+    cudaStream_t mstream = nullptr, fstream = nullptr;
+    cudaMemPool_t mpool = nullptr;
 };
 
 static int lane_make(ualm_ctx *c, Lane &l)
@@ -188,10 +208,19 @@ extern "C" int ualm_create(ualm_ctx_t **out, int device, int precision)
     c->device = device; c->precision = precision;
     if (const char *e = getenv("UALM_GROUPS")) c->group_mode = atoi(e);   // 0 = one warp per trajectory everywhere (developer switch)
     c->b = &c->lanes[0];
+    cudaMemPoolProps pp = {};
+    pp.allocType = cudaMemAllocationTypePinned;
+    pp.location.type = cudaMemLocationTypeDevice;
+    pp.location.id = device;
+    if (cudaStreamCreateWithFlags(&c->mstream, cudaStreamNonBlocking) != cudaSuccess || cudaStreamCreateWithFlags(&c->fstream, cudaStreamNonBlocking) != cudaSuccess ||
+        cudaMemPoolCreate(&c->mpool, &pp) != cudaSuccess) {
+        ualm_destroy(c);
+        return fail(UALM_ENOCUDA, "context map streams");
+    }
     if (precision != 64) {
         std::string em;
         const int rc = ualm_tp::tp_create(&c->tp, device, precision, &em);
-        if (rc != UALM_OK) { delete c; return fail(rc, em); }
+        if (rc != UALM_OK) { ualm_destroy(c); return fail(rc, em); }
         *out = c;
         return UALM_OK;
     }
@@ -214,8 +243,11 @@ extern "C" int ualm_destroy(ualm_ctx_t *c)
     cudaSetDevice(c->device);
     cudaDeviceSynchronize();
     if (c->tp) { ualm_tp::tp_destroy(c->tp); c->tp = nullptr; }
-    for (auto &v : c->envs) { v.cells.release(); v.cells64.release(); }
+    for (auto &v : c->envs) v.map.reset();
     for (auto &l : c->lanes) l.release();
+    if (c->fstream) { cudaStreamSynchronize(c->fstream); cudaStreamDestroy(c->fstream); }     // the grids' frees
+    if (c->mstream) cudaStreamDestroy(c->mstream);
+    if (c->mpool) cudaMemPoolDestroy(c->mpool);
     if (c->join) cudaStreamDestroy(c->join);
     if (c->cancel) cudaStreamDestroy(c->cancel);
     if (c->evA) cudaEventDestroy(c->evA);
@@ -306,13 +338,76 @@ extern "C" int ualm_select_env(ualm_ctx_t *c, int env)
     return UALM_OK;
 }
 
-static int map_geometry_set(Env &v, const ualm_map_geom_t *g)
+static void map_geometry_set(DevMap &m, const ualm_map_geom_t *g)
 {
-    DevMap &m = v.dm;
     for (int k = 0; k < 3; k++) { m.vn[k] = g->voxel_num[k]; m.origin[k] = g->origin[k]; m.maxb[k] = g->max_boundary[k]; }
     m.xy_res = g->xy_resolution; m.yaw_res = g->yaw_resolution;
     m.xy_inv = 1.0 / g->xy_resolution; m.yaw_inv = 1.0 / g->yaw_resolution; // uneven_map.cpp:104-105
+}
+
+static size_t map_ncell(const ualm_map_geom_t *g) { return (size_t)g->voxel_num[0] * g->voxel_num[1] * g->voxel_num[2]; }
+
+// a new grid version of `bytes` bytes, allocated on the map stream (usable once that stream is synchronised)
+static int map_version_new(ualm_ctx *c, size_t bytes, MapRef *out)
+{
+    MapRef v = std::make_shared<MapVer>();
+    v->fs = c->fstream;
+    const cudaError_t e = cudaMallocFromPoolAsync(&v->p, std::max<size_t>(bytes, 1), c->mpool, c->mstream);
+    if (e != cudaSuccess) {
+        v->p = nullptr;
+        cudaGetLastError();      // an allocation failure is not sticky: clear it, so no later launch check reports it
+        return fail(UALM_ENOCUDA, std::string("grid allocation: ") + cudaGetErrorString(e));
+    }
+    v->bytes = bytes;
+    *out = std::move(v);
+    return UALM_OK;
+}
+
+// ualm_set_map / ualm_set_map_f64: the host grid into the selected environment's CURRENT version, in place, so a lane that holds it
+// reads the new cells (ualm_set_map's contract).  The caller refused a batch in flight and synchronised the device
+static int map_write_current(ualm_ctx *c, const ualm_map_geom_t *g, const void *cells, size_t bytes, bool f64)
+{
+    Env &v = c->envs[c->sel_env];
+    v.have_map = false;         // until the copy below is complete (a failed copy leaves the environment unbound, not half bound)
+    if (!v.map) {
+        if (int rc = map_version_new(c, bytes, &v.map)) return rc;
+    } else if (v.map->bytes < bytes) {       // grown in place: the lanes that hold this version see the new buffer
+        CK(cudaFreeAsync(v.map->p, c->mstream));
+        v.map->p = nullptr; v.map->bytes = 0;
+        CK(cudaMallocFromPoolAsync(&v.map->p, bytes, c->mpool, c->mstream));
+        v.map->bytes = bytes;
+    }
+    CK(cudaMemcpyAsync(v.map->p, cells, bytes, cudaMemcpyHostToDevice, c->mstream));
+    CK(cudaStreamSynchronize(c->mstream));
+    DevMap &m = v.map->dm;
+    m.cells = f64 ? nullptr : (const float4 *)v.map->p;
+    m.cells64 = f64 ? (const double *)v.map->p : nullptr;
+    map_geometry_set(m, g);
+    if (c->tp) ualm_tp::tp_bind_map(c->tp, c->sel_env, g, m.cells);
     v.have_map = true;
+    return UALM_OK;
+}
+
+// ualm_update_map*: the complete float4 version nv becomes the selected environment's current grid.  The version it replaces is freed
+// once no lane holds it any more
+static void map_install(ualm_ctx *c, const ualm_map_geom_t *g, MapRef nv)
+{
+    Env &v = c->envs[c->sel_env];
+    nv->dm.cells = (const float4 *)nv->p;
+    nv->dm.cells64 = nullptr;
+    map_geometry_set(nv->dm, g);
+    if (c->tp) ualm_tp::tp_bind_map(c->tp, c->sel_env, g, nv->dm.cells);
+    v.map = std::move(nv);
+    v.have_map = true;
+}
+
+// lane l launches a batch of the environments in `mask`: it holds their current versions from now on, and lets go of the versions of
+// its previous launch.  That launch may still run (ualm_solve_resident twice on one lane), so the free stream first waits for its
+// completion: whatever only it held is freed after it.  A throughput lane is relaunched only once collected (ctx lanes not made)
+static int lane_hold(ualm_ctx *c, Lane &l, unsigned mask)
+{
+    if (l.made) CK(cudaStreamWaitEvent(c->fstream, l.ev1, 0));
+    for (int e = 0; e < UALM_MAX_ENVS; e++) l.vref[e] = (mask >> e) & 1u ? c->envs[e].map : nullptr;
     return UALM_OK;
 }
 
@@ -321,20 +416,8 @@ extern "C" int ualm_set_map(ualm_ctx_t *c, const ualm_map_geom_t *g, const float
     if (!c || !g || !cells) return fail(UALM_EINVAL, "null argument");
     if (int rc = lanes_idle(c, "ualm_set_map")) return rc;
     CK(cudaSetDevice(c->device));
-    // the engine's grid first: the context's copy (which serves the post-solve scan) and its flag change only once it is bound
-    if (c->tp) {
-        std::string em;
-        if (int rc = ualm_tp::tp_set_map(c->tp, c->sel_env, g, cells, &em)) return fail(rc, em);
-    }
     CK(cudaDeviceSynchronize());
-    const size_t ncell = (size_t)g->voxel_num[0] * g->voxel_num[1] * g->voxel_num[2];
-    Env &v = c->envs[c->sel_env];
-    v.have_map = false;         // until the copy below is complete (a failed copy leaves the environment unbound, not half bound)
-    CK(v.cells.ensure(ncell));
-    CK(cudaMemcpy(v.cells.p, cells, ncell * sizeof(float4), cudaMemcpyHostToDevice));
-    v.cells64.release();
-    v.dm.cells = v.cells.p; v.dm.cells64 = nullptr;
-    return map_geometry_set(v, g);
+    return map_write_current(c, g, cells, map_ncell(g) * sizeof(float4), false);
 }
 
 // the reference's own grid: UnevenMap::map_buffer is RXS2 {double z, sigma; Vector2d zb} = 4 doubles per cell (uneven_map.h:36-64)
@@ -344,19 +427,13 @@ extern "C" int ualm_set_map_f64(ualm_ctx_t *c, const ualm_map_geom_t *g, const d
     if (int rc = lanes_idle(c, "ualm_set_map_f64")) return rc;
     CK(cudaSetDevice(c->device));
     CK(cudaDeviceSynchronize());
-    const size_t ncell = (size_t)g->voxel_num[0] * g->voxel_num[1] * g->voxel_num[2];
+    const size_t ncell = map_ncell(g);
     if (repack_to_float || c->tp) {      // the throughput path always reads the float4 grid
         std::vector<float> f(4 * ncell);
         for (size_t q = 0; q < 4 * ncell; q++) f[q] = (float)cells[q];
         return ualm_set_map(c, g, f.data());
     }
-    Env &v = c->envs[c->sel_env];
-    v.have_map = false;         // until the copy below is complete
-    CK(v.cells64.ensure(4 * ncell));
-    CK(cudaMemcpy(v.cells64.p, cells, 4 * ncell * sizeof(double), cudaMemcpyHostToDevice));
-    v.cells.release();
-    v.dm.cells = nullptr; v.dm.cells64 = v.cells64.p;
-    return map_geometry_set(v, g);
+    return map_write_current(c, g, cells, 4 * ncell * sizeof(double), true);
 }
 
 // the one-warp-per-problem layout of every environment present in the lane's batch (sized by that environment's maxima)
@@ -631,6 +708,9 @@ static int solve_launch(ualm_ctx *c, bool publish)
     // (the upload checked that every environment of the batch is bound, and nothing unbinds one)
     if (!l->have_batch) return fail(UALM_ESTATE, "set_params, set_map and upload must precede solve");
     CK(cudaSetDevice(c->device));
+    unsigned mask = 0;
+    for (int e = 0; e < UALM_MAX_ENVS; e++) if (l->eoff[e + 1] > l->eoff[e]) mask |= 1u << e;
+    if (int rc = lane_hold(c, *l, mask)) return rc;
     l->last_launches = 0;
     // no stop request carries over: the words are cleared before the solve, and raises are queued after ev_clear
     if (l->h_stop) memset(l->h_stop, 0, sizeof(int) * l->h_stop_cap);
@@ -658,7 +738,7 @@ static int solve_launch(ualm_ctx *c, bool publish)
             DevParams dp = c->envs[cl.env].dp;
             dp.cancel = l->d_stop.p;
             dp.max_evals = c->max_evals;
-            solve_kernel<<<cl.grid, UALM_THREADS * UALM_WPB, cl.smem, st>>>(bp, dp, c->envs[cl.env].dm, cl.L);
+            solve_kernel<<<cl.grid, UALM_THREADS * UALM_WPB, cl.smem, st>>>(bp, dp, l->vref[cl.env]->dm, cl.L);
             CK(cudaGetLastError());
             l->last_launches++;
             if (ci > 0) { CK(cudaEventRecord(l->evs[ai], st)); CK(cudaStreamWaitEvent(l->stream, l->evs[ai], 0)); }
@@ -672,7 +752,11 @@ static int solve_launch(ualm_ctx *c, bool publish)
 extern "C" int ualm_solve_resident(ualm_ctx_t *c)
 {
     if (!c) return fail(UALM_EINVAL, "null ctx");
-    if (c->tp) TP_CALL(ualm_tp::tp_admit(c->tp, c->cur, err));      // joins the pool of running trajectories; its rounds run on the device, ualm_sync waits
+    if (c->tp) {     // joins the pool of running trajectories; its rounds run on the device, ualm_sync waits
+        std::string em;
+        if (int rc = ualm_tp::tp_admit(c->tp, c->cur, &em)) return fail(rc, em);
+        return lane_hold(c, c->lanes[c->cur], ualm_tp::tp_lane_env_mask(c->tp, c->cur));
+    }
     return solve_launch(c, false);
 }
 
@@ -779,7 +863,7 @@ extern "C" int ualm_submit_batch_env(ualm_ctx_t *c, int B, const int32_t *N, con
         if (!rc) rc = ualm_tp::tp_admit(c->tp, lane, &em, true);
         if (rc) return fail(rc, em);
         *ticket = lane; c->next_submit = (lane + 1) % depth;
-        return UALM_OK;
+        return lane_hold(c, c->lanes[lane], ualm_tp::tp_lane_env_mask(c->tp, lane));
     }
     if (c->lanes[lane].in_flight) return fail(UALM_ESTATE, "all lanes of this depth are in flight: ualm_wait_batch the oldest ticket first");
     const int keep = c->cur;
@@ -1065,7 +1149,7 @@ extern "C" int ualm_eval_batch(ualm_ctx_t *c, const double *x, const double *lam
         if ((rc = per_env(c, [&](int e, const BatchPtrs &bp, int cnt) {
                  BatchPtrs be = bp;
                  if (x) be.x0 = l->d_xev.p;
-                 eval_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(be, c->envs[e].dp, c->envs[e].dm, l->eL[e], rho);
+                 eval_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(be, c->envs[e].dp, c->envs[e].map->dm, l->eL[e], rho);
              })))
             return rc;
         if (f) CK(cudaMemcpyAsync(f, l->d_f.p, sizeof(double) * l->B, cudaMemcpyDeviceToHost, l->stream));
@@ -1088,7 +1172,7 @@ extern "C" int ualm_init_scaling_batch(ualm_ctx_t *c, double *scale_fx, double *
     CK(cudaSetDevice(c->device));
     if (l->B > 0) {
         if (int rc = per_env(c, [&](int e, const BatchPtrs &bp, int cnt) {
-                scaling_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].dm, l->eL[e]);
+                scaling_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].map->dm, l->eL[e]);
             }))
             return rc;
         if (scale_fx) CK(cudaMemcpyAsync(scale_fx, l->d_sfx.p, sizeof(double) * l->B, cudaMemcpyDeviceToHost, l->stream));
@@ -1117,9 +1201,9 @@ extern "C" int ualm_time_penalty_kernel(ualm_ctx_t *c, int reps, float *ms_per_l
     if ((rc = put(c, l->d_scale_cx.p, nullptr, 7 * l->tot_s, 1.0))) return rc;
     const int e = l->env[0];
     const BatchPtrs bp = batch_ptrs(c);
-    penalty_only_kernel<<<(l->B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].dm, l->eL[e], 1); // warm-up
+    penalty_only_kernel<<<(l->B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].map->dm, l->eL[e], 1); // warm-up
     CK(cudaEventRecord(l->ev0, l->stream));
-    penalty_only_kernel<<<(l->B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].dm, l->eL[e], reps);
+    penalty_only_kernel<<<(l->B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].map->dm, l->eL[e], reps);
     CK(cudaEventRecord(l->ev1, l->stream));
     CK(cudaGetLastError());
     CK(cudaEventSynchronize(l->ev1));
@@ -1166,15 +1250,17 @@ __global__ void piece_T_from_results(const ualm_result_t *res, int B, double *pi
 }
 } // namespace ualm
 
-// feasibility_kernel over a batch whose problem b is in environment env[b]: one launch with that environment's parameters and grid
-// when there is only one, else one launch per environment over its problem indices
-static int feasibility_launch(ualm_ctx *c, const BatchPtrs &bp, int B, const int32_t *env, double dt, double *d_out, cudaStream_t st)
+// feasibility_kernel over a batch whose problem b is in environment env[b]: one launch with that environment's parameters and the grid
+// version maps[env[b]] the batch was solved on when there is only one environment, else one launch per environment over its problem indices
+static int feasibility_launch(ualm_ctx *c, const BatchPtrs &bp, int B, const int32_t *env, const MapRef *maps, double dt, double *d_out, cudaStream_t st)
 {
     bool mixed = false;
     for (int b = 1; b < B; b++) mixed = mixed || env[b] != env[0];
+    for (int b = 0; b < B; b++)
+        if (!maps[env[b]]) return fail(UALM_ESTATE, "ualm_feasibility_batch: the batch was not solved by a launch of this context");
     if (!mixed) {
-        const Env &v = c->envs[B > 0 ? env[0] : 0];
-        feasibility_kernel<<<(B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(bp, v.dp, v.dm, dt, d_out, nullptr, B);
+        const int e = B > 0 ? env[0] : 0;
+        feasibility_kernel<<<(B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(bp, c->envs[e].dp, maps[e]->dm, dt, d_out, nullptr, B);
         CK(cudaGetLastError());
         return UALM_OK;
     }
@@ -1191,7 +1277,7 @@ static int feasibility_launch(ualm_ctx *c, const BatchPtrs &bp, int B, const int
     for (int e = 0; e < UALM_MAX_ENVS; e++) {
         const int cnt = off[e + 1] - off[e];
         if (cnt == 0) continue;
-        feasibility_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(bp, c->envs[e].dp, c->envs[e].dm, dt, d_out, t.idx.p + off[e], cnt);
+        feasibility_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(bp, c->envs[e].dp, maps[e]->dm, dt, d_out, t.idx.p + off[e], cnt);
         CK(cudaGetLastError());
     }
     CK(cudaStreamSynchronize(st));       // idx and its device copy are local
@@ -1199,8 +1285,8 @@ static int feasibility_launch(ualm_ctx *c, const BatchPtrs &bp, int B, const int
 }
 
 // the scan over coefficients that already sit on the device (B problems, ragged offsets from N / M, piece durations from the records)
-static int feasibility_from_device(ualm_ctx *c, int B, const int32_t *N, const int32_t *M, const int32_t *env, const ualm_result_t *d_res, const double *d_cxy,
-                                   const double *d_cyaw, double dt, double *out10)
+static int feasibility_from_device(ualm_ctx *c, int B, const int32_t *N, const int32_t *M, const int32_t *env, const MapRef *maps, const ualm_result_t *d_res,
+                                   const double *d_cxy, const double *d_cyaw, double dt, double *out10)
 {
     struct Tmp { DevBuf<ProbDesc> desc; DevBuf<double> pt, feas; ~Tmp() { desc.release(); pt.release(); feas.release(); } } t;
     std::vector<ProbDesc> desc(B);
@@ -1217,7 +1303,7 @@ static int feasibility_from_device(ualm_ctx *c, int B, const int32_t *N, const i
     BatchPtrs bp;
     memset(&bp, 0, sizeof(bp));
     bp.B = B; bp.desc = t.desc.p; bp.c_xy = const_cast<double *>(d_cxy); bp.c_yaw = const_cast<double *>(d_cyaw); bp.piece_T = t.pt.p;
-    if (int rc = feasibility_launch(c, bp, B, env, dt, t.feas.p, 0)) return rc;
+    if (int rc = feasibility_launch(c, bp, B, env, maps, dt, t.feas.p, 0)) return rc;
     CK(cudaMemcpy(out10, t.feas.p, sizeof(double) * 10 * B, cudaMemcpyDeviceToHost));
     return UALM_OK;
 }
@@ -1232,13 +1318,13 @@ extern "C" int ualm_feasibility_batch(ualm_ctx_t *c, double dt, double *out10)
             return fail(UALM_ESTATE, "ualm_feasibility_batch needs a solved, collected batch (ualm_sync / ualm_download first)");
         CK(cudaSetDevice(c->device));
         if (B == 0) return UALM_OK;
-        return feasibility_from_device(c, B, N, M, E, d_res, d_cxy, d_cyaw, dt, out10);
+        return feasibility_from_device(c, B, N, M, E, c->lanes[c->cur].vref, d_res, d_cxy, d_cyaw, dt, out10);
     }
     Lane *l = c->b;
     if (!l->have_batch || !l->solved) return fail(UALM_ESTATE, "ualm_feasibility_batch needs a solved resident batch");
     CK(cudaSetDevice(c->device));
     if (l->B == 0) return UALM_OK;
-    if (int rc = feasibility_launch(c, batch_ptrs(c), l->B, l->env.data(), dt, l->d_feas.p, l->stream)) return rc;
+    if (int rc = feasibility_launch(c, batch_ptrs(c), l->B, l->env.data(), l->vref, dt, l->d_feas.p, l->stream)) return rc;
     CK(cudaMemcpyAsync(out10, l->d_feas.p, sizeof(double) * 10 * l->B, cudaMemcpyDeviceToHost, l->stream));
     CK(cudaStreamSynchronize(l->stream));
     return UALM_OK;
@@ -1325,34 +1411,93 @@ __global__ void __launch_bounds__(64) map_build_kernel(UalmMapPrep prep, ualm_ma
 }
 } // namespace ualm
 
+// map_build_kernel on stream st: UnevenMap::init's preprocessing of the cloud on the host, then the cells into the device buffer dst
+// (scratch allocated and freed on st).  cells_out (optional): the grid to the host; kernel_ms (optional): CUDA-event time of the kernel.
+// Returns once st has completed the work
+static int map_build_on(cudaStream_t st, const float *pin, int64_t npts, const ualm_map_geom_t *g, double ex, double ey, double ez,
+                        int iter_num, float4 *dst, float *cells_out, float *kernel_ms)
+{
+    UalmMapHostPrep prep;
+    ualm_map_preprocess(pin, npts, ex, ey, ez, prep);
+    UalmMapPrep view = prep.view(ex, ey, ez, iter_num);
+    const long long total = (long long)map_ncell(g);
+    // scratch and events are released on every exit path (CK returns on the first CUDA error)
+    struct Scratch {
+        cudaStream_t st;
+        float *pts = nullptr; int *start = nullptr;
+        cudaEvent_t e0 = nullptr, e1 = nullptr;
+        ~Scratch()
+        {
+            if (pts) cudaFreeAsync(pts, st);
+            if (start) cudaFreeAsync(start, st);
+            if (e0) cudaEventDestroy(e0);
+            if (e1) cudaEventDestroy(e1);
+        }
+    } sc{st};
+    CK(cudaMallocAsync(&sc.pts, sizeof(float) * std::max<size_t>(prep.pts.size(), 3), st));
+    CK(cudaMallocAsync(&sc.start, sizeof(int) * std::max<size_t>(prep.start.size(), 1), st));
+    CK(cudaEventCreate(&sc.e0)); CK(cudaEventCreate(&sc.e1));
+    if (!prep.pts.empty()) CK(cudaMemcpyAsync(sc.pts, prep.pts.data(), sizeof(float) * prep.pts.size(), cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(sc.start, prep.start.data(), sizeof(int) * prep.start.size(), cudaMemcpyHostToDevice, st));
+    view.pts = sc.pts; view.start = sc.start;
+    CK(cudaEventRecord(sc.e0, st));
+    map_build_kernel<<<(unsigned)((total + 63) / 64), 64, 0, st>>>(view, *g, dst);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(sc.e1, st));
+    if (cells_out) CK(cudaMemcpyAsync(cells_out, dst, sizeof(float4) * total, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (kernel_ms) CK(cudaEventElapsedTime(kernel_ms, sc.e0, sc.e1));
+    return UALM_OK;
+}
+
 extern "C" int ualm_map_build_device(ualm_ctx_t *c, const float *pin, int64_t npts, const ualm_map_geom_t *g, double ex, double ey, double ez,
                                      int iter_num, float *cells, float *kernel_ms)
 {
     if (!c || !pin || !g || !cells || npts < 0) return fail(UALM_EINVAL, "null argument");
     CK(cudaSetDevice(c->device));
-    UalmMapHostPrep prep;
-    ualm_map_preprocess(pin, npts, ex, ey, ez, prep);
-    UalmMapPrep view = prep.view(ex, ey, ez, iter_num);
-    const long long total = (long long)g->voxel_num[0] * g->voxel_num[1] * g->voxel_num[2];
-    // scratch buffers and events are released on every exit path (CK returns on the first CUDA error)
-    struct Scratch {
-        DevBuf<float> pts; DevBuf<int> start; DevBuf<float4> cells;
-        cudaEvent_t e0 = nullptr, e1 = nullptr;
-        ~Scratch() { pts.release(); start.release(); cells.release(); if (e0) cudaEventDestroy(e0); if (e1) cudaEventDestroy(e1); }
-    } sc;
-    CK(sc.pts.ensure(std::max<size_t>(prep.pts.size(), 3)));
-    CK(sc.start.ensure(prep.start.size()));
-    CK(sc.cells.ensure((size_t)total));
-    CK(cudaEventCreate(&sc.e0)); CK(cudaEventCreate(&sc.e1));
-    if (!prep.pts.empty()) CK(cudaMemcpyAsync(sc.pts.p, prep.pts.data(), sizeof(float) * prep.pts.size(), cudaMemcpyHostToDevice, c->b->stream));
-    CK(cudaMemcpyAsync(sc.start.p, prep.start.data(), sizeof(int) * prep.start.size(), cudaMemcpyHostToDevice, c->b->stream));
-    view.pts = sc.pts.p; view.start = sc.start.p;
-    CK(cudaEventRecord(sc.e0, c->b->stream));
-    map_build_kernel<<<(unsigned)((total + 63) / 64), 64, 0, c->b->stream>>>(view, *g, sc.cells.p);
-    CK(cudaGetLastError());
-    CK(cudaEventRecord(sc.e1, c->b->stream));
-    CK(cudaMemcpyAsync(cells, sc.cells.p, sizeof(float4) * total, cudaMemcpyDeviceToHost, c->b->stream));
-    CK(cudaStreamSynchronize(c->b->stream));
-    if (kernel_ms) CK(cudaEventElapsedTime(kernel_ms, sc.e0, sc.e1));
+    struct Scratch { DevBuf<float4> cells; ~Scratch() { cells.release(); } } sc;
+    CK(sc.cells.ensure(map_ncell(g)));
+    return map_build_on(c->b->stream, pin, npts, g, ex, ey, ez, iter_num, sc.cells.p, cells, kernel_ms);
+}
+
+// ---------------------------------------------------------------------------------------------
+// Grid updates while batches are in flight: a new version is filled (or built) on the map stream, which no solve occupies, and made
+// current once complete.  Work launched before keeps the version it was launched with (MapVer, lane_hold)
+// ---------------------------------------------------------------------------------------------
+static int map_geom_check(const ualm_map_geom_t *g)
+{
+    for (int k = 0; k < 3; k++)
+        if (g->voxel_num[k] <= 0) return fail(UALM_EINVAL, "voxel_num must be > 0 in every dimension");
+    return UALM_OK;
+}
+
+extern "C" int ualm_update_map(ualm_ctx_t *c, const ualm_map_geom_t *g, const float *cells)
+{
+    if (!c || !g || !cells) return fail(UALM_EINVAL, "null argument");
+    if (int rc = map_geom_check(g)) return rc;
+    CK(cudaSetDevice(c->device));
+    const size_t bytes = map_ncell(g) * sizeof(float4);
+    MapRef nv;
+    if (int rc = map_version_new(c, bytes, &nv)) return rc;
+    const cudaError_t e = cudaMemcpyAsync(nv->p, cells, bytes, cudaMemcpyHostToDevice, c->mstream);
+    const cudaError_t s = cudaStreamSynchronize(c->mstream);       // complete on return; also before a failed version is freed
+    if (e != cudaSuccess || s != cudaSuccess) return fail(UALM_ENOCUDA, std::string("ualm_update_map: ") + cudaGetErrorString(e != cudaSuccess ? e : s));
+    map_install(c, g, std::move(nv));
+    return UALM_OK;
+}
+
+extern "C" int ualm_update_map_from_cloud(ualm_ctx_t *c, const float *pts, int64_t npts, const ualm_map_geom_t *g, double ex, double ey, double ez,
+                                          int iter_num, float *cells_out, float *kernel_ms)
+{
+    if (!c || !pts || !g || npts < 0) return fail(UALM_EINVAL, "null argument or npts < 0");
+    if (int rc = map_geom_check(g)) return rc;
+    CK(cudaSetDevice(c->device));
+    MapRef nv;
+    if (int rc = map_version_new(c, map_ncell(g) * sizeof(float4), &nv)) return rc;
+    if (int rc = map_build_on(c->mstream, pts, npts, g, ex, ey, ez, iter_num, (float4 *)nv->p, cells_out, kernel_ms)) {
+        cudaStreamSynchronize(c->mstream);      // before the version is freed
+        return rc;
+    }
+    map_install(c, g, std::move(nv));
     return UALM_OK;
 }

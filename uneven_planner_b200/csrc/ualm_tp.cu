@@ -92,7 +92,7 @@ struct TpEngine {
     int genv[TP_NGROUPS] = {};
     int max_evals = 0;
     int use_tma = 0;              // map corners of kb_kernel: 0 = direct gather through L1 (default: measured faster), 1 = TMA-staged tiles (UALM_TP_TMA=1)
-    Buf<float4> cells[UALM_MAX_ENVS];
+    // (the grids themselves belong to the context, which keeps every version a batch in flight was admitted with: tp_bind_map)
     // pool
     TpPool E;
     int capacity = 0;
@@ -258,7 +258,6 @@ void tp_destroy(TpEngine *e)
         if (l.ev0) cudaEventDestroy(l.ev0);
         if (l.ev1) cudaEventDestroy(l.ev1);
     }
-    for (auto &b : e->cells) b.release();
     e->st.release(); e->active.release(); e->n_active.release(); e->remaining.release(); e->vec.release(); e->cd.release(); e->gw.release();
     e->kb_cost.release(); e->lm_ys.release(); e->lm_alpha.release(); e->cr.release(); e->gdc.release(); e->gdt.release(); e->dual.release();
     e->hs.release(); e->hy.release(); e->wway.release(); e->wf.release(); e->wt.release(); e->wf_off.release(); e->wway_off.release();
@@ -323,17 +322,10 @@ int tp_set_budget(TpEngine *e, int max_evals, std::string *err)
     return UALM_OK;
 }
 
-int tp_set_map(TpEngine *e, int env, const ualm_map_geom_t *g, const float *cells, std::string *err)
+void tp_bind_map(TpEngine *e, int env, const ualm_map_geom_t *g, const float4 *cells)
 {
-    if (any_in_flight(e)) { if (err) *err = "ualm_set_map while a batch is in flight"; return UALM_ESTATE; }
-    e->have_map[env] = false;     // until the grid below is complete
-    TCK(cudaSetDevice(e->device));
-    TCK(cudaStreamSynchronize(e->stream));
-    const size_t ncell = (size_t)g->voxel_num[0] * g->voxel_num[1] * g->voxel_num[2];
-    TCK(e->cells[env].ensure(ncell));
-    TCK(cudaMemcpy(e->cells[env].p, cells, ncell * sizeof(float4), cudaMemcpyHostToDevice));
     TpMap &m = e->map[env];
-    m.cells = e->cells[env].p;
+    m.cells = cells;
     for (int k = 0; k < 3; k++) { m.vn[k] = g->voxel_num[k]; m.origin[k] = g->origin[k]; m.maxb[k] = g->max_boundary[k]; }
     m.xy_res = g->xy_resolution; m.yaw_res = g->yaw_resolution; m.xy_inv = 1.0 / g->xy_resolution; m.yaw_inv = 1.0 / g->yaw_resolution;
     // TMA descriptor of the grid: a 3-D float tensor {4 * Yaw, Y, X} (innermost first), box = 8 yaw layers x 8 x 8 cells
@@ -348,7 +340,7 @@ int tp_set_map(TpEngine *e, int env, const ualm_map_geom_t *g, const float *cell
         const cuuint64_t strides[2] = {(cuuint64_t)16 * g->voxel_num[2], (cuuint64_t)16 * g->voxel_num[2] * g->voxel_num[1]};
         const cuuint32_t box[3] = {4 * TP_TILE, TP_TILE, TP_TILE};
         const cuuint32_t estr[3] = {1, 1, 1};
-        const CUresult r = ((EncodeFn)fn)(&e->tmap[env], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void *)e->cells[env].p, dims, strides, box, estr,
+        const CUresult r = ((EncodeFn)fn)(&e->tmap[env], CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, (void *)cells, dims, strides, box, estr,
                                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                                           CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
         e->have_tmap[env] = (r == CUDA_SUCCESS) && g->voxel_num[2] >= TP_TILE && g->voxel_num[1] >= TP_TILE && g->voxel_num[0] >= TP_TILE;
@@ -356,7 +348,13 @@ int tp_set_map(TpEngine *e, int env, const ualm_map_geom_t *g, const float *cell
     if (getenv("UALM_DEBUG"))
         fprintf(stderr, "[ualm-tp] env %d: tensor map %s, TMA staging %s\n", env, e->have_tmap[env] ? "encoded" : "unavailable", (e->have_tmap[env] && e->use_tma) ? "on" : "off");
     e->have_map[env] = true;
-    return UALM_OK;
+}
+
+unsigned tp_lane_env_mask(TpEngine *e, int lane)
+{
+    unsigned mask = 0;
+    for (int v : e->lanes[lane].env) mask |= 1u << v;
+    return mask;
 }
 
 // (re)allocate the pool for `cap` slots with the current parameters; only when nothing is resident
@@ -664,8 +662,10 @@ static int set_attrs(TpEngine *e, std::string *err)
 // The body runs at least once and repeats until the group has no trajectory left to run.  Rounds are per-trajectory lockstep steps,
 // and compaction and publication only change which slots are listed and when results are copied out, so the loop computes what
 // host-queued rounds compute.  Everything a kernel reads from the engine is fixed at capture: the grids by glive[g], which stays
-// until the lane is collected; the pool's shared-memory layout and sizes by the maxima live now, which cover this batch; parameters,
-// grids and budget cannot change while a batch is in flight.  pub_gd: the descriptors publish_kernel walks (null: no publication)
+// until the lane is collected; the pool's shared-memory layout and sizes by the maxima live now, which cover this batch; parameters
+// and budget cannot change while a batch is in flight; a map grid replaced meanwhile (ualm_update_map) changes e->map only for later
+// captures, and the context keeps the version captured here allocated until the lane is admitted again.  pub_gd: the descriptors
+// publish_kernel walks (null: no publication)
 template <class R>
 static int launch_loop(TpEngine *e, int g, bool with_ks, const GatherDesc *pub_gd, int *launches, std::string *err)
 {

@@ -15,7 +15,11 @@ int tp_create(TpEngine **e, int device, int precision, std::string *err);
 void tp_destroy(TpEngine *e);
 // parameters / grid of environment `env` (0 <= env < UALM_MAX_ENVS)
 int tp_set_params(TpEngine *e, int env, const ualm_params_t *p, std::string *err);
-int tp_set_map(TpEngine *e, int env, const ualm_map_geom_t *g, const float *cells, std::string *err);
+// the grid the batches admitted from now on read: a device buffer of the context ([X][Y][Yaw] float4), which stays allocated and
+// unchanged while a batch admitted with it is in flight (ualm_api.cu keeps every such version).  Also encodes its TMA descriptor
+void tp_bind_map(TpEngine *e, int env, const ualm_map_geom_t *g, const float4 *cells);
+// bit e set: the lane's uploaded batch has a problem in environment e
+unsigned tp_lane_env_mask(TpEngine *e, int lane);
 // lanes = tickets: a lane holds one uploaded batch; admit puts it into the pool of running trajectories and launches the round loop
 // of each of its groups on the device, collect waits for those loops to end and gathers the batch's results on the device.  env[B]: environment of every
 // problem (NULL = all 0), in range and bound (the caller checks)
