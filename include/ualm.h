@@ -141,6 +141,26 @@ int ualm_update_map(ualm_ctx_t *ctx, const ualm_map_geom_t *g, const float *cell
  * there the call can last into the tail of the batches in flight (DESIGN.md section 3h). */
 int ualm_update_map_from_cloud(ualm_ctx_t *ctx, const float *pts, int64_t npts, const ualm_map_geom_t *g, double ellipsoid_x,
                                double ellipsoid_y, double ellipsoid_z, int iter_num, float *cells_out, float *kernel_ms);
+/* Replace the cell columns [ix0, ix0+nx) x [iy0, iy0+ny), all yaw layers, of the selected environment's current grid, with the
+ * guarantees of ualm_update_map: work launched before keeps its grid bit for bit, every later launch reads the new one, which is
+ * complete on the device on return, and the call never waits for running batches.  Every cell outside the box is bit for bit the
+ * previous grid's; a window never changes the geometry.  The new grid is a copy of the current one (staged through 8 MB of pinned
+ * host memory, so only the copy engines serve it) with the box written over it: the call moves the grid twice over PCIe plus the
+ * box, and never needs a free SM.
+ * cells: nx*ny*W float4 {z, sigma, zb.x, zb.y}, in the grid's own [x][y][yaw] order restricted to the box.
+ * No grid bound in the selected environment, or a double grid of ualm_set_map_f64: UALM_ESTATE.  A null argument, nx or ny <= 0,
+ * or a box outside voxel_num: UALM_EINVAL.  On any error the previous grid stays current. */
+int ualm_update_map_window(ualm_ctx_t *ctx, int ix0, int iy0, int nx, int ny, const float *cells);
+/* The same box, built on the device from a point cloud, e.g. a local scan.  The preprocessing of ualm_map_build_device runs on this
+ * cloud only, and the geometry is that of the current grid; inside the box the cells are bit for bit those a full
+ * ualm_map_build_device of the same cloud with that geometry produces.  A cloud cut down to the box plus the ellipsoid's reach gives
+ * the full cloud's cells up to float rounding (its bin grid starts elsewhere, so sums run in another order: DESIGN.md section 3h).
+ * cells_out (optional, host) receives the box's cells in the layout above; kernel_ms (optional) is the CUDA-event time of the cell
+ * kernel.  A null pts or npts < 0 is UALM_EINVAL as well.  Like ualm_update_map_from_cloud, the kernel needs a free SM slot, which on
+ * the parity path can mean the tail of the batches in flight. */
+int ualm_update_map_window_from_cloud(ualm_ctx_t *ctx, const float *pts, int64_t npts, int ix0, int iy0, int nx, int ny,
+                                      double ellipsoid_x, double ellipsoid_y, double ellipsoid_z, int iter_num, float *cells_out,
+                                      float *kernel_ms);
 
 /* ---- batch solve = B independent optimizeSE2Traj calls ----
  * Ragged inputs are packed back to back in problem order: inner_xy has sum 2(N_b-1) doubles,

@@ -185,6 +185,20 @@ public:
         onEnv(env, [&] { return ualm_update_map_from_cloud(ctx_, pts, npts, &geom, ellipsoid_x, ellipsoid_y, ellipsoid_z, iter_num, cells_out, kernel_ms); },
               "ualm_update_map_from_cloud");
     }
+    // Replace the cell columns [ix0, ix0+nx) x [iy0, iy0+ny), all yaw layers, of environment `env`'s grid while batches are in flight
+    // (ualm_update_map_window), same guarantees as updateEnvironment; cells: nx*ny*Yaw float4 in the grid's [x][y][yaw] order
+    void updateEnvironmentWindow(int env, int ix0, int iy0, int nx, int ny, const float *cells_xyzw)
+    {
+        onEnv(env, [&] { return ualm_update_map_window(ctx_, ix0, iy0, nx, ny, cells_xyzw); }, "ualm_update_map_window");
+    }
+    // the same box built on the device from a point cloud, e.g. a local scan (npts x 3 floats); cells_out (optional) receives the box
+    void updateEnvironmentWindowFromCloud(int env, const float *pts, int64_t npts, int ix0, int iy0, int nx, int ny, double ellipsoid_x = 0.2,
+                                          double ellipsoid_y = 0.1, double ellipsoid_z = 0.1, int iter_num = 2, float *cells_out = nullptr,
+                                          float *kernel_ms = nullptr)
+    {
+        onEnv(env, [&] { return ualm_update_map_window_from_cloud(ctx_, pts, npts, ix0, iy0, nx, ny, ellipsoid_x, ellipsoid_y, ellipsoid_z, iter_num, cells_out, kernel_ms); },
+              "ualm_update_map_window_from_cloud");
+    }
 
     // ---- single problem, the reference's call (alm_traj_opt.h:92-98), plain pointers ----
     // initStateXY/endStateXY: 2x3 column-major; innerPtsXY: 2 x (N-1) column-major; initYaw/endYaw: 3; innerPtsYaw: M-1

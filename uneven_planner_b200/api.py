@@ -49,6 +49,7 @@ class BatchALMTrajOpt:
         self.params = None
         self.env_params = {}
         self.env = 0            # the selected environment (ualm_select_env)
+        self.geoms = {}         # the geometry of each environment's grid, as last bound
         self.pb = None
 
     def close(self):
@@ -97,6 +98,7 @@ class BatchALMTrajOpt:
             self.select_env(env)
         if self.env == 0:
             self.map = mapdata
+        self.geoms[self.env] = mapdata.geom
         c64 = getattr(mapdata, "cells64", None)
         if c64 is not None:
             _check(self.L.ualm_set_map_f64(self.h, C.byref(mapdata.geom), c64.ctypes.data_as(dp), 1 if repack_to_float else 0))
@@ -114,6 +116,7 @@ class BatchALMTrajOpt:
             self.map = mapdata
         cells = np.ascontiguousarray(mapdata.cells, np.float32)
         _check(self.L.ualm_update_map(self.h, C.byref(mapdata.geom), cells.ctypes.data_as(C.POINTER(C.c_float))))
+        self.geoms[self.env] = mapdata.geom
         return self
 
     def update_environment_from_cloud(self, pts, geom=None, ellipsoid=(0.2, 0.1, 0.1), iter_num=2, env=None, name="map"):
@@ -133,7 +136,36 @@ class BatchALMTrajOpt:
         m = maps.UnevenMapData(geom, cells, name)
         if self.env == 0:
             self.map = m
+        self.geoms[self.env] = geom
         return m, ms.value
+
+    def update_environment_window(self, ix0, iy0, cells, env=None):
+        """ualm_update_map_window: replaces the cell columns [ix0, ix0+nx) x [iy0, iy0+ny), all yaw layers, of environment `env`'s grid
+        (None: the selected one) with `cells` = (nx, ny, Yaw, 4) float32, with update_environment's guarantees.  The geometry stays
+        the current grid's (maps.window_box turns a metric rectangle into a box).  self.map is not spliced: the host grid is not
+        copied for a window."""
+        if env is not None:
+            self.select_env(env)
+        cells = np.ascontiguousarray(cells, np.float32)
+        geom = self.geoms.get(self.env)
+        if cells.ndim != 4 or cells.shape[3] != 4 or (geom is not None and cells.shape[2] != geom.voxel_num[2]):
+            raise ValueError("cells must be (nx, ny, Yaw, 4) with the grid's Yaw, got %r" % (cells.shape,))
+        _check(self.L.ualm_update_map_window(self.h, int(ix0), int(iy0), cells.shape[0], cells.shape[1], cells.ctypes.data_as(C.POINTER(C.c_float))))
+        return self
+
+    def update_environment_window_from_cloud(self, pts, ix0, iy0, nx, ny, ellipsoid=(0.2, 0.1, 0.1), iter_num=2, env=None):
+        """ualm_update_map_window_from_cloud: the same box built on the device from a point cloud (e.g. a local scan) with the
+        current grid's geometry.  Returns (the box's cells, (nx, ny, Yaw, 4) float32; kernel ms)."""
+        if env is not None:
+            self.select_env(env)
+        pts = np.ascontiguousarray(pts, dtype=np.float32).reshape(-1, 3)
+        fp = C.POINTER(C.c_float)
+        geom = self.geoms.get(self.env)           # None: no grid bound, which the call refuses
+        cells = np.zeros((max(int(nx), 0), max(int(ny), 0), geom.voxel_num[2] if geom else 0, 4), np.float32)
+        ms = C.c_float()
+        _check(self.L.ualm_update_map_window_from_cloud(self.h, pts.ctypes.data_as(fp), pts.shape[0], int(ix0), int(iy0), int(nx), int(ny), ellipsoid[0],
+                                                        ellipsoid[1], ellipsoid[2], iter_num, cells.ctypes.data_as(fp) if cells.size else None, C.byref(ms)))
+        return cells, ms.value
 
     def reset_stream(self):
         _check(self.L.ualm_reset_stream(self.h))

@@ -58,6 +58,7 @@ struct MapVer {
     void *p = nullptr;
     size_t bytes = 0;
     DevMap dm = {};
+    ualm_map_geom_t geom = {};           // the geometry dm was set from (the geometry of a ualm_update_map_window* copy)
     ~MapVer() { if (p) cudaFreeAsync(p, fs); }
 };
 typedef std::shared_ptr<MapVer> MapRef;
@@ -164,6 +165,9 @@ struct ualm_ctx {
     // freed grid shares no pool block with other buffers and goes back to the device at the next synchronisation
     cudaStream_t mstream = nullptr, fstream = nullptr;
     cudaMemPool_t mpool = nullptr;
+    // pinned staging of ualm_update_map_window*'s grid copy (map_copy_ce), allocated at the first window
+    static constexpr size_t STAGE_BYTES = 8u << 20;
+    void *h_stage = nullptr;
 };
 
 static int lane_make(ualm_ctx *c, Lane &l)
@@ -248,6 +252,7 @@ extern "C" int ualm_destroy(ualm_ctx_t *c)
     if (c->fstream) { cudaStreamSynchronize(c->fstream); cudaStreamDestroy(c->fstream); }     // the grids' frees
     if (c->mstream) cudaStreamDestroy(c->mstream);
     if (c->mpool) cudaMemPoolDestroy(c->mpool);
+    if (c->h_stage) cudaFreeHost(c->h_stage);
     if (c->join) cudaStreamDestroy(c->join);
     if (c->cancel) cudaStreamDestroy(c->cancel);
     if (c->evA) cudaEventDestroy(c->evA);
@@ -338,14 +343,18 @@ extern "C" int ualm_select_env(ualm_ctx_t *c, int env)
     return UALM_OK;
 }
 
-static void map_geometry_set(DevMap &m, const ualm_map_geom_t *g)
+static void map_geometry_set(MapVer &v, const ualm_map_geom_t *g)
 {
+    DevMap &m = v.dm;
+    v.geom = *g;
     for (int k = 0; k < 3; k++) { m.vn[k] = g->voxel_num[k]; m.origin[k] = g->origin[k]; m.maxb[k] = g->max_boundary[k]; }
     m.xy_res = g->xy_resolution; m.yaw_res = g->yaw_resolution;
     m.xy_inv = 1.0 / g->xy_resolution; m.yaw_inv = 1.0 / g->yaw_resolution; // uneven_map.cpp:104-105
 }
 
 static size_t map_ncell(const ualm_map_geom_t *g) { return (size_t)g->voxel_num[0] * g->voxel_num[1] * g->voxel_num[2]; }
+// the cell box {ix0, iy0, nx, ny} of the whole grid
+static int4 map_box_all(const ualm_map_geom_t *g) { return make_int4(0, 0, g->voxel_num[0], g->voxel_num[1]); }
 
 // a new grid version of `bytes` bytes, allocated on the map stream (usable once that stream is synchronised)
 static int map_version_new(ualm_ctx *c, size_t bytes, MapRef *out)
@@ -382,7 +391,7 @@ static int map_write_current(ualm_ctx *c, const ualm_map_geom_t *g, const void *
     DevMap &m = v.map->dm;
     m.cells = f64 ? nullptr : (const float4 *)v.map->p;
     m.cells64 = f64 ? (const double *)v.map->p : nullptr;
-    map_geometry_set(m, g);
+    map_geometry_set(*v.map, g);
     if (c->tp) ualm_tp::tp_bind_map(c->tp, c->sel_env, g, m.cells);
     v.have_map = true;
     return UALM_OK;
@@ -395,7 +404,7 @@ static void map_install(ualm_ctx *c, const ualm_map_geom_t *g, MapRef nv)
     Env &v = c->envs[c->sel_env];
     nv->dm.cells = (const float4 *)nv->p;
     nv->dm.cells64 = nullptr;
-    map_geometry_set(nv->dm, g);
+    map_geometry_set(*nv, g);
     if (c->tp) ualm_tp::tp_bind_map(c->tp, c->sel_env, g, nv->dm.cells);
     v.map = std::move(nv);
     v.have_map = true;
@@ -1395,32 +1404,35 @@ extern "C" int ualm_mpc_export_batch(ualm_ctx_t *c, double dt, const double *ini
 
 // ---------------------------------------------------------------------------------------------
 // UnevenMap construction on the device (SURVEY 8f-1).  HBM-bound gather: one thread per cell, yaw fastest so that the 64
-// threads of a CTA share (x, y) and read the same few cloud bins through L1.
+// threads of a CTA share (x, y) and read the same few cloud bins through L1.  A launch covers the cell columns
+// [box.x, box.x + box.z) x [box.y, box.y + box.w), all yaw layers, and writes them at their places in the whole grid `cells`:
+// blockIdx.y is the x row of the box, whose ny * Yaw cells are contiguous in the grid.  The thread's cell and address are plain
+// functions of its indices and the parameters, so neither holds a register across ualm_map_cell.
 // ---------------------------------------------------------------------------------------------
 namespace ualm {
-__global__ void __launch_bounds__(64) map_build_kernel(UalmMapPrep prep, ualm_map_geom_t geom, float4 *cells)
+__global__ void __launch_bounds__(64) map_build_kernel(UalmMapPrep prep, ualm_map_geom_t geom, int4 box, float4 *cells)
 {
     const int W = geom.voxel_num[2], Y = geom.voxel_num[1];
-    const long long cell = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const long long total = (long long)geom.voxel_num[0] * Y * W;
-    if (cell >= total) return;
-    const int w = (int)(cell % W), y = (int)((cell / W) % Y), x = (int)(cell / ((long long)W * Y));
+    const long long k = (long long)blockIdx.x * blockDim.x + threadIdx.x;      // cell k of the box's x row
+    if (k >= (long long)box.w * W) return;
+    const int w = (int)(k % W), y = box.y + (int)(k / W), x = box.x + (int)blockIdx.y;
     float o[4];
     ualm_map_cell(prep, geom, x, y, w, o);
-    cells[cell] = make_float4(o[0], o[1], o[2], o[3]);
+    cells[((long long)x * Y + box.y) * W + k] = make_float4(o[0], o[1], o[2], o[3]);
 }
 } // namespace ualm
 
-// map_build_kernel on stream st: UnevenMap::init's preprocessing of the cloud on the host, then the cells into the device buffer dst
-// (scratch allocated and freed on st).  cells_out (optional): the grid to the host; kernel_ms (optional): CUDA-event time of the kernel.
-// Returns once st has completed the work
-static int map_build_on(cudaStream_t st, const float *pin, int64_t npts, const ualm_map_geom_t *g, double ex, double ey, double ez,
+// map_build_kernel on stream st: UnevenMap::init's preprocessing of the cloud on the host, then the cells of the cell box `box`
+// ({ix0, iy0, nx, ny}, all yaw layers) into their places in the whole-grid device buffer dst; the rest of dst is not touched (scratch
+// allocated and freed on st).  cells_out (optional): the box's cells to the host, [nx][ny][yaw] float4; kernel_ms (optional):
+// CUDA-event time of the kernel.  Returns once st has completed the work
+static int map_build_on(cudaStream_t st, const float *pin, int64_t npts, const ualm_map_geom_t *g, int4 box, double ex, double ey, double ez,
                         int iter_num, float4 *dst, float *cells_out, float *kernel_ms)
 {
     UalmMapHostPrep prep;
     ualm_map_preprocess(pin, npts, ex, ey, ez, prep);
     UalmMapPrep view = prep.view(ex, ey, ez, iter_num);
-    const long long total = (long long)map_ncell(g);
+    const long long row = (long long)box.w * g->voxel_num[2];        // cells per x row of the box
     // scratch and events are released on every exit path (CK returns on the first CUDA error)
     struct Scratch {
         cudaStream_t st;
@@ -1441,10 +1453,17 @@ static int map_build_on(cudaStream_t st, const float *pin, int64_t npts, const u
     CK(cudaMemcpyAsync(sc.start, prep.start.data(), sizeof(int) * prep.start.size(), cudaMemcpyHostToDevice, st));
     view.pts = sc.pts; view.start = sc.start;
     CK(cudaEventRecord(sc.e0, st));
-    map_build_kernel<<<(unsigned)((total + 63) / 64), 64, 0, st>>>(view, *g, dst);
-    CK(cudaGetLastError());
+    for (int x0 = 0; x0 < box.z; x0 += 65535) {          // gridDim.y <= 65535 x rows per launch
+        const int4 part = make_int4(box.x + x0, box.y, std::min(65535, box.z - x0), box.w);
+        map_build_kernel<<<dim3((unsigned)((row + 63) / 64), (unsigned)part.z), 64, 0, st>>>(view, *g, part, dst);
+        CK(cudaGetLastError());
+    }
     CK(cudaEventRecord(sc.e1, st));
-    if (cells_out) CK(cudaMemcpyAsync(cells_out, dst, sizeof(float4) * total, cudaMemcpyDeviceToHost, st));
+    if (cells_out) {
+        const size_t col = sizeof(float4) * g->voxel_num[2], pitch = col * g->voxel_num[1];
+        CK(cudaMemcpy2DAsync(cells_out, col * box.w, (const char *)dst + pitch * box.x + col * box.y, pitch, col * box.w, box.z,
+                             cudaMemcpyDeviceToHost, st));
+    }
     CK(cudaStreamSynchronize(st));
     if (kernel_ms) CK(cudaEventElapsedTime(kernel_ms, sc.e0, sc.e1));
     return UALM_OK;
@@ -1457,7 +1476,7 @@ extern "C" int ualm_map_build_device(ualm_ctx_t *c, const float *pin, int64_t np
     CK(cudaSetDevice(c->device));
     struct Scratch { DevBuf<float4> cells; ~Scratch() { cells.release(); } } sc;
     CK(sc.cells.ensure(map_ncell(g)));
-    return map_build_on(c->b->stream, pin, npts, g, ex, ey, ez, iter_num, sc.cells.p, cells, kernel_ms);
+    return map_build_on(c->b->stream, pin, npts, g, map_box_all(g), ex, ey, ez, iter_num, sc.cells.p, cells, kernel_ms);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1494,10 +1513,77 @@ extern "C" int ualm_update_map_from_cloud(ualm_ctx_t *c, const float *pts, int64
     CK(cudaSetDevice(c->device));
     MapRef nv;
     if (int rc = map_version_new(c, map_ncell(g) * sizeof(float4), &nv)) return rc;
-    if (int rc = map_build_on(c->mstream, pts, npts, g, ex, ey, ez, iter_num, (float4 *)nv->p, cells_out, kernel_ms)) {
+    if (int rc = map_build_on(c->mstream, pts, npts, g, map_box_all(g), ex, ey, ez, iter_num, (float4 *)nv->p, cells_out, kernel_ms)) {
         cudaStreamSynchronize(c->mstream);      // before the version is freed
         return rc;
     }
     map_install(c, g, std::move(nv));
     return UALM_OK;
+}
+
+// dst <- src (device, `bytes`) on the map stream through the copy engines only: chunks go to the pinned staging buffer and back.  A
+// device-to-device cudaMemcpyAsync runs as a copy kernel, which on the parity path waits for the solve's SMs like any kernel (the
+// driver ignored cudaMemcpyBatchAsync's cudaMemcpyFlagPreferOverlapWithCompute hint there: DESIGN.md section 3h).  The staging
+// buffer is allocated once per context (cudaFreeHost would synchronise the device) and reused in stream order
+static cudaError_t map_copy_ce(ualm_ctx *c, void *dst, const void *src, size_t bytes)
+{
+    if (!c->h_stage) {
+        const cudaError_t e = cudaHostAlloc(&c->h_stage, ualm_ctx::STAGE_BYTES, cudaHostAllocDefault);
+        if (e != cudaSuccess) { c->h_stage = nullptr; return e; }
+    }
+    for (size_t o = 0; o < bytes; o += ualm_ctx::STAGE_BYTES) {
+        const size_t n = std::min(ualm_ctx::STAGE_BYTES, bytes - o);
+        cudaError_t e = cudaMemcpyAsync(c->h_stage, (const char *)src + o, n, cudaMemcpyDeviceToHost, c->mstream);
+        if (e == cudaSuccess) e = cudaMemcpyAsync((char *)dst + o, c->h_stage, n, cudaMemcpyHostToDevice, c->mstream);
+        if (e != cudaSuccess) return e;
+    }
+    return cudaSuccess;
+}
+
+// ualm_update_map_window*: a new version that starts as a copy (map_copy_ce) of the selected environment's current one, with the
+// cell box {ix0, iy0, nx, ny} (all yaw layers) written over it by write(geometry, new cells) on the map stream, made current once
+// complete.  The geometry stays the current version's
+template <class F>
+static int map_window_update(ualm_ctx *c, int ix0, int iy0, int nx, int ny, const char *what, F write)
+{
+    if (nx <= 0 || ny <= 0) return fail(UALM_EINVAL, std::string(what) + ": nx and ny must be > 0");
+    const Env &v = c->envs[c->sel_env];
+    if (!v.have_map || !v.map) return fail(UALM_ESTATE, std::string(what) + ": the selected environment has no map grid bound");
+    if (!v.map->dm.cells) return fail(UALM_ESTATE, std::string(what) + ": the selected environment holds a double grid (ualm_set_map_f64); a window needs the float grid");
+    const MapRef cur = v.map;          // held until the copy below is complete
+    const ualm_map_geom_t g = cur->geom;
+    if (ix0 < 0 || iy0 < 0 || (long long)ix0 + nx > g.voxel_num[0] || (long long)iy0 + ny > g.voxel_num[1])
+        return fail(UALM_EINVAL, std::string(what) + ": the box is outside the grid's voxel_num");
+    CK(cudaSetDevice(c->device));
+    const size_t bytes = map_ncell(&g) * sizeof(float4);
+    MapRef nv;
+    if (int rc = map_version_new(c, bytes, &nv)) return rc;
+    const cudaError_t e = map_copy_ce(c, nv->p, cur->p, bytes);
+    const int rc = e != cudaSuccess ? fail(UALM_ENOCUDA, std::string(what) + ": " + cudaGetErrorString(e)) : write(g, (float4 *)nv->p);
+    const cudaError_t s = cudaStreamSynchronize(c->mstream);       // complete on return; also before a failed version is freed
+    if (rc) return rc;
+    if (s != cudaSuccess) return fail(UALM_ENOCUDA, std::string(what) + ": " + cudaGetErrorString(s));
+    map_install(c, &g, std::move(nv));
+    return UALM_OK;
+}
+
+extern "C" int ualm_update_map_window(ualm_ctx_t *c, int ix0, int iy0, int nx, int ny, const float *cells)
+{
+    if (!c || !cells) return fail(UALM_EINVAL, "null argument");
+    // one strided host-to-device copy: x row k of the box is ny*W float4, contiguous in the host array and one grid row apart in the
+    // new version.  Copy engines only, so it needs no free SM
+    return map_window_update(c, ix0, iy0, nx, ny, "ualm_update_map_window", [&](const ualm_map_geom_t &g, float4 *dst) {
+        const size_t col = sizeof(float4) * g.voxel_num[2], pitch = col * g.voxel_num[1];
+        CK(cudaMemcpy2DAsync((char *)dst + pitch * ix0 + col * iy0, pitch, cells, col * ny, col * ny, nx, cudaMemcpyHostToDevice, c->mstream));
+        return UALM_OK;
+    });
+}
+
+extern "C" int ualm_update_map_window_from_cloud(ualm_ctx_t *c, const float *pts, int64_t npts, int ix0, int iy0, int nx, int ny, double ex, double ey,
+                                                 double ez, int iter_num, float *cells_out, float *kernel_ms)
+{
+    if (!c || !pts || npts < 0) return fail(UALM_EINVAL, "null argument or npts < 0");
+    return map_window_update(c, ix0, iy0, nx, ny, "ualm_update_map_window_from_cloud", [&](const ualm_map_geom_t &g, float4 *dst) {
+        return map_build_on(c->mstream, pts, npts, &g, make_int4(ix0, iy0, nx, ny), ex, ey, ez, iter_num, dst, cells_out, kernel_ms);
+    });
 }

@@ -111,6 +111,21 @@ def build_from_cloud(pts, geom=None, ellipsoid=(0.2, 0.1, 0.1), iter_num=2, nthr
     return UnevenMapData(geom, cells, name)
 
 
+def window_box(geom, x0, y0, x1, y1):
+    """The cell box (ix0, iy0, nx, ny) of grid `geom` whose cell columns the metric rectangle [x0, x1] x [y0, y1] touches, clipped
+    to the grid (cell index = floor((x - origin) / xy_resolution), as UnevenMap::posToIndex), for ualm_update_map_window*.
+    Raises ValueError when the rectangle misses the grid."""
+    X, Y, _ = geom.voxel_num
+    inv = 1.0 / geom.xy_resolution
+    ix0 = max(0, math.floor((min(x0, x1) - geom.origin[0]) * inv))
+    iy0 = max(0, math.floor((min(y0, y1) - geom.origin[1]) * inv))
+    ix1 = min(X - 1, math.floor((max(x0, x1) - geom.origin[0]) * inv))
+    iy1 = min(Y - 1, math.floor((max(y0, y1) - geom.origin[1]) * inv))
+    if ix1 < ix0 or iy1 < iy0:
+        raise ValueError("the rectangle [%g, %g] x [%g, %g] is outside the grid" % (x0, x1, y0, y1))
+    return ix0, iy0, ix1 - ix0 + 1, iy1 - iy0 + 1
+
+
 def terrain_path(name):
     return os.path.join(BUILT_DIR, f"{name}.umap")
 
