@@ -293,6 +293,35 @@ int ualm_profile(ualm_ctx_t *ctx, int enable, long long *out16);
  * diverged solve) is not scanned: zeros and a sample count of -1. */
 int ualm_feasibility_batch(ualm_ctx_t *ctx, double dt, double *out10);
 
+/* Limits of ualm_check_trajectories' six tests, as in ualm_params_t. */
+typedef struct { double max_vel, max_acc_lon, max_acc_lat, max_kap, min_cxi, max_sig; } ualm_limits_t;
+/* The scan of ualm_feasibility_batch over B trajectories the caller holds, e.g. those ualm_wait_batch / ualm_poll_batch returned,
+ * against each problem's environment's grid as it is at the call (float or double; the version after every ualm_update_map* that
+ * returned before).  Read-only: no solve, record or lane is touched, and it may be called while batches are in flight.
+ * Inputs (host) in the layouts ualm_wait_batch returns: N[B], M[B], piece_T[2B] = {piece_T_xy, piece_T_yaw} of each record, packed
+ * c_xy (12 N_b each) and c_yaw (6 M_b each); env[B] (NULL = all 0); t_from[B] (NULL = all 0).
+ * Samples: the reference's t = 0, dt, 2dt.. formed by repeated addition, as ualm_feasibility_batch forms them; problem b keeps those
+ * with t >= t_from[b] and t < its duration (the sequence is not restarted at t_from, so every kept sample is bit for bit the full
+ * scan's).  out16[16 * b + ...]:
+ *   0..9   ualm_feasibility_batch's ten values over the kept samples (signed abs-max of vx, ax, ay, cur, max att, max sig, the
+ *          non-holonomic error summed in sample order, the number of kept samples, T_xy, T_yaw);
+ *   10..15 the time of the first kept sample with |vx| > max_vel, |ax| > max_acc_lon, |ay| > max_acc_lat, |cur| > max_kap,
+ *          att > -min_cxi (cos xi < min_cxi), sig > max_sig; -1 where none does.
+ * The limits and gravity are each problem's environment's (ualm_set_params) unless `limits` (non-NULL) sets the six limits for the
+ * whole call: a solve meets its constraints only at its int_K + 1 samples per piece, within epsilon_con, so a dense scan finds small
+ * excursions and a caller sets its own margin here.  With t_from = 0, columns 0..9 equal ualm_feasibility_batch's on the same grid.
+ * Not scanned (a sample count of -1, every time -1): a problem over the compiled limits (N > UALM_NMAX or M > UALM_MMAX; the rest of
+ * the row 0) and one that would need more than 4e6 samples (0..6 zero, T_xy and T_yaw kept).  A t_from at or past the end keeps no
+ * sample: the initial maxima (0, att -1, sig 0), a count of 0 and no violation.
+ * A null ctx or pointer, B < 0, dt <= 0 (or NaN), N or M < 1, a negative or NaN t_from or an env outside [0, UALM_MAX_ENVS) is
+ * UALM_EINVAL; an environment used without both parameters and a grid bound is UALM_ESTATE; out16 is not written on either.
+ * The kernels run on a stream of the context that no solve occupies, created at the greatest priority; the call synchronises that
+ * stream only.  On the throughput path a check gets SM slots between a batch's rounds; on the parity path the solve holds every SM
+ * until its work queue runs dry, so there a check made in flight runs in the tail of the batches (DESIGN.md section 3i). */
+int ualm_check_trajectories(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *piece_T, const double *c_xy,
+                            const double *c_yaw, const int32_t *env, const double *t_from, double dt, const ualm_limits_t *limits,
+                            double *out16);
+
 /* Hand-over to the MPC for the solved batch of the selected lane, on the device (SURVEY 8f-3):
  *   (1) the mpc_controller/SE2Traj message PlanManager publishes (plan_manager.cpp:151-185, msg/SE2Traj.msg:1-9): pos_pts = the
  *       start point of every xy piece and the end point, (N + 1) x {x, y} per problem, posT_pts = the N piece durations,

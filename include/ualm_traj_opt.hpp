@@ -288,6 +288,16 @@ public:
         check(ualm_mpc_export_batch(ctx_, dt, init_v, init_a, pos_pts, posT_pts, angle_pts, angleT_pts, c_mpc_xy, c_mpc_yaw, dev4), "ualm_mpc_export_batch");
     }
 
+    // The post-solve scan of B trajectories the caller holds (e.g. from waitBatch: piece_T = {piece_T_xy, piece_T_yaw} per record)
+    // against each environment's grid as it is now, over the samples t >= t_from[b] of the full scan, with the time of the first
+    // violation of each limit (ualm_check_trajectories).  env / t_from / limits may be null (all 0 / all 0 / each environment's own).
+    // out16: 16 doubles per trajectory.  May be called while batches are in flight
+    void checkTrajectories(int B, const int32_t *N, const int32_t *M, const double *piece_T, const double *c_xy, const double *c_yaw, const int32_t *env,
+                           const double *t_from, double dt, const ualm_limits_t *limits, double *out16)
+    {
+        check(ualm_check_trajectories(ctx_, B, N, M, piece_T, c_xy, c_yaw, env, t_from, dt, limits, out16), "ualm_check_trajectories");
+    }
+
     // The reference's whole chain for B (start, goal) pairs: KinoAstar::plan + PlanManager's resampler on host threads
     // (ualm_front_end_batch), then the batched optimizer.  packed[b] = index of pair b in the outputs or -1 (no path / over the
     // optimizer's limits); results / c_xy / c_yaw hold the packed problems back to back like optimizeBatch.  Returns their number.

@@ -39,6 +39,10 @@ class AstarMap(C.Structure):
                 ("occ2", C.POINTER(C.c_uint8))]
 
 
+class Limits(C.Structure):
+    _fields_ = [(n, C.c_double) for n in ("max_vel", "max_acc_lon", "max_acc_lat", "max_kap", "min_cxi", "max_sig")]
+
+
 class ResampleParams(C.Structure):
     _fields_ = [(n, C.c_double) for n in ("piece_len", "yaw_piece_times", "mean_vel", "init_time_times", "init_sig_vel")]
 
@@ -136,11 +140,12 @@ def lib():
         L.ualm_update_map_window.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, fp]
         L.ualm_update_map_window_from_cloud.argtypes = [vp, fp, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, fp,
                                                         C.POINTER(C.c_float)]
+        L.ualm_check_trajectories.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, ip, dp, C.c_double, C.POINTER(Limits), dp]
         for name in ("ualm_reset_stream", "ualm_set_map_f64", "ualm_max_lanes", "ualm_select_lane", "ualm_submit_batch", "ualm_wait_batch",
                      "ualm_wait_batch_for", "ualm_poll_batch", "ualm_cancel_problems", "ualm_set_budget",
                      "ualm_mark_begin", "ualm_mark_end", "ualm_solve_batch_multi", "ualm_pack_records_device_async", "ualm_select_env",
                      "ualm_upload_env", "ualm_solve_batch_env", "ualm_submit_batch_env", "ualm_solve_batch_multi_env", "ualm_update_map",
-                     "ualm_update_map_from_cloud", "ualm_update_map_window", "ualm_update_map_window_from_cloud"):
+                     "ualm_update_map_from_cloud", "ualm_update_map_window", "ualm_update_map_window_from_cloud", "ualm_check_trajectories"):
             getattr(L, name).restype = C.c_int
         for name in ("ualm_create", "ualm_destroy", "ualm_set_params", "ualm_set_map", "ualm_solve_batch",
                      "ualm_upload", "ualm_solve_resident", "ualm_sync", "ualm_download", "ualm_last_solve_ms",

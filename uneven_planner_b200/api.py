@@ -368,6 +368,46 @@ class BatchALMTrajOpt:
         _check(self.L.ualm_feasibility_batch(self.h, float(dt), out.ctypes.data_as(C.POINTER(C.c_double))))
         return out
 
+    def check_trajectories(self, N, M, piece_T, c_xy, c_yaw, env=None, t_from=None, dt=0.01, limits=None):
+        """ualm_check_trajectories: the post-solve scan of trajectories the caller holds, against each environment's grid as it is now,
+        over the samples t >= t_from of the full scan, with the time each limit is first broken.  N, M: [B]; piece_T: [B, 2]
+        (piece_T_xy, piece_T_yaw of the records); c_xy / c_yaw packed as wait() returns them; env: [B] or None (all 0); t_from: [B],
+        one number or None (0); limits: None (each environment's own), six numbers (max_vel, max_acc_lon, max_acc_lat, max_kap,
+        min_cxi, max_sig) or an object with those attributes, e.g. Params.  May be called while batches are in flight.
+        Returns [B, 16]: ualm_feasibility_batch's ten columns over the kept samples, then the six first-violation times (-1: none)."""
+        N = np.ascontiguousarray(N, np.int32).reshape(-1)
+        M = np.ascontiguousarray(M, np.int32).reshape(-1)
+        B = N.size
+        pt = np.ascontiguousarray(piece_T, np.float64).reshape(-1)
+        cxy = np.ascontiguousarray(c_xy, np.float64).reshape(-1)
+        cyaw = np.ascontiguousarray(c_yaw, np.float64).reshape(-1)
+        for a, n, name in ((M, B, "M"), (pt, 2 * B, "piece_T"), (cxy, 12 * int(N.astype(np.int64).sum()), "c_xy"),
+                           (cyaw, 6 * int(M.astype(np.int64).sum()), "c_yaw")):
+            if a.size != n:
+                raise ValueError("check_trajectories: %s has %d entries, the piece counts need %d" % (name, a.size, n))
+        e = None if env is None else np.ascontiguousarray(env, np.int32).reshape(-1)
+        tf = None if t_from is None else np.ascontiguousarray(np.broadcast_to(np.asarray(t_from, np.float64), (B,)))
+        if e is not None and e.size != B:
+            raise ValueError("check_trajectories: env must have B = %d entries" % B)
+        lim = None
+        if limits is not None:
+            names = [n for n, _ in _lib.Limits._fields_]
+            vals = [getattr(limits, n) for n in names] if hasattr(limits, "max_vel") else list(limits)
+            if len(vals) != 6:
+                raise ValueError("check_trajectories: limits must be six numbers %s" % (names,))
+            lim = _lib.Limits(*[float(v) for v in vals])
+        out = np.zeros((B, 16))
+        _check(self.L.ualm_check_trajectories(self.h, B, _p(N, ip), _p(M, ip), _p(pt), _p(cxy), _p(cyaw), _p(e, ip), _p(tf), float(dt),
+                                              None if lim is None else C.byref(lim), _p(out)))
+        return out
+
+    def check_results(self, pb, out, t_from=None, dt=0.01, limits=None):
+        """check_trajectories of batch `pb` as wait() / poll() returned it: out = (results, c_xy, c_yaw).  A record poll() has not
+        filled yet has zero durations and keeps no sample."""
+        res, cxy, cyaw = out
+        pt = np.array([(r.piece_T_xy, r.piece_T_yaw) for r in res], np.float64).reshape(pb.B, 2)
+        return self.check_trajectories(pb.N, pb.M, pt, cxy, cyaw, env=_env(pb), t_from=t_from, dt=dt, limits=limits)
+
     def build_map(self, pts, geom=None, ellipsoid=(0.2, 0.1, 0.1), iter_num=2, name="map"):
         """UnevenMap grid from a point cloud on the GPU (ualm_map_build_device): (UnevenMapData, kernel ms)."""
         from . import maps

@@ -168,6 +168,16 @@ struct ualm_ctx {
     // pinned staging of ualm_update_map_window*'s grid copy (map_copy_ce), allocated at the first window
     static constexpr size_t STAGE_BYTES = 8u << 20;
     void *h_stage = nullptr;
+    // ualm_check_trajectories: a stream no solve occupies, at the greatest priority, so its CTAs go ahead of queued lane launches when
+    // SM slots free up; cdone marks the end of a check's kernels, which the free stream waits for before the grids it read can go.
+    // Both are made at the first check, not at creation: streams share the device's hardware queues in creation order, and with one
+    // more stream made before the throughput engine's, its cancels right after a submit came too late (tests/test_gpu_cancel.py)
+    cudaStream_t cstream = nullptr;
+    cudaEvent_t cdone = nullptr;
+    // its inputs and outputs: one grow-only block, allocated and replaced in stream order on cstream (a block freed at every call would
+    // go back to the device at that call's synchronisation and be mapped again at the next)
+    void *cbuf = nullptr;
+    size_t cbuf_bytes = 0;
 };
 
 static int lane_make(ualm_ctx *c, Lane &l)
@@ -253,6 +263,9 @@ extern "C" int ualm_destroy(ualm_ctx_t *c)
     if (c->mstream) cudaStreamDestroy(c->mstream);
     if (c->mpool) cudaMemPoolDestroy(c->mpool);
     if (c->h_stage) cudaFreeHost(c->h_stage);
+    if (c->cbuf) { cudaFreeAsync(c->cbuf, c->cstream); cudaStreamSynchronize(c->cstream); }
+    if (c->cstream) cudaStreamDestroy(c->cstream);
+    if (c->cdone) cudaEventDestroy(c->cdone);
     if (c->join) cudaStreamDestroy(c->join);
     if (c->cancel) cudaStreamDestroy(c->cancel);
     if (c->evA) cudaEventDestroy(c->evA);
@@ -1336,6 +1349,90 @@ extern "C" int ualm_feasibility_batch(ualm_ctx_t *c, double dt, double *out10)
     if (int rc = feasibility_launch(c, batch_ptrs(c), l->B, l->env.data(), l->vref, dt, l->d_feas.p, l->stream)) return rc;
     CK(cudaMemcpyAsync(out10, l->d_feas.p, sizeof(double) * 10 * l->B, cudaMemcpyDeviceToHost, l->stream));
     CK(cudaStreamSynchronize(l->stream));
+    return UALM_OK;
+}
+
+// check_kernel over host trajectories, on the context's check stream, against each environment's grid version current at the call.
+// The context's block (cbuf) grows in stream order on that stream, and the versions are let go only after cdone (as lane_hold lets
+// go), so nothing here waits for a batch in flight
+extern "C" int ualm_check_trajectories(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *piece_T, const double *c_xy,
+                                       const double *c_yaw, const int32_t *env, const double *t_from, double dt, const ualm_limits_t *limits,
+                                       double *out16)
+{
+    if (!c || B < 0 || (B > 0 && (!N || !M || !piece_T || !c_xy || !c_yaw || !out16))) return fail(UALM_EINVAL, "ualm_check_trajectories: null argument or B < 0");
+    if (!(dt > 0.0)) return fail(UALM_EINVAL, "ualm_check_trajectories: dt must be > 0");
+    long long ncx = 0, ncy = 0;
+    for (int b = 0; b < B; b++) {
+        if (N[b] < 1 || M[b] < 1) return fail(UALM_EINVAL, "ualm_check_trajectories: piece counts must be >= 1");
+        if (t_from && !(t_from[b] >= 0.0)) return fail(UALM_EINVAL, "ualm_check_trajectories: t_from must be >= 0 (and not NaN)");
+        ncx += 12LL * N[b]; ncy += 6LL * M[b];
+    }
+    if (B == 0) return UALM_OK;
+    if (int rc = check_envs(c, B, env)) return rc;
+    CK(cudaSetDevice(c->device));
+    if (!c->cstream) {
+        int least = 0, greatest = 0;
+        CK(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+        CK(cudaStreamCreateWithPriority(&c->cstream, cudaStreamNonBlocking, greatest));
+    }
+    if (!c->cdone) CK(cudaEventCreateWithFlags(&c->cdone, cudaEventDisableTiming));
+    // problems grouped by environment, and the grid version each environment has now
+    std::vector<int> idx;
+    int off[UALM_MAX_ENVS + 1];
+    MapRef hold[UALM_MAX_ENVS];
+    for (int e = 0; e < UALM_MAX_ENVS; e++) {
+        off[e] = (int)idx.size();
+        for (int b = 0; b < B; b++) if ((env ? env[b] : 0) == e) idx.push_back(b);
+        if ((int)idx.size() > off[e]) hold[e] = c->envs[e].map;
+    }
+    off[UALM_MAX_ENVS] = B;
+    std::vector<ProbDesc> desc(B);
+    long long ocx = 0, ocy = 0;
+    for (int b = 0; b < B; b++) {
+        memset(&desc[b], 0, sizeof(ProbDesc));
+        desc[b].N = N[b]; desc[b].M = M[b]; desc[b].off_cxy = ocx; desc[b].off_cyaw = ocy;
+        desc[b].S = (N[b] > UALM_NMAX || M[b] > UALM_MMAX) ? 0 : 1;      // S == 0: over the compiled limits, not scanned
+        ocx += 12LL * N[b]; ocy += 6LL * M[b];
+    }
+    std::vector<double> tf;
+    if (!t_from) tf.assign(B, 0.0);
+    // the block: out 16B | piece_T 2B | t_from B | c_xy | c_yaw (doubles), then desc, then idx
+    const size_t nd = 16 * (size_t)B + 2 * (size_t)B + (size_t)B + (size_t)ncx + (size_t)ncy;
+    const size_t bytes = sizeof(double) * nd + sizeof(ProbDesc) * B + sizeof(int) * B;
+    const cudaStream_t st = c->cstream;
+    // declared after hold: on every exit cdone is recorded behind the kernels before the versions are let go
+    struct Done {
+        ualm_ctx *c;
+        ~Done() { if (cudaEventRecord(c->cdone, c->cstream) == cudaSuccess) cudaStreamWaitEvent(c->fstream, c->cdone, 0); }
+    } done{c};
+    if (c->cbuf_bytes < bytes) {       // the old block is freed behind the checks that used it
+        if (c->cbuf) CK(cudaFreeAsync(c->cbuf, st));
+        c->cbuf = nullptr; c->cbuf_bytes = 0;
+        CK(cudaMallocAsync(&c->cbuf, bytes, st));
+        c->cbuf_bytes = bytes;
+    }
+    double *d_out = (double *)c->cbuf, *d_pt = d_out + 16 * (size_t)B, *d_tf = d_pt + 2 * (size_t)B, *d_cxy = d_tf + B, *d_cyaw = d_cxy + ncx;
+    ProbDesc *d_desc = (ProbDesc *)(d_out + nd);
+    int *d_idx = (int *)(d_desc + B);
+    CK(cudaMemcpyAsync(d_pt, piece_T, sizeof(double) * 2 * B, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_tf, t_from ? t_from : tf.data(), sizeof(double) * B, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_cxy, c_xy, sizeof(double) * ncx, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_cyaw, c_yaw, sizeof(double) * ncy, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_desc, desc.data(), sizeof(ProbDesc) * B, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_idx, idx.data(), sizeof(int) * B, cudaMemcpyHostToDevice, st));
+    CheckPtrs a;
+    a.desc = d_desc; a.c_xy = d_cxy; a.c_yaw = d_cyaw; a.piece_T = d_pt; a.t_from = d_tf; a.out = d_out;
+    for (int e = 0; e < UALM_MAX_ENVS; e++) {
+        const int cnt = off[e + 1] - off[e];
+        if (cnt == 0) continue;
+        const ualm_params_t &hp = c->envs[e].hp;
+        const CheckLimits lim = limits ? CheckLimits{limits->max_vel, limits->max_acc_lon, limits->max_acc_lat, limits->max_kap, limits->min_cxi, limits->max_sig}
+                                       : CheckLimits{hp.max_vel, hp.max_acc_lon, hp.max_acc_lat, hp.max_kap, hp.min_cxi, hp.max_sig};
+        check_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(a, hold[e]->dm, c->envs[e].dp.gravity, lim, dt, d_idx + off[e], cnt);
+        CK(cudaGetLastError());
+    }
+    CK(cudaMemcpyAsync(out16, d_out, sizeof(double) * 16 * B, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
     return UALM_OK;
 }
 

@@ -2406,6 +2406,40 @@ struct AbsMax {   // "if (fabs(best) < fabs(v)) best = v" over samples in time o
         }
     }
 };
+// The values of one sample at time tm < the trajectory's duration: vx, ax, ay, cur, att and sig of getMaxVxAxAyCurAttSig and the
+// term getNonHolError sums.  feasibility_kernel and check_kernel both take their samples from here, so they compute the same bits
+struct FeasSample { R vx, ax, ay, cur, att, sig, term; };
+__device__ __forceinline__ FeasSample feas_sample(const DevMap &map, R gravity, const R *cxy, const R *cyaw, int N, int M, R Tx, R Ty, R tm)
+{
+    const int nx = 6 * N;
+    R tl = tm;
+    const int ip = locate_piece(N, Tx, tl);
+    R px, py, vxw, vyw, axw, ayw, yaw, dyaw, dd;
+    piece_eval(cxy + 6 * ip, tl, px, vxw, axw);
+    piece_eval(cxy + nx + 6 * ip, tl, py, vyw, ayw);
+    R ty = tm;
+    const int iy = locate_piece(M, Ty, ty);
+    piece_eval(cyaw + 6 * iy, ty, yaw, dyaw, dd);
+    R se2[3] = {px, py, yaw};
+    normSO2(se2[2]);                                  // getNormSE2Pos (se2traj.hpp:433-443)
+    R tv[7], tg[7][3];
+    map_get_all_with_grad(map, se2, tv, tg);          // values as getTerrainVariables (uneven_map.h:221-256)
+    const double2 sc = dev_sincos(yaw);
+    const R sy_ = sc.x, cy_ = sc.y;
+    const R vnorm = sqrt(vxw * vxw + vyw * vyw);
+    const R lon = axw * cy_ + ayw * sy_;
+    const R lat = -axw * sy_ + ayw * cy_;
+    FeasSample s;
+    s.vx = vnorm * tv[0];
+    s.ax = lon * tv[0] + gravity * tv[1];
+    s.ay = lat * tv[2] + gravity * tv[3];
+    const R wz = dyaw * tv[5];
+    s.cur = wz / sqrt(s.vx * s.vx + UALM_DELTA_SIGL);
+    s.att = -1.0 / tv[5];
+    s.sig = tv[6];
+    s.term = fabs(vxw * sy_ + vyw * (-cy_));
+    return s;
+}
 // idx: the n problems to scan (those of one environment, whose parameters and grid this launch carries), or null for 0 .. n - 1
 __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) feasibility_kernel(const __grid_constant__ BatchPtrs bp, const __grid_constant__ DevParams p,
         const __grid_constant__ DevMap map, R dt, R *out, const int *idx, int n)
@@ -2418,7 +2452,7 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) feasibility_kernel(co
         if (lane < 10) out[10 * (size_t)prob + lane] = 0.0;
         return;
     }
-    const int N = pd->N, M = pd->M, nx = 6 * N;
+    const int N = pd->N, M = pd->M;
     const R *cxy = bp.c_xy + pd->off_cxy, *cyaw = bp.c_yaw + pd->off_cyaw;
     const R Tx = bp.piece_T[2 * prob], Ty = bp.piece_T[2 * prob + 1];
     R tot_xy = 0.0, tot_yaw = 0.0;    // PolyTrajectory::getTotalDuration (se2traj.hpp:291-300), SE2: the smaller one (:415-418)
@@ -2447,34 +2481,12 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) feasibility_kernel(co
         const bool valid = tm < total;
         R term = 0.0;
         if (valid) {
-            R tl = tm;
-            const int ip = locate_piece(N, Tx, tl);
-            R px, py, vxw, vyw, axw, ayw, yaw, dyaw, dd;
-            piece_eval(cxy + 6 * ip, tl, px, vxw, axw);
-            piece_eval(cxy + nx + 6 * ip, tl, py, vyw, ayw);
-            R ty = tm;
-            const int iy = locate_piece(M, Ty, ty);
-            piece_eval(cyaw + 6 * iy, ty, yaw, dyaw, dd);
-            R se2[3] = {px, py, yaw};
-            normSO2(se2[2]);                                  // getNormSE2Pos (se2traj.hpp:433-443)
-            R tv[7], tg[7][3];
-            map_get_all_with_grad(map, se2, tv, tg);          // values as getTerrainVariables (uneven_map.h:221-256)
-            const double2 sc = dev_sincos(yaw);
-            const R sy_ = sc.x, cy_ = sc.y;
-            const R vnorm = sqrt(vxw * vxw + vyw * vyw);
-            const R lon = axw * cy_ + ayw * sy_;
-            const R lat = -axw * sy_ + ayw * cy_;
-            const R vx = vnorm * tv[0];
-            const R ax = lon * tv[0] + p.gravity * tv[1];
-            const R ay = lat * tv[2] + p.gravity * tv[3];
-            const R wz = dyaw * tv[5];
-            const R cur = wz / sqrt(vx * vx + UALM_DELTA_SIGL);
-            const R att = -1.0 / tv[5];
+            const FeasSample s = feas_sample(map, p.gravity, cxy, cyaw, N, M, Tx, Ty, tm);
             const int k = kbase + lane;
-            max_.see(ax, k); may.see(ay, k); mvx.see(vx, k); mcur.see(cur, k);
-            if (matt < att) matt = att;
-            if (msig < tv[6]) msig = tv[6];
-            term = fabs(vxw * sy_ + vyw * (-cy_));
+            max_.see(s.ax, k); may.see(s.ay, k); mvx.see(s.vx, k); mcur.see(s.cur, k);
+            if (matt < s.att) matt = s.att;
+            if (msig < s.sig) msig = s.sig;
+            term = s.term;
         }
         const int cnt = __popc(__ballot_sync(0xffffffffu, valid));   // the valid lanes are a prefix: t grows with the lane
         for (int l = 0; l < cnt; l++) err += __shfl_sync(0xffffffffu, term, l);
@@ -2492,6 +2504,91 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) feasibility_kernel(co
     if (lane == 0) {
         R *o = out + 10 * (size_t)prob;
         o[0] = mvx.val; o[1] = max_.val; o[2] = may.val; o[3] = mcur.val; o[4] = matt; o[5] = msig; o[6] = err; o[7] = (R)count; o[8] = Tx; o[9] = Ty;
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// The same scan of trajectories the caller holds (ualm_check_trajectories), restricted to the samples t >= t_from of the reference's
+// sequence t = 0, dt, 2dt.. (the sequence is not restarted at t_from, so every kept sample is bit for bit the full scan's), with the
+// time of the first kept sample that breaks each of six limits.  One warp per trajectory, one lane per sample; a first violation is
+// the earliest set lane of its ballot in the first chunk that has one.  Oracle: tests/check_oracle.cpp.
+// out[16 * problem + ...] = the ten values of feasibility_kernel over the kept samples, then the first-violation times of
+// |vx| > max_vel, |ax| > max_acc_lon, |ay| > max_acc_lat, |cur| > max_kap, att > -min_cxi, sig > max_sig (-1: none)
+// ---------------------------------------------------------------------------------------------
+struct CheckLimits { R max_vel, max_acc_lon, max_acc_lat, max_kap, min_cxi, max_sig; };
+struct CheckPtrs {
+    const ProbDesc *desc;          // N, M, off_cxy, off_cyaw; S == 0 marks a problem over the compiled limits
+    const R *c_xy, *c_yaw, *piece_T, *t_from;
+    R *out;
+};
+// idx: the n problems to check, those of one environment, whose grid, gravity and limits this launch carries
+__global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) check_kernel(const __grid_constant__ CheckPtrs a, const __grid_constant__ DevMap map, R gravity,
+        const __grid_constant__ CheckLimits lim, R dt, const int *idx, int n)
+{
+    const int lane = threadIdx.x & 31, w = blockIdx.x * UALM_WPB + (threadIdx.x >> 5);
+    if (w >= n) return;         // whole warp exits
+    const int prob = idx[w];
+    const ProbDesc *pd = a.desc + prob;
+    R *o = a.out + 16 * (size_t)prob;
+    const R Tx = a.piece_T[2 * prob], Ty = a.piece_T[2 * prob + 1];
+    const int N = pd->N, M = pd->M;
+    R tot_xy = 0.0, tot_yaw = 0.0;
+    for (int i = 0; i < N && pd->S; i++) tot_xy += Tx;
+    for (int i = 0; i < M && pd->S; i++) tot_yaw += Ty;
+    const R total = tot_xy < tot_yaw ? tot_xy : tot_yaw;
+    // over the compiled limits: zeros; more than 4e6 samples: zeros and the piece durations, as feasibility_kernel.  Both "not scanned"
+    if (pd->S == 0 || !(total / dt < 4.0e6)) {
+        if (lane < 16) o[lane] = lane == 7 || lane >= 10 ? -1.0 : pd->S && lane == 8 ? Tx : pd->S && lane == 9 ? Ty : 0.0;
+        return;
+    }
+    const R *cxy = a.c_xy + pd->off_cxy, *cyaw = a.c_yaw + pd->off_cyaw;
+    const R t0 = a.t_from[prob];
+    AbsMax mvx, max_, may, mcur;
+    mvx.init(); max_.init(); may.init(); mcur.init();
+    R matt = -1.0, msig = 0.0, err = 0.0;
+    R first[6] = {-1.0, -1.0, -1.0, -1.0, -1.0, -1.0};   // the same on every lane
+    unsigned found = 0;
+    long long count = 0;
+    R tbase = 0.0;
+    int kbase = 0;
+    while (true) {
+        R tm = 0.0, tt = tbase;
+        for (int i = 0; i < 32; i++) { if (i == lane) tm = tt; tt = tt + dt; }   // the reference's t += dt, same additions on every lane
+        const bool valid = tm < total, kept = valid && tm >= t0;
+        R term = 0.0;
+        unsigned viol = 0;
+        if (kept) {
+            const FeasSample s = feas_sample(map, gravity, cxy, cyaw, N, M, Tx, Ty, tm);
+            const int k = kbase + lane;
+            max_.see(s.ax, k); may.see(s.ay, k); mvx.see(s.vx, k); mcur.see(s.cur, k);
+            if (matt < s.att) matt = s.att;
+            if (msig < s.sig) msig = s.sig;
+            term = s.term;
+            viol = (fabs(s.vx) > lim.max_vel ? 1u : 0u) | (fabs(s.ax) > lim.max_acc_lon ? 2u : 0u) | (fabs(s.ay) > lim.max_acc_lat ? 4u : 0u) |
+                   (fabs(s.cur) > lim.max_kap ? 8u : 0u) | (s.att > -lim.min_cxi ? 16u : 0u) | (s.sig > lim.max_sig ? 32u : 0u);
+        }
+        const unsigned km = __ballot_sync(0xffffffffu, kept);   // the kept lanes are contiguous: t grows with the lane
+        for (unsigned m = km; m; m &= m - 1) err += __shfl_sync(0xffffffffu, term, __ffs(m) - 1);
+        count += __popc(km);
+#pragma unroll
+        for (int q = 0; q < 6; q++) {
+            const unsigned vm = __ballot_sync(0xffffffffu, (viol >> q) & 1u);
+            const R tv = __shfl_sync(0xffffffffu, tm, vm ? __ffs(vm) - 1 : 0);
+            if (vm && !((found >> q) & 1u)) { first[q] = tv; found |= 1u << q; }
+        }
+        if (__popc(__ballot_sync(0xffffffffu, valid)) < 32) break;
+        tbase = tt; kbase += 32;
+    }
+    mvx.reduce(); max_.reduce(); may.reduce(); mcur.reduce();
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) {
+        const R oa = __shfl_xor_sync(0xffffffffu, matt, off), os = __shfl_xor_sync(0xffffffffu, msig, off);
+        if (matt < oa) matt = oa;
+        if (msig < os) msig = os;
+    }
+    if (lane == 0) {
+        o[0] = mvx.val; o[1] = max_.val; o[2] = may.val; o[3] = mcur.val; o[4] = matt; o[5] = msig; o[6] = err; o[7] = (R)count; o[8] = Tx; o[9] = Ty;
+        for (int q = 0; q < 6; q++) o[10 + q] = first[q];
     }
 }
 
