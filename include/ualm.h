@@ -393,6 +393,43 @@ typedef struct {
 /* plan_manager/* parameters of the resampler (plan_manager.cpp:24-30; run_hill.yaml:57-62) */
 typedef struct { double piece_len, yaw_piece_times, mean_vel, init_time_times, init_sig_vel; } ualm_resample_params_t;
 
+/* Replanned problems of B trajectories the caller holds, from each robot's state at time t_from[b] on its trajectory to the goal of
+ * its original problem, submitted as one ticket.  Inputs (host) in the layouts ualm_wait_batch returns, as for ualm_check_trajectories:
+ * N[B], M[B], piece_T[2B] = {piece_T_xy, piece_T_yaw} of each record, packed c_xy (12 N_b each) and c_yaw (6 M_b each); bnd[18B], the
+ * original problems' boundary states; env[B] (NULL = all 0); t_from[B].  rp: the resampler's parameters (NULL = run_*.yaml's piece_len
+ * 0.3, yaw_piece_times 2, mean_vel 0.5, init_time_times 1.2; init_sig_vel is not used).  Row b is built as follows:
+ *   duration = min(N T_xy, M T_yaw), each summed by repeated addition as ualm_check_trajectories sums it;
+ *   the state at tau = t_from[b]: init_xy = [px, py, vx, vy, ax, ay], init_yaw = [yaw, dyaw, ddyaw] (yaw as the trajectory carries
+ *   it, not normalised), from the reference's piece lookup for uniform durations (se2traj.hpp:343-361);
+ *   the polyline: the point (x, y, yaw) at tau, the points at every t of the check's sequence t = 0, dt, 2dt.. (the same additions)
+ *   with tau < t < duration, then the goal (the position of bnd's end_xy, the angle of its end_yaw);
+ *   PlanManager's resampler on it, its steps in its order (yaw smoothing, pm.cpp:62-77; arc-length resampling and total_time,
+ *   pm.cpp:96-122, bit for bit ualm_resample_path's arithmetic): N', M', inner_xy, inner_yaw, total_time;
+ *   bnd' = [init_xy | bnd's end_xy | init_yaw | bnd's end_yaw] (a moving start state, within optimizeSE2Traj's 2 x 3 head state).
+ * The B problems are then submitted exactly as ualm_submit_batch_env submits the returned arrays with env, on the next lane of the
+ * `depth` ring: *ticket and row b of it = row b of the inputs, for ualm_poll_batch / ualm_cancel_problems / ualm_wait_batch(_for) and
+ * the budget as for any ticket.  Outputs: N_out[B], M_out[B], bnd_out[18B], total_time_out[B] and, optional, inner_xy_out /
+ * inner_yaw_out at a fixed stride of UALM_REPLAN_INNER_XY / UALM_REPLAN_INNER_YAW doubles per row, zeros past the row's points.
+ * A row over the compiled limits (N' > 64 or M' > 128) keeps its counts, zero inner points, and is submitted as ualm_submit_batch_env
+ * submits such a problem (a UALM_ELIMIT record from the first poll, zero coefficients).  The build's work per row is bounded: a
+ * polyline that would need more than 4095 waypoints of either kind, a yaw of magnitude 2^40 or more, or more than 65536 whole turns of
+ * yaw smoothing in all is cut short and reported as N' = M' = 4097, an over-limit row; its total_time is still its whole length's.
+ * The build is the same bits at every precision.
+ * A null ctx or pointer, B < 0, dt <= 0 (or NaN), depth outside [1, UALM_MAX_LANES], N or M < 1, a t_from that is negative, NaN or not
+ * before the row's duration, a duration / dt >= 4e6, a non-finite piece_T, c_xy or c_yaw entry (a diverged solve) or goal entry of bnd
+ * (6..11, 15..17), an rp field (but init_sig_vel) <= 0 or NaN, or an env out of range is UALM_EINVAL; an environment without
+ * parameters and a grid, or the next lane still in flight, is UALM_ESTATE.  These are decided before anything is built.  One refusal
+ * comes after the build: a row whose polyline has zero or non-finite length (a robot already at its goal; coordinates whose squares
+ * overflow) has no usable total_time and is UALM_EINVAL for the call.  On every refusal no output is written and no lane is taken.
+ * B = 0 is ualm_submit_batch_env with B = 0.  The build reads no grid; it runs on the stream of ualm_check_trajectories and synchronises that stream only, so in
+ * flight on the parity path it waits for SM slots in the batches' tail (DESIGN.md section 3j). */
+#define UALM_REPLAN_INNER_XY 126       /* 2 (64 - 1) */
+#define UALM_REPLAN_INNER_YAW 127      /* 128 - 1 */
+int ualm_submit_replan(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *piece_T, const double *c_xy,
+                       const double *c_yaw, const double *bnd, const int32_t *env, const double *t_from, double dt,
+                       const ualm_resample_params_t *rp, int depth, int *ticket, int32_t *N_out, int32_t *M_out, double *bnd_out,
+                       double *total_time_out, double *inner_xy_out, double *inner_yaw_out);
+
 /* KinoAstar::plan(start_state, end_state) (front_end/src/kino_astar.cpp:67-236): hybrid A* over (x, y, yaw) with 3 x 5 motion
  * primitives and a Dubins one-shot near the goal.  Writes the (x, y, yaw) polyline start .. goal and returns its number of points;
  * 0 = no path (start or goal occupied, open set exhausted, node pool exhausted), like the reference's empty vector.

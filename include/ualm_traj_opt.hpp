@@ -298,6 +298,20 @@ public:
         check(ualm_check_trajectories(ctx_, B, N, M, piece_T, c_xy, c_yaw, env, t_from, dt, limits, out16), "ualm_check_trajectories");
     }
 
+    // Replans B trajectories the caller holds (as for checkTrajectories, plus each one's original problem row bnd, 18 doubles) from the
+    // state at t_from[b] to the original goal, and submits the built problems as one ticket (ualm_submit_replan; wait on it with
+    // waitBatch).  rp may be null (run_*.yaml's resampler).  Outputs: the built N, M, bnd (18 per row), total_time and, optional,
+    // inner points at UALM_REPLAN_INNER_XY / UALM_REPLAN_INNER_YAW doubles per row.  Returns the ticket
+    int submitReplan(int B, const int32_t *N, const int32_t *M, const double *piece_T, const double *c_xy, const double *c_yaw, const double *bnd,
+                     const int32_t *env, const double *t_from, double dt, const ualm_resample_params_t *rp, int depth, int32_t *N_out, int32_t *M_out,
+                     double *bnd_out, double *total_time_out, double *inner_xy_out = nullptr, double *inner_yaw_out = nullptr)
+    {
+        int ticket = -1;
+        check(ualm_submit_replan(ctx_, B, N, M, piece_T, c_xy, c_yaw, bnd, env, t_from, dt, rp, depth, &ticket, N_out, M_out, bnd_out, total_time_out,
+                                 inner_xy_out, inner_yaw_out), "ualm_submit_replan");
+        return ticket;
+    }
+
     // The reference's whole chain for B (start, goal) pairs: KinoAstar::plan + PlanManager's resampler on host threads
     // (ualm_front_end_batch), then the batched optimizer.  packed[b] = index of pair b in the outputs or -1 (no path / over the
     // optimizer's limits); results / c_xy / c_yaw hold the packed problems back to back like optimizeBatch.  Returns their number.

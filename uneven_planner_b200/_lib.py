@@ -12,6 +12,7 @@ LIB_PATH = os.path.join(HERE, "libualm.so")
 
 UALM_OK, UALM_ENOCUDA, UALM_EINVAL, UALM_ESTATE, UALM_ELIMIT = 0, -1, -2, -3, -4
 UALM_RET_STOPPED = 3   # ret_code of a problem stopped by the evaluation budget, a deadline or a cancel (include/ualm.h)
+UALM_REPLAN_INNER_XY, UALM_REPLAN_INNER_YAW = 126, 127   # ualm_submit_replan's inner-point strides per row (include/ualm.h)
 UALM_MAX_ENVS = 4      # environments (parameter set + map grid) per context (include/ualm.h, ualm_select_env)
 
 
@@ -141,11 +142,14 @@ def lib():
         L.ualm_update_map_window_from_cloud.argtypes = [vp, fp, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, fp,
                                                         C.POINTER(C.c_float)]
         L.ualm_check_trajectories.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, ip, dp, C.c_double, C.POINTER(Limits), dp]
+        L.ualm_submit_replan.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, dp, ip, dp, C.c_double, C.POINTER(ResampleParams), C.c_int,
+                                         C.POINTER(C.c_int), ip, ip, dp, dp, dp, dp]
         for name in ("ualm_reset_stream", "ualm_set_map_f64", "ualm_max_lanes", "ualm_select_lane", "ualm_submit_batch", "ualm_wait_batch",
                      "ualm_wait_batch_for", "ualm_poll_batch", "ualm_cancel_problems", "ualm_set_budget",
                      "ualm_mark_begin", "ualm_mark_end", "ualm_solve_batch_multi", "ualm_pack_records_device_async", "ualm_select_env",
                      "ualm_upload_env", "ualm_solve_batch_env", "ualm_submit_batch_env", "ualm_solve_batch_multi_env", "ualm_update_map",
-                     "ualm_update_map_from_cloud", "ualm_update_map_window", "ualm_update_map_window_from_cloud", "ualm_check_trajectories"):
+                     "ualm_update_map_from_cloud", "ualm_update_map_window", "ualm_update_map_window_from_cloud", "ualm_check_trajectories",
+                     "ualm_submit_replan"):
             getattr(L, name).restype = C.c_int
         for name in ("ualm_create", "ualm_destroy", "ualm_set_params", "ualm_set_map", "ualm_solve_batch",
                      "ualm_upload", "ualm_solve_resident", "ualm_sync", "ualm_download", "ualm_last_solve_ms",

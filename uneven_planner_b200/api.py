@@ -408,6 +408,50 @@ class BatchALMTrajOpt:
         pt = np.array([(r.piece_T_xy, r.piece_T_yaw) for r in res], np.float64).reshape(pb.B, 2)
         return self.check_trajectories(pb.N, pb.M, pt, cxy, cyaw, env=_env(pb), t_from=t_from, dt=dt, limits=limits)
 
+    def submit_replan(self, pb, out, rows, t_from, dt=0.01, rparams=None, depth=2):
+        """ualm_submit_replan: replans rows `rows` of batch `pb` as wait() / poll() returned it (out = (results, c_xy, c_yaw)) from each
+        robot's state at time t_from (one number or one per row) on its trajectory to the row's original goal, with PlanManager's
+        resampler over the trajectory's samples t_from < t of the sequence t = 0, dt, 2dt.. (rparams: front_end.resample_params(), None
+        = its defaults), and submits the built problems as one ticket on the next lane of `depth`.  Returns (ticket, ProblemBatch of the
+        built problems, in the order of `rows`, with their environments); poll / wait / cancel / check_results work on it as on any."""
+        from . import problems
+        rows = np.asarray(rows)
+        if rows.ndim != 1 or (rows.size and not np.issubdtype(rows.dtype, np.integer)):
+            raise ValueError("submit_replan: rows must be a 1-D sequence of problem indices")
+        rows = rows.astype(np.int64)
+        if rows.size and (rows.min() < 0 or rows.max() >= pb.B):
+            raise ValueError("submit_replan: row index out of range [0, %d)" % pb.B)
+        res, cxy, cyaw = out
+        if len(res) != pb.B:
+            raise ValueError("submit_replan: out holds %d records, the batch has %d" % (len(res), pb.B))
+        B = rows.size
+        tf = np.ascontiguousarray(np.broadcast_to(np.asarray(t_from, np.float64), (B,)))
+        sub = pb.select(rows)
+        _, _, ocx, ocy = pb.offsets()
+        N, M = np.ascontiguousarray(sub.N, np.int32), np.ascontiguousarray(sub.M, np.int32)
+        pt = np.array([(res[i].piece_T_xy, res[i].piece_T_yaw) for i in rows], np.float64).reshape(B, 2)
+        c_xy = np.concatenate([cxy[ocx[i]:ocx[i + 1]] for i in rows]) if B else np.zeros(0)
+        c_yaw = np.concatenate([cyaw[ocy[i]:ocy[i + 1]] for i in rows]) if B else np.zeros(0)
+        bnd = np.ascontiguousarray(sub.bnd, np.float64).reshape(B, 18)
+        env = _env(sub)
+        rp = None if rparams is None else C.byref(rparams)
+        No, Mo = np.zeros(B, np.int32), np.zeros(B, np.int32)
+        bo, To = np.zeros((B, 18)), np.zeros(B)
+        ixy, iyaw = np.zeros((B, _lib.UALM_REPLAN_INNER_XY)), np.zeros((B, _lib.UALM_REPLAN_INNER_YAW))
+        t = C.c_int(-1)
+        _check(self.L.ualm_submit_replan(self.h, B, _p(N, ip), _p(M, ip), _p(pt), _p(c_xy), _p(c_yaw), _p(bnd), _p(env, ip), _p(tf), float(dt),
+                                         rp, int(depth), C.byref(t), _p(No, ip), _p(Mo, ip), _p(bo), _p(To), _p(ixy), _p(iyaw)))
+        # a row over the compiled limits (N 64, M 128): zeros, as the C call packs it
+        fits = lambda b: 2 * (No[b] - 1) <= _lib.UALM_REPLAN_INNER_XY and Mo[b] - 1 <= _lib.UALM_REPLAN_INNER_YAW
+        pxy = [ixy[b, :2 * (No[b] - 1)] if fits(b) else np.zeros(2 * (int(No[b]) - 1)) for b in range(B)]
+        pyaw = [iyaw[b, :Mo[b] - 1] if fits(b) else np.zeros(int(Mo[b]) - 1) for b in range(B)]
+        new = problems.ProblemBatch(No, Mo, bo, To, np.concatenate(pxy) if B else np.zeros(0), np.concatenate(pyaw) if B else np.zeros(0),
+                                    env=None if env is None else env.copy())
+        if not hasattr(self, "_tickets"):
+            self._tickets = {}
+        self._tickets[t.value] = (new, (None, env))
+        return t.value, new
+
     def build_map(self, pts, geom=None, ellipsoid=(0.2, 0.1, 0.1), iter_num=2, name="map"):
         """UnevenMap grid from a point cloud on the GPU (ualm_map_build_device): (UnevenMapData, kernel ms)."""
         from . import maps

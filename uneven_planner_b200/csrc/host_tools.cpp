@@ -12,6 +12,7 @@
 // Written from the behaviour of those files; shares no code with them.
 #include "ualm.h"
 #include "map_prep.h"
+#include "resample_stream.h"
 
 #include <algorithm>
 #include <atomic>
@@ -263,12 +264,8 @@ extern "C" int ualm_resample_path(const double *path_in, int npts, double piece_
 {
     if (!path_in || npts < 2 || !bnd || !inner_xy || !inner_yaw || !N || !M || !total_time) return UALM_EINVAL;
     std::vector<double> p(path_in, path_in + 3 * (size_t)npts);
-    // smooth yaw (pm.cpp:62-77)
-    for (int i = 0; i < npts - 1; i++) {
-        double dyaw = p[3 * (i + 1) + 2] - p[3 * i + 2];
-        while (dyaw >= M_PI / 2) { p[3 * (i + 1) + 2] -= M_PI * 2; dyaw = p[3 * (i + 1) + 2] - p[3 * i + 2]; }
-        while (dyaw <= -M_PI / 2) { p[3 * (i + 1) + 2] += M_PI * 2; dyaw = p[3 * (i + 1) + 2] - p[3 * i + 2]; }
-    }
+    // smooth yaw (pm.cpp:62-77); the steps of resample_stream.h, which replan_kernel takes one point at a time
+    for (int i = 0; i < npts - 1; i++) ualm_rs_smooth(p[3 * i + 2], p[3 * (i + 1) + 2]);
     // boundary states (pm.cpp:80-94): 2x3 column-major [p | v | a], yaw [psi,0,0]
     const double *f = &p[0], *l = &p[3 * (size_t)(npts - 1)];
     // sin / cos from ualm_detmath.h like every other trig call of the path (so the reference build of tests/test_ref_pin.py, whose
@@ -278,29 +275,12 @@ extern "C" int ualm_resample_path(const double *path_in, int npts, double piece_
     bnd[12] = f[2]; bnd[13] = 0; bnd[14] = 0;
     bnd[15] = l[2]; bnd[16] = 0; bnd[17] = 0;
     // arc-length resampling (pm.cpp:96-121)
-    double temp_len_yaw = 0.0, temp_len_pos = 0.0, total_len = 0.0;
-    const double piece_len_yaw = piece_len / yaw_piece_times;
-    int nxy = 0, nyaw = 0;
-    for (int k = 0; k < npts - 1; k++) {
-        const double *a = &p[3 * k], *b = &p[3 * (k + 1)];
-        const double temp_seg = std::sqrt((b[0] - a[0]) * (b[0] - a[0]) + (b[1] - a[1]) * (b[1] - a[1]));
-        temp_len_yaw += temp_seg; temp_len_pos += temp_seg; total_len += temp_seg;
-        while (temp_len_yaw > piece_len_yaw) {
-            if (nyaw >= max_inner_yaw) return UALM_ELIMIT;
-            inner_yaw[nyaw++] = a[2] + (1.0 - (temp_len_yaw - piece_len_yaw) / temp_seg) * (b[2] - a[2]);
-            temp_len_yaw -= piece_len_yaw;
-        }
-        while (temp_len_pos > piece_len) {
-            if (nxy >= max_inner_xy) return UALM_ELIMIT;
-            const double w = (1.0 - (temp_len_pos - piece_len) / temp_seg);
-            inner_xy[2 * nxy] = a[0] + w * (b[0] - a[0]);
-            inner_xy[2 * nxy + 1] = a[1] + w * (b[1] - a[1]);
-            nxy++;
-            temp_len_pos -= piece_len;
-        }
-    }
-    *total_time = total_len / mean_vel * init_time_times; // pm.cpp:122
-    *N = nxy + 1;
-    *M = nyaw + 1;
+    UalmResampleStream s;
+    ualm_rs_init(s, piece_len, yaw_piece_times);
+    for (int k = 0; k < npts - 1; k++)
+        if (!ualm_rs_segment(s, &p[3 * k], &p[3 * (k + 1)], inner_xy, max_inner_xy, inner_yaw, max_inner_yaw, true, 0)) return UALM_ELIMIT;
+    *total_time = ualm_rs_total_time(s, mean_vel, init_time_times); // pm.cpp:122
+    *N = (int32_t)(s.nxy + 1);
+    *M = (int32_t)(s.nyaw + 1);
     return UALM_OK;
 }

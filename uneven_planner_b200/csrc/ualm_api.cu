@@ -168,13 +168,13 @@ struct ualm_ctx {
     // pinned staging of ualm_update_map_window*'s grid copy (map_copy_ce), allocated at the first window
     static constexpr size_t STAGE_BYTES = 8u << 20;
     void *h_stage = nullptr;
-    // ualm_check_trajectories: a stream no solve occupies, at the greatest priority, so its CTAs go ahead of queued lane launches when
-    // SM slots free up; cdone marks the end of a check's kernels, which the free stream waits for before the grids it read can go.
+    // ualm_check_trajectories and ualm_submit_replan's build: a stream no solve occupies, at the greatest priority, so its CTAs go ahead
+    // of queued lane launches when SM slots free up; cdone marks the end of a check's kernels, which the free stream waits for before the grids it read can go.
     // Both are made at the first check, not at creation: streams share the device's hardware queues in creation order, and with one
     // more stream made before the throughput engine's, its cancels right after a submit came too late (tests/test_gpu_cancel.py)
     cudaStream_t cstream = nullptr;
     cudaEvent_t cdone = nullptr;
-    // its inputs and outputs: one grow-only block, allocated and replaced in stream order on cstream (a block freed at every call would
+    // their inputs and outputs: one grow-only block, allocated and replaced in stream order on cstream (a block freed at every call would
     // go back to the device at that call's synchronisation and be mapped again at the next)
     void *cbuf = nullptr;
     size_t cbuf_bytes = 0;
@@ -1352,6 +1352,28 @@ extern "C" int ualm_feasibility_batch(ualm_ctx_t *c, double dt, double *out10)
     return UALM_OK;
 }
 
+// the check stream (ualm_ctx::cstream), made at first use
+static int check_stream(ualm_ctx *c)
+{
+    if (!c->cstream) {
+        int least = 0, greatest = 0;
+        CK(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+        CK(cudaStreamCreateWithPriority(&c->cstream, cudaStreamNonBlocking, greatest));
+    }
+    return UALM_OK;
+}
+// cbuf of at least `bytes`, grown in stream order on the check stream: the old block is freed behind the work that used it
+static int check_block(ualm_ctx *c, size_t bytes)
+{
+    if (c->cbuf_bytes < bytes) {
+        if (c->cbuf) CK(cudaFreeAsync(c->cbuf, c->cstream));
+        c->cbuf = nullptr; c->cbuf_bytes = 0;
+        CK(cudaMallocAsync(&c->cbuf, bytes, c->cstream));
+        c->cbuf_bytes = bytes;
+    }
+    return UALM_OK;
+}
+
 // check_kernel over host trajectories, on the context's check stream, against each environment's grid version current at the call.
 // The context's block (cbuf) grows in stream order on that stream, and the versions are let go only after cdone (as lane_hold lets
 // go), so nothing here waits for a batch in flight
@@ -1370,11 +1392,7 @@ extern "C" int ualm_check_trajectories(ualm_ctx_t *c, int B, const int32_t *N, c
     if (B == 0) return UALM_OK;
     if (int rc = check_envs(c, B, env)) return rc;
     CK(cudaSetDevice(c->device));
-    if (!c->cstream) {
-        int least = 0, greatest = 0;
-        CK(cudaDeviceGetStreamPriorityRange(&least, &greatest));
-        CK(cudaStreamCreateWithPriority(&c->cstream, cudaStreamNonBlocking, greatest));
-    }
+    if (int rc = check_stream(c)) return rc;
     if (!c->cdone) CK(cudaEventCreateWithFlags(&c->cdone, cudaEventDisableTiming));
     // problems grouped by environment, and the grid version each environment has now
     std::vector<int> idx;
@@ -1405,12 +1423,7 @@ extern "C" int ualm_check_trajectories(ualm_ctx_t *c, int B, const int32_t *N, c
         ualm_ctx *c;
         ~Done() { if (cudaEventRecord(c->cdone, c->cstream) == cudaSuccess) cudaStreamWaitEvent(c->fstream, c->cdone, 0); }
     } done{c};
-    if (c->cbuf_bytes < bytes) {       // the old block is freed behind the checks that used it
-        if (c->cbuf) CK(cudaFreeAsync(c->cbuf, st));
-        c->cbuf = nullptr; c->cbuf_bytes = 0;
-        CK(cudaMallocAsync(&c->cbuf, bytes, st));
-        c->cbuf_bytes = bytes;
-    }
+    if (int rc = check_block(c, bytes)) return rc;
     double *d_out = (double *)c->cbuf, *d_pt = d_out + 16 * (size_t)B, *d_tf = d_pt + 2 * (size_t)B, *d_cxy = d_tf + B, *d_cyaw = d_cxy + ncx;
     ProbDesc *d_desc = (ProbDesc *)(d_out + nd);
     int *d_idx = (int *)(d_desc + B);
@@ -1434,6 +1447,105 @@ extern "C" int ualm_check_trajectories(ualm_ctx_t *c, int B, const int32_t *N, c
     CK(cudaMemcpyAsync(out16, d_out, sizeof(double) * 16 * B, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     return UALM_OK;
+}
+
+// replan_kernel on the check stream (it reads no grid, so no version is held), then the built arrays go through ualm_submit_batch_env.
+// Every refusal but one is decided before the build; that one (a polyline whose length gives no usable total_time) is decided before any
+// output is written or lane taken
+extern "C" int ualm_submit_replan(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *piece_T, const double *c_xy,
+                                  const double *c_yaw, const double *bnd, const int32_t *env, const double *t_from, double dt,
+                                  const ualm_resample_params_t *rp, int depth, int *ticket, int32_t *N_out, int32_t *M_out, double *bnd_out,
+                                  double *total_time_out, double *inner_xy_out, double *inner_yaw_out)
+{
+    if (!c || !ticket || B < 0 || (B > 0 && (!N || !M || !piece_T || !c_xy || !c_yaw || !bnd || !t_from || !N_out || !M_out || !bnd_out || !total_time_out)))
+        return fail(UALM_EINVAL, "ualm_submit_replan: null argument or B < 0");
+    if (!(dt > 0.0)) return fail(UALM_EINVAL, "ualm_submit_replan: dt must be > 0");
+    if (depth < 1 || depth > UALM_MAX_LANES) return fail(UALM_EINVAL, "ualm_submit_replan: depth out of range [1, UALM_MAX_LANES]");
+    const ualm_resample_params_t r = rp ? *rp : ualm_resample_params_t{0.3, 2.0, 0.5, 1.2, 0.0};   // run_*.yaml manager/*
+    if (!(r.piece_len > 0.0) || !(r.yaw_piece_times > 0.0) || !(r.mean_vel > 0.0) || !(r.init_time_times > 0.0))
+        return fail(UALM_EINVAL, "ualm_submit_replan: piece_len, yaw_piece_times, mean_vel and init_time_times must be > 0");
+    long long ncx = 0, ncy = 0;
+    for (int b = 0; b < B; b++) {
+        if (N[b] < 1 || M[b] < 1) return fail(UALM_EINVAL, "ualm_submit_replan: piece counts must be >= 1");
+        double tx = 0.0, ty = 0.0;      // replan_kernel's sums
+        for (int i = 0; i < N[b]; i++) tx += piece_T[2 * b];
+        for (int i = 0; i < M[b]; i++) ty += piece_T[2 * b + 1];
+        const double total = tx < ty ? tx : ty;
+        if (!(t_from[b] >= 0.0) || !(t_from[b] < total)) return fail(UALM_EINVAL, "ualm_submit_replan: t_from must be in [0, the trajectory's duration)");
+        if (!(total / dt < 4.0e6)) return fail(UALM_EINVAL, "ualm_submit_replan: duration / dt must be < 4e6");
+        if (!std::isfinite(piece_T[2 * b]) || !std::isfinite(piece_T[2 * b + 1])) return fail(UALM_EINVAL, "ualm_submit_replan: piece_T must be finite");
+        for (int k : {6, 7, 8, 9, 10, 11, 15, 16, 17})      // the goal entries bnd' takes
+            if (!std::isfinite(bnd[18 * (size_t)b + k])) return fail(UALM_EINVAL, "ualm_submit_replan: the goal entries of bnd must be finite");
+        ncx += 12LL * N[b]; ncy += 6LL * M[b];
+    }
+    // a diverged solve's coefficients: refused, not sampled
+    for (long long q = 0; q < ncx; q++) if (!std::isfinite(c_xy[q])) return fail(UALM_EINVAL, "ualm_submit_replan: c_xy must be finite");
+    for (long long q = 0; q < ncy; q++) if (!std::isfinite(c_yaw[q])) return fail(UALM_EINVAL, "ualm_submit_replan: c_yaw must be finite");
+    if (B == 0) return ualm_submit_batch_env(c, 0, N_out, M_out, bnd_out, total_time_out, nullptr, nullptr, env, depth, ticket);
+    if (int rc = check_envs(c, B, env)) return rc;
+    const int lane = c->next_submit % depth;
+    if (c->tp ? ualm_tp::tp_lane_in_flight(c->tp, lane) : c->lanes[lane].in_flight)
+        return fail(UALM_ESTATE, "all lanes of this depth are in flight: ualm_wait_batch the oldest ticket first");
+    CK(cudaSetDevice(c->device));
+    if (int rc = check_stream(c)) return rc;
+    std::vector<ProbDesc> desc(B);
+    long long ocx = 0, ocy = 0;
+    for (int b = 0; b < B; b++) {
+        memset(&desc[b], 0, sizeof(ProbDesc));
+        desc[b].N = N[b]; desc[b].M = M[b]; desc[b].off_cxy = ocx; desc[b].off_cyaw = ocy;
+        ocx += 12LL * N[b]; ocy += 6LL * M[b];
+    }
+    // the block: out (UALM_REPLAN_STRIDE B) | piece_T 2B | bnd 18B | t_from B | c_xy | c_yaw (doubles), then desc
+    const size_t nout = (size_t)UALM_REPLAN_STRIDE * B, nd = nout + 21 * (size_t)B + (size_t)ncx + (size_t)ncy;
+    const cudaStream_t st = c->cstream;
+    if (int rc = check_block(c, sizeof(double) * nd + sizeof(ProbDesc) * B)) return rc;
+    double *d_out = (double *)c->cbuf, *d_pt = d_out + nout, *d_bnd = d_pt + 2 * (size_t)B, *d_tf = d_bnd + 18 * (size_t)B, *d_cxy = d_tf + B,
+           *d_cyaw = d_cxy + ncx;
+    ProbDesc *d_desc = (ProbDesc *)(d_out + nd);
+    CK(cudaMemcpyAsync(d_pt, piece_T, sizeof(double) * 2 * B, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_bnd, bnd, sizeof(double) * 18 * B, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_tf, t_from, sizeof(double) * B, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_cxy, c_xy, sizeof(double) * ncx, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_cyaw, c_yaw, sizeof(double) * ncy, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_desc, desc.data(), sizeof(ProbDesc) * B, cudaMemcpyHostToDevice, st));
+    ReplanPtrs a;
+    a.desc = d_desc; a.c_xy = d_cxy; a.c_yaw = d_cyaw; a.piece_T = d_pt; a.bnd = d_bnd; a.t_from = d_tf; a.out = d_out;
+    const ReplanParams p{dt, r.piece_len, r.yaw_piece_times, r.mean_vel, r.init_time_times};
+    replan_kernel<<<(B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(a, p, B);
+    CK(cudaGetLastError());
+    std::vector<double> h(nout);
+    CK(cudaMemcpyAsync(h.data(), d_out, sizeof(double) * nout, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    // the one refusal after the build, before any output: a polyline of zero or non-finite length (a robot already at its goal, or
+    // coordinates so large that their squares overflow) has no total_time ualm_submit_batch_env would take
+    for (int b = 0; b < B; b++) {
+        const double T = h[(size_t)UALM_REPLAN_STRIDE * b + 18];
+        if (!(T > 0.0) || !std::isfinite(T)) return fail(UALM_EINVAL, "ualm_submit_replan: row " + std::to_string(b) + "'s polyline has zero or non-finite length");
+    }
+    // the outputs, and the packed inner arrays ualm_submit_batch_env takes (a row over the limits: zeros, never read).  The stream's
+    // bound keeps N', M' <= UALM_RS_MAX_WAYPOINTS + 2
+    long long pxy = 0, pyaw = 0;
+    for (int b = 0; b < B; b++) {
+        const double *o = &h[(size_t)UALM_REPLAN_STRIDE * b];
+        N_out[b] = (int32_t)o[19]; M_out[b] = (int32_t)o[20];
+        memcpy(bnd_out + 18 * (size_t)b, o, sizeof(double) * 18);
+        total_time_out[b] = o[18];
+        if (inner_xy_out) memcpy(inner_xy_out + (size_t)UALM_REPLAN_INNER_XY * b, o + 21, sizeof(double) * UALM_REPLAN_INNER_XY);
+        if (inner_yaw_out) memcpy(inner_yaw_out + (size_t)UALM_REPLAN_INNER_YAW * b, o + 21 + UALM_REPLAN_INNER_XY, sizeof(double) * UALM_REPLAN_INNER_YAW);
+        pxy += 2LL * (N_out[b] - 1); pyaw += M_out[b] - 1;
+    }
+    std::vector<double> ixy((size_t)pxy, 0.0), iyaw((size_t)pyaw, 0.0);
+    pxy = pyaw = 0;
+    for (int b = 0; b < B; b++) {
+        const double *o = &h[(size_t)UALM_REPLAN_STRIDE * b];
+        const long long nxy = 2LL * (N_out[b] - 1), nyaw = M_out[b] - 1;
+        if (N_out[b] <= UALM_NMAX && M_out[b] <= UALM_MMAX) {
+            memcpy(ixy.data() + pxy, o + 21, sizeof(double) * nxy);
+            memcpy(iyaw.data() + pyaw, o + 21 + UALM_REPLAN_INNER_XY, sizeof(double) * nyaw);
+        }
+        pxy += nxy; pyaw += nyaw;
+    }
+    return ualm_submit_batch_env(c, B, N_out, M_out, bnd_out, total_time_out, ixy.data(), iyaw.data(), env, depth, ticket);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -24,6 +24,7 @@
 #include "ualm.h"
 #include "ualm_detmath.h"
 #include "ualm_mailbox.h"
+#include "resample_stream.h"
 
 #define UALM_THREADS 32         // threads per warp slot
 #define UALM_WPB 4              // warp slots per CTA (4 / 2 / 1 trajectories with 1 / 2 / 4 warps each)
@@ -2589,6 +2590,94 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) check_kernel(const __
     if (lane == 0) {
         o[0] = mvx.val; o[1] = max_.val; o[2] = may.val; o[3] = mcur.val; o[4] = matt; o[5] = msig; o[6] = err; o[7] = (R)count; o[8] = Tx; o[9] = Ty;
         for (int q = 0; q < 6; q++) o[10 + q] = first[q];
+    }
+}
+
+// ---------------------------------------------------------------------------------------------
+// Replanned problems of trajectories the caller holds (ualm_submit_replan): the state at tau = t_from (locate_piece + piece_eval),
+// then PlanManager's resampler (resample_stream.h) over the polyline {the point at tau, the samples tau < t < duration of the
+// reference's sequence t = 0, dt, 2dt.. (the same additions as check_kernel), the goal of the original problem}.  One warp per row:
+// each chunk the lanes evaluate 32 sample times, then every lane runs the sequential resampler on the same points broadcast by
+// shuffle, and lane 0 writes.  Waypoints past the compiled limits are counted, not formed; such a row's inner points are zeros.  The
+// stream is bounded (ualm_rs_push), so a row's serial work is bounded whatever its lengths and yaws.
+// Oracle: tests/replan_oracle.cpp.
+// out[UALM_REPLAN_STRIDE * row + ...] = bnd' (18) | total_time | N' | M' | inner xy (2 (UALM_NMAX - 1)) | inner yaw (UALM_MMAX - 1)
+// ---------------------------------------------------------------------------------------------
+static_assert(UALM_REPLAN_INNER_XY == 2 * (UALM_NMAX - 1) && UALM_REPLAN_INNER_YAW == UALM_MMAX - 1, "ualm.h's replan strides");
+#define UALM_REPLAN_STRIDE (21 + UALM_REPLAN_INNER_XY + UALM_REPLAN_INNER_YAW)
+struct ReplanPtrs {
+    const ProbDesc *desc;          // N, M, off_cxy, off_cyaw of the trajectory
+    const R *c_xy, *c_yaw, *piece_T, *bnd, *t_from;
+    R *out;
+};
+struct ReplanParams { R dt, piece_len, yaw_piece_times, mean_vel, init_time_times; };
+// the host has checked N, M >= 1, 0 <= t_from < duration and duration / dt < 4e6 for every row
+__global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) replan_kernel(const __grid_constant__ ReplanPtrs a, const __grid_constant__ ReplanParams rp, int n)
+{
+    const int lane = threadIdx.x & 31, w = blockIdx.x * UALM_WPB + (threadIdx.x >> 5);
+    if (w >= n) return;         // whole warp exits
+    const ProbDesc *pd = a.desc + w;
+    const int N = pd->N, M = pd->M;
+    const R *cxy = a.c_xy + pd->off_cxy, *cyaw = a.c_yaw + pd->off_cyaw, *bnd = a.bnd + 18 * (size_t)w;
+    const R Tx = a.piece_T[2 * w], Ty = a.piece_T[2 * w + 1], t0 = a.t_from[w];
+    R *o = a.out + UALM_REPLAN_STRIDE * (size_t)w, *oxy = o + 21, *oyaw = oxy + UALM_REPLAN_INNER_XY;
+    for (int q = lane; q < UALM_REPLAN_INNER_XY + UALM_REPLAN_INNER_YAW; q += 32) oxy[q] = 0.0;
+    __syncwarp();
+    R tot_xy = 0.0, tot_yaw = 0.0;
+    for (int i = 0; i < N; i++) tot_xy += Tx;
+    for (int i = 0; i < M; i++) tot_yaw += Ty;
+    const R total = tot_xy < tot_yaw ? tot_xy : tot_yaw;
+    // the start state (every lane)
+    R px, py, vx, vy, ax, ay, yaw, dyaw, ddyaw;
+    {
+        R tl = t0;
+        const int ip = locate_piece(N, Tx, tl);
+        piece_eval(cxy + 6 * ip, tl, px, vx, ax);
+        piece_eval(cxy + 6 * N + 6 * ip, tl, py, vy, ay);
+        R ty = t0;
+        const int iy = locate_piece(M, Ty, ty);
+        piece_eval(cyaw + 6 * iy, ty, yaw, dyaw, ddyaw);
+    }
+    R *wxy = lane == 0 ? oxy : nullptr, *wyaw = lane == 0 ? oyaw : nullptr;
+    UalmResampleStream s;
+    ualm_rs_init(s, rp.piece_len, rp.yaw_piece_times);
+    ualm_rs_push(s, px, py, yaw, wxy, UALM_NMAX - 1, wyaw, UALM_MMAX - 1);
+    R tbase = 0.0;
+    while (true) {
+        R tm = 0.0, tt = tbase;
+        for (int i = 0; i < 32; i++) { if (i == lane) tm = tt; tt = tt + rp.dt; }   // check_kernel's additions
+        const bool valid = tm < total, kept = valid && tm > t0;
+        R x = 0.0, y = 0.0, h = 0.0;
+        if (kept) {     // feas_sample's evaluation
+            R tl = tm, d1, d2;
+            const int ip = locate_piece(N, Tx, tl);
+            piece_eval(cxy + 6 * ip, tl, x, d1, d2);
+            piece_eval(cxy + 6 * N + 6 * ip, tl, y, d1, d2);
+            R ty = tm;
+            const int iy = locate_piece(M, Ty, ty);
+            piece_eval(cyaw + 6 * iy, ty, h, d1, d2);
+        }
+        const unsigned km = __ballot_sync(0xffffffffu, kept);   // the kept lanes are contiguous: t grows with the lane
+        for (unsigned m = km; m; m &= m - 1) {
+            const int l = __ffs(m) - 1;
+            const R bx = __shfl_sync(0xffffffffu, x, l), by = __shfl_sync(0xffffffffu, y, l), bh = __shfl_sync(0xffffffffu, h, l);
+            ualm_rs_push(s, bx, by, bh, wxy, UALM_NMAX - 1, wyaw, UALM_MMAX - 1);
+        }
+        if (__popc(__ballot_sync(0xffffffffu, valid)) < 32) break;
+        tbase = tt;
+    }
+    ualm_rs_push(s, bnd[6], bnd[7], bnd[15], wxy, UALM_NMAX - 1, wyaw, UALM_MMAX - 1);   // the goal: end_xy's position, end_yaw's angle
+    // cut short (resample_stream.h: a huge or non-finite length or yaw): over the limits, N' = M' = UALM_RS_MAX_WAYPOINTS + 2
+    const long long Nn = s.cut ? UALM_RS_MAX_WAYPOINTS + 2 : s.nxy + 1, Mn = s.cut ? UALM_RS_MAX_WAYPOINTS + 2 : s.nyaw + 1;
+    if (Nn > UALM_NMAX || Mn > UALM_MMAX) {      // over the limits: the waypoints written before the count passed them go
+        __syncwarp();
+        for (int q = lane; q < UALM_REPLAN_INNER_XY + UALM_REPLAN_INNER_YAW; q += 32) oxy[q] = 0.0;
+    }
+    if (lane == 0) {
+        const R head[18] = {px, py, vx, vy, ax, ay, bnd[6], bnd[7], bnd[8], bnd[9], bnd[10], bnd[11], yaw, dyaw, ddyaw, bnd[15], bnd[16], bnd[17]};
+        for (int k = 0; k < 18; k++) o[k] = head[k];
+        o[18] = ualm_rs_total_time(s, rp.mean_vel, rp.init_time_times);
+        o[19] = (R)Nn; o[20] = (R)Mn;
     }
 }
 
