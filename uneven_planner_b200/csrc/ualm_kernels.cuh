@@ -191,6 +191,17 @@ __device__ __forceinline__ double lds64(unsigned a)
     return v;
 }
 __device__ __forceinline__ void sts64(unsigned a, double v) { asm volatile("st.shared.f64 [%0], %1;" ::"r"(a), "d"(v) : "memory"); }
+// 16-byte accesses (a must be 16-byte aligned)
+__device__ __forceinline__ double2 lds2f64(unsigned a)
+{
+    double2 v;
+    asm volatile("ld.shared.v2.f64 {%0, %1}, [%2];" : "=d"(v.x), "=d"(v.y) : "r"(a) : "memory");
+    return v;
+}
+__device__ __forceinline__ void sts2f64(unsigned a, double x, double y)
+{
+    asm volatile("st.shared.v2.f64 [%0], {%1, %2};" ::"r"(a), "d"(x), "d"(y) : "memory");
+}
 // a store under a predicate: keeps the compiler from turning a guarded store into a divergent branch
 __device__ __forceinline__ void sts64_if(bool p, unsigned a, double v)
 {
@@ -1401,28 +1412,45 @@ __device__ UALM_NOINLINE void accumulate_tasks(Traj &t, int gtid, int GT)
     }
 }
 
-// the cost chain of calConstrainCostGrad (alm_traj_opt.cpp:825-943) on the leader warp
+// the cost chain of calConstrainCostGrad (alm_traj_opt.cpp:825-943) on the leader warp: 8 terms per sample in sample order.
+// The terms are fetched 32 samples at a time by all lanes, one block ahead of the chain, and staged sample-major in the LU window
+// (idle from the end of minco_generate to the adjoint sweeps).  Every lane then runs the chain on the same values, reading two
+// terms per broadcast ld.shared.v2 one sample ahead of the adds.  Handing each term over by shuffle took two SHFL and two moves
+// per add, and those instructions competed with the co-resident warps for issue slots.
 __device__ UALM_NOINLINE void cost_chain(Traj &t, int lane)
 {
     const int S = t.S;
     const R *scr = t.scr;
-    // cost chain: 8 terms per sample in sample order on lane 0; the terms are fetched 32 samples at a time by all lanes
-    // and handed over by shuffles so the loads stay off the dependent chain
-    {
-        R cost = 0.0;
-        for (int s0 = 0; s0 < S; s0 += 32) {
-            const int s = s0 + lane;
-            R term[8];
+    const unsigned buf = t.win.a;        // 32 samples x 8 terms
+    R cost = 0.0;
+    R next[8];
 #pragma unroll
-            for (int k = 0; k < 8; k++) term[k] = (s < S) ? scr[(SF_COST0 + k) * S + s] : 0.0;
-            const int cnt = min(32, S - s0);
-            for (int l = 0; l < cnt; l++) {
+    for (int k = 0; k < 8; k++) next[k] = (lane < S) ? scr[(SF_COST0 + k) * S + lane] : 0.0;
+    for (int s0 = 0; s0 < S; s0 += 32) {
 #pragma unroll
-                for (int k = 0; k < 8; k++) cost += __shfl_sync(0xffffffffu, term[k], l);
-            }
+        for (int k = 0; k < 8; k += 2) sts2f64(buf + 64u * lane + 8u * k, next[k], next[k + 1]);
+        __syncwarp();
+        const int sn = s0 + 32 + lane;
+#pragma unroll
+        for (int k = 0; k < 8; k++) next[k] = (sn < S) ? scr[(SF_COST0 + k) * S + sn] : 0.0;
+        const int cnt = min(32, S - s0);
+        R cur[8];
+#pragma unroll
+        for (int k = 0; k < 8; k += 2) { const double2 v = lds2f64(buf + 8u * k); cur[k] = v.x; cur[k + 1] = v.y; }
+#pragma unroll 1
+        for (int l = 0; l < cnt; l++) {
+            R v[8];
+#pragma unroll
+            for (int k = 0; k < 8; k++) v[k] = cur[k];
+            const unsigned row = buf + 64u * (unsigned)min(l + 1, 31);
+#pragma unroll
+            for (int k = 0; k < 8; k += 2) { const double2 w = lds2f64(row + 8u * k); cur[k] = w.x; cur[k + 1] = w.y; }
+#pragma unroll
+            for (int k = 0; k < 8; k++) cost += v[k];
         }
-        if (lane == 0) t.sc[SC_CONSTR] = cost;
+        __syncwarp();                    // every lane has read the block before the next one overwrites it
     }
+    if (lane == 0) t.sc[SC_CONSTR] = cost;
 }
 
 // gdT(i) += B1 . adj  (se2traj.hpp:763-814); adj = solved adjoint vector (element stride st), Dim columns
