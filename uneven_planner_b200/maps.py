@@ -144,11 +144,15 @@ def get_terrain(name, build_if_missing=True):
     return None
 
 
-def synthetic_terrain(kind="bumps", seed=0, size=(200, 200, 64)):
+def synthetic_terrain(kind="bumps", seed=0, geom=None):
     """Analytic terrain z = h(x,y) turned into the same grid the builder produces (normal of the surface
     at the 0.12 m forward-shifted footprint centre, sigma from curvature).  Used by tests and as a clearly
-    labelled fallback when no .umap file is available; NOT one of the reference's terrains."""
-    geom = _lib.map_geometry()
+    labelled fallback when no .umap file is available; NOT one of the reference's terrains.
+    geom: the grid's geometry (None: the reference's 10 m x 10 m, 0.05 m, 0.1 rad).  The bumps are drawn for the 10 m square; their centres are
+    stretched to the grid's extent per axis and their widths by the larger of the two factors, so a rectangle is covered and the
+    default grid keeps its cells."""
+    geom = geom or _lib.map_geometry()
+    kx, ky = geom.max_boundary[0] / 5.0, geom.max_boundary[1] / 5.0      # exactly 1 on the default grid
     X, Y, W = geom.voxel_num
     xs = (np.arange(X) + 0.5) * geom.xy_resolution + geom.origin[0]
     ys = (np.arange(Y) + 0.5) * geom.xy_resolution + geom.origin[1]
@@ -163,16 +167,16 @@ def synthetic_terrain(kind="bumps", seed=0, size=(200, 200, 64)):
         a, b = 0.2, -0.1
         z = a * px + b * py; hx = np.full_like(px, a); hy = np.full_like(px, b); lap = np.zeros_like(px)
     elif kind == "hills":
-        # compactly supported bumps amp * (1 - r^2/s^2)^3 from + - * / only, and the 64 yaw cosines from libm: the grid is the same
+        # compactly supported bumps amp * (1 - r^2/s^2)^3 from + - * / only, and the yaw layers' cosines from libm: the grid is the same
         # bits on every host (numpy's vectorised exp / cos may differ in the last bit between CPUs), so outputs on it can be stored
         cw = np.array([math.cos(float(y)) for y in yaws]); sw = np.array([math.sin(float(y)) for y in yaws])
         px = gx + 0.12 * cw[None, None, :]
         py = gy + 0.12 * sw[None, None, :]
         z = np.zeros_like(px); hx = np.zeros_like(px); hy = np.zeros_like(px); lap = np.zeros_like(px)
         for _ in range(8):
-            cx, cy = rng.uniform(-4, 4, 2)
+            cx, cy = rng.uniform(-4, 4, 2) * (kx, ky)
             amp = rng.uniform(0.2, 0.8) * rng.choice([-1, 1])
-            s = rng.uniform(1.5, 3.0)
+            s = rng.uniform(1.5, 3.0) * max(kx, ky)
             s2 = s * s
             dx, dy = px - cx, py - cy
             r2 = dx * dx + dy * dy
@@ -184,9 +188,9 @@ def synthetic_terrain(kind="bumps", seed=0, size=(200, 200, 64)):
     else:
         z = np.zeros_like(px); hx = np.zeros_like(px); hy = np.zeros_like(px); lap = np.zeros_like(px)
         for _ in range(6):
-            cx, cy = rng.uniform(-4, 4, 2)
+            cx, cy = rng.uniform(-4, 4, 2) * (kx, ky)
             amp = rng.uniform(0.2, 0.8) * rng.choice([-1, 1])
-            s = rng.uniform(0.9, 2.0)
+            s = rng.uniform(0.9, 2.0) * max(kx, ky)
             e = amp * np.exp(-((px - cx) ** 2 + (py - cy) ** 2) / (2 * s * s))
             z += e
             hx += -e * (px - cx) / (s * s)

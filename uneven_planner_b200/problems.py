@@ -130,10 +130,18 @@ def from_paths(paths, **kw):
                         np.concatenate(xys) if xys else np.zeros(0), np.concatenate(yaws) if yaws else np.zeros(0))
 
 
+def _per_axis(v):
+    """(x, y) of a range bound given as one number or as a pair"""
+    x, y = np.broadcast_to(np.asarray(v, np.float64), (2,))
+    return float(x), float(y)
+
+
 def generate(mapdata, B, seed=0, max_rho=0.05, min_cnormal=0.8, lo=-4.5, hi=4.5, min_dist=1.5, radius=0.6, ds=0.06,
              n_max=56, max_tries=200000):
-    """B random SE(2) start/goal problems on `mapdata` (config 2/3 recipe, SURVEY 8d)."""
+    """B random SE(2) start/goal problems on `mapdata` (config 2/3 recipe, SURVEY 8d).  lo / hi: the range the positions are drawn
+    from, one number for both axes or an (x, y) pair for a map that is not square."""
     g = mapdata.geom
+    (lox, loy), (hix, hiy) = _per_axis(lo), _per_axis(hi)
     occ3, occ2 = mapdata.occupancy(min_cnormal, max_rho)
     X, Y, W = mapdata.shape
     rng = Rng(seed)
@@ -148,8 +156,8 @@ def generate(mapdata, B, seed=0, max_rho=0.05, min_cnormal=0.8, lo=-4.5, hi=4.5,
         tries += 1
         if tries > max_tries:
             raise RuntimeError("problem generator: too many rejections")
-        s = np.array([rng.uniform(lo, hi), rng.uniform(lo, hi), rng.uniform(-np.pi, np.pi)])
-        e = np.array([rng.uniform(lo, hi), rng.uniform(lo, hi), rng.uniform(-np.pi, np.pi)])
+        s = np.array([rng.uniform(lox, hix), rng.uniform(loy, hiy), rng.uniform(-np.pi, np.pi)])
+        e = np.array([rng.uniform(lox, hix), rng.uniform(loy, hiy), rng.uniform(-np.pi, np.pi)])
         if np.hypot(*(s[:2] - e[:2])) < min_dist:
             continue
         i = idx3(s)
@@ -180,6 +188,7 @@ def generate_astar(mapdata, B, seed=0, max_rho=0.05, min_cnormal=0.8, lo=-4.5, h
     over the optimizer's limits are skipped.  Deterministic in (map, B, seed), independent of the thread count."""
     from . import front_end
     g = mapdata.geom
+    (lox, loy), (hix, hiy) = _per_axis(lo), _per_axis(hi)
     view = front_end.MapView(mapdata, min_cnormal, max_rho)
     rng = Rng(seed)
     parts, starts, goals = [], [], []
@@ -187,8 +196,8 @@ def generate_astar(mapdata, B, seed=0, max_rho=0.05, min_cnormal=0.8, lo=-4.5, h
     while have < B:
         cs, cg = [], []
         while len(cs) < max(2 * (B - have), 64):
-            s = np.array([rng.uniform(lo, hi), rng.uniform(lo, hi), rng.uniform(-np.pi, np.pi)])
-            e = np.array([rng.uniform(lo, hi), rng.uniform(lo, hi), rng.uniform(-np.pi, np.pi)])
+            s = np.array([rng.uniform(lox, hix), rng.uniform(loy, hiy), rng.uniform(-np.pi, np.pi)])
+            e = np.array([rng.uniform(lox, hix), rng.uniform(loy, hiy), rng.uniform(-np.pi, np.pi)])
             if np.hypot(*(s[:2] - e[:2])) < min_dist:
                 continue
             cs.append(s); cg.append(e)
