@@ -72,18 +72,15 @@ struct Lane {
     cudaStream_t stream = nullptr, own_stream = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
     bool have_batch = false, solved = false, in_flight = false;
-    int B = 0, Nmax = 0, Mmax = 0, nmax = 0, Smax = 0, n_active = 0;
+    // the lane's uploaded batch, on both paths (the throughput engine reads it too: tp_upload)
+    BatchLayout batch;
     std::vector<ProbDesc> desc;
     std::vector<int> order;              // launch order over the ACTIVE problems (largest first)
-    std::vector<unsigned char> skip;     // problems over the compiled limits: not solved, ret_code = UALM_ELIMIT in their record
-    // environments: env[b] of every problem; eidx = all problems grouped by environment (ascending within one), environment e at
-    // [eoff[e], eoff[e + 1]).  The one-warp-per-problem kernels run once per environment present, over its slice of d_eidx
-    std::vector<int> env, eidx;
-    int eoff[UALM_MAX_ENVS + 1] = {};
+    // the one-warp-per-problem kernels run once per environment present, over its slice of d_eidx (batch.eidx)
     DevBuf<int> d_eidx;
     SmemLayout eL[UALM_MAX_ENVS];        // their layouts (maxima over the environment's problems)
     size_t esmem[UALM_MAX_ENVS] = {};
-    long long tot_x = 0, tot_s = 0, tot_cxy = 0, tot_cyaw = 0, tot_hist = 0, tot_scr = 0, tot_fac = 0, tot_ws = 0;
+    long long tot_hist = 0, tot_scr = 0, tot_fac = 0, tot_ws = 0;
     DevBuf<ProbDesc> d_desc;
     DevBuf<int> d_order;
     std::vector<int> group;      // warps per problem (1, 2 or 4)
@@ -311,11 +308,13 @@ extern "C" int ualm_reset_stream(ualm_ctx_t *c)
     return UALM_OK;
 }
 
+static bool lane_in_flight(ualm_ctx *c, int q) { return c->tp ? ualm_tp::tp_lane_in_flight(c->tp, q) : c->lanes[q].in_flight; }
+
 // binding is refused while a batch is in flight, on the parity lanes and on the throughput engine's
 static int lanes_idle(ualm_ctx *c, const char *what)
 {
     for (int q = 0; q < UALM_MAX_LANES; q++)
-        if (c->tp ? ualm_tp::tp_lane_in_flight(c->tp, q) : c->lanes[q].in_flight)
+        if (lane_in_flight(c, q))
             return fail(UALM_ESTATE, std::string(what) + " while a submitted batch is in flight (ualm_wait_batch first)");
     return UALM_OK;
 }
@@ -423,13 +422,13 @@ static void map_install(ualm_ctx *c, const ualm_map_geom_t *g, MapRef nv)
     v.have_map = true;
 }
 
-// lane l launches a batch of the environments in `mask`: it holds their current versions from now on, and lets go of the versions of
+// lane l launches its batch: it holds the current versions of the batch's environments from now on, and lets go of the versions of
 // its previous launch.  That launch may still run (ualm_solve_resident twice on one lane), so the free stream first waits for its
 // completion: whatever only it held is freed after it.  A throughput lane is relaunched only once collected (ctx lanes not made)
-static int lane_hold(ualm_ctx *c, Lane &l, unsigned mask)
+static int lane_hold(ualm_ctx *c, Lane &l)
 {
     if (l.made) CK(cudaStreamWaitEvent(c->fstream, l.ev1, 0));
-    for (int e = 0; e < UALM_MAX_ENVS; e++) l.vref[e] = (mask >> e) & 1u ? c->envs[e].map : nullptr;
+    for (int e = 0; e < UALM_MAX_ENVS; e++) l.vref[e] = (l.batch.env_mask >> e) & 1u ? c->envs[e].map : nullptr;
     return UALM_OK;
 }
 
@@ -462,12 +461,13 @@ extern "C" int ualm_set_map_f64(ualm_ctx_t *c, const ualm_map_geom_t *g, const d
 static int prepare_launch(ualm_ctx *c)
 {
     Lane *b = c->b;
+    const BatchLayout &L = b->batch;
     for (int e = 0; e < UALM_MAX_ENVS; e++) {
-        if (b->eoff[e + 1] == b->eoff[e]) continue;
+        if (L.eoff[e + 1] == L.eoff[e]) continue;
         int Nm = 1, Mm = 1, nm = 1, Sm = 1;
-        for (int q = b->eoff[e]; q < b->eoff[e + 1]; q++) {
-            const ProbDesc &d = b->desc[b->eidx[q]];
-            if (b->skip[b->eidx[q]]) continue;
+        for (int q = L.eoff[e]; q < L.eoff[e + 1]; q++) {
+            const ProbDesc &d = b->desc[L.eidx[q]];
+            if (L.skip[L.eidx[q]]) continue;
             Nm = std::max(Nm, d.N); Mm = std::max(Mm, d.M); nm = std::max(nm, d.n); Sm = std::max(Sm, d.S);
         }
         const DevParams &dp = c->envs[e].dp;
@@ -487,15 +487,84 @@ static int prepare_launch(ualm_ctx *c)
     return UALM_OK;
 }
 
+static int env_bound(ualm_ctx *c, int e)
+{
+    if (!c->envs[e].have_params || !c->envs[e].have_map)
+        return fail(UALM_ESTATE, "environment " + std::to_string(e) + " has no parameters or no map grid bound (ualm_select_env + ualm_set_params / ualm_set_map)");
+    return UALM_OK;
+}
 // env[B] (NULL = all 0): every index in range and every environment used fully bound, checked before anything is touched
 static int check_envs(ualm_ctx *c, int B, const int32_t *env)
 {
     for (int b = 0; b < (env ? B : 1); b++) {
         const int e = env ? env[b] : 0;
         if (e < 0 || e >= UALM_MAX_ENVS) return fail(UALM_EINVAL, "env index out of range [0, UALM_MAX_ENVS)");
-        if (!c->envs[e].have_params || !c->envs[e].have_map)
-            return fail(UALM_ESTATE, "environment " + std::to_string(e) + " has no parameters or no map grid bound (ualm_select_env + ualm_set_params / ualm_set_map)");
+        if (int rc = env_bound(c, e)) return rc;
     }
+    return UALM_OK;
+}
+// every environment of an uploaded batch still bound (a failed ualm_set_map leaves its environment unbound)
+static int check_envs(ualm_ctx *c, const BatchLayout &L)
+{
+    for (int e = 0; e < UALM_MAX_ENVS; e++)
+        if ((L.env_mask >> e) & 1u)
+            if (int rc = env_bound(c, e)) return rc;
+    return UALM_OK;
+}
+
+// the compiled limits (n <= 256: the L-BFGS register tile, UALM_NREG in ualm_kernels.cuh): a problem over them is not solved or
+// scanned, its record says UALM_ELIMIT, and the rest of its batch runs
+static bool over_limits(int N, int M) { return N > UALM_NMAX || M > UALM_MMAX; }
+
+// the problems of env[B] (NULL = all 0) grouped by environment, ascending within one: environment e at idx[off[e], off[e + 1])
+static void group_by_env(int B, const int32_t *env, std::vector<int> &idx, int off[UALM_MAX_ENVS + 1])
+{
+    idx.clear();
+    for (int e = 0; e < UALM_MAX_ENVS; e++) {
+        off[e] = (int)idx.size();
+        for (int b = 0; b < B; b++) if ((env ? env[b] : 0) == e) idx.push_back(b);
+    }
+    off[UALM_MAX_ENVS] = (int)idx.size();
+}
+
+// the layout of a batch (BatchLayout) for either path, from the arguments of ualm_upload_env; every argument is checked first
+static int batch_layout(ualm_ctx *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time, const double *inner_xy,
+                        const double *inner_yaw, const int32_t *env, BatchLayout *out)
+{
+    if (!c || B < 0 || (B > 0 && (!N || !M || !bnd || !total_time))) return fail(UALM_EINVAL, "bad argument");
+    if (int rc = check_envs(c, B, env)) return rc;
+    long long need_xy = 0, need_yaw = 0;
+    for (int b = 0; b < B; b++) {
+        if (N[b] < 1 || M[b] < 1) return fail(UALM_EINVAL, "piece counts must be >= 1");
+        if (!(total_time[b] > 0.0) || !std::isfinite(total_time[b])) return fail(UALM_EINVAL, "total_time must be finite and > 0");
+        need_xy += 2LL * (N[b] - 1); need_yaw += M[b] - 1;
+    }
+    if ((need_xy > 0 && !inner_xy) || (need_yaw > 0 && !inner_yaw)) return fail(UALM_EINVAL, "inner waypoint arrays are NULL but N > 1 or M > 1");
+    BatchLayout &L = *out;
+    L = BatchLayout();
+    L.B = B; L.N.assign(N, N + B); L.M.assign(M, M + B); L.env.assign(B, 0);
+    if (env) L.env.assign(env, env + B);
+    L.n.assign(B, 0); L.S.assign(B, 0); L.skip.assign(B, 0);
+    L.off_x.assign(B, 0); L.off_s.assign(B, 0); L.off_cxy.assign(B, 0); L.off_cyaw.assign(B, 0);
+    long long oixy = 0, oiyaw = 0;
+    for (int b = 0; b < B; b++) {
+        L.off_x[b] = L.tot_x; L.off_s[b] = L.tot_s; L.off_cxy[b] = L.tot_cxy; L.off_cyaw[b] = L.tot_cyaw;
+        L.tot_cxy += 12LL * N[b]; L.tot_cyaw += 6LL * M[b];
+        L.env_mask |= 1u << L.env[b];
+        const long long nxy = 2LL * (N[b] - 1), nyaw = M[b] - 1;
+        if (over_limits(N[b], M[b])) { L.skip[b] = 1; oixy += nxy; oiyaw += nyaw; continue; }
+        L.n[b] = 1 + 2 * (N[b] - 1) + (M[b] - 1); L.S[b] = N[b] * (c->envs[L.env[b]].dp.int_K + 1);
+        // x = [tau | Pxy | Pyaw]  (alm_traj_opt.cpp:205-216); logC2 (alm_traj_opt.h:238-241) is two IEEE ops + sqrt
+        const double T = total_time[b];
+        L.x0.push_back(T > 1.0 ? (std::sqrt(2.0 * T - 1.0) - 1.0) : (1.0 - std::sqrt(2.0 / T - 1.0)));
+        L.x0.insert(L.x0.end(), inner_xy + oixy, inner_xy + oixy + nxy);
+        L.x0.insert(L.x0.end(), inner_yaw + oiyaw, inner_yaw + oiyaw + nyaw);
+        oixy += nxy; oiyaw += nyaw;
+        L.tot_x += L.n[b]; L.tot_s += L.S[b];
+        L.Nmax = std::max(L.Nmax, N[b]); L.Mmax = std::max(L.Mmax, M[b]);
+        L.n_active++;
+    }
+    group_by_env(B, L.env.data(), L.eidx, L.eoff);
     return UALM_OK;
 }
 
@@ -503,8 +572,8 @@ static BatchPtrs batch_ptrs(ualm_ctx *c)
 {
     Lane *l = c->b;
     BatchPtrs b;
-    b.B = l->B;
-    b.n_active = l->n_active;
+    b.B = l->batch.B;
+    b.n_active = l->batch.n_active;
     b.queue = nullptr;
     b.n_leader_slots = 4;
     b.adopt = getenv("UALM_NOADOPT") ? 0 : 1;
@@ -525,10 +594,10 @@ static int per_env(ualm_ctx *c, F launch)
 {
     Lane *l = c->b;
     for (int e = 0; e < UALM_MAX_ENVS; e++) {
-        const int cnt = l->eoff[e + 1] - l->eoff[e];
+        const int cnt = l->batch.eoff[e + 1] - l->batch.eoff[e];
         if (cnt == 0) continue;
         BatchPtrs bp = batch_ptrs(c);
-        bp.order = l->d_eidx.p + l->eoff[e];
+        bp.order = l->d_eidx.p + l->batch.eoff[e];
         bp.n_active = cnt;
         launch(e, bp, cnt);
         CK(cudaGetLastError());
@@ -545,43 +614,23 @@ extern "C" int ualm_upload(ualm_ctx_t *c, int B, const int32_t *N, const int32_t
 extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
                                const double *inner_xy, const double *inner_yaw, const int32_t *env)
 {
-    if (!c || B < 0 || (B > 0 && (!N || !M || !bnd || !total_time))) return fail(UALM_EINVAL, "bad argument");
-    if (int rc = check_envs(c, B, env)) return rc;
-    if (c->tp) TP_CALL(ualm_tp::tp_upload(c->tp, c->cur, B, N, M, env, bnd, total_time, inner_xy, inner_yaw, err));
-    Lane *l = c->b;
-    if (l->in_flight) return fail(UALM_ESTATE, "ualm_upload into a lane whose submitted batch is still in flight");
     // validate everything before touching the lane; the lane holds no batch until this call has fully succeeded
-    long long need_xy = 0, need_yaw = 0;
-    for (int b = 0; b < B; b++) {
-        if (N[b] < 1 || M[b] < 1) return fail(UALM_EINVAL, "piece counts must be >= 1");
-        if (!(total_time[b] > 0.0) || !std::isfinite(total_time[b])) return fail(UALM_EINVAL, "total_time must be finite and > 0");
-        need_xy += 2LL * (N[b] - 1); need_yaw += M[b] - 1;
-    }
-    if ((need_xy > 0 && !inner_xy) || (need_yaw > 0 && !inner_yaw)) return fail(UALM_EINVAL, "inner waypoint arrays are NULL but N > 1 or M > 1");
+    BatchLayout lay;
+    if (int rc = batch_layout(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, &lay)) return rc;
+    if (lane_in_flight(c, c->cur)) return fail(UALM_ESTATE, "ualm_upload into a lane whose submitted batch is still in flight");
+    Lane *l = c->b;
     l->have_batch = false; l->solved = false;
+    l->batch = std::move(lay);
+    const BatchLayout &L = l->batch;
+    if (c->tp) TP_CALL(ualm_tp::tp_upload(c->tp, c->cur, L, bnd, total_time, err));
     CK(cudaSetDevice(c->device));
-    l->B = B; l->desc.assign(B, ProbDesc()); l->order.clear(); l->group.assign(B, 1); l->skip.assign(B, 0);
-    l->env.assign(B, 0);
-    if (env) l->env.assign(env, env + B);
-    l->Nmax = l->Mmax = l->nmax = l->Smax = 1;
+    l->desc.assign(B, ProbDesc()); l->order.clear(); l->group.assign(B, 1);
     for (int b = 0; b < B; b++) {
         ProbDesc &d = l->desc[b];
-        d.N = N[b]; d.M = M[b];
-        // compiled limits (n <= 256: the L-BFGS register tile, UALM_NREG in ualm_kernels.cuh): such a problem is not solved, its
-        // record says UALM_ELIMIT, and the rest of the batch runs
-        if (N[b] > UALM_NMAX || M[b] > UALM_MMAX) { l->skip[b] = 1; d.n = 0; d.S = 0; continue; }
-        d.n = 1 + 2 * (N[b] - 1) + (M[b] - 1); d.S = N[b] * (c->envs[l->env[b]].dp.int_K + 1);
-        l->Nmax = std::max(l->Nmax, d.N); l->Mmax = std::max(l->Mmax, d.M); l->nmax = std::max(l->nmax, d.n); l->Smax = std::max(l->Smax, d.S);
-        l->order.push_back(b);
+        d.N = L.N[b]; d.M = L.M[b]; d.n = L.n[b]; d.S = L.S[b];
+        if (!L.skip[b]) l->order.push_back(b);
     }
-    l->eidx.clear();
-    for (int e = 0; e < UALM_MAX_ENVS; e++) {
-        l->eoff[e] = (int)l->eidx.size();
-        for (int b = 0; b < B; b++) if (l->env[b] == e) l->eidx.push_back(b);
-    }
-    l->eoff[UALM_MAX_ENVS] = B;
-    l->n_active = (int)l->order.size();
-    const int BA = l->n_active;
+    const int BA = L.n_active;
     // launch order: most samples first (longest-processing-time-first keeps the tail short)
     std::stable_sort(l->order.begin(), l->order.end(), [&](int a, int b2) { return l->desc[a].S > l->desc[b2].S; });
     int rc0 = prepare_launch(c);
@@ -632,10 +681,10 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
             for (int gi = 0; gi < 3; gi++) {
                 const int G = gi == 0 ? 4 : gi == 1 ? 2 : 1;
                 if (lim[gi + 1] <= lim[gi]) continue;
-                std::stable_sort(ord.begin() + lim[gi], ord.begin() + lim[gi + 1], [&](int x, int y) { return l->env[x] < l->env[y]; });
+                std::stable_sort(ord.begin() + lim[gi], ord.begin() + lim[gi + 1], [&](int x, int y) { return L.env[x] < L.env[y]; });
                 for (long long a = lim[gi], b2; a < lim[gi + 1]; a = b2) {
-                    const int ce = l->env[ord[a]];
-                    for (b2 = a; b2 < lim[gi + 1] && l->env[ord[b2]] == ce; b2++) {}
+                    const int ce = L.env[ord[a]];
+                    for (b2 = a; b2 < lim[gi + 1] && L.env[ord[b2]] == ce; b2++) {}
                     const DevParams &ep = c->envs[ce].dp;
                     Lane::GClass cl;
                     cl.G = G; cl.env = ce; cl.r0 = (int)a; cl.r1 = (int)b2;
@@ -669,31 +718,25 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
                         cl.smem, cl.occ);
         }
     }
-    long long ox = 0, os = 0, ocx = 0, ocy = 0, oh = 0, oscr = 0, oixy = 0, oiyaw = 0, ofac = 0, ows = 0, oaux = 0;
-    std::vector<double> x0;
+    // the offsets of the parity path's own buffers (the layout has those of x, the samples and the coefficients)
+    long long oh = 0, oscr = 0, ofac = 0, ows = 0, oaux = 0;
     std::vector<ualm_result_t> res0(B);
     for (int b = 0; b < B; b++) {
         ProbDesc &d = l->desc[b];
-        const int m = c->envs[l->env[b]].dp.mem_size;
-        d.off_x = ox; d.off_s = os; d.off_cxy = ocx; d.off_cyaw = ocy; d.off_hist = oh; d.off_scr = oscr; d.off_fac = ofac; d.off_ws = ows;
+        const int m = c->envs[L.env[b]].dp.mem_size;
+        d.off_x = L.off_x[b]; d.off_s = L.off_s[b]; d.off_cxy = L.off_cxy[b]; d.off_cyaw = L.off_cyaw[b];
+        d.off_hist = oh; d.off_scr = oscr; d.off_fac = ofac; d.off_ws = ows;
         d.off_aux = oaux; oaux += 3LL * m;
         for (int k = 0; k < 18; k++) d.bnd[k] = bnd[(size_t)b * 18 + k];
         d.total_time = total_time[b];
         memset(&res0[b], 0, sizeof(ualm_result_t));
-        ocx += 12 * d.N; ocy += 6 * d.M;
-        const long long nxy = 2LL * (d.N - 1), nyw = d.M - 1;
-        if (l->skip[b]) { res0[b].ret_code = UALM_ELIMIT; oixy += nxy; oiyaw += nyw; continue; }
-        // x = [tau | Pxy | Pyaw]  (alm_traj_opt.cpp:205-216); logC2 (alm_traj_opt.h:238-241) is two IEEE ops + sqrt
-        const double T = total_time[b];
-        x0.push_back(T > 1.0 ? (std::sqrt(2.0 * T - 1.0) - 1.0) : (1.0 - std::sqrt(2.0 / T - 1.0)));
-        for (long long q = 0; q < nxy; q++) x0.push_back(inner_xy[oixy + q]);
-        for (long long q = 0; q < nyw; q++) x0.push_back(inner_yaw[oiyaw + q]);
-        oixy += nxy; oiyaw += nyw;
-        ox += d.n; os += d.S; oh += (long long)m * d.n; oscr += (long long)UALM_NFIELD * d.S;
+        if (L.skip[b]) { res0[b].ret_code = UALM_ELIMIT; continue; }
+        oh += (long long)m * d.n; oscr += (long long)UALM_NFIELD * d.S;
         ofac += 1LL * UALM_FW * ((6 * d.N + 2 * UALM_FPAD) + (6 * d.M + 2 * UALM_FPAD));
         ows += (long long)(12 * d.N + 6 * d.M) * 32 * l->group[b];
     }
-    l->tot_x = ox; l->tot_s = os; l->tot_cxy = ocx; l->tot_cyaw = ocy; l->tot_hist = oh; l->tot_scr = oscr; l->tot_fac = ofac; l->tot_ws = ows;
+    l->tot_hist = oh; l->tot_scr = oscr; l->tot_fac = ofac; l->tot_ws = ows;
+    const long long ox = L.tot_x, os = L.tot_s, ocx = L.tot_cxy, ocy = L.tot_cyaw;
     CK(l->d_desc.ensure(B)); CK(l->d_order.ensure(BA)); CK(l->d_queue.ensure(std::max<size_t>(l->cls.size(), 1))); CK(l->d_x0.ensure(ox)); CK(l->d_x.ensure(ox)); CK(l->d_grad.ensure(ox));
     CK(l->d_lambda.ensure(os)); CK(l->d_hx.ensure(os)); CK(l->d_mu.ensure(6 * os)); CK(l->d_gx.ensure(6 * os)); CK(l->d_scale_cx.ensure(7 * os));
     CK(l->d_lm_s.ensure(oh)); CK(l->d_lm_y.ensure(oh)); CK(l->d_scr.ensure(oscr));
@@ -708,8 +751,8 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
     if (B > 0) {
         CK(cudaMemcpyAsync(l->d_desc.p, l->desc.data(), sizeof(ProbDesc) * B, cudaMemcpyHostToDevice, l->stream));
         if (BA > 0) CK(cudaMemcpyAsync(l->d_order.p, l->order.data(), sizeof(int) * BA, cudaMemcpyHostToDevice, l->stream));
-        CK(cudaMemcpyAsync(l->d_eidx.p, l->eidx.data(), sizeof(int) * B, cudaMemcpyHostToDevice, l->stream));
-        if (ox > 0) CK(cudaMemcpyAsync(l->d_x0.p, x0.data(), sizeof(double) * ox, cudaMemcpyHostToDevice, l->stream));
+        CK(cudaMemcpyAsync(l->d_eidx.p, L.eidx.data(), sizeof(int) * B, cudaMemcpyHostToDevice, l->stream));
+        if (ox > 0) CK(cudaMemcpyAsync(l->d_x0.p, L.x0.data(), sizeof(double) * ox, cudaMemcpyHostToDevice, l->stream));
         // records of skipped problems (the kernels overwrite the others), zero coefficients and durations for them
         CK(cudaMemcpyAsync(l->d_res.p, res0.data(), sizeof(ualm_result_t) * B, cudaMemcpyHostToDevice, l->stream));
         if (BA < B) {
@@ -717,7 +760,7 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
             CK(cudaMemsetAsync(l->d_cyaw.p, 0, sizeof(double) * ocy, l->stream));
             CK(cudaMemsetAsync(l->d_pieceT.p, 0, sizeof(double) * 2 * B, l->stream));
         }
-        CK(cudaStreamSynchronize(l->stream)); // x0 / res0 are stack-local staging vectors
+        CK(cudaStreamSynchronize(l->stream)); // res0 is a stack-local staging vector
     }
     l->have_batch = true; l->solved = false;
     return UALM_OK;
@@ -727,20 +770,18 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
 static int solve_launch(ualm_ctx *c, bool publish)
 {
     Lane *l = c->b;
-    // (the upload checked that every environment of the batch is bound, and nothing unbinds one)
     if (!l->have_batch) return fail(UALM_ESTATE, "set_params, set_map and upload must precede solve");
+    if (int rc = check_envs(c, l->batch)) return rc;
     CK(cudaSetDevice(c->device));
-    unsigned mask = 0;
-    for (int e = 0; e < UALM_MAX_ENVS; e++) if (l->eoff[e + 1] > l->eoff[e]) mask |= 1u << e;
-    if (int rc = lane_hold(c, *l, mask)) return rc;
+    if (int rc = lane_hold(c, *l)) return rc;
     l->last_launches = 0;
     // no stop request carries over: the words are cleared before the solve, and raises are queued after ev_clear
     if (l->h_stop) memset(l->h_stop, 0, sizeof(int) * l->h_stop_cap);
-    CK(cudaMemsetAsync(l->d_stop.p, 0, sizeof(int) * std::max(l->B, 1), l->stream));
+    CK(cudaMemsetAsync(l->d_stop.p, 0, sizeof(int) * std::max(l->batch.B, 1), l->stream));
     CK(cudaEventRecord(l->ev_clear, l->stream));
     if (!l->cls.empty()) CK(cudaMemsetAsync(l->d_queue.p, 0, sizeof(int) * l->cls.size(), l->stream));   // every launch's queue full
     CK(cudaEventRecord(l->ev0, l->stream));
-    if (l->n_active > 0) {
+    if (l->batch.n_active > 0) {
         // the launches run concurrently: launch 0 on the lane stream, the others on auxiliary streams
         const int last = Lane::NAUX;
         CK(cudaEventRecord(l->evs[last], l->stream));
@@ -775,9 +816,10 @@ extern "C" int ualm_solve_resident(ualm_ctx_t *c)
 {
     if (!c) return fail(UALM_EINVAL, "null ctx");
     if (c->tp) {     // joins the pool of running trajectories; its rounds run on the device, ualm_sync waits
+        if (int rc = check_envs(c, c->b->batch)) return rc;
         std::string em;
         if (int rc = ualm_tp::tp_admit(c->tp, c->cur, &em)) return fail(rc, em);
-        return lane_hold(c, c->lanes[c->cur], ualm_tp::tp_lane_env_mask(c->tp, c->cur));
+        return lane_hold(c, *c->b);
     }
     return solve_launch(c, false);
 }
@@ -837,11 +879,12 @@ extern "C" int ualm_download(ualm_ctx_t *c, ualm_result_t *results, double *c_xy
     }
     if (!c || !c->b->solved) return fail(UALM_ESTATE, "nothing solved");
     Lane *l = c->b;
+    const BatchLayout &L = l->batch;
     CK(cudaSetDevice(c->device));
-    if (l->B > 0) {
-        if (results) CK(cudaMemcpyAsync(results, l->d_res.p, sizeof(ualm_result_t) * l->B, cudaMemcpyDeviceToHost, l->stream));
-        if (c_xy) CK(cudaMemcpyAsync(c_xy, l->d_cxy.p, sizeof(double) * l->tot_cxy, cudaMemcpyDeviceToHost, l->stream));
-        if (c_yaw) CK(cudaMemcpyAsync(c_yaw, l->d_cyaw.p, sizeof(double) * l->tot_cyaw, cudaMemcpyDeviceToHost, l->stream));
+    if (L.B > 0) {
+        if (results) CK(cudaMemcpyAsync(results, l->d_res.p, sizeof(ualm_result_t) * L.B, cudaMemcpyDeviceToHost, l->stream));
+        if (c_xy) CK(cudaMemcpyAsync(c_xy, l->d_cxy.p, sizeof(double) * L.tot_cxy, cudaMemcpyDeviceToHost, l->stream));
+        if (c_yaw) CK(cudaMemcpyAsync(c_yaw, l->d_cyaw.p, sizeof(double) * L.tot_cyaw, cudaMemcpyDeviceToHost, l->stream));
     }
     CK(cudaStreamSynchronize(l->stream));
     return UALM_OK;
@@ -876,24 +919,17 @@ extern "C" int ualm_submit_batch_env(ualm_ctx_t *c, int B, const int32_t *N, con
     if (!c || !ticket) return fail(UALM_EINVAL, "null argument");
     if (depth < 1 || depth > UALM_MAX_LANES) return fail(UALM_EINVAL, "depth out of range [1, UALM_MAX_LANES]");
     const int lane = c->next_submit % depth;
-    if (c->tp) {
-        if (ualm_tp::tp_lane_in_flight(c->tp, lane)) return fail(UALM_ESTATE, "all lanes of this depth are in flight: ualm_wait_batch the oldest ticket first");
-        if (B < 0 || (B > 0 && (!N || !M || !bnd || !total_time))) return fail(UALM_EINVAL, "bad argument");
-        if (int rc = check_envs(c, B, env)) return rc;
-        std::string em;
-        int rc = ualm_tp::tp_upload(c->tp, lane, B, N, M, env, bnd, total_time, inner_xy, inner_yaw, &em);
-        if (!rc) rc = ualm_tp::tp_admit(c->tp, lane, &em, true);
-        if (rc) return fail(rc, em);
-        *ticket = lane; c->next_submit = (lane + 1) % depth;
-        return lane_hold(c, c->lanes[lane], ualm_tp::tp_lane_env_mask(c->tp, lane));
-    }
-    if (c->lanes[lane].in_flight) return fail(UALM_ESTATE, "all lanes of this depth are in flight: ualm_wait_batch the oldest ticket first");
+    if (lane_in_flight(c, lane)) return fail(UALM_ESTATE, "all lanes of this depth are in flight: ualm_wait_batch the oldest ticket first");
     const int keep = c->cur;
     int rc = ualm_select_lane(c, lane);
     if (!rc) rc = ualm_upload_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env);
-    if (!rc) {
-        Lane &l = c->lanes[lane];
-        cudaError_t e = l.mbox.begin(B, N, M, l.skip.data());
+    Lane &l = c->lanes[lane];
+    if (!rc && c->tp) {
+        std::string em;
+        rc = ualm_tp::tp_admit(c->tp, lane, &em, true);
+        rc = rc ? fail(rc, em) : lane_hold(c, l);
+    } else if (!rc) {
+        cudaError_t e = l.mbox.begin(B, N, M, l.batch.skip.data());
         if (e != cudaSuccess) rc = fail(UALM_ENOCUDA, std::string("result mailbox: ") + cudaGetErrorString(e));
         if (!rc && l.h_stop_cap < (size_t)std::max(B, 1)) {      // the stop words' host mirror (solve_launch clears it)
             if (l.h_stop) cudaFreeHost(l.h_stop);
@@ -902,9 +938,10 @@ extern "C" int ualm_submit_batch_env(ualm_ctx_t *c, int B, const int32_t *N, con
             if (e != cudaSuccess) rc = fail(UALM_ENOCUDA, std::string("stop words: ") + cudaGetErrorString(e));
             else l.h_stop_cap = (size_t)std::max(B, 1);
         }
+        if (!rc) rc = solve_launch(c, true);
+        if (!rc) l.in_flight = true;
     }
-    if (!rc) rc = solve_launch(c, true);
-    if (!rc) { c->lanes[lane].in_flight = true; *ticket = lane; c->next_submit = (lane + 1) % depth; }
+    if (!rc) { *ticket = lane; c->next_submit = (lane + 1) % depth; }
     c->cur = keep; c->b = &c->lanes[keep];
     return rc;
 }
@@ -934,11 +971,12 @@ extern "C" int ualm_wait_batch(ualm_ctx_t *c, int ticket, ualm_result_t *results
 // mirror on the cancel stream, ordered after the clear of the lane's current batch
 static int raise_stop(ualm_ctx *c, Lane &l, int n, const int32_t *idx)
 {
+    const int B = l.batch.B;
     if (idx) for (int k = 0; k < n; k++) l.h_stop[idx[k]] = 1;
-    else for (int b = 0; b < l.B; b++) l.h_stop[b] = 1;
-    if (l.B == 0) return UALM_OK;
+    else for (int b = 0; b < B; b++) l.h_stop[b] = 1;
+    if (B == 0) return UALM_OK;
     CK(cudaStreamWaitEvent(c->cancel, l.ev_clear, 0));
-    CK(cudaMemcpyAsync(l.d_stop.p, l.h_stop, sizeof(int) * l.B, cudaMemcpyHostToDevice, c->cancel));
+    CK(cudaMemcpyAsync(l.d_stop.p, l.h_stop, sizeof(int) * B, cudaMemcpyHostToDevice, c->cancel));
     l.raised = true;
     return UALM_OK;
 }
@@ -1012,7 +1050,7 @@ extern "C" int ualm_cancel_problems(ualm_ctx_t *c, int ticket, int n, const int3
     Lane &l = c->lanes[ticket];
     if (!l.in_flight) return fail(UALM_ESTATE, "ticket is not in flight");
     for (int k = 0; k < n; k++)
-        if (idx[k] < 0 || idx[k] >= l.B) return fail(UALM_EINVAL, "problem index out of range [0, B)");
+        if (idx[k] < 0 || idx[k] >= l.batch.B) return fail(UALM_EINVAL, "problem index out of range [0, B)");
     if (n == 0) return UALM_OK;
     CK(cudaSetDevice(c->device));
     return raise_stop(c, l, n, idx);
@@ -1022,8 +1060,8 @@ extern "C" int ualm_set_budget(ualm_ctx_t *c, int32_t max_evals)
 {
     if (!c) return fail(UALM_EINVAL, "null ctx");
     if (max_evals < 0) return fail(UALM_EINVAL, "max_evals must be >= 0 (0 = no budget)");
-    if (c->tp) TP_CALL(ualm_tp::tp_set_budget(c->tp, max_evals, err));
     if (int rc = lanes_idle(c, "ualm_set_budget")) return rc;
+    if (c->tp) ualm_tp::tp_set_budget(c->tp, max_evals);
     c->max_evals = max_evals;
     return UALM_OK;
 }
@@ -1046,13 +1084,11 @@ extern "C" int ualm_solve_batch_multi_env(ualm_ctx_t **ctxs, int nctx, int B, co
     for (int r = 0; r < nctx; r++) if (!ctxs[r]) return fail(UALM_EINVAL, "null ctx in list");
     if (B == 0) return UALM_OK;
     if (!N || !M || !bnd || !total_time) return fail(UALM_EINVAL, "null argument");
-    for (int r = 0; r < nctx; r++) if (int rc = check_envs(ctxs[r], B, env)) return rc;
-    std::vector<long long> oxy(B + 1, 0), oyw(B + 1, 0), ocx(B + 1, 0), ocy(B + 1, 0);
-    for (int b = 0; b < B; b++) {
-        if (N[b] < 1 || M[b] < 1) return fail(UALM_EINVAL, "piece counts must be >= 1");
-        oxy[b + 1] = oxy[b] + 2LL * (N[b] - 1); oyw[b + 1] = oyw[b] + (M[b] - 1);
-        ocx[b + 1] = ocx[b] + 12LL * N[b]; ocy[b + 1] = ocy[b] + 6LL * M[b];
-    }
+    BatchLayout L;       // checked against ctxs[0], the coefficient offsets of the whole batch
+    if (int rc = batch_layout(ctxs[0], B, N, M, bnd, total_time, inner_xy, inner_yaw, env, &L)) return rc;
+    for (int r = 1; r < nctx; r++) if (int rc = check_envs(ctxs[r], B, env)) return rc;
+    std::vector<long long> oxy(B + 1, 0), oyw(B + 1, 0);
+    for (int b = 0; b < B; b++) { oxy[b + 1] = oxy[b] + 2LL * (N[b] - 1); oyw[b + 1] = oyw[b] + (M[b] - 1); }
     std::vector<int> ord(B);
     std::iota(ord.begin(), ord.end(), 0);
     std::stable_sort(ord.begin(), ord.end(), [&](int a, int b2) { return N[a] > N[b2]; });
@@ -1094,8 +1130,8 @@ extern "C" int ualm_solve_batch_multi_env(ualm_ctx_t **ctxs, int nctx, int B, co
         for (size_t q = 0; q < shard[r].size(); q++) {
             const int b = shard[r][q];
             if (results) results[b] = sub[r].res[q];
-            if (c_xy) memcpy(c_xy + ocx[b], sub[r].cxy.data() + px, sizeof(double) * 12 * N[b]);
-            if (c_yaw) memcpy(c_yaw + ocy[b], sub[r].cyw.data() + py, sizeof(double) * 6 * M[b]);
+            if (c_xy) memcpy(c_xy + L.off_cxy[b], sub[r].cxy.data() + px, sizeof(double) * 12 * N[b]);
+            if (c_yaw) memcpy(c_yaw + L.off_cyaw[b], sub[r].cyw.data() + py, sizeof(double) * 6 * M[b]);
             px += 12LL * N[b]; py += 6LL * M[b];
         }
     }
@@ -1110,10 +1146,10 @@ extern "C" int ualm_pack_records_device(ualm_ctx_t *c, double *d_records, int st
     }
     if (!c || !c->b->solved || !d_records) return fail(UALM_ESTATE, "nothing solved / null buffer");
     Lane *l = c->b;
-    if (stride < 12 + 12 * l->Nmax + 6 * l->Mmax) return fail(UALM_EINVAL, "record stride too small");
+    if (stride < 12 + 12 * l->batch.Nmax + 6 * l->batch.Mmax) return fail(UALM_EINVAL, "record stride too small");
     CK(cudaSetDevice(c->device));
-    if (l->B > 0) {
-        pack_records_kernel<<<l->B, 128, 0, l->stream>>>(batch_ptrs(c), l->B, d_records, stride);
+    if (l->batch.B > 0) {
+        pack_records_kernel<<<l->batch.B, 128, 0, l->stream>>>(batch_ptrs(c), l->batch.B, d_records, stride);
         CK(cudaGetLastError());
     }
     CK(cudaStreamSynchronize(l->stream));
@@ -1125,10 +1161,10 @@ extern "C" int ualm_pack_records_device_async(ualm_ctx_t *c, double *d_records, 
     if (c && c->tp) return ualm_pack_records_device(c, d_records, stride);     // the engine gathers a batch only once it is complete
     if (!c || !c->b->solved || !d_records) return fail(UALM_ESTATE, "nothing solved / null buffer");
     Lane *l = c->b;
-    if (stride < 12 + 12 * l->Nmax + 6 * l->Mmax) return fail(UALM_EINVAL, "record stride too small");
+    if (stride < 12 + 12 * l->batch.Nmax + 6 * l->batch.Mmax) return fail(UALM_EINVAL, "record stride too small");
     CK(cudaSetDevice(c->device));
-    if (l->B > 0) {
-        pack_records_kernel<<<l->B, 128, 0, l->stream>>>(batch_ptrs(c), l->B, d_records, stride);
+    if (l->batch.B > 0) {
+        pack_records_kernel<<<l->batch.B, 128, 0, l->stream>>>(batch_ptrs(c), l->batch.B, d_records, stride);
         CK(cudaGetLastError());
     }
     return UALM_OK;
@@ -1154,32 +1190,33 @@ extern "C" int ualm_eval_batch(ualm_ctx_t *c, const double *x, const double *lam
     if (c && c->tp) TP_CALL(ualm_tp::tp_eval(c->tp, c->cur, x, lambda, mu, scale_cx, scale_fx, rho, f, grad, hx, gx, c_xy, c_yaw, err));
     if (!c || !c->b->have_batch) return fail(UALM_ESTATE, "upload and set_map first");
     Lane *l = c->b;
-    if (l->n_active != l->B) return fail(UALM_ELIMIT, "ualm_eval_batch: the uploaded batch holds problems over the compiled limits");
+    const BatchLayout &L = l->batch;
+    if (L.n_active != L.B) return fail(UALM_ELIMIT, "ualm_eval_batch: the uploaded batch holds problems over the compiled limits");
     CK(cudaSetDevice(c->device));
     int rc;
     // the evaluation point goes to its own buffer: d_x0 keeps the uploaded initial guesses, which ualm_init_scaling_batch and a
     // later solve of the resident batch start from
     if (x) {
-        CK(l->d_xev.ensure(l->tot_x));
-        if ((rc = put(c, l->d_xev.p, x, l->tot_x, 0.0))) return rc;
+        CK(l->d_xev.ensure(L.tot_x));
+        if ((rc = put(c, l->d_xev.p, x, L.tot_x, 0.0))) return rc;
     }
-    if ((rc = put(c, l->d_lambda.p, lambda, l->tot_s, 0.0))) return rc;
-    if ((rc = put(c, l->d_mu.p, mu, 6 * l->tot_s, 0.0))) return rc;
-    if ((rc = put(c, l->d_scale_cx.p, scale_cx, 7 * l->tot_s, 1.0))) return rc;
-    if ((rc = put(c, l->d_sfx.p, scale_fx, l->B, 1.0))) return rc;
-    if (l->B > 0) {
+    if ((rc = put(c, l->d_lambda.p, lambda, L.tot_s, 0.0))) return rc;
+    if ((rc = put(c, l->d_mu.p, mu, 6 * L.tot_s, 0.0))) return rc;
+    if ((rc = put(c, l->d_scale_cx.p, scale_cx, 7 * L.tot_s, 1.0))) return rc;
+    if ((rc = put(c, l->d_sfx.p, scale_fx, L.B, 1.0))) return rc;
+    if (L.B > 0) {
         if ((rc = per_env(c, [&](int e, const BatchPtrs &bp, int cnt) {
                  BatchPtrs be = bp;
                  if (x) be.x0 = l->d_xev.p;
                  eval_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(be, c->envs[e].dp, c->envs[e].map->dm, l->eL[e], rho);
              })))
             return rc;
-        if (f) CK(cudaMemcpyAsync(f, l->d_f.p, sizeof(double) * l->B, cudaMemcpyDeviceToHost, l->stream));
-        if (grad) CK(cudaMemcpyAsync(grad, l->d_grad.p, sizeof(double) * l->tot_x, cudaMemcpyDeviceToHost, l->stream));
-        if (hx) CK(cudaMemcpyAsync(hx, l->d_hx.p, sizeof(double) * l->tot_s, cudaMemcpyDeviceToHost, l->stream));
-        if (gx) CK(cudaMemcpyAsync(gx, l->d_gx.p, sizeof(double) * 6 * l->tot_s, cudaMemcpyDeviceToHost, l->stream));
-        if (c_xy) CK(cudaMemcpyAsync(c_xy, l->d_cxy.p, sizeof(double) * l->tot_cxy, cudaMemcpyDeviceToHost, l->stream));
-        if (c_yaw) CK(cudaMemcpyAsync(c_yaw, l->d_cyaw.p, sizeof(double) * l->tot_cyaw, cudaMemcpyDeviceToHost, l->stream));
+        if (f) CK(cudaMemcpyAsync(f, l->d_f.p, sizeof(double) * L.B, cudaMemcpyDeviceToHost, l->stream));
+        if (grad) CK(cudaMemcpyAsync(grad, l->d_grad.p, sizeof(double) * L.tot_x, cudaMemcpyDeviceToHost, l->stream));
+        if (hx) CK(cudaMemcpyAsync(hx, l->d_hx.p, sizeof(double) * L.tot_s, cudaMemcpyDeviceToHost, l->stream));
+        if (gx) CK(cudaMemcpyAsync(gx, l->d_gx.p, sizeof(double) * 6 * L.tot_s, cudaMemcpyDeviceToHost, l->stream));
+        if (c_xy) CK(cudaMemcpyAsync(c_xy, l->d_cxy.p, sizeof(double) * L.tot_cxy, cudaMemcpyDeviceToHost, l->stream));
+        if (c_yaw) CK(cudaMemcpyAsync(c_yaw, l->d_cyaw.p, sizeof(double) * L.tot_cyaw, cudaMemcpyDeviceToHost, l->stream));
     }
     CK(cudaStreamSynchronize(l->stream));
     return UALM_OK;
@@ -1190,15 +1227,16 @@ extern "C" int ualm_init_scaling_batch(ualm_ctx_t *c, double *scale_fx, double *
     if (c && c->tp) TP_CALL(ualm_tp::tp_init_scaling(c->tp, c->cur, scale_fx, scale_cx, err));
     if (!c || !c->b->have_batch) return fail(UALM_ESTATE, "upload and set_map first");
     Lane *l = c->b;
-    if (l->n_active != l->B) return fail(UALM_ELIMIT, "ualm_init_scaling_batch: the uploaded batch holds problems over the compiled limits");
+    const BatchLayout &L = l->batch;
+    if (L.n_active != L.B) return fail(UALM_ELIMIT, "ualm_init_scaling_batch: the uploaded batch holds problems over the compiled limits");
     CK(cudaSetDevice(c->device));
-    if (l->B > 0) {
+    if (L.B > 0) {
         if (int rc = per_env(c, [&](int e, const BatchPtrs &bp, int cnt) {
                 scaling_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].map->dm, l->eL[e]);
             }))
             return rc;
-        if (scale_fx) CK(cudaMemcpyAsync(scale_fx, l->d_sfx.p, sizeof(double) * l->B, cudaMemcpyDeviceToHost, l->stream));
-        if (scale_cx) CK(cudaMemcpyAsync(scale_cx, l->d_scale_cx.p, sizeof(double) * 7 * l->tot_s, cudaMemcpyDeviceToHost, l->stream));
+        if (scale_fx) CK(cudaMemcpyAsync(scale_fx, l->d_sfx.p, sizeof(double) * L.B, cudaMemcpyDeviceToHost, l->stream));
+        if (scale_cx) CK(cudaMemcpyAsync(scale_cx, l->d_scale_cx.p, sizeof(double) * 7 * L.tot_s, cudaMemcpyDeviceToHost, l->stream));
     }
     CK(cudaStreamSynchronize(l->stream));
     return UALM_OK;
@@ -1210,22 +1248,22 @@ extern "C" int ualm_time_penalty_kernel(ualm_ctx_t *c, int reps, float *ms_per_l
     if (c && c->tp) TP_CALL(ualm_tp::tp_time_penalty(c->tp, c->cur, reps, (getenv("UALM_TP_TMA") && atoi(getenv("UALM_TP_TMA"))) ? 1 : 0, ms_per_launch, algorithmic_bytes, err));
     if (!c || !c->b->have_batch) return fail(UALM_ESTATE, "upload and set_map first");
     Lane *l = c->b;
-    if (l->n_active != l->B) return fail(UALM_ELIMIT, "ualm_time_penalty_kernel: the uploaded batch holds problems over the compiled limits");
-    for (int b = 1; b < l->B; b++)
-        if (l->env[b] != l->env[0]) return fail(UALM_EINVAL, "ualm_time_penalty_kernel: the uploaded batch mixes environments");
+    const BatchLayout &L = l->batch;
+    if (L.n_active != L.B) return fail(UALM_ELIMIT, "ualm_time_penalty_kernel: the uploaded batch holds problems over the compiled limits");
+    if (L.mixed()) return fail(UALM_EINVAL, "ualm_time_penalty_kernel: the uploaded batch mixes environments");
     if (ms_per_launch) *ms_per_launch = 0.f;
     if (algorithmic_bytes) *algorithmic_bytes = 0.0;
-    if (l->B == 0) return UALM_OK;
+    if (L.B == 0) return UALM_OK;
     CK(cudaSetDevice(c->device));
     int rc;
-    if ((rc = put(c, l->d_lambda.p, nullptr, l->tot_s, 0.0))) return rc;
-    if ((rc = put(c, l->d_mu.p, nullptr, 6 * l->tot_s, 0.0))) return rc;
-    if ((rc = put(c, l->d_scale_cx.p, nullptr, 7 * l->tot_s, 1.0))) return rc;
-    const int e = l->env[0];
+    if ((rc = put(c, l->d_lambda.p, nullptr, L.tot_s, 0.0))) return rc;
+    if ((rc = put(c, l->d_mu.p, nullptr, 6 * L.tot_s, 0.0))) return rc;
+    if ((rc = put(c, l->d_scale_cx.p, nullptr, 7 * L.tot_s, 1.0))) return rc;
+    const int e = L.env[0];
     const BatchPtrs bp = batch_ptrs(c);
-    penalty_only_kernel<<<(l->B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].map->dm, l->eL[e], 1); // warm-up
+    penalty_only_kernel<<<(L.B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].map->dm, l->eL[e], 1); // warm-up
     CK(cudaEventRecord(l->ev0, l->stream));
-    penalty_only_kernel<<<(l->B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].map->dm, l->eL[e], reps);
+    penalty_only_kernel<<<(L.B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].map->dm, l->eL[e], reps);
     CK(cudaEventRecord(l->ev1, l->stream));
     CK(cudaGetLastError());
     CK(cudaEventSynchronize(l->ev1));
@@ -1249,15 +1287,15 @@ extern "C" int ualm_profile(ualm_ctx_t *c, int enable, long long *out16)
     if (c->tp) TP_UNSUPPORTED("ualm_profile");
     Lane *l = c->b;
     CK(cudaSetDevice(c->device));
-    if (out16 && c->profile && l->solved && l->B > 0) {
-        std::vector<long long> h((size_t)l->B * UALM_NPROF);
+    if (out16 && c->profile && l->solved && l->batch.B > 0) {
+        std::vector<long long> h((size_t)l->batch.B * UALM_NPROF);
         CK(cudaMemcpyAsync(h.data(), l->d_prof.p, h.size() * sizeof(long long), cudaMemcpyDeviceToHost, l->stream));
         CK(cudaStreamSynchronize(l->stream));
         if (enable == 2) { // raw: out16 has room for B x 16 values, rows in problem order
             for (size_t q = 0; q < h.size(); q++) out16[q] = h[q];
         } else {
             for (int q = 0; q < UALM_NPROF; q++) out16[q] = 0;
-            for (int b = 0; b < l->B; b++) if (!l->skip[b]) for (int q = 0; q < UALM_NPROF; q++) out16[q] += h[(size_t)b * UALM_NPROF + q];
+            for (int b = 0; b < l->batch.B; b++) if (!l->batch.skip[b]) for (int q = 0; q < UALM_NPROF; q++) out16[q] += h[(size_t)b * UALM_NPROF + q];
         }
     }
     c->profile = enable != 0;
@@ -1272,82 +1310,91 @@ __global__ void piece_T_from_results(const ualm_result_t *res, int B, double *pi
 }
 } // namespace ualm
 
-// feasibility_kernel over a batch whose problem b is in environment env[b]: one launch with that environment's parameters and the grid
-// version maps[env[b]] the batch was solved on when there is only one environment, else one launch per environment over its problem indices
-static int feasibility_launch(ualm_ctx *c, const BatchPtrs &bp, int B, const int32_t *env, const MapRef *maps, double dt, double *d_out, cudaStream_t st)
+// descriptors of a scan over B trajectories of N[b] / M[b] pieces whose coefficients are packed in problem order; S == 0 marks a problem
+// over the compiled limits, which is not scanned
+static std::vector<ProbDesc> scan_descs(int B, const int32_t *N, const int32_t *M)
 {
-    bool mixed = false;
-    for (int b = 1; b < B; b++) mixed = mixed || env[b] != env[0];
-    for (int b = 0; b < B; b++)
-        if (!maps[env[b]]) return fail(UALM_ESTATE, "ualm_feasibility_batch: the batch was not solved by a launch of this context");
-    if (!mixed) {
-        const int e = B > 0 ? env[0] : 0;
-        feasibility_kernel<<<(B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(bp, c->envs[e].dp, maps[e]->dm, dt, d_out, nullptr, B);
-        CK(cudaGetLastError());
-        return UALM_OK;
-    }
-    struct Tmp { DevBuf<int> idx; ~Tmp() { idx.release(); } } t;
-    std::vector<int> idx;
-    int off[UALM_MAX_ENVS + 1];
-    for (int e = 0; e < UALM_MAX_ENVS; e++) {
-        off[e] = (int)idx.size();
-        for (int b = 0; b < B; b++) if (env[b] == e) idx.push_back(b);
-    }
-    off[UALM_MAX_ENVS] = (int)idx.size();
-    CK(t.idx.ensure(idx.size()));
-    CK(cudaMemcpyAsync(t.idx.p, idx.data(), sizeof(int) * idx.size(), cudaMemcpyHostToDevice, st));
-    for (int e = 0; e < UALM_MAX_ENVS; e++) {
-        const int cnt = off[e + 1] - off[e];
-        if (cnt == 0) continue;
-        feasibility_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(bp, c->envs[e].dp, maps[e]->dm, dt, d_out, t.idx.p + off[e], cnt);
-        CK(cudaGetLastError());
-    }
-    CK(cudaStreamSynchronize(st));       // idx and its device copy are local
-    return UALM_OK;
-}
-
-// the scan over coefficients that already sit on the device (B problems, ragged offsets from N / M, piece durations from the records)
-static int feasibility_from_device(ualm_ctx *c, int B, const int32_t *N, const int32_t *M, const int32_t *env, const MapRef *maps, const ualm_result_t *d_res,
-                                   const double *d_cxy, const double *d_cyaw, double dt, double *out10)
-{
-    struct Tmp { DevBuf<ProbDesc> desc; DevBuf<double> pt, feas; ~Tmp() { desc.release(); pt.release(); feas.release(); } } t;
     std::vector<ProbDesc> desc(B);
     long long ocx = 0, ocy = 0;
     for (int b = 0; b < B; b++) {
         memset(&desc[b], 0, sizeof(ProbDesc));
         desc[b].N = N[b]; desc[b].M = M[b]; desc[b].off_cxy = ocx; desc[b].off_cyaw = ocy;
-        desc[b].S = (N[b] > UALM_NMAX || M[b] > UALM_MMAX) ? 0 : 1;      // S == 0 marks a problem that was not solved
+        desc[b].S = over_limits(N[b], M[b]) ? 0 : 1;
         ocx += 12LL * N[b]; ocy += 6LL * M[b];
     }
-    CK(t.desc.ensure(B)); CK(t.pt.ensure(2 * (size_t)B)); CK(t.feas.ensure(10 * (size_t)B));
-    CK(cudaMemcpy(t.desc.p, desc.data(), sizeof(ProbDesc) * B, cudaMemcpyHostToDevice));
-    piece_T_from_results<<<(B + 127) / 128, 128>>>(d_res, B, t.pt.p);
+    return desc;
+}
+
+// a collected throughput batch as the BatchPtrs of the scans (feasibility, MPC export): descriptors of the lane's layout and piece
+// durations from the records, in device buffers this object owns
+struct TpScan {
+    DevBuf<ProbDesc> desc;
+    DevBuf<double> pt, feas;
     BatchPtrs bp;
-    memset(&bp, 0, sizeof(bp));
-    bp.B = B; bp.desc = t.desc.p; bp.c_xy = const_cast<double *>(d_cxy); bp.c_yaw = const_cast<double *>(d_cyaw); bp.piece_T = t.pt.p;
-    if (int rc = feasibility_launch(c, bp, B, env, maps, dt, t.feas.p, 0)) return rc;
-    CK(cudaMemcpy(out10, t.feas.p, sizeof(double) * 10 * B, cudaMemcpyDeviceToHost));
+    ~TpScan() { desc.release(); pt.release(); feas.release(); }
+};
+// what: the entry point, for the refusal of a lane with no collected batch
+static int tp_scan(ualm_ctx *c, const char *what, TpScan &s)
+{
+    const ualm_result_t *d_res; const double *d_cxy, *d_cyaw;
+    if (ualm_tp::tp_lane_outputs(c->tp, c->cur, &d_res, &d_cxy, &d_cyaw) != UALM_OK)
+        return fail(UALM_ESTATE, std::string(what) + " needs a solved, collected batch (ualm_sync / ualm_download first)");
+    CK(cudaSetDevice(c->device));
+    const BatchLayout &L = c->b->batch;
+    if (L.B == 0) return UALM_OK;
+    const std::vector<ProbDesc> desc = scan_descs(L.B, L.N.data(), L.M.data());
+    CK(s.desc.ensure(L.B)); CK(s.pt.ensure(2 * (size_t)L.B));
+    CK(cudaMemcpy(s.desc.p, desc.data(), sizeof(ProbDesc) * L.B, cudaMemcpyHostToDevice));
+    piece_T_from_results<<<(L.B + 127) / 128, 128>>>(d_res, L.B, s.pt.p);
+    memset(&s.bp, 0, sizeof(s.bp));
+    s.bp.B = L.B; s.bp.desc = s.desc.p; s.bp.c_xy = const_cast<double *>(d_cxy); s.bp.c_yaw = const_cast<double *>(d_cyaw); s.bp.piece_T = s.pt.p;
+    return UALM_OK;
+}
+
+// feasibility_kernel over the lane's batch: one launch with the parameters of its environment and the grid version maps[e] the batch
+// was solved on when there is only one environment, else one launch per environment over its problem indices
+static int feasibility_launch(ualm_ctx *c, const BatchPtrs &bp, const BatchLayout &L, const MapRef *maps, double dt, double *d_out, cudaStream_t st)
+{
+    for (int e = 0; e < UALM_MAX_ENVS; e++)
+        if (((L.env_mask >> e) & 1u) && !maps[e]) return fail(UALM_ESTATE, "ualm_feasibility_batch: the batch was not solved by a launch of this context");
+    if (!L.mixed()) {
+        const int e = L.env[0];
+        feasibility_kernel<<<(L.B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(bp, c->envs[e].dp, maps[e]->dm, dt, d_out, nullptr, L.B);
+        CK(cudaGetLastError());
+        return UALM_OK;
+    }
+    struct Tmp { DevBuf<int> idx; ~Tmp() { idx.release(); } } t;
+    CK(t.idx.ensure(L.B));
+    CK(cudaMemcpyAsync(t.idx.p, L.eidx.data(), sizeof(int) * L.B, cudaMemcpyHostToDevice, st));
+    for (int e = 0; e < UALM_MAX_ENVS; e++) {
+        const int cnt = L.eoff[e + 1] - L.eoff[e];
+        if (cnt == 0) continue;
+        feasibility_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(bp, c->envs[e].dp, maps[e]->dm, dt, d_out, t.idx.p + L.eoff[e], cnt);
+        CK(cudaGetLastError());
+    }
+    CK(cudaStreamSynchronize(st));       // the device copy of the indices is local
     return UALM_OK;
 }
 
 extern "C" int ualm_feasibility_batch(ualm_ctx_t *c, double dt, double *out10)
 {
     if (!c || !out10 || !(dt > 0.0)) return fail(UALM_EINVAL, "null argument or dt <= 0");
-    if (c->tp) {
-        const ualm_result_t *d_res; const double *d_cxy, *d_cyaw;
-        int B = 0; const int32_t *N = nullptr, *M = nullptr, *E = nullptr;
-        if (ualm_tp::tp_lane_outputs(c->tp, c->cur, &d_res, &d_cxy, &d_cyaw, &B, &N, &M, &E) != UALM_OK)
-            return fail(UALM_ESTATE, "ualm_feasibility_batch needs a solved, collected batch (ualm_sync / ualm_download first)");
-        CK(cudaSetDevice(c->device));
-        if (B == 0) return UALM_OK;
-        return feasibility_from_device(c, B, N, M, E, c->lanes[c->cur].vref, d_res, d_cxy, d_cyaw, dt, out10);
-    }
     Lane *l = c->b;
+    const BatchLayout &L = l->batch;
+    if (c->tp) {
+        TpScan s;
+        if (int rc = tp_scan(c, "ualm_feasibility_batch", s)) return rc;
+        if (L.B == 0) return UALM_OK;
+        CK(s.feas.ensure(10 * (size_t)L.B));
+        if (int rc = feasibility_launch(c, s.bp, L, l->vref, dt, s.feas.p, 0)) return rc;
+        CK(cudaMemcpy(out10, s.feas.p, sizeof(double) * 10 * L.B, cudaMemcpyDeviceToHost));
+        return UALM_OK;
+    }
     if (!l->have_batch || !l->solved) return fail(UALM_ESTATE, "ualm_feasibility_batch needs a solved resident batch");
     CK(cudaSetDevice(c->device));
-    if (l->B == 0) return UALM_OK;
-    if (int rc = feasibility_launch(c, batch_ptrs(c), l->B, l->env.data(), l->vref, dt, l->d_feas.p, l->stream)) return rc;
-    CK(cudaMemcpyAsync(out10, l->d_feas.p, sizeof(double) * 10 * l->B, cudaMemcpyDeviceToHost, l->stream));
+    if (L.B == 0) return UALM_OK;
+    if (int rc = feasibility_launch(c, batch_ptrs(c), L, l->vref, dt, l->d_feas.p, l->stream)) return rc;
+    CK(cudaMemcpyAsync(out10, l->d_feas.p, sizeof(double) * 10 * L.B, cudaMemcpyDeviceToHost, l->stream));
     CK(cudaStreamSynchronize(l->stream));
     return UALM_OK;
 }
@@ -1397,21 +1444,10 @@ extern "C" int ualm_check_trajectories(ualm_ctx_t *c, int B, const int32_t *N, c
     // problems grouped by environment, and the grid version each environment has now
     std::vector<int> idx;
     int off[UALM_MAX_ENVS + 1];
+    group_by_env(B, env, idx, off);
     MapRef hold[UALM_MAX_ENVS];
-    for (int e = 0; e < UALM_MAX_ENVS; e++) {
-        off[e] = (int)idx.size();
-        for (int b = 0; b < B; b++) if ((env ? env[b] : 0) == e) idx.push_back(b);
-        if ((int)idx.size() > off[e]) hold[e] = c->envs[e].map;
-    }
-    off[UALM_MAX_ENVS] = B;
-    std::vector<ProbDesc> desc(B);
-    long long ocx = 0, ocy = 0;
-    for (int b = 0; b < B; b++) {
-        memset(&desc[b], 0, sizeof(ProbDesc));
-        desc[b].N = N[b]; desc[b].M = M[b]; desc[b].off_cxy = ocx; desc[b].off_cyaw = ocy;
-        desc[b].S = (N[b] > UALM_NMAX || M[b] > UALM_MMAX) ? 0 : 1;      // S == 0: over the compiled limits, not scanned
-        ocx += 12LL * N[b]; ocy += 6LL * M[b];
-    }
+    for (int e = 0; e < UALM_MAX_ENVS; e++) if (off[e + 1] > off[e]) hold[e] = c->envs[e].map;
+    const std::vector<ProbDesc> desc = scan_descs(B, N, M);
     std::vector<double> tf;
     if (!t_from) tf.assign(B, 0.0);
     // the block: out 16B | piece_T 2B | t_from B | c_xy | c_yaw (doubles), then desc, then idx
@@ -1483,18 +1519,10 @@ extern "C" int ualm_submit_replan(ualm_ctx_t *c, int B, const int32_t *N, const 
     for (long long q = 0; q < ncy; q++) if (!std::isfinite(c_yaw[q])) return fail(UALM_EINVAL, "ualm_submit_replan: c_yaw must be finite");
     if (B == 0) return ualm_submit_batch_env(c, 0, N_out, M_out, bnd_out, total_time_out, nullptr, nullptr, env, depth, ticket);
     if (int rc = check_envs(c, B, env)) return rc;
-    const int lane = c->next_submit % depth;
-    if (c->tp ? ualm_tp::tp_lane_in_flight(c->tp, lane) : c->lanes[lane].in_flight)
-        return fail(UALM_ESTATE, "all lanes of this depth are in flight: ualm_wait_batch the oldest ticket first");
+    if (lane_in_flight(c, c->next_submit % depth)) return fail(UALM_ESTATE, "all lanes of this depth are in flight: ualm_wait_batch the oldest ticket first");
     CK(cudaSetDevice(c->device));
     if (int rc = check_stream(c)) return rc;
-    std::vector<ProbDesc> desc(B);
-    long long ocx = 0, ocy = 0;
-    for (int b = 0; b < B; b++) {
-        memset(&desc[b], 0, sizeof(ProbDesc));
-        desc[b].N = N[b]; desc[b].M = M[b]; desc[b].off_cxy = ocx; desc[b].off_cyaw = ocy;
-        ocx += 12LL * N[b]; ocy += 6LL * M[b];
-    }
+    const std::vector<ProbDesc> desc = scan_descs(B, N, M);      // (replan_kernel does not read S)
     // the block: out (UALM_REPLAN_STRIDE B) | piece_T 2B | bnd 18B | t_from B | c_xy | c_yaw (doubles), then desc
     const size_t nout = (size_t)UALM_REPLAN_STRIDE * B, nd = nout + 21 * (size_t)B + (size_t)ncx + (size_t)ncy;
     const cudaStream_t st = c->cstream;
@@ -1539,7 +1567,7 @@ extern "C" int ualm_submit_replan(ualm_ctx_t *c, int B, const int32_t *N, const 
     for (int b = 0; b < B; b++) {
         const double *o = &h[(size_t)UALM_REPLAN_STRIDE * b];
         const long long nxy = 2LL * (N_out[b] - 1), nyaw = M_out[b] - 1;
-        if (N_out[b] <= UALM_NMAX && M_out[b] <= UALM_MMAX) {
+        if (!over_limits(N_out[b], M_out[b])) {
             memcpy(ixy.data() + pxy, o + 21, sizeof(double) * nxy);
             memcpy(iyaw.data() + pyaw, o + 21 + UALM_REPLAN_INNER_XY, sizeof(double) * nyaw);
         }
@@ -1551,11 +1579,12 @@ extern "C" int ualm_submit_replan(ualm_ctx_t *c, int B, const int32_t *N, const 
 // ---------------------------------------------------------------------------------------------
 // SURVEY 8f-3: SE2Traj message + the MPC side's MINCO re-solve + planned-vs-tracked deviation for a solved batch (mpc_export_kernel)
 // ---------------------------------------------------------------------------------------------
-static int mpc_export_run(ualm_ctx *c, const BatchPtrs &bp, int B, const int32_t *N, const int32_t *M, double dt, const double *init_v, const double *init_a,
-                          double *pos_pts, double *posT_pts, double *angle_pts, double *angleT_pts, double *c_mpc_xy, double *c_mpc_yaw, double *dev4, cudaStream_t st)
+static int mpc_export_run(ualm_ctx *c, const BatchPtrs &bp, const BatchLayout &L, double dt, const double *init_v, const double *init_a, double *pos_pts,
+                          double *posT_pts, double *angle_pts, double *angleT_pts, double *c_mpc_xy, double *c_mpc_yaw, double *dev4, cudaStream_t st)
 {
+    const int B = L.B;
     long long sN = 0, sM = 0;
-    for (int b = 0; b < B; b++) { sN += N[b]; sM += M[b]; }
+    for (int b = 0; b < B; b++) { sN += L.N[b]; sM += L.M[b]; }
     struct Tmp { DevBuf<double> buf; ~Tmp() { buf.release(); } } t;
     const size_t n_pp = 2 * (size_t)(sN + B), n_pt = (size_t)sN, n_ap = (size_t)(sM + B), n_at = (size_t)sM, n_cx = 12 * (size_t)sN, n_cy = 6 * (size_t)sM, n_dv = 4 * (size_t)B;
     const size_t n_band = 13 * (6 * (size_t)sN + 6 * (size_t)sM);
@@ -1578,37 +1607,18 @@ extern "C" int ualm_mpc_export_batch(ualm_ctx_t *c, double dt, const double *ini
                                      double *angleT_pts, double *c_mpc_xy, double *c_mpc_yaw, double *dev4)
 {
     if (!c || !(dt > 0.0)) return fail(UALM_EINVAL, "null ctx or dt <= 0");
-    if (c->tp) {
-        const ualm_result_t *d_res; const double *d_cxy, *d_cyaw;
-        int B = 0; const int32_t *N = nullptr, *M = nullptr, *E = nullptr;     // (the hand-over reads no parameter and no grid)
-        if (ualm_tp::tp_lane_outputs(c->tp, c->cur, &d_res, &d_cxy, &d_cyaw, &B, &N, &M, &E) != UALM_OK)
-            return fail(UALM_ESTATE, "ualm_mpc_export_batch needs a solved, collected batch (ualm_sync / ualm_download first)");
-        CK(cudaSetDevice(c->device));
-        if (B == 0) return UALM_OK;
-        struct Tmp { DevBuf<ProbDesc> desc; DevBuf<double> pt; ~Tmp() { desc.release(); pt.release(); } } t;
-        std::vector<ProbDesc> desc(B);
-        long long ocx = 0, ocy = 0;
-        for (int b = 0; b < B; b++) {
-            memset(&desc[b], 0, sizeof(ProbDesc));
-            desc[b].N = N[b]; desc[b].M = M[b]; desc[b].off_cxy = ocx; desc[b].off_cyaw = ocy;
-            desc[b].S = (N[b] > UALM_NMAX || M[b] > UALM_MMAX) ? 0 : 1;
-            ocx += 12LL * N[b]; ocy += 6LL * M[b];
-        }
-        CK(t.desc.ensure(B)); CK(t.pt.ensure(2 * (size_t)B));
-        CK(cudaMemcpy(t.desc.p, desc.data(), sizeof(ProbDesc) * B, cudaMemcpyHostToDevice));
-        piece_T_from_results<<<(B + 127) / 128, 128>>>(d_res, B, t.pt.p);
-        BatchPtrs bp;
-        memset(&bp, 0, sizeof(bp));
-        bp.B = B; bp.desc = t.desc.p; bp.c_xy = const_cast<double *>(d_cxy); bp.c_yaw = const_cast<double *>(d_cyaw); bp.piece_T = t.pt.p;
-        return mpc_export_run(c, bp, B, N, M, dt, init_v, init_a, pos_pts, posT_pts, angle_pts, angleT_pts, c_mpc_xy, c_mpc_yaw, dev4, 0);
+    const BatchLayout &L = c->b->batch;
+    if (c->tp) {     // (the hand-over reads no parameter and no grid)
+        TpScan s;
+        if (int rc = tp_scan(c, "ualm_mpc_export_batch", s)) return rc;
+        if (L.B == 0) return UALM_OK;
+        return mpc_export_run(c, s.bp, L, dt, init_v, init_a, pos_pts, posT_pts, angle_pts, angleT_pts, c_mpc_xy, c_mpc_yaw, dev4, 0);
     }
     Lane *l = c->b;
     if (!l->have_batch || !l->solved) return fail(UALM_ESTATE, "ualm_mpc_export_batch needs a solved resident batch");
     CK(cudaSetDevice(c->device));
-    if (l->B == 0) return UALM_OK;
-    std::vector<int32_t> N(l->B), M(l->B);
-    for (int b = 0; b < l->B; b++) { N[b] = l->desc[b].N; M[b] = l->desc[b].M; }
-    return mpc_export_run(c, batch_ptrs(c), l->B, N.data(), M.data(), dt, init_v, init_a, pos_pts, posT_pts, angle_pts, angleT_pts, c_mpc_xy, c_mpc_yaw, dev4, l->stream);
+    if (L.B == 0) return UALM_OK;
+    return mpc_export_run(c, batch_ptrs(c), L, dt, init_v, init_a, pos_pts, posT_pts, angle_pts, angleT_pts, c_mpc_xy, c_mpc_yaw, dev4, l->stream);
 }
 
 // ---------------------------------------------------------------------------------------------

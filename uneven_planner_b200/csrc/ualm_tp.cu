@@ -45,16 +45,17 @@ struct Buf {
 };
 
 static_assert(TP_SUBGROUPS >= UALM_MAX_ENVS, "a lane runs the problems of environment k in its group k: one group per environment");
+// the C ABI skips the problems over its compiled limits (UALM_NMAX / UALM_MMAX of ualm_kernels.cuh, which this unit does not include);
+// the engine's strides must be those same limits, which ualm.h states as the inner points of a replanned row
+static_assert(2 * (TP_NMAX - 1) == UALM_REPLAN_INNER_XY && TP_MMAX - 1 == UALM_REPLAN_INNER_YAW, "TP_NMAX / TP_MMAX must be the compiled limits of ualm.h");
 
 struct TpLane {
     bool have_batch = false, in_flight = false, collected = false;
-    int B = 0, Nmax = 1, Mmax = 1, mode = 0;
-    std::vector<int32_t> N, M, env;
-    bool mixed = false;               // the batch holds problems of more than one environment
+    int mode = 0;
+    const BatchLayout *lay = nullptr;     // the uploaded batch's layout, owned by the context (tp_upload)
     std::vector<int> slots;
     std::vector<AdmitDesc> ad;
     std::vector<GatherDesc> gd;
-    long long tot_x = 0, tot_s = 0, tot_cxy = 0, tot_cyaw = 0;
     Buf<AdmitDesc> d_ad;
     Buf<GatherDesc> d_gd;
     Buf<GatherDesc> d_gdg;            // a submitted batch in several groups: d_gd once per group, other groups' problems without slot
@@ -84,7 +85,7 @@ struct TpEngine {
     cudaStream_t cstream = nullptr;       // stop-word raises: no group loop occupies it, so a raise reaches the rounds running
     cudaEvent_t evA = nullptr, evB = nullptr;
     // environments (ualm_select_env): parameters, grid and its TMA descriptor of each; group g runs with those of genv[g]
-    bool have_params[UALM_MAX_ENVS] = {}, have_map[UALM_MAX_ENVS] = {};
+    bool have_params[UALM_MAX_ENVS] = {};
     TpParams p[UALM_MAX_ENVS];
     TpMap map[UALM_MAX_ENVS];
     CUtensorMap tmap[UALM_MAX_ENVS];
@@ -273,12 +274,6 @@ void tp_destroy(TpEngine *e)
     delete e;
 }
 
-static bool any_in_flight(TpEngine *e)
-{
-    for (auto &l : e->lanes) if (l.in_flight) return true;
-    return false;
-}
-
 // the pool strides are sized by the largest int_K and mem_size over the bound environments
 static int max_K(const TpEngine *e)
 {
@@ -296,9 +291,6 @@ static int max_m(const TpEngine *e)
 int tp_set_params(TpEngine *e, int env, const ualm_params_t *p, std::string *err)
 {
     if (p->int_K < 1 || p->int_K > TP_KB_THREADS - 1) { if (err) *err = "int_K out of range [1,127] on the throughput path"; return UALM_ELIMIT; }
-    if (p->mem_size < 1 || p->mem_size > 1024) { if (err) *err = "mem_size out of range [1,1024]"; return UALM_ELIMIT; }
-    if (p->past < 0 || p->past > 16) { if (err) *err = "past out of range [0,16]"; return UALM_ELIMIT; }
-    if (any_in_flight(e)) { if (err) *err = "ualm_set_params while a batch is in flight"; return UALM_ESTATE; }
     TpParams &d = e->p[env];
     d.rho_T = p->rho_T; d.rho_ter = p->rho_ter; d.max_vel = p->max_vel; d.max_acc_lon = p->max_acc_lon; d.max_acc_lat = p->max_acc_lat;
     d.max_kap = p->max_kap; d.min_cxi = p->min_cxi; d.max_sig = p->max_sig; d.use_scaling = p->use_scaling; d.rho = p->rho;
@@ -314,12 +306,10 @@ int tp_set_params(TpEngine *e, int env, const ualm_params_t *p, std::string *err
     return UALM_OK;
 }
 
-int tp_set_budget(TpEngine *e, int max_evals, std::string *err)
+void tp_set_budget(TpEngine *e, int max_evals)
 {
-    if (any_in_flight(e)) { if (err) *err = "ualm_set_budget while a batch is in flight"; return UALM_ESTATE; }
     e->max_evals = max_evals;
     for (auto &p : e->p) p.max_evals = max_evals;
-    return UALM_OK;
 }
 
 void tp_bind_map(TpEngine *e, int env, const ualm_map_geom_t *g, const float4 *cells)
@@ -347,14 +337,6 @@ void tp_bind_map(TpEngine *e, int env, const ualm_map_geom_t *g, const float4 *c
     }
     if (getenv("UALM_DEBUG"))
         fprintf(stderr, "[ualm-tp] env %d: tensor map %s, TMA staging %s\n", env, e->have_tmap[env] ? "encoded" : "unavailable", (e->have_tmap[env] && e->use_tma) ? "on" : "off");
-    e->have_map[env] = true;
-}
-
-unsigned tp_lane_env_mask(TpEngine *e, int lane)
-{
-    unsigned mask = 0;
-    for (int v : e->lanes[lane].env) mask |= 1u << v;
-    return mask;
 }
 
 // (re)allocate the pool for `cap` slots with the current parameters; only when nothing is resident
@@ -390,62 +372,24 @@ static int pool_alloc(TpEngine *e, int cap, std::string *err)
     return UALM_OK;
 }
 
-int tp_upload(TpEngine *e, int lane, int B, const int32_t *N, const int32_t *M, const int32_t *env, const double *bnd, const double *total_time,
-              const double *inner_xy, const double *inner_yaw, std::string *err)
+int tp_upload(TpEngine *e, int lane, const BatchLayout &L, const double *bnd, const double *total_time, std::string *err)
 {
-    if (lane < 0 || lane >= TP_LANES) { if (err) *err = "lane out of range"; return UALM_EINVAL; }
     TpLane &l = e->lanes[lane];
-    if (l.in_flight) { if (err) *err = "ualm_upload into a lane whose batch is still in flight"; return UALM_ESTATE; }
-    for (int b = 0; b < (env ? B : 1); b++) {       // the engine's own state: every environment used has parameters and a grid
-        const int v = env ? env[b] : 0;
-        if (v < 0 || v >= UALM_MAX_ENVS) { if (err) *err = "env index out of range [0, UALM_MAX_ENVS)"; return UALM_EINVAL; }
-        if (!e->have_params[v] || !e->have_map[v]) { if (err) *err = "environment " + std::to_string(v) + " has no parameters or no map grid bound"; return UALM_ESTATE; }
-    }
-    long long need_xy = 0, need_yaw = 0;
-    for (int b = 0; b < B; b++) {
-        if (N[b] < 1 || M[b] < 1) { if (err) *err = "piece counts must be >= 1"; return UALM_EINVAL; }
-        if (!(total_time[b] > 0.0) || !std::isfinite(total_time[b])) { if (err) *err = "total_time must be finite and > 0"; return UALM_EINVAL; }
-        need_xy += 2LL * (N[b] - 1); need_yaw += M[b] - 1;
-    }
-    if ((need_xy > 0 && !inner_xy) || (need_yaw > 0 && !inner_yaw)) { if (err) *err = "inner waypoint arrays are NULL but N > 1 or M > 1"; return UALM_EINVAL; }
+    l.have_batch = false; l.collected = false; l.lay = &L;
     TCK(cudaSetDevice(e->device));
-    l.have_batch = false; l.collected = false;
-    l.B = B; l.N.assign(N, N + B); l.M.assign(M, M + B); l.ad.assign(B, AdmitDesc()); l.gd.assign(B, GatherDesc());
-    l.env.assign(B, 0);
-    if (env) l.env.assign(env, env + B);
-    l.mixed = false;
-    for (int b = 1; b < B; b++) l.mixed = l.mixed || l.env[b] != l.env[0];
-    l.Nmax = l.Mmax = 1;
-    std::vector<double> x0;
-    std::vector<long long> offs(B + 1, 0);
-    long long ox = 0, os = 0, ocx = 0, ocy = 0, oixy = 0, oiyw = 0;
+    const int B = L.B;
+    l.ad.assign(B, AdmitDesc()); l.gd.assign(B, GatherDesc());
     for (int b = 0; b < B; b++) {
         AdmitDesc &a = l.ad[b];
         GatherDesc &g = l.gd[b];
-        const bool skip = N[b] > TP_NMAX || M[b] > TP_MMAX;
-        a.slot = -1; a.N = N[b]; a.M = M[b]; a.ticket = lane; a.index = b; a.mode = skip ? -1 : 0; a.off_x = ox; a.total_time = total_time[b];
+        a.slot = -1; a.N = L.N[b]; a.M = L.M[b]; a.ticket = lane; a.index = b; a.mode = L.skip[b] ? -1 : 0; a.off_x = L.off_x[b]; a.total_time = total_time[b];
         for (int k = 0; k < 18; k++) a.bnd[k] = bnd[(size_t)b * 18 + k];
-        g.slot = -1; g.N = N[b]; g.M = M[b]; g.off_cxy = ocx; g.off_cyaw = ocy; g.off_x = ox; g.off_s = os;
-        offs[b] = os;
-        const long long nxy = 2LL * (N[b] - 1), nyw = M[b] - 1;
-        ocx += 12LL * N[b]; ocy += 6LL * M[b];
-        if (!skip) {
-            const double T = total_time[b];
-            x0.push_back(T > 1.0 ? (std::sqrt(2.0 * T - 1.0) - 1.0) : (1.0 - std::sqrt(2.0 / T - 1.0)));   // logC2, alm_traj_opt.h:238-241
-            for (long long q = 0; q < nxy; q++) x0.push_back(inner_xy[oixy + q]);
-            for (long long q = 0; q < nyw; q++) x0.push_back(inner_yaw[oiyw + q]);
-            ox += 1 + nxy + nyw; os += (long long)N[b] * (e->p[l.env[b]].int_K + 1);
-            l.Nmax = std::max(l.Nmax, (int)N[b]); l.Mmax = std::max(l.Mmax, (int)M[b]);
-        }
-        oixy += nxy; oiyw += nyw;
+        g.slot = -1; g.N = L.N[b]; g.M = L.M[b]; g.off_cxy = L.off_cxy[b]; g.off_cyaw = L.off_cyaw[b]; g.off_x = L.off_x[b]; g.off_s = L.off_s[b];
     }
-    offs[B] = os;
-    l.tot_x = ox; l.tot_s = os; l.tot_cxy = ocx; l.tot_cyaw = ocy;
-    TCK(l.d_ad.ensure(B)); TCK(l.d_gd.ensure(B)); TCK(l.d_x0.ensure(ox)); TCK(l.d_cxy.ensure(ocx)); TCK(l.d_cyaw.ensure(ocy)); TCK(l.d_res.ensure(B));
-    TCK(l.d_offs.ensure(B + 1));
-    if (B > 0) {
-        if (ox > 0) TCK(cudaMemcpyAsync(l.d_x0.p, x0.data(), sizeof(double) * ox, cudaMemcpyHostToDevice, e->stream));
-        TCK(cudaMemcpyAsync(l.d_offs.p, offs.data(), sizeof(long long) * (B + 1), cudaMemcpyHostToDevice, e->stream));
+    TCK(l.d_ad.ensure(B)); TCK(l.d_gd.ensure(B)); TCK(l.d_x0.ensure(L.tot_x)); TCK(l.d_cxy.ensure(L.tot_cxy)); TCK(l.d_cyaw.ensure(L.tot_cyaw));
+    TCK(l.d_res.ensure(B)); TCK(l.d_offs.ensure(B));
+    if (L.tot_x > 0) {
+        TCK(cudaMemcpyAsync(l.d_x0.p, L.x0.data(), sizeof(double) * L.tot_x, cudaMemcpyHostToDevice, e->stream));
         TCK(cudaStreamSynchronize(e->stream));
     }
     l.have_batch = true; l.mode = 0;
@@ -460,12 +404,10 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, bool p
 {
     TpLane &l = e->lanes[lane];
     if (!l.have_batch) { if (err) *err = "set_params, set_map and upload must precede the solve"; return UALM_ESTATE; }
-    for (int b = 0; b < l.B; b++)
-        if (!e->have_map[l.env[b]]) { if (err) *err = "environment " + std::to_string(l.env[b]) + " has no map grid bound"; return UALM_ESTATE; }
     if (l.in_flight) { if (err) *err = "lane already in flight"; return UALM_ESTATE; }
+    const BatchLayout &L = *l.lay;
     TCK(cudaSetDevice(e->device));
-    int need = 0;
-    for (int b = 0; b < l.B; b++) if (!(l.N[b] > TP_NMAX || l.M[b] > TP_MMAX)) need++;
+    const int need = L.n_active;
     // the pool grows only while nothing is resident; it is sized for TP_LANES batches of this size in flight (fewer when that
     // would take more than three quarters of the free device memory: 8 x 8192 float slots take ~43 GB of an 80 GB H100)
     int mult = TP_LANES;
@@ -486,7 +428,7 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, bool p
     // the lane's stop words: no request of its previous batch carries over (nothing raises them while the lane is not in flight, and
     // the raises of its previous batch were complete when that batch was collected)
     {
-        const size_t nw = (size_t)std::max(l.B, 1);
+        const size_t nw = (size_t)std::max(L.B, 1);
         TCK(l.d_stop.ensure(nw));
         if (l.h_stop_cap < nw) {         // (in powers of two: freeing pinned memory waits for the device)
             size_t c = 1024;
@@ -501,59 +443,54 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, bool p
         e->E.stop[lane] = l.d_stop.p;
     }
     l.slots.clear();
-    std::vector<ualm_result_t> res0(l.B);
+    std::vector<ualm_result_t> res0(L.B);
     int k = 0;
-    for (int b = 0; b < l.B; b++) {
+    for (int b = 0; b < L.B; b++) {
         memset(&res0[b], 0, sizeof(ualm_result_t));
-        const bool skip = l.N[b] > TP_NMAX || l.M[b] > TP_MMAX;
-        if (skip) { l.ad[b].slot = -1; l.gd[b].slot = -1; l.ad[b].mode = -1; res0[b].ret_code = UALM_ELIMIT; continue; }
+        if (L.skip[b]) { l.ad[b].slot = -1; l.gd[b].slot = -1; l.ad[b].mode = -1; res0[b].ret_code = UALM_ELIMIT; continue; }
         const int s = e->free_slots.back();
         e->free_slots.pop_back();
         l.slots.push_back(s);
         // a batch of one environment is dealt over the lane's e->sg groups; in a mixed batch group k runs environment k
-        const int g = lane * TP_SUBGROUPS + (l.mixed ? l.env[b] : single_group ? 0 : k % e->sg);
+        const int g = lane * TP_SUBGROUPS + (L.mixed() ? L.env[b] : single_group ? 0 : k % e->sg);
         l.ad[b].slot = s; l.ad[b].mode = mode; l.ad[b].group = g; l.gd[b].slot = s;
         e->glive[g]++;
-        e->genv[g] = l.env[b];
+        e->genv[g] = L.env[b];
         k++;
     }
     e->live += (int)l.slots.size();
-    e->Nmax_live = std::max(e->Nmax_live, l.Nmax); e->Mmax_live = std::max(e->Mmax_live, l.Mmax);
+    e->Nmax_live = std::max(e->Nmax_live, L.Nmax); e->Mmax_live = std::max(e->Mmax_live, L.Mmax);
     // compact descriptors of the admitted problems only (skipped ones keep their UALM_ELIMIT record), grouped by environment: one
     // admit_kernel launch per environment, with its own use_scaling and int_K.  offs: sample offsets in the caller's dual arrays
     std::vector<AdmitDesc> ad;
     std::vector<long long> offs;
     int eoff[UALM_MAX_ENVS + 1];
-    {
-        std::vector<long long> os_of(l.B, 0);
-        long long os = 0;
-        for (int b = 0; b < l.B; b++) if (l.ad[b].slot >= 0) { os_of[b] = os; os += (long long)l.N[b] * (e->p[l.env[b]].int_K + 1); }
-        for (int v = 0; v < UALM_MAX_ENVS; v++) {
-            eoff[v] = (int)ad.size();
-            for (int b = 0; b < l.B; b++) if (l.ad[b].slot >= 0 && l.env[b] == v) { ad.push_back(l.ad[b]); offs.push_back(os_of[b]); }
-        }
-        eoff[UALM_MAX_ENVS] = (int)ad.size();
+    for (int v = 0; v < UALM_MAX_ENVS; v++) {
+        eoff[v] = (int)ad.size();
+        for (int q = L.eoff[v]; q < L.eoff[v + 1]; q++)
+            if (!L.skip[L.eidx[q]]) { ad.push_back(l.ad[L.eidx[q]]); offs.push_back(L.off_s[L.eidx[q]]); }
     }
+    eoff[UALM_MAX_ENVS] = (int)ad.size();
     const int BA = (int)ad.size();
     TCK(cudaEventRecord(l.ev0, e->stream));
     l.launches = 0;
-    TCK(cudaMemcpyAsync(l.d_res.p, res0.data(), sizeof(ualm_result_t) * l.B, cudaMemcpyHostToDevice, e->stream));
-    if (BA < l.B) {
-        TCK(cudaMemsetAsync(l.d_cxy.p, 0, sizeof(double) * l.tot_cxy, e->stream));
-        TCK(cudaMemsetAsync(l.d_cyaw.p, 0, sizeof(double) * l.tot_cyaw, e->stream));
+    TCK(cudaMemcpyAsync(l.d_res.p, res0.data(), sizeof(ualm_result_t) * L.B, cudaMemcpyHostToDevice, e->stream));
+    if (BA < L.B) {
+        TCK(cudaMemsetAsync(l.d_cxy.p, 0, sizeof(double) * L.tot_cxy, e->stream));
+        TCK(cudaMemsetAsync(l.d_cyaw.p, 0, sizeof(double) * L.tot_cyaw, e->stream));
     }
     if (BA > 0) {
         TCK(cudaMemcpyAsync(l.d_ad.p, ad.data(), sizeof(AdmitDesc) * BA, cudaMemcpyHostToDevice, e->stream));
         TCK(cudaMemcpyAsync(l.d_offs.p, offs.data(), sizeof(long long) * BA, cudaMemcpyHostToDevice, e->stream));
-        TCK(cudaMemcpyAsync(l.d_gd.p, l.gd.data(), sizeof(GatherDesc) * l.B, cudaMemcpyHostToDevice, e->stream));
+        TCK(cudaMemcpyAsync(l.d_gd.p, l.gd.data(), sizeof(GatherDesc) * L.B, cudaMemcpyHostToDevice, e->stream));
         std::vector<GatherDesc> gdg;
         int ngroups = 0;
         for (int q = 0; q < TP_SUBGROUPS; q++) ngroups += e->glive[lane * TP_SUBGROUPS + q] > 0;
         if (publish && ngroups > 1) {    // per group: start_loops
-            gdg.resize((size_t)TP_SUBGROUPS * l.B);
+            gdg.resize((size_t)TP_SUBGROUPS * L.B);
             for (int q = 0; q < TP_SUBGROUPS; q++)
-                for (int b = 0; b < l.B; b++) {
-                    GatherDesc &d = gdg[(size_t)q * l.B + b];
+                for (int b = 0; b < L.B; b++) {
+                    GatherDesc &d = gdg[(size_t)q * L.B + b];
                     d = l.gd[b];
                     if (l.ad[b].slot < 0 || l.ad[b].group != lane * TP_SUBGROUPS + q) d.slot = -1;
                 }
@@ -588,15 +525,13 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, bool p
 
 int tp_admit(TpEngine *e, int lane, std::string *err, bool publish)
 {
-    if (lane < 0 || lane >= TP_LANES) { if (err) *err = "lane out of range"; return UALM_EINVAL; }
     TpLane &l = e->lanes[lane];
     if (publish && l.have_batch && !l.in_flight) {      // (admit_impl refuses the other cases)
-        std::vector<unsigned char> skip(l.B);
-        for (int b = 0; b < l.B; b++) skip[b] = l.N[b] > TP_NMAX || l.M[b] > TP_MMAX;
+        const BatchLayout &L = *l.lay;
         TCK(cudaSetDevice(e->device));
-        TCK(l.mbox.begin(l.B, l.N.data(), l.M.data(), skip.data()));
-        TCK(l.d_pub.ensure(l.B));
-        if (l.B > 0) TCK(cudaMemsetAsync(l.d_pub.p, 0, sizeof(int) * l.B, e->stream));   // ordered before admission's synchronise
+        TCK(l.mbox.begin(L.B, L.N.data(), L.M.data(), L.skip.data()));
+        TCK(l.d_pub.ensure(L.B));
+        if (L.B > 0) TCK(cudaMemsetAsync(l.d_pub.p, 0, sizeof(int) * L.B, e->stream));   // ordered before admission's synchronise
     }
     return admit_impl(e, lane, 0, false, publish, true, err);
 }
@@ -723,7 +658,7 @@ static int launch_loop(TpEngine *e, int g, bool with_ks, const GatherDesc *pub_g
     for (int r = 0; r < e->chunk && rc == UALM_OK; r++) rc = launch_round<R>(e, g, cs, false, tma, err);
     if (rc == UALM_OK) {
         compact_kernel<<<1, 1024, 0, cs>>>(e->E, e->capacity, g);
-        if (pub_gd) publish_kernel<R><<<l.B, 128, 0, cs>>>(e->E, pub_gd, l.B, l.d_pub.p, l.mbox.device());
+        if (pub_gd) publish_kernel<R><<<l.lay->B, 128, 0, cs>>>(e->E, pub_gd, l.lay->B, l.d_pub.p, l.mbox.device());
         loop_ctrl_kernel<<<1, 1, 0, cs>>>(L.h, e->n_active.p, e->gloop.p, g, e->chunk, body_launches);
         check(cudaGetLastError(), "loop body launch");
     }
@@ -756,7 +691,7 @@ static int start_loops(TpEngine *e, int lane, bool publish, std::string *err)
         const int g = lane * TP_SUBGROUPS + q;
         if (e->glive[g] <= 0) continue;
         // each group publishes only its own problems: a slot of another group may be in the middle of its round
-        const GatherDesc *pub = !publish ? nullptr : ngroups > 1 ? l.d_gdg.p + (size_t)q * l.B : l.d_gd.p;
+        const GatherDesc *pub = !publish ? nullptr : ngroups > 1 ? l.d_gdg.p + (size_t)q * l.lay->B : l.d_gd.p;
         const bool with_ks = (l.mode == 0 && e->p[e->genv[g]].use_scaling) || l.mode == 2;
         rc = e->f32() ? launch_loop<float>(e, g, with_ks, pub, &l.launches, err) : launch_loop<double>(e, g, with_ks, pub, &l.launches, err);
     }
@@ -769,9 +704,10 @@ static int start_loops(TpEngine *e, int lane, bool publish, std::string *err)
 // ordered after the clear; words only go from 0 to 1 while the batch runs, so the copy never lowers one
 static int raise_stop(TpEngine *e, TpLane &l, int n, const int32_t *idx, std::string *err)
 {
+    const int B = l.lay->B;
     if (idx) for (int k = 0; k < n; k++) l.h_stop[idx[k]] = 1;
-    else for (int b = 0; b < l.B; b++) l.h_stop[b] = 1;
-    if (l.B > 0) TCK(cudaMemcpyAsync(l.d_stop.p, l.h_stop, sizeof(int) * l.B, cudaMemcpyHostToDevice, e->cstream));
+    else for (int b = 0; b < B; b++) l.h_stop[b] = 1;
+    if (B > 0) TCK(cudaMemcpyAsync(l.d_stop.p, l.h_stop, sizeof(int) * B, cudaMemcpyHostToDevice, e->cstream));
     return UALM_OK;
 }
 
@@ -780,7 +716,7 @@ int tp_cancel(TpEngine *e, int lane, int n, const int32_t *idx, std::string *err
     TpLane &l = e->lanes[lane];
     if (!l.in_flight || !l.publish) { if (err) *err = "ticket is not in flight"; return UALM_ESTATE; }
     for (int k = 0; k < n; k++)
-        if (idx[k] < 0 || idx[k] >= l.B) { if (err) *err = "problem index out of range [0, B)"; return UALM_EINVAL; }
+        if (idx[k] < 0 || idx[k] >= l.lay->B) { if (err) *err = "problem index out of range [0, B)"; return UALM_EINVAL; }
     if (n == 0) return UALM_OK;
     TCK(cudaSetDevice(e->device));
     return raise_stop(e, l, n, idx, err);
@@ -800,10 +736,10 @@ static int loops_done(TpEngine *e, int lane, bool *done, std::string *err)
 
 int tp_collect(TpEngine *e, int lane, std::string *err, double timeout_ms)
 {
-    if (lane < 0 || lane >= TP_LANES) { if (err) *err = "lane out of range"; return UALM_EINVAL; }
     TpLane &l = e->lanes[lane];
     if (l.collected) return UALM_OK;
     if (!l.in_flight) { if (err) *err = "nothing in flight on this lane"; return UALM_ESTATE; }
+    const BatchLayout &L = *l.lay;
     TCK(cudaSetDevice(e->device));
     if (timeout_ms >= 0.0) {
         // deadline: yield-poll the lane's loops until it has passed, then raise every stop word of the batch and let the loops drain
@@ -831,20 +767,20 @@ int tp_collect(TpEngine *e, int lane, std::string *err, double timeout_ms)
     }
     // gather the batch's results into the lane's packed device outputs, free its slots
     const bool ev = l.mode != 0;
-    if (l.B > 0 && !l.slots.empty()) {
+    if (L.B > 0 && !l.slots.empty()) {
         if (ev) {
-            TCK(l.d_f.ensure(l.B)); TCK(l.d_grad.ensure(l.tot_x)); TCK(l.d_hx.ensure(l.tot_s)); TCK(l.d_gx.ensure(6 * l.tot_s)); TCK(l.d_sfx.ensure(l.B));
-            TCK(l.d_scx.ensure(7 * l.tot_s));
+            TCK(l.d_f.ensure(L.B)); TCK(l.d_grad.ensure(L.tot_x)); TCK(l.d_hx.ensure(L.tot_s)); TCK(l.d_gx.ensure(6 * L.tot_s)); TCK(l.d_sfx.ensure(L.B));
+            TCK(l.d_scx.ensure(7 * L.tot_s));
         }
-        TCK(l.d_xout.ensure(l.tot_x));
+        TCK(l.d_xout.ensure(L.tot_x));
 #define GATHER(R)                                                                                                                                          \
-        gather_kernel<R><<<l.B, 128, 0, e->stream>>>(e->E, l.d_gd.p, l.B, l.d_res.p, l.d_cxy.p, l.d_cyaw.p, l.d_xout.p, ev ? l.d_f.p : nullptr,            \
+        gather_kernel<R><<<L.B, 128, 0, e->stream>>>(e->E, l.d_gd.p, L.B, l.d_res.p, l.d_cxy.p, l.d_cyaw.p, l.d_xout.p, ev ? l.d_f.p : nullptr,            \
                                                      ev ? l.d_grad.p : nullptr, ev ? l.d_hx.p : nullptr, ev ? l.d_gx.p : nullptr, ev ? l.d_sfx.p : nullptr,    \
                                                      ev ? l.d_scx.p : nullptr)
         if (e->f32()) GATHER(float); else GATHER(double);
 #undef GATHER
         TCK(cudaGetLastError());
-        free_kernel<<<(l.B + 127) / 128, 128, 0, e->stream>>>(e->E, l.d_gd.p, l.B);
+        free_kernel<<<(L.B + 127) / 128, 128, 0, e->stream>>>(e->E, l.d_gd.p, L.B);
         TCK(cudaGetLastError());
         l.launches += 2;
     }
@@ -883,11 +819,12 @@ int tp_download(TpEngine *e, int lane, ualm_result_t *results, double *c_xy, dou
 {
     TpLane &l = e->lanes[lane];
     if (!l.collected) { int rc = tp_collect(e, lane, err); if (rc) return rc; }
+    const BatchLayout &L = *l.lay;
     TCK(cudaSetDevice(e->device));
-    if (l.B > 0) {
-        if (results) TCK(cudaMemcpyAsync(results, l.d_res.p, sizeof(ualm_result_t) * l.B, cudaMemcpyDeviceToHost, e->stream));
-        if (c_xy) TCK(cudaMemcpyAsync(c_xy, l.d_cxy.p, sizeof(double) * l.tot_cxy, cudaMemcpyDeviceToHost, e->stream));
-        if (c_yaw) TCK(cudaMemcpyAsync(c_yaw, l.d_cyaw.p, sizeof(double) * l.tot_cyaw, cudaMemcpyDeviceToHost, e->stream));
+    if (L.B > 0) {
+        if (results) TCK(cudaMemcpyAsync(results, l.d_res.p, sizeof(ualm_result_t) * L.B, cudaMemcpyDeviceToHost, e->stream));
+        if (c_xy) TCK(cudaMemcpyAsync(c_xy, l.d_cxy.p, sizeof(double) * L.tot_cxy, cudaMemcpyDeviceToHost, e->stream));
+        if (c_yaw) TCK(cudaMemcpyAsync(c_yaw, l.d_cyaw.p, sizeof(double) * L.tot_cyaw, cudaMemcpyDeviceToHost, e->stream));
     }
     TCK(cudaStreamSynchronize(e->stream));
     return UALM_OK;
@@ -917,9 +854,10 @@ int tp_pack_records(TpEngine *e, int lane, double *d_records, int stride, std::s
 {
     TpLane &l = e->lanes[lane];
     if (!l.collected) { int rc = tp_collect(e, lane, err); if (rc) return rc; }
-    if (stride < 12 + 12 * l.Nmax + 6 * l.Mmax) { if (err) *err = "record stride too small"; return UALM_EINVAL; }
-    if (l.B > 0) {
-        tp_pack_records_kernel<<<l.B, 128, 0, e->stream>>>(l.d_res.p, l.d_gd.p, l.d_cxy.p, l.d_cyaw.p, l.B, d_records, stride);
+    const BatchLayout &L = *l.lay;
+    if (stride < 12 + 12 * L.Nmax + 6 * L.Mmax) { if (err) *err = "record stride too small"; return UALM_EINVAL; }
+    if (L.B > 0) {
+        tp_pack_records_kernel<<<L.B, 128, 0, e->stream>>>(l.d_res.p, l.d_gd.p, l.d_cxy.p, l.d_cyaw.p, L.B, d_records, stride);
         TCK(cudaGetLastError());
     }
     TCK(cudaStreamSynchronize(e->stream));
@@ -927,7 +865,6 @@ int tp_pack_records(TpEngine *e, int lane, double *d_records, int stride, std::s
 }
 
 bool tp_lane_in_flight(TpEngine *e, int lane) { return e->lanes[lane].in_flight; }
-bool tp_lane_has_batch(TpEngine *e, int lane) { return e->lanes[lane].have_batch; }
 bool tp_lane_collected(TpEngine *e, int lane) { return e->lanes[lane].collected; }
 
 int tp_last_solve(TpEngine *e, int lane, float *ms, int *launches)
@@ -971,33 +908,34 @@ int tp_eval(TpEngine *e, int lane, const double *x, const double *lambda, const 
 {
     TpLane &l = e->lanes[lane];
     if (!l.have_batch) { if (err) *err = "upload and set_map first"; return UALM_ESTATE; }
-    for (int b = 0; b < l.B; b++) if (l.N[b] > TP_NMAX || l.M[b] > TP_MMAX) { if (err) *err = "batch holds problems over the compiled limits"; return UALM_ELIMIT; }
+    const BatchLayout &L = *l.lay;
+    if (L.n_active != L.B) { if (err) *err = "batch holds problems over the compiled limits"; return UALM_ELIMIT; }
     TCK(cudaSetDevice(e->device));
     // the evaluation point goes to its own buffer: d_x0 keeps the uploaded initial guesses, which ualm_init_scaling_batch and a
     // later solve of the resident batch start from
-    const bool xev = x && l.tot_x > 0;
+    const bool xev = x && L.tot_x > 0;
     if (xev) {
-        TCK(l.d_xev.ensure(l.tot_x));
-        TCK(cudaMemcpyAsync(l.d_xev.p, x, sizeof(double) * l.tot_x, cudaMemcpyHostToDevice, e->stream));
+        TCK(l.d_xev.ensure(L.tot_x));
+        TCK(cudaMemcpyAsync(l.d_xev.p, x, sizeof(double) * L.tot_x, cudaMemcpyHostToDevice, e->stream));
     }
     int rc;
-    if ((rc = put(e, l.d_lam, lambda, l.tot_s, l.has_lam, err))) return rc;
-    if ((rc = put(e, l.d_mu, mu, 6 * l.tot_s, l.has_mu, err))) return rc;
-    if ((rc = put(e, l.d_scin, scale_cx, 7 * l.tot_s, l.has_scx, err))) return rc;
-    if ((rc = put(e, l.d_sfin, scale_fx, l.B, l.has_sfx, err))) return rc;
+    if ((rc = put(e, l.d_lam, lambda, L.tot_s, l.has_lam, err))) return rc;
+    if ((rc = put(e, l.d_mu, mu, 6 * L.tot_s, l.has_mu, err))) return rc;
+    if ((rc = put(e, l.d_scin, scale_cx, 7 * L.tot_s, l.has_scx, err))) return rc;
+    if ((rc = put(e, l.d_sfin, scale_fx, L.B, l.has_sfx, err))) return rc;
     l.rho_eval = rho;
     l.has_xev = xev;
     rc = admit_impl(e, lane, 1, false, false, true, err);
     l.has_lam = l.has_mu = l.has_scx = l.has_sfx = l.has_xev = false;
     if (rc) return rc;
     if ((rc = tp_collect(e, lane, err))) return rc;
-    if (l.B > 0) {
-        if (f) TCK(cudaMemcpyAsync(f, l.d_f.p, sizeof(double) * l.B, cudaMemcpyDeviceToHost, e->stream));
-        if (grad) TCK(cudaMemcpyAsync(grad, l.d_grad.p, sizeof(double) * l.tot_x, cudaMemcpyDeviceToHost, e->stream));
-        if (hx) TCK(cudaMemcpyAsync(hx, l.d_hx.p, sizeof(double) * l.tot_s, cudaMemcpyDeviceToHost, e->stream));
-        if (gx) TCK(cudaMemcpyAsync(gx, l.d_gx.p, sizeof(double) * 6 * l.tot_s, cudaMemcpyDeviceToHost, e->stream));
-        if (c_xy) TCK(cudaMemcpyAsync(c_xy, l.d_cxy.p, sizeof(double) * l.tot_cxy, cudaMemcpyDeviceToHost, e->stream));
-        if (c_yaw) TCK(cudaMemcpyAsync(c_yaw, l.d_cyaw.p, sizeof(double) * l.tot_cyaw, cudaMemcpyDeviceToHost, e->stream));
+    if (L.B > 0) {
+        if (f) TCK(cudaMemcpyAsync(f, l.d_f.p, sizeof(double) * L.B, cudaMemcpyDeviceToHost, e->stream));
+        if (grad) TCK(cudaMemcpyAsync(grad, l.d_grad.p, sizeof(double) * L.tot_x, cudaMemcpyDeviceToHost, e->stream));
+        if (hx) TCK(cudaMemcpyAsync(hx, l.d_hx.p, sizeof(double) * L.tot_s, cudaMemcpyDeviceToHost, e->stream));
+        if (gx) TCK(cudaMemcpyAsync(gx, l.d_gx.p, sizeof(double) * 6 * L.tot_s, cudaMemcpyDeviceToHost, e->stream));
+        if (c_xy) TCK(cudaMemcpyAsync(c_xy, l.d_cxy.p, sizeof(double) * L.tot_cxy, cudaMemcpyDeviceToHost, e->stream));
+        if (c_yaw) TCK(cudaMemcpyAsync(c_yaw, l.d_cyaw.p, sizeof(double) * L.tot_cyaw, cudaMemcpyDeviceToHost, e->stream));
     }
     TCK(cudaStreamSynchronize(e->stream));
     l.collected = false;           // the lane holds evaluation outputs, not a solve
@@ -1008,14 +946,15 @@ int tp_init_scaling(TpEngine *e, int lane, double *scale_fx, double *scale_cx, s
 {
     TpLane &l = e->lanes[lane];
     if (!l.have_batch) { if (err) *err = "upload and set_map first"; return UALM_ESTATE; }
-    for (int b = 0; b < l.B; b++) if (l.N[b] > TP_NMAX || l.M[b] > TP_MMAX) { if (err) *err = "batch holds problems over the compiled limits"; return UALM_ELIMIT; }
+    const BatchLayout &L = *l.lay;
+    if (L.n_active != L.B) { if (err) *err = "batch holds problems over the compiled limits"; return UALM_ELIMIT; }
     TCK(cudaSetDevice(e->device));
     int rc = admit_impl(e, lane, 2, false, false, true, err);
     if (rc) return rc;
     if ((rc = tp_collect(e, lane, err))) return rc;
-    if (l.B > 0) {
-        if (scale_fx) TCK(cudaMemcpyAsync(scale_fx, l.d_sfx.p, sizeof(double) * l.B, cudaMemcpyDeviceToHost, e->stream));
-        if (scale_cx) TCK(cudaMemcpyAsync(scale_cx, l.d_scx.p, sizeof(double) * 7 * l.tot_s, cudaMemcpyDeviceToHost, e->stream));
+    if (L.B > 0) {
+        if (scale_fx) TCK(cudaMemcpyAsync(scale_fx, l.d_sfx.p, sizeof(double) * L.B, cudaMemcpyDeviceToHost, e->stream));
+        if (scale_cx) TCK(cudaMemcpyAsync(scale_cx, l.d_scx.p, sizeof(double) * 7 * L.tot_s, cudaMemcpyDeviceToHost, e->stream));
     }
     TCK(cudaStreamSynchronize(e->stream));
     l.collected = false;
@@ -1026,13 +965,14 @@ int tp_time_penalty(TpEngine *e, int lane, int reps, int use_tma, float *ms_per_
 {
     TpLane &l = e->lanes[lane];
     if (!l.have_batch) { if (err) *err = "upload and set_map first"; return UALM_ESTATE; }
-    if (l.mixed) { if (err) *err = "ualm_time_penalty_kernel: the uploaded batch mixes environments"; return UALM_EINVAL; }
+    const BatchLayout &L = *l.lay;
+    if (L.mixed()) { if (err) *err = "ualm_time_penalty_kernel: the uploaded batch mixes environments"; return UALM_EINVAL; }
     if (l.in_flight || e->live > 0) { if (err) *err = "ualm_time_penalty_kernel needs an idle pool"; return UALM_ESTATE; }
     if (ms_per_launch) *ms_per_launch = 0.f;
     if (algorithmic_bytes) *algorithmic_bytes = 0.0;
-    if (l.B == 0) return UALM_OK;
+    if (L.B == 0) return UALM_OK;
     TCK(cudaSetDevice(e->device));
-    const int v = l.env[0];
+    const int v = L.env[0];
     // admit as single evaluations (initial guess, zero duals, unit scales), run the forward half of a round, then time kb alone
     l.has_lam = l.has_mu = l.has_scx = l.has_sfx = false; l.rho_eval = e->p[v].rho;
     int rc = admit_impl(e, lane, 1, true, false, false, err);
@@ -1068,7 +1008,7 @@ int tp_time_penalty(TpEngine *e, int lane, int reps, int use_tma, float *ms_per_
         // SURVEY 8d: per trajectory per evaluation S * 45 e + (25 N + 13 M) e, e = element size of the sample data
         double bytes = 0;
         const double es = (double)e->esz();
-        for (int b = 0; b < l.B; b++) bytes += (double)l.N[b] * (e->p[v].int_K + 1) * 45 * es + (25.0 * l.N[b] + 13.0 * l.M[b]) * es;
+        for (int b = 0; b < L.B; b++) bytes += (double)L.N[b] * (e->p[v].int_K + 1) * 45 * es + (25.0 * L.N[b] + 13.0 * L.M[b]) * es;
         *algorithmic_bytes = bytes;
     }
     // finish the evaluations (the group's loop, queued behind the timed launches) and release the slots
@@ -1078,12 +1018,11 @@ int tp_time_penalty(TpEngine *e, int lane, int reps, int use_tma, float *ms_per_
     return rc;
 }
 
-int tp_lane_outputs(TpEngine *e, int lane, const ualm_result_t **d_res, const double **d_cxy, const double **d_cyaw, int *B, const int32_t **N,
-                    const int32_t **M, const int32_t **env)
+int tp_lane_outputs(TpEngine *e, int lane, const ualm_result_t **d_res, const double **d_cxy, const double **d_cyaw)
 {
     TpLane &l = e->lanes[lane];
     if (!l.collected) return UALM_ESTATE;
-    *d_res = l.d_res.p; *d_cxy = l.d_cxy.p; *d_cyaw = l.d_cyaw.p; *B = l.B; *N = l.N.data(); *M = l.M.data(); *env = l.env.data();
+    *d_res = l.d_res.p; *d_cxy = l.d_cxy.p; *d_cyaw = l.d_cyaw.p;
     return UALM_OK;
 }
 
