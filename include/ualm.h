@@ -67,6 +67,12 @@ typedef struct {
 /* geometry for map_size_x/y and resolutions exactly as UnevenMap::init computes it (uneven_map.cpp:96-114) */
 void ualm_map_geometry(double map_size_x, double map_size_y, double xy_resolution, double yaw_resolution,
                        ualm_map_geom_t *g);
+/* the same grid centred at (centre_x, centre_y) instead of the world origin: ualm_map_geometry's voxel counts, resolutions and yaw axis,
+ * with origin = centre - size / 2 and max_boundary = centre + size / 2 in x and y.  centre (0, 0) gives ualm_map_geometry's struct bit
+ * for bit.  Every cloud builder crops the cloud to [c - 10, c + 10]^2 about the grid's centre c = (origin + max_boundary) / 2 (the
+ * reference's fixed CropBox about the world origin, uneven_map.cpp:133-137, moved with the grid) */
+void ualm_map_geometry_at(double map_size_x, double map_size_y, double xy_resolution, double yaw_resolution, double centre_x,
+                          double centre_y, ualm_map_geom_t *g);
 
 /* ---- per-problem result record (what the reference prints / returns: alm_traj_opt.cpp:176,252,267,272-273;
  *      alm_traj_opt.h:142) ---- */
@@ -161,6 +167,31 @@ int ualm_update_map_window(ualm_ctx_t *ctx, int ix0, int iy0, int nx, int ny, co
 int ualm_update_map_window_from_cloud(ualm_ctx_t *ctx, const float *pts, int64_t npts, int ix0, int iy0, int nx, int ny,
                                       double ellipsoid_x, double ellipsoid_y, double ellipsoid_z, int iter_num, float *cells_out,
                                       float *kernel_ms);
+/* Move the selected environment's current grid by (dx, dy) whole cells, e.g. to keep a robot-centred grid around a robot that drives,
+ * with the guarantees of ualm_update_map_window: a new version, complete on the device on return, made current; work launched before
+ * keeps its grid and geometry bit for bit; every later launch, ualm_check_trajectories and ualm_submit_replan read the moved one; the
+ * call never waits for running batches.  On any error the previous grid stays current and nothing is written.
+ *   geometry: origin[0] + dx * xy_resolution and max_boundary[0] + dx * xy_resolution (one double expression each), likewise in y with
+ *             dy; voxel_num, the resolutions and the yaw axis stay.
+ *   cells:    new cell (x, y, w) is old cell (x + dx, y + dy, w) wherever that exists, bit for bit.  The cells without a source form at
+ *             most two boxes of the new grid, all yaw layers:
+ *               A, the x strip: [X - min(dx, X), X) x [0, Y) for dx > 0, [0, min(-dx, X)) x [0, Y) for dx < 0, none for dx = 0;
+ *               B, the y strip over the x columns not in A: [Y - min(dy, Y), Y) for dy > 0, [0, min(-dy, Y)) for dy < 0.
+ *             |dx| >= X or |dy| >= Y leaves no source: the whole grid is A and B.
+ *   `cells` (host) holds A's cells, then B's, each in the window layout ([x][y][yaw] float4 restricted to the box).
+ * The kept cells move from version to version through the 8 MB pinned staging buffer of the windows (each x row of the overlap is
+ * contiguous in both), so the host-cells form only needs the copy engines, on both paths.
+ * No grid bound in the selected environment, or a double grid of ualm_set_map_f64: UALM_ESTATE.  dx == dy == 0, a null ctx or cells:
+ * UALM_EINVAL. */
+int ualm_shift_map(ualm_ctx_t *ctx, int dx, int dy, const float *cells);
+/* The same shift with A and B built on the device from a point cloud, e.g. a local scan: the cloud is preprocessed once with the
+ * moved grid's crop, then map_build_kernel runs over both boxes.  Inside the boxes the cells are bit for bit those of a whole-grid
+ * ualm_map_build_device of the same cloud with the moved geometry.  cells_out (optional, host) receives them in `cells`'s layout;
+ * kernel_ms (optional) is the CUDA-event time of both launches.  A null pts or npts < 0 is UALM_EINVAL as well.  Like
+ * ualm_update_map_window_from_cloud, the kernel needs a free SM slot, which on the parity path can mean the tail of the batches in
+ * flight. */
+int ualm_shift_map_from_cloud(ualm_ctx_t *ctx, const float *pts, int64_t npts, int dx, int dy, double ellipsoid_x, double ellipsoid_y,
+                              double ellipsoid_z, int iter_num, float *cells_out, float *kernel_ms);
 
 /* ---- batch solve = B independent optimizeSE2Traj calls ----
  * Ragged inputs are packed back to back in problem order: inner_xy has sum 2(N_b-1) doubles,
@@ -350,8 +381,8 @@ int ualm_map_build_device(ualm_ctx_t *ctx, const float *pts, int64_t npts, const
  * ellipsoid = {0.2,0.1,0.1}, iter_num = 2 in every reference yaml. */
 int ualm_map_build(const float *pts, int64_t npts, const ualm_map_geom_t *g, double ellipsoid_x,
                    double ellipsoid_y, double ellipsoid_z, int iter_num, int nthreads, float *cells);
-/* the cloud ualm_map_build / ualm_map_build_device work on: UnevenMap::init's CropBox + 1 cm VoxelGrid (uneven_map.cpp:133-143), as xyz
- * floats.  Returns the number of points (pts_out may be NULL to query it; UALM_ELIMIT when max_pts is too small). */
+/* the cloud ualm_map_build / ualm_map_build_device work on for a grid centred at the world origin: UnevenMap::init's CropBox
+ * [-10, 10]^2 + 1 cm VoxelGrid (uneven_map.cpp:133-143), as xyz floats (a grid centred at c crops [c - 10, c + 10]^2 instead).  Returns the number of points (pts_out may be NULL to query it; UALM_ELIMIT when max_pts is too small). */
 int64_t ualm_map_preprocess_cloud(const float *pts, int64_t npts, double ellipsoid_x, double ellipsoid_y, double ellipsoid_z, float *pts_out,
                                   int64_t max_pts);
 /* occupancy (uneven_map.cpp:169-179): occ3[X*Y*Yaw], occ2[X*Y] (1 = occupied) */

@@ -199,6 +199,19 @@ public:
         onEnv(env, [&] { return ualm_update_map_window_from_cloud(ctx_, pts, npts, ix0, iy0, nx, ny, ellipsoid_x, ellipsoid_y, ellipsoid_z, iter_num, cells_out, kernel_ms); },
               "ualm_update_map_window_from_cloud");
     }
+    // Move environment `env`'s grid by (dx, dy) whole cells while batches are in flight (ualm_shift_map), same guarantees as
+    // updateEnvironmentWindow; cells: the uncovered boxes A then B, each in the window layout
+    void shiftEnvironment(int env, int dx, int dy, const float *cells_xyzw)
+    {
+        onEnv(env, [&] { return ualm_shift_map(ctx_, dx, dy, cells_xyzw); }, "ualm_shift_map");
+    }
+    // the same shift with A and B built on the device from a point cloud, e.g. a local scan; cells_out (optional) receives A then B
+    void shiftEnvironmentFromCloud(int env, const float *pts, int64_t npts, int dx, int dy, double ellipsoid_x = 0.2, double ellipsoid_y = 0.1,
+                                   double ellipsoid_z = 0.1, int iter_num = 2, float *cells_out = nullptr, float *kernel_ms = nullptr)
+    {
+        onEnv(env, [&] { return ualm_shift_map_from_cloud(ctx_, pts, npts, dx, dy, ellipsoid_x, ellipsoid_y, ellipsoid_z, iter_num, cells_out, kernel_ms); },
+              "ualm_shift_map_from_cloud");
+    }
 
     // ---- single problem, the reference's call (alm_traj_opt.h:92-98), plain pointers ----
     // initStateXY/endStateXY: 2x3 column-major; innerPtsXY: 2 x (N-1) column-major; initYaw/endYaw: 3; innerPtsYaw: M-1

@@ -72,6 +72,8 @@ def lib():
     L.ualm_default_params.restype = None
     L.ualm_map_geometry.argtypes = [C.c_double, C.c_double, C.c_double, C.c_double, C.POINTER(MapGeom)]
     L.ualm_map_geometry.restype = None
+    L.ualm_map_geometry_at.argtypes = [C.c_double] * 6 + [C.POINTER(MapGeom)]
+    L.ualm_map_geometry_at.restype = None
     L.ualm_map_build.argtypes = [fp, C.c_int64, C.POINTER(MapGeom), C.c_double, C.c_double, C.c_double, C.c_int,
                                  C.c_int, fp]
     L.ualm_map_occupancy.argtypes = [fp, C.POINTER(MapGeom), C.c_double, C.c_double, C.POINTER(C.c_uint8),
@@ -141,6 +143,8 @@ def lib():
         L.ualm_update_map_window.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, fp]
         L.ualm_update_map_window_from_cloud.argtypes = [vp, fp, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, fp,
                                                         C.POINTER(C.c_float)]
+        L.ualm_shift_map.argtypes = [vp, C.c_int, C.c_int, fp]
+        L.ualm_shift_map_from_cloud.argtypes = [vp, fp, C.c_int64, C.c_int, C.c_int, C.c_double, C.c_double, C.c_double, C.c_int, fp, C.POINTER(C.c_float)]
         L.ualm_check_trajectories.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, ip, dp, C.c_double, C.POINTER(Limits), dp]
         L.ualm_submit_replan.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, dp, ip, dp, C.c_double, C.POINTER(ResampleParams), C.c_int,
                                          C.POINTER(C.c_int), ip, ip, dp, dp, dp, dp]
@@ -149,7 +153,7 @@ def lib():
                      "ualm_mark_begin", "ualm_mark_end", "ualm_solve_batch_multi", "ualm_pack_records_device_async", "ualm_select_env",
                      "ualm_upload_env", "ualm_solve_batch_env", "ualm_submit_batch_env", "ualm_solve_batch_multi_env", "ualm_update_map",
                      "ualm_update_map_from_cloud", "ualm_update_map_window", "ualm_update_map_window_from_cloud", "ualm_check_trajectories",
-                     "ualm_submit_replan"):
+                     "ualm_submit_replan", "ualm_shift_map", "ualm_shift_map_from_cloud"):
             getattr(L, name).restype = C.c_int
         for name in ("ualm_create", "ualm_destroy", "ualm_set_params", "ualm_set_map", "ualm_solve_batch",
                      "ualm_upload", "ualm_solve_resident", "ualm_sync", "ualm_download", "ualm_last_solve_ms",
@@ -169,4 +173,11 @@ def default_params():
 def map_geometry(size_x=10.0, size_y=10.0, xy_res=0.05, yaw_res=0.1):
     g = MapGeom()
     lib().ualm_map_geometry(size_x, size_y, xy_res, yaw_res, C.byref(g))
+    return g
+
+
+def map_geometry_at(size_x=10.0, size_y=10.0, xy_res=0.05, yaw_res=0.1, centre_x=0.0, centre_y=0.0):
+    """map_geometry's grid centred at (centre_x, centre_y) (ualm_map_geometry_at)"""
+    g = MapGeom()
+    lib().ualm_map_geometry_at(size_x, size_y, xy_res, yaw_res, centre_x, centre_y, C.byref(g))
     return g

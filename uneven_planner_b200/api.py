@@ -167,6 +167,56 @@ class BatchALMTrajOpt:
                                                         ellipsoid[1], ellipsoid[2], iter_num, cells.ctypes.data_as(fp) if cells.size else None, C.byref(ms)))
         return cells, ms.value
 
+    def _shift_geom(self):
+        """the selected environment's geometry as this object last bound it; a shift needs it to lay out the strips and to return the
+        moved geometry, so a grid bound without this object (or none at all) is refused before the library is called"""
+        geom = self.geoms.get(self.env)
+        if geom is None:
+            raise UalmError("environment %d has no grid bound through set_environment / update_environment*: its geometry is unknown" % self.env)
+        return geom
+
+    def shift_environment(self, dx, dy, cells, env=None):
+        """ualm_shift_map: moves environment `env`'s grid (None: the selected one) by (dx, dy) whole cells, with
+        update_environment_window's guarantees.  `cells` holds the cells of the boxes maps.shift_boxes gives, one after the other: a
+        sequence of (nx, ny, Yaw, 4) float32 arrays, or one flat float32 array of them all.  Returns the moved geometry
+        (maps.shift_geometry).  self.map is not moved: the host grid is not copied for a shift."""
+        from . import maps
+        if env is not None:
+            self.select_env(env)
+        flat = np.ascontiguousarray(np.concatenate([np.asarray(c, np.float32).ravel() for c in cells])
+                                    if isinstance(cells, (list, tuple)) else np.asarray(cells, np.float32).ravel())
+        geom = self._shift_geom()
+        want = sum(b[2] * b[3] for b in maps.shift_boxes(geom, dx, dy)) * geom.voxel_num[2] * 4
+        if flat.size != want:
+            raise ValueError("cells must hold %d floats for the shift (%d, %d), got %d" % (want, dx, dy, flat.size))
+        _check(self.L.ualm_shift_map(self.h, int(dx), int(dy), flat.ctypes.data_as(C.POINTER(C.c_float))))
+        self.geoms[self.env] = g = maps.shift_geometry(geom, dx, dy)
+        return g
+
+    def shift_environment_from_cloud(self, pts, dx, dy, ellipsoid=(0.2, 0.1, 0.1), iter_num=2, env=None):
+        """ualm_shift_map_from_cloud: the same shift with the uncovered boxes built on the device from a point cloud (e.g. a local scan)
+        with the moved geometry.  Returns (the moved geometry; the boxes' cells, a list of (nx, ny, Yaw, 4) float32 arrays in
+        maps.shift_boxes's order; kernel ms)."""
+        from . import maps
+        if env is not None:
+            self.select_env(env)
+        pts = np.ascontiguousarray(pts, dtype=np.float32).reshape(-1, 3)
+        fp = C.POINTER(C.c_float)
+        geom = self._shift_geom()
+        boxes = maps.shift_boxes(geom, dx, dy)
+        W = geom.voxel_num[2]
+        flat = np.zeros(sum(b[2] * b[3] for b in boxes) * W * 4, np.float32)
+        ms = C.c_float()
+        _check(self.L.ualm_shift_map_from_cloud(self.h, pts.ctypes.data_as(fp), pts.shape[0], int(dx), int(dy), ellipsoid[0], ellipsoid[1],
+                                                ellipsoid[2], iter_num, flat.ctypes.data_as(fp) if flat.size else None, C.byref(ms)))
+        out, o = [], 0
+        for b in boxes:
+            n = b[2] * b[3] * W * 4
+            out.append(flat[o:o + n].reshape(b[2], b[3], W, 4))
+            o += n
+        self.geoms[self.env] = g = maps.shift_geometry(geom, dx, dy)
+        return g, out, ms.value
+
     def reset_stream(self):
         _check(self.L.ualm_reset_stream(self.h))
         return self

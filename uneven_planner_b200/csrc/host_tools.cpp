@@ -46,19 +46,31 @@ extern "C" void ualm_map_geometry(double sx, double sy, double xy_res, double ya
     g->voxel_num[2] = (int)std::ceil(size[2] / yaw_res);
 }
 
+extern "C" void ualm_map_geometry_at(double sx, double sy, double xy_res, double yaw_res, double cx, double cy, ualm_map_geom_t *g)
+{
+    ualm_map_geometry(sx, sy, xy_res, yaw_res, g);
+    const double c[2] = {cx, cy}, size[2] = {sx, sy};
+    for (int k = 0; k < 2; k++) {
+        g->origin[k] = c[k] - size[k] / 2.0;        // c = 0: -size / 2, ualm_map_geometry's value
+        g->max_boundary[k] = c[k] + size[k] / 2.0;
+    }
+}
+
 namespace {
 struct P3 { float x, y, z; };
 } // namespace
 
-void ualm_map_preprocess(const float *pin, int64_t npts, double ex, double ey, double ez, UalmMapHostPrep &out)
+void ualm_map_preprocess(const float *pin, int64_t npts, double ex, double ey, double ez, double cx, double cy, UalmMapHostPrep &out)
 {
-    // ---- CropBox [-10,10]x[-10,10]x[-0.01,5]  (uneven_map.cpp:133-137)
+    // ---- CropBox [cx-10,cx+10]x[cy-10,cy+10]x[-0.01,5]  (uneven_map.cpp:133-137, whose box is about the world origin: c = 0 there,
+    // where the double bounds are the reference's float bounds exactly)
+    const double xlo = cx - 10.0, xhi = cx + 10.0, ylo = cy - 10.0, yhi = cy + 10.0;
     std::vector<P3> crop;
     crop.reserve((size_t)npts);
     for (int64_t i = 0; i < npts; i++) {
         P3 p{pin[3 * i], pin[3 * i + 1], pin[3 * i + 2]};
         if (!(std::isfinite(p.x) && std::isfinite(p.y) && std::isfinite(p.z))) continue;
-        if (p.x < -10.0f || p.x > 10.0f || p.y < -10.0f || p.y > 10.0f || p.z < -0.01f || p.z > 5.0f) continue;
+        if (p.x < xlo || p.x > xhi || p.y < ylo || p.y > yhi || p.z < -0.01f || p.z > 5.0f) continue;
         crop.push_back(p);
     }
     // ---- VoxelGrid, leaf 1 cm: centroid of the points of each voxel (uneven_map.cpp:140-143)
@@ -110,7 +122,7 @@ extern "C" int64_t ualm_map_preprocess_cloud(const float *pin, int64_t npts, dou
 {
     if (!pin || npts < 0) return UALM_EINVAL;
     UalmMapHostPrep prep;
-    ualm_map_preprocess(pin, npts, ex, ey, ez, prep);
+    ualm_map_preprocess(pin, npts, ex, ey, ez, 0.0, 0.0, prep);      // the crop of a grid centred at the world origin
     const int64_t n = (int64_t)(prep.pts.size() / 3);
     if (pts_out) {
         if (n > max_pts) return UALM_ELIMIT;
@@ -124,7 +136,7 @@ extern "C" int ualm_map_build(const float *pin, int64_t npts, const ualm_map_geo
 {
     if (!pin || !g || !cells || npts < 0) return UALM_EINVAL;
     UalmMapHostPrep prep;
-    ualm_map_preprocess(pin, npts, ex, ey, ez, prep);
+    ualm_map_preprocess(pin, npts, ex, ey, ez, ualm_map_centre(*g, 0), ualm_map_centre(*g, 1), prep);
     const UalmMapPrep view = prep.view(ex, ey, ez, iter_num);
     const int X = g->voxel_num[0], Y = g->voxel_num[1], W = g->voxel_num[2];
     if (nthreads <= 0) nthreads = (int)std::max(1u, std::thread::hardware_concurrency());

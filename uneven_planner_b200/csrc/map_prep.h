@@ -22,4 +22,7 @@ struct UalmMapHostPrep {
         return g;
     }
 };
-void ualm_map_preprocess(const float *pin, int64_t npts, double ex, double ey, double ez, UalmMapHostPrep &out);
+// (cx, cy): the centre of the grid the cloud is for; the crop box is [cx - 10, cx + 10] x [cy - 10, cy + 10] x [-0.01, 5]
+void ualm_map_preprocess(const float *pin, int64_t npts, double ex, double ey, double ez, double cx, double cy, UalmMapHostPrep &out);
+// centre of grid g along axis k (0 = x, 1 = y); exactly 0 for every grid ualm_map_geometry makes
+inline double ualm_map_centre(const ualm_map_geom_t &g, int k) { return (g.origin[k] + g.max_boundary[k]) / 2.0; }

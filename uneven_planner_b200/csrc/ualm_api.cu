@@ -1641,17 +1641,17 @@ __global__ void __launch_bounds__(64) map_build_kernel(UalmMapPrep prep, ualm_ma
 }
 } // namespace ualm
 
-// map_build_kernel on stream st: UnevenMap::init's preprocessing of the cloud on the host, then the cells of the cell box `box`
-// ({ix0, iy0, nx, ny}, all yaw layers) into their places in the whole-grid device buffer dst; the rest of dst is not touched (scratch
-// allocated and freed on st).  cells_out (optional): the box's cells to the host, [nx][ny][yaw] float4; kernel_ms (optional):
-// CUDA-event time of the kernel.  Returns once st has completed the work
-static int map_build_on(cudaStream_t st, const float *pin, int64_t npts, const ualm_map_geom_t *g, int4 box, double ex, double ey, double ez,
-                        int iter_num, float4 *dst, float *cells_out, float *kernel_ms)
+// map_build_kernel on stream st: UnevenMap::init's preprocessing of the cloud on the host (cropped about g's centre), then the cells
+// of the cell boxes boxes[0 .. nbox) ({ix0, iy0, nx, ny}, all yaw layers; empty boxes are skipped) into their places in the whole-grid
+// device buffer dst; the rest of dst is not touched (scratch allocated and freed on st).  cells_out (optional): the boxes' cells to the
+// host one box after the other, each [nx][ny][yaw] float4; kernel_ms (optional): CUDA-event time of the kernels.  Returns once st has
+// completed the work
+static int map_build_on(cudaStream_t st, const float *pin, int64_t npts, const ualm_map_geom_t *g, const int4 *boxes, int nbox, double ex,
+                        double ey, double ez, int iter_num, float4 *dst, float *cells_out, float *kernel_ms)
 {
     UalmMapHostPrep prep;
-    ualm_map_preprocess(pin, npts, ex, ey, ez, prep);
+    ualm_map_preprocess(pin, npts, ex, ey, ez, ualm_map_centre(*g, 0), ualm_map_centre(*g, 1), prep);
     UalmMapPrep view = prep.view(ex, ey, ez, iter_num);
-    const long long row = (long long)box.w * g->voxel_num[2];        // cells per x row of the box
     // scratch and events are released on every exit path (CK returns on the first CUDA error)
     struct Scratch {
         cudaStream_t st;
@@ -1672,16 +1672,23 @@ static int map_build_on(cudaStream_t st, const float *pin, int64_t npts, const u
     CK(cudaMemcpyAsync(sc.start, prep.start.data(), sizeof(int) * prep.start.size(), cudaMemcpyHostToDevice, st));
     view.pts = sc.pts; view.start = sc.start;
     CK(cudaEventRecord(sc.e0, st));
-    for (int x0 = 0; x0 < box.z; x0 += 65535) {          // gridDim.y <= 65535 x rows per launch
-        const int4 part = make_int4(box.x + x0, box.y, std::min(65535, box.z - x0), box.w);
-        map_build_kernel<<<dim3((unsigned)((row + 63) / 64), (unsigned)part.z), 64, 0, st>>>(view, *g, part, dst);
-        CK(cudaGetLastError());
+    for (int b = 0; b < nbox; b++) {
+        const int4 box = boxes[b];
+        const long long row = (long long)box.w * g->voxel_num[2];        // cells per x row of the box
+        for (int x0 = 0; x0 < box.z && row > 0; x0 += 65535) {          // gridDim.y <= 65535 x rows per launch
+            const int4 part = make_int4(box.x + x0, box.y, std::min(65535, box.z - x0), box.w);
+            map_build_kernel<<<dim3((unsigned)((row + 63) / 64), (unsigned)part.z), 64, 0, st>>>(view, *g, part, dst);
+            CK(cudaGetLastError());
+        }
     }
     CK(cudaEventRecord(sc.e1, st));
-    if (cells_out) {
-        const size_t col = sizeof(float4) * g->voxel_num[2], pitch = col * g->voxel_num[1];
+    const size_t col = sizeof(float4) * g->voxel_num[2], pitch = col * g->voxel_num[1];
+    for (int b = 0; b < nbox && cells_out; b++) {
+        const int4 box = boxes[b];
+        if (box.z <= 0 || box.w <= 0) continue;
         CK(cudaMemcpy2DAsync(cells_out, col * box.w, (const char *)dst + pitch * box.x + col * box.y, pitch, col * box.w, box.z,
                              cudaMemcpyDeviceToHost, st));
+        cells_out += 4 * (size_t)box.z * box.w * g->voxel_num[2];
     }
     CK(cudaStreamSynchronize(st));
     if (kernel_ms) CK(cudaEventElapsedTime(kernel_ms, sc.e0, sc.e1));
@@ -1695,7 +1702,8 @@ extern "C" int ualm_map_build_device(ualm_ctx_t *c, const float *pin, int64_t np
     CK(cudaSetDevice(c->device));
     struct Scratch { DevBuf<float4> cells; ~Scratch() { cells.release(); } } sc;
     CK(sc.cells.ensure(map_ncell(g)));
-    return map_build_on(c->b->stream, pin, npts, g, map_box_all(g), ex, ey, ez, iter_num, sc.cells.p, cells, kernel_ms);
+    const int4 all = map_box_all(g);
+    return map_build_on(c->b->stream, pin, npts, g, &all, 1, ex, ey, ez, iter_num, sc.cells.p, cells, kernel_ms);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1732,7 +1740,8 @@ extern "C" int ualm_update_map_from_cloud(ualm_ctx_t *c, const float *pts, int64
     CK(cudaSetDevice(c->device));
     MapRef nv;
     if (int rc = map_version_new(c, map_ncell(g) * sizeof(float4), &nv)) return rc;
-    if (int rc = map_build_on(c->mstream, pts, npts, g, map_box_all(g), ex, ey, ez, iter_num, (float4 *)nv->p, cells_out, kernel_ms)) {
+    const int4 all = map_box_all(g);
+    if (int rc = map_build_on(c->mstream, pts, npts, g, &all, 1, ex, ey, ez, iter_num, (float4 *)nv->p, cells_out, kernel_ms)) {
         cudaStreamSynchronize(c->mstream);      // before the version is freed
         return rc;
     }
@@ -1740,21 +1749,25 @@ extern "C" int ualm_update_map_from_cloud(ualm_ctx_t *c, const float *pts, int64
     return UALM_OK;
 }
 
-// dst <- src (device, `bytes`) on the map stream through the copy engines only: chunks go to the pinned staging buffer and back.  A
-// device-to-device cudaMemcpyAsync runs as a copy kernel, which on the parity path waits for the solve's SMs like any kernel (the
-// driver ignored cudaMemcpyBatchAsync's cudaMemcpyFlagPreferOverlapWithCompute hint there: DESIGN.md section 3h).  The staging
-// buffer is allocated once per context (cudaFreeHost would synchronise the device) and reused in stream order
-static cudaError_t map_copy_ce(ualm_ctx *c, void *dst, const void *src, size_t bytes)
+// dst <- src (device, `rows` rows of `width` bytes, `dpitch` / `spitch` bytes apart) on the map stream through the copy engines only:
+// blocks of rows go to the pinned staging buffer and back, a row wider than the buffer in pieces.  A device-to-device cudaMemcpyAsync
+// runs as a copy kernel, which on the parity path waits for the solve's SMs like any kernel (the driver ignored cudaMemcpyBatchAsync's
+// cudaMemcpyFlagPreferOverlapWithCompute hint there: DESIGN.md section 3h).  The staging buffer is allocated once per context
+// (cudaFreeHost would synchronise the device) and reused in stream order
+static cudaError_t map_copy_ce(ualm_ctx *c, void *dst, size_t dpitch, const void *src, size_t spitch, size_t width, size_t rows)
 {
     if (!c->h_stage) {
         const cudaError_t e = cudaHostAlloc(&c->h_stage, ualm_ctx::STAGE_BYTES, cudaHostAllocDefault);
         if (e != cudaSuccess) { c->h_stage = nullptr; return e; }
     }
-    for (size_t o = 0; o < bytes; o += ualm_ctx::STAGE_BYTES) {
-        const size_t n = std::min(ualm_ctx::STAGE_BYTES, bytes - o);
-        cudaError_t e = cudaMemcpyAsync(c->h_stage, (const char *)src + o, n, cudaMemcpyDeviceToHost, c->mstream);
-        if (e == cudaSuccess) e = cudaMemcpyAsync((char *)dst + o, c->h_stage, n, cudaMemcpyHostToDevice, c->mstream);
-        if (e != cudaSuccess) return e;
+    for (size_t o = 0; o < width; o += ualm_ctx::STAGE_BYTES) {
+        const size_t w = std::min(ualm_ctx::STAGE_BYTES, width - o), k = ualm_ctx::STAGE_BYTES / w;     // k >= 1 rows per block
+        for (size_t r = 0; r < rows; r += k) {
+            const size_t n = std::min(k, rows - r);
+            cudaError_t e = cudaMemcpy2DAsync(c->h_stage, w, (const char *)src + r * spitch + o, spitch, w, n, cudaMemcpyDeviceToHost, c->mstream);
+            if (e == cudaSuccess) e = cudaMemcpy2DAsync((char *)dst + r * dpitch + o, dpitch, c->h_stage, w, w, n, cudaMemcpyHostToDevice, c->mstream);
+            if (e != cudaSuccess) return e;
+        }
     }
     return cudaSuccess;
 }
@@ -1774,10 +1787,10 @@ static int map_window_update(ualm_ctx *c, int ix0, int iy0, int nx, int ny, cons
     if (ix0 < 0 || iy0 < 0 || (long long)ix0 + nx > g.voxel_num[0] || (long long)iy0 + ny > g.voxel_num[1])
         return fail(UALM_EINVAL, std::string(what) + ": the box is outside the grid's voxel_num");
     CK(cudaSetDevice(c->device));
-    const size_t bytes = map_ncell(&g) * sizeof(float4);
+    const size_t pitch = sizeof(float4) * g.voxel_num[1] * g.voxel_num[2];      // one x row of the grid
     MapRef nv;
-    if (int rc = map_version_new(c, bytes, &nv)) return rc;
-    const cudaError_t e = map_copy_ce(c, nv->p, cur->p, bytes);
+    if (int rc = map_version_new(c, pitch * g.voxel_num[0], &nv)) return rc;
+    const cudaError_t e = map_copy_ce(c, nv->p, pitch, cur->p, pitch, pitch, g.voxel_num[0]);
     const int rc = e != cudaSuccess ? fail(UALM_ENOCUDA, std::string(what) + ": " + cudaGetErrorString(e)) : write(g, (float4 *)nv->p);
     const cudaError_t s = cudaStreamSynchronize(c->mstream);       // complete on return; also before a failed version is freed
     if (rc) return rc;
@@ -1803,6 +1816,81 @@ extern "C" int ualm_update_map_window_from_cloud(ualm_ctx_t *c, const float *pts
 {
     if (!c || !pts || npts < 0) return fail(UALM_EINVAL, "null argument or npts < 0");
     return map_window_update(c, ix0, iy0, nx, ny, "ualm_update_map_window_from_cloud", [&](const ualm_map_geom_t &g, float4 *dst) {
-        return map_build_on(c->mstream, pts, npts, &g, make_int4(ix0, iy0, nx, ny), ex, ey, ez, iter_num, dst, cells_out, kernel_ms);
+        const int4 box = make_int4(ix0, iy0, nx, ny);
+        return map_build_on(c->mstream, pts, npts, &g, &box, 1, ex, ey, ez, iter_num, dst, cells_out, kernel_ms);
+    });
+}
+
+// The cell boxes {ix0, iy0, nx, ny} of grid g moved by (dx, dy) cells whose cells have no source before the move: box[0] = A, the x
+// strip; box[1] = B, the y strip over the x columns not in A.  An empty box is {0, 0, 0, 0}
+static void map_shift_boxes(const ualm_map_geom_t &g, int dx, int dy, int4 box[2])
+{
+    const long long X = g.voxel_num[0], Y = g.voxel_num[1];
+    const long long ax = std::min<long long>(std::llabs((long long)dx), X), ay = std::min<long long>(std::llabs((long long)dy), Y);
+    box[0] = ax == 0 ? make_int4(0, 0, 0, 0) : make_int4(dx > 0 ? (int)(X - ax) : 0, 0, (int)ax, (int)Y);
+    box[1] = ay == 0 || ax == X ? make_int4(0, 0, 0, 0) : make_int4(dx < 0 ? (int)ax : 0, dy > 0 ? (int)(Y - ay) : 0, (int)(X - ax), (int)ay);
+}
+
+// ualm_shift_map*: a new version with the selected environment's current geometry moved by (dx, dy) cells, whose overlap with the current
+// version is copied over (map_copy_ce) and whose uncovered boxes A and B (map_shift_boxes) are written by write(moved geometry, boxes,
+// new cells) on the map stream, made current once complete
+template <class F>
+static int map_shift_update(ualm_ctx *c, int dx, int dy, const char *what, F write)
+{
+    if (dx == 0 && dy == 0) return fail(UALM_EINVAL, std::string(what) + ": dx and dy are both 0");
+    const Env &v = c->envs[c->sel_env];
+    if (!v.have_map || !v.map) return fail(UALM_ESTATE, std::string(what) + ": the selected environment has no map grid bound");
+    if (!v.map->dm.cells) return fail(UALM_ESTATE, std::string(what) + ": the selected environment holds a double grid (ualm_set_map_f64); a shift needs the float grid");
+    const MapRef cur = v.map;          // held until the copy below is complete
+    ualm_map_geom_t g = cur->geom;
+    g.origin[0] = g.origin[0] + dx * g.xy_resolution; g.max_boundary[0] = g.max_boundary[0] + dx * g.xy_resolution;
+    g.origin[1] = g.origin[1] + dy * g.xy_resolution; g.max_boundary[1] = g.max_boundary[1] + dy * g.xy_resolution;
+    int4 box[2];
+    map_shift_boxes(g, dx, dy, box);
+    CK(cudaSetDevice(c->device));
+    const long long X = g.voxel_num[0], Y = g.voxel_num[1];
+    const size_t col = sizeof(float4) * g.voxel_num[2], pitch = col * Y;
+    MapRef nv;
+    if (int rc = map_version_new(c, pitch * X, &nv)) return rc;
+    cudaError_t e = cudaSuccess;
+    // the overlap: new columns [x0, x0 + nxo) x [y0, y0 + nyo) from old (x + dx, y + dy); each x row of it is nyo * W float4, contiguous
+    // in both versions and one grid row apart
+    const long long nxo = X - std::min<long long>(std::llabs((long long)dx), X), nyo = Y - std::min<long long>(std::llabs((long long)dy), Y);
+    if (nxo > 0 && nyo > 0) {
+        const long long x0 = std::max(0, -dx), y0 = std::max(0, -dy);
+        e = map_copy_ce(c, (char *)nv->p + pitch * x0 + col * y0, pitch, (const char *)cur->p + pitch * (x0 + dx) + col * (y0 + dy), pitch,
+                        col * nyo, nxo);
+    }
+    const int rc = e != cudaSuccess ? fail(UALM_ENOCUDA, std::string(what) + ": " + cudaGetErrorString(e)) : write(g, box, (float4 *)nv->p);
+    const cudaError_t s = cudaStreamSynchronize(c->mstream);       // complete on return; also before a failed version is freed
+    if (rc) return rc;
+    if (s != cudaSuccess) return fail(UALM_ENOCUDA, std::string(what) + ": " + cudaGetErrorString(s));
+    map_install(c, &g, std::move(nv));
+    return UALM_OK;
+}
+
+extern "C" int ualm_shift_map(ualm_ctx_t *c, int dx, int dy, const float *cells)
+{
+    if (!c || !cells) return fail(UALM_EINVAL, "null argument");
+    // A then B from the host array, one strided host-to-device copy each (as a window's): copy engines only
+    return map_shift_update(c, dx, dy, "ualm_shift_map", [&](const ualm_map_geom_t &g, const int4 *box, float4 *dst) {
+        const size_t col = sizeof(float4) * g.voxel_num[2], pitch = col * g.voxel_num[1];
+        const char *src = (const char *)cells;
+        for (int b = 0; b < 2; b++) {
+            if (box[b].z <= 0 || box[b].w <= 0) continue;
+            CK(cudaMemcpy2DAsync((char *)dst + pitch * box[b].x + col * box[b].y, pitch, src, col * box[b].w, col * box[b].w, box[b].z,
+                                 cudaMemcpyHostToDevice, c->mstream));
+            src += col * box[b].w * box[b].z;
+        }
+        return UALM_OK;
+    });
+}
+
+extern "C" int ualm_shift_map_from_cloud(ualm_ctx_t *c, const float *pts, int64_t npts, int dx, int dy, double ex, double ey, double ez, int iter_num,
+                                         float *cells_out, float *kernel_ms)
+{
+    if (!c || !pts || npts < 0) return fail(UALM_EINVAL, "null argument or npts < 0");
+    return map_shift_update(c, dx, dy, "ualm_shift_map_from_cloud", [&](const ualm_map_geom_t &g, const int4 *box, float4 *dst) {
+        return map_build_on(c->mstream, pts, npts, &g, box, 2, ex, ey, ez, iter_num, dst, cells_out, kernel_ms);
     });
 }

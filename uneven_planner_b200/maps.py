@@ -20,7 +20,9 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 BUILT_DIR = os.path.join(ROOT, "maps_built")          # git-ignored, travels with gpurun snapshots
 REF_MAPS = "/root/reference/src/uneven_planner/uneven_map/maps"   # only present in the build container
-MAGIC = b"UMAP0001"
+MAGIC = b"UMAP0001"            # a grid map_geometry rebuilds from the header's extents and resolutions: 64-byte header
+MAGIC_V2 = b"UMAP0002"         # any other grid (e.g. one moved with ualm_shift_map), stored raw: 128-byte header
+HEADER_BYTES = {MAGIC: 64, MAGIC_V2: 128}
 
 # per-terrain cloud files and occupancy thresholds live in configs.TERRAINS (one table, derived from the reference's yaml files)
 from .configs import TERRAINS  # noqa: E402
@@ -58,23 +60,35 @@ class UnevenMapData:
         return self._occ[key]
 
     def save(self, path):
+        """A grid that map_geometry rebuilds bit for bit from its extents (2 |origin|) and resolutions is written as UMAP0001, whose header
+        holds those; any other (off-centre, or centred with bounds map_geometry does not give, e.g. after shifts away and back) as
+        UMAP0002, whose header holds voxel_num, origin, max_boundary and both resolutions raw."""
         g = self.geom
         os.makedirs(os.path.dirname(path), exist_ok=True)
+        v1 = struct.pack("<4d", abs(g.origin[0]) * 2, abs(g.origin[1]) * 2, g.xy_resolution, g.yaw_resolution)
         with open(path + ".tmp", "wb") as f:
-            hdr = MAGIC + struct.pack("<3i", *g.voxel_num) + struct.pack("<4d", abs(g.origin[0]) * 2, abs(g.origin[1]) * 2,
-                                                                       g.xy_resolution, g.yaw_resolution)
-            f.write(hdr.ljust(64, b"\0"))
+            if bytes(_lib.map_geometry(*struct.unpack("<4d", v1))) == bytes(g):
+                hdr = MAGIC + struct.pack("<3i", *g.voxel_num) + v1
+            else:
+                hdr = MAGIC_V2 + struct.pack("<3i", *g.voxel_num) + struct.pack("<8d", *g.origin, *g.max_boundary, g.xy_resolution,
+                                                                              g.yaw_resolution)
+            f.write(hdr.ljust(HEADER_BYTES[hdr[:8]], b"\0"))
             f.write(self.cells.tobytes())
         os.replace(path + ".tmp", path)
 
     @staticmethod
     def load(path, name=None):
         with open(path, "rb") as f:
-            hdr = f.read(64)
-            assert hdr[:8] == MAGIC, "not a .umap file"
+            magic = f.read(8)
+            assert magic in HEADER_BYTES, "not a .umap file"
+            hdr = magic + f.read(HEADER_BYTES[magic] - 8)
             X, Y, W = struct.unpack("<3i", hdr[8:20])
-            sx, sy, rx, ry = struct.unpack("<4d", hdr[20:52])
-            geom = _lib.map_geometry(sx, sy, rx, ry)
+            if magic == MAGIC:
+                sx, sy, rx, ry = struct.unpack("<4d", hdr[20:52])
+                geom = _lib.map_geometry(sx, sy, rx, ry)
+            else:
+                v = struct.unpack("<8d", hdr[20:84])
+                geom = _lib.MapGeom((X, Y, W), v[0:3], v[3:6], v[6], v[7])
             assert tuple(geom.voxel_num) == (X, Y, W)
             cells = np.frombuffer(f.read(), dtype=np.float32).reshape(X, Y, W, 4)
         return UnevenMapData(geom, cells, name or os.path.basename(path))
@@ -124,6 +138,31 @@ def window_box(geom, x0, y0, x1, y1):
     if ix1 < ix0 or iy1 < iy0:
         raise ValueError("the rectangle [%g, %g] x [%g, %g] is outside the grid" % (x0, x1, y0, y1))
     return ix0, iy0, ix1 - ix0 + 1, iy1 - iy0 + 1
+
+
+def shift_geometry(geom, dx, dy):
+    """The geometry of grid `geom` moved by (dx, dy) whole cells, with ualm_shift_map's expressions (origin + d * xy_resolution and
+    max_boundary + d * xy_resolution, in x and y)."""
+    g = _lib.MapGeom.from_buffer_copy(geom)
+    r = geom.xy_resolution
+    g.origin[0] = geom.origin[0] + dx * r
+    g.max_boundary[0] = geom.max_boundary[0] + dx * r
+    g.origin[1] = geom.origin[1] + dy * r
+    g.max_boundary[1] = geom.max_boundary[1] + dy * r
+    return g
+
+
+def shift_boxes(geom, dx, dy):
+    """The cell boxes (ix0, iy0, nx, ny) of grid `geom` moved by (dx, dy) cells whose cells have no source before the move, in the
+    order ualm_shift_map takes their cells: A, the x strip, then B, the y strip over the x columns not in A.  Empty boxes are left out."""
+    X, Y, _ = geom.voxel_num
+    ax, ay = min(abs(dx), X), min(abs(dy), Y)
+    boxes = []
+    if ax:
+        boxes.append((X - ax if dx > 0 else 0, 0, ax, Y))
+    if ay and ax < X:
+        boxes.append((ax if dx < 0 else 0, Y - ay if dy > 0 else 0, X - ax, ay))
+    return boxes
 
 
 def terrain_path(name):
