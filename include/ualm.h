@@ -30,7 +30,7 @@ extern "C" {
 #define UALM_ENOCUDA (-1)   /* no usable CUDA device / CUDA runtime error (message via ualm_last_error) */
 #define UALM_EINVAL (-2)    /* bad argument */
 #define UALM_ESTATE (-3)    /* call order (no map / no params / nothing uploaded) */
-#define UALM_ELIMIT (-4)    /* problem exceeds compiled limits (N, M, int_K) */
+#define UALM_ELIMIT (-4)    /* problem exceeds compiled limits (N, M; int_K, mem_size, past in ualm_set_params) */
 
 /* ret_code of a problem whose solve was stopped early (no such exit exists in the reference; it is modelled on its earlyExit).
  * Three causes stop a problem: its evaluation budget (ualm_set_budget), a deadline (ualm_wait_batch_for, which cancels every
@@ -81,7 +81,10 @@ typedef struct {
                                 the evaluation budget (ualm_set_budget), a deadline (ualm_wait_batch_for) or a cancel
                                 (ualm_cancel_problems) stopped it, see above;
                                 UALM_ELIMIT (-4): this problem exceeds the compiled limits (N <= 64, M <= 128) and was not solved --
-                                the rest of its batch is unaffected */
+                                the rest of its batch is unaffected.  Every problem within them is solved at any int_K that
+                                ualm_set_params accepts, in any batch, bit for bit what it gives alone: on the parity path one
+                                whose shared-memory layout does not fit four one-warp slots to a CTA is given a group of two or
+                                four warps (with UALM_GROUPS=0, a developer switch, ualm_upload refuses such a batch instead) */
     int32_t outer_iters;
     int32_t n_evals;         /* cost+gradient evaluations */
     int32_t n_lbfgs_iters;   /* accepted line searches */

@@ -13,6 +13,7 @@
 #include <cstdlib>
 #include <cstring>
 #include <memory>
+#include <mutex>
 #include <numeric>
 #include <string>
 #include <thread>
@@ -79,7 +80,8 @@ struct Lane {
     // the one-warp-per-problem kernels run once per environment present, over its slice of d_eidx (batch.eidx)
     DevBuf<int> d_eidx;
     SmemLayout eL[UALM_MAX_ENVS];        // their layouts (maxima over the environment's problems)
-    size_t esmem[UALM_MAX_ENVS] = {};
+    size_t esmem[UALM_MAX_ENVS] = {};    // dynamic shared memory of one of their CTAs: ewpb slots of eL
+    int ewpb[UALM_MAX_ENVS] = {};        // their warps per CTA
     long long tot_hist = 0, tot_scr = 0, tot_fac = 0, tot_ws = 0;
     DevBuf<ProbDesc> d_desc;
     DevBuf<int> d_order;
@@ -457,11 +459,73 @@ extern "C" int ualm_set_map_f64(ualm_ctx_t *c, const ualm_map_geom_t *g, const d
     return map_write_current(c, g, cells, 4 * ncell * sizeof(double), true);
 }
 
-// the one-warp-per-problem layout of every environment present in the lane's batch (sized by that environment's maxima)
+// Per device: the dynamic shared memory a CTA of every parity kernel may use (the opt-in per-block maximum, 227 KB on an H100,
+// less the largest static shared memory of those kernels), and how far their dynamic shared-memory attribute has been raised.  The
+// attribute belongs to the function on the current device, so it is kept per device, and only ever raised (kernels of another
+// lane or context on the same device may be in flight with a larger size)
+struct SmemDev { size_t cap = 0, raised = 0; };
+static std::mutex g_smem_mu;
+static std::vector<SmemDev> g_smem;
+
+static int smem_dev(ualm_ctx *c, SmemDev **out)
+{
+    if ((size_t)c->device >= g_smem.size()) g_smem.resize(c->device + 1);
+    SmemDev &s = g_smem[c->device];
+    if (!s.cap) {
+        CK(cudaSetDevice(c->device));
+        int optin = 0;
+        CK(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, c->device));
+        size_t stat = 0;
+        const void *ks[] = {(const void *)solve_kernel, (const void *)eval_kernel, (const void *)scaling_kernel, (const void *)penalty_only_kernel};
+        for (const void *k : ks) {
+            cudaFuncAttributes fa;
+            CK(cudaFuncGetAttributes(&fa, k));
+            stat = std::max(stat, fa.sharedSizeBytes);
+        }
+        if ((size_t)optin <= stat) return fail(UALM_ENOCUDA, "device has too little shared memory per block");
+        s.cap = (size_t)optin - stat;
+    }
+    *out = &s;
+    return UALM_OK;
+}
+
+static int smem_cap(ualm_ctx *c, size_t *cap)
+{
+    std::lock_guard<std::mutex> g(g_smem_mu);
+    SmemDev *s;
+    if (int rc = smem_dev(c, &s)) return rc;
+    *cap = s->cap;
+    return UALM_OK;
+}
+
+// the parity kernels' attribute on the context's device raised to at least `bytes` (at most the device's cap)
+static int smem_raise(ualm_ctx *c, size_t bytes)
+{
+    std::lock_guard<std::mutex> g(g_smem_mu);
+    SmemDev *s;
+    if (int rc = smem_dev(c, &s)) return rc;
+    if (bytes <= s->raised) return UALM_OK;
+    CK(cudaSetDevice(c->device));
+    CK(cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    CK(cudaFuncSetAttribute(eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    CK(cudaFuncSetAttribute(scaling_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    CK(cudaFuncSetAttribute(penalty_only_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    s->raised = bytes;
+    return UALM_OK;
+}
+
+// one trajectory slot of layout L fits four to a CTA of `cap` bytes (a one-warp solve launch)
+static bool fits_four(const SmemLayout &L, size_t cap) { return (size_t)UALM_WPB * L.total_doubles * sizeof(double) <= cap; }
+
+// the one-warp-per-problem layout of every environment present in the lane's batch (sized by that environment's maxima), and how
+// many of those warps share a CTA: up to UALM_WPB, as many as a CTA's shared memory holds (eval_kernel, scaling_kernel and
+// penalty_only_kernel take their warps per CTA from blockDim)
 static int prepare_launch(ualm_ctx *c)
 {
     Lane *b = c->b;
     const BatchLayout &L = b->batch;
+    size_t cap = 0;
+    if (int rc = smem_cap(c, &cap)) return rc;
     for (int e = 0; e < UALM_MAX_ENVS; e++) {
         if (L.eoff[e + 1] == L.eoff[e]) continue;
         int Nm = 1, Mm = 1, nm = 1, Sm = 1;
@@ -472,17 +536,12 @@ static int prepare_launch(ualm_ctx *c)
         }
         const DevParams &dp = c->envs[e].dp;
         b->eL[e] = make_layout(Nm, Mm, nm, dp.mem_size, dp.past, dp.int_K, Sm);
-        b->esmem[e] = (size_t)b->eL[e].total_doubles * sizeof(double) * UALM_WPB;
-        if (b->esmem[e] > 227 * 1024) return fail(UALM_ELIMIT, "problem too large for shared memory (N/M/int_K too big)");
-        // the attribute is per function, not per lane: only ever raise it (another lane's kernels may be in flight with a larger size)
-        static size_t smem_max = 0;
-        if (b->esmem[e] > smem_max) {
-            smem_max = b->esmem[e];
-            CK(cudaFuncSetAttribute(solve_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
-            CK(cudaFuncSetAttribute(eval_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
-            CK(cudaFuncSetAttribute(scaling_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
-            CK(cudaFuncSetAttribute(penalty_only_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem_max));
-        }
+        const size_t slot = (size_t)b->eL[e].total_doubles * sizeof(double);
+        b->ewpb[e] = (int)std::min<size_t>(UALM_WPB, cap / slot);
+        // within the compiled limits (N <= 64, M <= 128, int_K <= 128, past <= 16) a slot is under 64 KB: three fit at least
+        if (b->ewpb[e] < 1) return fail(UALM_ELIMIT, "problem too large for shared memory (N/M/int_K too big)");
+        b->esmem[e] = slot * b->ewpb[e];
+        if (int rc = smem_raise(c, b->esmem[e])) return rc;
     }
     return UALM_OK;
 }
@@ -633,6 +692,15 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
     const int BA = L.n_active;
     // launch order: most samples first (longest-processing-time-first keeps the tail short)
     std::stable_sort(l->order.begin(), l->order.end(), [&](int a, int b2) { return l->desc[a].S > l->desc[b2].S; });
+    // a problem whose own layout does not fit four to a CTA (N, M and int_K near their limits) is solved by a group of two or four
+    // warps (a G=4 CTA holds one slot, a G=2 CTA two): these "wide" problems go first, so the group-size ranges below give them one
+    size_t cap = 0;
+    if (int rc = smem_cap(c, &cap)) return rc;
+    const long long n_wide = std::stable_partition(l->order.begin(), l->order.end(), [&](int b2) {
+        const ProbDesc &d = l->desc[b2];
+        const DevParams &ep = c->envs[L.env[b2]].dp;
+        return !fits_four(make_layout(d.N, d.M, d.n, ep.mem_size, ep.past, ep.int_K, d.S), cap);
+    }) - l->order.begin();
     int rc0 = prepare_launch(c);
     if (rc0) return rc0;
     // Warp groups and launches.  Problems are sorted by size; the largest get 4 or 2 warps (helpers for the parallel phases) as
@@ -673,6 +741,11 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
                 K4 = (long long)(BA * (getenv("UALM_F4") ? atof(getenv("UALM_F4")) : 0.0));
                 K2 = std::min<long long>(BA - K4, (long long)(BA * (getenv("UALM_F2") ? atof(getenv("UALM_F2")) : 0.0))) & ~1LL;
             }
+            if (K4 + K2 < n_wide) {
+                if (!c->group_mode && !forced)
+                    return fail(UALM_ELIMIT, "UALM_GROUPS=0: a problem's shared-memory layout does not fit four one-warp slots per CTA (N/M/int_K too big)");
+                K2 = n_wide - K4;
+            }
             // rank ranges per group size; within one, the problems of each environment (a launch holds one: its parameters and grid
             // are the launch's grid constants)
             std::vector<Lane::GClass> cls;
@@ -684,18 +757,23 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
                 std::stable_sort(ord.begin() + lim[gi], ord.begin() + lim[gi + 1], [&](int x, int y) { return L.env[x] < L.env[y]; });
                 for (long long a = lim[gi], b2; a < lim[gi + 1]; a = b2) {
                     const int ce = L.env[ord[a]];
-                    for (b2 = a; b2 < lim[gi + 1] && L.env[ord[b2]] == ce; b2++) {}
                     const DevParams &ep = c->envs[ce].dp;
                     Lane::GClass cl;
-                    cl.G = G; cl.env = ce; cl.r0 = (int)a; cl.r1 = (int)b2;
+                    cl.G = G; cl.env = ce; cl.r0 = (int)a;
+                    // the range's problems of one environment; a one-warp launch also ends before a problem that would take the
+                    // layout of its maxima past four slots per CTA (each problem of that range fits alone: the wide ones come first)
                     int Nm = 1, Mm = 1, nm = 1, Sm = 1;
-                    for (long long r = a; r < b2; r++) {
-                        const ProbDesc &d = l->desc[ord[r]];
-                        Nm = std::max(Nm, d.N); Mm = std::max(Mm, d.M); nm = std::max(nm, d.n); Sm = std::max(Sm, d.S);
+                    for (b2 = a; b2 < lim[gi + 1] && L.env[ord[b2]] == ce; b2++) {
+                        const ProbDesc &d = l->desc[ord[b2]];
+                        const int N2 = std::max(Nm, d.N), M2 = std::max(Mm, d.M), n2 = std::max(nm, d.n), S2 = std::max(Sm, d.S);
+                        if (G == 1 && b2 > a && !fits_four(make_layout(N2, M2, n2, ep.mem_size, ep.past, ep.int_K, S2), cap)) break;
+                        Nm = N2; Mm = M2; nm = n2; Sm = S2;
                     }
+                    cl.r1 = (int)b2;
                     cl.L = make_layout(Nm, Mm, nm, ep.mem_size, ep.past, ep.int_K, Sm);
                     const int per = 4 / G;                         // trajectory slots per CTA
                     cl.smem = ((size_t)per * cl.L.total_doubles + (size_t)(4 - per) * RINGD) * sizeof(double);
+                    if (int rc = smem_raise(c, cl.smem)) return rc;
                     CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&cl.occ, solve_kernel, UALM_THREADS * UALM_WPB, cl.smem));
                     cl.n_ctas = (int)((b2 - a + per - 1) / per);
                     cl.grid = (int)std::min<long long>(cl.n_ctas, (long long)std::max(cl.occ, 1) * dev_sms);
@@ -1208,7 +1286,8 @@ extern "C" int ualm_eval_batch(ualm_ctx_t *c, const double *x, const double *lam
         if ((rc = per_env(c, [&](int e, const BatchPtrs &bp, int cnt) {
                  BatchPtrs be = bp;
                  if (x) be.x0 = l->d_xev.p;
-                 eval_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(be, c->envs[e].dp, c->envs[e].map->dm, l->eL[e], rho);
+                 const int wpb = l->ewpb[e];
+                 eval_kernel<<<(cnt + wpb - 1) / wpb, UALM_THREADS * wpb, l->esmem[e], l->stream>>>(be, c->envs[e].dp, c->envs[e].map->dm, l->eL[e], rho);
              })))
             return rc;
         if (f) CK(cudaMemcpyAsync(f, l->d_f.p, sizeof(double) * L.B, cudaMemcpyDeviceToHost, l->stream));
@@ -1232,7 +1311,8 @@ extern "C" int ualm_init_scaling_batch(ualm_ctx_t *c, double *scale_fx, double *
     CK(cudaSetDevice(c->device));
     if (L.B > 0) {
         if (int rc = per_env(c, [&](int e, const BatchPtrs &bp, int cnt) {
-                scaling_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].map->dm, l->eL[e]);
+                const int wpb = l->ewpb[e];
+                scaling_kernel<<<(cnt + wpb - 1) / wpb, UALM_THREADS * wpb, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].map->dm, l->eL[e]);
             }))
             return rc;
         if (scale_fx) CK(cudaMemcpyAsync(scale_fx, l->d_sfx.p, sizeof(double) * L.B, cudaMemcpyDeviceToHost, l->stream));
@@ -1261,9 +1341,10 @@ extern "C" int ualm_time_penalty_kernel(ualm_ctx_t *c, int reps, float *ms_per_l
     if ((rc = put(c, l->d_scale_cx.p, nullptr, 7 * L.tot_s, 1.0))) return rc;
     const int e = L.env[0];
     const BatchPtrs bp = batch_ptrs(c);
-    penalty_only_kernel<<<(L.B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].map->dm, l->eL[e], 1); // warm-up
+    const int wpb = l->ewpb[e];
+    penalty_only_kernel<<<(L.B + wpb - 1) / wpb, UALM_THREADS * wpb, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].map->dm, l->eL[e], 1); // warm-up
     CK(cudaEventRecord(l->ev0, l->stream));
-    penalty_only_kernel<<<(L.B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].map->dm, l->eL[e], reps);
+    penalty_only_kernel<<<(L.B + wpb - 1) / wpb, UALM_THREADS * wpb, l->esmem[e], l->stream>>>(bp, c->envs[e].dp, c->envs[e].map->dm, l->eL[e], reps);
     CK(cudaEventRecord(l->ev1, l->stream));
     CK(cudaGetLastError());
     CK(cudaEventSynchronize(l->ev1));

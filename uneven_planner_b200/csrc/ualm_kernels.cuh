@@ -2331,7 +2331,7 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) solve_kernel(const __
 __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) eval_kernel(const __grid_constant__ BatchPtrs bp, const __grid_constant__ DevParams p, const __grid_constant__ DevMap map,
         const __grid_constant__ SmemLayout L, R rho)
 {
-    const int lane = threadIdx.x & 31, wslot = blockIdx.x * UALM_WPB + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31, wslot = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);   // 1 .. UALM_WPB warps per CTA
     if (wslot >= bp.n_active) return;   // whole warp exits; warps never synchronise with each other
     const unsigned sm = (unsigned)__cvta_generic_to_shared(ualm_smem) + 8u * (unsigned)((threadIdx.x >> 5) * L.total_doubles);
     const int prob = bp.order[wslot];
@@ -2353,7 +2353,7 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) eval_kernel(const __g
 __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) scaling_kernel(const __grid_constant__ BatchPtrs bp, const __grid_constant__ DevParams p, const __grid_constant__ DevMap map,
         const __grid_constant__ SmemLayout L)
 {
-    const int lane = threadIdx.x & 31, wslot = blockIdx.x * UALM_WPB + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31, wslot = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);   // 1 .. UALM_WPB warps per CTA
     if (wslot >= bp.n_active) return;   // whole warp exits; warps never synchronise with each other
     const unsigned sm = (unsigned)__cvta_generic_to_shared(ualm_smem) + 8u * (unsigned)((threadIdx.x >> 5) * L.total_doubles);
     const int prob = bp.order[wslot];
@@ -2372,7 +2372,7 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) scaling_kernel(const 
 __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) penalty_only_kernel(const __grid_constant__ BatchPtrs bp, const __grid_constant__ DevParams p, const __grid_constant__ DevMap map,
         const __grid_constant__ SmemLayout L, int reps)
 {
-    const int lane = threadIdx.x & 31, wslot = blockIdx.x * UALM_WPB + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31, wslot = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);   // 1 .. UALM_WPB warps per CTA
     if (wslot >= bp.n_active) return;   // whole warp exits; warps never synchronise with each other
     const unsigned sm = (unsigned)__cvta_generic_to_shared(ualm_smem) + 8u * (unsigned)((threadIdx.x >> 5) * L.total_doubles);
     const int prob = bp.order[wslot];
