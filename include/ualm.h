@@ -277,6 +277,30 @@ int ualm_cancel_problems(ualm_ctx_t *ctx, int ticket, int n, const int32_t *idx)
  * ualm_solve_resident, ualm_submit_batch, ualm_solve_batch_multi through each context): max_evals = 0 (the default) is none,
  * negative values are UALM_EINVAL.  Refused (UALM_ESTATE) while a submitted batch is in flight. */
 int ualm_set_budget(ualm_ctx_t *ctx, int32_t max_evals);
+/* Urgent work: urgent = 1 makes the calls after it urgent until urgent = 0: ualm_submit_batch / ualm_submit_batch_env,
+ * ualm_submit_replan (its build and the ticket it submits) and ualm_check_trajectories.  No other call changes.  Any other value or
+ * a null ctx is UALM_EINVAL.  Allowed at any time, also while batches are in flight; like ualm_set_budget it acts on the calls made
+ * after it.
+ * Every record, coefficient, built replan row and check row is bit for bit what the same call gives without urgency, and so is
+ * every other ticket's, on both paths: urgency only changes when work runs.
+ * Parity path (precision 64): from the point an urgent piece of work is reached on its stream, every non-urgent solve launch of the
+ * context (every ticket, and the batches of ualm_solve_resident / ualm_solve_batch) stops taking new problems from its work queue.
+ * A problem already running is never interrupted; a launch's CTAs exit once their slots are between problems (a slot that stops may
+ * join its CTA mate's problem, as at the end of the queue).  The held launches resume on the device, without a host call, when the
+ * urgent work no longer needs slots: for an urgent ticket once every one of its problems has been taken (started, not finished),
+ * so a ticket larger than the resident slots holds others back only until its last wave has started; for an urgent check or replan
+ * build once its kernels have completed.  The urgent ticket's launches run on streams of the greatest priority.
+ * Throughput path (precision 32 / 65): an urgent ticket's admission and round loops run on streams of the greatest priority.  The
+ * check and the replan build run on the greatest-priority check stream on both paths anyway, so urgency changes nothing else there.
+ * Bound: the launches of a held solve wait at most 2 s in all (by the device's global timer, summed over every hold it meets); after
+ * that the solve resumes and takes no further hold for the rest of its run, so a hold that is never released can only slow work
+ * down, never hang the device.  The hold of an urgent ticket is raised after the submit's host-side allocations: a submit whose lane
+ * must grow first waits for the device, as without urgency, and nothing is held meanwhile.  Cost: on the parity path every hold
+ * leaves the SMs it empties idle until the urgent work is placed, so frequent urgent calls lower the throughput of everything else
+ * (DESIGN.md section 3k).
+ * Polls, cancels, deadlines (ualm_wait_batch_for) and the budget behave as documented on urgent and on held tickets; a held ticket's
+ * deadline drain can be delayed by the hold, at most by the bound. */
+int ualm_set_urgent(ualm_ctx_t *ctx, int urgent);
 int ualm_mark_begin(ualm_ctx_t *ctx);
 int ualm_mark_end(ualm_ctx_t *ctx, float *ms);
 

@@ -151,6 +151,9 @@ public:
     void init() { check(ualm_set_params(ctx_, &params), "ualm_set_params"); }
     // evaluation budget per problem of the following solves (0 = none); a stopped problem returns UALM_RET_STOPPED (ualm.h)
     void setBudget(int max_evals) { check(ualm_set_budget(ctx_, max_evals), "ualm_set_budget"); }
+    // ualm_set_urgent: the submitBatch / submitReplan / checkTrajectories calls after it go ahead of the batches in flight, with the same
+    // results, until setUrgent(false)
+    void setUrgent(bool urgent) { check(ualm_set_urgent(ctx_, urgent ? 1 : 0), "ualm_set_urgent"); }
 
     // ALMTrajOpt::setEnvironment(UnevenMap::Ptr): the map grid (UnevenMap::map_buffer is private in the reference,
     // uneven_map.h:91, so the maintainer-side binding passes geometry + a float4 view of the cells; INTEGRATION.md)

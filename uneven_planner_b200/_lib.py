@@ -129,6 +129,7 @@ def lib():
         L.ualm_poll_batch.argtypes = [vp, C.c_int, C.c_double, ip, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(Result), dp, dp]
         L.ualm_cancel_problems.argtypes = [vp, C.c_int, C.c_int, ip]
         L.ualm_set_budget.argtypes = [vp, C.c_int32]
+        L.ualm_set_urgent.argtypes = [vp, C.c_int]
         L.ualm_mark_begin.argtypes = [vp]
         L.ualm_mark_end.argtypes = [vp, C.POINTER(C.c_float)]
         L.ualm_solve_batch_multi.argtypes = [C.POINTER(vp), C.c_int, C.c_int, ip, ip, dp, dp, dp, dp, C.POINTER(Result), dp, dp]
@@ -149,7 +150,7 @@ def lib():
         L.ualm_submit_replan.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, dp, ip, dp, C.c_double, C.POINTER(ResampleParams), C.c_int,
                                          C.POINTER(C.c_int), ip, ip, dp, dp, dp, dp]
         for name in ("ualm_reset_stream", "ualm_set_map_f64", "ualm_max_lanes", "ualm_select_lane", "ualm_submit_batch", "ualm_wait_batch",
-                     "ualm_wait_batch_for", "ualm_poll_batch", "ualm_cancel_problems", "ualm_set_budget",
+                     "ualm_wait_batch_for", "ualm_poll_batch", "ualm_cancel_problems", "ualm_set_budget", "ualm_set_urgent",
                      "ualm_mark_begin", "ualm_mark_end", "ualm_solve_batch_multi", "ualm_pack_records_device_async", "ualm_select_env",
                      "ualm_upload_env", "ualm_solve_batch_env", "ualm_submit_batch_env", "ualm_solve_batch_multi_env", "ualm_update_map",
                      "ualm_update_map_from_cloud", "ualm_update_map_window", "ualm_update_map_window_from_cloud", "ualm_check_trajectories",

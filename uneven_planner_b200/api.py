@@ -8,6 +8,7 @@ A context holds up to UALM_MAX_ENVS environments (parameter set + map grid): ini
 bind environment k, and a batch whose `env` array is set solves every problem in its own environment (ProblemBatch.env).
 All compute happens inside libualm.so on the GPU; this file only marshals numpy arrays.
 """
+import contextlib
 import ctypes as C
 
 import numpy as np
@@ -236,8 +237,21 @@ class BatchALMTrajOpt:
         _check(self.L.ualm_mark_end(self.h, C.byref(ms)))
         return ms.value
 
-    def submit(self, pb, depth=2, host=None):
-        """ualm_submit_batch: returns a ticket; `host` = optional pre-made (N, M, bnd, T, ixy, iyaw) host arrays (e.g. pinned)."""
+    @contextlib.contextmanager
+    def _urgency(self, urgent):
+        """ualm_set_urgent(urgent) around one call, and the context's flag back to 0 after it"""
+        if not urgent:
+            yield
+            return
+        _check(self.L.ualm_set_urgent(self.h, 1))
+        try:
+            yield
+        finally:
+            _check(self.L.ualm_set_urgent(self.h, 0))
+
+    def submit(self, pb, depth=2, host=None, urgent=False):
+        """ualm_submit_batch: returns a ticket; `host` = optional pre-made (N, M, bnd, T, ixy, iyaw) host arrays (e.g. pinned).
+        urgent: the ticket goes ahead of the batches in flight (ualm_set_urgent), with the same results."""
         if host is None:
             host = [np.ascontiguousarray(a) for a in (pb.N.astype(np.int32), pb.M.astype(np.int32), pb.bnd.astype(np.float64),
                                                         pb.total_time.astype(np.float64), pb.inner_xy.astype(np.float64),
@@ -245,8 +259,9 @@ class BatchALMTrajOpt:
         N, M, bnd, T, ixy, iyaw = host
         t = C.c_int(-1)
         env = _env(pb)
-        _check(self.L.ualm_submit_batch_env(self.h, pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), _p(env, ip), int(depth),
-                                            C.byref(t)))
+        with self._urgency(urgent):
+            _check(self.L.ualm_submit_batch_env(self.h, pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), _p(env, ip), int(depth),
+                                                C.byref(t)))
         if not hasattr(self, "_tickets"):
             self._tickets = {}
         self._tickets[t.value] = (pb, (host, env))
@@ -451,19 +466,21 @@ class BatchALMTrajOpt:
                                               None if lim is None else C.byref(lim), _p(out)))
         return out
 
-    def check_results(self, pb, out, t_from=None, dt=0.01, limits=None):
+    def check_results(self, pb, out, t_from=None, dt=0.01, limits=None, urgent=False):
         """check_trajectories of batch `pb` as wait() / poll() returned it: out = (results, c_xy, c_yaw).  A record poll() has not
-        filled yet has zero durations and keeps no sample."""
+        filled yet has zero durations and keeps no sample.  urgent: the check goes ahead of the batches in flight (ualm_set_urgent)."""
         res, cxy, cyaw = out
         pt = np.array([(r.piece_T_xy, r.piece_T_yaw) for r in res], np.float64).reshape(pb.B, 2)
-        return self.check_trajectories(pb.N, pb.M, pt, cxy, cyaw, env=_env(pb), t_from=t_from, dt=dt, limits=limits)
+        with self._urgency(urgent):
+            return self.check_trajectories(pb.N, pb.M, pt, cxy, cyaw, env=_env(pb), t_from=t_from, dt=dt, limits=limits)
 
-    def submit_replan(self, pb, out, rows, t_from, dt=0.01, rparams=None, depth=2):
+    def submit_replan(self, pb, out, rows, t_from, dt=0.01, rparams=None, depth=2, urgent=False):
         """ualm_submit_replan: replans rows `rows` of batch `pb` as wait() / poll() returned it (out = (results, c_xy, c_yaw)) from each
         robot's state at time t_from (one number or one per row) on its trajectory to the row's original goal, with PlanManager's
         resampler over the trajectory's samples t_from < t of the sequence t = 0, dt, 2dt.. (rparams: front_end.resample_params(), None
         = its defaults), and submits the built problems as one ticket on the next lane of `depth`.  Returns (ticket, ProblemBatch of the
-        built problems, in the order of `rows`, with their environments); poll / wait / cancel / check_results work on it as on any."""
+        built problems, in the order of `rows`, with their environments); poll / wait / cancel / check_results work on it as on any.
+        urgent: the build and the ticket go ahead of the batches in flight (ualm_set_urgent)."""
         from . import problems
         rows = np.asarray(rows)
         if rows.ndim != 1 or (rows.size and not np.issubdtype(rows.dtype, np.integer)):
@@ -489,8 +506,9 @@ class BatchALMTrajOpt:
         bo, To = np.zeros((B, 18)), np.zeros(B)
         ixy, iyaw = np.zeros((B, _lib.UALM_REPLAN_INNER_XY)), np.zeros((B, _lib.UALM_REPLAN_INNER_YAW))
         t = C.c_int(-1)
-        _check(self.L.ualm_submit_replan(self.h, B, _p(N, ip), _p(M, ip), _p(pt), _p(c_xy), _p(c_yaw), _p(bnd), _p(env, ip), _p(tf), float(dt),
-                                         rp, int(depth), C.byref(t), _p(No, ip), _p(Mo, ip), _p(bo), _p(To), _p(ixy), _p(iyaw)))
+        with self._urgency(urgent):
+            _check(self.L.ualm_submit_replan(self.h, B, _p(N, ip), _p(M, ip), _p(pt), _p(c_xy), _p(c_yaw), _p(bnd), _p(env, ip), _p(tf), float(dt),
+                                             rp, int(depth), C.byref(t), _p(No, ip), _p(Mo, ip), _p(bo), _p(To), _p(ixy), _p(iyaw)))
         # a row over the compiled limits (N 64, M 128): zeros, as the C call packs it
         fits = lambda b: 2 * (No[b] - 1) <= _lib.UALM_REPLAN_INNER_XY and Mo[b] - 1 <= _lib.UALM_REPLAN_INNER_YAW
         pxy = [ixy[b, :2 * (No[b] - 1)] if fits(b) else np.zeros(2 * (int(No[b]) - 1)) for b in range(B)]

@@ -12,6 +12,7 @@
 #include <cmath>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <memory>
 #include <mutex>
 #include <numeric>
@@ -89,10 +90,18 @@ struct Lane {
     // one solve launch: the problems order[r0, r1) of one group size and one environment, taken from a work queue by grid CTAs
     struct GClass { int G = 1, n_ctas = 0, grid = 0, r0 = 0, r1 = 0, occ = 1, env = 0; size_t smem = 0; SmemLayout L; };
     std::vector<GClass> cls;
-    DevBuf<int> d_queue;         // one work counter per launch, zeroed before the launches
+    DevBuf<int> d_queue;         // one work counter per launch, then the lane's three hold words (BatchPtrs::hctl); zeroed before the launches
+    // each launch runs as a CUDA graph: WHILE (problems of its queue untaken) { hold_gate_kernel -> solve_kernel -> solve_loop_ctrl_kernel }
+    // (solve_loop_run), one per launch index, built at its first use and updated in place after
+    struct SolveLoop { cudaGraph_t G = nullptr; cudaGraphNode_t gate = nullptr, solve = nullptr, ctrl = nullptr; cudaGraphConditionalHandle h = 0; cudaGraphExec_t exec = nullptr; };
+    std::vector<SolveLoop> loops;
+    std::vector<cudaGraphExec_t> retired;    // executable graphs an update could not reuse, destroyed at release
     enum { NAUX = 7 };
     cudaStream_t aux[NAUX] = {};
     cudaEvent_t evs[NAUX + 1] = {};
+    // an urgent ticket's launches (ualm_set_urgent): streams of the greatest priority, made at the lane's first urgent ticket (a stream
+    // made earlier changes which hardware queue every later stream shares)
+    cudaStream_t ustream[NAUX + 1] = {};
     DevBuf<double> d_x0, d_x, d_xev, d_lambda, d_mu, d_scale_cx, d_hx, d_gx, d_lm_s, d_lm_y, d_lm_aux, d_fac, d_scr, d_ws, d_cxy, d_cyaw, d_f, d_grad, d_sfx;
     DevBuf<ualm_result_t> d_res;
     DevBuf<long long> d_prof;
@@ -123,6 +132,15 @@ struct Lane {
                                   &d_scr, &d_ws, &d_cxy, &d_cyaw, &d_f, &d_grad, &d_sfx};
         for (auto *b : bufs) b->release();
         d_res.release(); d_prof.release(); d_pieceT.release(); d_feas.release();
+        for (auto &g : loops) {
+            if (g.exec) cudaGraphExecDestroy(g.exec);
+            if (g.G) cudaGraphDestroy(g.G);
+        }
+        loops.clear();
+        for (auto x : retired) cudaGraphExecDestroy(x);
+        retired.clear();
+        for (auto &s : ustream) if (s) cudaStreamDestroy(s);
+        for (auto &s : ustream) s = nullptr;
         if (!made) return;
         for (int q = 0; q < NAUX; q++) if (aux[q]) cudaStreamDestroy(aux[q]);
         for (int q = 0; q < NAUX + 1; q++) if (evs[q]) cudaEventDestroy(evs[q]);
@@ -177,7 +195,13 @@ struct ualm_ctx {
     // go back to the device at that call's synchronisation and be mapped again at the next)
     void *cbuf = nullptr;
     size_t cbuf_bytes = 0;
+    // urgent work (ualm_set_urgent).  d_hold: the hold bytes the solve launches read (BatchPtrs::hold), byte q < UALM_MAX_LANES raised by
+    // lane q's urgent ticket, byte UALM_MAX_LANES by an urgent check or replan build; raised and lowered by copies from h_hold = {0, 1}
+    // (pinned), which need no SM
+    bool urgent = false;
+    unsigned char *d_hold = nullptr, *h_hold = nullptr;
 };
+static_assert(UALM_MAX_LANES + 1 <= UALM_HOLD_BYTES, "one hold byte per lane and one for the check stream");
 
 static int lane_make(ualm_ctx *c, Lane &l)
 {
@@ -243,6 +267,10 @@ extern "C" int ualm_create(ualm_ctx_t **out, int device, int precision)
         if (e1 == cudaSuccess) e1 = cudaStreamCreateWithFlags(&c->cancel, cudaStreamNonBlocking);
         if (e1 == cudaSuccess) e1 = cudaEventCreate(&c->evA);
         if (e1 == cudaSuccess) e1 = cudaEventCreate(&c->evB);
+        if (e1 == cudaSuccess) e1 = cudaMalloc(&c->d_hold, UALM_HOLD_BYTES);
+        if (e1 == cudaSuccess) e1 = cudaMemset(c->d_hold, 0, UALM_HOLD_BYTES);
+        if (e1 == cudaSuccess) e1 = cudaHostAlloc(&c->h_hold, 2, cudaHostAllocDefault);
+        if (e1 == cudaSuccess) { c->h_hold[0] = 0; c->h_hold[1] = 1; }
         if (e1 != cudaSuccess) rc = fail(UALM_ENOCUDA, std::string("context streams/events: ") + cudaGetErrorString(e1));
     }
     if (rc != UALM_OK) { const std::string keep = g_err; ualm_destroy(c); g_err = keep; return rc; }   // no leak on a failed create
@@ -269,6 +297,8 @@ extern "C" int ualm_destroy(ualm_ctx_t *c)
     if (c->cancel) cudaStreamDestroy(c->cancel);
     if (c->evA) cudaEventDestroy(c->evA);
     if (c->evB) cudaEventDestroy(c->evB);
+    if (c->d_hold) cudaFree(c->d_hold);
+    if (c->h_hold) cudaFreeHost(c->h_hold);
     delete c;
     return UALM_OK;
 }
@@ -643,6 +673,7 @@ static BatchPtrs batch_ptrs(ualm_ctx *c)
     b.scale_fx_io = l->d_sfx.p;
     b.prof = c->profile ? l->d_prof.p : nullptr;
     b.mbox = ualm_mbox::Ptrs{};
+    b.hold = nullptr; b.hctl = nullptr; b.urgent_slot = -1; b.n_urgent = 0;
     return b;
 }
 
@@ -670,8 +701,11 @@ extern "C" int ualm_upload(ualm_ctx_t *c, int B, const int32_t *N, const int32_t
     return ualm_upload_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, nullptr);
 }
 
-extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
-                               const double *inner_xy, const double *inner_yaw, const int32_t *env)
+// ualm_upload_env; `before_device` (parity path, may be empty) runs after every host-side allocation and free of the upload and before
+// its first device operation: ualm_submit_batch_env raises an urgent ticket's hold there, where nothing of the call waits for the device
+// any more
+static int upload_env(ualm_ctx *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time, const double *inner_xy,
+                      const double *inner_yaw, const int32_t *env, const std::function<int()> &before_device)
 {
     // validate everything before touching the lane; the lane holds no batch until this call has fully succeeded
     BatchLayout lay;
@@ -815,17 +849,18 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
     }
     l->tot_hist = oh; l->tot_scr = oscr; l->tot_fac = ofac; l->tot_ws = ows;
     const long long ox = L.tot_x, os = L.tot_s, ocx = L.tot_cxy, ocy = L.tot_cyaw;
-    CK(l->d_desc.ensure(B)); CK(l->d_order.ensure(BA)); CK(l->d_queue.ensure(std::max<size_t>(l->cls.size(), 1))); CK(l->d_x0.ensure(ox)); CK(l->d_x.ensure(ox)); CK(l->d_grad.ensure(ox));
+    CK(l->d_desc.ensure(B)); CK(l->d_order.ensure(BA)); CK(l->d_queue.ensure(l->cls.size() + 3)); CK(l->d_x0.ensure(ox)); CK(l->d_x.ensure(ox)); CK(l->d_grad.ensure(ox));
     CK(l->d_lambda.ensure(os)); CK(l->d_hx.ensure(os)); CK(l->d_mu.ensure(6 * os)); CK(l->d_gx.ensure(6 * os)); CK(l->d_scale_cx.ensure(7 * os));
     CK(l->d_lm_s.ensure(oh)); CK(l->d_lm_y.ensure(oh)); CK(l->d_scr.ensure(oscr));
     CK(l->d_ws.ensure(ows)); CK(l->d_fac.ensure(ofac)); CK(l->d_lm_aux.ensure((size_t)std::max(oaux, 1LL)));
     CK(l->d_eidx.ensure(B));
     CK(l->d_stop.ensure((size_t)std::max(B, 1)));
-    // factor arrays: entries outside the band-in-matrix positions (and the pad rows) are never written and must read 0
-    if (ofac > 0) CK(cudaMemsetAsync(l->d_fac.p, 0, sizeof(double) * ofac, l->stream));
     CK(l->d_prof.ensure((size_t)std::max(B, 1) * UALM_NPROF));
     CK(l->d_pieceT.ensure((size_t)std::max(B, 1) * 2)); CK(l->d_feas.ensure((size_t)std::max(B, 1) * 10));
     CK(l->d_cxy.ensure(ocx)); CK(l->d_cyaw.ensure(ocy)); CK(l->d_res.ensure(B)); CK(l->d_f.ensure(B)); CK(l->d_sfx.ensure(B));
+    if (before_device) if (int rc = before_device()) return rc;
+    // factor arrays: entries outside the band-in-matrix positions (and the pad rows) are never written and must read 0
+    if (ofac > 0) CK(cudaMemsetAsync(l->d_fac.p, 0, sizeof(double) * ofac, l->stream));
     if (B > 0) {
         CK(cudaMemcpyAsync(l->d_desc.p, l->desc.data(), sizeof(ProbDesc) * B, cudaMemcpyHostToDevice, l->stream));
         if (BA > 0) CK(cudaMemcpyAsync(l->d_order.p, l->order.data(), sizeof(int) * BA, cudaMemcpyHostToDevice, l->stream));
@@ -843,31 +878,125 @@ extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int
     l->have_batch = true; l->solved = false;
     return UALM_OK;
 }
+extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
+                               const double *inner_xy, const double *inner_yaw, const int32_t *env)
+{
+    return upload_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, {});
+}
 
-// the solve launches of the selected lane's batch; `publish`: every problem also goes to the lane's mailbox as it ends (submit only)
-static int solve_launch(ualm_ctx *c, bool publish)
+// raise (1) or lower (0) hold byte `slot` (ualm_ctx::d_hold) in the order of stream st
+static int hold_set(ualm_ctx *c, int slot, int v, cudaStream_t st)
+{
+    CK(cudaMemcpyAsync(c->d_hold + slot, c->h_hold + v, 1, cudaMemcpyHostToDevice, st));
+    return UALM_OK;
+}
+
+// the lane's greatest-priority streams (Lane::ustream), made at its first urgent ticket
+static int lane_priority_streams(Lane &l)
+{
+    if (!l.ustream[0]) {
+        int least = 0, greatest = 0;
+        CK(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+        for (auto &s : l.ustream) CK(cudaStreamCreateWithPriority(&s, cudaStreamNonBlocking, greatest));
+    }
+    return UALM_OK;
+}
+
+// lowers a hold on every exit of a call that raised it, unless the raise is handed on (armed = false)
+struct HoldGuard {
+    ualm_ctx *c;
+    int slot;
+    cudaStream_t st;
+    bool armed;
+    ~HoldGuard() { if (armed) cudaMemcpyAsync(c->d_hold + slot, c->h_hold, 1, cudaMemcpyHostToDevice, st); }
+};
+
+// launch ci of the selected lane's solve on stream st: its loop graph (Lane::SolveLoop) with this launch's arguments.  The handle
+// starts every graph launch at 1, so the body runs at least once; without a hold it runs exactly once.  A graph is updated in place,
+// never destroyed while the device may run it: destroying an executable graph waits for the device
+static int solve_loop_run(Lane &l, size_t ci, const BatchPtrs &bp, const DevParams &dp, const DevMap &dm, const Lane::GClass &cl, cudaStream_t st)
+{
+    if (l.loops.size() <= ci) l.loops.resize(ci + 1);
+    Lane::SolveLoop &g = l.loops[ci];
+    BatchPtrs a_bp = bp;
+    DevParams a_dp = dp;
+    DevMap a_dm = dm;
+    SmemLayout a_L = cl.L;
+    unsigned char *a_hold = bp.hold;
+    int *a_hctl = bp.hctl, a_urgent = bp.urgent_slot >= 0, a_n = bp.n_active;
+    const int *a_queue = bp.queue;
+    if (!g.G) CK(cudaGraphCreate(&g.G, 0));
+    if (!g.h) CK(cudaGraphConditionalHandleCreate(&g.h, g.G, 1, cudaGraphCondAssignDefault));
+    cudaGraphConditionalHandle a_h = g.h;
+    void *gate_args[] = {&a_hold, &a_hctl, &a_urgent};
+    void *solve_args[] = {&a_bp, &a_dp, &a_dm, &a_L};
+    void *ctrl_args[] = {&a_h, &a_queue, &a_n};
+    cudaKernelNodeParams gp = {}, sp = {}, cp = {};
+    gp.func = (void *)hold_gate_kernel; gp.gridDim = dim3(1); gp.blockDim = dim3(1); gp.kernelParams = gate_args;
+    sp.func = (void *)solve_kernel; sp.gridDim = dim3(cl.grid); sp.blockDim = dim3(UALM_THREADS * UALM_WPB); sp.sharedMemBytes = (unsigned)cl.smem;
+    sp.kernelParams = solve_args;
+    cp.func = (void *)solve_loop_ctrl_kernel; cp.gridDim = dim3(1); cp.blockDim = dim3(1); cp.kernelParams = ctrl_args;
+    if (!g.gate) {
+        cudaGraphNodeParams wp = {};
+        wp.type = cudaGraphNodeTypeConditional;
+        wp.conditional.handle = g.h;
+        wp.conditional.type = cudaGraphCondTypeWhile;
+        wp.conditional.size = 1;
+        cudaGraphNode_t wn;
+        CK(cudaGraphAddNode(&wn, g.G, nullptr, 0, &wp));
+        const cudaGraph_t body = wp.conditional.phGraph_out[0];
+        CK(cudaGraphAddKernelNode(&g.gate, body, nullptr, 0, &gp));
+        CK(cudaGraphAddKernelNode(&g.solve, body, &g.gate, 1, &sp));
+        CK(cudaGraphAddKernelNode(&g.ctrl, body, &g.solve, 1, &cp));
+    } else {
+        CK(cudaGraphKernelNodeSetParams(g.gate, &gp));
+        CK(cudaGraphKernelNodeSetParams(g.solve, &sp));
+        CK(cudaGraphKernelNodeSetParams(g.ctrl, &cp));
+    }
+    if (g.exec) {
+        cudaGraphExecUpdateResultInfo info;
+        if (cudaGraphExecUpdate(g.exec, g.G, &info) != cudaSuccess) {     // kept until the lane's release: destroying it would wait
+            cudaGetLastError();                                             // for the device, possibly under a hold this call raised
+            l.retired.push_back(g.exec);
+            g.exec = nullptr;
+        }
+    }
+    if (!g.exec) CK(cudaGraphInstantiate(&g.exec, g.G, 0));
+    CK(cudaGraphLaunch(g.exec, st));
+    return UALM_OK;
+}
+
+// the solve launches of the selected lane's batch; `publish`: every problem also goes to the lane's mailbox as it ends (submit only);
+// `urgent`: an urgent ticket (ualm_set_urgent) that has raised the lane's hold byte (ualm_submit_batch_env); its launches run on the lane's
+// greatest-priority streams and ignore holds, and the take of its last problem lowers the byte (slot_next)
+static int solve_launch(ualm_ctx *c, bool publish, bool urgent = false)
 {
     Lane *l = c->b;
     if (!l->have_batch) return fail(UALM_ESTATE, "set_params, set_map and upload must precede solve");
     if (int rc = check_envs(c, l->batch)) return rc;
     CK(cudaSetDevice(c->device));
     if (int rc = lane_hold(c, *l)) return rc;
+    if (urgent) if (int rc = lane_priority_streams(*l)) return rc;
     l->last_launches = 0;
     // no stop request carries over: the words are cleared before the solve, and raises are queued after ev_clear
     if (l->h_stop) memset(l->h_stop, 0, sizeof(int) * l->h_stop_cap);
     CK(cudaMemsetAsync(l->d_stop.p, 0, sizeof(int) * std::max(l->batch.B, 1), l->stream));
     CK(cudaEventRecord(l->ev_clear, l->stream));
-    if (!l->cls.empty()) CK(cudaMemsetAsync(l->d_queue.p, 0, sizeof(int) * l->cls.size(), l->stream));   // every launch's queue full
+    // every launch's queue full, the lane's hold words zero
+    CK(cudaMemsetAsync(l->d_queue.p, 0, sizeof(int) * (l->cls.size() + 3), l->stream));
     CK(cudaEventRecord(l->ev0, l->stream));
     if (l->batch.n_active > 0) {
-        // the launches run concurrently: launch 0 on the lane stream, the others on auxiliary streams
+        // the launches run concurrently: launch 0 on the lane stream, the others on auxiliary streams (an urgent ticket's: on the
+        // lane's priority streams, joined back to the lane stream)
         const int last = Lane::NAUX;
+        const cudaStream_t base = urgent ? l->ustream[last] : l->stream;
         CK(cudaEventRecord(l->evs[last], l->stream));
+        if (urgent) CK(cudaStreamWaitEvent(base, l->evs[last], 0));
         for (size_t ci = 0; ci < l->cls.size(); ci++) {
             auto &cl = l->cls[ci];
             if (cl.grid == 0) continue;
             const int ai = (int)((ci - 1) % Lane::NAUX);
-            cudaStream_t st = ci == 0 ? l->stream : l->aux[ai];
+            cudaStream_t st = ci == 0 ? base : urgent ? l->ustream[ai] : l->aux[ai];
             if (ci > 0) CK(cudaStreamWaitEvent(st, l->evs[last], 0));
             BatchPtrs bp = batch_ptrs(c);
             bp.queue = l->d_queue.p + ci;
@@ -875,15 +1004,19 @@ static int solve_launch(ualm_ctx *c, bool publish)
             bp.n_active = cl.r1 - cl.r0;
             bp.n_leader_slots = 4 / cl.G;
             if (publish) bp.mbox = l->mbox.device();
+            bp.hold = c->d_hold;
+            bp.hctl = l->d_queue.p + l->cls.size();
+            bp.urgent_slot = urgent ? c->cur : -1;
+            bp.n_urgent = l->batch.n_active;
             // the launch's environment: its parameters and grid are the launch's grid constants, the solve reads them as before
             DevParams dp = c->envs[cl.env].dp;
             dp.cancel = l->d_stop.p;
             dp.max_evals = c->max_evals;
-            solve_kernel<<<cl.grid, UALM_THREADS * UALM_WPB, cl.smem, st>>>(bp, dp, l->vref[cl.env]->dm, cl.L);
-            CK(cudaGetLastError());
+            if (int rc = solve_loop_run(*l, ci, bp, dp, l->vref[cl.env]->dm, cl, st)) return rc;
             l->last_launches++;
-            if (ci > 0) { CK(cudaEventRecord(l->evs[ai], st)); CK(cudaStreamWaitEvent(l->stream, l->evs[ai], 0)); }
+            if (ci > 0) { CK(cudaEventRecord(l->evs[ai], st)); CK(cudaStreamWaitEvent(base, l->evs[ai], 0)); }
         }
+        if (urgent) { CK(cudaEventRecord(l->evs[last], base)); CK(cudaStreamWaitEvent(l->stream, l->evs[last], 0)); }
     }
     CK(cudaEventRecord(l->ev1, l->stream));
     l->solved = true;
@@ -1000,24 +1133,38 @@ extern "C" int ualm_submit_batch_env(ualm_ctx_t *c, int B, const int32_t *N, con
     if (lane_in_flight(c, lane)) return fail(UALM_ESTATE, "all lanes of this depth are in flight: ualm_wait_batch the oldest ticket first");
     const int keep = c->cur;
     int rc = ualm_select_lane(c, lane);
-    if (!rc) rc = ualm_upload_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env);
     Lane &l = c->lanes[lane];
-    if (!rc && c->tp) {
-        std::string em;
-        rc = ualm_tp::tp_admit(c->tp, lane, &em, true);
-        rc = rc ? fail(rc, em) : lane_hold(c, l);
-    } else if (!rc) {
+    // an urgent ticket with a problem to solve raises the lane's hold byte on the lane stream once the upload has made every host-side
+    // allocation and free (they can wait for the device, and under a raised hold the device would wait for this call) and before its
+    // device work, which needs SM slots too.  The same holds for the mailbox, the stop words' mirror and the priority streams, made
+    // there first.  Every refusal after the raise lowers it; after a solve_launch the launches' last take lowers it
+    bool urgent = false;
+    HoldGuard guard{c, lane, l.stream, false};
+    auto before_device = [&]() -> int {
         cudaError_t e = l.mbox.begin(B, N, M, l.batch.skip.data());
-        if (e != cudaSuccess) rc = fail(UALM_ENOCUDA, std::string("result mailbox: ") + cudaGetErrorString(e));
-        if (!rc && l.h_stop_cap < (size_t)std::max(B, 1)) {      // the stop words' host mirror (solve_launch clears it)
+        if (e != cudaSuccess) return fail(UALM_ENOCUDA, std::string("result mailbox: ") + cudaGetErrorString(e));
+        if (l.h_stop_cap < (size_t)std::max(B, 1)) {      // the stop words' host mirror (solve_launch clears it)
             if (l.h_stop) cudaFreeHost(l.h_stop);
             l.h_stop = nullptr; l.h_stop_cap = 0;
             e = cudaHostAlloc(&l.h_stop, sizeof(int) * std::max(B, 1), cudaHostAllocDefault);
-            if (e != cudaSuccess) rc = fail(UALM_ENOCUDA, std::string("stop words: ") + cudaGetErrorString(e));
-            else l.h_stop_cap = (size_t)std::max(B, 1);
+            if (e != cudaSuccess) return fail(UALM_ENOCUDA, std::string("stop words: ") + cudaGetErrorString(e));
+            l.h_stop_cap = (size_t)std::max(B, 1);
         }
-        if (!rc) rc = solve_launch(c, true);
-        if (!rc) l.in_flight = true;
+        urgent = c->urgent && l.batch.n_active > 0;
+        if (!urgent) return UALM_OK;
+        if (int r = lane_priority_streams(l)) return r;
+        if (int r = hold_set(c, lane, 1, l.stream)) return r;
+        guard.armed = true;
+        return UALM_OK;
+    };
+    if (!rc) rc = upload_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, before_device);
+    if (!rc && c->tp) {
+        std::string em;
+        rc = ualm_tp::tp_admit(c->tp, lane, &em, true, c->urgent);
+        rc = rc ? fail(rc, em) : lane_hold(c, l);
+    } else if (!rc) {
+        rc = solve_launch(c, true, urgent);
+        if (!rc) { l.in_flight = true; guard.armed = false; }
     }
     if (!rc) { *ticket = lane; c->next_submit = (lane + 1) % depth; }
     c->cur = keep; c->b = &c->lanes[keep];
@@ -1132,6 +1279,14 @@ extern "C" int ualm_cancel_problems(ualm_ctx_t *c, int ticket, int n, const int3
     if (n == 0) return UALM_OK;
     CK(cudaSetDevice(c->device));
     return raise_stop(c, l, n, idx);
+}
+
+extern "C" int ualm_set_urgent(ualm_ctx_t *c, int urgent)
+{
+    if (!c) return fail(UALM_EINVAL, "null ctx");
+    if (urgent != 0 && urgent != 1) return fail(UALM_EINVAL, "urgent must be 0 or 1");
+    c->urgent = urgent == 1;
+    return UALM_OK;
 }
 
 extern "C" int ualm_set_budget(ualm_ctx_t *c, int32_t max_evals)
@@ -1540,6 +1695,12 @@ extern "C" int ualm_check_trajectories(ualm_ctx_t *c, int B, const int32_t *N, c
         ualm_ctx *c;
         ~Done() { if (cudaEventRecord(c->cdone, c->cstream) == cudaSuccess) cudaStreamWaitEvent(c->fstream, c->cdone, 0); }
     } done{c};
+    // urgent: the hold of the check stream, from before the copies to the end of the kernels
+    HoldGuard urgent{c, UALM_MAX_LANES, st, false};
+    if (c->urgent && c->d_hold) {     // (parity path: the throughput path has no hold)
+        if (int rc = hold_set(c, UALM_MAX_LANES, 1, st)) return rc;
+        urgent.armed = true;
+    }
     if (int rc = check_block(c, bytes)) return rc;
     double *d_out = (double *)c->cbuf, *d_pt = d_out + 16 * (size_t)B, *d_tf = d_pt + 2 * (size_t)B, *d_cxy = d_tf + B, *d_cyaw = d_cxy + ncx;
     ProbDesc *d_desc = (ProbDesc *)(d_out + nd);
@@ -1560,6 +1721,10 @@ extern "C" int ualm_check_trajectories(ualm_ctx_t *c, int B, const int32_t *N, c
                                        : CheckLimits{hp.max_vel, hp.max_acc_lon, hp.max_acc_lat, hp.max_kap, hp.min_cxi, hp.max_sig};
         check_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(a, hold[e]->dm, c->envs[e].dp.gravity, lim, dt, d_idx + off[e], cnt);
         CK(cudaGetLastError());
+    }
+    if (urgent.armed) {
+        urgent.armed = false;
+        if (int rc = hold_set(c, UALM_MAX_LANES, 0, st)) return rc;
     }
     CK(cudaMemcpyAsync(out16, d_out, sizeof(double) * 16 * B, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
@@ -1607,6 +1772,13 @@ extern "C" int ualm_submit_replan(ualm_ctx_t *c, int B, const int32_t *N, const 
     // the block: out (UALM_REPLAN_STRIDE B) | piece_T 2B | bnd 18B | t_from B | c_xy | c_yaw (doubles), then desc
     const size_t nout = (size_t)UALM_REPLAN_STRIDE * B, nd = nout + 21 * (size_t)B + (size_t)ncx + (size_t)ncy;
     const cudaStream_t st = c->cstream;
+    // urgent: the hold of the check stream over the build, lowered behind its kernel before any refusal can follow; the ticket is
+    // urgent by itself (ualm_submit_batch_env)
+    HoldGuard urgent{c, UALM_MAX_LANES, st, false};
+    if (c->urgent && c->d_hold) {     // (parity path: the throughput path has no hold)
+        if (int rc = hold_set(c, UALM_MAX_LANES, 1, st)) return rc;
+        urgent.armed = true;
+    }
     if (int rc = check_block(c, sizeof(double) * nd + sizeof(ProbDesc) * B)) return rc;
     double *d_out = (double *)c->cbuf, *d_pt = d_out + nout, *d_bnd = d_pt + 2 * (size_t)B, *d_tf = d_bnd + 18 * (size_t)B, *d_cxy = d_tf + B,
            *d_cyaw = d_cxy + ncx;
@@ -1622,6 +1794,10 @@ extern "C" int ualm_submit_replan(ualm_ctx_t *c, int B, const int32_t *N, const 
     const ReplanParams p{dt, r.piece_len, r.yaw_piece_times, r.mean_vel, r.init_time_times};
     replan_kernel<<<(B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(a, p, B);
     CK(cudaGetLastError());
+    if (urgent.armed) {
+        urgent.armed = false;
+        if (int rc = hold_set(c, UALM_MAX_LANES, 0, st)) return rc;
+    }
     std::vector<double> h(nout);
     CK(cudaMemcpyAsync(h.data(), d_out, sizeof(double) * nout, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));

@@ -120,7 +120,31 @@ struct BatchPtrs {
     R *f_out, *grad_out, *scale_fx_io;
     long long *prof;         // optional [grid][UALM_NPROF] phase cycle counters (lane 0 of each warp)
     ualm_mbox::Ptrs mbox;    // solve_kernel: the lane's result mailbox (ualm_poll_batch), flag null = publish nothing
+    // solve_kernel, urgent work (ualm_set_urgent): the context's UALM_HOLD_BYTES hold bytes (null = no holds), any of them raised =
+    // urgent work needs SM slots; the lane's words {problems its urgent launches have taken, 1 = this solve takes no further hold,
+// microseconds its gates have waited};
+    // urgent_slot >= 0: the launch is urgent, ignores holds, and the take of the lane's n_urgent-th problem lowers hold byte urgent_slot
+    unsigned char *hold;
+    int *hctl;
+    int urgent_slot, n_urgent;
 };
+
+// hold bytes: one per lane (its urgent ticket) and one for the check stream (an urgent check or replan build).  The host raises and
+// lowers them by copies, which need no SM; a slot of a non-urgent launch reads them before each take
+#define UALM_HOLD_BYTES 32
+static_assert(UALM_HOLD_BYTES % 8 == 0, "read as 8-byte words");
+// the longest a held launch waits (hold_gate_kernel): after it, its solve takes no further hold, so a hold never released only slows
+// work down
+#define UALM_HOLD_BOUND_NS 2000000000ull
+
+__device__ __forceinline__ bool hold_raised(const unsigned char *hold)
+{
+    const volatile unsigned long long *h = (const volatile unsigned long long *)hold;
+    unsigned long long v = 0;
+#pragma unroll
+    for (int k = 0; k < UALM_HOLD_BYTES / 8; k++) v |= h[k];
+    return v != 0;
+}
 
 // per-sample scratch fields (SoA: scratch[field * S + s])
 enum {
@@ -2147,7 +2171,8 @@ __device__ UALM_NOINLINE void join_mate(Traj &t, const BatchPtrs &bp, const DevP
 // leader of a slot between two problems: take the next problem of the launch's queue (largest first) and hand it to the helpers.
 // Returns the problem; -1 when the slot is done; -2 when the queue is empty and the group's warps join the mate's trajectory
 // (`adopt` = the CTA's two adoption state words, null without adoption; `probs` = the problems the slots published).  A slot
-// that has been joined takes no further problem.
+// that has been joined takes no further problem.  A slot of a non-urgent launch under a hold (hold_raised) takes nothing and ends
+// as at the end of the queue; the problems it leaves are taken by the next pass of the launch's loop (ualm_api.cu: solve_loop_run)
 __device__ UALM_NOINLINE int slot_next(Traj &t, const BatchPtrs &bp, int *adopt, int *probs, int slot, int lane)
 {
     bool joined = false;
@@ -2161,8 +2186,13 @@ __device__ UALM_NOINLINE int slot_next(Traj &t, const BatchPtrs &bp, int *adopt,
     int next = -1;
     if (!joined) {
         if (lane == 0) {
-            const int q = atomicAdd(bp.queue, 1);
-            next = q < bp.n_active ? bp.order[q] : -1;
+            const bool held = bp.urgent_slot < 0 && bp.hold && hold_raised(bp.hold) && !((volatile int *)bp.hctl)[1];
+            if (!held) {
+                const int q = atomicAdd(bp.queue, 1);
+                next = q < bp.n_active ? bp.order[q] : -1;
+                if (next >= 0 && bp.urgent_slot >= 0 && atomicAdd(bp.hctl, 1) == bp.n_urgent - 1)
+                    ((volatile unsigned char *)bp.hold)[bp.urgent_slot] = 0;     // the urgent ticket's last problem is taken
+            }
         }
         next = __shfl_sync(0xffffffffu, next, 0);
     }
@@ -2325,6 +2355,31 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) solve_kernel(const __
     int prob;
     while ((prob = slot_next(t, bp, adopt, s_prob, slot, lane)) >= 0) solve_problem(t, bp, p, map, L, sm, slot, adopt ? adopt + slot : nullptr, prob, lane);
     if (prob == -2) join_mate(t, bp, p, map, L, sbase, 1 - slot, ((volatile int *)s_prob)[1 - slot], 2, lane);
+}
+
+// the two ends of a pass of a solve launch's loop (ualm_api.cu: solve_loop_run).  The gate holds a non-urgent launch back while a hold
+// is raised.  hctl[2] sums the microseconds the gates of the lane's solve have waited (all passes, all launches); when the sum reaches
+// UALM_HOLD_BOUND_NS the gate marks the solve as taking no further hold (hctl[1]) and lets it go, so the solve waits at most that long
+// in all.  The control kernel repeats the pass while the launch's queue has problems no slot took
+__global__ void hold_gate_kernel(const unsigned char *hold, int *hctl, int urgent)
+{
+    if (urgent || ((volatile int *)hctl)[1]) return;
+    const long long budget = (long long)(UALM_HOLD_BOUND_NS / 1000ull) - ((volatile int *)hctl)[2];
+    unsigned long long t0, now;
+    asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
+    now = t0;
+    bool bound = budget <= 0;
+    while (!bound && hold_raised(hold)) {
+        __nanosleep(4000);
+        asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
+        bound = (long long)((now - t0) / 1000ull) >= budget;
+    }
+    atomicAdd(hctl + 2, (int)((now - t0) / 1000ull));
+    if (bound) ((volatile int *)hctl)[1] = 1;
+}
+__global__ void solve_loop_ctrl_kernel(cudaGraphConditionalHandle h, const int *queue, int n_active)
+{
+    cudaGraphSetConditional(h, *(const volatile int *)queue < n_active ? 1u : 0u);
 }
 
 // one innerCallback evaluation per problem at caller-provided x / duals (kernel-level parity)

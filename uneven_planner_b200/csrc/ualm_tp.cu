@@ -104,6 +104,12 @@ struct TpEngine {
     // trajectory only holds up the rounds of its own group
     cudaStream_t gstream[TP_NGROUPS] = {};
     cudaEvent_t gev[TP_NGROUPS] = {};
+    // an urgent ticket (ualm_set_urgent): its admission on ustream and its group loops on ugstream[g], all of the greatest priority and
+    // made at their first use (a stream made earlier changes which hardware queue every later stream shares); each is ordered after the
+    // work queued on the stream it stands in for, and that stream waits for it, so everything that waits for or queries the engine's
+    // own streams sees the urgent work
+    cudaStream_t ustream = nullptr, ugstream[TP_NGROUPS] = {};
+    cudaEvent_t uev = nullptr;
     // the round loop of each group (launch_loop), one per variant (with / without ks_kernel in the first round, with / without
     // publish_kernel): its graph keeps its conditional node and handle for the engine's life, and every admission replaces the other
     // nodes and updates the executable graph in place.  Destroying an executable graph waits for the device, which would hold the
@@ -249,8 +255,11 @@ void tp_destroy(TpEngine *e)
             if (L.G) cudaGraphDestroy(L.G);
         }
         if (e->gstream[g]) cudaStreamDestroy(e->gstream[g]);
+        if (e->ugstream[g]) cudaStreamDestroy(e->ugstream[g]);
         if (e->gev[g]) cudaEventDestroy(e->gev[g]);
     }
+    if (e->ustream) cudaStreamDestroy(e->ustream);
+    if (e->uev) cudaEventDestroy(e->uev);
     for (auto &l : e->lanes) {
         l.d_ad.release(); l.d_gd.release(); l.d_gdg.release(); l.d_x0.release(); l.d_xev.release(); l.d_cxy.release(); l.d_cyaw.release(); l.d_xout.release(); l.d_f.release(); l.d_grad.release();
         l.d_hx.release(); l.d_gx.release(); l.d_sfx.release(); l.d_scx.release(); l.d_lam.release(); l.d_mu.release(); l.d_scin.release(); l.d_sfin.release();
@@ -396,17 +405,18 @@ int tp_upload(TpEngine *e, int lane, const BatchLayout &L, const double *bnd, co
     return UALM_OK;
 }
 
-static int start_loops(TpEngine *e, int lane, bool publish, std::string *err);
+static int start_loops(TpEngine *e, int lane, bool publish, std::string *err, bool urgent = false);
 
 // admission of the lane's uploaded batch into the pool; loops: launch its groups' round loops (tp_time_penalty launches them itself
 // after its own rounds)
-static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, bool publish, bool loops, std::string *err)
+static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, bool publish, bool loops, std::string *err, bool urgent = false)
 {
     TpLane &l = e->lanes[lane];
     if (!l.have_batch) { if (err) *err = "set_params, set_map and upload must precede the solve"; return UALM_ESTATE; }
     if (l.in_flight) { if (err) *err = "lane already in flight"; return UALM_ESTATE; }
     const BatchLayout &L = *l.lay;
     TCK(cudaSetDevice(e->device));
+    const cudaStream_t as = urgent ? e->ustream : e->stream;     // (tp_admit made ustream and ordered it after the engine's stream)
     const int need = L.n_active;
     // the pool grows only while nothing is resident; it is sized for TP_LANES batches of this size in flight (fewer when that
     // would take more than three quarters of the free device memory: 8 x 8192 float slots take ~43 GB of an 80 GB H100)
@@ -439,7 +449,7 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, bool p
             l.h_stop_cap = c;
         }
         memset(l.h_stop, 0, sizeof(int) * l.h_stop_cap);
-        TCK(cudaMemsetAsync(l.d_stop.p, 0, sizeof(int) * nw, e->stream));
+        TCK(cudaMemsetAsync(l.d_stop.p, 0, sizeof(int) * nw, as));
         e->E.stop[lane] = l.d_stop.p;
     }
     l.slots.clear();
@@ -472,17 +482,17 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, bool p
     }
     eoff[UALM_MAX_ENVS] = (int)ad.size();
     const int BA = (int)ad.size();
-    TCK(cudaEventRecord(l.ev0, e->stream));
+    TCK(cudaEventRecord(l.ev0, as));
     l.launches = 0;
-    TCK(cudaMemcpyAsync(l.d_res.p, res0.data(), sizeof(ualm_result_t) * L.B, cudaMemcpyHostToDevice, e->stream));
+    TCK(cudaMemcpyAsync(l.d_res.p, res0.data(), sizeof(ualm_result_t) * L.B, cudaMemcpyHostToDevice, as));
     if (BA < L.B) {
-        TCK(cudaMemsetAsync(l.d_cxy.p, 0, sizeof(double) * L.tot_cxy, e->stream));
-        TCK(cudaMemsetAsync(l.d_cyaw.p, 0, sizeof(double) * L.tot_cyaw, e->stream));
+        TCK(cudaMemsetAsync(l.d_cxy.p, 0, sizeof(double) * L.tot_cxy, as));
+        TCK(cudaMemsetAsync(l.d_cyaw.p, 0, sizeof(double) * L.tot_cyaw, as));
     }
     if (BA > 0) {
-        TCK(cudaMemcpyAsync(l.d_ad.p, ad.data(), sizeof(AdmitDesc) * BA, cudaMemcpyHostToDevice, e->stream));
-        TCK(cudaMemcpyAsync(l.d_offs.p, offs.data(), sizeof(long long) * BA, cudaMemcpyHostToDevice, e->stream));
-        TCK(cudaMemcpyAsync(l.d_gd.p, l.gd.data(), sizeof(GatherDesc) * L.B, cudaMemcpyHostToDevice, e->stream));
+        TCK(cudaMemcpyAsync(l.d_ad.p, ad.data(), sizeof(AdmitDesc) * BA, cudaMemcpyHostToDevice, as));
+        TCK(cudaMemcpyAsync(l.d_offs.p, offs.data(), sizeof(long long) * BA, cudaMemcpyHostToDevice, as));
+        TCK(cudaMemcpyAsync(l.d_gd.p, l.gd.data(), sizeof(GatherDesc) * L.B, cudaMemcpyHostToDevice, as));
         std::vector<GatherDesc> gdg;
         int ngroups = 0;
         for (int q = 0; q < TP_SUBGROUPS; q++) ngroups += e->glive[lane * TP_SUBGROUPS + q] > 0;
@@ -495,11 +505,11 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, bool p
                     if (l.ad[b].slot < 0 || l.ad[b].group != lane * TP_SUBGROUPS + q) d.slot = -1;
                 }
             TCK(l.d_gdg.ensure(gdg.size()));
-            TCK(cudaMemcpyAsync(l.d_gdg.p, gdg.data(), sizeof(GatherDesc) * gdg.size(), cudaMemcpyHostToDevice, e->stream));
+            TCK(cudaMemcpyAsync(l.d_gdg.p, gdg.data(), sizeof(GatherDesc) * gdg.size(), cudaMemcpyHostToDevice, as));
         }
-        TCK(cudaMemsetAsync(e->gloop.p + lane * TP_SUBGROUPS, 0, sizeof(GroupLoop) * TP_SUBGROUPS, e->stream));
+        TCK(cudaMemsetAsync(e->gloop.p + lane * TP_SUBGROUPS, 0, sizeof(GroupLoop) * TP_SUBGROUPS, as));
         e->h_remaining[lane] = BA;
-        TCK(cudaMemcpyAsync(e->remaining.p + lane, e->h_remaining + lane, sizeof(int), cudaMemcpyHostToDevice, e->stream));
+        TCK(cudaMemcpyAsync(e->remaining.p + lane, e->h_remaining + lane, sizeof(int), cudaMemcpyHostToDevice, as));
         const double *x0 = l.has_xev ? l.d_xev.p : l.d_x0.p;
         const double *lam = l.has_lam ? l.d_lam.p : nullptr, *mu = l.has_mu ? l.d_mu.p : nullptr, *scx = l.has_scx ? l.d_scin.p : nullptr,
                      *sfx = l.has_sfx ? l.d_sfin.p : nullptr;
@@ -507,23 +517,34 @@ static int admit_impl(TpEngine *e, int lane, int mode, bool single_group, bool p
             const int n = eoff[v + 1] - eoff[v];
             if (n == 0) continue;
             const TpParams &p = e->p[v];
-            if (e->f32()) admit_kernel<float><<<n, 128, 0, e->stream>>>(e->E, l.d_ad.p + eoff[v], x0, n, p.use_scaling, p.int_K, lam, mu, scx, sfx, l.rho_eval, l.d_offs.p + eoff[v]);
-            else admit_kernel<double><<<n, 128, 0, e->stream>>>(e->E, l.d_ad.p + eoff[v], x0, n, p.use_scaling, p.int_K, lam, mu, scx, sfx, l.rho_eval, l.d_offs.p + eoff[v]);
+            if (e->f32()) admit_kernel<float><<<n, 128, 0, as>>>(e->E, l.d_ad.p + eoff[v], x0, n, p.use_scaling, p.int_K, lam, mu, scx, sfx, l.rho_eval, l.d_offs.p + eoff[v]);
+            else admit_kernel<double><<<n, 128, 0, as>>>(e->E, l.d_ad.p + eoff[v], x0, n, p.use_scaling, p.int_K, lam, mu, scx, sfx, l.rho_eval, l.d_offs.p + eoff[v]);
             TCK(cudaGetLastError());
             l.launches++;
         }
         // host-synchronised: ad / offs / res0 / gdg are stack-local staging vectors, and the lane's group loops start after the
         // admission (which also cleared the lane's stop words: a raise on the cancel stream lands after that clear)
-        TCK(cudaStreamSynchronize(e->stream));
+        TCK(cudaStreamSynchronize(as));
     } else {
         e->h_remaining[lane] = 0;
-        TCK(cudaStreamSynchronize(e->stream));
+        TCK(cudaStreamSynchronize(as));
     }
     l.in_flight = true; l.collected = false; l.mode = mode; l.publish = publish;
-    return loops ? start_loops(e, lane, publish, err) : UALM_OK;
+    return loops ? start_loops(e, lane, publish, err, urgent) : UALM_OK;
 }
 
-int tp_admit(TpEngine *e, int lane, std::string *err, bool publish)
+// the engine's priority stream for urgent work: *s, made at its first use
+static int priority_stream(cudaStream_t *s, std::string *err)
+{
+    if (!*s) {
+        int least = 0, greatest = 0;
+        TCK(cudaDeviceGetStreamPriorityRange(&least, &greatest));
+        TCK(cudaStreamCreateWithPriority(s, cudaStreamNonBlocking, greatest));
+    }
+    return UALM_OK;
+}
+
+int tp_admit(TpEngine *e, int lane, std::string *err, bool publish, bool urgent)
 {
     TpLane &l = e->lanes[lane];
     if (publish && l.have_batch && !l.in_flight) {      // (admit_impl refuses the other cases)
@@ -533,7 +554,14 @@ int tp_admit(TpEngine *e, int lane, std::string *err, bool publish)
         TCK(l.d_pub.ensure(L.B));
         if (L.B > 0) TCK(cudaMemsetAsync(l.d_pub.p, 0, sizeof(int) * L.B, e->stream));   // ordered before admission's synchronise
     }
-    return admit_impl(e, lane, 0, false, publish, true, err);
+    if (urgent) {
+        TCK(cudaSetDevice(e->device));
+        if (int rc = priority_stream(&e->ustream, err)) return rc;
+        if (!e->uev) TCK(cudaEventCreateWithFlags(&e->uev, cudaEventDisableTiming));
+        TCK(cudaEventRecord(e->uev, e->stream));
+        TCK(cudaStreamWaitEvent(e->ustream, e->uev, 0));
+    }
+    return admit_impl(e, lane, 0, false, publish, true, err, urgent);
 }
 
 static size_t kb_smem_bytes(TpEngine *e, bool tma)
@@ -602,7 +630,7 @@ static int set_attrs(TpEngine *e, std::string *err)
 // captures, and the context keeps the version captured here allocated until the lane is admitted again.  pub_gd: the descriptors
 // publish_kernel walks (null: no publication)
 template <class R>
-static int launch_loop(TpEngine *e, int g, bool with_ks, const GatherDesc *pub_gd, int *launches, std::string *err)
+static int launch_loop(TpEngine *e, int g, bool with_ks, const GatherDesc *pub_gd, int *launches, std::string *err, bool urgent)
 {
     TpLane &l = e->lanes[g / TP_SUBGROUPS];
     TpEngine::Loop &L = e->loops[g][(with_ks ? 2 : 0) + (pub_gd ? 1 : 0)];
@@ -675,12 +703,22 @@ static int launch_loop(TpEngine *e, int g, bool with_ks, const GatherDesc *pub_g
         }
     }
     if (!L.exec && !check(cudaGraphInstantiate(&L.exec, L.G, 0), "cudaGraphInstantiate")) return rc;
-    if (check(cudaGraphLaunch(L.exec, e->gstream[g]), "cudaGraphLaunch")) *launches += 3 + (with_ks ? 1 : 0);   // the prologue's; loop_ctrl_kernel counts the body's
+    // an urgent ticket's loop: on the group's priority stream, between two joins with the group's stream (the graph's kernel nodes
+    // take the priority of the stream it is launched into)
+    cudaStream_t ls = e->gstream[g];
+    if (urgent) {
+        if (int prc = priority_stream(&e->ugstream[g], err)) return prc;
+        if (!check(cudaEventRecord(e->gev[g], e->gstream[g]), "cudaEventRecord") || !check(cudaStreamWaitEvent(e->ugstream[g], e->gev[g], 0), "cudaStreamWaitEvent"))
+            return rc;
+        ls = e->ugstream[g];
+    }
+    if (check(cudaGraphLaunch(L.exec, ls), "cudaGraphLaunch")) *launches += 3 + (with_ks ? 1 : 0);   // the prologue's; loop_ctrl_kernel counts the body's
+    if (urgent && rc == UALM_OK && check(cudaEventRecord(e->gev[g], ls), "cudaEventRecord")) check(cudaStreamWaitEvent(e->gstream[g], e->gev[g], 0), "cudaStreamWaitEvent");
     return rc;
 }
 
 // launch the round loop of every live group of `lane` (after its admission); publish: its problems go to the mailbox as they end
-static int start_loops(TpEngine *e, int lane, bool publish, std::string *err)
+static int start_loops(TpEngine *e, int lane, bool publish, std::string *err, bool urgent)
 {
     TpLane &l = e->lanes[lane];
     int rc = e->f32() ? set_attrs<float>(e, err) : set_attrs<double>(e, err);
@@ -693,7 +731,7 @@ static int start_loops(TpEngine *e, int lane, bool publish, std::string *err)
         // each group publishes only its own problems: a slot of another group may be in the middle of its round
         const GatherDesc *pub = !publish ? nullptr : ngroups > 1 ? l.d_gdg.p + (size_t)q * l.lay->B : l.d_gd.p;
         const bool with_ks = (l.mode == 0 && e->p[e->genv[g]].use_scaling) || l.mode == 2;
-        rc = e->f32() ? launch_loop<float>(e, g, with_ks, pub, &l.launches, err) : launch_loop<double>(e, g, with_ks, pub, &l.launches, err);
+        rc = e->f32() ? launch_loop<float>(e, g, with_ks, pub, &l.launches, err, urgent) : launch_loop<double>(e, g, with_ks, pub, &l.launches, err, urgent);
     }
     return rc;
 }

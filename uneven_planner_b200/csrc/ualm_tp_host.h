@@ -45,7 +45,7 @@ void tp_bind_map(TpEngine *e, int env, const ualm_map_geom_t *g, const float4 *c
 int tp_upload(TpEngine *e, int lane, const BatchLayout &L, const double *bnd, const double *total_time, std::string *err);
 // asynchronous: the batch runs to completion without further calls.  publish: the group loops copy the batch's problems into the
 // lane's result mailbox as they finish (ualm_submit_batch, for tp_poll)
-int tp_admit(TpEngine *e, int lane, std::string *err, bool publish = false);
+int tp_admit(TpEngine *e, int lane, std::string *err, bool publish = false, bool urgent = false);   // urgent: admission and group loops on greatest-priority streams
 // ualm_poll_batch on a lane admitted with publish: reads the mailbox only (wait_ms > 0: yield-polls its flags until a problem is
 // new or wait_ms has passed); it neither synchronises nor queues anything
 int tp_poll(TpEngine *e, int lane, double wait_ms, int32_t *idx, int *n_new, int *n_pending, ualm_result_t *results, double *c_xy, double *c_yaw,
