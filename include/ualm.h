@@ -389,8 +389,15 @@ int ualm_check_trajectories(ualm_ctx_t *ctx, int B, const int32_t *N, const int3
  *       MinJerkOpt::generate (minco_traj.hpp:365-444): c_mpc_xy / c_mpc_yaw in the layout of ualm_solve_batch's c_xy / c_yaw,
  *       bit-identical to that header compiled unmodified (tests/test_ref_pin.py + tests/test_gpu_mpc_export.py);
  *   (3) dev4[4 * b + ..] = {max |planned - tracked| position (m), its time, max |planned - tracked| yaw (rad), its time}, sampled
- *       every dt: the planned spline carries the boundary speed of plan_manager.cpp:93-94, the message does not.
- * Any output pointer may be NULL.  Unsolved problems (ret_code UALM_ELIMIT) produce zeros. */
+ *       every dt: the planned spline carries the boundary speed of plan_manager.cpp:93-94, the message does not.  The samples are
+ *       t = 0, dt, 2dt, .. formed by repeated addition, kept while t < the shorter of the two durations (each the piece duration
+ *       added once per piece); each time is that of the earliest sample among equal maxima (0 when the deviation is 0 throughout).
+ *       A problem that would need 4e6 samples or more (duration / dt >= 4e6) is not scanned: {-1, 0, -1, 0}, while its message and
+ *       re-solve are still written.
+ * Any output pointer may be NULL.  Unsolved problems (ret_code UALM_ELIMIT) produce zeros.  The inputs are each problem's records as
+ * the solve returned them, so a problem stopped by a budget, a deadline or a cancel is handed over with the trajectory it carries.
+ * A null ctx, or dt <= 0 or NaN, is UALM_EINVAL; a lane without a solved batch (on the throughput path: not yet collected by
+ * ualm_sync / ualm_download / a wait) is UALM_ESTATE; no output is written on either. */
 int ualm_mpc_export_batch(ualm_ctx_t *ctx, double dt, const double *init_v, const double *init_a, double *pos_pts, double *posT_pts,
                           double *angle_pts, double *angleT_pts, double *c_mpc_xy, double *c_mpc_yaw, double *dev4);
 

@@ -190,11 +190,14 @@ def test_resident_batch_is_invalidated_by_its_inputs(gpu, bumps_map):
     first = opt.download()
     p2 = _lib.default_params(); p2.int_K = 8; p2.mem_size = 16
     opt.init(p2)
-    for call in (opt.solve_resident, opt.eval_batch, lambda: opt.feasibility(0.01), opt.download):
+    for call in (opt.solve_resident, opt.eval_batch, lambda: opt.feasibility(0.01), opt.download, lambda: opt.mpc_export(pb.N, pb.M)):
         with pytest.raises(gpu.UalmError):
             call()
     opt.init(params)
-    opt.upload(pb); opt.solve_resident()
+    opt.upload(pb)
+    with pytest.raises(gpu.UalmError):
+        opt.mpc_export(pb.N, pb.M)       # uploaded, not yet solved
+    opt.solve_resident()
     _same(pb, first, opt.download())
     # a rejected upload (validated before anything is touched) leaves the resident batch exactly as it was
     bad = pb.select(np.arange(pb.B)); bad.total_time[2] = 0.0

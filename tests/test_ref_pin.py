@@ -257,8 +257,8 @@ def test_reference_plan_manager_callback_matches_host_tools_and_oracle(ref, buil
 def test_mpc_side_minco_resolve_matches_oracle_bitwise(ref, orc, built, bumps_map):
     """SURVEY 8f-3: the MPC rebuilds the trajectory it tracks from the SE2Traj message with its own MINCO copy
     (mpc_controller/include/utils/minco_traj.hpp:336-460; TrajAnalyzer::setTraj, traj_anal.hpp:125-181: piece start points as
-    waypoints, zero boundary velocity / acceleration).  That re-solve, done by the unmodified reference header, equals the oracle's
-    MINCO on the same message bit for bit -- and differs from the back-end's own spline only by the boundary speed the back-end
+    waypoints, the message's boundary velocity / acceleration: zero as the reference publishes them, and nonzero as a replan hands
+    them over).  That re-solve, done by the unmodified reference header, equals the oracle's MINCO on the same message bit for bit -- and differs from the back-end's own spline only by the boundary speed the back-end
     uses (init_sig_vel, plan_manager.cpp:93-94)."""
     import pyoracle as po
     from uneven_planner_b200 import _lib, problems
@@ -274,18 +274,22 @@ def test_mpc_side_minco_resolve_matches_oracle_bitwise(ref, orc, built, bumps_ma
             cm = c.reshape(Dim, 6 * P_)
             start = cm[:, 0::6]                                  # piece start points = the message's pos_pts / angle_pts
             end = np.array([_end_value(cm[d], P_, dur) for d in range(Dim)])
-            head = np.zeros((3, Dim)); tail = np.zeros((3, Dim))
-            head[0] = start[:, 0]; tail[0] = end                 # init_v = init_a = 0 in the message (plan_manager.cpp:153-158)
-            inPs = np.ascontiguousarray(start[:, 1:].T).ravel()  # Dim x (P-1) column-major
-            ts = np.full(P_, dur)
-            c_mpc = np.zeros(6 * P_ * Dim); c_orc = np.zeros(6 * P_ * Dim)
-            assert ref.ref_mpc_minco(Dim, P_, P(inPs if inPs.size else np.zeros(1)), P(ts), P(np.ascontiguousarray(head).ravel()),
-                                     P(np.ascontiguousarray(tail).ravel()), P(c_mpc)) == 0
-            orc.orc_minco_generate(Dim, P_, P(inPs if inPs.size else np.zeros(1)), P(ts), P(np.ascontiguousarray(head).ravel()),
-                                   P(np.ascontiguousarray(tail).ravel()), P(c_orc))
-            assert np.array_equal(c_mpc, c_orc)
-            # the re-solved spline interpolates the same waypoints; it deviates from the back-end spline near the ends only
-            assert np.allclose(c_mpc.reshape(Dim, 6 * P_)[:, 0::6], start, atol=1e-9)
+            # init_v = init_a = 0 is what the reference publishes (plan_manager.cpp:153-158); a caller handing over a replan passes the
+            # robot's current {x, y, yaw} velocity and acceleration (all six values distinct, so a swapped index differs)
+            for v, a in (((0.0, 0.0, 0.0), (0.0, 0.0, 0.0)), ((0.7, -0.3, 0.25), (-1.1, 0.4, -0.6))):
+                head = np.zeros((3, Dim)); tail = np.zeros((3, Dim))
+                head[0] = start[:, 0]; tail[0] = end
+                head[1], head[2] = (v[:2], a[:2]) if Dim == 2 else (v[2:], a[2:])
+                inPs = np.ascontiguousarray(start[:, 1:].T).ravel()  # Dim x (P-1) column-major
+                ts = np.full(P_, dur)
+                c_mpc = np.zeros(6 * P_ * Dim); c_orc = np.zeros(6 * P_ * Dim)
+                assert ref.ref_mpc_minco(Dim, P_, P(inPs if inPs.size else np.zeros(1)), P(ts), P(np.ascontiguousarray(head).ravel()),
+                                         P(np.ascontiguousarray(tail).ravel()), P(c_mpc)) == 0
+                orc.orc_minco_generate(Dim, P_, P(inPs if inPs.size else np.zeros(1)), P(ts), P(np.ascontiguousarray(head).ravel()),
+                                       P(np.ascontiguousarray(tail).ravel()), P(c_orc))
+                assert np.array_equal(c_mpc, c_orc), (i, Dim, v, a)
+                # the re-solved spline interpolates the same waypoints; it deviates from the back-end spline near the ends only
+                assert np.allclose(c_mpc.reshape(Dim, 6 * P_)[:, 0::6], start, atol=1e-9)
 
 
 @pytest.mark.parametrize("use_scaling", [1, 0])
