@@ -4,21 +4,12 @@ TEST INFRASTRUCTURE.  The library is compiled on first use, with the oracle's ow
 directory: the tree is not written.
 """
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 from concurrent.futures import ThreadPoolExecutor
 
 import numpy as np
 
 import pyoracle as po
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-SRC = os.path.join(HERE, "budget_oracle.cpp")
-DEPS = [SRC, os.path.join(ROOT, "oracle", "oracle.cpp"), os.path.join(ROOT, "oracle", "oracle.h"), os.path.join(ROOT, "include", "ualm_detmath.h")]
-FLAGS = ["-O3", "-std=c++14", "-fPIC", "-ffp-contract=off", "-w", "-shared"]   # oracle/Makefile's CXXFLAGS
+from harness import load_oracle_ext
 
 _lib = None
 
@@ -26,17 +17,7 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        cxx = os.environ.get("CXX", "g++")
-        h = hashlib.sha256((cxx + " ".join(FLAGS)).encode())
-        for p in DEPS:
-            with open(p, "rb") as f:
-                h.update(f.read())
-        out = os.path.join(tempfile.gettempdir(), "ualm_budget_oracle_%d_%s.so" % (os.getuid(), h.hexdigest()[:16]))
-        if not os.path.exists(out):
-            tmp = "%s.%d.tmp" % (out, os.getpid())
-            subprocess.run([cxx] + FLAGS + ["-o", tmp, SRC], check=True)
-            os.replace(tmp, out)
-        L = C.CDLL(out)
+        L = load_oracle_ext("budget_oracle.cpp", "budget_oracle")
         L.orc_solve_budget.argtypes = [C.POINTER(po.OParams), C.POINTER(po.OMap), C.POINTER(po.OProblem), C.c_int, C.POINTER(po.OResult),
                                        po.dp, po.dp, po.dp]
         _lib = L

@@ -5,25 +5,14 @@ TEST INFRASTRUCTURE.  The library is compiled on first use, with the oracle's ow
 directory: the tree is not written.  Load it (lib()) before solving from several threads.
 """
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 import threading
 
 import numpy as np
 
 import pyoracle as po
-
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-SRC = os.path.join(HERE, "cancel_oracle.cpp")
-DEPS = [SRC, os.path.join(ROOT, "oracle", "oracle.cpp"), os.path.join(ROOT, "oracle", "oracle.h"), os.path.join(ROOT, "include", "ualm_detmath.h")]
-FLAGS = ["-O3", "-std=c++14", "-fPIC", "-ffp-contract=off", "-w", "-shared"]   # oracle/Makefile's CXXFLAGS
+from harness import RECORD, load_oracle_ext
 
 STOPPED = 3
-RECORD = ("ret_code", "outer_iters", "n_evals", "n_lbfgs_iters", "last_lbfgs_ret", "max_bound", "inner_cost", "jerk_cost", "total_T",
-          "res_h", "res_g", "scale_fx", "rho_final")
 
 _lib = None
 _lock = threading.Lock()
@@ -38,17 +27,7 @@ def lib():
 
 
 def _load():
-    cxx = os.environ.get("CXX", "g++")
-    h = hashlib.sha256((cxx + " ".join(FLAGS)).encode())
-    for p in DEPS:
-        with open(p, "rb") as f:
-            h.update(f.read())
-    out = os.path.join(tempfile.gettempdir(), "ualm_cancel_oracle_%d_%s.so" % (os.getuid(), h.hexdigest()[:16]))
-    if not os.path.exists(out):
-        tmp = "%s.%d.tmp" % (out, os.getpid())
-        subprocess.run([cxx] + FLAGS + ["-o", tmp, SRC], check=True)
-        os.replace(tmp, out)
-    L = C.CDLL(out)
+    L = load_oracle_ext("cancel_oracle.cpp", "cancel_oracle")
     L.orc_solve_cancel.argtypes = [C.POINTER(po.OParams), C.POINTER(po.OMap), C.POINTER(po.OProblem), C.c_int, C.POINTER(po.OResult),
                                    po.dp, po.dp, po.dp]
     L.orc_stop_tests.argtypes = [C.POINTER(po.OParams), C.POINTER(po.OMap), C.POINTER(po.OProblem), C.c_int, C.POINTER(C.c_int),

@@ -5,20 +5,12 @@ TEST INFRASTRUCTURE.  The library is compiled on first use, with the oracle's ow
 directory: the tree is not written.
 """
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
 import pyoracle as po
+from harness import load_oracle_ext
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-SRC = os.path.join(HERE, "check_oracle.cpp")
-DEPS = [SRC, os.path.join(ROOT, "oracle", "oracle.cpp"), os.path.join(ROOT, "oracle", "oracle.h"), os.path.join(ROOT, "include", "ualm_detmath.h")]
-FLAGS = ["-O3", "-std=c++14", "-fPIC", "-ffp-contract=off", "-w", "-shared"]   # oracle/Makefile's CXXFLAGS
 LIMIT_NAMES = ("max_vel", "max_acc_lon", "max_acc_lat", "max_kap", "min_cxi", "max_sig")
 NO_LIMITS = (np.inf, np.inf, np.inf, np.inf, -np.inf, np.inf)      # no test fires
 
@@ -28,17 +20,7 @@ _lib = None
 def lib():
     global _lib
     if _lib is None:
-        cxx = os.environ.get("CXX", "g++")
-        h = hashlib.sha256((cxx + " ".join(FLAGS)).encode())
-        for p in DEPS:
-            with open(p, "rb") as f:
-                h.update(f.read())
-        out = os.path.join(tempfile.gettempdir(), "ualm_check_oracle_%d_%s.so" % (os.getuid(), h.hexdigest()[:16]))
-        if not os.path.exists(out):
-            tmp = "%s.%d.tmp" % (out, os.getpid())
-            subprocess.run([cxx] + FLAGS + ["-o", tmp, SRC], check=True)
-            os.replace(tmp, out)
-        L = C.CDLL(out)
+        L = load_oracle_ext("check_oracle.cpp", "check_oracle")
         L.orc_check.argtypes = [C.POINTER(po.OMap), C.c_double, C.c_int, C.c_int, po.dp, po.dp, C.c_double, C.c_double, C.c_double, C.c_double,
                                 po.dp, po.dp, po.dp]
         L.orc_check.restype = None

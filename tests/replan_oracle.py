@@ -5,18 +5,11 @@ TEST INFRASTRUCTURE.  The library is compiled on first use, with the oracle's ow
 directory: the tree is not written.
 """
 import ctypes as C
-import hashlib
-import os
-import subprocess
-import tempfile
 
 import numpy as np
 
-HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
-SRC = os.path.join(HERE, "replan_oracle.cpp")
-DEPS = [SRC, os.path.join(ROOT, "oracle", "oracle.cpp"), os.path.join(ROOT, "oracle", "oracle.h"), os.path.join(ROOT, "include", "ualm_detmath.h")]
-FLAGS = ["-O3", "-std=c++14", "-fPIC", "-ffp-contract=off", "-w", "-shared"]   # oracle/Makefile's CXXFLAGS
+from harness import load_oracle_ext
+
 CAP_XY, CAP_YAW = 63, 127                 # the compiled limits N 64, M 128: inner points per row
 STRIDE = 21 + 2 * CAP_XY + CAP_YAW        # bnd' 18 | total_time | N' | M' | inner xy | inner yaw
 DEFAULT_RP = (0.3, 2.0, 0.5, 1.2)         # run_*.yaml manager/*: piece_len, yaw_piece_times, mean_vel, init_time_times
@@ -32,17 +25,7 @@ def _P(a):
 def lib():
     global _lib
     if _lib is None:
-        cxx = os.environ.get("CXX", "g++")
-        h = hashlib.sha256((cxx + " ".join(FLAGS)).encode())
-        for p in DEPS:
-            with open(p, "rb") as f:
-                h.update(f.read())
-        out = os.path.join(tempfile.gettempdir(), "ualm_replan_oracle_%d_%s.so" % (os.getuid(), h.hexdigest()[:16]))
-        if not os.path.exists(out):
-            tmp = "%s.%d.tmp" % (out, os.getpid())
-            subprocess.run([cxx] + FLAGS + ["-o", tmp, SRC], check=True)
-            os.replace(tmp, out)
-        L = C.CDLL(out)
+        L = load_oracle_ext("replan_oracle.cpp", "replan_oracle")
         ll = C.POINTER(C.c_longlong)
         L.orc_resample.argtypes = [dp, C.c_int, C.c_double, C.c_double, C.c_double, C.c_double, dp, C.c_longlong, dp, C.c_longlong, ll, ll, dp, dp,
                                    C.c_int, C.POINTER(C.c_int)]

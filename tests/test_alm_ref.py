@@ -20,162 +20,17 @@ import sys
 import numpy as np
 import pytest
 
+
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import alm_ref as ar  # noqa: E402
-from test_gpu_tp_shapes import _cat, _inputs, _offsets, case_batch  # noqa: E402
+from workloads import ALM_TOL, KEYS, LOOSE, _inputs, alm_block_errors, alm_check, near_face, restated, table_entry  # noqa: E402
 
-INT_K = [1, 16, 64, 127]
-TERRAINS = ["hill", "desert", "volcano", "forest"]
-RHO = 8.0
-# the bounds, about 10x the worst relative error measured over the whole table (restatement against the oracle, x86-64):
-#   f 8.9e-14 (N1_M128 at its guess); gradient 3.6e-12 (tau part, forest), 7.3e-13 (yaw waypoints), 6.6e-13 (xy waypoints, forest);
-#   hx 6.5e-12, a cancellation: at an initial guess the yaw follows the path tangent and hx ~ 1e-3 |v| (border_cells);
-#   gx 1.0e-13 (curvature, volcano); c_xy 3.8e-14, c_yaw 5.3e-13 (N1_M128); scale_fx 8.2e-14 (forest);
-#   scale_cx 9.5e-12 entry by entry (lateral acceleration, volcano)
-TOL = dict(f=1e-12, grad=4e-11, hx=1e-10, hx_cancel=1e-10, con=1e-12, coef=5e-12, sfx=1e-12, scx=1e-10)
-LOOSE = 1e-3            # f and gradient of a problem that holds a near-face sample
 MAX_NEAR_FACE = 1e-3    # share of the table's samples that may be near a face
-KIND = dict(f="f", grad_tau="grad", grad_xy="grad", grad_yaw="grad", hx="hx", hx_cancel="hx_cancel", c_xy="coef", c_yaw="coef", scale_fx="sfx",
-            **{"gx%d" % t: "con" for t in range(6)}, **{"scale_cx%d" % t: "scx" for t in range(7)})
 
 
-# ------------------------------------------------------------------ the table
-def _pairs(pb):
-    """every problem twice: at its initial guess (even index) and at a perturbed point (odd index)"""
-    return pb.select(np.repeat(np.arange(pb.B), 2))
-
-
-def cases():
-    """test_gpu_tp_shapes' case batch and a fast tight turn (4 m/s on a 0.8 m radius: 20 m/s^2 lateral), where the lateral
-    acceleration limit is active, each at its guess and perturbed"""
-    from test_gpu_minco_fused import _arc_problem
-    fast = _pairs(_arc_problem(8, 16, radius=0.8, arc=np.pi, speed=4.0))
-    return _cat([case_batch(), fast])
-
-
-def ridge():
-    """a corrugated grid: the normal tilts by up to 37 degrees in x with a 1 m period, so that cos_xi has a large gradient and, on the
-    one-piece problems (x = tau alone), initScaling's attitude scales are set by their tau component"""
-    from uneven_planner_b200 import _lib, maps
-    g = _lib.map_geometry()
-    X, Y, W = g.voxel_num
-    xs = (np.arange(X) + 0.5) * g.xy_resolution + g.origin[0]
-    cells = np.zeros((X, Y, W, 4), np.float32)
-    cells[..., 1] = (0.02 * (1.0 + np.cos(2 * np.pi * xs)))[:, None, None]
-    cells[..., 2] = (0.6 * np.sin(2 * np.pi * xs))[:, None, None]
-    return maps.UnevenMapData(g, cells, "ridge")
-
-
-def table_entry(key, terrain, bumps_map):
-    """(batch, params, grid) of one entry of the case table"""
-    from uneven_planner_b200 import _lib, configs, maps, problems
-    if key.startswith("K"):
-        p = _lib.default_params()
-        p.int_K = int(key[1:])
-        return cases(), p, bumps_map
-    if key in TERRAINS:
-        return cases(), configs.params_for(key), terrain(key)
-    if key == "tilt":
-        return cases(), _lib.default_params(), maps.synthetic_terrain("tilt")
-    if key == "ridge":
-        return cases(), _lib.default_params(), ridge()
-    assert key == "generated"
-    gen = [problems.generate(bumps_map, 6, seed=23), problems.generate(terrain("hill"), 6, seed=29, **configs.gen_kwargs("hill"))]
-    return _pairs(_cat(gen)), _lib.default_params(), None
-
-
-KEYS = ["K%d" % k for k in INT_K] + TERRAINS + ["tilt", "ridge", "generated"]
-
-
-def restated(pb, params, mapdata, Ks, inputs):
-    """the restatement's evaluation at `inputs` and initScaling at the initial guess of every problem (problem i with params[i] on
-    mapdata[i]), in the layout of test_gpu_tp_shapes._per_problem, plus the per-sample flags"""
-    xs, lam, mu, scx, sfx = inputs
-    offx, offs, _, _ = _offsets(pb, Ks)
-    grids = {id(m): ar.Grid(m) for m in mapdata}
-    out = []
-    for i in range(pb.B):
-        prob, p, g = ar.Problem(pb, i), params[i], grids[id(mapdata[i])]
-        r = ar.evaluate(prob, p, g, xs[offx[i]:offx[i + 1]], lam[offs[i]:offs[i + 1]], mu[6 * offs[i]:6 * offs[i + 1]],
-                        scx[7 * offs[i]:7 * offs[i + 1]], sfx[i], RHO)
-        if i % 2 == 1 and np.array_equal(pb.bnd[i], pb.bnd[i - 1]) and np.array_equal(pb.x0(i), pb.x0(i - 1)):
-            r["sfx"], r["scx"], r["near_face_scaling"] = out[i - 1]["sfx"], out[i - 1]["scx"], out[i - 1]["near_face_scaling"]
-        else:                                   # the perturbed twin of a problem shares its initial guess and so its initScaling
-            r["sfx"], r["scx"], r["near_face_scaling"] = ar.init_scaling(prob, p, g)
-        out.append(r)
-    return out
-
-
-def oracle(pb, params, mapdata, Ks, inputs):
-    from test_gpu_tp_shapes import _oracle
+def alm_oracle(pb, params, mapdata, Ks, inputs):
+    from workloads import _oracle
     return _oracle(pb, params, mapdata, Ks, inputs)
-
-
-# ------------------------------------------------------------------ the comparison
-def _blocks(N, g, o, cancel=False):
-    """(name, got, want, whole vector of want, per-entry) for every block of one problem's outputs; cancel: hx is a cancellation
-    (test_gpu_tp_shapes.TOLS) and is reported as hx_cancel"""
-    nxy = 2 * (N - 1)
-    con = np.concatenate([o["hx"], o["gx"]])
-    out = [("f", [g["f"]], [o["f"]], [o["f"]], False),
-           ("grad_tau", g["grad"][:1], o["grad"][:1], o["grad"], False),
-           ("grad_xy", g["grad"][1:1 + nxy], o["grad"][1:1 + nxy], o["grad"], False),
-           ("grad_yaw", g["grad"][1 + nxy:], o["grad"][1 + nxy:], o["grad"], False),
-           ("hx_cancel" if cancel else "hx", g["hx"], o["hx"], con, False),
-           ("c_xy", g["c_xy"], o["c_xy"], o["c_xy"], False),
-           ("c_yaw", g["c_yaw"], o["c_yaw"], o["c_yaw"], False),
-           ("scale_fx", [g["sfx"]], [o["sfx"]], [o["sfx"]], False)]
-    out += [("gx%d" % t, g["gx"][t::6], o["gx"][t::6], con, False) for t in range(6)]
-    out += [("scale_cx%d" % t, g["scx"][t::7], o["scx"][t::7], o["scx"], True) for t in range(7)]
-    return out
-
-
-def block_errors(pb, got, want, near=None, cancel=None, entrywise_scales=True):
-    """{block: (worst relative error over the batch, problem)}.  A block is measured by the norm of its difference over its own
-    norm; a block that is zero up to fp64 rounding (below 1e-9 of its whole vector) against its whole vector; scale_cx entry by
-    entry.  near[i]: problem i's near-face samples (a bool per sample), left out of the per-sample blocks; the error of f and the
-    gradient of such a problem is reported under "<block>_near".  entrywise_scales=False: scale_cx by norm too, the measure
-    test_gpu_tp_shapes.TOLS bound for the float kernels """
-    worst = {}
-    for i in range(pb.B):
-        N = int(pb.N[i])
-        nf = None if near is None else np.asarray(near[i], bool)
-        for name, a, b, whole, entrywise in _blocks(N, got[i], want[i], cancel is not None and cancel[i]):
-            a = np.asarray(a, np.float64)
-            b = np.asarray(b, np.float64)
-            whole = np.asarray(whole, np.float64)
-            if nf is not None and nf.any():
-                if name.startswith(("hx", "gx", "scale_cx")):
-                    keep = ~nf
-                    a, b = a[keep], b[keep]
-                elif name.startswith(("f", "grad")):
-                    name += "_near"
-            if b.size == 0:
-                continue
-            if entrywise and entrywise_scales:
-                err = float(np.max(np.abs(a - b) / np.abs(b)))
-            else:
-                d = float(np.linalg.norm(a - b))
-                nb, nw = float(np.linalg.norm(b)), float(np.linalg.norm(whole))
-                if nb <= 1e-9 * nw:
-                    nb = nw
-                err = d / nb if nb > 0 else (0.0 if d == 0 else np.inf)
-            if not np.isfinite(a).all():
-                err = np.inf
-            if err > worst.get(name, (-1.0, None))[0]:
-                worst[name] = (err, i)
-    return worst
-
-
-def check(worst, tol, loose, what):
-    bad = {k: v for k, v in worst.items()
-           if not v[0] <= (loose if k.endswith("_near") else tol[KIND[k]])}
-    assert not bad, (what, bad)
-
-
-def near_face(ref):
-    """per problem: the samples near a cell face in the evaluation or in initScaling"""
-    return [r["near_face"] | r["near_face_scaling"] for r in ref]
 
 
 # ------------------------------------------------------------------ fixtures
@@ -195,7 +50,7 @@ def table(built, terrain, bumps_map):
             ps = [p] * pb.B
             Ks = [p.int_K] * pb.B
             inputs = _inputs(pb, Ks, seed=KEYS.index(key))
-            cache[key] = (pb, ps, ms, Ks, inputs, restated(pb, ps, ms, Ks, inputs), oracle(pb, ps, ms, Ks, inputs))
+            cache[key] = (pb, ps, ms, Ks, inputs, restated(pb, ps, ms, Ks, inputs), alm_oracle(pb, ps, ms, Ks, inputs))
         return cache[key]
     return get
 
@@ -207,10 +62,10 @@ def test_oracle_matches_restatement_per_block(table, key):
     near = near_face(ref)
     n = sum(int(v.sum()) for v in near)
     S = sum(len(v) for v in near)
-    worst = block_errors(pb, want, ref, near)
+    worst = alm_block_errors(pb, want, ref, near)
     print("%s: %d of %d samples near a face; worst %s" % (key, n, S, {k: "%.1e" % v[0] for k, v in sorted(worst.items())}))
     assert n <= MAX_NEAR_FACE * S, (key, n, S)
-    check(worst, TOL, LOOSE, key)
+    alm_check(worst, ALM_TOL, LOOSE, key)
 
 
 # ------------------------------------------------------------------ what the table reaches (fails if it stops reaching an edge)

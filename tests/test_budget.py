@@ -11,6 +11,8 @@ sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import budget_oracle as bo  # noqa: E402
 from uneven_planner_b200 import configs, problems
 
+from harness import solve_diff
+
 NAMES = ["hill", "desert", "volcano", "forest"]
 STOPPED = 3
 
@@ -22,17 +24,6 @@ def _golden_problems(terrain, golden, name):
     return m, gold, pb, po.params_from(configs.params_for(name))
 
 
-def _same(a, b):
-    """bit-identical records and outputs of two oracle solves"""
-    ra, rb = a[0], b[0]
-    for f in ("ret_code", "outer_iters", "n_evals", "n_lbfgs_iters", "last_lbfgs_ret", "max_bound"):
-        assert getattr(ra, f) == getattr(rb, f), f
-    for f in ("inner_cost", "jerk_cost", "total_T", "res_h", "res_g", "scale_fx", "rho_final"):
-        assert getattr(ra, f) == getattr(rb, f), f
-    for x, y in zip(a[1:], b[1:]):
-        assert np.array_equal(x, y)
-
-
 @pytest.mark.parametrize("name", NAMES)
 def test_no_budget_and_large_budget_match_golden(terrain, golden, name):
     m, gold, pb, prm = _golden_problems(terrain, golden, name)
@@ -41,7 +32,7 @@ def test_no_budget_and_large_budget_match_golden(terrain, golden, name):
     for max_evals in (0, int(gold["n_evals"].max()) + 1):
         out = bo.solve_batch(prm, om, pb, max_evals, threads=4)
         for o, f in zip(out, free):
-            _same(o, f)          # the oracle's orc_solve
+            assert not solve_diff(o, f), solve_diff(o, f)          # the oracle's orc_solve
         assert np.array_equal(np.array([r[0].ret_code for r in out]), gold["ret_code"]), max_evals
         assert np.array_equal(np.array([r[0].n_evals for r in out]), gold["n_evals"]), max_evals
         assert np.array_equal(np.array([r[0].outer_iters for r in out]), gold["outer_iters"]), max_evals
@@ -61,7 +52,7 @@ def test_small_budgets(terrain, golden, name):
         for i, (o, f) in enumerate(zip(out, free)):
             r = o[0]
             if r.ret_code != STOPPED:
-                _same(o, f)          # no stop acted on it: the unbudgeted result
+                assert not solve_diff(o, f), solve_diff(o, f)          # no stop acted on it: the unbudgeted result
                 continue
             n_stopped += 1
             assert max_evals <= r.n_evals <= max_evals + 64, (max_evals, i, r.n_evals)

@@ -1,22 +1,17 @@
 """The C++ host-side mirror of the reference's ALMTrajOpt interface (include/ualm_traj_opt.hpp)."""
-import os
 import struct
 import subprocess
 
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+from harness import build_driver
 
 
 @pytest.fixture(scope="module")
 def driver(built, tmp_path_factory):
     d = tmp_path_factory.mktemp("cpp")
-    exe = str(d / "adapter_driver")
-    lib = os.path.join(ROOT, "uneven_planner_b200")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "adapter_driver.cpp"),
-                    "-o", exe, "-L", lib, "-lualm", "-Wl,-rpath," + lib], check=True)
-    return exe
+    return build_driver("adapter_driver", d)
 
 
 def _write_case(path, m, pb, i):
@@ -33,10 +28,7 @@ def _write_case(path, m, pb, i):
 def test_result_containers_and_mpc_message_export(built, tmp_path):
     """make_traj / Piece::getValue / locatePieceIdx / toSE2TrajMsg of include/ualm_traj_opt.hpp against hand-computed values
     (se2traj.hpp:106-118, 343-367, 682-695; plan_manager.cpp:151-185) -- host only."""
-    exe = str(tmp_path / "msg_driver")
-    lib = os.path.join(ROOT, "uneven_planner_b200")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "msg_driver.cpp"),
-                    "-o", exe, "-L", lib, "-lualm", "-Wl,-rpath," + lib], check=True)
+    exe = build_driver("msg_driver", tmp_path)
     r = subprocess.run([exe], capture_output=True, text=True)
     assert r.returncode == 0 and r.stdout.strip() == "OK", r.stdout
 
@@ -94,11 +86,7 @@ def test_adapter_matches_batch_api(driver, bumps_map, tmp_path):
 @pytest.fixture(scope="module")
 def chain_driver(built, tmp_path_factory):
     d = tmp_path_factory.mktemp("cppchain")
-    exe = str(d / "chain_driver")
-    lib = os.path.join(ROOT, "uneven_planner_b200")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "chain_driver.cpp"),
-                    "-o", exe, "-L", lib, "-lualm", "-Wl,-rpath," + lib], check=True)
-    return exe
+    return build_driver("chain_driver", d)
 
 
 def _write_chain_case(path, m, starts, goals):

@@ -6,24 +6,9 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from uneven_planner_b200 import configs, problems
+from uneven_planner_b200 import problems
 
-NAMES = ["hill", "desert", "volcano", "forest"]
-
-
-def mixed_golden_batch(terrain, golden):
-    """(maps, params, goldens, per-terrain batches, mixed batch, perm): the golden problems of the four terrains, terrain k in
-    environment k, interleaved (problem i of every terrain, then problem i + 1, ...).  mixed = concat(batches).select(perm)."""
-    maps, params, golds, pbs = [], [], [], []
-    for name in NAMES:
-        m = terrain(name)
-        gold = golden(name, m)
-        maps.append(m); params.append(configs.params_for(name)); golds.append(gold)
-        pbs.append(problems.generate(m, int(gold["B"]), seed=int(gold["seed"]), **configs.gen_kwargs(name)))
-    cat = problems.concat(pbs, range(len(NAMES)))
-    start = np.concatenate([[0], np.cumsum([p.B for p in pbs])])
-    perm = np.array([start[k] + i for i in range(max(p.B for p in pbs)) for k in range(len(pbs)) if i < pbs[k].B])
-    return maps, params, golds, pbs, cat.select(perm), perm
+from workloads import NAMES, mixed_golden_batch
 
 
 def test_env_entry_points_exported_and_reject_null_context(built):

@@ -6,18 +6,16 @@ The table is test_alm_ref's (the edge cases at int_K 1, 16, 64 and 127, the four
 two grids, the constant tilt), plus the shapes of test_gpu_parity_limits at int_K 128 and one batch that mixes the four
 terrains' parameter sets and grids in one context.  The comparison is test_alm_ref.block_errors: every block against its own
 norm, scale_cx entry by entry at precision 64, near-face samples left out of the per-sample blocks."""
-import os
-import sys
 
 import numpy as np
 import pytest
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import test_alm_ref as tar  # noqa: E402
-from test_gpu_parity_limits import SHAPES, _shape  # noqa: E402
-from test_gpu_tp_shapes import TOLS, _cat, _inputs, _per_problem  # noqa: E402
+import workloads
+from harness import cat, gpu  # noqa: F401
+from workloads import SHAPES, TOLS, _inputs, _per_problem, _shape
 
-KEYS = tar.KEYS + ["limits", "mixed"]
+
+KEYS = workloads.KEYS + ["limits", "mixed"]
 # the throughput path takes int_K up to 127, so the int_K 128 shapes run on the parity path only
 RUNS = [(64, k) for k in KEYS] + [(p, k) for p in (65, 32) for k in KEYS if k != "limits"]
 
@@ -25,9 +23,9 @@ RUNS = [(64, k) for k in KEYS] + [(p, k) for p in (65, 32) for k in KEYS if k !=
 def _tol(prec):
     """(bounds by block kind, bound of a near-face problem's f and gradient) at a precision"""
     if prec == 64:
-        return tar.TOL, tar.LOOSE
+        return workloads.ALM_TOL, workloads.LOOSE
     t = TOLS[prec]
-    return dict(t, hx=t["con"]), max(tar.LOOSE, t["grad"])
+    return dict(t, hx=t["con"]), max(workloads.LOOSE, t["grad"])
 
 
 def _entry(key, terrain, bumps_map):
@@ -36,30 +34,21 @@ def _entry(key, terrain, bumps_map):
     if key == "limits":
         p = _lib.default_params()
         p.int_K = 128
-        pb = tar._pairs(_cat([_shape(N, M) for N, M in SHAPES.values()]))
+        pb = workloads.alm_pairs(cat([_shape(N, M) for N, M in SHAPES.values()]))
         return pb, [p] * pb.B, [bumps_map] * pb.B
     if key == "mixed":
-        one = tar.cases()
+        one = workloads.alm_cases()
         parts, ps, ms = [], [], []
-        for e, name in enumerate(tar.TERRAINS):
-            idx = [k for k in range(one.B) if (k // 2) % len(tar.TERRAINS) == e]
+        for e, name in enumerate(workloads.TERRAINS):
+            idx = [k for k in range(one.B) if (k // 2) % len(workloads.TERRAINS) == e]
             sel = one.select(idx)
             parts.append(sel)
             ps += [configs.params_for(name)] * sel.B
             ms += [terrain(name)] * sel.B
-        return _cat(parts), ps, ms
-    pb, p, m = tar.table_entry(key, terrain, bumps_map)
+        return cat(parts), ps, ms
+    pb, p, m = workloads.table_entry(key, terrain, bumps_map)
     ms = [m] * pb.B if m is not None else [bumps_map] * (pb.B // 2) + [terrain("hill")] * (pb.B - pb.B // 2)
     return pb, [p] * pb.B, ms
-
-
-@pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
 
 
 @pytest.fixture(scope="module")
@@ -77,7 +66,7 @@ def table(built, terrain, bumps_map):
             pb.env = np.array([pairs.index((id(p), id(m))) for p, m in zip(ps, ms)], np.int32)
             Ks = [p.int_K for p in ps]
             inputs = _inputs(pb, Ks, seed=KEYS.index(key))
-            cache[key] = (pb, ps, ms, Ks, inputs, tar.restated(pb, ps, ms, Ks, inputs))
+            cache[key] = (pb, ps, ms, Ks, inputs, workloads.restated(pb, ps, ms, Ks, inputs))
         return cache[key]
     return get
 
@@ -91,7 +80,7 @@ def _run(gpu, pb, ps, ms, prec, inputs, Ks):
             opt.init(ps[i], env=e).set_environment(ms[i], env=e)
         opt.upload(pb)
         xs, lam, mu, scx, sfx = inputs
-        ev = opt.eval_batch(xs, lam, mu, scx, sfx, rho=tar.RHO)
+        ev = opt.eval_batch(xs, lam, mu, scx, sfx, rho=workloads.RHO)
         s_fx, s_cx = opt.init_scaling_batch()
     finally:
         opt.close()
@@ -107,7 +96,7 @@ def test_kernels_match_restatement_per_block(gpu, table, prec, key):
     cancel = [i % 2 == 0 or Ks[i] == 1 for i in range(pb.B)]
     # scale_cx entry by entry on the parity path; by norm on the throughput path, as TOLS are stated (at precision 32 one scale
     # entry at int_K 127 measures 7.7e-3 on an H100, its block 3.1e-4 against the bound 2e-3)
-    worst = tar.block_errors(pb, got, ref, tar.near_face(ref), cancel if prec != 64 else None, entrywise_scales=prec == 64)
+    worst = workloads.alm_block_errors(pb, got, ref, workloads.near_face(ref), cancel if prec != 64 else None, entrywise_scales=prec == 64)
     print("precision %d, %s: worst %s" % (prec, key, {k: "%.1e" % v[0] for k, v in sorted(worst.items())}))
     tol, loose = _tol(prec)
-    tar.check(worst, tol, loose, (prec, key))
+    workloads.alm_check(worst, tol, loose, (prec, key))

@@ -7,16 +7,11 @@ import os
 import numpy as np
 import pytest
 
+from harness import gpu  # noqa: F401
+from workloads import _with_oversize
+
+
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
 
 
 def _same(pb, a, b):
@@ -135,21 +130,6 @@ def test_double_map_grid_is_read_without_rounding(gpu, bumps_map):
     _same(pb, res_r, res_f)
     assert any(res_f[0][i].inner_cost != res[i].inner_cost for i in range(pb.B))
     opt.close()
-
-
-def _with_oversize(pb, at):
-    """a copy of pb with one problem of N = 70, M = 140 (over the compiled limits 64 / 128) inserted at index `at`"""
-    from uneven_planner_b200 import problems
-    oxy, oyaw, _, _ = pb.offsets()
-    N, M = 70, 140
-    t = np.linspace(0.0, 1.0, N + 1)[1:-1]
-    ixy = np.column_stack([-4.0 + 8.0 * t, -4.0 + 8.0 * t]).ravel()
-    iyaw = np.full(M - 1, np.pi / 4)
-    bnd = np.zeros(18); bnd[0:2] = -4.0; bnd[6:8] = 4.0; bnd[12] = bnd[15] = np.pi / 4
-    return problems.ProblemBatch(np.insert(pb.N, at, N).astype(np.int32), np.insert(pb.M, at, M).astype(np.int32),
-                                 np.insert(pb.bnd, at, bnd, axis=0), np.insert(pb.total_time, at, 30.0),
-                                 np.concatenate([pb.inner_xy[:oxy[at]], ixy, pb.inner_xy[oxy[at]:]]),
-                                 np.concatenate([pb.inner_yaw[:oyaw[at]], iyaw, pb.inner_yaw[oyaw[at]:]]))
 
 
 def test_problem_over_the_limits_fails_alone(gpu, bumps_map):

@@ -10,32 +10,18 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import budget_oracle as bo  # noqa: E402
+from harness import RECORD, ctx, gpu, same_problem  # noqa: F401, E402
+
 
 pytestmark = pytest.mark.gpu
 
 STOPPED = 3
-RECORD = ("ret_code", "outer_iters", "n_evals", "n_lbfgs_iters", "last_lbfgs_ret", "max_bound", "inner_cost", "jerk_cost", "total_T",
-          "res_h", "res_g", "scale_fx", "rho_final")
-
-
-@pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
 
 
 @pytest.fixture(scope="module")
 def work(hill_map):
     from uneven_planner_b200 import configs, problems
     return hill_map, configs.params_for("hill"), problems.generate(hill_map, 1024, seed=0, **configs.gen_kwargs("hill"))
-
-
-def _ctx(gpu, work, precision):
-    m, params, _ = work
-    return gpu.BatchALMTrajOpt(precision=precision).init(params).set_environment(m)
 
 
 @pytest.fixture(scope="module")
@@ -45,18 +31,11 @@ def free(gpu, work):
 
     def get(precision):
         if precision not in cache:
-            opt = _ctx(gpu, work, precision)
+            opt = ctx(gpu, precision, work[1], work[0])
             cache[precision] = opt.optimize(work[2])
             opt.close()
         return cache[precision]
     return get
-
-
-def _same_problem(pb, a, b, i):
-    """problem i bit-identical in two GPU solves (whole record, coefficients)"""
-    _, _, ocx, ocy = pb.offsets()
-    return bytes(a[0][i]) == bytes(b[0][i]) and np.array_equal(a[1][ocx[i]:ocx[i + 1]], b[1][ocx[i]:ocx[i + 1]]) and \
-        np.array_equal(a[2][ocy[i]:ocy[i + 1]], b[2][ocy[i]:ocy[i + 1]])
 
 
 def _check_budgeted(pb, out, ref, max_evals):
@@ -68,7 +47,7 @@ def _check_budgeted(pb, out, ref, max_evals):
             n_stop += 1
             assert max_evals <= r.n_evals <= max_evals + 64, (i, r.n_evals)
         else:
-            assert _same_problem(pb, out, ref, i), i
+            assert same_problem(pb, out, ref, i, values=True), i
     return n_stop
 
 
@@ -76,7 +55,7 @@ def _check_budgeted(pb, out, ref, max_evals):
 def test_parity_budget_matches_oracle(gpu, work, max_evals):
     import pyoracle as po
     m, params, pb = work
-    opt = _ctx(gpu, work, 64).set_budget(max_evals)
+    opt = ctx(gpu, 64, work[1], work[0]).set_budget(max_evals)
     res, cxy, cyaw = opt.optimize(pb)
     opt.close()
     ores = bo.solve_batch(po.params_from(params), po.OracleMap(m), pb, max_evals, threads=min(32, os.cpu_count()))
@@ -94,16 +73,16 @@ def test_parity_budget_matches_oracle(gpu, work, max_evals):
 def test_budget_above_every_problem_changes_nothing(gpu, work, free, precision):
     pb = work[2]
     ref = free(precision)
-    opt = _ctx(gpu, work, precision).set_budget(max(r.n_evals for r in ref[0]) + 1)
+    opt = ctx(gpu, precision, work[1], work[0]).set_budget(max(r.n_evals for r in ref[0]) + 1)
     out = opt.optimize(pb)
     opt.close()
-    assert all(_same_problem(pb, out, ref, i) for i in range(pb.B))
+    assert all(same_problem(pb, out, ref, i, values=True) for i in range(pb.B))
 
 
 @pytest.mark.parametrize("precision", [32, 65])
 def test_throughput_budget_50(gpu, work, free, precision):
     pb = work[2]
-    opt = _ctx(gpu, work, precision).set_budget(50)
+    opt = ctx(gpu, precision, work[1], work[0]).set_budget(50)
     out = opt.optimize(pb)
     opt.close()
     assert _check_budgeted(pb, out, free(precision), 50) > 0
@@ -113,7 +92,7 @@ def test_throughput_budget_50(gpu, work, free, precision):
 def test_deadline(gpu, work, free, precision):
     pb = work[2]
     ref = free(precision)
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     t0 = time.perf_counter()
     out = opt.wait(opt.submit(pb, depth=1), timeout_ms=0)
     ms0 = (time.perf_counter() - t0) * 1e3
@@ -123,7 +102,7 @@ def test_deadline(gpu, work, free, precision):
             n_stop += 1
             assert out[0][i].n_lbfgs_iters >= 1
         else:
-            assert _same_problem(pb, out, ref, i), i
+            assert same_problem(pb, out, ref, i, values=True), i
     assert n_stop > 0
     # the post-solve scan and the MPC hand-over work on the stopped batch (lane 0)
     opt.pb = pb
@@ -131,12 +110,12 @@ def test_deadline(gpu, work, free, precision):
     assert opt.mpc_export(pb.N, pb.M)["c_mpc_xy"].size == 12 * int(pb.N.sum())
     # the lane is reusable and its next batch starts without a stop request
     out2 = opt.wait(opt.submit(pb, depth=1))
-    assert all(_same_problem(pb, out2, ref, i) for i in range(pb.B))
+    assert all(same_problem(pb, out2, ref, i, values=True) for i in range(pb.B))
     # a generous deadline is ualm_wait_batch
     t0 = time.perf_counter()
     out3 = opt.wait(opt.submit(pb, depth=1), timeout_ms=600000.0)
     ms3 = (time.perf_counter() - t0) * 1e3
-    assert all(_same_problem(pb, out3, ref, i) for i in range(pb.B))
+    assert all(same_problem(pb, out3, ref, i, values=True) for i in range(pb.B))
     opt.close()
     print("precision %d: wait_batch_for(0) %.1f ms (%d of %d stopped), generous deadline %.1f ms" % (precision, ms0, n_stop, pb.B, ms3))
 
@@ -145,7 +124,7 @@ def test_deadline(gpu, work, free, precision):
 def test_budget_argument_and_state_checks(gpu, work, precision):
     from uneven_planner_b200 import _lib
     pb = work[2].select(np.arange(8))
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     with pytest.raises(gpu.UalmError, match="error %d" % _lib.UALM_EINVAL):
         opt.set_budget(-1)
     t = opt.submit(pb, depth=1)

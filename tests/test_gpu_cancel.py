@@ -16,31 +16,18 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import cancel_oracle as co  # noqa: E402
+from harness import build_driver, ctx, gpu, part, same_bytes, same_problem  # noqa: F401, E402
+
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 STOPPED = 3
-
-
-@pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
 
 
 @pytest.fixture(scope="module")
 def work(hill_map):
     from uneven_planner_b200 import configs, problems
     return hill_map, configs.params_for("hill"), problems.generate(hill_map, 1024, seed=0, **configs.gen_kwargs("hill"))
-
-
-def _ctx(gpu, work, precision):
-    m, params, _ = work
-    return gpu.BatchALMTrajOpt(precision=precision).init(params).set_environment(m)
 
 
 @pytest.fixture(scope="module")
@@ -50,26 +37,11 @@ def free(gpu, work):
 
     def get(precision):
         if precision not in cache:
-            opt = _ctx(gpu, work, precision)
+            opt = ctx(gpu, precision, work[1], work[0])
             cache[precision] = opt.optimize(work[2])
             opt.close()
         return cache[precision]
     return get
-
-
-def _same(a, b):
-    return bytes(a[0]) == bytes(b[0]) and a[1].tobytes() == b[1].tobytes() and a[2].tobytes() == b[2].tobytes()
-
-
-def _part(pb, out, i):
-    _, _, ocx, ocy = pb.offsets()
-    return out[0][i], out[1][ocx[i]:ocx[i + 1]], out[2][ocy[i]:ocy[i + 1]]
-
-
-def _same_problem(pb, a, b, i):
-    ra, xa, ya = _part(pb, a, i)
-    rb, xb, yb = _part(pb, b, i)
-    return bytes(ra) == bytes(rb) and xa.tobytes() == xb.tobytes() and ya.tobytes() == yb.tobytes()
 
 
 class Poller:
@@ -126,24 +98,24 @@ def test_parity_cancel_matches_oracle(gpu, work, free):
     import pyoracle as po
     m, params, pb = work
     ref = free(64)
-    opt = _ctx(gpu, work, 64)
+    opt = ctx(gpu, 64, work[1], work[0])
     polled, waited, a, b, c, before = _run_three_groups(opt, pb, seed=1)
     opt.close()
-    assert _same(polled, waited)
+    assert same_bytes(polled, waited)
     cancelled = np.union1d(np.union1d(a, b), c)
     for i in np.setdiff1d(np.arange(pb.B), cancelled):
-        assert _same_problem(pb, polled, ref, i), i
+        assert same_problem(pb, polled, ref, i), i
     for k, i in enumerate(c):                     # already final: unchanged
-        assert bytes(polled[0][i]) == before[k] and _same_problem(pb, polled, ref, i), i
+        assert bytes(polled[0][i]) == before[k] and same_problem(pb, polled, ref, i), i
     stopped = [int(i) for i in cancelled if polled[0][i].ret_code == STOPPED]
     for i in cancelled:
         if polled[0][i].ret_code != STOPPED:
-            assert _same_problem(pb, polled, ref, i), i
+            assert same_problem(pb, polled, ref, i), i
     prm, om = po.params_from(params), po.OracleMap(m)
     co.lib()                                      # compiled once, before the threads use it
 
     def check(i):
-        r, cxy, cyaw = _part(pb, polled, i)
+        r, cxy, cyaw = part(pb, polled, i)
         return i, co.match_stopped(prm, om, pb, i, r, cxy, cyaw)
     with ThreadPoolExecutor(min(32, os.cpu_count() or 1)) as ex:
         found = list(ex.map(check, stopped))
@@ -158,10 +130,10 @@ def test_parity_cancel_matches_oracle(gpu, work, free):
 def test_throughput_cancel(gpu, work, free, precision):
     pb = work[2]
     ref = free(precision)
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     polled, waited, a, b, c, before = _run_three_groups(opt, pb, seed=2)
     opt.close()
-    assert _same(polled, waited)
+    assert same_bytes(polled, waited)
     cancelled = np.union1d(np.union1d(a, b), c)
     n_stop = 0
     for i in range(pb.B):
@@ -170,7 +142,7 @@ def test_throughput_cancel(gpu, work, free, precision):
             assert r.n_lbfgs_iters >= 1, i
             n_stop += 1
         else:
-            assert _same_problem(pb, polled, ref, i), i
+            assert same_problem(pb, polled, ref, i), i
     for k, i in enumerate(c):
         assert bytes(polled[0][i]) == before[k]
     assert n_stop > 0
@@ -181,7 +153,7 @@ def test_throughput_cancel(gpu, work, free, precision):
 def test_other_ticket_and_next_batch_unaffected(gpu, work, precision):
     pb = work[2]
     A, B2 = pb.select(np.arange(0, 256)), pb.select(np.arange(256, 512))
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     refA, refB = opt.optimize(A), opt.optimize(B2)
     ta, tb = opt.submit(A, depth=2), opt.submit(B2, depth=2)
     assert ta != tb
@@ -193,16 +165,16 @@ def test_other_ticket_and_next_batch_unaffected(gpu, work, precision):
             if p.pending:
                 p.poll(1.0)
         assert time.perf_counter() - t0 < 600.0
-    assert _same(pa.out, opt.wait(ta)) and _same(pbp.out, opt.wait(tb))
-    assert _same(pbp.out, refB)                           # the other ticket, bit for bit
+    assert same_bytes(pa.out, opt.wait(ta)) and same_bytes(pbp.out, opt.wait(tb))
+    assert same_bytes(pbp.out, refB)                           # the other ticket, bit for bit
     for i in range(A.B):
         if i % 2 or pa.out[0][i].ret_code != STOPPED:
-            assert _same_problem(A, pa.out, refA, i), i
+            assert same_problem(A, pa.out, refA, i), i
     # the next batch on the cancelled ticket's lane, without cancels: no word carries over
     t = opt.submit(A, depth=2)
     assert t == ta
     again = Poller(opt, t, A).drain()
-    assert _same(again, opt.wait(t)) and _same(again, refA)
+    assert same_bytes(again, opt.wait(t)) and same_bytes(again, refA)
     opt.close()
 
 
@@ -210,10 +182,10 @@ def test_other_ticket_and_next_batch_unaffected(gpu, work, precision):
 def test_cancel_everything_right_after_submit(gpu, work, free, precision):
     pb = work[2]
     ref = free(precision)
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     t = opt.submit(pb, depth=1)        # warm-up: the free drain time
     t0 = time.perf_counter()
-    assert _same(Poller(opt, t, pb).drain(), ref)
+    assert same_bytes(Poller(opt, t, pb).drain(), ref)
     free_s = time.perf_counter() - t0
     opt.wait(t)
     t = opt.submit(pb, depth=1)
@@ -221,11 +193,11 @@ def test_cancel_everything_right_after_submit(gpu, work, free, precision):
     opt.cancel(t, np.arange(pb.B))
     out = Poller(opt, t, pb).drain()
     drain_s = time.perf_counter() - t0
-    assert _same(out, opt.wait(t))
+    assert same_bytes(out, opt.wait(t))
     rc = np.array([r.ret_code for r in out[0]])
     for i in range(pb.B):
         if rc[i] != STOPPED:
-            assert _same_problem(pb, out, ref, i), i
+            assert same_problem(pb, out, ref, i), i
     assert (rc == STOPPED).any()
     opt.close()
     print("precision %d: %d of %d stopped; drained in %.1f ms after cancelling all, %.1f ms without cancels" %
@@ -250,13 +222,13 @@ def test_cancel_in_a_mixed_environment_batch(gpu, work, terrain, precision):
     cut = np.concatenate(cut)
     opt.cancel(t, cut)
     out = Poller(opt, t, mixed).drain()
-    assert _same(out, opt.wait(t))
+    assert same_bytes(out, opt.wait(t))
     stops = [0, 0]
     for i in range(mixed.B):
         if i in cut and out[0][i].ret_code == STOPPED:
             stops[int(mixed.env[i])] += 1
         else:
-            assert _same_problem(mixed, out, ref, i), i
+            assert same_problem(mixed, out, ref, i), i
     assert stops[0] > 0 and stops[1] > 0, stops
     opt.close()
 
@@ -267,7 +239,7 @@ def test_cancel_refusals(gpu, work, precision):
     from uneven_planner_b200 import _lib
     EINVAL, ESTATE = _lib.UALM_EINVAL, _lib.UALM_ESTATE
     pb = work[2].select(np.arange(64))
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     ref = opt.optimize(pb)
     L, h = opt.L, opt.h
     ip = C.POINTER(C.c_int32)
@@ -283,7 +255,7 @@ def test_cancel_refusals(gpu, work, precision):
     assert raw(5, [0]) == ESTATE                                          # never submitted
     assert raw(t, [], n=0, null=True) == 0 and raw(t, []) == 0
     out = Poller(opt, t, pb).drain()
-    assert _same(out, opt.wait(t)) and _same(out, ref)                    # the refused calls raised nothing
+    assert same_bytes(out, opt.wait(t)) and same_bytes(out, ref)                    # the refused calls raised nothing
     assert raw(t, [0]) == ESTATE                                          # already waited
     opt.upload(pb)                                                        # a batch of the three-step path is not a ticket
     opt.solve_resident()
@@ -305,10 +277,7 @@ def _write_case(path, m, pb):
 def test_cpp_cancel_problems(gpu, work, tmp_path, precision):
     """cancelProblems through include/ualm_traj_opt.hpp (checked by the driver)"""
     m, _, pb = work
-    exe = str(tmp_path / "cancel_driver")
-    lib = os.path.join(ROOT, "uneven_planner_b200")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "cancel_driver.cpp"),
-                    "-o", exe, "-L", lib, "-lualm", "-Wl,-rpath," + lib], check=True)
+    exe = build_driver("cancel_driver", tmp_path)
     case = str(tmp_path / "case.bin")
     _write_case(case, m, pb.select(np.arange(128)))
     r = subprocess.run([exe, case, str(precision)], capture_output=True, text=True)

@@ -3,47 +3,25 @@ on, with the time each limit is first broken, on both paths and while batches ar
 and desert (G1), solved with the hill parameters; the CPU reference is tests/check_oracle.cpp."""
 import collections
 import ctypes as C
-import os
 import struct
 import subprocess
 
 import numpy as np
 import pytest
 
+from harness import bits, box_cells, build_driver, ctx, gpu, pending, pieces, same_pieces, splice  # noqa: F401
+from workloads import hill_desert_world
+
+
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PRECISIONS = [64, 32, 65]
 BOX = (60, 80, 40, 40)                # a 2 m x 2 m window of the 10 m grid, where the hill problems run
 DT = 0.01
 
 
 @pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
-
-
-@pytest.fixture(scope="module")
 def world(gpu, golden):
-    from uneven_planner_b200 import configs, maps, problems
-    g0, g1 = maps.stand_in_terrain("hill"), maps.stand_in_terrain("desert")
-    kw = configs.gen_kwargs("hill")
-    gold = golden("hill", g0)
-    gold_pb = problems.generate(g0, int(gold["B"]), seed=int(gold["seed"]), **kw)
-    bench = problems.generate(g0, 1024, seed=0, **kw)
-    return dict(g0=g0, g1=g1, params=configs.params_for("hill"), gold=gold, gold_pb=gold_pb, bench=bench,
-                a64=problems.concat([gold_pb, bench], [0, 0]), b=problems.generate(g0, 256, seed=7, **kw))
-
-
-def _ctx(gpu, world, precision, grid):
-    return gpu.BatchALMTrajOpt(precision=precision).init(world["params"]).set_environment(grid)
-
-
-def _bits(a):
-    return np.ascontiguousarray(a, np.float64).view(np.uint64)
+    return hill_desert_world(golden)
 
 
 def _piece_T(res):
@@ -58,33 +36,6 @@ def _total(N, M, Tx, Ty):
     for _ in range(M):
         ty += Ty
     return min(tx, ty)
-
-
-def _pieces(pb, out):
-    res, cxy, cyaw = out
-    _, _, ocx, ocy = pb.offsets()
-    return [(bytes(res[i]), cxy[ocx[i]:ocx[i + 1]].copy(), cyaw[ocy[i]:ocy[i + 1]].copy()) for i in range(pb.B)]
-
-
-def _same(a, b):
-    return len(a) == len(b) and all(x[0] == y[0] and np.array_equal(x[1], y[1]) and np.array_equal(x[2], y[2]) for x, y in zip(a, b))
-
-
-def _pending(opt, t, pb):
-    return opt.poll(t, opt.outputs(pb), 0.0)[1]
-
-
-def _box(cells, box):
-    ix0, iy0, nx, ny = box
-    return cells[ix0:ix0 + nx, iy0:iy0 + ny]
-
-
-def _splice(base, cells, box, name="spliced"):
-    from uneven_planner_b200 import maps
-    out = base.cells.copy()
-    ix0, iy0, nx, ny = box
-    out[ix0:ix0 + nx, iy0:iy0 + ny] = cells
-    return maps.UnevenMapData(base.geom, out, name)
 
 
 def _t_from(pb, out, kind):
@@ -118,13 +69,13 @@ def test_full_check_is_the_lane_scan(gpu, world, precision):
     where the scan's maximum breaks the environment's limit"""
     pb = world["a64"]
     p = world["params"]
-    opt = _ctx(gpu, world, precision, world["g0"])
+    opt = ctx(gpu, precision, world["params"], world["g0"])
     out = opt.optimize(pb)
     feas = opt.feasibility(DT)
     chk = opt.check_results(pb, out)
     opt.close()
     assert chk.shape == (pb.B, 16)
-    assert np.array_equal(_bits(chk[:, :10]), _bits(feas))
+    assert np.array_equal(bits(chk[:, :10]), bits(feas))
     breaks = np.stack([np.abs(chk[:, 0]) > p.max_vel, np.abs(chk[:, 1]) > p.max_acc_lon, np.abs(chk[:, 2]) > p.max_acc_lat,
                        np.abs(chk[:, 3]) > p.max_kap, chk[:, 4] > -p.min_cxi, chk[:, 5] > p.max_sig], 1)
     assert np.array_equal(chk[:, 10:] >= 0.0, breaks & (chk[:, 7:8] > 0))
@@ -164,7 +115,7 @@ def _against_oracle(opt, envs, pb, out):
         for lims in (None, tight):
             got = opt.check_results(pb, out, t_from=tf, limits=lims)
             ref = _oracle_rows(envs, pb, out, tf, lims)
-            bad = np.nonzero(np.any(_bits(got) != _bits(ref), axis=1))[0]
+            bad = np.nonzero(np.any(bits(got) != bits(ref), axis=1))[0]
             assert bad.size == 0, (kind, lims, bad[:5], got[bad[:2]], ref[bad[:2]])
             if lims is not None:
                 fired |= np.any(got[:, 10:] >= 0.0, axis=0)
@@ -179,7 +130,7 @@ def test_check_matches_the_oracle(gpu, world):
     from uneven_planner_b200 import problems
     pb = problems.concat([world["gold_pb"], world["bench"].select(np.arange(250))], [0, 0])
     p = world["params"]
-    opt = _ctx(gpu, world, 64, world["g0"])
+    opt = ctx(gpu, 64, world["params"], world["g0"])
     out = opt.optimize(pb)
     _against_oracle(opt, {0: (po.OracleMap(world["g0"]), p.gravity, limits_of(p))}, pb, out)
     opt.close()
@@ -231,9 +182,9 @@ def _far_from_box(pb, out, geom, box, cells=2):
 @pytest.mark.parametrize("precision", PRECISIONS)
 def test_check_after_an_update_reads_the_new_grid(gpu, world, precision, variant):
     g0, g1, pb = world["g0"], world["g1"], world["b"]
-    win = _box(g1.cells, BOX)
-    spliced = _splice(g0, win, BOX)
-    opt = _ctx(gpu, world, precision, g0)
+    win = box_cells(g1.cells, BOX)
+    spliced = splice(g0, win, BOX)
+    opt = ctx(gpu, precision, world["params"], g0)
     out = opt.optimize(pb)
     tf = _t_from(pb, out, 0)
     before = opt.check_results(pb, out, t_from=tf)
@@ -243,14 +194,14 @@ def test_check_after_an_update_reads_the_new_grid(gpu, world, precision, variant
         opt.update_environment(spliced)
     after = opt.check_results(pb, out, t_from=tf)
     opt.close()
-    fresh = _ctx(gpu, world, precision, spliced)
+    fresh = ctx(gpu, precision, world["params"], spliced)
     ref = fresh.check_results(pb, out, t_from=tf)
     fresh.close()
-    assert np.array_equal(_bits(after), _bits(ref))
+    assert np.array_equal(bits(after), bits(ref))
     far = _far_from_box(pb, out, g0.geom, BOX)
     assert far.any() and not far.all()
-    assert np.array_equal(_bits(after[far]), _bits(before[far]))
-    assert np.any(_bits(after) != _bits(before))
+    assert np.array_equal(bits(after[far]), bits(before[far]))
+    assert np.any(bits(after) != bits(before))
 
 
 # ---- in flight ----------------------------------------------------------------------------------
@@ -262,22 +213,22 @@ def test_check_while_a_batch_is_in_flight(gpu, world, precision):
     the check waits for SM slots in the batch's tail (DESIGN.md section 3i), so only its result is asserted there"""
     A = world["a64"] if precision == 64 else world["bench"]
     E = world["b"]
-    opt = _ctx(gpu, world, precision, world["g0"])
+    opt = ctx(gpu, precision, world["params"], world["g0"])
     out_e = opt.wait(opt.submit(E, depth=2))
     tf = _t_from(E, out_e, 1)
     idle = opt.check_results(E, out_e, t_from=tf)
     ta = opt.submit(A, depth=2)
-    assert _pending(opt, ta, A) > 0
+    assert pending(opt, ta, A) > 0
     chk = opt.check_results(E, out_e, t_from=tf)
     if precision != 64:
-        assert _pending(opt, ta, A) > 0
-    got_a = _pieces(A, opt.wait(ta))
+        assert pending(opt, ta, A) > 0
+    got_a = pieces(A, opt.wait(ta))
     opt.close()
-    assert np.array_equal(_bits(chk), _bits(idle))
-    o = _ctx(gpu, world, precision, world["g0"])
-    ref_a = _pieces(A, o.optimize(A))
+    assert np.array_equal(bits(chk), bits(idle))
+    o = ctx(gpu, precision, world["params"], world["g0"])
+    ref_a = pieces(A, o.optimize(A))
     o.close()
-    assert _same(got_a, ref_a)
+    assert same_pieces(got_a, ref_a)
     if precision == 64:
         g, n = world["gold"], world["gold_pb"].B
         assert [int(np.frombuffer(p[0], dtype=np.int32, count=1)[0]) for p in got_a[:n]] == [int(x) for x in g["ret_code"]]
@@ -293,9 +244,9 @@ def test_refused_checks_write_nothing(gpu, world, precision):
     L = _lib.lib()
     dp, ip = C.POINTER(C.c_double), C.POINTER(C.c_int32)
     pb = world["b"].select(np.arange(16))
-    opt = _ctx(gpu, world, precision, world["g0"])
+    opt = ctx(gpu, precision, world["params"], world["g0"])
     out = opt.optimize(pb)
-    before = _pieces(pb, out)
+    before = pieces(pb, out)
     res, cxy, cyaw = out
     N, M = np.ascontiguousarray(pb.N, np.int32), np.ascontiguousarray(pb.M, np.int32)
     pt = np.ascontiguousarray(_piece_T(res))
@@ -323,7 +274,7 @@ def test_refused_checks_write_nothing(gpu, world, precision):
     assert call(env=env) == ESTATE
     assert np.all(o == 7.0)
     assert call(B=0) == _lib.UALM_OK and np.all(o == 7.0)
-    assert _same(_pieces(pb, opt.optimize(pb)), before)
+    assert same_pieces(pieces(pb, opt.optimize(pb)), before)
     # over the compiled limits, and too many samples: not scanned
     big = np.array([65], np.int32)
     r = opt.check_trajectories(big, [4], [[0.1, 0.1]], np.zeros(12 * 65), np.zeros(24))
@@ -338,7 +289,7 @@ def test_checks_do_not_leak(gpu, world, precision):
     import torch
     depth = 3 if precision == 64 else 8
     pb = world["b"]
-    opt = _ctx(gpu, world, precision, world["g0"])
+    opt = ctx(gpu, precision, world["params"], world["g0"])
 
     def fill():
         return [opt.wait(t) for t in [opt.submit(pb, depth=depth) for _ in range(depth)]][-1]
@@ -349,7 +300,7 @@ def test_checks_do_not_leak(gpu, world, precision):
     q = collections.deque()
     for i in range(20):
         src = world["g1"] if i % 2 == 0 else world["g0"]
-        opt.update_environment_window(BOX[0], BOX[1], _box(src.cells, BOX))
+        opt.update_environment_window(BOX[0], BOX[1], box_cells(src.cells, BOX))
         if len(q) == depth:
             last = opt.wait(q.popleft())
         chk = opt.check_results(pb, last, t_from=0.5)
@@ -367,13 +318,10 @@ def test_checks_do_not_leak(gpu, world, precision):
 
 def test_cpp_check_between_submit_and_window(gpu, world, tmp_path):
     from uneven_planner_b200 import _lib
-    exe = str(tmp_path / "check_driver")
-    lib = os.path.join(ROOT, "uneven_planner_b200")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "check_driver.cpp"), "-o", exe,
-                    "-L", lib, "-lualm", "-Wl,-rpath," + lib], check=True)
+    exe = build_driver("check_driver", tmp_path)
     g0, g1 = world["g0"], world["g1"]
     pb = world["bench"].select(np.arange(8))
-    win = np.ascontiguousarray(_box(g1.cells, BOX))
+    win = np.ascontiguousarray(box_cells(g1.cells, BOX))
     tf = np.array([0.0, 0.5, 1.0, 1.5, 2.0, 2.5, 3.0, 100.0])
     case = str(tmp_path / "check.bin")
     with open(case, "wb") as f:
@@ -397,5 +345,5 @@ def test_cpp_check_between_submit_and_window(gpu, world, tmp_path):
     rows = [ln.split() for ln in r.stdout.strip().splitlines()]
     assert [(int(x[0]), int(x[1])) for x in rows] == [(p, i) for p in range(2) for i in range(pb.B)]
     got = np.array([[float(v) for v in x[2:]] for x in rows])
-    assert np.array_equal(_bits(got), _bits(np.concatenate([c0, c1])))
-    assert np.any(_bits(c0) != _bits(c1))
+    assert np.array_equal(bits(got), bits(np.concatenate([c0, c1])))
+    assert np.any(bits(c0) != bits(c1))

@@ -2,29 +2,18 @@
 each problem in its own environment (parameter set + map grid), gives every problem exactly the result it has in a batch of its
 environment alone -- on the parity path (also against the goldens, pipelined, budgeted and under a deadline), through the phase
 entry points, and on the throughput path.  Workload: the golden problems of hill, desert, volcano and forest (tests/test_envs.py)."""
-import os
 import struct
 import subprocess
-import sys
 
 import numpy as np
 import pytest
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from test_envs import NAMES, mixed_golden_batch  # noqa: E402
+from harness import build_driver, ctx, gpu, pieces, same_values  # noqa: F401
+from workloads import NAMES, mixed_golden_batch
+
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 STOPPED = 3
-
-
-@pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
 
 
 @pytest.fixture(scope="module")
@@ -34,24 +23,6 @@ def work(terrain, golden):
     env = np.searchsorted(start, perm, side="right") - 1
     where = [(int(e), int(q - start[e])) for e, q in zip(env, perm)]        # mixed problem i = problem j of terrain e
     return dict(maps=maps, params=params, golds=golds, pbs=pbs, mixed=mixed, where=where)
-
-
-def _mixed_ctx(gpu, work, precision=64):
-    opt = gpu.BatchALMTrajOpt(precision=precision)
-    for e in range(len(NAMES)):
-        opt.init(work["params"][e], env=e).set_environment(work["maps"][e], env=e)
-    return opt
-
-
-def _pieces(pb, out):
-    """per problem: (record bytes, c_xy, c_yaw)"""
-    res, cxy, cyaw = out
-    _, _, ocx, ocy = pb.offsets()
-    return [(bytes(res[i]), cxy[ocx[i]:ocx[i + 1]], cyaw[ocy[i]:ocy[i + 1]]) for i in range(pb.B)]
-
-
-def _same(a, b):
-    return a[0] == b[0] and np.array_equal(a[1], b[1]) and np.array_equal(a[2], b[2])
 
 
 @pytest.fixture(scope="module")
@@ -64,7 +35,7 @@ def single(gpu, work):
             out = []
             for e in range(len(NAMES)):
                 opt = gpu.BatchALMTrajOpt(precision=precision).init(work["params"][e]).set_environment(work["maps"][e]).set_budget(budget)
-                out.append(_pieces(work["pbs"][e], opt.optimize(work["pbs"][e])))
+                out.append(pieces(work["pbs"][e], opt.optimize(work["pbs"][e])))
                 opt.close()
             cache[(precision, budget)] = out
         return cache[(precision, budget)]
@@ -73,13 +44,13 @@ def single(gpu, work):
 
 def _check_mixed(work, got, ref):
     for i, (e, j) in enumerate(work["where"]):
-        assert _same(got[i], ref[e][j]), (i, NAMES[e], j)
+        assert same_values(got[i], ref[e][j]), (i, NAMES[e], j)
 
 
 def test_parity_mixed_golden_batch(gpu, work, single):
     from uneven_planner_b200 import _lib
     mixed = work["mixed"]
-    opt = _mixed_ctx(gpu, work)
+    opt = ctx(gpu, 64, work["params"], work["maps"])
     out = opt.optimize(mixed)
     opt.close()
     res, cxy, cyaw = out
@@ -92,27 +63,27 @@ def test_parity_mixed_golden_batch(gpu, work, single):
         assert (r.ret_code, r.n_evals, r.outer_iters, r.inner_cost) == (g["ret_code"][j], g["n_evals"][j], g["outer_iters"][j], g["inner_cost"][j]), (i, NAMES[e])
         assert np.array_equal(cxy[ocx[i]:ocx[i + 1]], g["c_xy"][gcx[j]:gcx[j + 1]]), (i, NAMES[e])
         assert np.array_equal(cyaw[ocy[i]:ocy[i + 1]], g["c_yaw"][gcy[j]:gcy[j + 1]]), (i, NAMES[e])
-    _check_mixed(work, _pieces(mixed, out), single(64))
+    _check_mixed(work, pieces(mixed, out), single(64))
     assert len(_lib.Result._fields_) == 17      # the record bytes compared cover res_h, res_g and the piece durations
 
 
 def test_parity_pipelined_budget_and_deadline(gpu, work, single):
     mixed = work["mixed"]
-    opt = _mixed_ctx(gpu, work).set_budget(50)
+    opt = ctx(gpu, 64, work["params"], work["maps"]).set_budget(50)
     tickets = [opt.submit(mixed, depth=3) for _ in range(3)]
     for t in tickets:
-        _check_mixed(work, _pieces(mixed, opt.wait(t)), single(64, 50))
+        _check_mixed(work, pieces(mixed, opt.wait(t)), single(64, 50))
     assert any(single(64, 50)[e][j][0] != single(64)[e][j][0] for e, j in work["where"])     # the budget acted
     opt.set_budget(0)
     free = single(64)
     out = opt.wait(opt.submit(mixed, depth=1), timeout_ms=5.0)
-    got = _pieces(mixed, out)
+    got = pieces(mixed, out)
     for i, (e, j) in enumerate(work["where"]):
         r = out[0][i]
         assert r.ret_code in (0, 1, 2, STOPPED), i
         if r.ret_code != STOPPED:
-            assert _same(got[i], free[e][j]), i
-    _check_mixed(work, _pieces(mixed, opt.wait(opt.submit(mixed, depth=1))), free)     # the lane is reusable
+            assert same_values(got[i], free[e][j]), i
+    _check_mixed(work, pieces(mixed, opt.wait(opt.submit(mixed, depth=1))), free)     # the lane is reusable
     opt.close()
 
 
@@ -141,7 +112,7 @@ def test_other_entry_points_per_environment(gpu, work):
                              c_mpc=_split(ex["c_mpc_xy"], 12 * pb.N)[i], dev=ex["dev"][i]))
         return rows
 
-    opt = _mixed_ctx(gpu, work)
+    opt = ctx(gpu, 64, work["params"], work["maps"])
     got = run(opt, mixed, [K[e] for e in mixed.env])
     opt.close()
     ref = []
@@ -158,11 +129,11 @@ def test_other_entry_points_per_environment(gpu, work):
 def test_throughput_mixed_alone_and_at_depth_4(gpu, work, single, precision):
     mixed = work["mixed"]
     ref = single(precision)
-    opt = _mixed_ctx(gpu, work, precision)
-    _check_mixed(work, _pieces(mixed, opt.optimize(mixed)), ref)
+    opt = ctx(gpu, precision, work["params"], work["maps"])
+    _check_mixed(work, pieces(mixed, opt.optimize(mixed)), ref)
     tickets = [opt.submit(mixed, depth=4) for _ in range(4)]
     for t in tickets:
-        _check_mixed(work, _pieces(mixed, opt.wait(t)), ref)
+        _check_mixed(work, pieces(mixed, opt.wait(t)), ref)
     feas = opt.feasibility(0.01)
     assert feas.shape == (mixed.B, 10) and (feas[:, 7] > 0).all()
     with pytest.raises(gpu.UalmError, match="mixes environments"):
@@ -175,7 +146,7 @@ def test_throughput_mixed_alone_and_at_depth_4(gpu, work, single, precision):
 def test_env_argument_and_state_checks(gpu, work, precision):
     from uneven_planner_b200 import _lib, problems
     mixed = work["mixed"]
-    opt = _mixed_ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work["params"], work["maps"])
     err = lambda code: pytest.raises(gpu.UalmError, match="error %d" % code)
     for bad in (4, -1):
         with err(_lib.UALM_EINVAL):
@@ -202,28 +173,25 @@ def test_env_argument_and_state_checks(gpu, work, precision):
         opt.solve_resident()
     # env = NULL is environment 0 for every problem
     one = work["pbs"][0]
-    a = _pieces(one, opt.optimize(one))
+    a = pieces(one, opt.optimize(one))
     zero = one.select(np.arange(one.B))
     zero.env = np.zeros(one.B, np.int32)
-    b = _pieces(zero, opt.optimize(zero))
-    assert all(_same(x, y) for x, y in zip(a, b))
+    b = pieces(zero, opt.optimize(zero))
+    assert all(same_values(x, y) for x, y in zip(a, b))
     ref = opt.optimize(mixed)
     opt.close()
     if precision == 64:
         # ualm_solve_batch_multi_env over two contexts (on one device here) equals the single-context result
-        opts = [_mixed_ctx(gpu, work) for _ in range(2)]
+        opts = [ctx(gpu, 64, work["params"], work["maps"]) for _ in range(2)]
         got = gpu.solve_batch_multi(opts, mixed)
         for o in opts:
             o.close()
-        assert all(_same(x, y) for x, y in zip(_pieces(mixed, got), _pieces(mixed, ref)))
+        assert all(same_values(x, y) for x, y in zip(pieces(mixed, got), pieces(mixed, ref)))
 
 
 def test_cpp_adapter_environment_overloads(gpu, bumps_map, tmp_path):
     from uneven_planner_b200 import _lib, problems
-    exe = str(tmp_path / "env_driver")
-    lib = os.path.join(ROOT, "uneven_planner_b200")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "env_driver.cpp"), "-o", exe,
-                    "-L", lib, "-lualm", "-Wl,-rpath," + lib], check=True)
+    exe = build_driver("env_driver", tmp_path)
     pb = problems.generate(bumps_map, 6, seed=5)
     pb.env = np.array([0, 1, 1, 0, 1, 0], np.int32)
     case = str(tmp_path / "envs.bin")

@@ -4,16 +4,10 @@ same resampled problems: bit-identical on the parity path."""
 import numpy as np
 import pytest
 
+from harness import gpu  # noqa: F401
+
+
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
 
 
 def test_start_goal_batch_through_the_front_end_matches_oracle(gpu, hill_map):

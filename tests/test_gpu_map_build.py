@@ -61,7 +61,7 @@ def test_device_map_matches_the_reference_build(opt):
     """ualm_map_build_device against the reference's OWN constructMap + filter (oracle/_ref/librefmap.so = uneven_map.cpp compiled
     unmodified, tests/test_ref_pin.py) on the same preprocessed cloud: float32 cells = the reference's doubles rounded, up to 2 ulps,
     except the <= 0.02 % of cells at the rim of the empty patch (degenerate footprints)."""
-    from test_ref_pin import analytic_cloud, preprocessed, reference_construct_map
+    from workloads import analytic_cloud, preprocessed, reference_construct_map
     pts = analytic_cloud(1.1, 100, seed=1, hole=(0.35, -0.3, 0.14))
     geom, ref = reference_construct_map(preprocessed(pts), 1.6)
     dev, _ = opt.build_map(pts, geom)

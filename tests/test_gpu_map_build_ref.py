@@ -10,7 +10,8 @@ import numpy as np
 import pytest
 
 import map_build_ref as mref
-from test_map_build_ref import SCENARIOS, _host, assert_matches_reference, reference, scenario, terrain
+from harness import bits
+from workloads import SCENARIOS, _host, assert_matches_reference, reference, terrain
 
 pytestmark = pytest.mark.gpu
 
@@ -26,15 +27,11 @@ def opt(built):
     o.close()
 
 
-def _bits(a):
-    return np.ascontiguousarray(a, np.float32).view(np.uint32)
-
-
 @pytest.mark.parametrize("name", list(SCENARIOS))
 def test_device_builder_matches_host_and_reference(opt, name):
     s, rows = reference(name)
     dev, _ = opt.build_map(s["pts"], s["geom"], ellipsoid=s["ellipsoid"], iter_num=s["iter_num"])
-    assert np.array_equal(_bits(dev.cells), _bits(_host(s)))
+    assert np.array_equal(bits(dev.cells, np.float32), bits(_host(s), np.float32))
     assert_matches_reference(dev.cells, s, rows, name)
 
 
@@ -70,7 +67,7 @@ def test_cloud_forms_match_the_reference_on_the_wall_off_centre(opt):
     # the whole grid, with the cells handed back
     m, _ = opt.update_environment_from_cloud(pts, geom)
     _assert_box(m.cells, rows, geom, (0, 0, X, Y), "update")
-    assert np.array_equal(_bits(m.cells), _bits(maps.build_from_cloud(pts, geom).cells))
+    assert np.array_equal(bits(m.cells, np.float32), bits(maps.build_from_cloud(pts, geom).cells, np.float32))
     # a window at the cloud's edge (the last columns of the grid, the cloud ending 0.25 m past them)
     box = (X - 6, 3, 6, 9)
     win, _ = opt.update_environment_window_from_cloud(pts, *box)

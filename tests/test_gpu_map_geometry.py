@@ -17,50 +17,19 @@ reaching the edges, or the window problems stop reading the boxes, that the devi
 Nothing here is timed, and out-of-range boxes are only ever offered to the library's argument checks."""
 import ctypes as C
 import functools
-import os
-import sys
 
 import numpy as np
 import pytest
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import test_gpu_tp_shapes as shapes  # noqa: E402
-from test_gpu_map_window import _cloud  # noqa: E402
-from test_gpu_minco_fused import _arc_problem  # noqa: E402
-from test_map_geometry import GRIDS, SMALL, geometry, grid  # noqa: E402
+import workloads
+from harness import alone, bits, cat, ctx, gpu, pieces, same_pieces, splice  # noqa: F401
+from workloads import BATCH_CASES, DT, GRIDS, SMALL, THREADS, _arc_problem, _cloud, _parity_evaluation, _scan_and_check, generated, geometry, grid, hand_cases
 
-THREADS = min(32, os.cpu_count() or 1)
+
 PRECISIONS = [64, 65, 32]
 TP = [65, 32]
-DT = 0.01
 WAIT_MS = 300000.0        # no wait here is unbounded: a batch that has not finished by then is stopped and the test fails
 N_GEN = 24
-BATCH_CASES = ("border_x", "border_y", "off_x", "off_y", "off_lo_x", "off_lo_y", "yaw_seam")
-
-
-# ------------------------------------------------------------------ batches
-def hand_cases(geom):
-    """problems placed from the grid's own bounds: an arc inside the last cell column in x / in y (clamped upper neighbours), paths
-    that leave through the +x, +y, -x and -y sides (the last two pass the clamped first cells on their way), and an arc whose yaw
-    runs over +-pi"""
-    from uneven_planner_b200 import problems
-    bx, by = geom.max_boundary[0], geom.max_boundary[1]
-    ox, oy = geom.origin[0], geom.origin[1]
-    return {
-        "border_x": _arc_problem(12, 20, radius=4.99, arc=0.3, start=-0.15, centre=(bx - 5.0, 0.1)),
-        "border_y": _arc_problem(12, 20, radius=4.99, arc=0.3, start=0.5 * np.pi - 0.15, centre=(-0.1, by - 5.0)),
-        "off_x": problems.from_paths([problems.dubins([bx - 0.8, 0.0, 0.0], [bx + 0.6, 0.3, 0.2])]),
-        "off_y": problems.from_paths([problems.dubins([0.2, by - 0.8, 0.5 * np.pi], [-0.1, by + 0.6, 0.5 * np.pi + 0.2])]),
-        "off_lo_x": problems.from_paths([problems.dubins([ox + 0.8, 0.3, np.pi], [ox - 0.6, 0.1, np.pi - 0.2])]),
-        "off_lo_y": problems.from_paths([problems.dubins([-0.3, oy + 0.8, -0.5 * np.pi], [0.1, oy - 0.6, -0.5 * np.pi + 0.2])]),
-        "yaw_seam": _arc_problem(10, 24, radius=2.0, arc=0.4 * np.pi, start=0.3 * np.pi),      # yaw 0.8 pi .. 1.2 pi
-    }
-
-
-def generated(m, n, seed):
-    from uneven_planner_b200 import problems
-    g = m.geom
-    return problems.generate(m, n, seed=seed, lo=(g.origin[0] + 0.5, g.origin[1] + 0.5), hi=(g.max_boundary[0] - 0.5, g.max_boundary[1] - 0.5))
 
 
 @functools.lru_cache(maxsize=None)
@@ -68,7 +37,7 @@ def batch(name):
     """N_GEN generated problems on grid `name`, then BATCH_CASES"""
     m = grid(name)
     hc = hand_cases(m.geom)
-    return shapes._cat([generated(m, N_GEN, GRIDS[name][5])] + [hc[k] for k in BATCH_CASES])
+    return cat([generated(m, N_GEN, GRIDS[name][5])] + [hc[k] for k in BATCH_CASES])
 
 
 def window_cases(geom):
@@ -136,7 +105,7 @@ def test_batches_reach_the_rectangle_and_its_edges(built):
             o = po.eval_one(op, om, one, 0, one.x0(0))
             got[case] = sides(one, o["c_xy"], g, p.int_K)
             if case == "yaw_seam":
-                assert shapes.reach(one, o["c_xy"], o["c_yaw"], g, p.int_K)["seam"] and not got[case], name
+                assert workloads.reach(one, o["c_xy"], o["c_yaw"], g, p.int_K)["seam"] and not got[case], name
         # fine_yaw's 183 cells in x reach 0.02 m past its 7.3 m, so no sample inside the map has a clamped upper neighbour in x there
         assert got["border_x"] == ({"hi_x"} if name != "fine_yaw" else set()) and got["border_y"] == {"hi_y"}, (name, got)
         assert got["off_x"] >= {"hi_x", "off_hi_x"} - ({"hi_x"} if name == "fine_yaw" else set()) and got["off_y"] >= {"hi_y", "off_hi_y"}, (name, got)
@@ -145,67 +114,16 @@ def test_batches_reach_the_rectangle_and_its_edges(built):
     # every box of the window tests is read by some problem of their batch: the oracle's constraint values change with each splice
     for name in ("wide", "tall"):
         base = grid(name)
-        pb = shapes._cat([batch(name)] + window_cases(base.geom))
+        pb = cat([batch(name)] + window_cases(base.geom))
         other = window_source(name)
         before = [po.eval_one(op, po.OracleMap(base), pb, i, pb.x0(i))["gx"].tobytes() for i in range(pb.B)]
         for box in _boxes(*base.shape[:2]):
             ix0, iy0, nx, ny = box
-            om = po.OracleMap(_splice(base, other.cells[ix0:ix0 + nx, iy0:iy0 + ny], box))
+            om = po.OracleMap(splice(base, other.cells[ix0:ix0 + nx, iy0:iy0 + ny], box))
             assert [po.eval_one(op, om, pb, i, pb.x0(i))["gx"].tobytes() for i in range(pb.B)] != before, (name, box)
 
 
 # ------------------------------------------------------------------ fixtures and helpers
-@pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
-
-
-def _pieces(pb, out):
-    """per problem: (record bytes, c_xy, c_yaw)"""
-    res, cxy, cyaw = out
-    _, _, ocx, ocy = pb.offsets()
-    return [(bytes(res[i]), cxy[ocx[i]:ocx[i + 1]].copy(), cyaw[ocy[i]:ocy[i + 1]].copy()) for i in range(pb.B)]
-
-
-def _same(a, b):
-    return len(a) == len(b) and all(x[0] == y[0] and np.array_equal(x[1], y[1]) and np.array_equal(x[2], y[2]) for x, y in zip(a, b))
-
-
-def _bits32(a):
-    return np.ascontiguousarray(a, np.float32).view(np.uint32)
-
-
-def _bits64(a):
-    return np.ascontiguousarray(a, np.float64).view(np.uint64)
-
-
-def _ctx(gpu, precision, m, params=None, env=None):
-    """a context of `precision` bound to grid m; env: environment variables set while the context is created"""
-    from uneven_planner_b200 import _lib
-    old = {k: os.environ.get(k) for k in (env or {})}
-    os.environ.update(env or {})
-    try:
-        return gpu.BatchALMTrajOpt(precision=precision).init(params or _lib.default_params()).set_environment(m)
-    finally:
-        for k, v in old.items():
-            if v is None:
-                os.environ.pop(k)
-            else:
-                os.environ[k] = v
-
-
-def _alone(gpu, precision, m, pb, params=None, env=None, feas=False):
-    opt = _ctx(gpu, precision, m, params, env)
-    out = opt.optimize(pb)
-    f = opt.feasibility(DT) if feas else None
-    opt.close()
-    return _pieces(pb, out), f
-
-
 def _wait(opt, ticket, pb):
     """wait with a bound; a batch that had to be stopped fails the test"""
     from uneven_planner_b200 import _lib
@@ -214,67 +132,13 @@ def _wait(opt, ticket, pb):
     return out
 
 
-def _parity_evaluation(opt, pb, params, oracle_map, seed=0):
-    """one evaluation at random duals and a perturbed point, and initScaling, of the parity context `opt` against the oracle on
-    `oracle_map`: bit for bit.  Returns the evaluation, with the oracle's constraint values of every problem as `oracle_gx`"""
-    import pyoracle as po
-    K = params.int_K
-    inputs = shapes._inputs(pb, [K] * pb.B, seed=seed)
-    xs, lam, mu, scx, sfx = inputs
-    offx, offs, ocx, ocy = shapes._offsets(pb, [K] * pb.B)
-    opt.upload(pb)
-    ev = opt.eval_batch(xs, lam, mu, scx, sfx, rho=shapes.RHO)
-    s_fx, s_cx = opt.init_scaling_batch()
-    op, om = po.params_from(params), po.OracleMap(oracle_map)
-    ev["oracle_gx"] = []
-    for i in range(pb.B):
-        o = po.eval_one(op, om, pb, i, xs[offx[i]:offx[i + 1]], lam[offs[i]:offs[i + 1]], mu[6 * offs[i]:6 * offs[i + 1]],
-                        scx[7 * offs[i]:7 * offs[i + 1]], sfx[i], shapes.RHO)
-        ev["oracle_gx"].append(o["gx"].tobytes())
-        assert ev["f"][i] == o["f"], i
-        assert np.array_equal(ev["grad"][offx[i]:offx[i + 1]], o["grad"]), i
-        assert np.array_equal(ev["hx"][offs[i]:offs[i + 1]], o["hx"]) and np.array_equal(ev["gx"][6 * offs[i]:6 * offs[i + 1]], o["gx"]), i
-        assert np.array_equal(ev["c_xy"][ocx[i]:ocx[i + 1]], o["c_xy"]) and np.array_equal(ev["c_yaw"][ocy[i]:ocy[i + 1]], o["c_yaw"]), i
-        osfx, oscx = po.init_scaling(op, om, pb, i)
-        assert s_fx[i] == osfx and np.array_equal(s_cx[7 * offs[i]:7 * offs[i + 1]], oscx), i
-    return ev
-
-
-def _scan_and_check(opt, m, params, pb, out):
-    """the lane's scan against orc_feasibility, and ualm_check_trajectories from t = 0 and from mid-trajectory against
-    tests/check_oracle.cpp, on the coefficients and piece durations of `out`: bit for bit"""
-    import pyoracle as po
-    from check_oracle import check, limits_of
-    res, cxy, cyaw = out
-    feas = opt.feasibility(DT)
-    om = po.OracleMap(m)
-    _, _, ocx, ocy = pb.offsets()
-    total = np.zeros(pb.B)
-    for i in range(pb.B):
-        r, N, M = res[i], int(pb.N[i]), int(pb.M[i])
-        assert r.piece_T_xy == feas[i, 8] and r.piece_T_yaw == feas[i, 9], i
-        ref = po.feasibility(om, params.gravity, N, M, cxy[ocx[i]:ocx[i + 1]], cyaw[ocy[i]:ocy[i + 1]], r.piece_T_xy, r.piece_T_yaw, DT)
-        assert np.array_equal(feas[i, :8], ref), (i, feas[i, :8], ref)
-        total[i] = min(N * r.piece_T_xy, M * r.piece_T_yaw)
-    for tf in (np.zeros(pb.B), 0.4 * total):
-        got = opt.check_results(pb, out, t_from=tf)
-        for i in range(pb.B):
-            ref = check(om, params.gravity, int(pb.N[i]), int(pb.M[i]), cxy[ocx[i]:ocx[i + 1]], cyaw[ocy[i]:ocy[i + 1]], res[i].piece_T_xy,
-                        res[i].piece_T_yaw, DT, tf[i], limits_of(params))
-            assert np.array_equal(_bits64(got[i]), _bits64(ref)), (i, tf[i], got[i], ref)
-        if not tf.any():
-            assert np.array_equal(_bits64(got[:, :10]), _bits64(feas))
-        else:
-            assert np.all(got[:, 7] < feas[:, 7]) and np.all(got[:, 7] > 0)
-
-
 # ------------------------------------------------------------------ a. parity path, one evaluation
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", list(GRIDS))
 def test_parity_evaluation_bitwise(gpu, name):
     from uneven_planner_b200 import _lib
     m, params = grid(name), _lib.default_params()
-    opt = _ctx(gpu, 64, m, params)
+    opt = ctx(gpu, 64, params, m)
     _parity_evaluation(opt, batch(name), params, m)
     opt.close()
 
@@ -292,10 +156,10 @@ def test_parity_evaluation_bitwise_double_grid(gpu, repack):
     opt = gpu.BatchALMTrajOpt().init(params).set_environment(m64, repack_to_float=bool(repack))
     ev = _parity_evaluation(opt, batch("wide"), params, seen)
     opt.close()
-    plain = _ctx(gpu, 64, base, params)
+    plain = ctx(gpu, 64, params, base)
     plain.upload(batch("wide"))
-    xs, lam, mu, scx, sfx = shapes._inputs(batch("wide"), [params.int_K] * batch("wide").B, seed=0)
-    assert not np.array_equal(plain.eval_batch(xs, lam, mu, scx, sfx, rho=shapes.RHO)["grad"], ev["grad"])      # the double grid's own values were read
+    xs, lam, mu, scx, sfx = workloads._inputs(batch("wide"), [params.int_K] * batch("wide").B, seed=0)
+    assert not np.array_equal(plain.eval_batch(xs, lam, mu, scx, sfx, rho=workloads.RHO)["grad"], ev["grad"])      # the double grid's own values were read
     plain.close()
 
 
@@ -304,10 +168,10 @@ def test_parity_evaluation_bitwise_double_grid(gpu, repack):
 @pytest.mark.parametrize("name,pname", [(n, "hill") for n in SMALL] + [("coarse", "forest")])
 def test_parity_solves_scan_and_check_match_oracle(gpu, name, pname):
     import pyoracle as po
-    from test_gpu_parity import _assert_solve_parity
+    from workloads import _assert_solve_parity
     from uneven_planner_b200 import configs
     m, params, pb = grid(name), configs.params_for(pname), batch(name)
-    opt = _ctx(gpu, 64, m, params)
+    opt = ctx(gpu, 64, params, m)
     out = opt.optimize(pb)
     ores = po.solve_batch(po.params_from(params), po.OracleMap(m), pb, threads=THREADS)
     _assert_solve_parity(pb, out[0], out[1], out[2], ores)
@@ -325,7 +189,7 @@ def _tiny():
     geom = _lib.map_geometry(10.0, 0.35, 0.05, 0.1)
     assert tuple(geom.voxel_num) == (200, 7, 64)
     m = maps.synthetic_terrain("hills", seed=206, geom=geom)
-    pb = shapes._cat([_arc_problem(12, 20, radius=40.0, arc=0.1, start=-0.5 * np.pi - 0.05, centre=(0.0, 40.011)),     # along x, |y| < 0.07
+    pb = cat([_arc_problem(12, 20, radius=40.0, arc=0.1, start=-0.5 * np.pi - 0.05, centre=(0.0, 40.011)),     # along x, |y| < 0.07
                       _arc_problem(3, 5, radius=0.12, arc=1.5 * np.pi, centre=(0.013, 0.011))])
     return m, pb.select(np.repeat(np.arange(pb.B), 2))
 
@@ -341,16 +205,16 @@ def test_throughput_evaluation_per_block_and_tile_staging(gpu, capfd, prec, name
     pb = pb if name == "tiny" else pb.select(np.repeat(np.arange(pb.B), 2))      # each at its guess (even) and perturbed (odd)
     params = _lib.default_params()
     Ks = [params.int_K] * pb.B
-    inputs = shapes._inputs(pb, Ks, seed=3)
-    want = shapes._oracle(pb, [params] * pb.B, [m] * pb.B, Ks, inputs)
-    direct, again = shapes.run_tp(gpu, pb, params, m, prec, inputs)
+    inputs = workloads._inputs(pb, Ks, seed=3)
+    want = workloads._oracle(pb, [params] * pb.B, [m] * pb.B, Ks, inputs)
+    direct, again = workloads.run_tp(gpu, pb, params, m, prec, inputs)
     capfd.readouterr()
-    tma, _ = shapes.run_tp(gpu, pb, params, m, prec, inputs, env={"UALM_TP_TMA": "1", "UALM_DEBUG": "1"})
+    tma, _ = workloads.run_tp(gpu, pb, params, m, prec, inputs, env={"UALM_TP_TMA": "1", "UALM_DEBUG": "1"})
     log = capfd.readouterr().err
     assert ("tensor map unavailable, TMA staging off" if name == "tiny" else "tensor map encoded, TMA staging on") in log, log
     for i in range(pb.B):
-        assert shapes._same(direct[i], again[i]) and shapes._same(direct[i], tma[i]), i
-    shapes._check(shapes.block_errors(pb, direct, want, Ks), prec, (prec, name))
+        assert workloads._same(direct[i], again[i]) and workloads._same(direct[i], tma[i]), i
+    workloads._check(workloads.block_errors(pb, direct, want, Ks), prec, (prec, name))
 
 
 # ------------------------------------------------------------------ d, e. throughput path, whole solves, their scan and check
@@ -361,8 +225,8 @@ def test_throughput_solves_scan_and_check(gpu, prec, name):
     import pyoracle as po
     from uneven_planner_b200 import _lib
     m, params = grid(name), _lib.default_params()
-    pb = shapes._cat([batch(name), generated(m, 64, GRIDS[name][5] + 50)])
-    opt = _ctx(gpu, prec, m, params)
+    pb = cat([batch(name), generated(m, 64, GRIDS[name][5] + 50)])
+    opt = ctx(gpu, prec, params, m)
     out = opt.optimize(pb)
     res, cxy, cyaw = out
     _, _, ocx, ocy = pb.offsets()
@@ -380,7 +244,7 @@ def test_throughput_solves_scan_and_check(gpu, prec, name):
         _, left = opt.poll(t, polled, wait_ms=500.0)
         spins += 1
     assert left == 0, "the submitted batch did not finish"
-    assert _same(_pieces(pb, polled), _pieces(pb, out)) and _same(_pieces(pb, _wait(opt, t, pb)), _pieces(pb, out))
+    assert same_pieces(pieces(pb, polled), pieces(pb, out)) and same_pieces(pieces(pb, _wait(opt, t, pb)), pieces(pb, out))
     opt.close()
     # the converged share of the generated problems against the oracle's on the same problems: test_population_matches_oracle's 0.06
     # on 256 problems is 2.3 standard deviations of a share near 0.8; on these 88 that is 0.10, the bound here.  Worst measured over
@@ -410,19 +274,11 @@ def test_device_builder_equals_host_builder(gpu, name):
     dev, ms = o.build_map(pts, geom)
     o.close()
     assert ms > 0.0 and dev.shape == tuple(geom.voxel_num)
-    assert np.array_equal(_bits32(dev.cells), _bits32(host.cells))
+    assert np.array_equal(bits(dev.cells, np.float32), bits(host.cells, np.float32))
     assert host.cells[..., 1].std() > 0 and host.cells[..., 2].std() > 0
 
 
 # ------------------------------------------------------------------ g. windows
-def _splice(base, win, box, name="spliced"):
-    from uneven_planner_b200 import maps
-    out = base.cells.copy()
-    ix0, iy0, nx, ny = box
-    out[ix0:ix0 + nx, iy0:iy0 + ny] = win
-    return maps.UnevenMapData(base.geom, out, name)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", ["wide", "tall"])
 def test_windows_on_a_rectangle(gpu, name):
@@ -431,17 +287,17 @@ def test_windows_on_a_rectangle(gpu, name):
     and leave the grid as it is"""
     from uneven_planner_b200 import _lib, maps
     base, params = grid(name), _lib.default_params()
-    pb = shapes._cat([batch(name)] + window_cases(base.geom))
+    pb = cat([batch(name)] + window_cases(base.geom))
     X, Y, W = base.shape
     other = window_source(name)
-    opt = _ctx(gpu, 64, base, params)
+    opt = ctx(gpu, 64, params, base)
     ref = base
     seen = _parity_evaluation(opt, pb, params, ref)["oracle_gx"]
     for box in _boxes(X, Y):
         ix0, iy0, nx, ny = box
         win = other.cells[ix0:ix0 + nx, iy0:iy0 + ny]
         opt.update_environment_window(ix0, iy0, win)
-        ref = _splice(ref, win, box)
+        ref = splice(ref, win, box)
         now = _parity_evaluation(opt, pb, params, ref)["oracle_gx"]
         assert now != seen, box
         seen = now
@@ -468,21 +324,21 @@ def test_cloud_windows_on_a_rectangle(gpu, prec, name):
     o = gpu.BatchALMTrajOpt()
     full, _ = o.build_map(pts, geom)
     o.close()
-    pb = shapes._cat([generated(base, 12, 7)] + window_cases(geom))
-    opt = _ctx(gpu, prec, base)
+    pb = cat([generated(base, 12, 7)] + window_cases(geom))
+    opt = ctx(gpu, prec, _lib.default_params(), base)
     ref = base
-    seen = _pieces(pb, opt.optimize(pb))
+    seen = pieces(pb, opt.optimize(pb))
     for box in _boxes(X, Y):
         ix0, iy0, nx, ny = box
         cells, ms = opt.update_environment_window_from_cloud(pts, *box)
         assert ms > 0.0 and cells.shape == (nx, ny, W, 4)
-        assert np.array_equal(_bits32(cells), _bits32(full.cells[ix0:ix0 + nx, iy0:iy0 + ny])), box
-        ref = _splice(ref, cells, box)
-        now = _pieces(pb, opt.optimize(pb))
-        assert _same(now, _alone(gpu, prec, ref, pb)[0]) and not _same(now, seen), box
+        assert np.array_equal(bits(cells, np.float32), bits(full.cells[ix0:ix0 + nx, iy0:iy0 + ny], np.float32)), box
+        ref = splice(ref, cells, box)
+        now = pieces(pb, opt.optimize(pb))
+        assert same_pieces(now, alone(ctx(gpu, prec, _lib.default_params(), ref), pb)[0]) and not same_pieces(now, seen), box
         seen = now
     assert _refuses_windows_outside(opt, X, Y, pts)
-    assert _same(_pieces(pb, opt.optimize(pb)), seen)
+    assert same_pieces(pieces(pb, opt.optimize(pb)), seen)
     opt.close()
 
 
@@ -514,7 +370,7 @@ def test_geometry_change_in_flight(gpu, prec, tma):
     wide, fine = grid("wide"), grid("fine_yaw")
     B, Cb = batch("wide"), batch("fine_yaw")
     L = _lib.lib()
-    opt = _ctx(gpu, prec, sq, env=env)
+    opt = ctx(gpu, prec, _lib.default_params(), sq, env=env)
     ta = opt.submit(A, depth=3)
     assert opt.poll(ta, opt.outputs(A), 0.0)[1] > 0
     opt.update_environment(wide)
@@ -528,17 +384,17 @@ def test_geometry_change_in_flight(gpu, prec, tma):
     tw = opt.submit(B, depth=4)
     opt.update_environment(fine)
     tc = opt.submit(Cb, depth=4)
-    got = {k: _pieces(pb, _wait(opt, t, pb)) for k, t, pb in (("a", ta, A), ("b", tb, B), ("w", tw, B), ("c", tc, Cb))}
+    got = {k: pieces(pb, _wait(opt, t, pb)) for k, t, pb in (("a", ta, A), ("b", tb, B), ("w", tw, B), ("c", tc, Cb))}
     opt.select_lane(ta)
     opt.pb = A
     scan_a = opt.feasibility(DT)
     opt.close()
-    ref_a, ref_scan = _alone(gpu, prec, sq, A, env=env, feas=True)
-    assert _same(got["a"], ref_a) and np.array_equal(_bits64(scan_a), _bits64(ref_scan))
-    assert _same(got["b"], _alone(gpu, prec, wide, B, env=env)[0])
-    assert _same(got["w"], _alone(gpu, prec, _splice(wide, win, (236, 40, 4, 40)), B, env=env)[0])
-    assert _same(got["c"], _alone(gpu, prec, fine, Cb, env=env)[0])
-    assert not _same(got["b"], got["w"])          # border_x runs through the window
+    ref_a, ref_scan = alone(ctx(gpu, prec, _lib.default_params(), sq, env=env), A, feas=True)
+    assert same_pieces(got["a"], ref_a) and np.array_equal(bits(scan_a), bits(ref_scan))
+    assert same_pieces(got["b"], alone(ctx(gpu, prec, _lib.default_params(), wide, env=env), B)[0])
+    assert same_pieces(got["w"], alone(ctx(gpu, prec, _lib.default_params(), splice(wide, win, (236, 40, 4, 40)), env=env), B)[0])
+    assert same_pieces(got["c"], alone(ctx(gpu, prec, _lib.default_params(), fine, env=env), Cb)[0])
+    assert not same_pieces(got["b"], got["w"])          # border_x runs through the window
 
 
 # ------------------------------------------------------------------ i. environments of different geometry in one context
@@ -559,19 +415,19 @@ def test_environments_of_different_geometry(gpu, prec):
         opt.init(params, env=e).set_environment(grids[e], env=e)
     solved = opt.optimize(mixed)
     waited = _wait(opt, opt.submit(mixed, depth=2), mixed)
-    assert _same(_pieces(mixed, solved), _pieces(mixed, waited))
+    assert same_pieces(pieces(mixed, solved), pieces(mixed, waited))
     chk = opt.check_results(mixed, solved, t_from=1.0)
     opt.close()
-    got = _pieces(mixed, solved)
+    got = pieces(mixed, solved)
     for e in range(4):
-        o = _ctx(gpu, prec, grids[e], params)
+        o = ctx(gpu, prec, params, grids[e])
         out = o.optimize(subs[e])
         alone_chk = o.check_results(subs[e], out, t_from=1.0)
         o.close()
-        alone = _pieces(subs[e], out)
+        alone = pieces(subs[e], out)
         rows = [i for i, q in enumerate(perm) if first[e] <= q < first[e + 1]]
         assert len(rows) == subs[e].B
         for i in rows:
             j = int(perm[i] - first[e])
-            assert _same([got[i]], [alone[j]]), (e, i, j)
-            assert np.array_equal(_bits64(chk[i]), _bits64(alone_chk[j])), (e, i, j)
+            assert same_pieces([got[i]], [alone[j]]), (e, i, j)
+            assert np.array_equal(bits(chk[i]), bits(alone_chk[j])), (e, i, j)

@@ -16,49 +16,22 @@ What each comparison is:
     strips as uint32 against the box of a whole-grid device build with the moved geometry."""
 import collections
 import functools
-import os
 import struct
 import subprocess
-import sys
 
 import numpy as np
 import pytest
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import test_gpu_tp_shapes as shapes  # noqa: E402
-from test_gpu_map_geometry import (BATCH_CASES, THREADS, _parity_evaluation, _scan_and_check, generated, hand_cases)  # noqa: E402
-from test_gpu_map_window import _cloud  # noqa: E402
-from test_map_geometry import GRIDS, grid  # noqa: E402
+import workloads
+from harness import alone, bits, build_driver, cat, ctx, gpu, pending, pieces, same_pieces  # noqa: F401
+from workloads import BATCH_CASES, GRIDS, THREADS, _cloud, _parity_evaluation, _scan_and_check, generated, grid, hand_cases
+
 
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PRECISIONS = [64, 32, 65]
 TP = [65, 32]
 DT = 0.01
 X0 = Y0 = 100                 # the hill stand-in's cell offset in the world
-
-
-@pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
-
-
-def _pieces(pb, out):
-    res, cxy, cyaw = out
-    _, _, ocx, ocy = pb.offsets()
-    return [(bytes(res[i]), cxy[ocx[i]:ocx[i + 1]].copy(), cyaw[ocy[i]:ocy[i + 1]].copy()) for i in range(pb.B)]
-
-
-def _same(a, b):
-    return len(a) == len(b) and all(x[0] == y[0] and np.array_equal(x[1], y[1]) and np.array_equal(x[2], y[2]) for x, y in zip(a, b))
-
-
-def _bits(a):
-    return np.ascontiguousarray(a, np.float32).view(np.uint32)
 
 
 def _moved(pb, cx, cy):
@@ -84,7 +57,7 @@ def _batch(m, n, seed):
     ext = (g.max_boundary[0] - g.origin[0], g.max_boundary[1] - g.origin[1])
     centred = _lib.map_geometry(ext[0], ext[1], g.xy_resolution, g.yaw_resolution)
     hc = hand_cases(centred)
-    return shapes._cat([generated(m, n, seed)] + [_moved(hc[k], *_centre(g)) for k in BATCH_CASES])
+    return cat([generated(m, n, seed)] + [_moved(hc[k], *_centre(g)) for k in BATCH_CASES])
 
 
 # ------------------------------------------------------------------ off-centre grids against the oracle
@@ -107,7 +80,7 @@ def off_batch(name, cx, cy):
 @pytest.mark.parametrize("name", ["square", "wide", "fine_yaw"])
 def test_off_centre_parity_evaluation_solves_scan_and_check(gpu, name, centre):
     import pyoracle as po
-    from test_gpu_parity import _assert_solve_parity
+    from workloads import _assert_solve_parity
     from uneven_planner_b200 import _lib
     m, params, pb = off_grid(name, *centre), _lib.default_params(), off_batch(name, *centre)
     opt = gpu.BatchALMTrajOpt(precision=64).init(params).set_environment(m)
@@ -152,17 +125,17 @@ def test_off_centre_throughput_evaluation_per_block(gpu, capfd, prec, r):
     pb = pb.select(np.repeat(np.arange(pb.B), 2))
     params = _lib.default_params()
     Ks = [params.int_K] * pb.B
-    inputs = shapes._inputs(pb, Ks, seed=3)
-    want = shapes._oracle(pb, [params] * pb.B, [m] * pb.B, Ks, inputs)
-    direct, again = shapes.run_tp(gpu, pb, params, m, prec, inputs)
-    tma, _ = shapes.run_tp(gpu, pb, params, m, prec, inputs, env={"UALM_TP_TMA": "1"})
+    inputs = workloads._inputs(pb, Ks, seed=3)
+    want = workloads._oracle(pb, [params] * pb.B, [m] * pb.B, Ks, inputs)
+    direct, again = workloads.run_tp(gpu, pb, params, m, prec, inputs)
+    tma, _ = workloads.run_tp(gpu, pb, params, m, prec, inputs, env={"UALM_TP_TMA": "1"})
     for i in range(pb.B):
-        assert shapes._same(direct[i], again[i]) and shapes._same(direct[i], tma[i]), i
-    worst = shapes.block_errors(pb, direct, want, Ks)
+        assert workloads._same(direct[i], again[i]) and workloads._same(direct[i], tma[i]), i
+    worst = workloads.block_errors(pb, direct, want, Ks)
     with capfd.disabled():
         print("\nTP_ORIGIN_ERR prec=%d |origin|=%g %s" % (prec, float(np.hypot(*c)), " ".join("%s=%.2e" % (k, v[0]) for k, v in sorted(worst.items()))))
     far = TP_EXCEEDS.get((prec, r), {})
-    shapes._check({k: v for k, v in worst.items() if k not in far}, prec, (prec, c))
+    workloads._check({k: v for k, v in worst.items() if k not in far}, prec, (prec, c))
     assert all(worst[k][0] <= bound for k, bound in far.items()), (prec, c, {k: worst[k] for k in far})
 
 
@@ -188,18 +161,6 @@ def _strips(m_new, geom_old, dx, dy):
     return [m_new.cells[ix0:ix0 + nx, iy0:iy0 + ny] for ix0, iy0, nx, ny in maps.shift_boxes(geom_old, dx, dy)]
 
 
-def _ctx(gpu, world, precision, m):
-    return gpu.BatchALMTrajOpt(precision=precision).init(world["params"]).set_environment(m)
-
-
-def _alone(gpu, world, precision, m, pb, feas=False):
-    opt = _ctx(gpu, world, precision, m)
-    out = opt.optimize(pb)
-    f = opt.feasibility(DT) if feas else None
-    opt.close()
-    return _pieces(pb, out), f
-
-
 def _start(d):
     """the start offset on one axis from which a shift by d stays inside the 400-cell world"""
     return 100 if abs(d) <= 100 else (0 if d > 0 else 200)
@@ -223,15 +184,11 @@ def test_host_cells_shift_equals_the_world_slice(gpu, world, precision):
         g = opt.shift_environment(dx, dy, _strips(new, g_old, dx, dy))
         assert bytes(g) == bytes(new.geom)
         pb = _batch(new, 24, 40 + abs(dx) + 3 * abs(dy))
-        got = _pieces(pb, opt.optimize(pb))
-        assert _same(got, _alone(gpu, world, precision, new, pb)[0]), (dx, dy)
+        got = pieces(pb, opt.optimize(pb))
+        assert same_pieces(got, alone(ctx(gpu, precision, world["params"], new), pb)[0]), (dx, dy)
         if abs(dx) < 150 and abs(dy) < 150:        # the grid moved under the problems: a lone solve on the old grid differs
-            assert not _same(got, _alone(gpu, world, precision, old, pb)[0]), (dx, dy)
+            assert not same_pieces(got, alone(ctx(gpu, precision, world["params"], old), pb)[0]), (dx, dy)
     opt.close()
-
-
-def _pending(opt, t, pb):
-    return opt.poll(t, opt.outputs(pb), 0.0)[1]
 
 
 @pytest.mark.parametrize("precision", PRECISIONS)
@@ -244,16 +201,16 @@ def test_batch_in_flight_keeps_its_grid_and_geometry(gpu, world, golden, precisi
     dx, dy = 7, -4
     new = _slice(world, X0 + dx, Y0 + dy, maps.shift_geometry(g0.geom, dx, dy))
     B = _batch(new, 96, 5)
-    opt = _ctx(gpu, world, precision, g0)
+    opt = ctx(gpu, precision, world["params"], g0)
     ta = opt.submit(A, depth=2)
-    assert _pending(opt, ta, A) > 0
+    assert pending(opt, ta, A) > 0
     opt.shift_environment(dx, dy, _strips(new, g0.geom, dx, dy))
-    assert _pending(opt, ta, A) > 0               # the host-cells shift returned while the batch ran, on both paths
+    assert pending(opt, ta, A) > 0               # the host-cells shift returned while the batch ran, on both paths
     tb = opt.submit(B, depth=2)
-    got_a, got_b = _pieces(A, opt.wait(ta)), _pieces(B, opt.wait(tb))
+    got_a, got_b = pieces(A, opt.wait(ta)), pieces(B, opt.wait(tb))
     opt.close()
-    assert _same(got_a, _alone(gpu, world, precision, g0, A)[0])
-    assert _same(got_b, _alone(gpu, world, precision, new, B)[0])
+    assert same_pieces(got_a, alone(ctx(gpu, precision, world["params"], g0), A)[0])
+    assert same_pieces(got_b, alone(ctx(gpu, precision, world["params"], new), B)[0])
     if precision == 64:
         n = gold_pb.B
         rec = [np.frombuffer(p[0], dtype=np.int32, count=3) for p in got_a[:n]]
@@ -272,7 +229,7 @@ def test_repeated_shifts_in_flight_follow_a_curve(gpu, world, precision):
     depth = 3 if precision == 64 else 8
     g0 = world["g0"]
     pb = _batch(g0, 64, 3)
-    opt = _ctx(gpu, world, precision, g0)
+    opt = ctx(gpu, precision, world["params"], g0)
 
     def fill():
         for t in [opt.submit(pb, depth=depth) for _ in range(depth)]:
@@ -299,11 +256,11 @@ def test_repeated_shifts_in_flight_follow_a_curve(gpu, world, precision):
     free1 = torch.cuda.mem_get_info()[0]
     end = _slice(world, ox, oy, geom)
     last = _batch(end, 48, 9)
-    got = _pieces(last, opt.optimize(last))
+    got = pieces(last, opt.optimize(last))
     opt.close()
     assert (ox, oy) != (X0, Y0)
     assert free0 - free1 <= g0.cells.nbytes, (free0, free1)
-    assert _same(got, _alone(gpu, world, precision, end, last)[0])
+    assert same_pieces(got, alone(ctx(gpu, precision, world["params"], end), last)[0])
 
 
 @pytest.mark.parametrize("precision", PRECISIONS)
@@ -323,12 +280,12 @@ def test_four_environments_only_the_shifted_one_changes(gpu, world, precision):
     t1 = opt.submit(mixed, depth=2)
     opt.shift_environment(dx, dy, _strips(new2, grids[2].geom, dx, dy), env=2)
     t2 = opt.submit(mixed, depth=2)
-    first, second = _pieces(mixed, opt.wait(t1)), _pieces(mixed, opt.wait(t2))
+    first, second = pieces(mixed, opt.wait(t1)), pieces(mixed, opt.wait(t2))
     opt.close()
 
     def alone(e, grid):
         o = gpu.BatchALMTrajOpt(precision=precision).init(params[e]).set_environment(grid)
-        out = _pieces(subs[e], o.optimize(subs[e]))
+        out = pieces(subs[e], o.optimize(subs[e]))
         o.close()
         return out
     ref = [alone(e, grids[e]) for e in range(4)]
@@ -336,10 +293,10 @@ def test_four_environments_only_the_shifted_one_changes(gpu, world, precision):
     o = 0
     for e in range(4):
         n = subs[e].B
-        assert _same(first[o:o + n], ref[e]), e
-        assert _same(second[o:o + n], ref2 if e == 2 else ref[e]), e
+        assert same_pieces(first[o:o + n], ref[e]), e
+        assert same_pieces(second[o:o + n], ref2 if e == 2 else ref[e]), e
         o += n
-    assert not _same(ref[2], ref2)
+    assert not same_pieces(ref[2], ref2)
 
 
 @pytest.mark.parametrize("precision", PRECISIONS)
@@ -350,8 +307,8 @@ def test_refused_shifts_keep_the_grid(gpu, world, precision):
     fp = C.POINTER(C.c_float)
     g0 = world["g0"]
     pb = _batch(g0, 32, 2)
-    opt = _ctx(gpu, world, precision, g0)
-    before = _pieces(pb, opt.optimize(pb))
+    opt = ctx(gpu, precision, world["params"], g0)
+    before = pieces(pb, opt.optimize(pb))
     cells = np.ascontiguousarray(g0.cells)
     cp = cells.ctypes.data_as(fp)
     pts = np.zeros((4, 3), np.float32)
@@ -368,13 +325,13 @@ def test_refused_shifts_keep_the_grid(gpu, world, precision):
     opt.select_env(1)                                                # no grid bound there
     assert both(1, 0) == ESTATE
     opt.select_env(0)
-    assert _same(_pieces(pb, opt.optimize(pb)), before)
+    assert same_pieces(pieces(pb, opt.optimize(pb)), before)
     opt.close()
     if precision == 64:
-        o = _ctx(gpu, world, precision, maps.UnevenMapData(g0.geom, g0.cells, "f64", cells64=g0.cells.astype(np.float64)))
-        before = _pieces(pb, o.optimize(pb))
+        o = ctx(gpu, precision, world["params"], maps.UnevenMapData(g0.geom, g0.cells, "f64", cells64=g0.cells.astype(np.float64)))
+        before = pieces(pb, o.optimize(pb))
         assert both(1, 0, h=o.h) == ESTATE
-        assert _same(_pieces(pb, o.optimize(pb)), before)
+        assert same_pieces(pieces(pb, o.optimize(pb)), before)
         o.close()
 
 
@@ -412,9 +369,9 @@ CLOUD_SHIFTS = [(-40, 0), (10, -3), (0, 12), (-3, -5)]
 @pytest.mark.parametrize("precision", PRECISIONS)
 def test_cloud_shift_strips_and_solve(gpu, world, cloud, precision):
     from uneven_planner_b200 import configs, maps, problems
-    assert np.array_equal(_bits(cloud["dev"].cells), _bits(cloud["host"].cells))      # off-centre: the builders agree bit for bit
+    assert np.array_equal(bits(cloud["dev"].cells, np.float32), bits(cloud["host"].cells, np.float32))      # off-centre: the builders agree bit for bit
     assert np.count_nonzero(cloud["dev"].cells[..., 1]) > 0.9 * cloud["dev"].cells[..., 1].size
-    opt = _ctx(gpu, world, precision, cloud["dev"])
+    opt = ctx(gpu, precision, world["params"], cloud["dev"])
     cur = cloud["dev"]
     hole = False
     for dx, dy in CLOUD_SHIFTS:
@@ -425,14 +382,14 @@ def test_cloud_shift_strips_and_solve(gpu, world, cloud, precision):
         o.close()
         boxes = maps.shift_boxes(cur.geom, dx, dy)
         for (ix0, iy0, nx, ny), c in zip(boxes, strips):
-            assert np.array_equal(_bits(c), _bits(full.cells[ix0:ix0 + nx, iy0:iy0 + ny])), (dx, dy)
+            assert np.array_equal(bits(c, np.float32), bits(full.cells[ix0:ix0 + nx, iy0:iy0 + ny], np.float32)), (dx, dy)
             hole |= bool(np.all(c[..., 1:] == 0.0, axis=(2, 3)).any())       # cells whose ellipsoids hold no point
         cur = maps.UnevenMapData(g2, _moved_cells(cur.cells, dx, dy, strips, boxes), "moved")
         lo = (g2.origin[0] + 0.5, g2.origin[1] + 0.5)
         hi = (g2.max_boundary[0] - 0.5, g2.max_boundary[1] - 0.5)
         pb = problems.generate(cur, 48, seed=3 + abs(dx) + 7 * abs(dy), lo=lo, hi=hi, min_dist=1.0, **configs.gen_kwargs("hill"))
-        got = _pieces(pb, opt.optimize(pb))
-        assert _same(got, _alone(gpu, world, precision, cur, pb)[0]), (dx, dy)
+        got = pieces(pb, opt.optimize(pb))
+        assert same_pieces(got, alone(ctx(gpu, precision, world["params"], cur), pb)[0]), (dx, dy)
     assert hole                                                         # the first strip covered the empty patch
     opt.close()
 
@@ -443,7 +400,7 @@ FAR = (31.4, -17.25)          # a grid centre whose crop box [c - 10, c + 10]^2 
 @pytest.fixture(scope="module")
 def far(gpu):
     """a 4 m grid centred at FAR and a seeded surface around it reaching 3.5 m each way, so that shifts of up to 1.5 m stay on it"""
-    from test_map_shift import _cloud_at
+    from workloads import _cloud_at
     from uneven_planner_b200 import _lib
     return dict(pts=_cloud_at(*FAR, n=120000, half=3.5, seed=2), geom=_lib.map_geometry_at(4.0, 4.0, 0.05, 0.1, *FAR))
 
@@ -459,14 +416,14 @@ def test_device_builders_crop_about_the_grid_centre_far_from_the_origin(gpu, wor
     o = gpu.BatchALMTrajOpt()
     dev, _ = o.build_map(pts, geom)
     o.close()
-    assert np.array_equal(_bits(dev.cells), _bits(host.cells))
-    opt = _ctx(gpu, world, 32, world["g0"])
+    assert np.array_equal(bits(dev.cells, np.float32), bits(host.cells, np.float32))
+    opt = ctx(gpu, 32, world["params"], world["g0"])
     upd, _ = opt.update_environment_from_cloud(pts, geom)
-    assert np.array_equal(_bits(upd.cells), _bits(host.cells))
+    assert np.array_equal(bits(upd.cells, np.float32), bits(host.cells, np.float32))
     box = (10, 25, 30, 20)
     win, _ = opt.update_environment_window_from_cloud(pts, *box)
     opt.close()
-    assert np.array_equal(_bits(win), _bits(host.cells[box[0]:box[0] + box[2], box[1]:box[1] + box[3]]))
+    assert np.array_equal(bits(win, np.float32), bits(host.cells[box[0]:box[0] + box[2], box[1]:box[1] + box[3]], np.float32))
 
 
 @pytest.mark.parametrize("precision", [64, 32])
@@ -476,19 +433,19 @@ def test_cloud_shift_far_from_the_origin(gpu, world, far, precision):
     from uneven_planner_b200 import configs, maps, problems
     pts = far["pts"]
     cur = maps.build_from_cloud(pts, far["geom"])
-    opt = _ctx(gpu, world, precision, cur)
+    opt = ctx(gpu, precision, world["params"], cur)
     for dx, dy in [(12, -7), (-30, 4)]:
         g2, strips, _ = opt.shift_environment_from_cloud(pts, dx, dy)
         want = maps.build_from_cloud(pts, g2)
         boxes = maps.shift_boxes(cur.geom, dx, dy)
         for (ix0, iy0, nx, ny), c in zip(boxes, strips):
-            assert np.array_equal(_bits(c), _bits(want.cells[ix0:ix0 + nx, iy0:iy0 + ny])), (dx, dy)
+            assert np.array_equal(bits(c, np.float32), bits(want.cells[ix0:ix0 + nx, iy0:iy0 + ny], np.float32)), (dx, dy)
             assert np.count_nonzero(c[..., 1]) > 0.9 * c[..., 1].size, (dx, dy)
         cur = maps.UnevenMapData(g2, _moved_cells(cur.cells, dx, dy, strips, boxes), "moved")
         lo = (g2.origin[0] + 0.5, g2.origin[1] + 0.5)
         hi = (g2.max_boundary[0] - 0.5, g2.max_boundary[1] - 0.5)
         pb = problems.generate(cur, 32, seed=5 + abs(dx), lo=lo, hi=hi, min_dist=1.0, **configs.gen_kwargs("hill"))
-        assert _same(_pieces(pb, opt.optimize(pb)), _alone(gpu, world, precision, cur, pb)[0]), (dx, dy)
+        assert same_pieces(pieces(pb, opt.optimize(pb)), alone(ctx(gpu, precision, world["params"], cur), pb)[0]), (dx, dy)
     opt.close()
 
 
@@ -498,14 +455,14 @@ def test_cloud_shift_returns_while_a_batch_runs(gpu, world):
     g0 = world["g0"]
     A = world["bench"]
     pts = _cloud(100000, 7.0, 6)
-    opt = _ctx(gpu, world, 32, g0)
+    opt = ctx(gpu, 32, world["params"], g0)
     ta = opt.submit(A, depth=2)
-    assert _pending(opt, ta, A) > 0
+    assert pending(opt, ta, A) > 0
     g2, strips, _ = opt.shift_environment_from_cloud(pts, 20, 0)
-    assert _pending(opt, ta, A) > 0
-    got_a = _pieces(A, opt.wait(ta))
+    assert pending(opt, ta, A) > 0
+    got_a = pieces(A, opt.wait(ta))
     opt.close()
-    assert _same(got_a, _alone(gpu, world, 32, g0, A)[0])
+    assert same_pieces(got_a, alone(ctx(gpu, 32, world["params"], g0), A)[0])
     assert bytes(g2) == bytes(maps.shift_geometry(g0.geom, 20, 0)) and strips[0].shape == (20, 200, 64, 4)
 
 
@@ -522,7 +479,7 @@ def test_check_and_replan_after_a_shift(gpu, world):
     pb = _batch(g0, 24, 12)
     dx, dy = -30, 0
     new = _slice(world, X0 + dx, Y0 + dy, maps.shift_geometry(g0.geom, dx, dy))
-    opt = _ctx(gpu, world, 64, g0)
+    opt = ctx(gpu, 64, world["params"], g0)
     out = opt.optimize(pb)
     before = opt.check_results(pb, out)
     opt.shift_environment(dx, dy, _strips(new, g0.geom, dx, dy))
@@ -538,19 +495,16 @@ def test_check_and_replan_after_a_shift(gpu, world):
     rows = np.arange(pb.B - len(BATCH_CASES))
     rows = rows[[res[i].ret_code == 0 for i in rows]][:12]
     ticket, rp = opt.submit_replan(pb, out, rows, 0.3)
-    got_r = _pieces(rp, opt.wait(ticket))
+    got_r = pieces(rp, opt.wait(ticket))
     opt.close()
     rp.env = None
-    assert _same(got_r, _alone(gpu, world, 64, new, rp)[0])
+    assert same_pieces(got_r, alone(ctx(gpu, 64, world["params"], new), rp)[0])
 
 
 # ------------------------------------------------------------------ C++
 def test_cpp_shifts_between_submits(gpu, world, tmp_path):
     from uneven_planner_b200 import _lib, maps
-    exe = str(tmp_path / "map_shift_driver")
-    lib = os.path.join(ROOT, "uneven_planner_b200")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "map_shift_driver.cpp"), "-o", exe,
-                    "-L", lib, "-lualm", "-Wl,-rpath," + lib], check=True)
+    exe = build_driver("map_shift_driver", tmp_path)
     g0 = world["g0"]
     pb = world["bench"].select(np.arange(8))
     dx, dy, dx2, dy2 = 5, -3, -2, 4
@@ -579,7 +533,7 @@ def test_cpp_shifts_between_submits(gpu, world, tmp_path):
     t3 = opt.submit(pb, depth=3)
     outs = [opt.wait(t1), opt.wait(t2), opt.wait(t3)]
     opt.close()
-    assert np.array_equal(np.fromfile(cloud_out, np.uint32), np.concatenate([_bits(c).ravel() for c in cs]))
+    assert np.array_equal(np.fromfile(cloud_out, np.uint32), np.concatenate([bits(c, np.float32).ravel() for c in cs]))
     _, _, ocx, _ = pb.offsets()
     want = ["%d %d %d %d %r %r" % (p, i, outs[p][0][i].ret_code, outs[p][0][i].n_evals, float(outs[p][0][i].inner_cost), float(outs[p][1][ocx[i] + 1]))
             for p in range(3) for i in range(pb.B)]

@@ -4,65 +4,23 @@ scan of its lane); every later launch reads the new grid; superseded grids are f
 stand-ins of hill (G0) and desert (G1), same geometry, solved with the hill parameters."""
 import collections
 import ctypes as C
-import os
 import struct
 import subprocess
 
 import numpy as np
 import pytest
 
+from harness import alone, build_driver, ctx, gpu, pending, pieces, same_pieces  # noqa: F401
+from workloads import hill_desert_world
+
+
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PRECISIONS = [64, 32, 65]
 
 
 @pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
-
-
-@pytest.fixture(scope="module")
 def world(gpu, golden):
-    from uneven_planner_b200 import configs, maps, problems
-    g0, g1 = maps.stand_in_terrain("hill"), maps.stand_in_terrain("desert")
-    kw = configs.gen_kwargs("hill")
-    gold = golden("hill", g0)
-    gold_pb = problems.generate(g0, int(gold["B"]), seed=int(gold["seed"]), **kw)
-    bench = problems.generate(g0, 1024, seed=0, **kw)
-    return dict(g0=g0, g1=g1, params=configs.params_for("hill"), gold=gold, gold_pb=gold_pb, bench=bench,
-                a64=problems.concat([gold_pb, bench], [0, 0]), b=problems.generate(g1, 256, seed=7, **kw))
-
-
-def _ctx(gpu, world, precision, grid):
-    return gpu.BatchALMTrajOpt(precision=precision).init(world["params"]).set_environment(grid)
-
-
-def _pieces(pb, out):
-    """per problem: (record bytes, c_xy, c_yaw)"""
-    res, cxy, cyaw = out
-    _, _, ocx, ocy = pb.offsets()
-    return [(bytes(res[i]), cxy[ocx[i]:ocx[i + 1]].copy(), cyaw[ocy[i]:ocy[i + 1]].copy()) for i in range(pb.B)]
-
-
-def _same(a, b):
-    return len(a) == len(b) and all(x[0] == y[0] and np.array_equal(x[1], y[1]) and np.array_equal(x[2], y[2]) for x, y in zip(a, b))
-
-
-def _alone(gpu, world, precision, grid, pb, feas=False):
-    """pb solved alone on a fresh context bound to `grid`: (pieces, scan or None)"""
-    opt = _ctx(gpu, world, precision, grid)
-    out = opt.optimize(pb)
-    f = opt.feasibility(0.01) if feas else None
-    opt.close()
-    return _pieces(pb, out), f
-
-
-def _pending(opt, t, pb):
-    return opt.poll(t, opt.outputs(pb), 0.0)[1]
+    return hill_desert_world(golden, b_grid="g1")
 
 
 def _scan(opt, ticket, pb):
@@ -77,20 +35,20 @@ def _scan(opt, ticket, pb):
 def test_batch_in_flight_keeps_its_grid_and_its_scan(gpu, world, precision):
     A = world["a64"] if precision == 64 else world["bench"]
     B = world["b"]
-    opt = _ctx(gpu, world, precision, world["g0"])
+    opt = ctx(gpu, precision, world["params"], world["g0"])
     ta = opt.submit(A, depth=2)
-    assert _pending(opt, ta, A) > 0
+    assert pending(opt, ta, A) > 0
     opt.update_environment(world["g1"])
     tb = opt.submit(B, depth=2)
-    got_a, got_b = _pieces(A, opt.wait(ta)), _pieces(B, opt.wait(tb))
+    got_a, got_b = pieces(A, opt.wait(ta)), pieces(B, opt.wait(tb))
     scan_a = _scan(opt, ta, A)
     opt.close()
-    ref_a, ref_scan = _alone(gpu, world, precision, world["g0"], A, feas=True)
-    assert _same(got_a, ref_a)
-    assert _same(got_b, _alone(gpu, world, precision, world["g1"], B)[0])
+    ref_a, ref_scan = alone(ctx(gpu, precision, world["params"], world["g0"]), A, feas=True)
+    assert same_pieces(got_a, ref_a)
+    assert same_pieces(got_b, alone(ctx(gpu, precision, world["params"], world["g1"]), B)[0])
     assert np.array_equal(scan_a, ref_scan)
     # the scan of A's coefficients against G1 differs: ualm_set_map writes into the grid the lane holds, as it always has
-    ref = _ctx(gpu, world, precision, world["g0"])
+    ref = ctx(gpu, precision, world["params"], world["g0"])
     ref.optimize(A)
     ref.set_environment(world["g1"])
     assert not np.array_equal(ref.feasibility(0.01), ref_scan)
@@ -123,21 +81,21 @@ def test_mixed_environments_only_the_updated_one_changes(gpu, world, precision):
     t1 = opt.submit(mixed, depth=2)
     opt.update_environment(new2, env=2)
     t2 = opt.submit(mixed, depth=2)
-    first, second = _pieces(mixed, opt.wait(t1)), _pieces(mixed, opt.wait(t2))
+    first, second = pieces(mixed, opt.wait(t1)), pieces(mixed, opt.wait(t2))
     opt.close()
 
     def alone(e, grid):
         o = gpu.BatchALMTrajOpt(precision=precision).init(params[e]).set_environment(grid)
-        out = _pieces(subs[e], o.optimize(subs[e]))
+        out = pieces(subs[e], o.optimize(subs[e]))
         o.close()
         return out
     ref = [alone(e, grids[e]) for e in range(4)]
     ref2 = alone(2, new2)
     for i, q in enumerate(perm):
         e, j = divmod(int(q), 256)
-        assert _same([first[i]], [ref[e][j]]), (i, e)
-        assert _same([second[i]], [(ref2 if e == 2 else ref[e])[j]]), (i, e)
-    assert any(not _same([ref[2][j]], [ref2[j]]) for j in range(256))      # the update changed environment 2's solves
+        assert same_pieces([first[i]], [ref[e][j]]), (i, e)
+        assert same_pieces([second[i]], [(ref2 if e == 2 else ref[e])[j]]), (i, e)
+    assert any(not same_pieces([ref[2][j]], [ref2[j]]) for j in range(256))      # the update changed environment 2's solves
 
 
 def _cloud(n, half, seed):
@@ -164,24 +122,24 @@ def cloud_world(world):
 def test_update_from_cloud(gpu, world, cloud_world, precision):
     cw = cloud_world
     A = world["bench"]
-    opt = _ctx(gpu, world, precision, world["g0"])
+    opt = ctx(gpu, precision, world["params"], world["g0"])
     ta = opt.submit(A, depth=2)
     m, ms = opt.update_environment_from_cloud(cw["pts"], cw["geom"])
     if precision != 64:
         # returned while the batch in flight still had problems running.  (The parity solve's CTAs hold every SM's register file
         # until its work queue runs dry, so there the build kernel only starts in the batch's tail: DESIGN section 3h)
-        assert _pending(opt, ta, A) > 0
+        assert pending(opt, ta, A) > 0
     assert ms > 0.0
     assert np.array_equal(m.cells.view(np.uint32), cw["host"].cells.view(np.uint32))
     tc = opt.submit(cw["pb"], depth=2)
-    got = _pieces(cw["pb"], opt.wait(tc))
+    got = pieces(cw["pb"], opt.wait(tc))
     opt.wait(ta)
     opt.close()
-    ref = _ctx(gpu, world, precision, world["g0"])
+    ref = ctx(gpu, precision, world["params"], world["g0"])
     ref.set_environment(cw["host"])
-    want = _pieces(cw["pb"], ref.wait(ref.submit(cw["pb"], depth=2)))
+    want = pieces(cw["pb"], ref.wait(ref.submit(cw["pb"], depth=2)))
     ref.close()
-    assert _same(got, want)
+    assert same_pieces(got, want)
 
 
 @pytest.mark.parametrize("precision", PRECISIONS)
@@ -189,7 +147,7 @@ def test_updates_do_not_leak(gpu, world, precision):
     import torch
     depth = 3 if precision == 64 else 8
     pb = world["b"]
-    opt = _ctx(gpu, world, precision, world["g0"])
+    opt = ctx(gpu, precision, world["params"], world["g0"])
 
     def fill():
         for t in [opt.submit(pb, depth=depth) for _ in range(depth)]:
@@ -219,8 +177,8 @@ def test_refused_and_failed_updates_keep_the_grid(gpu, world, precision):
     L = _lib.lib()
     fp = C.POINTER(C.c_float)
     pb = world["b"]
-    opt = _ctx(gpu, world, precision, world["g0"])
-    before = _pieces(pb, opt.optimize(pb))
+    opt = ctx(gpu, precision, world["params"], world["g0"])
+    before = pieces(pb, opt.optimize(pb))
     g = world["g1"].geom
     cells = world["g1"].cells.ctypes.data_as(fp)
     pts = np.zeros((4, 3), np.float32)
@@ -241,16 +199,13 @@ def test_refused_and_failed_updates_keep_the_grid(gpu, world, precision):
     huge = _lib.map_geometry()
     huge.voxel_num[0] = huge.voxel_num[1] = 200000
     assert L.ualm_update_map_from_cloud(opt.h, ptsp, 4, C.byref(huge), 0.2, 0.1, 0.1, 2, None, None) == _lib.UALM_ENOCUDA
-    assert _same(_pieces(pb, opt.optimize(pb)), before)
+    assert same_pieces(pieces(pb, opt.optimize(pb)), before)
     opt.close()
 
 
 def test_cpp_update_environment_between_submits(gpu, world, tmp_path):
     from uneven_planner_b200 import _lib
-    exe = str(tmp_path / "map_update_driver")
-    lib = os.path.join(ROOT, "uneven_planner_b200")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "map_update_driver.cpp"), "-o", exe,
-                    "-L", lib, "-lualm", "-Wl,-rpath," + lib], check=True)
+    exe = build_driver("map_update_driver", tmp_path)
     g0, g1 = world["g0"], world["g1"]
     pb = world["bench"].select(np.arange(8))
     case = str(tmp_path / "update.bin")

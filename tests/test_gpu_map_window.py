@@ -5,66 +5,24 @@ grid's.  Work launched before a window keeps its grid; every later launch reads 
 and desert (G1), solved with the hill parameters; for clouds, the seeded analytic cloud of tests/test_gpu_map_build.py on its 4 m grid."""
 import collections
 import ctypes as C
-import os
 import struct
 import subprocess
 
 import numpy as np
 import pytest
 
+from harness import alone, bits, box_cells, build_driver, ctx, gpu, pending, pieces, same_pieces, splice  # noqa: F401
+from workloads import _cloud, hill_desert_world
+
+
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PRECISIONS = [64, 32, 65]
 BOX = (60, 80, 40, 40)                # a 2 m x 2 m window of the 10 m grid, where the hill problems run
 
 
 @pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
-
-
-@pytest.fixture(scope="module")
 def world(gpu, golden):
-    from uneven_planner_b200 import configs, maps, problems
-    g0, g1 = maps.stand_in_terrain("hill"), maps.stand_in_terrain("desert")
-    kw = configs.gen_kwargs("hill")
-    gold = golden("hill", g0)
-    gold_pb = problems.generate(g0, int(gold["B"]), seed=int(gold["seed"]), **kw)
-    bench = problems.generate(g0, 1024, seed=0, **kw)
-    return dict(g0=g0, g1=g1, params=configs.params_for("hill"), gold=gold, gold_pb=gold_pb, bench=bench,
-                a64=problems.concat([gold_pb, bench], [0, 0]), b=problems.generate(g0, 256, seed=7, **kw))
-
-
-def _ctx(gpu, world, precision, grid):
-    return gpu.BatchALMTrajOpt(precision=precision).init(world["params"]).set_environment(grid)
-
-
-def _pieces(pb, out):
-    """per problem: (record bytes, c_xy, c_yaw)"""
-    res, cxy, cyaw = out
-    _, _, ocx, ocy = pb.offsets()
-    return [(bytes(res[i]), cxy[ocx[i]:ocx[i + 1]].copy(), cyaw[ocy[i]:ocy[i + 1]].copy()) for i in range(pb.B)]
-
-
-def _same(a, b):
-    return len(a) == len(b) and all(x[0] == y[0] and np.array_equal(x[1], y[1]) and np.array_equal(x[2], y[2]) for x, y in zip(a, b))
-
-
-def _alone(gpu, world, precision, grid, pb, feas=False):
-    """pb solved alone on a fresh context bound to `grid` with ualm_set_map: (pieces, scan or None)"""
-    opt = _ctx(gpu, world, precision, grid)
-    out = opt.optimize(pb)
-    f = opt.feasibility(0.01) if feas else None
-    opt.close()
-    return _pieces(pb, out), f
-
-
-def _pending(opt, t, pb):
-    return opt.poll(t, opt.outputs(pb), 0.0)[1]
+    return hill_desert_world(golden)
 
 
 def _scan(opt, ticket, pb):
@@ -73,24 +31,6 @@ def _scan(opt, ticket, pb):
     f = opt.feasibility(0.01)
     opt.select_lane(0)
     return f
-
-
-def _box(cells, box):
-    ix0, iy0, nx, ny = box
-    return cells[ix0:ix0 + nx, iy0:iy0 + ny]
-
-
-def _splice(base, cells, box, name="spliced"):
-    """base's grid with `cells` in the box, done in numpy"""
-    from uneven_planner_b200 import maps
-    out = base.cells.copy()
-    ix0, iy0, nx, ny = box
-    out[ix0:ix0 + nx, iy0:iy0 + ny] = cells
-    return maps.UnevenMapData(base.geom, out, name)
-
-
-def _bits(a):
-    return np.ascontiguousarray(a, np.float32).view(np.uint32)
 
 
 # ---- host cells ---------------------------------------------------------------------------------
@@ -102,32 +42,20 @@ def test_host_cells_window_equals_the_spliced_grid(gpu, world, precision):
     g0, g1, pb = world["g0"], world["g1"], world["b"]
     X, Y, _ = g0.shape
     boxes = [BOX, (0, 30, 25, 120), (X - 35, Y - 50, 35, 50), (100, 100, 1, 1)]
-    opt = _ctx(gpu, world, precision, g0)
-    before = _pieces(pb, opt.optimize(pb))
+    opt = ctx(gpu, precision, world["params"], g0)
+    before = pieces(pb, opt.optimize(pb))
     ref = g0
     for k, box in enumerate(boxes):
-        opt.update_environment_window(box[0], box[1], _box(g1.cells, box))
-        ref = _splice(ref, _box(g1.cells, box), box)
-        got = _pieces(pb, opt.optimize(pb))
-        assert _same(got, _alone(gpu, world, precision, ref, pb)[0]), box
+        opt.update_environment_window(box[0], box[1], box_cells(g1.cells, box))
+        ref = splice(ref, box_cells(g1.cells, box), box)
+        got = pieces(pb, opt.optimize(pb))
+        assert same_pieces(got, alone(ctx(gpu, precision, world["params"], ref), pb)[0]), box
         if k == 0:
-            assert not _same(got, before)        # the window is where the problems run
+            assert not same_pieces(got, before)        # the window is where the problems run
     opt.close()
 
 
 # ---- clouds -------------------------------------------------------------------------------------
-
-def _cloud(n, half, seed, hole=True):
-    """a seeded analytic surface with noise and an empty patch (as tests/test_gpu_map_build.py)"""
-    rng = np.random.default_rng(seed)
-    xy = rng.uniform(-half, half, (n, 2))
-    z = 0.4 * np.exp(-((xy[:, 0] - 0.5) ** 2 + (xy[:, 1] + 0.3) ** 2) / 0.8) + 0.15 * np.sin(2.0 * xy[:, 0]) * np.cos(1.5 * xy[:, 1]) + 0.3
-    z += rng.normal(0.0, 0.004, n)
-    pts = np.column_stack([xy, z]).astype(np.float32)
-    if hole:   # an empty patch around (-1, 1): cells there take the "no points in the ellipsoid" branch
-        keep = ~((np.abs(pts[:, 0] + 1.0) < 0.35) & (np.abs(pts[:, 1] - 1.0) < 0.35))
-        pts = pts[keep]
-    return pts
 
 
 # boxes of the 4 m, 80 x 80 x 64 grid: 2 m x 2 m in the middle, one that covers the empty patch (cells 13..27 x 53..67), one at the edges
@@ -152,23 +80,23 @@ def small(gpu, world):
 def test_cloud_window_cells_and_solve(gpu, world, small, precision):
     """cells_out is bit for bit the box of a whole-grid build of the same cloud (device and host); a solve after the update equals a
     lone solve on the previous grid with that box spliced in"""
-    assert np.array_equal(_bits(small["dev"].cells), _bits(small["host"].cells))
+    assert np.array_equal(bits(small["dev"].cells, np.float32), bits(small["host"].cells, np.float32))
     pb = small["pb"]
-    opt = _ctx(gpu, world, precision, small["base"])
-    before = _pieces(pb, opt.optimize(pb))
+    opt = ctx(gpu, precision, world["params"], small["base"])
+    before = pieces(pb, opt.optimize(pb))
     ref = small["base"]
     for box in CLOUD_BOXES:
         cells, ms = opt.update_environment_window_from_cloud(small["pts"], *box)
         assert ms > 0.0
         assert cells.shape == (box[2], box[3], small["geom"].voxel_num[2], 4)
-        assert np.array_equal(_bits(cells), _bits(_box(small["dev"].cells, box))), box
-        assert np.array_equal(_bits(cells), _bits(_box(small["host"].cells, box))), box
-        ref = _splice(ref, cells, box)
-        got = _pieces(pb, opt.optimize(pb))
-        assert _same(got, _alone(gpu, world, precision, ref, pb)[0]), box
-    assert not _same(got, before)
+        assert np.array_equal(bits(cells, np.float32), bits(box_cells(small["dev"].cells, box), np.float32)), box
+        assert np.array_equal(bits(cells, np.float32), bits(box_cells(small["host"].cells, box), np.float32)), box
+        ref = splice(ref, cells, box)
+        got = pieces(pb, opt.optimize(pb))
+        assert same_pieces(got, alone(ctx(gpu, precision, world["params"], ref), pb)[0]), box
+    assert not same_pieces(got, before)
     # the cells at the empty patch's centre, whose ellipsoids (reach 0.32 m) hold no point, took the "no points" branch (sigma 0, zb 0)
-    patch = _box(ref.cells, (19, 59, 2, 2))
+    patch = box_cells(ref.cells, (19, 59, 2, 2))
     assert np.all(patch[..., 1:] == 0.0)
     opt.close()
 
@@ -180,7 +108,7 @@ def test_local_scan_window_matches_the_full_cloud(gpu, world, small):
     g = small["geom"]
     pts = small["pts"]
     margin = 0.2 + 0.12 + 0.2              # box_r + the 0.12 m forward shift, and the empty patch's half width for the nearest point
-    opt = _ctx(gpu, world, 64, small["base"])
+    opt = ctx(gpu, 64, world["params"], small["base"])
     for box in CLOUD_BOXES:
         ix0, iy0, nx, ny = box
         x0, y0 = g.origin[0] + ix0 * g.xy_resolution, g.origin[1] + iy0 * g.xy_resolution
@@ -188,7 +116,7 @@ def test_local_scan_window_matches_the_full_cloud(gpu, world, small):
         local = pts[(pts[:, 0] >= x0 - margin) & (pts[:, 0] <= x1 + margin) & (pts[:, 1] >= y0 - margin) & (pts[:, 1] <= y1 + margin)]
         assert len(local) < len(pts) // 2
         cells, _ = opt.update_environment_window_from_cloud(local, *box)
-        ref = _box(small["host"].cells, box).astype(np.float64)
+        ref = box_cells(small["host"].cells, box).astype(np.float64)
         d = np.abs(cells.astype(np.float64) - ref)
         rel = (d / np.maximum(np.abs(ref), 1e-3)).max(axis=-1)
         assert (rel > 3e-7).mean() <= 2e-4, (box, (rel > 3e-7).mean(), rel.max())
@@ -218,31 +146,31 @@ def test_batch_in_flight_keeps_its_grid_and_its_scan(gpu, world, big_cloud, prec
     A = world["a64"] if precision == 64 else world["bench"]
     B = world["b"]
     g0 = world["g0"]
-    opt = _ctx(gpu, world, precision, g0)
+    opt = ctx(gpu, precision, world["params"], g0)
     ta = opt.submit(A, depth=2)
-    assert _pending(opt, ta, A) > 0
+    assert pending(opt, ta, A) > 0
     if variant == "cells":
-        win = _box(world["g1"].cells, BOX)
+        win = box_cells(world["g1"].cells, BOX)
         opt.update_environment_window(BOX[0], BOX[1], win)
     else:
         win, _ = opt.update_environment_window_from_cloud(big_cloud, *BOX)
     if precision != 64 or variant == "cells":
         # returned while the batch in flight still ran.  (On the parity path a cloud window's kernel waits for a free SM slot,
         # which its solve frees only in the batch's tail: DESIGN section 3h)
-        assert _pending(opt, ta, A) > 0
+        assert pending(opt, ta, A) > 0
     tb = opt.submit(B, depth=2)
-    got_a, got_b = _pieces(A, opt.wait(ta)), _pieces(B, opt.wait(tb))
+    got_a, got_b = pieces(A, opt.wait(ta)), pieces(B, opt.wait(tb))
     scan_a = _scan(opt, ta, A)
     opt.close()
     if variant == "cloud":
         o = gpu.BatchALMTrajOpt()
         full, _ = o.build_map(big_cloud, g0.geom)
         o.close()
-        assert np.array_equal(_bits(win), _bits(_box(full.cells, BOX)))
-    spliced = _splice(g0, win, BOX)
-    ref_a, ref_scan = _alone(gpu, world, precision, g0, A, feas=True)
-    assert _same(got_a, ref_a)
-    assert _same(got_b, _alone(gpu, world, precision, spliced, B)[0])
+        assert np.array_equal(bits(win, np.float32), bits(box_cells(full.cells, BOX), np.float32))
+    spliced = splice(g0, win, BOX)
+    ref_a, ref_scan = alone(ctx(gpu, precision, world["params"], g0), A, feas=True)
+    assert same_pieces(got_a, ref_a)
+    assert same_pieces(got_b, alone(ctx(gpu, precision, world["params"], spliced), B)[0])
     assert np.array_equal(scan_a, ref_scan)
     if precision == 64:
         g, n = world["gold"], world["gold_pb"].B      # A's first problems are the golden ones
@@ -266,29 +194,29 @@ def test_mixed_environments_only_the_updated_one_changes(gpu, world, precision):
     perm = np.array([256 * e + i for i in range(256) for e in range(4)])
     mixed = cat.select(perm)
     box = (50, 50, 100, 100)
-    win = _box(maps.stand_in_terrain("mountain").cells, box)
-    new2 = _splice(grids[2], win, box)
+    win = box_cells(maps.stand_in_terrain("mountain").cells, box)
+    new2 = splice(grids[2], win, box)
     opt = gpu.BatchALMTrajOpt(precision=precision)
     for e in range(4):
         opt.init(params[e], env=e).set_environment(grids[e], env=e)
     t1 = opt.submit(mixed, depth=2)
     opt.update_environment_window(box[0], box[1], win, env=2)
     t2 = opt.submit(mixed, depth=2)
-    first, second = _pieces(mixed, opt.wait(t1)), _pieces(mixed, opt.wait(t2))
+    first, second = pieces(mixed, opt.wait(t1)), pieces(mixed, opt.wait(t2))
     opt.close()
 
     def alone(e, grid):
         o = gpu.BatchALMTrajOpt(precision=precision).init(params[e]).set_environment(grid)
-        out = _pieces(subs[e], o.optimize(subs[e]))
+        out = pieces(subs[e], o.optimize(subs[e]))
         o.close()
         return out
     ref = [alone(e, grids[e]) for e in range(4)]
     ref2 = alone(2, new2)
     for i, q in enumerate(perm):
         e, j = divmod(int(q), 256)
-        assert _same([first[i]], [ref[e][j]]), (i, e)
-        assert _same([second[i]], [(ref2 if e == 2 else ref[e])[j]]), (i, e)
-    assert any(not _same([ref[2][j]], [ref2[j]]) for j in range(256))      # the window changed environment 2's solves
+        assert same_pieces([first[i]], [ref[e][j]]), (i, e)
+        assert same_pieces([second[i]], [(ref2 if e == 2 else ref[e])[j]]), (i, e)
+    assert any(not same_pieces([ref[2][j]], [ref2[j]]) for j in range(256))      # the window changed environment 2's solves
 
 
 # ---- refusals, memory, C++ ----------------------------------------------------------------------
@@ -300,8 +228,8 @@ def test_refused_windows_keep_the_grid(gpu, world, precision):
     fp = C.POINTER(C.c_float)
     pb = world["b"]
     X, Y, W = world["g0"].shape
-    opt = _ctx(gpu, world, precision, world["g0"])
-    before = _pieces(pb, opt.optimize(pb))
+    opt = ctx(gpu, precision, world["params"], world["g0"])
+    before = pieces(pb, opt.optimize(pb))
     cells = np.ascontiguousarray(world["g1"].cells[:X, :Y])          # big enough for every box below
     cp = cells.ctypes.data_as(fp)
     pts = np.zeros((4, 3), np.float32)
@@ -321,14 +249,14 @@ def test_refused_windows_keep_the_grid(gpu, world, precision):
     opt.select_env(1)                                                # no grid bound there
     assert both(0, 0, 4, 4) == ESTATE
     opt.select_env(0)
-    assert _same(_pieces(pb, opt.optimize(pb)), before)
+    assert same_pieces(pieces(pb, opt.optimize(pb)), before)
     opt.close()
     if precision == 64:        # the double grid of ualm_set_map_f64 is not windowed
         g0 = world["g0"]
-        o = _ctx(gpu, world, precision, maps.UnevenMapData(g0.geom, g0.cells, "f64", cells64=g0.cells.astype(np.float64)))
-        before = _pieces(pb, o.optimize(pb))
+        o = ctx(gpu, precision, world["params"], maps.UnevenMapData(g0.geom, g0.cells, "f64", cells64=g0.cells.astype(np.float64)))
+        before = pieces(pb, o.optimize(pb))
         assert both(0, 0, 4, 4, h=o.h) == ESTATE
-        assert _same(_pieces(pb, o.optimize(pb)), before)
+        assert same_pieces(pieces(pb, o.optimize(pb)), before)
         o.close()
 
 
@@ -337,7 +265,7 @@ def test_windows_do_not_leak(gpu, world, precision):
     import torch
     depth = 3 if precision == 64 else 8
     pb = world["b"]
-    opt = _ctx(gpu, world, precision, world["g0"])
+    opt = ctx(gpu, precision, world["params"], world["g0"])
 
     def fill():
         for t in [opt.submit(pb, depth=depth) for _ in range(depth)]:
@@ -348,7 +276,7 @@ def test_windows_do_not_leak(gpu, world, precision):
     q = collections.deque()
     for i in range(20):
         src = world["g1"] if i % 2 == 0 else world["g0"]
-        opt.update_environment_window(BOX[0], BOX[1], _box(src.cells, BOX))
+        opt.update_environment_window(BOX[0], BOX[1], box_cells(src.cells, BOX))
         if len(q) == depth:
             opt.wait(q.popleft())
         q.append(opt.submit(pb, depth=depth))
@@ -364,13 +292,10 @@ def test_windows_do_not_leak(gpu, world, precision):
 
 def test_cpp_window_updates_between_submits(gpu, world, big_cloud, tmp_path):
     from uneven_planner_b200 import _lib
-    exe = str(tmp_path / "map_window_driver")
-    lib = os.path.join(ROOT, "uneven_planner_b200")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "map_window_driver.cpp"), "-o", exe,
-                    "-L", lib, "-lualm", "-Wl,-rpath," + lib], check=True)
+    exe = build_driver("map_window_driver", tmp_path)
     g0, g1 = world["g0"], world["g1"]
     pb = world["bench"].select(np.arange(8))
-    win = np.ascontiguousarray(_box(g1.cells, BOX))
+    win = np.ascontiguousarray(box_cells(g1.cells, BOX))
     pts = big_cloud[:100000]
     case = str(tmp_path / "window.bin")
     with open(case, "wb") as f:
@@ -393,7 +318,7 @@ def test_cpp_window_updates_between_submits(gpu, world, big_cloud, tmp_path):
     t3 = opt.submit(pb, depth=3)
     outs = [opt.wait(t1), opt.wait(t2), opt.wait(t3)]
     opt.close()
-    assert np.array_equal(np.fromfile(cloud_out, np.uint32), _bits(cw).ravel())
+    assert np.array_equal(np.fromfile(cloud_out, np.uint32), bits(cw, np.float32).ravel())
     _, _, ocx, _ = pb.offsets()
     want = ["%d %d %d %d %r %r" % (p, i, outs[p][0][i].ret_code, outs[p][0][i].n_evals, float(outs[p][0][i].inner_cost), float(outs[p][1][ocx[i] + 1]))
             for p in range(3) for i in range(pb.B)]

@@ -5,37 +5,11 @@ boundary rows."""
 import numpy as np
 import pytest
 
+from harness import gpu  # noqa: F401
+from workloads import _arc_problem
+
+
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
-
-
-def _arc_problem(N, M, zero_ends=False, radius=2.5, arc=1.5 * np.pi, speed=0.5, centre=(0.0, 0.0), start=0.0):
-    """One problem whose waypoints lie on a circular arc around `centre` (the map centre by default), from polar angle `start`
-    counter-clockwise over `arc`: N xy pieces, M yaw pieces.  zero_ends: zero boundary velocity and acceleration, so that those
-    right-hand-side rows are exact zeros."""
-    from uneven_planner_b200 import problems
-    length = radius * arc
-    T = 1.2 * length / speed
-    a = start + arc * np.linspace(0.0, 1.0, N + 1)
-    rel = radius * np.stack([np.cos(a), np.sin(a)], axis=1)
-    pts = rel + np.asarray(centre, np.float64)
-    yaw = start + arc * np.linspace(0.0, 1.0, M + 1) + 0.5 * np.pi
-    tan0, tan1 = np.array([-np.sin(a[0]), np.cos(a[0])]), np.array([-np.sin(a[-1]), np.cos(a[-1])])
-    v = 0.0 if zero_ends else speed
-    acc0 = np.zeros(2) if zero_ends else -speed ** 2 / radius * rel[0] / radius
-    acc1 = np.zeros(2) if zero_ends else -speed ** 2 / radius * rel[-1] / radius
-    dyaw = 0.0 if zero_ends else speed / radius
-    bnd = np.concatenate([pts[0], v * tan0, acc0, pts[-1], v * tan1, acc1, [yaw[0], dyaw, 0.0, yaw[-1], dyaw, 0.0]])
-    return problems.ProblemBatch(np.array([N], np.int32), np.array([M], np.int32), bnd.reshape(1, 18), np.array([T]),
-                                 pts[1:-1].ravel().copy(), yaw[1:-1].copy())
 
 
 CASES = {

@@ -12,14 +12,14 @@ mpc_ref, dev_ref) on the records the solve returned, at precisions 64, 65 and 32
 at nonzero boundary derivatives, at several dt and at the 4e6-sample guard, at tied maxima of both deviations, and after every way a
 batch ends (another lane, a budget, a deadline, a cancel, a replan, a problem over the limits)."""
 import ctypes as C
-import os
-import sys
 
 import numpy as np
 import pytest
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from test_mpc_handover import DEV_GUARD, INIT_A, INIT_V, dev_ref, deviation_samples, message_ref, mpc_ref, scan_length  # noqa: E402
+from harness import cat, ctx, gpu  # noqa: F401
+from uneven_planner_b200 import _lib
+from workloads import DEV_GUARD, INIT_A, INIT_V, dev_ref, deviation_samples, message_ref, mpc_ref, scan_length
+
 
 pytestmark = pytest.mark.gpu
 dp = C.POINTER(C.c_double)
@@ -29,32 +29,11 @@ OUTS = ("pos_pts", "posT_pts", "angle_pts", "angleT_pts", "c_mpc_xy", "c_mpc_yaw
 
 
 @pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
-
-
-@pytest.fixture(scope="module")
 def orc(built):
     import pyoracle as po
     L = po.lib()
     L.orc_minco_generate.argtypes = [C.c_int, C.c_int, dp, dp, dp, dp, dp]
     return L
-
-
-def _ctx(gpu, mapdata, prec):
-    from uneven_planner_b200 import _lib
-    return gpu.BatchALMTrajOpt(precision=prec).init(_lib.default_params()).set_environment(mapdata)
-
-
-def _cat(pbs):
-    from uneven_planner_b200 import problems
-    out = problems.concat(pbs, [0] * len(pbs))
-    out.env = None
-    return out
 
 
 def _views(pb, ex, i):
@@ -101,7 +80,7 @@ def _export(gpu, opt, pb, out, orc, dt=0.01, init_v=None, init_a=None):
 def test_message_and_mpc_resolve_of_a_solved_batch(gpu, orc, bumps_map, prec):
     from uneven_planner_b200 import problems
     pb = problems.generate(bumps_map, 24, seed=12)
-    opt = _ctx(gpu, bumps_map, prec)
+    opt = ctx(gpu, prec, _lib.default_params(), bumps_map)
     out = opt.optimize(pb)
     ex = opt.mpc_export(pb.N, pb.M, dt=0.01)
     opt.close()
@@ -116,7 +95,7 @@ def test_message_and_mpc_resolve_of_a_solved_batch(gpu, orc, bumps_map, prec):
 
 def test_export_needs_a_solved_batch_and_skips_oversize_problems(gpu, bumps_map):
     from uneven_planner_b200 import _lib, problems
-    from test_gpu_boundary import _with_oversize
+    from workloads import _with_oversize
     params = _lib.default_params()
     pb = problems.generate(bumps_map, 6, seed=5)
     opt = gpu.BatchALMTrajOpt().init(params).set_environment(bumps_map)
@@ -137,11 +116,11 @@ def test_export_needs_a_solved_batch_and_skips_oversize_problems(gpu, bumps_map)
 def edge_batches(built, bumps_map):
     """the edge cases of test_gpu_tp_shapes (N1_M1, N1_M128, N64_M128, N40_M3, T < 1 s, yaw seam, off the map, ...) with one generated
     problem after them (B % 4 == 1: a partly filled last CTA), seven generated problems (B % 4 == 3) and one problem alone"""
-    from test_gpu_tp_shapes import case_batch
+    from workloads import case_batch
     from uneven_planner_b200 import problems
     gen = problems.generate(bumps_map, 8, seed=12)
     cases = case_batch()
-    return [_cat([cases, gen.select([0])]), gen.select(range(1, 8)), cases.select([cases.B - 1])]
+    return [cat([cases, gen.select([0])]), gen.select(range(1, 8)), cases.select([cases.B - 1])]
 
 
 @pytest.fixture(scope="module")
@@ -153,7 +132,7 @@ def solved_edges(gpu, edge_batches, bumps_map):
         if prec not in cache:
             runs = []
             for pb in edge_batches:
-                opt = _ctx(gpu, bumps_map, prec)
+                opt = ctx(gpu, prec, _lib.default_params(), bumps_map)
                 runs.append((pb, opt, opt.optimize(pb)))
             cache[prec] = runs
         return cache[prec]
@@ -263,7 +242,7 @@ def test_tied_maxima_keep_the_earliest_sample(gpu, orc, bumps_map, prec):
     from uneven_planner_b200 import problems
     pb = problems.generate(bumps_map, 16, seed=1)
     pb.bnd[:, [2, 3, 4, 5, 8, 9, 10, 11, 13, 14, 16, 17]] = 0.0
-    opt = _ctx(gpu, bumps_map, prec)
+    opt = ctx(gpu, prec, _lib.default_params(), bumps_map)
     out = opt.optimize(pb)
     seen = set()
     for dt in (0.01, 0.005):
@@ -285,7 +264,7 @@ def small(built, bumps_map):
 def test_export_reads_the_selected_lane(gpu, orc, bumps_map, small, prec):
     """two tickets on lanes 0 and 1: each lane exports its own batch"""
     a, b = small.select(range(0, 13)), small.select(range(13, 40))
-    opt = _ctx(gpu, bumps_map, prec)
+    opt = ctx(gpu, prec, _lib.default_params(), bumps_map)
     ta, tb = opt.submit(a, depth=2), opt.submit(b, depth=2)
     assert (ta, tb) == (0, 1)
     oa, ob = opt.wait(ta), opt.wait(tb)
@@ -299,7 +278,7 @@ def test_export_reads_the_selected_lane(gpu, orc, bumps_map, small, prec):
 @pytest.mark.parametrize("prec", PRECISIONS)
 def test_export_after_a_budget(gpu, orc, bumps_map, small, prec):
     from uneven_planner_b200 import _lib
-    opt = _ctx(gpu, bumps_map, prec).set_budget(3)
+    opt = ctx(gpu, prec, _lib.default_params(), bumps_map).set_budget(3)
     out = opt.optimize(small)
     assert sum(r.ret_code == _lib.UALM_RET_STOPPED for r in out[0]) > small.B // 2
     _export(gpu, opt, small, out, orc, init_v=INIT_V, init_a=INIT_A)
@@ -309,7 +288,7 @@ def test_export_after_a_budget(gpu, orc, bumps_map, small, prec):
 @pytest.mark.parametrize("prec", PRECISIONS)
 def test_export_after_a_deadline_and_a_cancel(gpu, orc, bumps_map, small, prec):
     from uneven_planner_b200 import _lib
-    opt = _ctx(gpu, bumps_map, prec)
+    opt = ctx(gpu, prec, _lib.default_params(), bumps_map)
     out = opt.wait(opt.submit(small, depth=1), timeout_ms=0)
     assert any(r.ret_code == _lib.UALM_RET_STOPPED for r in out[0])
     _export(gpu, opt, small, out, orc, dt=0.0137)
@@ -325,7 +304,7 @@ def test_export_after_a_deadline_and_a_cancel(gpu, orc, bumps_map, small, prec):
 def test_export_of_a_replan(gpu, orc, bumps_map, small, prec):
     """a replan ticket, exported on its lane with the robot's state at the replan time as the message's boundary derivatives"""
     pb = small.select(range(8))
-    opt = _ctx(gpu, bumps_map, prec)
+    opt = ctx(gpu, prec, _lib.default_params(), bumps_map)
     out = opt.optimize(pb)
     t, new = opt.submit_replan(pb, out, [0, 3, 5], 0.5)
     got = opt.wait(t)
@@ -339,10 +318,10 @@ def test_export_of_a_replan(gpu, orc, bumps_map, small, prec):
 
 @pytest.mark.parametrize("prec", [65, 32])
 def test_throughput_export_skips_a_problem_over_the_limits(gpu, orc, bumps_map, small, prec):
-    from test_gpu_boundary import _with_oversize
+    from workloads import _with_oversize
     from uneven_planner_b200 import _lib
     pbx = _with_oversize(small.select(range(6)), 2)
-    opt = _ctx(gpu, bumps_map, prec)
+    opt = ctx(gpu, prec, _lib.default_params(), bumps_map)
     out = opt.optimize(pbx)
     assert out[0][2].ret_code == _lib.UALM_ELIMIT
     ex = opt.mpc_export(pbx.N, pbx.M, init_v=INIT_V, init_a=INIT_A)
@@ -370,7 +349,7 @@ def test_throughput_export_needs_a_collected_batch(gpu, bumps_map, small, prec):
     """on the throughput path a batch solved but not yet synchronised is refused (UALM_ESTATE), then exported once collected"""
     from uneven_planner_b200 import _lib
     pb = small.select(range(5))
-    opt = _ctx(gpu, bumps_map, prec)
+    opt = ctx(gpu, prec, _lib.default_params(), bumps_map)
     opt.upload(pb)
     opt.solve_resident()
     sN, sM = int(pb.N.sum()), int(pb.M.sum())

@@ -10,19 +10,13 @@ import os
 import numpy as np
 import pytest
 
+from harness import gpu  # noqa: F401
+from workloads import _assert_solve_parity
+
+
 pytestmark = pytest.mark.gpu
 
-REL_TOL = 0.0          # bitwise; the north-star bound is 1e-5
 NORTH_STAR_TOL = 1e-5
-
-
-@pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
 
 
 def _offsets(pb, K):
@@ -32,13 +26,6 @@ def _offsets(pb, K):
     return offx, offs, ocx, ocy
 
 
-def _rel(a, b):
-    a = np.asarray(a, dtype=np.float64); b = np.asarray(b, dtype=np.float64)
-    if a.size == 0:
-        return 0.0
-    return float(np.linalg.norm(a - b) / max(np.linalg.norm(b), 1e-300))
-
-
 def _solve_both(gpu, mapdata, pb, params):
     import pyoracle as po
     opt = gpu.BatchALMTrajOpt().init(params).set_environment(mapdata)
@@ -46,18 +33,6 @@ def _solve_both(gpu, mapdata, pb, params):
     ores = po.solve_batch(po.params_from(params), po.OracleMap(mapdata), pb, threads=min(32, os.cpu_count()))
     opt.close()
     return res, cxy, cyaw, ores
-
-
-def _assert_solve_parity(pb, res, cxy, cyaw, ores):
-    _, _, ocx, ocy = pb.offsets()
-    for i in range(pb.B):
-        r, ocxy, ocyaw, _ = ores[i]
-        g = res[i]
-        assert (g.ret_code, g.outer_iters, g.n_evals, g.n_lbfgs_iters, g.last_lbfgs_ret) == \
-               (r.ret_code, r.outer_iters, r.n_evals, r.n_lbfgs_iters, r.last_lbfgs_ret), i
-        assert abs(g.inner_cost - r.inner_cost) <= REL_TOL * abs(r.inner_cost), i
-        assert _rel(cxy[ocx[i]:ocx[i + 1]], ocxy) <= REL_TOL and _rel(cyaw[ocy[i]:ocy[i + 1]], ocyaw) <= REL_TOL, i
-        assert g.res_h == r.res_h and g.res_g == r.res_g and g.total_T == r.total_T and g.jerk_cost == r.jerk_cost
 
 
 # ------------------------------------------------------------------ kernel-level: one innerCallback evaluation
@@ -153,7 +128,7 @@ def test_cuda_matches_reference_build_directly(gpu, bumps_map):
     import ctypes as C
     import contextlib
     from uneven_planner_b200 import _lib, problems
-    from test_ref_pin import REF, _ref_solve
+    from workloads import REF, _ref_solve
     if not os.path.exists(REF):
         pytest.skip("oracle/_ref/libref.so not present (built where /root/reference exists; travels with the snapshot)")
     L = C.CDLL(REF)

@@ -18,19 +18,17 @@ and at its largest shared-memory layouts:
 
 test_case_table_reaches_the_edges (no GPU) restates make_layout and fails if the case table stops reaching any of it, and pins the
 largest int_K whose N = 64, M = 128 layout fits four slots to a CTA."""
-import contextlib
 import functools
 import os
 import re
-import sys
 
 import numpy as np
 import pytest
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import test_solver_control as sc  # noqa: E402
-from test_gpu_minco_fused import _arc_problem  # noqa: E402
-from test_gpu_tp_shapes import CASES as TP_CASES, RHO, _inputs, _oracle, _per_problem  # noqa: E402
+import workloads
+from harness import cat, environ, gpu, same_values, solve_diff, split  # noqa: F401
+from workloads import RHO, SHAPES, TP_CASES, _arc_problem, _inputs, _oracle, _per_problem, _shape
+
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 CSRC = os.path.join(ROOT, "uneven_planner_b200", "csrc")
@@ -40,8 +38,6 @@ PASTS = (0, 16)
 SMEM_OPTIN = 227 * 1024        # shared memory one CTA may use on an H100 (cudaDevAttrMaxSharedMemoryPerBlockOptin)
 RESERVED_SMEM = 1024           # shared memory the device reserves per CTA on sm_80 and later
 PARITY_KERNELS = ("solve_kernel", "eval_kernel", "scaling_kernel", "penalty_only_kernel")
-SHAPES = {"N64_M128": (64, 128), "N63_M127": (63, 127), "N48_M128": (48, 128), "N64_M64": (64, 64), "N64_M1": (64, 1),
-          "N1_M128": (1, 128), "N2_M1": (2, 1), "N1_M1": (1, 1)}
 MAP_EDGES = ("border_cells", "off_map", "yaw_seam", "short_path")
 
 
@@ -109,17 +105,9 @@ def _long(mapdata, B, seed):
     return problems.generate(mapdata, B, seed=seed, min_dist=9.0, n_max=64)
 
 
-def _cat(pbs, envs=None):
-    from uneven_planner_b200 import problems
-    out = problems.concat(pbs, envs or [0] * len(pbs))
-    if envs is None:
-        out.env = None
-    return out
-
-
 def case_batch(mapdata):
     """the shapes, the map-edge cases and three long generated problems, once each (at their initial guesses)"""
-    return _cat([_arc_problem(N, M, arc=0.5 * np.pi if N == 1 else 1.5 * np.pi) for N, M in SHAPES.values()] +
+    return cat([_arc_problem(N, M, arc=0.5 * np.pi if N == 1 else 1.5 * np.pi) for N, M in SHAPES.values()] +
                 [TP_CASES[k]() for k in MAP_EDGES] + [_long(mapdata, 3, seed=17)])
 
 
@@ -133,33 +121,9 @@ def _params(K=None, past=None):
     return p
 
 
-def _shape(N, M):
-    return _arc_problem(N, M, arc=0.5 * np.pi if N == 1 else 1.5 * np.pi)
-
-
 # ------------------------------------------------------------------ running the path
-@contextlib.contextmanager
-def _environ(env):
-    old = {k: os.environ.get(k) for k in env}
-    os.environ.update(env)
-    try:
-        yield
-    finally:
-        for k, v in old.items():
-            if v is None:
-                os.environ.pop(k)
-            else:
-                os.environ[k] = v
-
-
 # the group sizes: UALM_GROUPS is read at ualm_create, UALM_F4 / UALM_F2 at upload, so each covers both
 MODES = {"four_warps": {}, "two_warps": {"UALM_F4": "0", "UALM_F2": "1"}, "one_warp": {"UALM_GROUPS": "0"}}
-
-
-def _split(pb, out):
-    res, cxy, cyaw = out
-    _, _, ocx, ocy = pb.offsets()
-    return [(res[i], cxy[ocx[i]:ocx[i + 1]], cyaw[ocy[i]:ocy[i + 1]]) for i in range(pb.B)]
 
 
 def _solve(gpu, params, mapdata, pb, budget=0, mode="four_warps", prec=64, feas=False):
@@ -167,7 +131,7 @@ def _solve(gpu, params, mapdata, pb, budget=0, mode="four_warps", prec=64, feas=
     also the post-solve scan and ualm_check_trajectories of the solved batch"""
     ps = params if isinstance(params, list) else [params]
     ms = mapdata if isinstance(mapdata, list) else [mapdata]
-    with _environ(MODES[mode]):
+    with environ(MODES[mode]):
         opt = gpu.BatchALMTrajOpt(precision=prec)
         try:
             for e in range(len(ps)):
@@ -177,25 +141,13 @@ def _solve(gpu, params, mapdata, pb, budget=0, mode="four_warps", prec=64, feas=
             extra = (opt.feasibility(0.01), opt.check_results(pb, out)) if feas else None
         finally:
             opt.close()
-    return (_split(pb, out), extra) if feas else _split(pb, out)
+    return (split(pb, out), extra) if feas else split(pb, out)
 
 
 def _same_bits(a, b):
     """equal entry by entry, as the rest of the suite compares the parity path with the oracle (0.0 == -0.0; NaN == NaN)"""
     a, b = np.atleast_1d(np.asarray(a, np.float64)), np.atleast_1d(np.asarray(b, np.float64))
     return a.shape == b.shape and np.array_equal(a, b, equal_nan=True)
-
-
-def _bitwise(got, want, what):
-    g, gx, gy = got
-    w, wx, wy = want
-    assert all(getattr(g, f) == getattr(w, f) or (getattr(g, f) != getattr(g, f) and getattr(w, f) != getattr(w, f)) for f in sc.RECORD), \
-        (what, [(f, getattr(g, f), getattr(w, f)) for f in sc.RECORD if getattr(g, f) != getattr(w, f)])
-    assert _same_bits(gx, wx) and _same_bits(gy, wy), what
-
-
-def _same_bytes(a, b):
-    return bytes(a[0]) == bytes(b[0]) and _same_bits(a[1], b[1]) and _same_bits(a[2], b[2])
 
 
 def _fit_mask(pb, K, past):
@@ -208,7 +160,7 @@ def _every_group_size(gpu, params, mapdata, pb, budget, what):
     base = _solve(gpu, params, mapdata, pb, budget)
     two = _solve(gpu, params, mapdata, pb, budget, "two_warps")
     for i in range(pb.B):
-        assert _same_bytes(two[i], base[i]), (what, "two_warps", i)
+        assert same_values(two[i], base[i], equal_nan=True), (what, "two_warps", i)
     fit = _fit_mask(pb, params.int_K, params.past)
     if not fit.all():
         with pytest.raises(gpu.UalmError, match="error -4: UALM_GROUPS=0"):
@@ -217,7 +169,7 @@ def _every_group_size(gpu, params, mapdata, pb, budget, what):
     if idx.size:
         one = _solve(gpu, params, mapdata, pb.select(idx), budget, "one_warp")
         for j, i in enumerate(idx):
-            assert _same_bytes(one[j], base[i]), (what, "one_warp", int(i))
+            assert same_values(one[j], base[i], equal_nan=True), (what, "one_warp", int(i))
     return base
 
 
@@ -233,15 +185,6 @@ def _feasibility_against_oracle(pb, params, mapdata, out, feas, chk, what):
 
 
 # ------------------------------------------------------------------ fixtures
-@pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
-
-
 @pytest.fixture(scope="module")
 def cases(bumps_map):
     return case_batch(bumps_map)
@@ -279,10 +222,10 @@ def test_budgeted_solves_bitwise_in_every_group_size(gpu, cases, bumps_map, K):
     the 30-evaluation solves against the oracle's"""
     p = _params(K)
     for k in BUDGETS:
-        want = sc.oracle(p, bumps_map, cases, k)
+        want = workloads.oracle(p, bumps_map, cases, k)
         got = _every_group_size(gpu, p, bumps_map, cases, k, (K, k))
         for i in range(cases.B):
-            _bitwise(got[i], want[i], (K, k, i))
+            assert not solve_diff(got[i], want[i], equal_nan=True), ((K, k, i), solve_diff(got[i], want[i], equal_nan=True))
     out, (feas, chk) = _solve(gpu, p, bumps_map, cases, 30, feas=True)
     _feasibility_against_oracle(cases, p, bumps_map, out, feas, chk, K)
 
@@ -292,10 +235,10 @@ def test_budgeted_solves_bitwise_in_every_group_size(gpu, cases, bumps_map, K):
 def test_unbudgeted_solves_bitwise(gpu, cases, bumps_map, K):
     """the oracle's own solve of every case, past the four-slot boundary and at the largest int_K"""
     p = _params(K)
-    want = sc.oracle(p, bumps_map, cases)
+    want = workloads.oracle(p, bumps_map, cases)
     out, (feas, chk) = _solve(gpu, p, bumps_map, cases, feas=True)
     for i in range(cases.B):
-        _bitwise(out[i], want[i], (K, i))
+        assert not solve_diff(out[i], want[i], equal_nan=True), ((K, i), solve_diff(out[i], want[i], equal_nan=True))
     _feasibility_against_oracle(cases, p, bumps_map, out, feas, chk, K)
 
 
@@ -309,9 +252,9 @@ def test_largest_problem_on_both_sides_of_four_slots(gpu, bumps_map, past):
     pb = _shape(64, 128)
     for K in (k0, k0 + 1, 128):
         p = _params(K, past)
-        want = sc.oracle(p, bumps_map, pb, 30)
+        want = workloads.oracle(p, bumps_map, pb, 30)
         got = _every_group_size(gpu, p, bumps_map, pb, 30, (past, K))
-        _bitwise(got[0], want[0], (past, K))
+        assert not solve_diff(got[0], want[0], equal_nan=True), ((past, K), solve_diff(got[0], want[0], equal_nan=True))
         inputs = _inputs(pb, [K], seed=past + K)
         w = _oracle(pb, [p], [bumps_map], [K], inputs)[0]
         opt = gpu.BatchALMTrajOpt(precision=64).init(p).set_environment(bumps_map)
@@ -331,12 +274,12 @@ def test_pair_over_only_as_maxima(gpu, bumps_map, past):
     """N = 64, M = 1 and N = 1, M = 128 at int_K = 128: each fits four slots to a CTA, their maxima do not; as single warps they
     are two launches"""
     p = _params(128, past)
-    pb = _cat([_shape(64, 1), _shape(1, 128)])
+    pb = cat([_shape(64, 1), _shape(1, 128)])
     assert _fit_mask(pb, 128, past).all() and not fits_four([(64, 1), (1, 128)], 128, past)
-    want = sc.oracle(p, bumps_map, pb, 30)
+    want = workloads.oracle(p, bumps_map, pb, 30)
     got = _every_group_size(gpu, p, bumps_map, pb, 30, past)
     for i in range(pb.B):
-        _bitwise(got[i], want[i], (past, i))
+        assert not solve_diff(got[i], want[i], equal_nan=True), ((past, i), solve_diff(got[i], want[i], equal_nan=True))
 
 
 @pytest.mark.gpu
@@ -346,21 +289,22 @@ def test_one_large_problem_among_ordinary_ones(gpu, hill_map, past):
     for bit the oracle's, the 31 byte for byte as without it, in every group size"""
     K = largest_fitting_K(64, 128, past) + 1
     p = _params(K, past)
-    ordinary = sc.bench_problems(hill_map, 31)
-    pb = _cat([ordinary.select(range(0, 13)), _shape(64, 128), ordinary.select(range(13, 31))])
+    ordinary = workloads.bench_problems(hill_map, 31)
+    pb = cat([ordinary.select(range(0, 13)), _shape(64, 128), ordinary.select(range(13, 31))])
     at = 13
     rest = [i for i in range(pb.B) if i != at]
     alone = _solve(gpu, p, hill_map, ordinary, 30)
     got = _every_group_size(gpu, p, hill_map, pb, 30, past)
     assert all(r.ret_code in (0, 1, 2, 3) and r.n_evals > 0 for r, _, _ in got), [r.ret_code for r, _, _ in got]
     for j, i in enumerate(rest):
-        assert _same_bytes(got[i], alone[j]), (past, i)
-    _bitwise(got[at], sc.oracle(p, hill_map, pb.select([at]), 30)[0], (past, "large"))
+        assert same_values(got[i], alone[j], equal_nan=True), (past, i)
+    want = workloads.oracle(p, hill_map, pb.select([at]), 30)[0]
+    assert not solve_diff(got[at], want, equal_nan=True), ((past, "large"), solve_diff(got[at], want, equal_nan=True))
     # unbudgeted: the large problem still does not hold the others back
     full = _solve(gpu, p, hill_map, pb)
     full_alone = _solve(gpu, p, hill_map, ordinary)
     for j, i in enumerate(rest):
-        assert _same_bytes(full[i], full_alone[j]), (past, "unbudgeted", i)
+        assert same_values(full[i], full_alone[j], equal_nan=True), (past, "unbudgeted", i)
 
 
 @pytest.mark.gpu
@@ -369,20 +313,20 @@ def test_two_environments_in_one_batch(gpu, bumps_map, hill_map):
     one interleaved batch: each problem bit for bit the oracle's with its own environment, and byte for byte each environment alone"""
     ps = [_params(128), _params()]
     ms = [bumps_map, hill_map]
-    pbs = [_cat([_shape(64, 128), _shape(63, 127), _long(bumps_map, 2, seed=5)]),
-           _cat([_shape(64, 128), _long(hill_map, 3, seed=9)])]
-    mixed = _cat(pbs, [0, 1])
+    pbs = [cat([_shape(64, 128), _shape(63, 127), _long(bumps_map, 2, seed=5)]),
+           cat([_shape(64, 128), _long(hill_map, 3, seed=9)])]
+    mixed = cat(pbs, [0, 1])
     order = np.array([0, 4, 1, 5, 2, 6, 3, 7])
     mixed = mixed.select(order)
     for mode in ("four_warps", "two_warps"):
         got = _solve(gpu, ps, ms, mixed, 30, mode)
         for e in range(2):
             alone = _solve(gpu, ps[e], ms[e], pbs[e], 30, mode)
-            want = sc.oracle(ps[e], ms[e], pbs[e], 30)
+            want = workloads.oracle(ps[e], ms[e], pbs[e], 30)
             for j in range(pbs[e].B):
                 i = int(np.nonzero(order == 4 * e + j)[0][0])
-                assert _same_bytes(got[i], alone[j]), (mode, e, j)
-                _bitwise(alone[j], want[j], (mode, e, j))
+                assert same_values(got[i], alone[j], equal_nan=True), (mode, e, j)
+                assert not solve_diff(alone[j], want[j], equal_nan=True), ((mode, e, j), solve_diff(alone[j], want[j], equal_nan=True))
 
 
 # ------------------------------------------------------------------ the throughput path at int_K = 127
@@ -390,12 +334,12 @@ def test_two_environments_in_one_batch(gpu, bumps_map, hill_map):
 def test_throughput_solves_at_int_K_127(gpu, cases, bumps_map):
     """precision 65, budget 30: every decided trajectory within test_solver_control's rule"""
     p = _params(127)
-    ref, mask = sc.decided(p, bumps_map, cases, 65, 30)
+    ref, mask = workloads.decided(p, bumps_map, cases, 65, 30)
     got = _solve(gpu, p, bumps_map, cases, 30, prec=65)
     n = 0
     for i in np.nonzero(mask)[0]:
-        same, err = sc.trajectory_error(got[i], ref[i])
-        assert same and err <= sc.TOLC[65], (int(i), err)
+        same, err = workloads.trajectory_error(got[i], ref[i])
+        assert same and err <= workloads.TOLC[65], (int(i), err)
         n += 1
     print("precision 65, int_K 127, budget 30: %d of %d trajectories decided" % (n, cases.B))
     assert n >= cases.B // 2, n

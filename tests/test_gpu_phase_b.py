@@ -6,16 +6,10 @@ import os
 import numpy as np
 import pytest
 
+from harness import gpu  # noqa: F401
+
+
 pytestmark = pytest.mark.gpu
-
-
-@pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
 
 
 def _params(use_scaling=1, int_K=None):

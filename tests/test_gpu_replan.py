@@ -10,46 +10,24 @@ import subprocess
 import numpy as np
 import pytest
 
+from harness import bits, box_cells, build_driver, ctx, gpu, pending, pieces, same_pieces, splice  # noqa: F401
+from workloads import hill_desert_world
+
+
 pytestmark = pytest.mark.gpu
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PRECISIONS = [64, 32, 65]
 BOX = (60, 80, 40, 40)                # a 2 m x 2 m window of the 10 m grid, where the hill problems run
 DT = 0.01
 
 
 @pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
-
-
-@pytest.fixture(scope="module")
 def world(gpu, golden):
-    from uneven_planner_b200 import configs, maps, problems
-    g0, g1 = maps.stand_in_terrain("hill"), maps.stand_in_terrain("desert")
-    kw = configs.gen_kwargs("hill")
-    gold = golden("hill", g0)
-    gold_pb = problems.generate(g0, int(gold["B"]), seed=int(gold["seed"]), **kw)
-    bench = problems.generate(g0, 1024, seed=0, **kw)
-    params = configs.params_for("hill")
-    opt = gpu.BatchALMTrajOpt().init(params).set_environment(g0)
-    held = opt.optimize(gold_pb)                   # the trajectories the caller holds: the golden problems solved on the parity path
-    b = problems.generate(g0, 256, seed=7, **kw)
-    held_b = opt.optimize(b)
+    w = hill_desert_world(golden)
+    opt = gpu.BatchALMTrajOpt().init(w["params"]).set_environment(w["g0"])
+    w["held"] = opt.optimize(w["gold_pb"])         # the trajectories the caller holds: the golden problems solved on the parity path
+    w["held_b"] = opt.optimize(w["b"])
     opt.close()
-    return dict(g0=g0, g1=g1, params=params, gold=gold, gold_pb=gold_pb, bench=bench, held=held, b=b, held_b=held_b,
-                a64=problems.concat([gold_pb, bench], [0, 0]))
-
-
-def _ctx(gpu, world, precision, grid):
-    return gpu.BatchALMTrajOpt(precision=precision).init(world["params"]).set_environment(grid)
-
-
-def _bits(a):
-    return np.ascontiguousarray(a, np.float64).view(np.uint64)
+    return w
 
 
 def _total(N, M, Tx, Ty):
@@ -95,36 +73,9 @@ def _t_from(pb, out, kind, dt=DT):
 
 
 def _same_pb(a, b):
-    return (np.array_equal(a.N, b.N) and np.array_equal(a.M, b.M) and np.array_equal(_bits(a.bnd), _bits(b.bnd)) and
-            np.array_equal(_bits(a.total_time), _bits(b.total_time)) and np.array_equal(_bits(a.inner_xy), _bits(b.inner_xy)) and
-            np.array_equal(_bits(a.inner_yaw), _bits(b.inner_yaw)))
-
-
-def _pieces(pb, out):
-    res, cxy, cyaw = out
-    _, _, ocx, ocy = pb.offsets()
-    return [(bytes(res[i]), cxy[ocx[i]:ocx[i + 1]].copy(), cyaw[ocy[i]:ocy[i + 1]].copy()) for i in range(pb.B)]
-
-
-def _same(a, b):
-    return len(a) == len(b) and all(x[0] == y[0] and np.array_equal(x[1], y[1]) and np.array_equal(x[2], y[2]) for x, y in zip(a, b))
-
-
-def _pending(opt, t, pb):
-    return opt.poll(t, opt.outputs(pb), 0.0)[1]
-
-
-def _box(cells, box):
-    ix0, iy0, nx, ny = box
-    return cells[ix0:ix0 + nx, iy0:iy0 + ny]
-
-
-def _splice(base, cells, box, name="spliced"):
-    from uneven_planner_b200 import maps
-    out = base.cells.copy()
-    ix0, iy0, nx, ny = box
-    out[ix0:ix0 + nx, iy0:iy0 + ny] = cells
-    return maps.UnevenMapData(base.geom, out, name)
+    return (np.array_equal(a.N, b.N) and np.array_equal(a.M, b.M) and np.array_equal(bits(a.bnd), bits(b.bnd)) and
+            np.array_equal(bits(a.total_time), bits(b.total_time)) and np.array_equal(bits(a.inner_xy), bits(b.inner_xy)) and
+            np.array_equal(bits(a.inner_yaw), bits(b.inner_yaw)))
 
 
 def _rp(vals):
@@ -141,16 +92,16 @@ def test_built_problems_are_the_reference(gpu, world, precision):
     import replan_oracle as ro
     pb, out = world["gold_pb"], world["held"]
     rows = np.arange(pb.B)
-    opt = _ctx(gpu, world, precision, world["g0"])
+    opt = ctx(gpu, precision, world["params"], world["g0"])
     for dt, rp in ((DT, None), (0.023, None), (DT, (0.21, 3.0, 0.7, 1.4))):
         for kind in range(5):
             tf = _t_from(pb, out, kind, dt)
             t, new = opt.submit_replan(pb, out, rows, tf, dt=dt, rparams=_rp(rp))
-            got = _pieces(new, opt.wait(t))
+            got = pieces(new, opt.wait(t))
             ref = ro.problems_of(ro.rows(pb, out, rows, tf, dt, rp or ro.DEFAULT_RP))
             assert _same_pb(new, ref), (dt, rp, kind)
             if kind == 0 and rp is None and dt == DT:
-                assert _same(got, _pieces(new, opt.wait(opt.submit(new))))
+                assert same_pieces(got, pieces(new, opt.wait(opt.submit(new))))
     opt.close()
 
 
@@ -168,13 +119,13 @@ def test_padded_outputs_of_the_c_call(gpu, world):
     bnd = np.ascontiguousarray(pb.bnd, np.float64)
     No, Mo, bo, To = np.zeros(B, np.int32), np.zeros(B, np.int32), np.zeros((B, 18)), np.zeros(B)
     ixy, iyaw = np.full((B, 126), 7.0), np.full((B, 127), 7.0)
-    opt = _ctx(gpu, world, 64, world["g0"])
+    opt = ctx(gpu, 64, world["params"], world["g0"])
     t = C.c_int(-1)
     assert _lib.lib().ualm_submit_replan(opt.h, B, P(N, ip), P(M, ip), P(pt), P(cxy), P(cyaw), P(bnd), None, P(tf), DT, None, 2, C.byref(t),
                                           P(No, ip), P(Mo, ip), P(bo), P(To), P(ixy), P(iyaw)) == 0
     ref = ro.rows(pb, world["held"], np.arange(B), tf)
-    assert np.array_equal(_bits(ixy), _bits(ref[:, 21:147])) and np.array_equal(_bits(iyaw), _bits(ref[:, 147:]))
-    assert np.array_equal(No, ref[:, 19]) and np.array_equal(Mo, ref[:, 20]) and np.array_equal(_bits(bo), _bits(ref[:, :18]))
+    assert np.array_equal(bits(ixy), bits(ref[:, 21:147])) and np.array_equal(bits(iyaw), bits(ref[:, 147:]))
+    assert np.array_equal(No, ref[:, 19]) and np.array_equal(Mo, ref[:, 20]) and np.array_equal(bits(bo), bits(ref[:, :18]))
     opt._tickets = {t.value: (ro.problems_of(ref), None)}
     opt.wait(t.value)
     opt.close()
@@ -196,17 +147,17 @@ def test_mixed_environments(gpu, world):
     rows = np.arange(1, mixed.B, 3)        # every environment: the batch interleaves them
     tf = _t_from(mixed, out, 1)[rows]
     t, new = opt.submit_replan(mixed, out, rows, tf)
-    got = _pieces(new, opt.wait(t))
+    got = pieces(new, opt.wait(t))
     assert np.array_equal(new.env, mixed.env[rows]) and len(set(new.env.tolist())) == 4
     assert _same_pb(new, ro.problems_of(ro.rows(mixed, out, rows, tf), new.env))
-    assert _same(got, _pieces(new, opt.wait(opt.submit(new))))
+    assert same_pieces(got, pieces(new, opt.wait(opt.submit(new))))
     opt.close()
     for e in range(4):                               # each environment's rows alone on a context of that environment only
         k = np.nonzero(new.env == e)[0]
         one = new.select(k)
         one.env = None
         o = gpu.BatchALMTrajOpt().init(params[e]).set_environment(grids[e])
-        assert _same([got[i] for i in k], _pieces(one, o.optimize(one)))
+        assert same_pieces([got[i] for i in k], pieces(one, o.optimize(one)))
         o.close()
 
 
@@ -219,20 +170,20 @@ def test_rows_over_the_limits(gpu, world, precision):
     last = np.array([_seq(_total(int(pb.N[i]), int(pb.M[i]), out[0][i].piece_T_xy, out[0][i].piece_T_yaw), DT)[-1] for i in range(pb.B)])
     tf = np.where(np.arange(pb.B) % 2 == 0, 0.0, last)
     rp = (0.05, 2.0, 0.5, 1.2)
-    opt = _ctx(gpu, world, precision, world["g0"])
+    opt = ctx(gpu, precision, world["params"], world["g0"])
     t, new = opt.submit_replan(pb, out, np.arange(pb.B), tf, rparams=_rp(rp))
     over = (new.N > 64) | (new.M > 128)
     assert over.any() and not over.all()
     buf = opt.outputs(new)
     idx, _ = opt.poll(t, buf, 0.0)
     assert set(np.nonzero(over)[0].tolist()) <= set(idx.tolist())
-    got = _pieces(new, opt.wait(t))
+    got = pieces(new, opt.wait(t))
     _, _, ocx, ocy = new.offsets()
     for i in np.nonzero(over)[0]:
         assert buf[0][i].ret_code == _lib.UALM_ELIMIT and not buf[1][ocx[i]:ocx[i + 1]].any() and not buf[2][ocy[i]:ocy[i + 1]].any()
     fit = np.nonzero(~over)[0]
     sub = new.select(fit)
-    assert _same([got[i] for i in fit], _pieces(sub, opt.wait(opt.submit(sub))))
+    assert same_pieces([got[i] for i in fit], pieces(sub, opt.wait(opt.submit(sub))))
     opt.close()
 
 
@@ -248,7 +199,7 @@ def test_the_ticket_is_any_ticket(gpu, world, precision):
     pb, out = world["b"], world["held_b"]
     rows = np.arange(0, 256, 2)
     tf = _t_from(pb, out, 3)[rows]
-    opt = _ctx(gpu, world, precision, world["g0"])
+    opt = ctx(gpu, precision, world["params"], world["g0"])
     t, new = opt.submit_replan(pb, out, rows, tf)
     buf = opt.outputs(new)
     seen = set()
@@ -257,22 +208,22 @@ def test_the_ticket_is_any_ticket(gpu, world, precision):
         seen |= set(idx.tolist())
         if left == 0:
             break
-    waited = _pieces(new, opt.wait(t))
-    assert seen == set(range(new.B)) and _same(_pieces(new, buf), waited)
-    lone = _pieces(new, opt.wait(opt.submit(new)))
-    assert _same(waited, lone)
+    waited = pieces(new, opt.wait(t))
+    assert seen == set(range(new.B)) and same_pieces(pieces(new, buf), waited)
+    lone = pieces(new, opt.wait(opt.submit(new)))
+    assert same_pieces(waited, lone)
     t2, new2 = opt.submit_replan(pb, out, rows, tf)
-    assert _same(_pieces(new2, opt.wait(t2, timeout_ms=600000.0)), lone)
+    assert same_pieces(pieces(new2, opt.wait(t2, timeout_ms=600000.0)), lone)
     t3, _ = opt.submit_replan(pb, out, rows, tf)
     stop = np.arange(5, new.B, 3)
     opt.cancel(t3, stop)
-    got = _pieces(new, opt.wait(t3))
+    got = pieces(new, opt.wait(t3))
     opt.close()
     codes = [int(np.frombuffer(g[0], np.int32, count=1)[0]) for g in got]
     assert sum(codes[i] == _lib.UALM_RET_STOPPED for i in stop) >= len(stop) // 2
     assert all(codes[i] == _lib.UALM_RET_STOPPED or got[i][0] == lone[i][0] for i in stop)
     keep = np.setdiff1d(np.arange(new.B), stop)
-    assert _same([got[i] for i in keep], [lone[i] for i in keep])
+    assert same_pieces([got[i] for i in keep], [lone[i] for i in keep])
     if precision == 64:
         ref = ro.problems_of(ro.rows(pb, out, rows, tf))
         sel = np.arange(64)
@@ -296,22 +247,22 @@ def test_replan_while_a_batch_is_in_flight(gpu, world, precision):
     pb, out = world["b"], world["held_b"]
     rows = np.arange(256)
     tf = _t_from(pb, out, 2)
-    opt = _ctx(gpu, world, precision, world["g0"])
+    opt = ctx(gpu, precision, world["params"], world["g0"])
     t0, _ = opt.submit_replan(pb, out, rows, tf, depth=3)
     idle = opt.wait(t0)
     ta = opt.submit(A, depth=3)
-    assert _pending(opt, ta, A) > 0
+    assert pending(opt, ta, A) > 0
     tr, new = opt.submit_replan(pb, out, rows, tf, depth=3)
     if precision != 64:
-        assert _pending(opt, ta, A) > 0
-    got_r = _pieces(new, opt.wait(tr))
-    got_a = _pieces(A, opt.wait(ta))
+        assert pending(opt, ta, A) > 0
+    got_r = pieces(new, opt.wait(tr))
+    got_a = pieces(A, opt.wait(ta))
     opt.close()
-    assert _same(got_r, _pieces(new, idle))
-    o = _ctx(gpu, world, precision, world["g0"])
-    ref_a = _pieces(A, o.optimize(A))
+    assert same_pieces(got_r, pieces(new, idle))
+    o = ctx(gpu, precision, world["params"], world["g0"])
+    ref_a = pieces(A, o.optimize(A))
     o.close()
-    assert _same(got_a, ref_a)
+    assert same_pieces(got_a, ref_a)
     if precision == 64:
         g, n = world["gold"], world["gold_pb"].B
         assert [int(np.frombuffer(p[0], dtype=np.int32, count=1)[0]) for p in got_a[:n]] == [int(x) for x in g["ret_code"]]
@@ -325,19 +276,19 @@ def test_replan_after_a_window_update(gpu, world, precision):
     bound to the grid spliced in numpy"""
     g0, g1 = world["g0"], world["g1"]
     pb, out = world["b"], world["held_b"]
-    win = _box(g1.cells, BOX)
-    spliced = _splice(g0, win, BOX)
-    opt = _ctx(gpu, world, precision, g0)
+    win = box_cells(g1.cells, BOX)
+    spliced = splice(g0, win, BOX)
+    opt = ctx(gpu, precision, world["params"], g0)
     t0 = opt.submit(pb, depth=2)
     opt.update_environment_window(BOX[0], BOX[1], win)
     t, new = opt.submit_replan(pb, out, np.arange(pb.B), _t_from(pb, out, 0), depth=2)
-    got = _pieces(new, opt.wait(t))
+    got = pieces(new, opt.wait(t))
     opt.wait(t0)
     opt.close()
-    fresh = _ctx(gpu, world, precision, spliced)
-    ref = _pieces(new, fresh.optimize(new))
+    fresh = ctx(gpu, precision, world["params"], spliced)
+    ref = pieces(new, fresh.optimize(new))
     fresh.close()
-    assert _same(got, ref)
+    assert same_pieces(got, ref)
 
 
 # ---- refusals, memory, C++ ----------------------------------------------------------------------
@@ -348,9 +299,9 @@ def test_refused_replans_write_nothing_and_take_no_lane(gpu, world, precision):
     L = _lib.lib()
     dp, ip = C.POINTER(C.c_double), C.POINTER(C.c_int32)
     pb = world["b"].select(np.arange(16))
-    opt = _ctx(gpu, world, precision, world["g0"])
+    opt = ctx(gpu, precision, world["params"], world["g0"])
     out = opt.optimize(pb)
-    before = _pieces(pb, out)
+    before = pieces(pb, out)
     res, cxy, cyaw = out
     N, M = np.ascontiguousarray(pb.N, np.int32), np.ascontiguousarray(pb.M, np.int32)
     pt = np.array([(r.piece_T_xy, r.piece_T_yaw) for r in res], np.float64)
@@ -406,13 +357,13 @@ def test_refused_replans_write_nothing_and_take_no_lane(gpu, world, precision):
     # no lane was taken by the refusals: the next submit gets the ticket it would have got
     nxt = opt.submit(pb, depth=3)
     assert nxt == (t_ok + 1) % 3
-    assert _same(_pieces(pb, opt.wait(nxt)), before)
+    assert same_pieces(pieces(pb, opt.wait(nxt)), before)
     # B = 0 is an empty submit
     assert call(B=0, n=None, m=None, p=None, cx=None, cy=None, bd=None, tf=None, no=None, mo=None, b_=None, to=None, depth=3) == 0
     assert tk.value == (nxt + 1) % 3
     opt._tickets[tk.value] = (pb.select([]), None)
     opt.wait(tk.value)
-    assert _same(_pieces(pb, opt.optimize(pb)), before)
+    assert same_pieces(pieces(pb, opt.optimize(pb)), before)
     opt.close()
 
 
@@ -421,7 +372,7 @@ def test_replans_do_not_leak(gpu, world, precision):
     import torch
     depth = 3 if precision == 64 else 8
     pb, held = world["b"], world["held_b"]
-    opt = _ctx(gpu, world, precision, world["g0"])
+    opt = ctx(gpu, precision, world["params"], world["g0"])
 
     def fill():
         return [opt.wait(t) for t in [opt.submit(pb, depth=depth) for _ in range(depth)]][-1]
@@ -432,7 +383,7 @@ def test_replans_do_not_leak(gpu, world, precision):
     q = collections.deque()
     for i in range(20):
         src = world["g1"] if i % 2 == 0 else world["g0"]
-        opt.update_environment_window(BOX[0], BOX[1], _box(src.cells, BOX))
+        opt.update_environment_window(BOX[0], BOX[1], box_cells(src.cells, BOX))
         if len(q) >= depth - 1:
             opt.wait(q.popleft())
         if i % 2 == 0:
@@ -451,10 +402,7 @@ def test_replans_do_not_leak(gpu, world, precision):
 
 def test_cpp_replan_between_submit_and_wait(gpu, world, tmp_path):
     from uneven_planner_b200 import _lib
-    exe = str(tmp_path / "replan_driver")
-    lib = os.path.join(ROOT, "uneven_planner_b200")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "replan_driver.cpp"), "-o", exe,
-                    "-L", lib, "-lualm", "-Wl,-rpath," + lib], check=True)
+    exe = build_driver("replan_driver", tmp_path)
     g0 = world["g0"]
     pb = world["bench"].select(np.arange(8))
     tf = np.array([0.0, 0.5, 1.0, 1.5, 2.0, 2.5, 0.25, 0.75])
@@ -480,11 +428,11 @@ def test_cpp_replan_between_submit_and_wait(gpu, world, tmp_path):
     assert [int(x[0]) for x in head] == list(range(pb.B))
     assert [(int(x[1]), int(x[2])) for x in head] == list(zip(new.N.tolist(), new.M.tolist()))
     got = np.array([[float(v) for v in x[3:22]] for x in head])
-    assert np.array_equal(_bits(got), _bits(np.concatenate([new.total_time[:, None], new.bnd], 1)))
+    assert np.array_equal(bits(got), bits(np.concatenate([new.total_time[:, None], new.bnd], 1)))
     assert [int(x[22]) for x in head] == [r_.ret_code for r_ in res]
-    assert np.array_equal(_bits([float(x[23]) for x in head]), _bits([r_.total_T for r_ in res]))
+    assert np.array_equal(bits([float(x[23]) for x in head]), bits([r_.total_T for r_ in res]))
     coef = np.array([float(v) for v in lines[pb.B:]])
-    assert np.array_equal(_bits(coef), _bits(np.concatenate([cxy, cyaw])))
+    assert np.array_equal(bits(coef), bits(np.concatenate([cxy, cyaw])))
 
 
 @pytest.mark.parametrize("precision", PRECISIONS)
@@ -502,9 +450,9 @@ def test_degenerate_inputs_are_refused_or_cut_short(gpu, world, precision):
     res8 = (_lib.Result * 8)(*[out0[0][i] for i in sel])
     out = (res8, out0[1][:ocx[8]].copy(), out0[2][:ocy[8]].copy())
     tf = _t_from(pb, out, 2)
-    opt = _ctx(gpu, world, precision, world["g0"])
+    opt = ctx(gpu, precision, world["params"], world["g0"])
     t_ok, ref_new = opt.submit_replan(pb, out, np.arange(8), tf, depth=3)
-    ref_got = _pieces(ref_new, opt.wait(t_ok))
+    ref_got = pieces(ref_new, opt.wait(t_ok))
 
     def bad_pb(k, v):
         b = pb.select(np.arange(8))
@@ -529,9 +477,9 @@ def test_degenerate_inputs_are_refused_or_cut_short(gpu, world, precision):
         buf = opt.outputs(new)
         idx, _ = opt.poll(t, buf, 0.0)
         assert 3 in idx.tolist() and buf[0][3].ret_code == _lib.UALM_ELIMIT
-        got = _pieces(new, opt.wait(t))
+        got = pieces(new, opt.wait(t))
         assert not got[3][1].any() and not got[3][2].any()
         assert _same_pb(new, ro.problems_of(ro.rows(b, out, np.arange(8), tf)))
         keep = [i for i in range(8) if i != 3]
-        assert _same([got[i] for i in keep], [ref_got[i] for i in keep])
+        assert same_pieces([got[i] for i in keep], [ref_got[i] for i in keep])
     opt.close()

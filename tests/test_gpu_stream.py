@@ -3,7 +3,6 @@ exactly once, bit for bit what ualm_wait_batch returns for it (and, on the parit
 mix, problems over the limits come back at once, and budgets and deadlines keep their meaning.  Workload: BASELINE configs[1]'s
 recipe (hill terrain or its stand-in, hill parameters)."""
 import ctypes as C
-import os
 import struct
 import subprocess
 import time
@@ -11,31 +10,19 @@ import time
 import numpy as np
 import pytest
 
+from harness import build_driver, ctx, gpu, same_bytes, same_problem  # noqa: F401
+
+
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 STOPPED = 3
 ip = C.POINTER(C.c_int32)
-
-
-@pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
 
 
 @pytest.fixture(scope="module")
 def work(hill_map):
     from uneven_planner_b200 import configs, problems
     return hill_map, configs.params_for("hill"), problems.generate(hill_map, 256, seed=0, **configs.gen_kwargs("hill"))
-
-
-def _ctx(gpu, work, precision):
-    m, params, _ = work
-    return gpu.BatchALMTrajOpt(precision=precision).init(params).set_environment(m)
 
 
 def _poll_all(opt, ticket, pb, wait_ms=1.0, limit_s=600.0):
@@ -55,25 +42,14 @@ def _poll_all(opt, ticket, pb, wait_ms=1.0, limit_s=600.0):
     return out, polls
 
 
-def _same(a, b):
-    """two (results, c_xy, c_yaw) byte for byte"""
-    return bytes(a[0]) == bytes(b[0]) and a[1].tobytes() == b[1].tobytes() and a[2].tobytes() == b[2].tobytes()
-
-
-def _same_problem(pb, a, b, i):
-    _, _, ocx, ocy = pb.offsets()
-    return bytes(a[0][i]) == bytes(b[0][i]) and a[1][ocx[i]:ocx[i + 1]].tobytes() == b[1][ocx[i]:ocx[i + 1]].tobytes() and \
-        a[2][ocy[i]:ocy[i + 1]].tobytes() == b[2][ocy[i]:ocy[i + 1]].tobytes()
-
-
 @pytest.mark.parametrize("precision", [64, 32, 65])
 def test_polled_equals_waited(gpu, work, golden, precision):
     m, _, pb = work
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     t = opt.submit(pb, depth=1)
     polled, polls = _poll_all(opt, t, pb)
     waited = opt.wait(t)
-    assert _same(polled, waited)
+    assert same_bytes(polled, waited)
     if precision == 64:
         # the batch starts with the committed golden problems (same generator, seed and terrain): bit for bit the oracle's
         gold = golden("hill", m)
@@ -92,7 +68,7 @@ def test_three_tickets_polled_interleaved(gpu, work, precision):
     pb = work[2]
     parts = [pb.select(np.arange(0, 96)), pb.select(np.arange(96, 160)), pb.select(np.arange(160, 256))]
     ref = []
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     for p in parts:
         ref.append(opt.optimize(p))
     tickets = [opt.submit(p, depth=3) for p in parts]
@@ -110,8 +86,8 @@ def test_three_tickets_polled_interleaved(gpu, work, precision):
         assert time.perf_counter() - t0 < 600.0
     for k, t in enumerate(tickets):
         assert (seen[k] == 1).all()
-        assert _same(outs[k], opt.wait(t))
-        assert _same(outs[k], ref[k])
+        assert same_bytes(outs[k], opt.wait(t))
+        assert same_bytes(outs[k], ref[k])
     opt.close()
 
 
@@ -131,13 +107,13 @@ def _spread_batch(m):
 @pytest.mark.parametrize("precision", [64, 32])
 def test_short_problems_come_back_before_the_long_ones(gpu, work, precision):
     pb = _spread_batch(work[0])
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     ref = opt.optimize(pb)
     t = opt.submit(pb, depth=1)
     polled, polls = _poll_all(opt, t, pb)
     assert any(n > 0 and pend > 0 for n, pend in polls), polls
-    assert _same(polled, opt.wait(t))
-    assert _same(polled, ref)
+    assert same_bytes(polled, opt.wait(t))
+    assert same_bytes(polled, ref)
     opt.close()
     print("precision %d: polls (returned, pending) %s" % (precision, [p for p in polls if p[0] > 0]))
 
@@ -163,7 +139,7 @@ def test_problem_over_the_limits_comes_back_first(gpu, work, precision):
     base = work[2].select(np.arange(24))
     at = 9
     pb = _with_oversized(base, at)
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     ref = opt.optimize(base)
     t = opt.submit(pb, depth=1)
     out = opt.outputs(pb)
@@ -181,7 +157,7 @@ def test_problem_over_the_limits_comes_back_first(gpu, work, precision):
         assert time.perf_counter() - t0 < 600.0
     assert (seen == 1).all()
     waited = opt.wait(t)
-    assert _same(out, waited)
+    assert same_bytes(out, waited)
     for i in range(pb.B):                       # the rest of the batch is unaffected
         if i != at:
             j = i if i < at else i - 1
@@ -195,7 +171,7 @@ def test_problem_over_the_limits_comes_back_first(gpu, work, precision):
 @pytest.mark.parametrize("precision", [64, 32])
 def test_polls_then_a_deadline(gpu, work, precision):
     pb = work[2]
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     free = opt.optimize(pb)
     t = opt.submit(pb, depth=1)
     out = opt.outputs(pb)
@@ -211,15 +187,15 @@ def test_polls_then_a_deadline(gpu, work, precision):
     n_stop = 0
     for i in range(pb.B):
         if i in polled:
-            assert _same_problem(pb, out, waited, i), i
+            assert same_problem(pb, out, waited, i), i
         if waited[0][i].ret_code == STOPPED:
             n_stop += 1
         else:
-            assert _same_problem(pb, waited, free, i), i
+            assert same_problem(pb, waited, free, i), i
     # the lane's next batch starts without a stop request and streams again
     t = opt.submit(pb, depth=1)
     again, _ = _poll_all(opt, t, pb)
-    assert _same(again, opt.wait(t)) and _same(again, free)
+    assert same_bytes(again, opt.wait(t)) and same_bytes(again, free)
     opt.close()
     print("precision %d: %d problems returned by the polls, %d stopped by the deadline" % (precision, polled.size, n_stop))
 
@@ -227,11 +203,11 @@ def test_polls_then_a_deadline(gpu, work, precision):
 @pytest.mark.parametrize("precision", [64, 32])
 def test_budget_stopped_problems_stream(gpu, work, precision):
     pb = work[2]
-    opt = _ctx(gpu, work, precision).set_budget(50)
+    opt = ctx(gpu, precision, work[1], work[0]).set_budget(50)
     ref = opt.optimize(pb)
     t = opt.submit(pb, depth=1)
     polled, _ = _poll_all(opt, t, pb)
-    assert _same(polled, opt.wait(t)) and _same(polled, ref)
+    assert same_bytes(polled, opt.wait(t)) and same_bytes(polled, ref)
     assert any(r.ret_code == STOPPED for r in polled[0])
     opt.close()
 
@@ -248,7 +224,7 @@ def test_poll_refusals(gpu, work, precision):
     from uneven_planner_b200 import _lib
     EINVAL, ESTATE = _lib.UALM_EINVAL, _lib.UALM_ESTATE
     pb = work[2].select(np.arange(16))
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     t = opt.submit(pb, depth=1)
     assert _raw_poll(opt, -1) == EINVAL and _raw_poll(opt, _lib.lib().ualm_max_lanes()) == EINVAL
     assert _raw_poll(opt, 5) == ESTATE                       # never submitted
@@ -282,10 +258,7 @@ def _write_case(path, m, pb):
 def test_cpp_poll_batch(gpu, work, tmp_path, precision):
     """pollBatch through include/ualm_traj_opt.hpp: the union of the polled results equals waitBatch (checked by the driver)"""
     m, _, pb = work
-    exe = str(tmp_path / "stream_driver")
-    lib = os.path.join(ROOT, "uneven_planner_b200")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "stream_driver.cpp"),
-                    "-o", exe, "-L", lib, "-lualm", "-Wl,-rpath," + lib], check=True)
+    exe = build_driver("stream_driver", tmp_path)
     case = str(tmp_path / "case.bin")
     _write_case(case, m, pb.select(np.arange(64)))
     r = subprocess.run([exe, case, str(precision)], capture_output=True, text=True)

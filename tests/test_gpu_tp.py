@@ -12,19 +12,11 @@ import os
 import numpy as np
 import pytest
 
+from harness import gpu  # noqa: F401
+from workloads import TOL
+
+
 pytestmark = pytest.mark.gpu
-
-TOL = {65: dict(f=1e-9, grad=1e-9, con=1e-9, coef=1e-10, sfx=1e-9, scx=1e-8),
-       32: dict(f=1e-4, grad=1e-4, con=1e-4, coef=1e-10, sfx=1e-6, scx=2e-3)}
-
-
-@pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
 
 
 def _rel(a, b):
@@ -156,7 +148,7 @@ def test_results_do_not_depend_on_batching_or_tile_staging(gpu, hill_map):
 def test_limits_and_state_checks(gpu, bumps_map):
     """a problem over the compiled limits fails alone (UALM_ELIMIT record); calls out of order are refused"""
     from uneven_planner_b200 import _lib, problems
-    from test_gpu_boundary import _with_oversize
+    from workloads import _with_oversize
     params = _lib.default_params()
     pb = problems.generate(bumps_map, 9, seed=31)
     opt = gpu.BatchALMTrajOpt(precision=32).init(params)

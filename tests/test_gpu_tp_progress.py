@@ -7,29 +7,18 @@ import time
 import numpy as np
 import pytest
 
+from harness import ctx, gpu, same_bytes, same_problem  # noqa: F401
+
+
 pytestmark = pytest.mark.gpu
 
 STOPPED = 3
 
 
 @pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
-
-
-@pytest.fixture(scope="module")
 def work(hill_map):
     from uneven_planner_b200 import configs, problems
     return hill_map, configs.params_for("hill"), problems.generate(hill_map, 1024, seed=0, **configs.gen_kwargs("hill"))
-
-
-def _ctx(gpu, work, precision):
-    m, params, _ = work
-    return gpu.BatchALMTrajOpt(precision=precision).init(params).set_environment(m)
 
 
 @pytest.fixture(scope="module")
@@ -39,26 +28,11 @@ def free(gpu, work):
 
     def get(precision):
         if precision not in cache:
-            opt = _ctx(gpu, work, precision)
+            opt = ctx(gpu, precision, work[1], work[0])
             cache[precision] = opt.optimize(work[2])
             opt.close()
         return cache[precision]
     return get
-
-
-def _same(a, b):
-    return bytes(a[0]) == bytes(b[0]) and a[1].tobytes() == b[1].tobytes() and a[2].tobytes() == b[2].tobytes()
-
-
-def _part(pb, out, i):
-    _, _, ocx, ocy = pb.offsets()
-    return out[0][i], out[1][ocx[i]:ocx[i + 1]], out[2][ocy[i]:ocy[i + 1]]
-
-
-def _same_problem(pb, a, b, i):
-    ra, xa, ya = _part(pb, a, i)
-    rb, xb, yb = _part(pb, b, i)
-    return bytes(ra) == bytes(rb) and xa.tobytes() == xb.tobytes() and ya.tobytes() == yb.tobytes()
 
 
 def _wait_time(opt, pb):
@@ -78,15 +52,15 @@ def _idle(T):
 def test_batch_completes_without_host_calls(gpu, work, free, precision):
     pb = work[2]
     ref = free(precision)
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     T = _wait_time(opt, pb)
     t = opt.submit(pb, depth=1)
     time.sleep(_idle(T))
     out = opt.outputs(pb)
     idx, pending = opt.poll(t, out, 0.0)
     assert idx.size == pb.B and pending == 0, (idx.size, pending)
-    assert _same(out, ref)
-    assert _same(opt.wait(t), ref)
+    assert same_bytes(out, ref)
+    assert same_bytes(opt.wait(t), ref)
     opt.close()
     print("precision %d: wait %.1f ms; all %d problems published during a sleep of %.1f s" % (precision, 1e3 * T, pb.B, _idle(T)))
 
@@ -95,7 +69,7 @@ def test_batch_completes_without_host_calls(gpu, work, free, precision):
 def test_eight_tickets_complete_without_host_calls(gpu, work, precision):
     pb = work[2]
     parts = [pb.select(np.arange(k * 128, (k + 1) * 128)) for k in range(8)]
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     refs = [opt.optimize(p) for p in parts]
     T = _wait_time(opt, pb)
     tickets = [opt.submit(p, depth=8) for p in parts]
@@ -105,13 +79,13 @@ def test_eight_tickets_complete_without_host_calls(gpu, work, precision):
         out = opt.outputs(p)
         idx, pending = opt.poll(t, out, 0.0)
         assert idx.size == p.B and pending == 0, (t, idx.size, pending)
-        assert _same(out, r), t
+        assert same_bytes(out, r), t
     for t, r in zip(tickets, refs):
-        assert _same(opt.wait(t), r), t
+        assert same_bytes(opt.wait(t), r), t
     for t, p, r in zip(tickets, parts, refs):         # every lane takes its next batch
         t2 = opt.submit(p, depth=8)
         assert t2 == t
-        assert _same(opt.wait(t2), r)
+        assert same_bytes(opt.wait(t2), r)
     opt.close()
 
 
@@ -134,9 +108,9 @@ def test_mixed_environment_batch_completes_without_host_calls(gpu, work, terrain
     out = opt.outputs(mixed)
     idx, pending = opt.poll(t, out, 0.0)
     assert idx.size == mixed.B and pending == 0, (idx.size, pending)
-    assert _same(out, ref) and _same(opt.wait(t), ref)
+    assert same_bytes(out, ref) and same_bytes(opt.wait(t), ref)
     t = opt.submit(mixed, depth=1)
-    assert _same(opt.wait(t), ref)
+    assert same_bytes(opt.wait(t), ref)
     opt.close()
 
 
@@ -144,7 +118,7 @@ def test_mixed_environment_batch_completes_without_host_calls(gpu, work, terrain
 def test_cancel_reaches_a_running_batch(gpu, work, free, precision):
     pb = work[2]
     ref = free(precision)
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     T = _wait_time(opt, pb)
     t = opt.submit(pb, depth=1)
     time.sleep(T / 4)
@@ -154,11 +128,11 @@ def test_cancel_reaches_a_running_batch(gpu, work, free, precision):
     out = opt.outputs(pb)
     idx, pending = opt.poll(t, out, 0.0)
     assert idx.size == pb.B and pending == 0, (idx.size, pending)
-    assert _same(out, opt.wait(t))
+    assert same_bytes(out, opt.wait(t))
     stopped = [i for i in range(pb.B) if out[0][i].ret_code == STOPPED]
     for i in range(pb.B):
         if out[0][i].ret_code != STOPPED:
-            assert _same_problem(pb, out, ref, i), i
+            assert same_problem(pb, out, ref, i), i
     assert stopped
     assert all(out[0][i].n_lbfgs_iters >= 1 for i in stopped)
     assert np.mean([r.n_evals for r in out[0]]) < np.mean([r.n_evals for r in ref[0]])
@@ -170,17 +144,17 @@ def test_cancel_reaches_a_running_batch(gpu, work, free, precision):
 def test_budget_and_deadline_under_the_device_loop(gpu, work, free, precision):
     pb = work[2]
     ref = free(precision)
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     opt.set_budget(50)
     budget_ref = opt.optimize(pb)
-    assert _same(opt.wait(opt.submit(pb, depth=1)), budget_ref)
+    assert same_bytes(opt.wait(opt.submit(pb, depth=1)), budget_ref)
     opt.set_budget(0)
     out = opt.wait(opt.submit(pb, depth=1), timeout_ms=0)
     rc = np.array([r.ret_code for r in out[0]])
     assert (rc == STOPPED).any()
     for i in np.flatnonzero(rc != STOPPED):
-        assert _same_problem(pb, out, ref, i), i
-    assert _same(opt.wait(opt.submit(pb, depth=1)), ref)         # the lane is reusable
+        assert same_problem(pb, out, ref, i), i
+    assert same_bytes(opt.wait(opt.submit(pb, depth=1)), ref)         # the lane is reusable
     opt.close()
 
 
@@ -189,7 +163,7 @@ def test_phase_entry_points_run_through_the_device_loop(gpu, work, precision):
     """eval_batch (at the uploaded initial guesses) and init_scaling_batch repeat byte for byte, and around them the resident
     batch solves to optimize's bytes"""
     pb = work[2].select(np.arange(256))
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work[1], work[0])
     ref = opt.optimize(pb)
     opt.upload(pb)
     ev = [opt.eval_batch() for _ in range(2)]
@@ -199,7 +173,7 @@ def test_phase_entry_points_run_through_the_device_loop(gpu, work, precision):
     assert sc[0][0].tobytes() == sc[1][0].tobytes() and sc[0][1].tobytes() == sc[1][1].tobytes()
     opt.solve_resident()
     opt.sync()
-    assert _same(opt.download(), ref)
+    assert same_bytes(opt.download(), ref)
     # and in the other order on the same lane: the solve leaves nothing the phase calls see
     again = opt.eval_batch(), opt.init_scaling_batch()
     for k in ev[0]:

@@ -13,21 +13,13 @@ import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import cancel_oracle as co  # noqa: E402
+from harness import build_driver, ctx, gpu, part, pending, same_bytes, same_problem  # noqa: F401, E402
+
 
 pytestmark = pytest.mark.gpu
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 STOPPED = 3
 DEPTH = {64: 3, 32: 8, 65: 8}
-
-
-@pytest.fixture(scope="module")
-def gpu(built):
-    import torch
-    if not torch.cuda.is_available():
-        pytest.skip("no CUDA device")
-    from uneven_planner_b200 import api
-    return api
 
 
 @pytest.fixture(scope="module")
@@ -40,10 +32,6 @@ def work(hill_map, golden):
                 big=problems.generate(hill_map, 4096, seed=11, **kw), small=problems.generate(hill_map, 16, seed=12, **kw))
 
 
-def _ctx(gpu, work, precision=64):
-    return gpu.BatchALMTrajOpt(precision=precision).init(work["params"]).set_environment(work["m"])
-
-
 @pytest.fixture(scope="module")
 def free(gpu, work):
     """(precision, batch name, budget) -> the batch solved alone on a fresh context"""
@@ -52,32 +40,13 @@ def free(gpu, work):
     def get(precision, name, budget=0):
         key = (precision, name, budget)
         if key not in cache:
-            opt = _ctx(gpu, work, precision)
+            opt = ctx(gpu, precision, work["params"], work["m"])
             if budget:
                 opt.set_budget(budget)
             cache[key] = opt.optimize(work[name])
             opt.close()
         return cache[key]
     return get
-
-
-def _same(a, b):
-    return bytes(a[0]) == bytes(b[0]) and a[1].tobytes() == b[1].tobytes() and a[2].tobytes() == b[2].tobytes()
-
-
-def _part(pb, out, i):
-    _, _, ocx, ocy = pb.offsets()
-    return out[0][i], out[1][ocx[i]:ocx[i + 1]], out[2][ocy[i]:ocy[i + 1]]
-
-
-def _same_problem(pb, a, b, i):
-    ra, xa, ya = _part(pb, a, i)
-    rb, xb, yb = _part(pb, b, i)
-    return bytes(ra) == bytes(rb) and xa.tobytes() == xb.tobytes() and ya.tobytes() == yb.tobytes()
-
-
-def _pending(opt, t, pb):
-    return opt.poll(t, opt.outputs(pb), 0.0)[1]
 
 
 def _drain(opt, t, pb, limit_s=600.0):
@@ -93,14 +62,14 @@ def _drain(opt, t, pb, limit_s=600.0):
 
 @pytest.mark.parametrize("precision", [64, 32, 65])
 def test_urgent_ticket_bits(gpu, work, free, precision):
-    opt = _ctx(gpu, work, precision)
+    opt = ctx(gpu, precision, work["params"], work["m"])
     d = DEPTH[precision]
     t0, t1 = opt.submit(work["pb"], depth=d), opt.submit(work["pb"], depth=d)
     tu = opt.submit(work["gold_pb"], depth=d, urgent=True)
     outs = [opt.wait(tu), opt.wait(t0), opt.wait(t1)]
     opt.close()
-    assert _same(outs[0], free(precision, "gold_pb"))
-    assert _same(outs[1], free(precision, "pb")) and _same(outs[2], free(precision, "pb"))
+    assert same_bytes(outs[0], free(precision, "gold_pb"))
+    assert same_bytes(outs[1], free(precision, "pb")) and same_bytes(outs[2], free(precision, "pb"))
     if precision == 64:
         g = work["gold"]
         res, cxy, cyaw = outs[0]
@@ -119,20 +88,20 @@ def _race(opt, work, urgent):
     tu = opt.submit(small, depth=3, urgent=urgent)
     _drain(opt, tu, small)
     ms = 1e3 * (time.perf_counter() - s)
-    left = _pending(opt, t1, big)
+    left = pending(opt, t1, big)
     outs = [opt.wait(tu), opt.wait(t0), opt.wait(t1)]
     return left, ms, outs
 
 
 def test_urgent_ticket_goes_ahead(gpu, work, free):
-    opt = _ctx(gpu, work)
+    opt = ctx(gpu, 64, work["params"], work["m"])
     left_n, ms_n, _ = _race(opt, work, False)
     left_u, ms_u, outs = _race(opt, work, True)
     opt.close()
     print("16 problems behind two 4096-problem tickets: urgent complete after %.1f ms with %d of background ticket 1 pending; "
           "not urgent %.1f ms with %d pending (background ticket 1)" % (ms_u, left_u, ms_n, left_n))
     assert left_u > work["big"].B // 2
-    assert _same(outs[0], free(64, "small"))
+    assert same_bytes(outs[0], free(64, "small"))
 
 
 def test_urgent_ticket_that_grows_its_lane(gpu, work, free):
@@ -142,7 +111,7 @@ def test_urgent_ticket_that_grows_its_lane(gpu, work, free):
     big, pb, small = work["big"], work["pb"], work["small"]
 
     def run(urgent):
-        opt = _ctx(gpu, work)
+        opt = ctx(gpu, 64, work["params"], work["m"])
         for _ in range(3):
             opt.wait(opt.submit(small, depth=3))
         t0, t1 = opt.submit(big, depth=3), opt.submit(big, depth=3)
@@ -161,22 +130,22 @@ def test_urgent_ticket_that_grows_its_lane(gpu, work, free):
           "not urgent: call %.1f ms, complete %.1f ms, everything %.1f ms" % tuple(1e3 * x for x in u[:3] + n[:3]))
     assert u[2] < n[2] + 0.5
     assert u[1] - u[0] < 1.0
-    assert _same(u[3][0], free(64, "pb")) and _same(u[3][1], n[3][1]) and _same(u[3][2], n[3][2])
+    assert same_bytes(u[3][0], free(64, "pb")) and same_bytes(u[3][1], n[3][1]) and same_bytes(u[3][2], n[3][2])
 
 
 def test_urgent_check_and_replan_in_flight(gpu, work, free):
     pb, big = work["gold_pb"], work["big"]
     held = free(64, "gold_pb")
     rows, tf = np.arange(pb.B), np.full(pb.B, 0.5)
-    opt = _ctx(gpu, work)
+    opt = ctx(gpu, 64, work["params"], work["m"])
     chk_idle = opt.check_results(pb, held)
     tr, new_idle = opt.submit_replan(pb, held, rows, tf, depth=3)
     rep_idle = opt.wait(tr)
     t0, t1 = opt.submit(big, depth=3), opt.submit(big, depth=3)
     chk = opt.check_results(pb, held, urgent=True)
-    left_c = _pending(opt, t1, big)
+    left_c = pending(opt, t1, big)
     tr, new = opt.submit_replan(pb, held, rows, tf, depth=3, urgent=True)
-    left_r = _pending(opt, t1, big)
+    left_r = pending(opt, t1, big)
     rep = opt.wait(tr)
     opt.cancel(t0, np.arange(big.B))
     opt.cancel(t1, np.arange(big.B))
@@ -187,14 +156,14 @@ def test_urgent_check_and_replan_in_flight(gpu, work, free):
     assert chk.tobytes() == chk_idle.tobytes()
     for a in ("N", "M", "bnd", "total_time", "inner_xy", "inner_yaw"):
         assert np.asarray(getattr(new, a)).tobytes() == np.asarray(getattr(new_idle, a)).tobytes(), a
-    assert _same(rep, rep_idle)
+    assert same_bytes(rep, rep_idle)
 
 
 def test_interplay_with_cancel_deadline_and_budget(gpu, work, free):
     import pyoracle as po
     pb, small = work["pb"], work["small"]
     ref, ref_small = free(64, "pb"), free(64, "small")
-    opt = _ctx(gpu, work)
+    opt = ctx(gpu, 64, work["params"], work["m"])
     # cancels of a held ticket and of the urgent ticket
     t0 = opt.submit(pb, depth=3)
     tu = opt.submit(small, depth=3, urgent=True)
@@ -209,31 +178,31 @@ def test_interplay_with_cancel_deadline_and_budget(gpu, work, free):
     out1 = opt.wait(t1, timeout_ms=5.0)
     outu2 = opt.wait(tu2)
     opt.close()
-    assert _same(outu2, ref_small)
+    assert same_bytes(outu2, ref_small)
     stopped = []
     for out, b, r, cut in ((out0, pb, ref, cut0), (outu, small, ref_small, cutu), (out1, pb, ref, np.arange(pb.B))):
         for i in range(b.B):
             if i in cut and out[0][i].ret_code == STOPPED:
                 stopped.append((b, out, i))
             else:
-                assert _same_problem(b, out, r, i), i
+                assert same_problem(b, out, r, i), i
     assert any(o is out1 for _, o, _ in stopped)
     prm, om = po.params_from(work["params"]), po.OracleMap(work["m"])
     co.lib()
     rng = np.random.default_rng(3)
     pick = [stopped[k] for k in rng.choice(len(stopped), min(24, len(stopped)), replace=False)]
     for b, out, i in pick:
-        r, cxy, cyaw = _part(b, out, i)
+        r, cxy, cyaw = part(b, out, i)
         assert co.match_stopped(prm, om, b, i, r, cxy, cyaw) is not None, i
     # a budget: the urgent ticket and the held ones, each bit for bit its free solve under the same budget
     budget = 40
-    opt = _ctx(gpu, work)
+    opt = ctx(gpu, 64, work["params"], work["m"])
     opt.set_budget(budget)
     t0 = opt.submit(pb, depth=3)
     tu = opt.submit(small, depth=3, urgent=True)
     outu, out0 = opt.wait(tu), opt.wait(t0)
     opt.close()
-    assert _same(outu, free(64, "small", budget)) and _same(out0, free(64, "pb", budget))
+    assert same_bytes(outu, free(64, "small", budget)) and same_bytes(out0, free(64, "pb", budget))
     assert any(r.ret_code == STOPPED for r in out0[0])
 
 
@@ -242,7 +211,7 @@ def test_no_leaked_hold(gpu, work, free):
     L = _lib.lib()
     big, small, gold_pb = work["big"], work["small"], work["gold_pb"]
     held = free(64, "gold_pb")
-    opt = _ctx(gpu, work)
+    opt = ctx(gpu, 64, work["params"], work["m"])
     opt.wait(opt.submit(big, depth=1))                          # warm-up
     alone = _drain(opt, opt.submit(big, depth=1), big)
     opt.wait(0)
@@ -288,10 +257,7 @@ def test_no_leaked_hold(gpu, work, free):
 def test_cpp_set_urgent(gpu, work, tmp_path, precision):
     """setUrgent through include/ualm_traj_opt.hpp around submitBatch / checkTrajectories / submitReplan (checked by the driver)"""
     from uneven_planner_b200 import maps
-    exe = str(tmp_path / "urgent_driver")
-    lib = os.path.join(ROOT, "uneven_planner_b200")
-    subprocess.run(["g++", "-O2", "-std=c++14", "-I", os.path.join(ROOT, "include"), os.path.join(ROOT, "tests", "cpp", "urgent_driver.cpp"), "-o", exe,
-                    "-L", lib, "-lualm", "-Wl,-rpath," + lib], check=True)
+    exe = build_driver("urgent_driver", tmp_path)
     g0 = maps.stand_in_terrain("hill")
     pb = work["pb"].select(np.arange(0, 1024, 32))
     tf = np.full(pb.B, 0.5)

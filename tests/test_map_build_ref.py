@@ -21,138 +21,7 @@ import pytest
 
 import map_build_ref as mref
 
-
-# ------------------------------------------------------------------------------------------------------ clouds
-def _one_per_voxel(p):
-    """float32 points, the first of each 1 cm voxel kept (the builder's VoxelGrid then returns them unchanged)"""
-    p = np.asarray(p, np.float64).astype(np.float32)
-    keys = np.floor(p * (np.float32(1.0) / np.float32(0.01))).astype(np.int64)
-    _, first = np.unique(keys, axis=0, return_index=True)
-    return np.ascontiguousarray(p[np.sort(first)])
-
-
-def _lattice(cx, cy, half, step, rng, jitter=0.35):
-    g = np.arange(-half, half + 1e-9, step)
-    gx, gy = np.meshgrid(g, g, indexing="ij")
-    x = gx.ravel() + rng.uniform(-jitter, jitter, gx.size) * step
-    y = gy.ravel() + rng.uniform(-jitter, jitter, gy.size) * step
-    return x, y
-
-
-def terrain(kind, cx=0.0, cy=0.0, half=0.75, seed=0):
-    """one scenario's cloud about (cx, cy), coordinates relative to the centre in the formulas"""
-    rng = np.random.default_rng(seed)
-    x, y = _lattice(0.0, 0.0, half, 0.025, rng)
-    if kind == "smooth":
-        z = 0.5 + 0.3 * np.sin(1.3 * x) * np.cos(0.9 * y) + rng.normal(0, 0.003, x.size)
-    elif kind == "slope68":                 # 68 degrees: z rises 2.475 m per metre in x
-        x, y = _lattice(0.0, 0.0, half, 0.012, rng)
-        z = 2.5 + np.tan(np.radians(68.0)) * x + rng.normal(0, 0.002, x.size)
-    elif kind == "step":                    # a 0.4 m step along x = 0.05
-        z = np.where(x < 0.05, 0.3, 0.7) + rng.normal(0, 0.002, x.size)
-    elif kind in ("sparse", "very_sparse"):  # 3 % of a 1.2 cm / 2.5 cm lattice: footprints of a few points, of one or two
-        if kind == "sparse":
-            x, y = _lattice(0.0, 0.0, half, 0.012, rng)
-        keep = rng.uniform(size=x.size) < 0.03
-        x, y = x[keep], y[keep]
-        z = 0.4 + 0.2 * np.sin(2.0 * x) + rng.normal(0, 0.003, x.size)
-    elif kind == "corner":                  # only the corner x, y < -0.2 of the grid
-        keep = (x < -0.2) & (y < -0.2)
-        x, y = x[keep], y[keep]
-        z = 0.6 + 0.1 * x - 0.05 * y + rng.normal(0, 0.002, x.size)
-    elif kind == "plane":                   # one exact float height
-        z = np.full(x.size, 0.5)
-    elif kind == "hole":
-        keep = x ** 2 + (y - 0.1) ** 2 > 0.25 ** 2
-        x, y = x[keep], y[keep]
-        z = 0.5 + 0.3 * np.sin(1.3 * x) * np.cos(0.9 * y) + rng.normal(0, 0.003, x.size)
-    elif kind == "wall":                    # a vertical wall up to 1.2 m on flat ground, along (3, 4) / 5 through the centre
-        z = 0.02 + rng.uniform(0, 0.004, x.size)
-        gs, gz = np.meshgrid(np.arange(-0.9, 0.9, 0.02), np.arange(0.04, 1.2, 0.02), indexing="ij")
-        k = np.round((gs.ravel() + rng.uniform(-0.006, 0.006, gs.size)) * 256)   # at (0.75 k, k) / 256: on the plane 4x = 3y exactly
-        x = np.concatenate([x, 0.75 * k / 256])
-        y = np.concatenate([y, k / 256])
-        z = np.concatenate([z, gz.ravel() + rng.uniform(-0.006, 0.006, gz.size)])
-    else:
-        raise ValueError(kind)
-    return _one_per_voxel(np.column_stack([np.asarray(x, np.float64) + cx, np.asarray(y, np.float64) + cy, z]))
-
-
-def grid(name, cx=0.0, cy=0.0):
-    from uneven_planner_b200 import _lib
-    size = {"square": (1.0, 1.0, 0.05, 0.1), "fine_yaw": (0.73, 0.5, 0.04, 0.05), "coarse": (1.4, 1.2, 0.1, 0.2)}[name]
-    return _lib.map_geometry_at(*size, cx, cy)
-
-
-# name: (terrain, grid, centre, iter_num, ellipsoid, largest ambiguous share, largest plausibility-only share, least counts the
-# scenario must reach).  The shares bound what was measured: ambiguous / plausibility-only cells of all cells, 0 / 0 on every
-# scenario but wall 654 / 0 of 25600, wall_it3 93 / 0 of 5376, wall_far 1019 / 0 of 31369, sparse 21 / 18, very_sparse_it3 1310 / 1235 of
-# 5376, corner 93 / 70, hole 95 / 62, corner_far 130 / 113.  Plausibility-only cells are those whose footprint was degenerate before
-# the last iteration, so that every later iteration depends on an arbitrary normal.
-SCENARIOS = {
-    "smooth": ("smooth", "square", (0.0, 0.0), 2, (0.2, 0.1, 0.1), 0.0, 0.0, {}),
-    "smooth_it1": ("smooth", "square", (0.0, 0.0), 1, (0.2, 0.1, 0.1), 0.0, 0.0, {}),
-    "smooth_it3_flat_ellipsoid": ("smooth", "square", (0.0, 0.0), 3, (0.3, 0.15, 0.05), 0.0, 0.0, {}),
-    "smooth_fine_yaw": ("smooth", "fine_yaw", (0.0, 0.0), 2, (0.2, 0.1, 0.1), 0.0, 0.0, {}),
-    "smooth_coarse_tall_ellipsoid": ("smooth", "coarse", (0.0, 0.0), 2, (0.1, 0.1, 0.25), 0.0, 0.0, {"clamped_queries": 1}),
-    "slope68": ("slope68", "square", (0.0, 0.0), 2, (0.2, 0.1, 0.1), 0.0, 0.0, {}),
-    "slope68_it3": ("slope68", "square", (0.0, 0.0), 3, (0.2, 0.1, 0.1), 0.0, 0.0, {}),
-    "wall": ("wall", "square", (0.0, 0.0), 2, (0.2, 0.1, 0.1), 0.03, 0.0, {"nanc_it0": 1, "ties": 1, "empty_it1": 1}),
-    "wall_it3_tall_ellipsoid": ("wall", "coarse", (0.0, 0.0), 3, (0.1, 0.1, 0.25), 0.03, 0.0, {"nanc_it0": 1}),
-    "step": ("step", "square", (0.0, 0.0), 2, (0.2, 0.1, 0.1), 0.0, 0.0, {}),
-    "sparse": ("sparse", "square", (0.0, 0.0), 2, (0.2, 0.1, 0.1), 0.001, 0.001, {"degenerate_it0": 1}),
-    "very_sparse_it3": ("very_sparse", "coarse", (0.0, 0.0), 3, (0.3, 0.15, 0.05), 0.25, 0.24, {"n1": 1, "degenerate_it2": 1, "empty_it0": 1}),
-    "corner": ("corner", "square", (0.0, 0.0), 2, (0.2, 0.1, 0.1), 0.004, 0.003, {"clamped_queries": 1000, "far_nearest": 1000, "empty_it0": 1000, "n1": 1}),
-    "plane": ("plane", "square", (0.0, 0.0), 2, (0.2, 0.1, 0.1), 0.0, 0.0, {}),
-    "hole": ("hole", "square", (0.0, 0.0), 2, (0.2, 0.1, 0.1), 0.004, 0.003, {"empty_it0": 1}),
-    "smooth_off_centre": ("smooth", "square", (31.4, -17.25), 2, (0.2, 0.1, 0.1), 0.0, 0.0, {}),
-    "wall_far": ("wall", "fine_yaw", (300.0, 150.0), 2, (0.2, 0.1, 0.1), 0.035, 0.0, {"nanc_it0": 1}),
-    "corner_far": ("corner", "square", (300.0, 150.0), 3, (0.1, 0.1, 0.25), 0.006, 0.005, {"clamped_queries": 1000, "far_nearest": 1000}),
-}
-
-
-def scenario(name):
-    kind, gname, (cx, cy), iter_num, ell, share, plausible, reach = SCENARIOS[name]
-    pts = terrain(kind, cx, cy)
-    return dict(pts=pts, geom=grid(gname, cx, cy), iter_num=iter_num, ellipsoid=ell, share=share, plausible=plausible, reach=reach)
-
-
-_REF = {}
-
-
-def reference(name):
-    """(scenario, reference rows); the reference runs once per scenario and process"""
-    if name not in _REF:
-        s = scenario(name)
-        cen, cnt, _ = mref.preprocess(s["pts"], *_centre(s["geom"]))
-        assert cnt.max() == 1 and cen.shape[0] == s["pts"].shape[0]          # the cloud is its own preprocessing
-        _REF[name] = (s, mref.Reference(s["pts"], s["ellipsoid"], s["iter_num"]).build(s["geom"]))
-    return _REF[name]
-
-
-def _centre(g):
-    return (0.5 * (g.origin[0] + g.max_boundary[0]), 0.5 * (g.origin[1] + g.max_boundary[1]))
-
-
-def assert_matches_reference(cells, s, rows, label=""):
-    """the assertion every builder's grid is held to (the host builder here, the device builders in test_gpu_map_build_ref.py);
-    returns the cells that matched only a NaN-c variant"""
-    bad, nanc_only, dev = mref.compare(rows, cells)
-    f = rows["features"]
-    assert bad.size == 0, (label, bad.size, f, [(int(c), np.asarray(cells).reshape(-1, 4)[c]) for c in bad[:5]])
-    assert dev["z_ulp"] <= 1 and dev["zbx_ulp"] <= 1 and dev["zby_ulp"] <= 1 and dev["sigma_ulp"] <= 1, (label, dev)
-    assert max(dev["z_abs_small"], dev["zbx_abs_small"], dev["zby_abs_small"]) <= mref.VALUE_ABS, (label, dev)
-    assert dev["sigma_abs_small"] <= mref.SIGMA_ABS, (label, dev)
-    assert f["ambiguous"] <= s["share"] * f["cells"], (label, f)
-    assert f["plausible_only"] <= s["plausible"] * f["cells"], (label, f)
-    for k, least in s["reach"].items():
-        assert f[k] >= least, (label, k, f)
-    return nanc_only
-
-
-def _host(s, nthreads=0):
-    from uneven_planner_b200 import maps
-    return maps.build_from_cloud(s["pts"], s["geom"], ellipsoid=s["ellipsoid"], iter_num=s["iter_num"], nthreads=nthreads).cells
+from workloads import SCENARIOS, _host, assert_matches_reference, reference, scenario, terrain
 
 
 # cells of the wall scenario whose normal came out horizontal with zb.x^2 + zb.y^2 rounded above 1 after the first iteration, so
@@ -338,7 +207,7 @@ def test_float64_reference_against_the_reference_build(built, name):
     """where oracle/_ref/librefmap.so exists (the reference's own constructMap + filter), its cells are one of this reference's
     variants, and it writes the NaN-c cells the host builder writes, the same cells with the same values: if it wrote the wall's
     normal there instead, map_cell.h would be wrong on them.  Elsewhere it skips like the other pins of test_ref_pin.py."""
-    from test_ref_pin import reference_construct_map
+    from workloads import reference_construct_map
     s = scenario(name)
     geom, ref64 = reference_construct_map(s["pts"], 1.0, iter_num=s["iter_num"], ellipsoid=s["ellipsoid"])
     assert bytes(geom) == bytes(s["geom"])

@@ -12,39 +12,12 @@ What each comparison is:
   * the front end on `wide` and `tall`: properties of the returned paths only -- there is no second implementation to compare with
     where the reference's sources are absent."""
 import ctypes as C
-import functools
 import os
-import sys
 
 import numpy as np
 import pytest
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-
-# name: (size x, size y [m], xy resolution [m], yaw resolution [rad], cells, terrain seed: one whose bumps reach every edge)
-GRIDS = {
-    "wide": (12.0, 6.0, 0.05, 0.1, (240, 120, 64), 206),        # X > Y
-    "tall": (6.0, 12.0, 0.05, 0.1, (120, 240, 64), 211),        # X < Y, as many cells as `wide`
-    "coarse": (9.0, 7.0, 0.1, 0.2, (90, 70, 32), 206),          # other resolutions; only the yaw count is a multiple of 8
-    "fine_yaw": (7.3, 5.0, 0.04, 0.05, (183, 125, 127), 206),   # odd counts, ceil rounds up in x, an odd number of yaw layers
-    "site": (20.0, 10.0, 0.05, 0.1, (400, 200, 64), 206),       # the largest extent the builder's crop box keeps; 82 MB of float4
-}
-SMALL = ["wide", "tall", "coarse", "fine_yaw"]
-
-
-def geometry(name):
-    from uneven_planner_b200 import _lib
-    sx, sy, rxy, ryaw, _, _ = GRIDS[name]
-    return _lib.map_geometry(sx, sy, rxy, ryaw)
-
-
-@functools.lru_cache(maxsize=None)
-def grid(name):
-    """the `hills` terrain (the same bits on every host) on grid `name`"""
-    from uneven_planner_b200 import maps
-    m = maps.synthetic_terrain("hills", seed=GRIDS[name][5], geom=geometry(name))
-    m.name = name
-    return m
+from workloads import GRIDS, OUTSIDE, SMALL, _norm_so2, geometry, grid, in_map, query_poses, ref_query
 
 
 def test_grid_table(built):
@@ -73,105 +46,6 @@ def test_default_terrain_and_generator_keep_their_bits(built):
     assert a.shape == (200, 200, 64) and np.array_equal(a.cells.view(np.uint32), b.cells.view(np.uint32))
     p, q = problems.generate(a, 6, seed=5, lo=-4.0, hi=4.0), problems.generate(a, 6, seed=5, lo=(-4.0, -4.0), hi=(4.0, 4.0))
     assert np.array_equal(p.bnd, q.bnd) and np.array_equal(p.inner_xy, q.inner_xy) and np.array_equal(p.inner_yaw, q.inner_yaw)
-
-
-# ------------------------------------------------------------------ 1a. the oracle's map query against a plain reference
-def _norm_so2(a):
-    while a < -np.pi:
-        a += 2 * np.pi
-    while a > np.pi:
-        a -= 2 * np.pi
-    return a
-
-
-def in_map(geom, pos):
-    """UnevenMap::isInMap (uneven_map.h:437-454)"""
-    o, b = geom.origin, geom.max_boundary
-    return not (any(pos[k] < o[k] + 1e-4 for k in range(3)) or any(pos[k] > b[k] - 1e-4 for k in range(3)))
-
-
-def ref_query(cells, geom, pos):
-    """UnevenMap::getAllWithGrad in float64: cells is the [X, Y, W, 4] array, indexed as an array.  Returns (values[7], grads[7, 3])."""
-    X, Y, W = geom.voxel_num
-    rxy, ryaw = geom.xy_resolution, geom.yaw_resolution
-    ixy, iyaw = 1.0 / rxy, 1.0 / ryaw
-    org = np.array(list(geom.origin))
-    pos = np.asarray(pos, np.float64)
-    rs, rg = np.zeros(3), np.zeros((4, 3))
-    if in_map(geom, pos):
-        pm = pos - 0.5 * np.array([rxy, rxy, ryaw])
-        pm[2] = _norm_so2(pm[2])
-        inv = np.array([ixy, ixy, iyaw])
-        idx = np.floor((pm - org) * inv).astype(int)
-        centre = (idx + 0.5) * np.array([rxy, rxy, ryaw]) + org
-        d = (pos - centre) * inv
-        d[2] = np.arctan2(np.sin(pos[2] - centre[2]), np.cos(pos[2] - centre[2])) * iyaw
-        xs = np.clip([idx[0], idx[0] + 1], 0, X - 1)
-        ys = np.clip([idx[1], idx[1] + 1], 0, Y - 1)
-        ws = np.mod([idx[2], idx[2] + 1], W)
-        v = cells[np.ix_(xs, ys, ws)][..., 1:].astype(np.float64)          # [x, y, w, (sigma, zbx, zby)]
-        vx = v[0] * (1 - d[0]) + v[1] * d[0]                                # [y, w, 3]
-        vy = vx[0] * (1 - d[1]) + vx[1] * d[1]                              # [w, 3]
-        rs = vy[0] * (1 - d[2]) + vy[1] * d[2]
-        rg[:3, 2] = (vy[1] - vy[0]) * iyaw
-        dy = vx[1] - vx[0]                                                  # [w, 3]
-        rg[:3, 1] = (dy[0] * (1 - d[2]) + dy[1] * d[2]) * ixy
-        dx = v[1] - v[0]                                                    # [y, w, 3]
-        rg[:3, 0] = ((1 - d[2]) * (1 - d[1]) * dx[0, 0] + (1 - d[2]) * d[1] * dx[1, 0] + d[2] * (1 - d[1]) * dx[0, 1] + d[2] * d[1] * dx[1, 1]) * ixy
-        c = np.sqrt(1.0 - rs[1] ** 2 - rs[2] ** 2)
-        rg[3] = -(rg[1] * rs[1] + rg[2] * rs[2]) / c
-    c = np.sqrt(1.0 - rs[1] ** 2 - rs[2] ** 2)
-    inv_c = 1.0 / c
-    cy, sy = np.cos(pos[2]), np.sin(pos[2])
-    t = cy * rs[1] + sy * rs[2]
-    s = -(-sy * rs[1] + cy * rs[2])
-    q = np.sqrt(1.0 - t * t)
-    iq = 1.0 / q
-    iq3 = iq ** 3
-    dt = rg[1] * cy + rg[2] * sy
-    ds = -(rg[1] * -sy + rg[2] * cy)
-    dt[2] -= s
-    ds[2] += t
-    values = np.array([iq, -c * t * iq, q * inv_c, s * iq, c, inv_c, rs[0]])
-    grads = np.stack([t * iq3 * dt, -(t * iq * rg[3] + iq3 * c * dt), -inv_c * (t * iq * dt + q * inv_c * rg[3]), iq * ds + t * iq3 * s * dt,
-                      rg[3], -inv_c * inv_c * rg[3], rg[0]])
-    return values, grads
-
-
-OUTSIDE = np.array([1.0, 0.0, 1.0, 0.0, 1.0, 1.0, 0.0])      # zero terrain: flat ground, no roughness, zero gradients
-
-
-def query_poses(geom, n=2000, seed=0):
-    """seeded poses over the rectangle enlarged by 0.2 m, then the edges: the first and last cell of each axis, the four corners just
-    inside and just outside the 1e-4 margin, yaw at +-pi -+ 1e-6, at origin[2], and around the last yaw layer's centre, from where
-    the upper neighbour is layer 0"""
-    rng = np.random.default_rng(seed)
-    o, b = np.array(list(geom.origin)), np.array(list(geom.max_boundary))
-    W = geom.voxel_num[2]
-    rxy, ryaw = geom.xy_resolution, geom.yaw_resolution
-    pts = [np.column_stack([rng.uniform(o[0] - 0.2, b[0] + 0.2, n), rng.uniform(o[1] - 0.2, b[1] + 0.2, n), rng.uniform(-np.pi, np.pi, n)])]
-    mid = 0.5 * (o + b) + np.array([0.013, -0.017, 0.3])
-    edge = []
-    for k in range(2):
-        for f in (0.2, 0.7, 1.3):                       # below the first cell's centre (clamped), inside it, in the second
-            for at in (o[k] + f * rxy, b[k] - f * rxy):
-                p = mid.copy()
-                p[k] = at
-                edge.append(p)
-    for sx in (0, 1):
-        for sy in (0, 1):
-            for eps in (2e-4, 0.5e-4):                   # inside / outside the margin
-                x = o[0] + eps if sx == 0 else b[0] - eps
-                y = o[1] + eps if sy == 0 else b[1] - eps
-                edge.append(np.array([x, y, 0.4]))
-    last = _norm_so2(o[2] + (W - 0.5) * ryaw)
-    for yaw in (np.pi - 1e-6, -np.pi + 1e-6, o[2], o[2] + 2e-4, last, last - 0.3 * ryaw, last + 0.3 * ryaw, -np.pi + 0.3 * ryaw, np.pi - 0.3 * ryaw):
-        edge.append(np.array([mid[0], mid[1], yaw]))
-    for f in (0.3, 0.6):                                 # every layer pair once, the seam pair included
-        for w in range(W):
-            edge.append(np.array([mid[0], mid[1], _norm_so2(o[2] + (w + 0.5 + f) * ryaw)]))
-    pts.append(np.array(edge))
-    return np.vstack(pts)
 
 
 @pytest.mark.parametrize("name", list(GRIDS))
@@ -302,7 +176,7 @@ def test_host_builder_rectangle_shares_its_rows_with_the_square(built, axis):
     a cloud point on an ellipsoid's surface can change sides, which moves that cell's mean and covariance: up to 0.02 % of the cells
     may differ by more than 2 float ulps (the share tests/test_ref_pin.py allows at the rim of a hole).  Measured on an x86-64 host
     (the builder runs on host threads), both ways round: no cell of the 204 800 differs in any bit."""
-    from test_gpu_map_window import _cloud
+    from workloads import _cloud
     from uneven_planner_b200 import _lib, maps
     pts = _cloud(60000, 2.3, 0)
     size = [4.0, 4.0]
@@ -317,7 +191,6 @@ def test_host_builder_rectangle_shares_its_rows_with_the_square(built, axis):
     # and a wrong row offset or stride is not within that share: the neighbouring rows are nowhere near
     off = square.cells[21:61] if axis == 0 else square.cells[:, 21:61]
     assert (ulp_distance(rect.cells, off).max(axis=-1) > 2).mean() > 0.5
-
 
 
 # ------------------------------------------------------------------ 1e. the front end (a property test: no reference to compare with)
@@ -400,7 +273,7 @@ def test_front_end_goal_inside_one_rectangle_and_outside_the_other(built):
 @pytest.mark.parametrize("name", ["wide", "fine_yaw"])
 def test_reference_map_query_matches_oracle_bitwise_on_a_rectangle(built, name):
     """UnevenMap::getAllWithGrad of the reference build against orc_map_query, as tests/test_ref_pin.py does on the 10 m square"""
-    from test_ref_pin import REF
+    from workloads import REF
     import pyoracle as po
     if not os.path.exists(REF):
         pytest.skip("oracle/_ref/libref.so not present (built where the reference's sources exist)")

@@ -1,15 +1,13 @@
 """Grids at any origin and the host side of ualm_shift_map (no GPU): maps.shift_boxes / maps.shift_geometry, ualm_map_geometry_at,
 the .umap file of a grid that is not centred at the world origin, the host builder's crop box moved with the grid, and the oracle's
 map query on off-centre grids against the float64 numpy restatement of tests/test_map_geometry.py (1e-12 relative, in / out exact)."""
-import os
 import struct
-import sys
 
 import numpy as np
 import pytest
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from test_map_geometry import OUTSIDE, grid, in_map, query_poses, ref_query  # noqa: E402
+from workloads import OUTSIDE, _cloud_at, grid, in_map, query_poses, ref_query
+
 
 CENTRES = [(31.4, -17.25), (-100.0, 250.0), (300.0, 300.0)]
 
@@ -128,13 +126,6 @@ def test_umap_symmetric_grid_that_map_geometry_does_not_give_is_v2(built, tmp_pa
 
 def _zero_cells(g):
     return np.zeros(tuple(g.voxel_num) + (4,), np.float32)
-
-
-def _cloud_at(cx, cy, n=40000, half=2.2, seed=0):
-    rng = np.random.default_rng(seed)
-    xy = rng.uniform(-half, half, (n, 2))
-    z = 0.3 + 0.2 * np.sin(1.7 * xy[:, 0]) * np.cos(1.3 * xy[:, 1]) + rng.normal(0.0, 0.003, n)
-    return np.column_stack([xy[:, 0] + cx, xy[:, 1] + cy, z]).astype(np.float32)
 
 
 def test_host_builder_crops_about_the_grid_centre(built):

@@ -18,146 +18,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-dp = C.POINTER(C.c_double)
-DEV_GUARD = 4.0e6          # mpc_export_kernel scans only when total / dt < DEV_GUARD
-INIT_V = (0.7, -0.3, 0.25)   # every component distinct, and distinct from INIT_A's: a swapped index changes the result
-INIT_A = (-1.1, 0.4, -0.6)
-
-
-def _P(a):
-    return a.ctypes.data_as(dp)
-
-
-@pytest.fixture(scope="module")
-def orc(built):
-    import pyoracle as po
-    L = po.lib()
-    L.orc_minco_generate.argtypes = [C.c_int, C.c_int, dp, dp, dp, dp, dp]
-    return L
-
-
-# ------------------------------------------------------------------ the references
-def summed(dur, P):
-    """the duration of P pieces of `dur` as the kernel and PolyTrajectory::getTotalDuration form it: added one piece at a time"""
-    total = 0.0
-    for _ in range(P):
-        total += dur
-    return total
-
-
-def locate(P, dur, t):
-    """PolyTrajectory::locatePieceIdx (se2traj.hpp:343-361) for uniform durations, over an array of times: (piece index, local time)"""
-    t = np.array(t, dtype=np.float64, copy=True).reshape(-1)
-    idx = np.zeros(t.size, np.int64)
-    act = np.nonzero(t > dur)[0]
-    while act.size:
-        t[act] -= dur
-        idx[act] += 1
-        act = act[(idx[act] < P) & (t[act] > dur)]
-    last = idx == P
-    idx[last] -= 1
-    t[last] += dur
-    return idx, t
-
-
-def evaluate(c, P, dur, t):
-    """Piece::getValue (se2traj.hpp:106-118) of the P-piece spline with coefficients c (6 per piece, low -> high) at times t"""
-    idx, tl = locate(P, dur, t)
-    c6 = np.asarray(c, np.float64)[:6 * P].reshape(P, 6)[idx]
-    v = np.zeros(tl.size)
-    tn = np.ones(tl.size)
-    for k in range(6):
-        v = v + tn * c6[:, k]
-        tn = tn * tl
-    return v
-
-
-def message_ref(c_xy, c_yaw, N, M, Tx, Ty):
-    """the SE2Traj message of one planned trajectory: pos_pts (N + 1, 2), posT_pts (N), angle_pts (M + 1), angleT_pts (M)"""
-    c_xy, c_yaw = np.asarray(c_xy, np.float64), np.asarray(c_yaw, np.float64)
-    pos = np.empty((N + 1, 2))
-    pos[:N, 0], pos[:N, 1] = c_xy[0:6 * N:6], c_xy[6 * N::6]
-    end = summed(Tx, N)
-    pos[N, 0], pos[N, 1] = evaluate(c_xy[:6 * N], N, Tx, end)[0], evaluate(c_xy[6 * N:], N, Tx, end)[0]
-    ang = np.empty(M + 1)
-    ang[:M] = c_yaw[0::6]
-    ang[M] = evaluate(c_yaw, M, Ty, summed(Ty, M))[0]
-    return dict(pos_pts=pos, posT_pts=np.full(N, Tx), angle_pts=ang, angleT_pts=np.full(M, Ty))
-
-
-def minco(orc, pts, dur, v0, a0):
-    """orc_minco_generate over the points pts (P + 1, Dim) with uniform durations, head (pts[0], v0, a0), tail (pts[P], 0, 0):
-    the 6P x Dim coefficients, column-major"""
-    pts = np.asarray(pts, np.float64)
-    Pn, Dim = pts.shape[0] - 1, pts.shape[1]
-    head = np.ascontiguousarray(np.stack([pts[0], np.asarray(v0, np.float64), np.asarray(a0, np.float64)]))   # Dim x 3 column-major
-    tail = np.zeros((3, Dim))
-    tail[0] = pts[Pn]
-    inPs = np.ascontiguousarray(pts[1:Pn]).ravel()        # Dim x (P - 1) column-major == (P - 1) x Dim row-major
-    c = np.zeros(6 * Pn * Dim)
-    orc.orc_minco_generate(Dim, Pn, _P(inPs if inPs.size else np.zeros(1)), _P(np.full(Pn, float(dur))), _P(head.ravel()),
-                           _P(np.ascontiguousarray(tail).ravel()), _P(c))
-    return c
-
-
-def mpc_ref(orc, message, Tx, Ty, init_v=None, init_a=None):
-    """the MPC side's re-solve of a message (TrajAnalyzer::setTraj, traj_anal.hpp:125-181): (c_mpc_xy, c_mpc_yaw); init_v / init_a
-    = {x, y, yaw}, None = zero"""
-    v = np.zeros(3) if init_v is None else np.asarray(init_v, np.float64)
-    a = np.zeros(3) if init_a is None else np.asarray(init_a, np.float64)
-    cx = minco(orc, message["pos_pts"], Tx, v[:2], a[:2])
-    cy = minco(orc, np.asarray(message["angle_pts"]).reshape(-1, 1), Ty, v[2:], a[2:])
-    return cx, cy
-
-
-def scan_times(total, dt):
-    """the samples 0, dt, 2dt, .. by repeated addition (cumsum adds in order), kept while t < total"""
-    n = int(total / dt) + 64
-    while True:
-        t = np.cumsum(np.concatenate([[0.0], np.full(n - 1, dt)]))
-        if t[-1] >= total:
-            return t[:int(np.searchsorted(t, total, side="left"))]
-        n *= 2
-
-
-def first_max(vals, t):
-    """(largest value, its earliest sample time); (0, 0) when no value exceeds 0 (the kernel starts from 0 and keeps strict
-    increases, so a NaN is never kept)"""
-    hit = vals > 0.0
-    if not hit.any():
-        return 0.0, 0.0
-    m = vals[hit].max()
-    return float(m), float(t[int(np.argmax(vals == m))])
-
-
-def deviation_samples(c_xy, c_yaw, m_xy, m_yaw, N, M, Tx, Ty, dt):
-    """(sample times, position deviation, yaw deviation) of the scan, or None when the kernel does not scan"""
-    total_xy, total_yaw = summed(Tx, N), summed(Ty, M)
-    total = total_xy if total_xy < total_yaw else total_yaw
-    if not (total / dt < DEV_GUARD):
-        return None
-    t = scan_times(total, dt)
-    nx = 6 * N
-    dx = evaluate(c_xy[:nx], N, Tx, t) - evaluate(m_xy[:nx], N, Tx, t)
-    dy = evaluate(c_xy[nx:], N, Tx, t) - evaluate(m_xy[nx:], N, Tx, t)
-    ep = np.sqrt(dx * dx + dy * dy)
-    ey = np.abs(evaluate(c_yaw, M, Ty, t) - evaluate(m_yaw, M, Ty, t))
-    return t, ep, ey
-
-
-def dev_ref(c_xy, c_yaw, m_xy, m_yaw, N, M, Tx, Ty, dt):
-    """dev4 of one problem: {max position deviation, its time, max yaw deviation, its time}"""
-    s = deviation_samples(c_xy, c_yaw, m_xy, m_yaw, N, M, Tx, Ty, dt)
-    if s is None:
-        return np.array([-1.0, 0.0, -1.0, 0.0])
-    t, ep, ey = s
-    return np.array(first_max(ep, t) + first_max(ey, t))
-
-
-def scan_length(N, M, Tx, Ty, dt):
-    """total / dt as the kernel's guard forms it"""
-    a, b = summed(Tx, N), summed(Ty, M)
-    return (a if a < b else b) / dt
+from workloads import DEV_GUARD, INIT_A, INIT_V, dev_ref, evaluate, first_max, message_ref, minco, mpc_ref, orc, summed
 
 
 # ------------------------------------------------------------------ the references against plain loops

@@ -13,13 +13,7 @@ import os
 import numpy as np
 import pytest
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "oracle", "_ref", "libref.so")
-dp = C.POINTER(C.c_double)
-
-
-def P(a):
-    return None if a is None else a.ctypes.data_as(dp)
+from workloads import P, REF, ROOT, RefParams, _ref_solve, analytic_cloud, dp, preprocessed, reference_construct_map
 
 
 @pytest.fixture(scope="module")
@@ -108,37 +102,6 @@ def test_lbfgs_header_matches_oracle_bitwise(ref, orc, n, mem, past):
     assert rr == ro and ir.value == io.value
     assert fr[0] == fo[0] and np.array_equal(xr, xo)
     assert fr[0] < 1e-6 and np.allclose(xr, 1.0, atol=1e-2)
-
-
-# ---------------------------------------------------------------------------------------------------------------------
-# the whole path: ALMTrajOpt::optimizeSE2Traj of back_end/src/alm_traj_opt.cpp (unmodified) vs the oracle
-# ---------------------------------------------------------------------------------------------------------------------
-class RefParams(C.Structure):
-    _fields_ = [(n, C.c_double) for n in ("rho_T", "rho_ter", "max_vel", "max_acc_lon", "max_acc_lat", "max_kap", "min_cxi", "max_sig")] + \
-               [("use_scaling", C.c_int)] + \
-               [(n, C.c_double) for n in ("rho", "beta", "gamma", "epsilon_con", "max_iter", "g_epsilon", "min_step", "inner_max_iter", "delta")] + \
-               [("mem_size", C.c_int), ("past", C.c_int), ("int_K", C.c_int), ("gravity", C.c_double)]
-
-
-def _ref_solve(L, params, mapdata, pb, i):
-    g = mapdata.geom
-    rp = RefParams()
-    for n, _ in RefParams._fields_:
-        setattr(rp, n, getattr(params, n))
-    cells = np.ascontiguousarray(mapdata.cells, dtype=np.float64)
-    N, M = int(pb.N[i]), int(pb.M[i])
-    S = N * (params.int_K + 1)
-    oxy, oyaw, _, _ = pb.offsets()
-    ixy = np.ascontiguousarray(pb.inner_xy[oxy[i]:oxy[i + 1]]); iyaw = np.ascontiguousarray(pb.inner_yaw[oyaw[i]:oyaw[i + 1]])
-    out = dict(c_xy=np.zeros(12 * N), c_yaw=np.zeros(6 * M), piece_T=np.zeros(2), lam=np.zeros(S), mu=np.zeros(6 * S), hx=np.zeros(S),
-               gx=np.zeros(6 * S), sfx=np.zeros(1), scx=np.zeros(7 * S), rho=np.zeros(1), feas=np.zeros(7))
-    vn = (C.c_int * 3)(*g.voxel_num); org = (C.c_double * 3)(*g.origin); mxb = (C.c_double * 3)(*g.max_boundary)
-    L.ref_alm_solve.restype = C.c_int
-    ret = L.ref_alm_solve(C.byref(rp), P(cells), vn, org, mxb, C.c_double(g.xy_resolution), C.c_double(g.yaw_resolution), N, M,
-                          P(np.ascontiguousarray(pb.bnd[i])), C.c_double(float(pb.total_time[i])), P(ixy if ixy.size else np.zeros(1)),
-                          P(iyaw if iyaw.size else np.zeros(1)), 0, P(out["c_xy"]), P(out["c_yaw"]), P(out["piece_T"]), P(out["lam"]), P(out["mu"]),
-                          P(out["hx"]), P(out["gx"]), P(out["sfx"]), P(out["scx"]), P(out["rho"]), P(out["feas"]))
-    return ret, out
 
 
 @pytest.mark.parametrize("which,use_scaling", [("bumps", 1), ("bumps", 0), ("hill", 1), ("volcano", 1), ("forest", 0)])
@@ -366,51 +329,6 @@ def test_reference_map_query_matches_oracle_bitwise(ref, built, request):
                 assert np.array_equal(vr, vo) and np.array_equal(gr, go), pnt
         finally:
             ref.ref_map_destroy(h)
-
-
-# ---------------------------------------------------------------- UnevenMap construction (SURVEY 8f-1)
-REFMAP = os.path.join(ROOT, "oracle", "_ref", "librefmap.so")
-
-
-def reference_construct_map(cloud, size, iter_num=2, ellipsoid=(0.2, 0.1, 0.1)):
-    """UnevenMap::constructMap + filter of the reference's uneven_map.cpp (compiled unmodified, oracle/ref_map_driver.cpp) on an already
-    preprocessed cloud: cells [X, Y, Yaw, 4] in double."""
-    from uneven_planner_b200 import _lib
-    if not os.path.exists(REFMAP):
-        pytest.skip("oracle/_ref/librefmap.so not built (needs the reference sources at build time)")
-    R = C.CDLL(REFMAP)
-    geom = _lib.map_geometry(size, size, 0.05, 0.1)
-    X, Y, W = geom.voxel_num
-    cells = np.zeros((X * Y * W, 4))
-    vn = (C.c_int * 3)()
-    cloud = np.ascontiguousarray(cloud, dtype=np.float32)
-    R.ref_map_construct(cloud.ctypes.data_as(C.POINTER(C.c_float)), int(cloud.shape[0]), C.c_double(size), C.c_double(size), C.c_double(0.05), C.c_double(0.1),
-                        C.c_double(ellipsoid[0]), C.c_double(ellipsoid[1]), C.c_double(ellipsoid[2]), int(iter_num), cells.ctypes.data_as(C.POINTER(C.c_double)), vn)
-    assert tuple(vn) == (X, Y, W)
-    return geom, cells.reshape(X, Y, W, 4)
-
-
-def analytic_cloud(half, n, seed, hole=None):
-    """jittered grid on an analytic surface with noise (and an optional empty patch)"""
-    rng = np.random.default_rng(seed)
-    gx, gy = np.meshgrid(np.linspace(-half, half, n), np.linspace(-half, half, n), indexing="ij")
-    px = (gx + rng.uniform(-0.008, 0.008, gx.shape)).ravel(); py = (gy + rng.uniform(-0.008, 0.008, gy.shape)).ravel()
-    pz = 0.5 + 0.3 * np.sin(1.3 * px) * np.cos(0.9 * py) + 0.15 * np.exp(-((px - 0.5) ** 2 + (py + 0.3) ** 2) / 0.18) + rng.normal(0, 0.003, px.shape)
-    pts = np.column_stack([px, py, pz]).astype(np.float32)
-    if hole is not None:
-        pts = pts[~((np.abs(pts[:, 0] - hole[0]) < hole[2]) & (np.abs(pts[:, 1] - hole[1]) < hole[2]))]
-    return pts
-
-
-def preprocessed(pts, ellipsoid=(0.2, 0.1, 0.1)):
-    """the cloud the builders work on (UnevenMap::init's CropBox + VoxelGrid, through the host tool)"""
-    from uneven_planner_b200 import _lib
-    L = _lib.lib()
-    fp = C.POINTER(C.c_float)
-    out = np.zeros((pts.shape[0], 3), np.float32)
-    k = L.ualm_map_preprocess_cloud(pts.ctypes.data_as(fp), pts.shape[0], ellipsoid[0], ellipsoid[1], ellipsoid[2], out.ctypes.data_as(fp), pts.shape[0])
-    assert k > 0
-    return np.ascontiguousarray(out[:k])
 
 
 def test_reference_constructMap_matches_host_builder(built):

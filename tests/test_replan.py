@@ -6,9 +6,7 @@ import pytest
 
 import replan_oracle as ro
 
-
-def _bits(a):
-    return np.ascontiguousarray(a, np.float64).view(np.uint64)
+from harness import bits
 
 
 def _same_resample(path, rp=ro.DEFAULT_RP):
@@ -16,9 +14,9 @@ def _same_resample(path, rp=ro.DEFAULT_RP):
     N, M, bnd, T, ixy, iyaw = problems.resample(path, *rp)
     N2, M2, T2, ixy2, iyaw2, sm = ro.resample(path, rp)
     assert (N, M) == (N2, M2)
-    assert _bits([T]) == _bits([T2])
-    assert np.array_equal(_bits(ixy), _bits(ixy2)) and np.array_equal(_bits(iyaw), _bits(iyaw2))
-    assert _bits([bnd[12], bnd[15]]).tolist() == _bits([sm[0, 2], sm[-1, 2]]).tolist()   # first yaw as given, last one smoothed
+    assert bits([T]) == bits([T2])
+    assert np.array_equal(bits(ixy), bits(ixy2)) and np.array_equal(bits(iyaw), bits(iyaw2))
+    assert bits([bnd[12], bnd[15]]).tolist() == bits([sm[0, 2], sm[-1, 2]]).tolist()   # first yaw as given, last one smoothed
 
 
 @pytest.fixture(scope="module")
@@ -77,9 +75,9 @@ def test_polyline_times_are_the_check_sequence(trajs):
             for t_from in (0.0, t_k, 0.5 * Tx, 2.0 * Tx, seq[-1], 0.37 * seq[-1] + 0.0031):
                 pts, ts, head = ro.polyline(N, M, cxy, cyaw, Tx, Ty, bnd, t_from, dt)
                 assert ts[0] == t_from and ts[-1] == -1.0
-                assert np.array_equal(_bits(ts[1:-1]), _bits(seq[seq > t_from]))
+                assert np.array_equal(bits(ts[1:-1]), bits(seq[seq > t_from]))
                 assert np.array_equal(pts[-1], [bnd[6], bnd[7], bnd[15]])
-                assert _bits(pts[0]).tolist() == _bits(head[[0, 1, 6]]).tolist()
+                assert bits(pts[0]).tolist() == bits(head[[0, 1, 6]]).tolist()
                 row = ro.replan(N, M, cxy, cyaw, Tx, Ty, bnd, t_from, dt)
                 assert np.array_equal(row[:6], head[:6]) and np.array_equal(row[12:15], head[6:9])
                 assert np.array_equal(row[6:12], bnd[6:12]) and np.array_equal(row[15:18], bnd[15:18])
