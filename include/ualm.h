@@ -56,6 +56,24 @@ typedef struct {
 /* run_hill.yaml defaults (plan_manager/params/run_hill.yaml:30-55) */
 void ualm_default_params(ualm_params_t *p);
 
+/* ---- per-problem parameters: what describes one vehicle and one request ----
+ * The first eight members of ualm_params_t, in its order: the two cost weights (rho_T, time against smoothness; rho_ter, the sigma^2
+ * terrain cost) and the six limits.  None of them shapes a buffer or a shared-memory layout, so every problem of a batch may carry its
+ * own row.  int_K, mem_size, past, use_scaling, gravity and the ALM / L-BFGS settings stay per environment.
+ * The *_pp entry points take their *_env counterpart's arguments plus pp[B] (NULL = every problem uses its environment's values; each
+ * *_env entry point is its *_pp form with pp = NULL).  Contract:
+ *   bits:      problem b with row pp[b] gives, bit for bit, the record and coefficients the same problem gets in a batch of an
+ *              environment whose ualm_params_t is env[b]'s with these eight fields replaced, at every precision; at precision 64 that is
+ *              the CPU oracle's solve with those parameters;
+ *   phases:    ualm_eval_batch, ualm_init_scaling_batch and ualm_time_penalty_kernel on a batch uploaded with rows use each problem's
+ *              row; ualm_feasibility_batch and ualm_mpc_export_batch read no limit and do not change;
+ *   tickets:   polls, cancels, the budget, deadlines, urgency, map updates and the lane ring act as on any ticket;
+ *   refusals:  a non-finite field in any row is UALM_EINVAL, decided before anything is touched: nothing is written and no lane is
+ *              taken.  Every other refusal is the *_env form's. */
+typedef struct {
+    double rho_T, rho_ter, max_vel, max_acc_lon, max_acc_lat, max_kap, min_cxi, max_sig;
+} ualm_problem_params_t;
+
 /* ---- environment: what ALMTrajOpt reads of UnevenMap (uneven_map.h:258-377, 398-454) ---- */
 typedef struct {
     int    voxel_num[3];     /* X, Y, Yaw cells (uneven_map.cpp:108-110) */
@@ -219,6 +237,12 @@ int ualm_upload_env(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, 
 int ualm_solve_batch_env(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
                          const double *inner_xy, const double *inner_yaw, const int32_t *env, ualm_result_t *results, double *c_xy,
                          double *c_yaw);
+/* ... with a parameter row per problem (ualm_problem_params_t above) */
+int ualm_upload_pp(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
+                   const double *inner_xy, const double *inner_yaw, const int32_t *env, const ualm_problem_params_t *pp);
+int ualm_solve_batch_pp(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
+                        const double *inner_xy, const double *inner_yaw, const int32_t *env, const ualm_problem_params_t *pp,
+                        ualm_result_t *results, double *c_xy, double *c_yaw);
 int ualm_solve_resident(ualm_ctx_t *ctx);
 int ualm_sync(ualm_ctx_t *ctx);
 int ualm_download(ualm_ctx_t *ctx, ualm_result_t *results, double *c_xy, double *c_yaw);
@@ -243,6 +267,9 @@ int ualm_submit_batch(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M
                       const double *inner_xy, const double *inner_yaw, int depth, int *ticket);
 int ualm_submit_batch_env(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
                           const double *inner_xy, const double *inner_yaw, const int32_t *env, int depth, int *ticket);
+int ualm_submit_batch_pp(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
+                         const double *inner_xy, const double *inner_yaw, const int32_t *env, const ualm_problem_params_t *pp, int depth,
+                         int *ticket);
 int ualm_wait_batch(ualm_ctx_t *ctx, int ticket, ualm_result_t *results, double *c_xy, double *c_yaw);
 /* ualm_wait_batch with a deadline: if the batch is not complete timeout_ms after the call, every problem of the batch is cancelled
  * as by ualm_cancel_problems (the problems still running stop at their next stop test with UALM_RET_STOPPED), the batch drains
@@ -315,6 +342,10 @@ int ualm_solve_batch_multi(ualm_ctx_t **ctxs, int nctx, int B, const int32_t *N,
 int ualm_solve_batch_multi_env(ualm_ctx_t **ctxs, int nctx, int B, const int32_t *N, const int32_t *M, const double *bnd,
                                const double *total_time, const double *inner_xy, const double *inner_yaw, const int32_t *env,
                                ualm_result_t *results, double *c_xy, double *c_yaw);
+/* pp rows are dealt with their problems */
+int ualm_solve_batch_multi_pp(ualm_ctx_t **ctxs, int nctx, int B, const int32_t *N, const int32_t *M, const double *bnd,
+                              const double *total_time, const double *inner_xy, const double *inner_yaw, const int32_t *env,
+                              const ualm_problem_params_t *pp, ualm_result_t *results, double *c_xy, double *c_yaw);
 
 /* Fixed-stride result records for the multi-GPU all-gather: writes B records of `stride` doubles into
  * a DEVICE buffer (e.g. a torch tensor): [ret, outer, evals, iters, cost, jerk, T, res_h, res_g, N, M, pad,
@@ -379,6 +410,12 @@ typedef struct { double max_vel, max_acc_lon, max_acc_lat, max_kap, min_cxi, max
 int ualm_check_trajectories(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *piece_T, const double *c_xy,
                             const double *c_yaw, const int32_t *env, const double *t_from, double dt, const ualm_limits_t *limits,
                             double *out16);
+/* The same with a parameter row per trajectory: row b's six limits are `limits` when that is non-NULL (call-wide, as above), otherwise
+ * pp[b]'s, otherwise its environment's.  Gravity stays the environment's.  A non-finite field of pp is UALM_EINVAL (with out16 not
+ * written), also when `limits` is given. */
+int ualm_check_trajectories_pp(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *piece_T, const double *c_xy,
+                               const double *c_yaw, const int32_t *env, const ualm_problem_params_t *pp, const double *t_from, double dt,
+                               const ualm_limits_t *limits, double *out16);
 
 /* Hand-over to the MPC for the solved batch of the selected lane, on the device (SURVEY 8f-3):
  *   (1) the mpc_controller/SE2Traj message PlanManager publishes (plan_manager.cpp:151-185, msg/SE2Traj.msg:1-9): pos_pts = the
@@ -494,6 +531,13 @@ int ualm_submit_replan(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *
                        const double *c_yaw, const double *bnd, const int32_t *env, const double *t_from, double dt,
                        const ualm_resample_params_t *rp, int depth, int *ticket, int32_t *N_out, int32_t *M_out, double *bnd_out,
                        double *total_time_out, double *inner_xy_out, double *inner_yaw_out);
+/* The same with a parameter row per trajectory: row b of the ticket solves with pp[b] (ualm_submit_batch_pp of the returned arrays).
+ * The build reads no parameter and gives the same bits.  A non-finite field of pp is refused with the refusals decided before the
+ * build. */
+int ualm_submit_replan_pp(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *piece_T, const double *c_xy,
+                          const double *c_yaw, const double *bnd, const int32_t *env, const ualm_problem_params_t *pp, const double *t_from,
+                          double dt, const ualm_resample_params_t *rp, int depth, int *ticket, int32_t *N_out, int32_t *M_out,
+                          double *bnd_out, double *total_time_out, double *inner_xy_out, double *inner_yaw_out);
 
 /* KinoAstar::plan(start_state, end_state) (front_end/src/kino_astar.cpp:67-236): hybrid A* over (x, y, yaw) with 3 x 5 motion
  * primitives and a Dubins one-shot near the goal.  Writes the (x, y, yaw) polyline start .. goal and returns its number of points;

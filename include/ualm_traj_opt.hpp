@@ -257,6 +257,12 @@ public:
     {
         check(ualm_solve_batch_env(ctx_, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, results, c_xy, c_yaw), "ualm_solve_batch_env");
     }
+    // ... and each problem's own vehicle limits and cost weights (pp[B], nullptr = its environment's; ualm_problem_params_t)
+    void optimizeBatch(int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time, const double *inner_xy,
+                       const double *inner_yaw, const int32_t *env, const ualm_problem_params_t *pp, ualm_result_t *results, double *c_xy, double *c_yaw)
+    {
+        check(ualm_solve_batch_pp(ctx_, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, pp, results, c_xy, c_yaw), "ualm_solve_batch_pp");
+    }
 
     // pipelined form: submit returns once the batch is uploaded and queued (up to `depth` batches in flight), wait collects it
     int submitBatch(int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time, const double *inner_xy,
@@ -271,6 +277,13 @@ public:
     {
         int ticket = -1;
         check(ualm_submit_batch_env(ctx_, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, depth, &ticket), "ualm_submit_batch_env");
+        return ticket;
+    }
+    int submitBatch(int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time, const double *inner_xy,
+                    const double *inner_yaw, const int32_t *env, const ualm_problem_params_t *pp, int depth)
+    {
+        int ticket = -1;
+        check(ualm_submit_batch_pp(ctx_, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, pp, depth, &ticket), "ualm_submit_batch_pp");
         return ticket;
     }
     void waitBatch(int ticket, ualm_result_t *results, double *c_xy, double *c_yaw) { check(ualm_wait_batch(ctx_, ticket, results, c_xy, c_yaw), "ualm_wait_batch"); }
@@ -313,6 +326,12 @@ public:
     {
         check(ualm_check_trajectories(ctx_, B, N, M, piece_T, c_xy, c_yaw, env, t_from, dt, limits, out16), "ualm_check_trajectories");
     }
+    // the same with each trajectory's own limits from its row pp[b] where `limits` is null (ualm_check_trajectories_pp)
+    void checkTrajectories(int B, const int32_t *N, const int32_t *M, const double *piece_T, const double *c_xy, const double *c_yaw, const int32_t *env,
+                           const ualm_problem_params_t *pp, const double *t_from, double dt, const ualm_limits_t *limits, double *out16)
+    {
+        check(ualm_check_trajectories_pp(ctx_, B, N, M, piece_T, c_xy, c_yaw, env, pp, t_from, dt, limits, out16), "ualm_check_trajectories_pp");
+    }
 
     // Replans B trajectories the caller holds (as for checkTrajectories, plus each one's original problem row bnd, 18 doubles) from the
     // state at t_from[b] to the original goal, and submits the built problems as one ticket (ualm_submit_replan; wait on it with
@@ -325,6 +344,16 @@ public:
         int ticket = -1;
         check(ualm_submit_replan(ctx_, B, N, M, piece_T, c_xy, c_yaw, bnd, env, t_from, dt, rp, depth, &ticket, N_out, M_out, bnd_out, total_time_out,
                                  inner_xy_out, inner_yaw_out), "ualm_submit_replan");
+        return ticket;
+    }
+    // the same with row b of the ticket solved with pp[b] (ualm_submit_replan_pp)
+    int submitReplan(int B, const int32_t *N, const int32_t *M, const double *piece_T, const double *c_xy, const double *c_yaw, const double *bnd,
+                     const int32_t *env, const ualm_problem_params_t *pp, const double *t_from, double dt, const ualm_resample_params_t *rp, int depth,
+                     int32_t *N_out, int32_t *M_out, double *bnd_out, double *total_time_out, double *inner_xy_out = nullptr, double *inner_yaw_out = nullptr)
+    {
+        int ticket = -1;
+        check(ualm_submit_replan_pp(ctx_, B, N, M, piece_T, c_xy, c_yaw, bnd, env, pp, t_from, dt, rp, depth, &ticket, N_out, M_out, bnd_out,
+                                    total_time_out, inner_xy_out, inner_yaw_out), "ualm_submit_replan_pp");
         return ticket;
     }
 

@@ -7,6 +7,8 @@ return UALM_ENOCUDA (raised as RuntimeError) when no CUDA device is usable.
 import ctypes as C
 import os
 
+import numpy as np
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libualm.so")
 
@@ -23,6 +25,14 @@ class Params(C.Structure):
                [(n, C.c_double) for n in ("rho", "beta", "gamma", "epsilon_con", "max_iter",
                                           "g_epsilon", "min_step", "inner_max_iter", "delta")] + \
                [("mem_size", C.c_int), ("past", C.c_int), ("int_K", C.c_int), ("gravity", C.c_double)]
+
+
+PROBLEM_FIELDS = ("rho_T", "rho_ter", "max_vel", "max_acc_lon", "max_acc_lat", "max_kap", "min_cxi", "max_sig")
+
+
+class ProblemParams(C.Structure):
+    """ualm_problem_params_t: the first eight members of Params, one row per problem (include/ualm.h)"""
+    _fields_ = [(n, C.c_double) for n in PROBLEM_FIELDS]
 
 
 class MapGeom(C.Structure):
@@ -149,6 +159,17 @@ def lib():
         L.ualm_check_trajectories.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, ip, dp, C.c_double, C.POINTER(Limits), dp]
         L.ualm_submit_replan.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, dp, ip, dp, C.c_double, C.POINTER(ResampleParams), C.c_int,
                                          C.POINTER(C.c_int), ip, ip, dp, dp, dp, dp]
+        pp = C.POINTER(ProblemParams)
+        L.ualm_upload_pp.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, dp, ip, pp]
+        L.ualm_solve_batch_pp.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, dp, ip, pp, C.POINTER(Result), dp, dp]
+        L.ualm_submit_batch_pp.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, dp, ip, pp, C.c_int, C.POINTER(C.c_int)]
+        L.ualm_solve_batch_multi_pp.argtypes = [C.POINTER(vp), C.c_int, C.c_int, ip, ip, dp, dp, dp, dp, ip, pp, C.POINTER(Result), dp, dp]
+        L.ualm_check_trajectories_pp.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, ip, pp, dp, C.c_double, C.POINTER(Limits), dp]
+        L.ualm_submit_replan_pp.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, dp, ip, pp, dp, C.c_double, C.POINTER(ResampleParams), C.c_int,
+                                            C.POINTER(C.c_int), ip, ip, dp, dp, dp, dp]
+        for name in ("ualm_upload_pp", "ualm_solve_batch_pp", "ualm_submit_batch_pp", "ualm_solve_batch_multi_pp", "ualm_check_trajectories_pp",
+                     "ualm_submit_replan_pp"):
+            getattr(L, name).restype = C.c_int
         for name in ("ualm_reset_stream", "ualm_set_map_f64", "ualm_max_lanes", "ualm_select_lane", "ualm_submit_batch", "ualm_wait_batch",
                      "ualm_wait_batch_for", "ualm_poll_batch", "ualm_cancel_problems", "ualm_set_budget", "ualm_set_urgent",
                      "ualm_mark_begin", "ualm_mark_end", "ualm_solve_batch_multi", "ualm_pack_records_device_async", "ualm_select_env",
@@ -169,6 +190,12 @@ def default_params():
     p = Params()
     lib().ualm_default_params(C.byref(p))
     return p
+
+
+def problem_params(params):
+    """The row ProblemBatch.params takes for a vehicle described by `params` (a Params, or any object with its eight per-problem
+    fields): float64 [8] in ualm_problem_params_t's order."""
+    return np.array([float(getattr(params, n)) for n in PROBLEM_FIELDS], np.float64)
 
 
 def map_geometry(size_x=10.0, size_y=10.0, xy_res=0.05, yaw_res=0.1):

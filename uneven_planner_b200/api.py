@@ -6,6 +6,8 @@
     optimize(problems)      <- B x ALMTrajOpt::optimizeSE2Traj(...) (alm_traj_opt.h:92-98), then getTraj()
 A context holds up to UALM_MAX_ENVS environments (parameter set + map grid): init(params, env=k) / set_environment(map, env=k)
 bind environment k, and a batch whose `env` array is set solves every problem in its own environment (ProblemBatch.env).
+A batch whose `params` rows are set solves every problem with its own vehicle limits and cost weights (ProblemBatch.params,
+_lib.problem_params); everything else comes from its environment.
 All compute happens inside libualm.so on the GPU; this file only marshals numpy arrays.
 """
 import contextlib
@@ -27,6 +29,20 @@ def _p(a, t=dp):
 def _env(pb):
     """int32 environment index per problem, or None (= all environment 0)"""
     return None if getattr(pb, "env", None) is None else np.ascontiguousarray(pb.env, np.int32)
+
+
+def _pp(pb):
+    """float64 [B, 8] parameter rows (ualm_problem_params_t), or None (= every problem uses its environment's)"""
+    pp = getattr(pb, "params", None)
+    if pp is None:
+        return None
+    pp = np.ascontiguousarray(pp, np.float64)
+    if pp.shape != (pb.B, 8):
+        raise ValueError("params must be float64 [B, 8] = [%d, 8], got %r" % (pb.B, pp.shape))
+    return pp
+
+
+ppp = C.POINTER(_lib.ProblemParams)
 
 
 class UalmError(RuntimeError):
@@ -258,13 +274,13 @@ class BatchALMTrajOpt:
                                                         pb.inner_yaw.astype(np.float64))]
         N, M, bnd, T, ixy, iyaw = host
         t = C.c_int(-1)
-        env = _env(pb)
+        env, pp = _env(pb), _pp(pb)
         with self._urgency(urgent):
-            _check(self.L.ualm_submit_batch_env(self.h, pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), _p(env, ip), int(depth),
-                                                C.byref(t)))
+            _check(self.L.ualm_submit_batch_pp(self.h, pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), _p(env, ip), _p(pp, ppp),
+                                               int(depth), C.byref(t)))
         if not hasattr(self, "_tickets"):
             self._tickets = {}
-        self._tickets[t.value] = (pb, (host, env))
+        self._tickets[t.value] = (pb, (host, env, pp))
         return t.value
 
     def wait(self, ticket, out=None, timeout_ms=None):
@@ -334,9 +350,9 @@ class BatchALMTrajOpt:
         self._keep = [np.ascontiguousarray(a) for a in (pb.N.astype(np.int32), pb.M.astype(np.int32), pb.bnd.astype(np.float64),
                                                         pb.total_time.astype(np.float64), pb.inner_xy.astype(np.float64),
                                                         pb.inner_yaw.astype(np.float64))]
-        self._keep.append(_env(pb))
-        N, M, bnd, T, ixy, iyaw, env = self._keep
-        _check(self.L.ualm_upload_env(self.h, pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), _p(env, ip)))
+        self._keep += [_env(pb), _pp(pb)]
+        N, M, bnd, T, ixy, iyaw, env, pp = self._keep
+        _check(self.L.ualm_upload_pp(self.h, pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), _p(env, ip), _p(pp, ppp)))
 
     def solve_resident(self):
         _check(self.L.ualm_solve_resident(self.h))
@@ -366,9 +382,9 @@ class BatchALMTrajOpt:
         res = (Result * pb.B)()
         cxy = np.zeros(int(12 * N.astype(np.int64).sum()))
         cyaw = np.zeros(int(6 * M.astype(np.int64).sum()))
-        env = _env(pb)
-        _check(self.L.ualm_solve_batch_env(self.h, pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), _p(env, ip), res, _p(cxy),
-                                           _p(cyaw)))
+        env, pp = _env(pb), _pp(pb)
+        _check(self.L.ualm_solve_batch_pp(self.h, pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), _p(env, ip), _p(pp, ppp), res,
+                                          _p(cxy), _p(cyaw)))
         return res, cxy, cyaw
 
     def pack_records(self, dev_ptr, stride, wait=True):
@@ -433,12 +449,13 @@ class BatchALMTrajOpt:
         _check(self.L.ualm_feasibility_batch(self.h, float(dt), out.ctypes.data_as(C.POINTER(C.c_double))))
         return out
 
-    def check_trajectories(self, N, M, piece_T, c_xy, c_yaw, env=None, t_from=None, dt=0.01, limits=None):
+    def check_trajectories(self, N, M, piece_T, c_xy, c_yaw, env=None, t_from=None, dt=0.01, limits=None, params=None):
         """ualm_check_trajectories: the post-solve scan of trajectories the caller holds, against each environment's grid as it is now,
         over the samples t >= t_from of the full scan, with the time each limit is first broken.  N, M: [B]; piece_T: [B, 2]
         (piece_T_xy, piece_T_yaw of the records); c_xy / c_yaw packed as wait() returns them; env: [B] or None (all 0); t_from: [B],
         one number or None (0); limits: None (each environment's own), six numbers (max_vel, max_acc_lon, max_acc_lat, max_kap,
-        min_cxi, max_sig) or an object with those attributes, e.g. Params.  May be called while batches are in flight.
+        min_cxi, max_sig) or an object with those attributes, e.g. Params; params: None or [B, 8] parameter rows, whose limits each
+        row takes where `limits` is None (ualm_check_trajectories_pp).  May be called while batches are in flight.
         Returns [B, 16]: ualm_feasibility_batch's ten columns over the kept samples, then the six first-violation times (-1: none)."""
         N = np.ascontiguousarray(N, np.int32).reshape(-1)
         M = np.ascontiguousarray(M, np.int32).reshape(-1)
@@ -461,25 +478,30 @@ class BatchALMTrajOpt:
             if len(vals) != 6:
                 raise ValueError("check_trajectories: limits must be six numbers %s" % (names,))
             lim = _lib.Limits(*[float(v) for v in vals])
+        pp = None if params is None else np.ascontiguousarray(params, np.float64)
+        if pp is not None and pp.shape != (B, 8):
+            raise ValueError("check_trajectories: params must be [B, 8] = [%d, 8], got %r" % (B, pp.shape))
         out = np.zeros((B, 16))
-        _check(self.L.ualm_check_trajectories(self.h, B, _p(N, ip), _p(M, ip), _p(pt), _p(cxy), _p(cyaw), _p(e, ip), _p(tf), float(dt),
-                                              None if lim is None else C.byref(lim), _p(out)))
+        _check(self.L.ualm_check_trajectories_pp(self.h, B, _p(N, ip), _p(M, ip), _p(pt), _p(cxy), _p(cyaw), _p(e, ip), _p(pp, ppp), _p(tf),
+                                                 float(dt), None if lim is None else C.byref(lim), _p(out)))
         return out
 
     def check_results(self, pb, out, t_from=None, dt=0.01, limits=None, urgent=False):
         """check_trajectories of batch `pb` as wait() / poll() returned it: out = (results, c_xy, c_yaw).  A record poll() has not
-        filled yet has zero durations and keeps no sample.  urgent: the check goes ahead of the batches in flight (ualm_set_urgent)."""
+        filled yet has zero durations and keeps no sample.  The limits are `limits` when given, else the batch's parameter rows', else each
+        environment's.  urgent: the check goes ahead of the batches in flight (ualm_set_urgent)."""
         res, cxy, cyaw = out
         pt = np.array([(r.piece_T_xy, r.piece_T_yaw) for r in res], np.float64).reshape(pb.B, 2)
         with self._urgency(urgent):
-            return self.check_trajectories(pb.N, pb.M, pt, cxy, cyaw, env=_env(pb), t_from=t_from, dt=dt, limits=limits)
+            return self.check_trajectories(pb.N, pb.M, pt, cxy, cyaw, env=_env(pb), t_from=t_from, dt=dt, limits=limits, params=_pp(pb))
 
     def submit_replan(self, pb, out, rows, t_from, dt=0.01, rparams=None, depth=2, urgent=False):
         """ualm_submit_replan: replans rows `rows` of batch `pb` as wait() / poll() returned it (out = (results, c_xy, c_yaw)) from each
         robot's state at time t_from (one number or one per row) on its trajectory to the row's original goal, with PlanManager's
         resampler over the trajectory's samples t_from < t of the sequence t = 0, dt, 2dt.. (rparams: front_end.resample_params(), None
         = its defaults), and submits the built problems as one ticket on the next lane of `depth`.  Returns (ticket, ProblemBatch of the
-        built problems, in the order of `rows`, with their environments); poll / wait / cancel / check_results work on it as on any.
+        built problems, in the order of `rows`, with their environments and parameter rows, which the ticket solves with); poll / wait /
+        cancel / check_results work on it as on any.
         urgent: the build and the ticket go ahead of the batches in flight (ualm_set_urgent)."""
         from . import problems
         rows = np.asarray(rows)
@@ -500,24 +522,24 @@ class BatchALMTrajOpt:
         c_xy = np.concatenate([cxy[ocx[i]:ocx[i + 1]] for i in rows]) if B else np.zeros(0)
         c_yaw = np.concatenate([cyaw[ocy[i]:ocy[i + 1]] for i in rows]) if B else np.zeros(0)
         bnd = np.ascontiguousarray(sub.bnd, np.float64).reshape(B, 18)
-        env = _env(sub)
+        env, pp = _env(sub), _pp(sub)
         rp = None if rparams is None else C.byref(rparams)
         No, Mo = np.zeros(B, np.int32), np.zeros(B, np.int32)
         bo, To = np.zeros((B, 18)), np.zeros(B)
         ixy, iyaw = np.zeros((B, _lib.UALM_REPLAN_INNER_XY)), np.zeros((B, _lib.UALM_REPLAN_INNER_YAW))
         t = C.c_int(-1)
         with self._urgency(urgent):
-            _check(self.L.ualm_submit_replan(self.h, B, _p(N, ip), _p(M, ip), _p(pt), _p(c_xy), _p(c_yaw), _p(bnd), _p(env, ip), _p(tf), float(dt),
-                                             rp, int(depth), C.byref(t), _p(No, ip), _p(Mo, ip), _p(bo), _p(To), _p(ixy), _p(iyaw)))
+            _check(self.L.ualm_submit_replan_pp(self.h, B, _p(N, ip), _p(M, ip), _p(pt), _p(c_xy), _p(c_yaw), _p(bnd), _p(env, ip), _p(pp, ppp), _p(tf),
+                                                float(dt), rp, int(depth), C.byref(t), _p(No, ip), _p(Mo, ip), _p(bo), _p(To), _p(ixy), _p(iyaw)))
         # a row over the compiled limits (N 64, M 128): zeros, as the C call packs it
         fits = lambda b: 2 * (No[b] - 1) <= _lib.UALM_REPLAN_INNER_XY and Mo[b] - 1 <= _lib.UALM_REPLAN_INNER_YAW
         pxy = [ixy[b, :2 * (No[b] - 1)] if fits(b) else np.zeros(2 * (int(No[b]) - 1)) for b in range(B)]
         pyaw = [iyaw[b, :Mo[b] - 1] if fits(b) else np.zeros(int(Mo[b]) - 1) for b in range(B)]
         new = problems.ProblemBatch(No, Mo, bo, To, np.concatenate(pxy) if B else np.zeros(0), np.concatenate(pyaw) if B else np.zeros(0),
-                                    env=None if env is None else env.copy())
+                                    env=None if env is None else env.copy(), params=None if pp is None else pp.copy())
         if not hasattr(self, "_tickets"):
             self._tickets = {}
-        self._tickets[t.value] = (new, (None, env))
+        self._tickets[t.value] = (new, (None, env, pp))
         return t.value, new
 
     def build_map(self, pts, geom=None, ellipsoid=(0.2, 0.1, 0.1), iter_num=2, name="map"):
@@ -543,7 +565,7 @@ class BatchALMTrajOpt:
 
 
 def solve_batch_multi(opts, pb):
-    """ualm_solve_batch_multi_env: one host process, one BatchALMTrajOpt per device (same params and maps bound on each)."""
+    """ualm_solve_batch_multi_pp: one host process, one BatchALMTrajOpt per device (same params and maps bound on each)."""
     L = opts[0].L
     hs = (C.c_void_p * len(opts))(*[o.h for o in opts])
     N = np.ascontiguousarray(pb.N, np.int32); M = np.ascontiguousarray(pb.M, np.int32)
@@ -551,7 +573,7 @@ def solve_batch_multi(opts, pb):
     ixy = np.ascontiguousarray(pb.inner_xy, np.float64); iyaw = np.ascontiguousarray(pb.inner_yaw, np.float64)
     res = (Result * pb.B)()
     cxy = np.zeros(int(12 * N.astype(np.int64).sum())); cyaw = np.zeros(int(6 * M.astype(np.int64).sum()))
-    env = _env(pb)
-    _check(L.ualm_solve_batch_multi_env(hs, len(opts), pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), _p(env, ip), res, _p(cxy),
-                                        _p(cyaw)))
+    env, pp = _env(pb), _pp(pb)
+    _check(L.ualm_solve_batch_multi_pp(hs, len(opts), pb.B, _p(N, ip), _p(M, ip), _p(bnd), _p(T), _p(ixy), _p(iyaw), _p(env, ip), _p(pp, ppp), res,
+                                       _p(cxy), _p(cyaw)))
     return res, cxy, cyaw

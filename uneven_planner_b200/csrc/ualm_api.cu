@@ -370,8 +370,7 @@ extern "C" int ualm_set_params(ualm_ctx_t *c, const ualm_params_t *p)
     Env &v = c->envs[c->sel_env];
     v.hp = *p;
     DevParams &d = v.dp;
-    d.rho_T = p->rho_T; d.rho_ter = p->rho_ter; d.max_vel = p->max_vel; d.max_acc_lon = p->max_acc_lon; d.max_acc_lat = p->max_acc_lat;
-    d.max_kap = p->max_kap; d.min_cxi = p->min_cxi; d.max_sig = p->max_sig; d.use_scaling = p->use_scaling; d.rho = p->rho;
+    d.use_scaling = p->use_scaling; d.rho = p->rho;
     d.beta = p->beta; d.gamma = p->gamma; d.epsilon_con = p->epsilon_con; d.max_iter = p->max_iter; d.g_epsilon = p->g_epsilon;
     d.min_step = p->min_step; d.delta = p->delta; d.inner_max_iter = (int)p->inner_max_iter; d.mem_size = p->mem_size; d.past = p->past;
     d.int_K = p->int_K; d.gravity = p->gravity;
@@ -616,11 +615,22 @@ static void group_by_env(int B, const int32_t *env, std::vector<int> &idx, int o
     off[UALM_MAX_ENVS] = (int)idx.size();
 }
 
-// the layout of a batch (BatchLayout) for either path, from the arguments of ualm_upload_env; every argument is checked first
+// pp[B] (NULL = none): every field of every row finite
+static_assert(sizeof(ualm_problem_params_t) == 8 * sizeof(double), "eight doubles, the first eight members of ualm_params_t");
+static int check_pp(int B, const ualm_problem_params_t *pp)
+{
+    for (int b = 0; pp && b < B; b++)
+        for (int k = 0; k < 8; k++)
+            if (!std::isfinite((&pp[b].rho_T)[k])) return fail(UALM_EINVAL, "problem parameter row " + std::to_string(b) + " has a non-finite field");
+    return UALM_OK;
+}
+
+// the layout of a batch (BatchLayout) for either path, from the arguments of ualm_upload_pp; every argument is checked first
 static int batch_layout(ualm_ctx *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time, const double *inner_xy,
-                        const double *inner_yaw, const int32_t *env, BatchLayout *out)
+                        const double *inner_yaw, const int32_t *env, const ualm_problem_params_t *pp, BatchLayout *out)
 {
     if (!c || B < 0 || (B > 0 && (!N || !M || !bnd || !total_time))) return fail(UALM_EINVAL, "bad argument");
+    if (int rc = check_pp(B, pp)) return rc;
     if (int rc = check_envs(c, B, env)) return rc;
     long long need_xy = 0, need_yaw = 0;
     for (int b = 0; b < B; b++) {
@@ -635,6 +645,9 @@ static int batch_layout(ualm_ctx *c, int B, const int32_t *N, const int32_t *M, 
     if (env) L.env.assign(env, env + B);
     L.n.assign(B, 0); L.S.assign(B, 0); L.skip.assign(B, 0);
     L.off_x.assign(B, 0); L.off_s.assign(B, 0); L.off_cxy.assign(B, 0); L.off_cyaw.assign(B, 0);
+    L.pp.resize(8 * (size_t)B);
+    for (int b = 0; b < B; b++)
+        memcpy(&L.pp[8 * (size_t)b], pp ? (const double *)&pp[b] : &c->envs[L.env[b]].hp.rho_T, 8 * sizeof(double));
     long long oixy = 0, oiyaw = 0;
     for (int b = 0; b < B; b++) {
         L.off_x[b] = L.tot_x; L.off_s[b] = L.tot_s; L.off_cxy[b] = L.tot_cxy; L.off_cyaw[b] = L.tot_cyaw;
@@ -698,18 +711,18 @@ static int per_env(ualm_ctx *c, F launch)
 extern "C" int ualm_upload(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
                            const double *inner_xy, const double *inner_yaw)
 {
-    return ualm_upload_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, nullptr);
+    return ualm_upload_pp(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, nullptr, nullptr);
 }
 
-// ualm_upload_env; `before_device` (parity path, may be empty) runs after every host-side allocation and free of the upload and before
+// ualm_upload_pp; `before_device` (parity path, may be empty) runs after every host-side allocation and free of the upload and before
 // its first device operation: ualm_submit_batch_env raises an urgent ticket's hold there, where nothing of the call waits for the device
 // any more
 static int upload_env(ualm_ctx *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time, const double *inner_xy,
-                      const double *inner_yaw, const int32_t *env, const std::function<int()> &before_device)
+                      const double *inner_yaw, const int32_t *env, const ualm_problem_params_t *pp, const std::function<int()> &before_device)
 {
     // validate everything before touching the lane; the lane holds no batch until this call has fully succeeded
     BatchLayout lay;
-    if (int rc = batch_layout(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, &lay)) return rc;
+    if (int rc = batch_layout(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, pp, &lay)) return rc;
     if (lane_in_flight(c, c->cur)) return fail(UALM_ESTATE, "ualm_upload into a lane whose submitted batch is still in flight");
     Lane *l = c->b;
     l->have_batch = false; l->solved = false;
@@ -840,6 +853,7 @@ static int upload_env(ualm_ctx *c, int B, const int32_t *N, const int32_t *M, co
         d.off_hist = oh; d.off_scr = oscr; d.off_fac = ofac; d.off_ws = ows;
         d.off_aux = oaux; oaux += 3LL * m;
         for (int k = 0; k < 18; k++) d.bnd[k] = bnd[(size_t)b * 18 + k];
+        for (int k = 0; k < 8; k++) d.pp[k] = L.pp[8 * (size_t)b + k];
         d.total_time = total_time[b];
         memset(&res0[b], 0, sizeof(ualm_result_t));
         if (L.skip[b]) { res0[b].ret_code = UALM_ELIMIT; continue; }
@@ -881,7 +895,12 @@ static int upload_env(ualm_ctx *c, int B, const int32_t *N, const int32_t *M, co
 extern "C" int ualm_upload_env(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
                                const double *inner_xy, const double *inner_yaw, const int32_t *env)
 {
-    return upload_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, {});
+    return ualm_upload_pp(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, nullptr);
+}
+extern "C" int ualm_upload_pp(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
+                              const double *inner_xy, const double *inner_yaw, const int32_t *env, const ualm_problem_params_t *pp)
+{
+    return upload_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, pp, {});
 }
 
 // raise (1) or lower (0) hold byte `slot` (ualm_ctx::d_hold) in the order of stream st
@@ -1110,7 +1129,13 @@ extern "C" int ualm_solve_batch_env(ualm_ctx_t *c, int B, const int32_t *N, cons
                                     const double *inner_xy, const double *inner_yaw, const int32_t *env, ualm_result_t *results, double *c_xy,
                                     double *c_yaw)
 {
-    int rc = ualm_upload_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env);
+    return ualm_solve_batch_pp(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, nullptr, results, c_xy, c_yaw);
+}
+extern "C" int ualm_solve_batch_pp(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
+                                   const double *inner_xy, const double *inner_yaw, const int32_t *env, const ualm_problem_params_t *pp,
+                                   ualm_result_t *results, double *c_xy, double *c_yaw)
+{
+    int rc = ualm_upload_pp(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, pp);
     if (rc) return rc;
     rc = ualm_solve_resident(c);
     if (rc) return rc;
@@ -1127,7 +1152,14 @@ extern "C" int ualm_submit_batch(ualm_ctx_t *c, int B, const int32_t *N, const i
 extern "C" int ualm_submit_batch_env(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
                                      const double *inner_xy, const double *inner_yaw, const int32_t *env, int depth, int *ticket)
 {
+    return ualm_submit_batch_pp(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, nullptr, depth, ticket);
+}
+extern "C" int ualm_submit_batch_pp(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *bnd, const double *total_time,
+                                    const double *inner_xy, const double *inner_yaw, const int32_t *env, const ualm_problem_params_t *pp, int depth,
+                                    int *ticket)
+{
     if (!c || !ticket) return fail(UALM_EINVAL, "null argument");
+    if (int rc = check_pp(B, pp)) return rc;
     if (depth < 1 || depth > UALM_MAX_LANES) return fail(UALM_EINVAL, "depth out of range [1, UALM_MAX_LANES]");
     const int lane = c->next_submit % depth;
     if (lane_in_flight(c, lane)) return fail(UALM_ESTATE, "all lanes of this depth are in flight: ualm_wait_batch the oldest ticket first");
@@ -1157,7 +1189,7 @@ extern "C" int ualm_submit_batch_env(ualm_ctx_t *c, int B, const int32_t *N, con
         guard.armed = true;
         return UALM_OK;
     };
-    if (!rc) rc = upload_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, before_device);
+    if (!rc) rc = upload_env(c, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, pp, before_device);
     if (!rc && c->tp) {
         std::string em;
         rc = ualm_tp::tp_admit(c->tp, lane, &em, true, c->urgent);
@@ -1313,12 +1345,18 @@ extern "C" int ualm_solve_batch_multi_env(ualm_ctx_t **ctxs, int nctx, int B, co
                                           const double *total_time, const double *inner_xy, const double *inner_yaw, const int32_t *env,
                                           ualm_result_t *results, double *c_xy, double *c_yaw)
 {
+    return ualm_solve_batch_multi_pp(ctxs, nctx, B, N, M, bnd, total_time, inner_xy, inner_yaw, env, nullptr, results, c_xy, c_yaw);
+}
+extern "C" int ualm_solve_batch_multi_pp(ualm_ctx_t **ctxs, int nctx, int B, const int32_t *N, const int32_t *M, const double *bnd,
+                                         const double *total_time, const double *inner_xy, const double *inner_yaw, const int32_t *env,
+                                         const ualm_problem_params_t *pp, ualm_result_t *results, double *c_xy, double *c_yaw)
+{
     if (!ctxs || nctx < 1 || B < 0) return fail(UALM_EINVAL, "bad argument");
     for (int r = 0; r < nctx; r++) if (!ctxs[r]) return fail(UALM_EINVAL, "null ctx in list");
     if (B == 0) return UALM_OK;
     if (!N || !M || !bnd || !total_time) return fail(UALM_EINVAL, "null argument");
     BatchLayout L;       // checked against ctxs[0], the coefficient offsets of the whole batch
-    if (int rc = batch_layout(ctxs[0], B, N, M, bnd, total_time, inner_xy, inner_yaw, env, &L)) return rc;
+    if (int rc = batch_layout(ctxs[0], B, N, M, bnd, total_time, inner_xy, inner_yaw, env, pp, &L)) return rc;
     for (int r = 1; r < nctx; r++) if (int rc = check_envs(ctxs[r], B, env)) return rc;
     std::vector<long long> oxy(B + 1, 0), oyw(B + 1, 0);
     for (int b = 0; b < B; b++) { oxy[b + 1] = oxy[b] + 2LL * (N[b] - 1); oyw[b + 1] = oyw[b] + (M[b] - 1); }
@@ -1331,12 +1369,13 @@ extern "C" int ualm_solve_batch_multi_env(ualm_ctx_t **ctxs, int nctx, int B, co
         shard[(rnd % 2 == 0) ? k : nctx - 1 - k].push_back(ord[pos]);
     }
     for (auto &s : shard) std::sort(s.begin(), s.end());
-    struct Sub { std::vector<int32_t> N, M, E; std::vector<double> bnd, T, ixy, iyw, cxy, cyw; std::vector<ualm_result_t> res; };
+    struct Sub { std::vector<int32_t> N, M, E; std::vector<ualm_problem_params_t> P; std::vector<double> bnd, T, ixy, iyw, cxy, cyw; std::vector<ualm_result_t> res; };
     std::vector<Sub> sub(nctx);
     for (int r = 0; r < nctx; r++) {
         Sub &s = sub[r];
         for (int b : shard[r]) {
             s.N.push_back(N[b]); s.M.push_back(M[b]); s.T.push_back(total_time[b]); s.E.push_back(env ? env[b] : 0);
+            if (pp) s.P.push_back(pp[b]);
             s.bnd.insert(s.bnd.end(), bnd + 18 * (size_t)b, bnd + 18 * (size_t)b + 18);
             if (oxy[b + 1] > oxy[b]) s.ixy.insert(s.ixy.end(), inner_xy + oxy[b], inner_xy + oxy[b + 1]);
             if (oyw[b + 1] > oyw[b]) s.iyw.insert(s.iyw.end(), inner_yaw + oyw[b], inner_yaw + oyw[b + 1]);
@@ -1350,8 +1389,8 @@ extern "C" int ualm_solve_batch_multi_env(ualm_ctx_t **ctxs, int nctx, int B, co
     // upload + launch everywhere first (asynchronous per device), then collect
     for (int r = 0; r < nctx; r++) {
         if (shard[r].empty()) continue;
-        int rc = ualm_upload_env(ctxs[r], (int)shard[r].size(), sub[r].N.data(), sub[r].M.data(), sub[r].bnd.data(), sub[r].T.data(), sub[r].ixy.data(),
-                                 sub[r].iyw.data(), sub[r].E.data());
+        int rc = ualm_upload_pp(ctxs[r], (int)shard[r].size(), sub[r].N.data(), sub[r].M.data(), sub[r].bnd.data(), sub[r].T.data(), sub[r].ixy.data(),
+                                sub[r].iyw.data(), sub[r].E.data(), pp ? sub[r].P.data() : nullptr);
         if (!rc) rc = ualm_solve_resident(ctxs[r]);
         if (rc) return rc;
     }
@@ -1664,6 +1703,12 @@ extern "C" int ualm_check_trajectories(ualm_ctx_t *c, int B, const int32_t *N, c
                                        const double *c_yaw, const int32_t *env, const double *t_from, double dt, const ualm_limits_t *limits,
                                        double *out16)
 {
+    return ualm_check_trajectories_pp(c, B, N, M, piece_T, c_xy, c_yaw, env, nullptr, t_from, dt, limits, out16);
+}
+extern "C" int ualm_check_trajectories_pp(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *piece_T, const double *c_xy,
+                                          const double *c_yaw, const int32_t *env, const ualm_problem_params_t *pp, const double *t_from, double dt,
+                                          const ualm_limits_t *limits, double *out16)
+{
     if (!c || B < 0 || (B > 0 && (!N || !M || !piece_T || !c_xy || !c_yaw || !out16))) return fail(UALM_EINVAL, "ualm_check_trajectories: null argument or B < 0");
     if (!(dt > 0.0)) return fail(UALM_EINVAL, "ualm_check_trajectories: dt must be > 0");
     long long ncx = 0, ncy = 0;
@@ -1672,6 +1717,7 @@ extern "C" int ualm_check_trajectories(ualm_ctx_t *c, int B, const int32_t *N, c
         if (t_from && !(t_from[b] >= 0.0)) return fail(UALM_EINVAL, "ualm_check_trajectories: t_from must be >= 0 (and not NaN)");
         ncx += 12LL * N[b]; ncy += 6LL * M[b];
     }
+    if (int rc = check_pp(B, pp)) return rc;
     if (B == 0) return UALM_OK;
     if (int rc = check_envs(c, B, env)) return rc;
     CK(cudaSetDevice(c->device));
@@ -1686,9 +1732,16 @@ extern "C" int ualm_check_trajectories(ualm_ctx_t *c, int B, const int32_t *N, c
     const std::vector<ProbDesc> desc = scan_descs(B, N, M);
     std::vector<double> tf;
     if (!t_from) tf.assign(B, 0.0);
-    // the block: out 16B | piece_T 2B | t_from B | c_xy | c_yaw (doubles), then desc, then idx
+    // each row's limits: the call's, else its parameter row's, else its environment's
+    std::vector<CheckLimits> lims(B);
+    for (int b = 0; b < B; b++) {
+        const double *q = pp ? &pp[b].rho_T : &c->envs[env ? env[b] : 0].hp.rho_T;
+        lims[b] = limits ? CheckLimits{limits->max_vel, limits->max_acc_lon, limits->max_acc_lat, limits->max_kap, limits->min_cxi, limits->max_sig}
+                         : CheckLimits{q[2], q[3], q[4], q[5], q[6], q[7]};
+    }
+    // the block: out 16B | piece_T 2B | t_from B | c_xy | c_yaw (doubles), then desc, then the limits, then idx
     const size_t nd = 16 * (size_t)B + 2 * (size_t)B + (size_t)B + (size_t)ncx + (size_t)ncy;
-    const size_t bytes = sizeof(double) * nd + sizeof(ProbDesc) * B + sizeof(int) * B;
+    const size_t bytes = sizeof(double) * nd + sizeof(ProbDesc) * B + sizeof(CheckLimits) * B + sizeof(int) * B;
     const cudaStream_t st = c->cstream;
     // declared after hold: on every exit cdone is recorded behind the kernels before the versions are let go
     struct Done {
@@ -1704,22 +1757,21 @@ extern "C" int ualm_check_trajectories(ualm_ctx_t *c, int B, const int32_t *N, c
     if (int rc = check_block(c, bytes)) return rc;
     double *d_out = (double *)c->cbuf, *d_pt = d_out + 16 * (size_t)B, *d_tf = d_pt + 2 * (size_t)B, *d_cxy = d_tf + B, *d_cyaw = d_cxy + ncx;
     ProbDesc *d_desc = (ProbDesc *)(d_out + nd);
-    int *d_idx = (int *)(d_desc + B);
+    CheckLimits *d_lim = (CheckLimits *)(d_desc + B);
+    int *d_idx = (int *)(d_lim + B);
     CK(cudaMemcpyAsync(d_pt, piece_T, sizeof(double) * 2 * B, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_tf, t_from ? t_from : tf.data(), sizeof(double) * B, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_cxy, c_xy, sizeof(double) * ncx, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_cyaw, c_yaw, sizeof(double) * ncy, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_desc, desc.data(), sizeof(ProbDesc) * B, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_lim, lims.data(), sizeof(CheckLimits) * B, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_idx, idx.data(), sizeof(int) * B, cudaMemcpyHostToDevice, st));
     CheckPtrs a;
     a.desc = d_desc; a.c_xy = d_cxy; a.c_yaw = d_cyaw; a.piece_T = d_pt; a.t_from = d_tf; a.out = d_out;
     for (int e = 0; e < UALM_MAX_ENVS; e++) {
         const int cnt = off[e + 1] - off[e];
         if (cnt == 0) continue;
-        const ualm_params_t &hp = c->envs[e].hp;
-        const CheckLimits lim = limits ? CheckLimits{limits->max_vel, limits->max_acc_lon, limits->max_acc_lat, limits->max_kap, limits->min_cxi, limits->max_sig}
-                                       : CheckLimits{hp.max_vel, hp.max_acc_lon, hp.max_acc_lat, hp.max_kap, hp.min_cxi, hp.max_sig};
-        check_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(a, hold[e]->dm, c->envs[e].dp.gravity, lim, dt, d_idx + off[e], cnt);
+        check_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(a, hold[e]->dm, c->envs[e].dp.gravity, d_lim, dt, d_idx + off[e], cnt);
         CK(cudaGetLastError());
     }
     if (urgent.armed) {
@@ -1739,10 +1791,19 @@ extern "C" int ualm_submit_replan(ualm_ctx_t *c, int B, const int32_t *N, const 
                                   const ualm_resample_params_t *rp, int depth, int *ticket, int32_t *N_out, int32_t *M_out, double *bnd_out,
                                   double *total_time_out, double *inner_xy_out, double *inner_yaw_out)
 {
+    return ualm_submit_replan_pp(c, B, N, M, piece_T, c_xy, c_yaw, bnd, env, nullptr, t_from, dt, rp, depth, ticket, N_out, M_out, bnd_out,
+                                 total_time_out, inner_xy_out, inner_yaw_out);
+}
+extern "C" int ualm_submit_replan_pp(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *piece_T, const double *c_xy,
+                                     const double *c_yaw, const double *bnd, const int32_t *env, const ualm_problem_params_t *pp, const double *t_from,
+                                     double dt, const ualm_resample_params_t *rp, int depth, int *ticket, int32_t *N_out, int32_t *M_out,
+                                     double *bnd_out, double *total_time_out, double *inner_xy_out, double *inner_yaw_out)
+{
     if (!c || !ticket || B < 0 || (B > 0 && (!N || !M || !piece_T || !c_xy || !c_yaw || !bnd || !t_from || !N_out || !M_out || !bnd_out || !total_time_out)))
         return fail(UALM_EINVAL, "ualm_submit_replan: null argument or B < 0");
     if (!(dt > 0.0)) return fail(UALM_EINVAL, "ualm_submit_replan: dt must be > 0");
     if (depth < 1 || depth > UALM_MAX_LANES) return fail(UALM_EINVAL, "ualm_submit_replan: depth out of range [1, UALM_MAX_LANES]");
+    if (int rc = check_pp(B, pp)) return rc;
     const ualm_resample_params_t r = rp ? *rp : ualm_resample_params_t{0.3, 2.0, 0.5, 1.2, 0.0};   // run_*.yaml manager/*
     if (!(r.piece_len > 0.0) || !(r.yaw_piece_times > 0.0) || !(r.mean_vel > 0.0) || !(r.init_time_times > 0.0))
         return fail(UALM_EINVAL, "ualm_submit_replan: piece_len, yaw_piece_times, mean_vel and init_time_times must be > 0");
@@ -1763,7 +1824,7 @@ extern "C" int ualm_submit_replan(ualm_ctx_t *c, int B, const int32_t *N, const 
     // a diverged solve's coefficients: refused, not sampled
     for (long long q = 0; q < ncx; q++) if (!std::isfinite(c_xy[q])) return fail(UALM_EINVAL, "ualm_submit_replan: c_xy must be finite");
     for (long long q = 0; q < ncy; q++) if (!std::isfinite(c_yaw[q])) return fail(UALM_EINVAL, "ualm_submit_replan: c_yaw must be finite");
-    if (B == 0) return ualm_submit_batch_env(c, 0, N_out, M_out, bnd_out, total_time_out, nullptr, nullptr, env, depth, ticket);
+    if (B == 0) return ualm_submit_batch_pp(c, 0, N_out, M_out, bnd_out, total_time_out, nullptr, nullptr, env, pp, depth, ticket);
     if (int rc = check_envs(c, B, env)) return rc;
     if (lane_in_flight(c, c->next_submit % depth)) return fail(UALM_ESTATE, "all lanes of this depth are in flight: ualm_wait_batch the oldest ticket first");
     CK(cudaSetDevice(c->device));
@@ -1830,7 +1891,7 @@ extern "C" int ualm_submit_replan(ualm_ctx_t *c, int B, const int32_t *N, const 
         }
         pxy += nxy; pyaw += nyaw;
     }
-    return ualm_submit_batch_env(c, B, N_out, M_out, bnd_out, total_time_out, ixy.data(), iyaw.data(), env, depth, ticket);
+    return ualm_submit_batch_pp(c, B, N_out, M_out, bnd_out, total_time_out, ixy.data(), iyaw.data(), env, pp, depth, ticket);
 }
 
 // ---------------------------------------------------------------------------------------------

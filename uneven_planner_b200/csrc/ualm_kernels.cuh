@@ -60,8 +60,8 @@ enum {
     LBFGSERR_INCREASEGRADIENT,
 };
 
+// what is per environment; the eight per-problem values (ualm_problem_params_t) travel in ProbDesc::pp and are read from SC_PP
 struct DevParams {
-    R rho_T, rho_ter, max_vel, max_acc_lon, max_acc_lat, max_kap, min_cxi, max_sig;
     int use_scaling;
     R rho, beta, gamma, epsilon_con, max_iter;
     R g_epsilon, min_step, delta;
@@ -95,6 +95,7 @@ struct ProbDesc {
     long long off_aux;    // 3 * mem_size of the problem's environment (lm_aux)
     R bnd[18];
     R total_time;
+    R pp[8];              // the problem's ualm_problem_params_t (its row, or its environment's values): copied to SC_PP by traj_setup
 };
 
 struct BatchPtrs {
@@ -200,8 +201,12 @@ enum {
     SC_TX1 = 0, SC_TX2, SC_TX3, SC_TX4, SC_TX5, SC_TY1, SC_TY2, SC_TY3, SC_TY4, SC_TY5,
     SC_SCALE_FX, SC_RHO, SC_F, SC_JERK, SC_CONSTR, SC_TAUCOST, SC_JERKRAW, SC_RTY, SC_CMD,
     SC_STOPPED,  // != 0: the stop predicate fired inside the inner solve that just ended
-    SC_PROB      // the problem a CMD_NEXT hands to the helpers
+    SC_PROB,     // the problem a CMD_NEXT hands to the helpers
+    // the problem's ualm_problem_params_t, written by the leader's traj_setup: every warp of the group (helpers, a mate that joins)
+    // reads them here, and the launch's DevParams holds only what is per environment
+    SC_PP = 24, SC_RHO_T = SC_PP, SC_RHO_TER, SC_MAX_VEL, SC_MAX_ACC_LON, SC_MAX_ACC_LAT, SC_MAX_KAP, SC_MIN_CXI, SC_MAX_SIG
 };
+static_assert(SC_MAX_SIG < 48, "the scalar slots of SmemLayout::sc");
 
 // Handles to shared memory: a 32-bit address in the shared state space.  Accesses through them are explicit ld.shared /
 // st.shared with 32-bit address arithmetic.  (Plain `double*` members become generic loads, and C++ references into the
@@ -1184,6 +1189,12 @@ __device__ UALM_NOINLINE void sample_tables(Traj &t, int lane)
 // calConstrainCostGrad, phase A: one lane per sample (alm_traj_opt.cpp:710-964).  Writes hx/gx, the 8 cost
 // terms and the per-sample gradients to the scratch; phase B accumulates them in the reference's order.
 // ---------------------------------------------------------------------------------------------
+// the square of limit `slot` of the problem's row, formed as the reference forms it (max_vel * max_vel)
+__device__ __forceinline__ R sq_at(const Traj &t, int slot)
+{
+    const R v = t.sc[slot];
+    return v * v;
+}
 __device__ UALM_NOINLINE void penalty_samples(Traj &t, const DevMap &map, const DevParams &p, int gtid, int GT)
 {
     const int S = t.S, K = t.K;
@@ -1191,10 +1202,10 @@ __device__ UALM_NOINLINE void penalty_samples(Traj &t, const DevMap &map, const 
     const R rrho = ((__double_as_longlong(rho) & 0xFFFFFFFFFFFFFll) == 0xFFFFFFFFFFFFFll) ? __longlong_as_double(0x7ff8000000000000ll) : 1.0 / rho;   // RN(1/rho): x / rho below is formed as div_by_recip(x, rho, rrho), bit-identical to the IEEE quotient
     const R step = t.sc[SC_TX1] / (R)K;
     R *scr = t.scr;
-    // parameters (kernel-parameter space through a generic pointer) and trajectory pointers (a struct in local memory) once
-    const R gravity = p.gravity, rho_ter = p.rho_ter, min_cxi = p.min_cxi, max_sig = p.max_sig;
-    const R max_vel2 = p.max_vel * p.max_vel, max_alon2 = p.max_acc_lon * p.max_acc_lon, max_alat2 = p.max_acc_lat * p.max_acc_lat,
-            max_kap2 = p.max_kap * p.max_kap;
+    // parameters (kernel-parameter space through a generic pointer) and trajectory pointers (a struct in local memory) once.  The
+    // problem's row is read from its slot where it is used (sq_at: the squared limits), which keeps it out of the registers the
+    // sample loop holds
+    const R gravity = p.gravity;
     const bool use_scaling = p.use_scaling != 0;
     R *const lambda_p = t.lambda, *const mu_p = t.mu, *const scale_p = t.scale_cx, *const hx_p = t.hx, *const gx_p = t.gx;
     for (int s = gtid; s < S; s += GT) {
@@ -1221,8 +1232,8 @@ __device__ UALM_NOINLINE void penalty_samples(Traj &t, const DevMap &map, const 
         R *gx6 = gx_p + 6 * (size_t)s;
 
         R omega;
-        if (j == 0 || j == K) omega = 0.5 * rho_ter * step * scale_fx;
-        else omega = rho_ter * step * scale_fx;
+        if (j == 0 || j == K) omega = 0.5 * t.sc[SC_RHO_TER] * step * scale_fx;
+        else omega = t.sc[SC_RHO_TER] * step * scale_fx;
         const R user_cost = omega * sigma * sigma;
         scr[(SF_COST0 + 0) * S + s] = user_cost;
         scr[SF_USER * S + s] = user_cost;
@@ -1241,7 +1252,7 @@ __device__ UALM_NOINLINE void penalty_samples(Traj &t, const DevMap &map, const 
         }
         { // longitude velocity
             const R m_ = mu6[0];
-            const R gv = (vx * vx - max_vel2) * sc7[1];
+            const R gv = (vx * vx - sq_at(t, SC_MAX_VEL)) * sc7[1];
             gx6[0] = gv;
             if (rho * gv + m_ > 0) {
                 scr[(SF_COST0 + 2) * S + s] = gv * (m_ + 0.5 * rho * gv);
@@ -1251,7 +1262,7 @@ __device__ UALM_NOINLINE void penalty_samples(Traj &t, const DevMap &map, const 
         }
         { // longitude acceleration
             const R m_ = mu6[1];
-            const R gv = (ax * ax - max_alon2) * sc7[2];
+            const R gv = (ax * ax - sq_at(t, SC_MAX_ACC_LON)) * sc7[2];
             gx6[1] = gv;
             if (rho * gv + m_ > 0) {
                 scr[(SF_COST0 + 3) * S + s] = gv * (m_ + 0.5 * rho * gv);
@@ -1261,7 +1272,7 @@ __device__ UALM_NOINLINE void penalty_samples(Traj &t, const DevMap &map, const 
         }
         { // latitude acceleration
             const R m_ = mu6[2];
-            const R gv = (ay * ay - max_alat2) * sc7[3];
+            const R gv = (ay * ay - sq_at(t, SC_MAX_ACC_LAT)) * sc7[3];
             gx6[2] = gv;
             if (rho * gv + m_ > 0) {
                 scr[(SF_COST0 + 4) * S + s] = gv * (m_ + 0.5 * rho * gv);
@@ -1272,8 +1283,8 @@ __device__ UALM_NOINLINE void penalty_samples(Traj &t, const DevMap &map, const 
         { // curvature
             const R m_ = mu6[3];
             R gv;
-            if (use_scaling) gv = (curv_snorm - max_kap2) * sc7[4];
-            else gv = (curv_snorm - max_kap2) * UALM_CUR_SCALE;
+            if (use_scaling) gv = (curv_snorm - sq_at(t, SC_MAX_KAP)) * sc7[4];
+            else gv = (curv_snorm - sq_at(t, SC_MAX_KAP)) * UALM_CUR_SCALE;
             gx6[3] = gv;
             if (rho * gv + m_ > 0) {
                 const R denominator = 1.0 / (vx * vx + UALM_DELTA_SIGL);
@@ -1286,7 +1297,7 @@ __device__ UALM_NOINLINE void penalty_samples(Traj &t, const DevMap &map, const 
         }
         { // attitude
             const R m_ = mu6[4];
-            const R gv = (min_cxi - cos_xi) * sc7[5];
+            const R gv = ((R)t.sc[SC_MIN_CXI] - cos_xi) * sc7[5];
             gx6[4] = gv;
             if (rho * gv + m_ > 0) {
                 scr[(SF_COST0 + 6) * S + s] = gv * (m_ + 0.5 * rho * gv);
@@ -1298,8 +1309,8 @@ __device__ UALM_NOINLINE void penalty_samples(Traj &t, const DevMap &map, const 
         { // surface variation
             const R m_ = mu6[5];
             R gv;
-            if (use_scaling) gv = (sigma - max_sig) * sc7[6];
-            else gv = (sigma - max_sig) * UALM_SIG_SCALE;
+            if (use_scaling) gv = (sigma - t.sc[SC_MAX_SIG]) * sc7[6];
+            else gv = (sigma - t.sc[SC_MAX_SIG]) * UALM_SIG_SCALE;
             gx6[5] = gv;
             if (rho * gv + m_ > 0) {
                 scr[(SF_COST0 + 7) * S + s] = gv * (m_ + 0.5 * rho * gv);
@@ -1591,11 +1602,12 @@ __device__ UALM_NOINLINE void evaluate(Traj &t, const DevMap &map, const DevPara
         const R tau = t.x[0];
         R jerk_c = t.sc[SC_JERKRAW] * scale_fx;
         if (p.use_scaling) jerk_c *= UALM_SCALE_TRICK_JERK;
-        const R tau_cost = p.rho_T * expC2(tau) * scale_fx;
+        const R rho_T = t.sc[SC_RHO_T];
+        const R tau_cost = rho_T * expC2(tau) * scale_fx;
         R sx = 0.0, sy = 0.0;
         for (int i = 0; i < N; i++) sx += t.gTxy[i];
         for (int i = 0; i < M; i++) sy += t.gTyaw[i];
-        const R grad_Tsum = p.rho_T * scale_fx + sx / (R)N + sy / (R)M;
+        const R grad_Tsum = rho_T * scale_fx + sx / (R)N + sy / (R)M;
         t.g[0] = grad_Tsum * getTtoTauGrad(tau);
         t.sc[SC_JERK] = jerk_c; t.sc[SC_TAUCOST] = tau_cost;
         t.sc[SC_F] = jerk_c + t.sc[SC_CONSTR] + tau_cost;
@@ -1856,6 +1868,7 @@ __device__ UALM_NOINLINE void scaling_rounds(Traj &t, const DevMap &map, const D
     R *wy = t.wsw + (size_t)nx * st + lane;     // y column
     R *ww = t.wsw + (size_t)2 * nx * st + lane; // yaw
     R *scr = t.scr;
+    const R rho_ter = t.sc[SC_RHO_TER];
     for (int s0 = 0; s0 < S; s0 += GT) {
         const int s = s0 + gtid;
         const bool act = s < S;
@@ -1868,7 +1881,7 @@ __device__ UALM_NOINLINE void scaling_rounds(Traj &t, const DevMap &map, const D
             sample_kin(t, map, p.gravity, i, t.s1tab[j], t.base[i], q);
             t.yawidx[s] = (unsigned short)q.yaw_idx;
             // user-defined cost -> f gradient pieces (alm_traj_opt.cpp:507-519), parked in the sample scratch
-            const R omega = (j == 0 || j == K) ? 0.5 * p.rho_ter * step : p.rho_ter * step;
+            const R omega = (j == 0 || j == K) ? 0.5 * rho_ter * step : rho_ter * step;
             const R sigma = q.tv[6];
             const R user_cost = omega * sigma * sigma;
             R gs[3];
@@ -2072,7 +2085,7 @@ __device__ UALM_NOINLINE void init_scaling(Traj &t, const DevMap &map, const Dev
         R sx = 0.0, sy = 0.0, m1 = 0.0, m2 = 0.0;
         for (int i = 0; i < N; i++) sx += t.gTxy[i];
         for (int i = 0; i < M; i++) sy += t.gTyaw[i];
-        const R grad_Tsum_fx = p.rho_T + sx / (R)N + sy / (R)M;
+        const R grad_Tsum_fx = t.sc[SC_RHO_T] + sx / (R)N + sy / (R)M;
         const R gdTau_fx = grad_Tsum_fx * dTdtau;
         for (int i = 0; i < N - 1; i++) { m1 = fmax(m1, fabs(t.gCxy[6 * i + 5])); m1 = fmax(m1, fabs(t.gCxy[6 * i + 5 + nx])); }
         for (int i = 0; i < M - 1; i++) m2 = fmax(m2, fabs(t.gCyaw[6 * i + 5]));
@@ -2115,6 +2128,7 @@ __device__ UALM_NOINLINE void traj_setup(Traj &t, const BatchPtrs &bp, const Dev
     __shared__ long long s_prof_all[UALM_WPB][UALM_NPROF + 1];
     long long *s_prof = s_prof_all[threadIdx.x >> 5];
     const int ln = threadIdx.x & 31;
+    if (wig == 0 && ln < 8) t.sc[SC_PP + ln] = pd->pp[ln];   // the leader; its helpers read them after its next post
     if (ln < UALM_NPROF + 1) s_prof[ln] = 0;
     t.prof = s_prof; t.plast = s_prof + UALM_NPROF;
     UALM_SYNC();
@@ -2605,13 +2619,14 @@ struct CheckPtrs {
     const R *c_xy, *c_yaw, *piece_T, *t_from;
     R *out;
 };
-// idx: the n problems to check, those of one environment, whose grid, gravity and limits this launch carries
+// idx: the n problems to check, those of one environment, whose grid and gravity this launch carries; lims[problem]: its limits
 __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) check_kernel(const __grid_constant__ CheckPtrs a, const __grid_constant__ DevMap map, R gravity,
-        const __grid_constant__ CheckLimits lim, R dt, const int *idx, int n)
+        const CheckLimits *lims, R dt, const int *idx, int n)
 {
     const int lane = threadIdx.x & 31, w = blockIdx.x * UALM_WPB + (threadIdx.x >> 5);
     if (w >= n) return;         // whole warp exits
     const int prob = idx[w];
+    const CheckLimits lim = lims[prob];
     const ProbDesc *pd = a.desc + prob;
     R *o = a.out + 16 * (size_t)prob;
     const R Tx = a.piece_T[2 * prob], Ty = a.piece_T[2 * prob + 1];

@@ -301,8 +301,7 @@ int tp_set_params(TpEngine *e, int env, const ualm_params_t *p, std::string *err
 {
     if (p->int_K < 1 || p->int_K > TP_KB_THREADS - 1) { if (err) *err = "int_K out of range [1,127] on the throughput path"; return UALM_ELIMIT; }
     TpParams &d = e->p[env];
-    d.rho_T = p->rho_T; d.rho_ter = p->rho_ter; d.max_vel = p->max_vel; d.max_acc_lon = p->max_acc_lon; d.max_acc_lat = p->max_acc_lat;
-    d.max_kap = p->max_kap; d.min_cxi = p->min_cxi; d.max_sig = p->max_sig; d.use_scaling = p->use_scaling; d.rho = p->rho;
+    d.use_scaling = p->use_scaling; d.rho = p->rho;
     d.beta = p->beta; d.gamma = p->gamma; d.epsilon_con = p->epsilon_con; d.max_iter = p->max_iter; d.g_epsilon = p->g_epsilon;
     d.min_step = p->min_step; d.delta = p->delta; d.inner_max_iter = (int)p->inner_max_iter; d.mem_size = p->mem_size; d.past = p->past;
     d.int_K = p->int_K; d.gravity = p->gravity; d.max_evals = e->max_evals;
@@ -393,6 +392,7 @@ int tp_upload(TpEngine *e, int lane, const BatchLayout &L, const double *bnd, co
         GatherDesc &g = l.gd[b];
         a.slot = -1; a.N = L.N[b]; a.M = L.M[b]; a.ticket = lane; a.index = b; a.mode = L.skip[b] ? -1 : 0; a.off_x = L.off_x[b]; a.total_time = total_time[b];
         for (int k = 0; k < 18; k++) a.bnd[k] = bnd[(size_t)b * 18 + k];
+        for (int k = 0; k < 8; k++) a.pp[k] = L.pp[8 * (size_t)b + k];
         g.slot = -1; g.N = L.N[b]; g.M = L.M[b]; g.off_cxy = L.off_cxy[b]; g.off_cyaw = L.off_cyaw[b]; g.off_x = L.off_x[b]; g.off_s = L.off_s[b];
     }
     TCK(l.d_ad.ensure(B)); TCK(l.d_gd.ensure(B)); TCK(l.d_x0.ensure(L.tot_x)); TCK(l.d_cxy.ensure(L.tot_cxy)); TCK(l.d_cyaw.ensure(L.tot_cyaw));

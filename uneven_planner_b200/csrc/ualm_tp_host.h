@@ -18,6 +18,8 @@ struct BatchLayout {
     std::vector<unsigned char> skip;
     std::vector<long long> off_x, off_s, off_cxy, off_cyaw;
     std::vector<double> x0;
+    // pp[8 b ..]: problem b's ualm_problem_params_t (the batch's row, or its environment's first eight ualm_params_t fields)
+    std::vector<double> pp;
     long long tot_x = 0, tot_s = 0, tot_cxy = 0, tot_cyaw = 0;
     // every problem grouped by environment (ascending within one, skipped ones included): environment e at eidx[eoff[e], eoff[e + 1])
     std::vector<int> eidx;

@@ -72,8 +72,8 @@ enum {
     LBERR_WIDTHTOOSMALL, LBERR_INVALIDPARAMETERS, LBERR_INCREASEGRADIENT,
 };
 
+// what is per environment; the eight per-problem values (ualm_problem_params_t) are the slot's TpState::pp
 struct TpParams {
-    double rho_T, rho_ter, max_vel, max_acc_lon, max_acc_lat, max_kap, min_cxi, max_sig;
     int use_scaling;
     double rho, beta, gamma, epsilon_con, max_iter, g_epsilon, min_step, delta;
     int inner_max_iter, mem_size, past, int_K;
@@ -98,6 +98,7 @@ struct TpState {
     double tau, T, Tx, Ty, jerk_raw;          // of the last forward solve (the state getTraj() / the dual update see, SURVEY Q1)
     double f_last;
     double bnd[18];
+    double pp[8];           // the problem's ualm_problem_params_t (its row, or its environment's values), written by admit_kernel
 };
 
 struct TpPool {
@@ -517,8 +518,9 @@ __device__ void finish_eval(const TpPool &E, const TpParams &p, const SlotView &
     kp.mark(KP_FIN_SWEEP);
     if (lane == 0) {
         const double tau = st->tau;
-        v.g[0] = (p.rho_T * scale_fx + sx / (double)N + sy / (double)M) * dTdtau(tau);
-        st->f_last = st->jerk_raw * js + E.kb_cost[v.slot] + p.rho_T * st->T * scale_fx;
+        const double rho_T = st->pp[0];
+        v.g[0] = (rho_T * scale_fx + sx / (double)N + sy / (double)M) * dTdtau(tau);
+        st->f_last = st->jerk_raw * js + E.kb_cost[v.slot] + rho_T * st->T * scale_fx;
     }
     __syncwarp();
     kp.mark(KP_FIN_POST);
@@ -886,7 +888,7 @@ __global__ void loop_ctrl_kernel(cudaGraphConditionalHandle h, const int *n_acti
 // admission: problem b of a submitted batch -> slot.  One launch covers problems of one environment (use_scaling, K are its own);
 // off_s[b]: sample offset of ad[b] in the caller's dual arrays, sfx is indexed by the problem's index in its batch
 // ---------------------------------------------------------------------------------------------------------------------
-struct AdmitDesc { int slot, N, M, ticket, index, mode, group, pad1; long long off_x; double total_time; double bnd[18]; };
+struct AdmitDesc { int slot, N, M, ticket, index, mode, group, pad1; long long off_x; double total_time; double bnd[18]; double pp[8]; };
 
 template <class R>
 __global__ void admit_kernel(const __grid_constant__ TpPool E, const AdmitDesc *ad, const double *x0, int B, int use_scaling, int K,
@@ -914,6 +916,7 @@ __global__ void admit_kernel(const __grid_constant__ TpPool E, const AdmitDesc *
     if (threadIdx.x == 0) {
         st->N = a.N; st->M = a.M; st->n = n; st->S = S; st->ticket = a.ticket; st->index = a.index;
         for (int k = 0; k < 18; k++) st->bnd[k] = a.bnd[k];
+        for (int k = 0; k < 8; k++) st->pp[k] = a.pp[k];
         st->mode = a.mode; st->group = a.group;
         st->need_scale = ((a.mode == 0 && use_scaling) || a.mode == 2) ? 1 : 0;
         st->phase = PH_NEW;

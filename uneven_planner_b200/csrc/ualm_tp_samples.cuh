@@ -340,9 +340,10 @@ __global__ void __launch_bounds__(TP_KB_THREADS) kb_kernel(const __grid_constant
     if (TMA && tid == 0) { mbar_init(&sh.bar, TP_MAXPPC); mbar_fence_init(); }   // every chunk: TP_MAXPPC arrivals (one per piece slot)
     const int ppc = max(1, min(TP_MAXPPC, TP_KB_THREADS / K1));
     const R Tx = (R)st->Tx, Ty = (R)st->Ty, step = Tx / (R)K, rho = (R)st->rho, scale_fx = (R)st->scale_fx;
-    const R gravity = (R)p.gravity, rho_ter = (R)p.rho_ter, min_cxi = (R)p.min_cxi, max_sig = (R)p.max_sig;
-    const R max_vel2 = (R)(p.max_vel * p.max_vel), max_alon2 = (R)(p.max_acc_lon * p.max_acc_lon), max_alat2 = (R)(p.max_acc_lat * p.max_acc_lat),
-            max_kap2 = (R)(p.max_kap * p.max_kap);
+    // the limits and rho_ter are the slot's (its problem's row), formed in double and then cast
+    const double *pp = st->pp;
+    const R gravity = (R)p.gravity, rho_ter = (R)pp[1], min_cxi = (R)pp[6], max_sig = (R)pp[7];
+    const R max_vel2 = (R)(pp[2] * pp[2]), max_alon2 = (R)(pp[3] * pp[3]), max_alat2 = (R)(pp[4] * pp[4]), max_kap2 = (R)(pp[5] * pp[5]);
     const bool use_scaling = p.use_scaling != 0;
     R *du = (R *)E.dual + (size_t)slot * TP_NDUAL * E.Smax;
     R *gdc = (R *)E.gdc + (size_t)slot * TP_CSTRIDE;
@@ -565,7 +566,7 @@ __global__ void __launch_bounds__(TP_KB_THREADS) ks_kernel(const __grid_constant
     for (int q = tid; q < ny; q += TP_KB_THREADS) { cyaw[q] = (R)cd[TP_CYAW + q]; zy[q] = (R)zd[TP_CYAW + q]; gfy[q] = 0; }
     for (int q = tid; q < M; q += TP_KB_THREADS) gT[N + q] = 0;
     const int ppc = max(1, min(TP_MAXPPC, TP_KB_THREADS / K1));
-    const R Tx = (R)st->Tx, Ty = (R)st->Ty, step = Tx / (R)K, gravity = (R)p.gravity, rho_ter = (R)p.rho_ter;
+    const R Tx = (R)st->Tx, Ty = (R)st->Ty, step = Tx / (R)K, gravity = (R)p.gravity, rho_ter = (R)st->pp[1];
     const R dtdtau = (R)dTdtau(st->tau);
     R ix[6], iy[6];
     ix[0] = iy[0] = 1;
@@ -733,7 +734,7 @@ __global__ void __launch_bounds__(TP_KB_THREADS) ks_kernel(const __grid_constant
     if (tid == 0) {
         double m = 0.0, a = 0.0, b = 0.0;
         for (int w = 0; w < TP_KB_THREADS / 32; w++) { m = fmax(m, s_red[w][0]); a += s_red[w][1]; b += s_red[w][2]; }
-        const double gtau = (p.rho_T + a / (double)N + b / (double)M) * dTdtau(st->tau);
+        const double gtau = (st->pp[0] + a / (double)N + b / (double)M) * dTdtau(st->tau);
         st->scale_fx = 1.0 / fmax(1.0, fmax(m, fabs(gtau)));
         st->need_scale = 0;
     }

@@ -46,6 +46,9 @@ class ProblemBatch:
     starts: np.ndarray = None
     goals: np.ndarray = None
     env: np.ndarray = None   # int32 [B]: environment of every problem (include/ualm.h, ualm_select_env); None = all environment 0
+    # float64 [B, 8]: every problem's vehicle limits and cost weights (ualm_problem_params_t, rows of _lib.problem_params); None = each
+    # problem uses its environment's
+    params: np.ndarray = None
 
     @property
     def B(self):
@@ -72,7 +75,8 @@ class ProblemBatch:
                             np.concatenate([self.inner_yaw[oyaw[i]:oyaw[i + 1]] for i in idx]) if len(idx) else np.zeros(0),
                             None if self.starts is None else self.starts[idx].copy(),
                             None if self.goals is None else self.goals[idx].copy(),
-                            None if self.env is None else self.env[idx].copy())
+                            None if self.env is None else self.env[idx].copy(),
+                            None if self.params is None else self.params[idx].copy())
 
     def x0(self, i):
         """Initial decision vector [tau | Pxy | Pyaw] of problem i (alm_traj_opt.cpp:205-216)."""
@@ -83,15 +87,19 @@ class ProblemBatch:
 
 
 def concat(batches, envs):
-    """One batch of the problems of `batches` back to back, batch k's in environment envs[k] (a mixed batch; select() reorders it)."""
+    """One batch of the problems of `batches` back to back, batch k's in environment envs[k] (a mixed batch; select() reorders it).
+    Parameter rows are carried when every batch has them."""
     if len(batches) != len(envs):
         raise ValueError("one environment per batch")
+    if len({b.params is None for b in batches}) > 1:
+        raise ValueError("concat: either every batch or none carries parameter rows")
     cat = lambda f, empty: np.concatenate([getattr(b, f) for b in batches]) if batches else empty
     have = lambda f: all(getattr(b, f) is not None for b in batches)
     return ProblemBatch(cat("N", np.zeros(0, np.int32)).astype(np.int32), cat("M", np.zeros(0, np.int32)).astype(np.int32),
                         cat("bnd", np.zeros((0, 18))), cat("total_time", np.zeros(0)), cat("inner_xy", np.zeros(0)), cat("inner_yaw", np.zeros(0)),
                         cat("starts", None) if batches and have("starts") else None, cat("goals", None) if batches and have("goals") else None,
-                        np.concatenate([np.full(b.B, int(e), np.int32) for b, e in zip(batches, envs)]) if batches else np.zeros(0, np.int32))
+                        np.concatenate([np.full(b.B, int(e), np.int32) for b, e in zip(batches, envs)]) if batches else np.zeros(0, np.int32),
+                        np.concatenate([np.asarray(b.params, np.float64).reshape(-1, 8) for b in batches]) if batches and have("params") else None)
 
 
 def dubins(start, goal, radius=0.6, ds=0.06, max_pts=4096):
