@@ -144,7 +144,7 @@ def test_cuda_matches_reference_build_directly(gpu, bumps_map):
         assert np.array_equal(out["c_xy"], cxy[ocx[i]:ocx[i + 1]]) and np.array_equal(out["c_yaw"], cyaw[ocy[i]:ocy[i + 1]]), i
         assert out["piece_T"][0] == feas[i, 8] and out["piece_T"][1] == feas[i, 9] and out["rho"][0] == res[i].rho_final, i
         assert out["sfx"][0] == res[i].scale_fx and np.abs(out["hx"]).max() == res[i].res_h, i
-        assert np.array_equal(out["feas"], feas[i, :7]), i          # the reference's post-solve report vs feasibility_kernel
+        assert np.array_equal(out["feas"], feas[i, :7]), i          # the reference's post-solve report vs the lane scan
     opt.close()
 
 

@@ -159,7 +159,7 @@ def test_limits_and_state_checks(gpu, bumps_map):
     pbx = _with_oversize(pb, 4)
     res, cxy, cyaw = opt.optimize(pbx)
     _, _, ocx, _ = pbx.offsets()
-    assert res[4].ret_code == _lib.UALM_ELIMIT and not cxy[ocx[4]:ocx[5]].any()
+    assert res[4].ret_code == _lib.UALM_ELIMIT and not cxy[ocx[4]:ocx[5]].any() and not opt.feasibility(0.01)[4].any()
     keep = [i for i in range(pbx.B) if i != 4]
     assert [(res[i].ret_code, res[i].n_evals, res[i].inner_cost) for i in keep] == [(r.ret_code, r.n_evals, r.inner_cost) for r in ref[0]]
     opt.close()

@@ -177,7 +177,7 @@ def test_eval_batch_leaves_the_uploaded_initial_guesses(gpu, cases, bumps_map, p
 @pytest.mark.parametrize("name", ["hill", "forest"])
 @pytest.mark.parametrize("prec", PRECISIONS)
 def test_solves_at_edge_shapes(gpu, cases, terrain, prec, name):
-    """complete records, finite coefficients, total_T = N piece_T_xy summed, and the post-solve scan (feasibility_kernel) equal to
+    """complete records, finite coefficients, total_T = N piece_T_xy summed, and the post-solve scan (ualm_feasibility_batch) equal to
     the oracle's bit for bit on the path's own coefficients and piece durations"""
     import pyoracle as po
     from uneven_planner_b200 import configs

@@ -870,7 +870,7 @@ static int upload_env(ualm_ctx *c, int B, const int32_t *N, const int32_t *M, co
     CK(l->d_eidx.ensure(B));
     CK(l->d_stop.ensure((size_t)std::max(B, 1)));
     CK(l->d_prof.ensure((size_t)std::max(B, 1) * UALM_NPROF));
-    CK(l->d_pieceT.ensure((size_t)std::max(B, 1) * 2)); CK(l->d_feas.ensure((size_t)std::max(B, 1) * 10));
+    CK(l->d_pieceT.ensure((size_t)std::max(B, 1) * 2)); CK(l->d_feas.ensure((size_t)std::max(B, 1) * 16));
     CK(l->d_cxy.ensure(ocx)); CK(l->d_cyaw.ensure(ocy)); CK(l->d_res.ensure(B)); CK(l->d_f.ensure(B)); CK(l->d_sfx.ensure(B));
     if (before_device) if (int rc = before_device()) return rc;
     // factor arrays: entries outside the band-in-matrix positions (and the pad rows) are never written and must read 0
@@ -1586,8 +1586,11 @@ __global__ void piece_T_from_results(const ualm_result_t *res, int B, double *pi
 } // namespace ualm
 
 // descriptors of a scan over B trajectories of N[b] / M[b] pieces whose coefficients are packed in problem order; S == 0 marks a problem
-// over the compiled limits, which is not scanned
-static std::vector<ProbDesc> scan_descs(int B, const int32_t *N, const int32_t *M)
+// over the compiled limits, which is not scanned.  pp[2..7] carry the six limits check_kernel tests: `limits` when given, else the
+// problem's parameter row (rows: 8 doubles each, as ualm_problem_params_t; null = none), else its environment's
+static_assert(sizeof(ualm_limits_t) == 6 * sizeof(double), "ualm_problem_params_t's six limits, in its order");
+static std::vector<ProbDesc> scan_descs(const ualm_ctx *c, int B, const int32_t *N, const int32_t *M, const int32_t *env, const double *rows,
+                                        const ualm_limits_t *limits)
 {
     std::vector<ProbDesc> desc(B);
     long long ocx = 0, ocy = 0;
@@ -1595,18 +1598,21 @@ static std::vector<ProbDesc> scan_descs(int B, const int32_t *N, const int32_t *
         memset(&desc[b], 0, sizeof(ProbDesc));
         desc[b].N = N[b]; desc[b].M = M[b]; desc[b].off_cxy = ocx; desc[b].off_cyaw = ocy;
         desc[b].S = over_limits(N[b], M[b]) ? 0 : 1;
+        memcpy(desc[b].pp, rows ? rows + 8 * (size_t)b : &c->envs[env ? env[b] : 0].hp.rho_T, 8 * sizeof(double));
+        if (limits) memcpy(desc[b].pp + 2, limits, sizeof(ualm_limits_t));
         ocx += 12LL * N[b]; ocy += 6LL * M[b];
     }
     return desc;
 }
 
 // a collected throughput batch as the BatchPtrs of the scans (feasibility, MPC export): descriptors of the lane's layout and piece
-// durations from the records, in device buffers this object owns
+// durations from the records, in device buffers this object owns, with the scan's index list and rows
 struct TpScan {
     DevBuf<ProbDesc> desc;
     DevBuf<double> pt, feas;
+    DevBuf<int> idx;
     BatchPtrs bp;
-    ~TpScan() { desc.release(); pt.release(); feas.release(); }
+    ~TpScan() { desc.release(); pt.release(); feas.release(); idx.release(); }
 };
 // what: the entry point, for the refusal of a lane with no collected batch
 static int tp_scan(ualm_ctx *c, const char *what, TpScan &s)
@@ -1617,7 +1623,7 @@ static int tp_scan(ualm_ctx *c, const char *what, TpScan &s)
     CK(cudaSetDevice(c->device));
     const BatchLayout &L = c->b->batch;
     if (L.B == 0) return UALM_OK;
-    const std::vector<ProbDesc> desc = scan_descs(L.B, L.N.data(), L.M.data());
+    const std::vector<ProbDesc> desc = scan_descs(c, L.B, L.N.data(), L.M.data(), L.env.data(), L.pp.data(), nullptr);
     CK(s.desc.ensure(L.B)); CK(s.pt.ensure(2 * (size_t)L.B));
     CK(cudaMemcpy(s.desc.p, desc.data(), sizeof(ProbDesc) * L.B, cudaMemcpyHostToDevice));
     piece_T_from_results<<<(L.B + 127) / 128, 128>>>(d_res, L.B, s.pt.p);
@@ -1626,51 +1632,50 @@ static int tp_scan(ualm_ctx *c, const char *what, TpScan &s)
     return UALM_OK;
 }
 
-// feasibility_kernel over the lane's batch: one launch with the parameters of its environment and the grid version maps[e] the batch
-// was solved on when there is only one environment, else one launch per environment over its problem indices
-static int feasibility_launch(ualm_ctx *c, const BatchPtrs &bp, const BatchLayout &L, const MapRef *maps, double dt, double *d_out, cudaStream_t st)
+// check_kernel once per environment present: over its problems d_idx[eoff[e], eoff[e + 1]), against grid version maps[e] with its gravity
+static int scan_launch(ualm_ctx *c, const CheckPtrs &a, const int *d_idx, const int *eoff, const MapRef *maps, double dt, cudaStream_t st)
 {
-    for (int e = 0; e < UALM_MAX_ENVS; e++)
-        if (((L.env_mask >> e) & 1u) && !maps[e]) return fail(UALM_ESTATE, "ualm_feasibility_batch: the batch was not solved by a launch of this context");
-    if (!L.mixed()) {
-        const int e = L.env[0];
-        feasibility_kernel<<<(L.B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(bp, c->envs[e].dp, maps[e]->dm, dt, d_out, nullptr, L.B);
-        CK(cudaGetLastError());
-        return UALM_OK;
-    }
-    struct Tmp { DevBuf<int> idx; ~Tmp() { idx.release(); } } t;
-    CK(t.idx.ensure(L.B));
-    CK(cudaMemcpyAsync(t.idx.p, L.eidx.data(), sizeof(int) * L.B, cudaMemcpyHostToDevice, st));
     for (int e = 0; e < UALM_MAX_ENVS; e++) {
-        const int cnt = L.eoff[e + 1] - L.eoff[e];
+        const int cnt = eoff[e + 1] - eoff[e];
         if (cnt == 0) continue;
-        feasibility_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(bp, c->envs[e].dp, maps[e]->dm, dt, d_out, t.idx.p + L.eoff[e], cnt);
+        check_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(a, maps[e]->dm, c->envs[e].dp.gravity, dt, d_idx + eoff[e], cnt);
         CK(cudaGetLastError());
     }
-    CK(cudaStreamSynchronize(st));       // the device copy of the indices is local
     return UALM_OK;
 }
 
+// the scan of the lane's solved batch, every sample, on the grid versions it was solved on.  A problem over the compiled limits was
+// not solved: its row is zeros
 extern "C" int ualm_feasibility_batch(ualm_ctx_t *c, double dt, double *out10)
 {
     if (!c || !out10 || !(dt > 0.0)) return fail(UALM_EINVAL, "null argument or dt <= 0");
     Lane *l = c->b;
     const BatchLayout &L = l->batch;
+    TpScan s;
+    CheckPtrs a{};
+    const int *d_idx;
+    cudaStream_t st;
     if (c->tp) {
-        TpScan s;
         if (int rc = tp_scan(c, "ualm_feasibility_batch", s)) return rc;
         if (L.B == 0) return UALM_OK;
-        CK(s.feas.ensure(10 * (size_t)L.B));
-        if (int rc = feasibility_launch(c, s.bp, L, l->vref, dt, s.feas.p, 0)) return rc;
-        CK(cudaMemcpy(out10, s.feas.p, sizeof(double) * 10 * L.B, cudaMemcpyDeviceToHost));
-        return UALM_OK;
+        CK(s.feas.ensure(16 * (size_t)L.B)); CK(s.idx.ensure(L.B));
+        CK(cudaMemcpy(s.idx.p, L.eidx.data(), sizeof(int) * L.B, cudaMemcpyHostToDevice));
+        a.desc = s.bp.desc; a.c_xy = s.bp.c_xy; a.c_yaw = s.bp.c_yaw; a.piece_T = s.bp.piece_T; a.out = s.feas.p;
+        d_idx = s.idx.p; st = 0;
+    } else {
+        if (!l->have_batch || !l->solved) return fail(UALM_ESTATE, "ualm_feasibility_batch needs a solved resident batch");
+        CK(cudaSetDevice(c->device));
+        if (L.B == 0) return UALM_OK;
+        const BatchPtrs bp = batch_ptrs(c);
+        a.desc = bp.desc; a.c_xy = bp.c_xy; a.c_yaw = bp.c_yaw; a.piece_T = bp.piece_T; a.out = l->d_feas.p;
+        d_idx = l->d_eidx.p; st = l->stream;
     }
-    if (!l->have_batch || !l->solved) return fail(UALM_ESTATE, "ualm_feasibility_batch needs a solved resident batch");
-    CK(cudaSetDevice(c->device));
-    if (L.B == 0) return UALM_OK;
-    if (int rc = feasibility_launch(c, batch_ptrs(c), L, l->vref, dt, l->d_feas.p, l->stream)) return rc;
-    CK(cudaMemcpyAsync(out10, l->d_feas.p, sizeof(double) * 10 * L.B, cudaMemcpyDeviceToHost, l->stream));
-    CK(cudaStreamSynchronize(l->stream));
+    for (int e = 0; e < UALM_MAX_ENVS; e++)
+        if (((L.env_mask >> e) & 1u) && !l->vref[e]) return fail(UALM_ESTATE, "ualm_feasibility_batch: the batch was not solved by a launch of this context");
+    if (int rc = scan_launch(c, a, d_idx, L.eoff, l->vref, dt, st)) return rc;
+    CK(cudaMemcpy2DAsync(out10, 10 * sizeof(double), a.out, 16 * sizeof(double), 10 * sizeof(double), L.B, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    for (int b = 0; b < L.B; b++) if (L.skip[b]) memset(out10 + 10 * (size_t)b, 0, 10 * sizeof(double));
     return UALM_OK;
 }
 
@@ -1696,6 +1701,62 @@ static int check_block(ualm_ctx *c, size_t bytes)
     return UALM_OK;
 }
 
+// Trajectories the caller holds (ualm_check_trajectories, ualm_submit_replan), in the layouts ualm_wait_batch returns
+struct Held {
+    int B;
+    const int32_t *N, *M;
+    const double *piece_T, *c_xy, *c_yaw, *t_from;     // t_from: null = 0 for every row (the check only)
+    long long ncx = 0, ncy = 0;                          // coefficients, 12 N and 6 M summed (held_counts)
+};
+// every row has N, M >= 1; counts the coefficients
+static int held_counts(const char *what, Held &h)
+{
+    for (int b = 0; b < h.B; b++) {
+        if (h.N[b] < 1 || h.M[b] < 1) return fail(UALM_EINVAL, std::string(what) + ": piece counts must be >= 1");
+        h.ncx += 12LL * h.N[b]; h.ncy += 6LL * h.M[b];
+    }
+    return UALM_OK;
+}
+// h staged on the check stream in the context's block, grown in stream order: out (nout doubles) | piece_T 2B | t_from B | bnd 18B
+// (when given) | c_xy | c_yaw, then the descriptors, then B ints of idx (when given).  Under urgent work the hold of the check stream
+// (urgent: unarmed, on that stream) is raised before the copies; the caller lowers it behind its kernel (hold_lower), `urgent` on any
+// earlier exit.  a: the block as check_kernel reads it
+struct Staged { CheckPtrs a; double *bnd; int *idx; };
+static int stage_held(ualm_ctx *c, const Held &h, const std::vector<ProbDesc> &desc, size_t nout, const double *bnd, const std::vector<int> *idx,
+                      HoldGuard &urgent, Staged &s)
+{
+    const int B = h.B;
+    const cudaStream_t st = c->cstream;
+    if (c->urgent && c->d_hold) {     // (parity path: the throughput path has no hold)
+        if (int rc = hold_set(c, UALM_MAX_LANES, 1, st)) return rc;
+        urgent.armed = true;
+    }
+    const size_t nbnd = bnd ? 18 * (size_t)B : 0, nd = nout + 3 * (size_t)B + nbnd + (size_t)h.ncx + (size_t)h.ncy;
+    if (int rc = check_block(c, sizeof(double) * nd + sizeof(ProbDesc) * B + (idx ? sizeof(int) * B : 0))) return rc;
+    double *d_out = (double *)c->cbuf, *d_pt = d_out + nout, *d_tf = d_pt + 2 * (size_t)B, *d_bnd = d_tf + B, *d_cxy = d_bnd + nbnd,
+           *d_cyaw = d_cxy + h.ncx;
+    ProbDesc *d_desc = (ProbDesc *)(d_out + nd);
+    int *d_idx = (int *)(d_desc + B);
+    CK(cudaMemcpyAsync(d_pt, h.piece_T, sizeof(double) * 2 * B, cudaMemcpyHostToDevice, st));
+    if (h.t_from) CK(cudaMemcpyAsync(d_tf, h.t_from, sizeof(double) * B, cudaMemcpyHostToDevice, st));
+    if (bnd) CK(cudaMemcpyAsync(d_bnd, bnd, sizeof(double) * nbnd, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_cxy, h.c_xy, sizeof(double) * h.ncx, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_cyaw, h.c_yaw, sizeof(double) * h.ncy, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(d_desc, desc.data(), sizeof(ProbDesc) * B, cudaMemcpyHostToDevice, st));
+    if (idx) CK(cudaMemcpyAsync(d_idx, idx->data(), sizeof(int) * B, cudaMemcpyHostToDevice, st));
+    s.a.desc = d_desc; s.a.c_xy = d_cxy; s.a.c_yaw = d_cyaw; s.a.piece_T = d_pt; s.a.t_from = h.t_from ? d_tf : nullptr; s.a.out = d_out;
+    s.bnd = bnd ? d_bnd : nullptr;
+    s.idx = idx ? d_idx : nullptr;
+    return UALM_OK;
+}
+// lowers a raised hold in the order of its stream, here rather than on exit
+static int hold_lower(HoldGuard &g)
+{
+    if (!g.armed) return UALM_OK;
+    g.armed = false;
+    return hold_set(g.c, g.slot, 0, g.st);
+}
+
 // check_kernel over host trajectories, on the context's check stream, against each environment's grid version current at the call.
 // The context's block (cbuf) grows in stream order on that stream, and the versions are let go only after cdone (as lane_hold lets
 // go), so nothing here waits for a batch in flight
@@ -1711,12 +1772,10 @@ extern "C" int ualm_check_trajectories_pp(ualm_ctx_t *c, int B, const int32_t *N
 {
     if (!c || B < 0 || (B > 0 && (!N || !M || !piece_T || !c_xy || !c_yaw || !out16))) return fail(UALM_EINVAL, "ualm_check_trajectories: null argument or B < 0");
     if (!(dt > 0.0)) return fail(UALM_EINVAL, "ualm_check_trajectories: dt must be > 0");
-    long long ncx = 0, ncy = 0;
-    for (int b = 0; b < B; b++) {
-        if (N[b] < 1 || M[b] < 1) return fail(UALM_EINVAL, "ualm_check_trajectories: piece counts must be >= 1");
-        if (t_from && !(t_from[b] >= 0.0)) return fail(UALM_EINVAL, "ualm_check_trajectories: t_from must be >= 0 (and not NaN)");
-        ncx += 12LL * N[b]; ncy += 6LL * M[b];
-    }
+    Held held{B, N, M, piece_T, c_xy, c_yaw, t_from};
+    if (int rc = held_counts("ualm_check_trajectories", held)) return rc;
+    for (int b = 0; t_from && b < B; b++)
+        if (!(t_from[b] >= 0.0)) return fail(UALM_EINVAL, "ualm_check_trajectories: t_from must be >= 0 (and not NaN)");
     if (int rc = check_pp(B, pp)) return rc;
     if (B == 0) return UALM_OK;
     if (int rc = check_envs(c, B, env)) return rc;
@@ -1729,57 +1788,19 @@ extern "C" int ualm_check_trajectories_pp(ualm_ctx_t *c, int B, const int32_t *N
     group_by_env(B, env, idx, off);
     MapRef hold[UALM_MAX_ENVS];
     for (int e = 0; e < UALM_MAX_ENVS; e++) if (off[e + 1] > off[e]) hold[e] = c->envs[e].map;
-    const std::vector<ProbDesc> desc = scan_descs(B, N, M);
-    std::vector<double> tf;
-    if (!t_from) tf.assign(B, 0.0);
-    // each row's limits: the call's, else its parameter row's, else its environment's
-    std::vector<CheckLimits> lims(B);
-    for (int b = 0; b < B; b++) {
-        const double *q = pp ? &pp[b].rho_T : &c->envs[env ? env[b] : 0].hp.rho_T;
-        lims[b] = limits ? CheckLimits{limits->max_vel, limits->max_acc_lon, limits->max_acc_lat, limits->max_kap, limits->min_cxi, limits->max_sig}
-                         : CheckLimits{q[2], q[3], q[4], q[5], q[6], q[7]};
-    }
-    // the block: out 16B | piece_T 2B | t_from B | c_xy | c_yaw (doubles), then desc, then the limits, then idx
-    const size_t nd = 16 * (size_t)B + 2 * (size_t)B + (size_t)B + (size_t)ncx + (size_t)ncy;
-    const size_t bytes = sizeof(double) * nd + sizeof(ProbDesc) * B + sizeof(CheckLimits) * B + sizeof(int) * B;
-    const cudaStream_t st = c->cstream;
+    const std::vector<ProbDesc> desc = scan_descs(c, B, N, M, env, pp ? &pp[0].rho_T : nullptr, limits);
     // declared after hold: on every exit cdone is recorded behind the kernels before the versions are let go
     struct Done {
         ualm_ctx *c;
         ~Done() { if (cudaEventRecord(c->cdone, c->cstream) == cudaSuccess) cudaStreamWaitEvent(c->fstream, c->cdone, 0); }
     } done{c};
-    // urgent: the hold of the check stream, from before the copies to the end of the kernels
-    HoldGuard urgent{c, UALM_MAX_LANES, st, false};
-    if (c->urgent && c->d_hold) {     // (parity path: the throughput path has no hold)
-        if (int rc = hold_set(c, UALM_MAX_LANES, 1, st)) return rc;
-        urgent.armed = true;
-    }
-    if (int rc = check_block(c, bytes)) return rc;
-    double *d_out = (double *)c->cbuf, *d_pt = d_out + 16 * (size_t)B, *d_tf = d_pt + 2 * (size_t)B, *d_cxy = d_tf + B, *d_cyaw = d_cxy + ncx;
-    ProbDesc *d_desc = (ProbDesc *)(d_out + nd);
-    CheckLimits *d_lim = (CheckLimits *)(d_desc + B);
-    int *d_idx = (int *)(d_lim + B);
-    CK(cudaMemcpyAsync(d_pt, piece_T, sizeof(double) * 2 * B, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_tf, t_from ? t_from : tf.data(), sizeof(double) * B, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_cxy, c_xy, sizeof(double) * ncx, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_cyaw, c_yaw, sizeof(double) * ncy, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_desc, desc.data(), sizeof(ProbDesc) * B, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_lim, lims.data(), sizeof(CheckLimits) * B, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_idx, idx.data(), sizeof(int) * B, cudaMemcpyHostToDevice, st));
-    CheckPtrs a;
-    a.desc = d_desc; a.c_xy = d_cxy; a.c_yaw = d_cyaw; a.piece_T = d_pt; a.t_from = d_tf; a.out = d_out;
-    for (int e = 0; e < UALM_MAX_ENVS; e++) {
-        const int cnt = off[e + 1] - off[e];
-        if (cnt == 0) continue;
-        check_kernel<<<(cnt + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(a, hold[e]->dm, c->envs[e].dp.gravity, d_lim, dt, d_idx + off[e], cnt);
-        CK(cudaGetLastError());
-    }
-    if (urgent.armed) {
-        urgent.armed = false;
-        if (int rc = hold_set(c, UALM_MAX_LANES, 0, st)) return rc;
-    }
-    CK(cudaMemcpyAsync(out16, d_out, sizeof(double) * 16 * B, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    HoldGuard urgent{c, UALM_MAX_LANES, c->cstream, false};
+    Staged s;
+    if (int rc = stage_held(c, held, desc, 16 * (size_t)B, nullptr, &idx, urgent, s)) return rc;
+    if (int rc = scan_launch(c, s.a, s.idx, off, hold, dt, c->cstream)) return rc;
+    if (int rc = hold_lower(urgent)) return rc;
+    CK(cudaMemcpyAsync(out16, s.a.out, sizeof(double) * 16 * B, cudaMemcpyDeviceToHost, c->cstream));
+    CK(cudaStreamSynchronize(c->cstream));
     return UALM_OK;
 }
 
@@ -1807,60 +1828,40 @@ extern "C" int ualm_submit_replan_pp(ualm_ctx_t *c, int B, const int32_t *N, con
     const ualm_resample_params_t r = rp ? *rp : ualm_resample_params_t{0.3, 2.0, 0.5, 1.2, 0.0};   // run_*.yaml manager/*
     if (!(r.piece_len > 0.0) || !(r.yaw_piece_times > 0.0) || !(r.mean_vel > 0.0) || !(r.init_time_times > 0.0))
         return fail(UALM_EINVAL, "ualm_submit_replan: piece_len, yaw_piece_times, mean_vel and init_time_times must be > 0");
-    long long ncx = 0, ncy = 0;
+    Held held{B, N, M, piece_T, c_xy, c_yaw, t_from};
+    if (int rc = held_counts("ualm_submit_replan", held)) return rc;
     for (int b = 0; b < B; b++) {
-        if (N[b] < 1 || M[b] < 1) return fail(UALM_EINVAL, "ualm_submit_replan: piece counts must be >= 1");
-        double tx = 0.0, ty = 0.0;      // replan_kernel's sums
-        for (int i = 0; i < N[b]; i++) tx += piece_T[2 * b];
-        for (int i = 0; i < M[b]; i++) ty += piece_T[2 * b + 1];
-        const double total = tx < ty ? tx : ty;
-        if (!(t_from[b] >= 0.0) || !(t_from[b] < total)) return fail(UALM_EINVAL, "ualm_submit_replan: t_from must be in [0, the trajectory's duration)");
-        if (!(total / dt < 4.0e6)) return fail(UALM_EINVAL, "ualm_submit_replan: duration / dt must be < 4e6");
+        const TrajDur d = traj_duration(N[b], M[b], piece_T[2 * b], piece_T[2 * b + 1]);    // replan_kernel's duration
+        if (!(t_from[b] >= 0.0) || !(t_from[b] < d.total)) return fail(UALM_EINVAL, "ualm_submit_replan: t_from must be in [0, the trajectory's duration)");
+        if (!d.scannable(dt)) return fail(UALM_EINVAL, "ualm_submit_replan: duration / dt must be < 4e6");
         if (!std::isfinite(piece_T[2 * b]) || !std::isfinite(piece_T[2 * b + 1])) return fail(UALM_EINVAL, "ualm_submit_replan: piece_T must be finite");
         for (int k : {6, 7, 8, 9, 10, 11, 15, 16, 17})      // the goal entries bnd' takes
             if (!std::isfinite(bnd[18 * (size_t)b + k])) return fail(UALM_EINVAL, "ualm_submit_replan: the goal entries of bnd must be finite");
-        ncx += 12LL * N[b]; ncy += 6LL * M[b];
     }
     // a diverged solve's coefficients: refused, not sampled
-    for (long long q = 0; q < ncx; q++) if (!std::isfinite(c_xy[q])) return fail(UALM_EINVAL, "ualm_submit_replan: c_xy must be finite");
-    for (long long q = 0; q < ncy; q++) if (!std::isfinite(c_yaw[q])) return fail(UALM_EINVAL, "ualm_submit_replan: c_yaw must be finite");
+    for (long long q = 0; q < held.ncx; q++) if (!std::isfinite(c_xy[q])) return fail(UALM_EINVAL, "ualm_submit_replan: c_xy must be finite");
+    for (long long q = 0; q < held.ncy; q++) if (!std::isfinite(c_yaw[q])) return fail(UALM_EINVAL, "ualm_submit_replan: c_yaw must be finite");
     if (B == 0) return ualm_submit_batch_pp(c, 0, N_out, M_out, bnd_out, total_time_out, nullptr, nullptr, env, pp, depth, ticket);
     if (int rc = check_envs(c, B, env)) return rc;
     if (lane_in_flight(c, c->next_submit % depth)) return fail(UALM_ESTATE, "all lanes of this depth are in flight: ualm_wait_batch the oldest ticket first");
     CK(cudaSetDevice(c->device));
     if (int rc = check_stream(c)) return rc;
-    const std::vector<ProbDesc> desc = scan_descs(B, N, M);      // (replan_kernel does not read S)
-    // the block: out (UALM_REPLAN_STRIDE B) | piece_T 2B | bnd 18B | t_from B | c_xy | c_yaw (doubles), then desc
-    const size_t nout = (size_t)UALM_REPLAN_STRIDE * B, nd = nout + 21 * (size_t)B + (size_t)ncx + (size_t)ncy;
+    const std::vector<ProbDesc> desc = scan_descs(c, B, N, M, env, nullptr, nullptr);      // (replan_kernel reads neither S nor the limits)
+    const size_t nout = (size_t)UALM_REPLAN_STRIDE * B;
     const cudaStream_t st = c->cstream;
-    // urgent: the hold of the check stream over the build, lowered behind its kernel before any refusal can follow; the ticket is
-    // urgent by itself (ualm_submit_batch_env)
+    // urgent: the hold is lowered behind the build's kernel before any refusal can follow; the ticket is urgent by itself
+    // (ualm_submit_batch_env)
     HoldGuard urgent{c, UALM_MAX_LANES, st, false};
-    if (c->urgent && c->d_hold) {     // (parity path: the throughput path has no hold)
-        if (int rc = hold_set(c, UALM_MAX_LANES, 1, st)) return rc;
-        urgent.armed = true;
-    }
-    if (int rc = check_block(c, sizeof(double) * nd + sizeof(ProbDesc) * B)) return rc;
-    double *d_out = (double *)c->cbuf, *d_pt = d_out + nout, *d_bnd = d_pt + 2 * (size_t)B, *d_tf = d_bnd + 18 * (size_t)B, *d_cxy = d_tf + B,
-           *d_cyaw = d_cxy + ncx;
-    ProbDesc *d_desc = (ProbDesc *)(d_out + nd);
-    CK(cudaMemcpyAsync(d_pt, piece_T, sizeof(double) * 2 * B, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_bnd, bnd, sizeof(double) * 18 * B, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_tf, t_from, sizeof(double) * B, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_cxy, c_xy, sizeof(double) * ncx, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_cyaw, c_yaw, sizeof(double) * ncy, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(d_desc, desc.data(), sizeof(ProbDesc) * B, cudaMemcpyHostToDevice, st));
+    Staged s;
+    if (int rc = stage_held(c, held, desc, nout, bnd, nullptr, urgent, s)) return rc;
     ReplanPtrs a;
-    a.desc = d_desc; a.c_xy = d_cxy; a.c_yaw = d_cyaw; a.piece_T = d_pt; a.bnd = d_bnd; a.t_from = d_tf; a.out = d_out;
+    a.desc = s.a.desc; a.c_xy = s.a.c_xy; a.c_yaw = s.a.c_yaw; a.piece_T = s.a.piece_T; a.bnd = s.bnd; a.t_from = s.a.t_from; a.out = s.a.out;
     const ReplanParams p{dt, r.piece_len, r.yaw_piece_times, r.mean_vel, r.init_time_times};
     replan_kernel<<<(B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(a, p, B);
     CK(cudaGetLastError());
-    if (urgent.armed) {
-        urgent.armed = false;
-        if (int rc = hold_set(c, UALM_MAX_LANES, 0, st)) return rc;
-    }
+    if (int rc = hold_lower(urgent)) return rc;
     std::vector<double> h(nout);
-    CK(cudaMemcpyAsync(h.data(), d_out, sizeof(double) * nout, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(h.data(), s.a.out, sizeof(double) * nout, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     // the one refusal after the build, before any output: a polyline of zero or non-finite length (a robot already at its goal, or
     // coordinates so large that their squares overflow) has no total_time ualm_submit_batch_env would take

@@ -2464,12 +2464,8 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) penalty_only_kernel(c
 }
 
 // ---------------------------------------------------------------------------------------------
-// Post-solve quality scan (SURVEY 8f-4): ALMTrajOpt::getMaxVxAxAyCurAttSig (alm_traj_opt.h:170-229) and
-// SE2Trajectory::getNonHolError (se2traj.hpp:551-561) of every solved trajectory, one warp per trajectory, one lane per sample
-// time.  The reference walks t = 0, dt, 2dt.. by repeated addition and keeps "the first sample with the largest |value|":
-// here every lane forms the same sequence of additions and keeps its own slice, the warp reduces by (|value|, earliest sample),
-// and the non-holonomic error is summed in sample order -- bit-identical to the sequential loops (oracle: orc_feasibility).
-// out[10 * problem + ...] = {max_vx, max_ax, max_ay, max_cur, max_att, max_sig, nonhol_error, samples, T_xy piece, T_yaw piece}
+// Sampling a trajectory as the reference does: its duration, its sample times t = 0, dt, 2dt.. and its value at a time.  The scan,
+// the replan build and the hand-over to the MPC all sample through these helpers, so their samples are the same bits.
 // ---------------------------------------------------------------------------------------------
 __device__ __forceinline__ int locate_piece(int P, R dur, R &t)   // PolyTrajectory::locatePieceIdx (se2traj.hpp:343-361), uniform durations
 {
@@ -2490,6 +2486,52 @@ __device__ __forceinline__ void piece_eval(const R *c, R t, R &v, R &dv, R &ddv)
     int m = 1; n = 2;
     for (int k = 2; k <= 5; k++) { ddv += (R)(m * n) * tn * c[k]; tn *= t; m++; n++; }
 }
+// PolyTrajectory::getTotalDuration (se2traj.hpp:291-300) of the xy and the yaw part, each summed piece by piece; an SE2 trajectory
+// lasts the smaller (:415-418).  A diverged solve can leave an astronomically long (or non-finite) duration, over which the
+// reference's scan would run (almost) forever: such a trajectory is not scanned.  The host validates replan input with the same sums
+struct TrajDur {
+    R xy, yaw, total;
+    __host__ __device__ __forceinline__ bool scannable(R dt) const { return total / dt < 4.0e6; }
+};
+__host__ __device__ __forceinline__ TrajDur traj_duration(int N, int M, R Tx, R Ty)
+{
+    TrajDur d{0.0, 0.0, 0.0};
+    for (int i = 0; i < N; i++) d.xy += Tx;
+    for (int i = 0; i < M; i++) d.yaw += Ty;
+    d.total = d.xy < d.yaw ? d.xy : d.yaw;
+    return d;
+}
+// The lane's sample time in the chunk of 32 that starts at tbase, which moves on to the next chunk's start.  The reference forms its
+// samples by t += dt: every lane makes the same 32 additions, so each sample is bit for bit the sequential loop's
+__device__ __forceinline__ R chunk_time(R &tbase, R dt, int lane)
+{
+    R tm = 0.0, tt = tbase;
+    for (int i = 0; i < 32; i++) { if (i == lane) tm = tt; tt = tt + dt; }
+    tbase = tt;
+    return tm;
+}
+// Position, velocity and acceleration of the xy part at time txy and the yaw part at time tyaw (PolyTrajectory::getValue / getVel /
+// getAcc, se2traj.hpp:363-391).  ip, tl and iy, ty locate the pieces, for a second trajectory of the same piece durations
+struct SE2Eval { R x, y, yaw, vx, vy, dyaw, ax, ay, ddyaw; int ip, iy; R tl, ty; };
+__device__ __forceinline__ SE2Eval se2_eval(const R *cxy, const R *cyaw, int N, int M, R Tx, R Ty, R txy, R tyaw)
+{
+    SE2Eval e;
+    e.tl = txy;
+    e.ip = locate_piece(N, Tx, e.tl);
+    piece_eval(cxy + 6 * e.ip, e.tl, e.x, e.vx, e.ax);
+    piece_eval(cxy + 6 * N + 6 * e.ip, e.tl, e.y, e.vy, e.ay);
+    e.ty = tyaw;
+    e.iy = locate_piece(M, Ty, e.ty);
+    piece_eval(cyaw + 6 * e.iy, e.ty, e.yaw, e.dyaw, e.ddyaw);
+    return e;
+}
+
+// ---------------------------------------------------------------------------------------------
+// Post-solve quality scan (SURVEY 8f-4): ALMTrajOpt::getMaxVxAxAyCurAttSig (alm_traj_opt.h:170-229) and
+// SE2Trajectory::getNonHolError (se2traj.hpp:551-561), one warp per trajectory, one lane per sample time.  The reference keeps "the
+// first sample with the largest |value|": every lane keeps its own slice, the warp reduces by (|value|, earliest sample), and the
+// non-holonomic error is summed in sample order -- bit-identical to the sequential loops (oracle: orc_feasibility).
+// ---------------------------------------------------------------------------------------------
 struct AbsMax {   // "if (fabs(best) < fabs(v)) best = v" over samples in time order
     R val; int idx;
     __device__ __forceinline__ void init() { val = 0.0; idx = 0x7fffffff; }
@@ -2505,143 +2547,68 @@ struct AbsMax {   // "if (fabs(best) < fabs(v)) best = v" over samples in time o
     }
 };
 // The values of one sample at time tm < the trajectory's duration: vx, ax, ay, cur, att and sig of getMaxVxAxAyCurAttSig and the
-// term getNonHolError sums.  feasibility_kernel and check_kernel both take their samples from here, so they compute the same bits
+// term getNonHolError sums
 struct FeasSample { R vx, ax, ay, cur, att, sig, term; };
 __device__ __forceinline__ FeasSample feas_sample(const DevMap &map, R gravity, const R *cxy, const R *cyaw, int N, int M, R Tx, R Ty, R tm)
 {
-    const int nx = 6 * N;
-    R tl = tm;
-    const int ip = locate_piece(N, Tx, tl);
-    R px, py, vxw, vyw, axw, ayw, yaw, dyaw, dd;
-    piece_eval(cxy + 6 * ip, tl, px, vxw, axw);
-    piece_eval(cxy + nx + 6 * ip, tl, py, vyw, ayw);
-    R ty = tm;
-    const int iy = locate_piece(M, Ty, ty);
-    piece_eval(cyaw + 6 * iy, ty, yaw, dyaw, dd);
-    R se2[3] = {px, py, yaw};
+    const SE2Eval e = se2_eval(cxy, cyaw, N, M, Tx, Ty, tm, tm);
+    R se2[3] = {e.x, e.y, e.yaw};
     normSO2(se2[2]);                                  // getNormSE2Pos (se2traj.hpp:433-443)
     R tv[7], tg[7][3];
     map_get_all_with_grad(map, se2, tv, tg);          // values as getTerrainVariables (uneven_map.h:221-256)
-    const double2 sc = dev_sincos(yaw);
+    const double2 sc = dev_sincos(e.yaw);
     const R sy_ = sc.x, cy_ = sc.y;
-    const R vnorm = sqrt(vxw * vxw + vyw * vyw);
-    const R lon = axw * cy_ + ayw * sy_;
-    const R lat = -axw * sy_ + ayw * cy_;
+    const R vnorm = sqrt(e.vx * e.vx + e.vy * e.vy);
+    const R lon = e.ax * cy_ + e.ay * sy_;
+    const R lat = -e.ax * sy_ + e.ay * cy_;
     FeasSample s;
     s.vx = vnorm * tv[0];
     s.ax = lon * tv[0] + gravity * tv[1];
     s.ay = lat * tv[2] + gravity * tv[3];
-    const R wz = dyaw * tv[5];
+    const R wz = e.dyaw * tv[5];
     s.cur = wz / sqrt(s.vx * s.vx + UALM_DELTA_SIGL);
     s.att = -1.0 / tv[5];
     s.sig = tv[6];
-    s.term = fabs(vxw * sy_ + vyw * (-cy_));
+    s.term = fabs(e.vx * sy_ + e.vy * (-cy_));
     return s;
 }
-// idx: the n problems to scan (those of one environment, whose parameters and grid this launch carries), or null for 0 .. n - 1
-__global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) feasibility_kernel(const __grid_constant__ BatchPtrs bp, const __grid_constant__ DevParams p,
-        const __grid_constant__ DevMap map, R dt, R *out, const int *idx, int n)
-{
-    const int lane = threadIdx.x & 31, w = blockIdx.x * UALM_WPB + (threadIdx.x >> 5);
-    if (w >= n) return;         // whole warp exits
-    const int prob = idx ? idx[w] : w;
-    const ProbDesc *pd = bp.desc + prob;
-    if (pd->S == 0) {            // over the compiled limits: not solved (ret_code = UALM_ELIMIT)
-        if (lane < 10) out[10 * (size_t)prob + lane] = 0.0;
-        return;
-    }
-    const int N = pd->N, M = pd->M;
-    const R *cxy = bp.c_xy + pd->off_cxy, *cyaw = bp.c_yaw + pd->off_cyaw;
-    const R Tx = bp.piece_T[2 * prob], Ty = bp.piece_T[2 * prob + 1];
-    R tot_xy = 0.0, tot_yaw = 0.0;    // PolyTrajectory::getTotalDuration (se2traj.hpp:291-300), SE2: the smaller one (:415-418)
-    for (int i = 0; i < N; i++) tot_xy += Tx;
-    for (int i = 0; i < M; i++) tot_yaw += Ty;
-    const R total = tot_xy < tot_yaw ? tot_xy : tot_yaw;
-    // a diverged solve can leave an astronomically long (or non-finite) duration: the reference's scan would then run (almost) forever.
-    // Such a trajectory is reported as "not scanned": zeros and a sample count of -1.
-    if (!(total / dt < 4.0e6)) {
-        if (lane == 0) {
-            R *o = out + 10 * (size_t)prob;
-            for (int q = 0; q < 7; q++) o[q] = 0.0;
-            o[7] = -1.0; o[8] = Tx; o[9] = Ty;
-        }
-        return;
-    }
-    AbsMax mvx, max_, may, mcur;
-    mvx.init(); max_.init(); may.init(); mcur.init();
-    R matt = -1.0, msig = 0.0, err = 0.0;
-    long long count = 0;
-    R tbase = 0.0;
-    int kbase = 0;
-    while (true) {
-        R tm = 0.0, tt = tbase;
-        for (int i = 0; i < 32; i++) { if (i == lane) tm = tt; tt = tt + dt; }   // the reference's t += 0.01, same additions on every lane
-        const bool valid = tm < total;
-        R term = 0.0;
-        if (valid) {
-            const FeasSample s = feas_sample(map, p.gravity, cxy, cyaw, N, M, Tx, Ty, tm);
-            const int k = kbase + lane;
-            max_.see(s.ax, k); may.see(s.ay, k); mvx.see(s.vx, k); mcur.see(s.cur, k);
-            if (matt < s.att) matt = s.att;
-            if (msig < s.sig) msig = s.sig;
-            term = s.term;
-        }
-        const int cnt = __popc(__ballot_sync(0xffffffffu, valid));   // the valid lanes are a prefix: t grows with the lane
-        for (int l = 0; l < cnt; l++) err += __shfl_sync(0xffffffffu, term, l);
-        count += cnt;
-        if (cnt < 32) break;
-        tbase = tt; kbase += 32;
-    }
-    mvx.reduce(); max_.reduce(); may.reduce(); mcur.reduce();
-#pragma unroll
-    for (int off = 16; off >= 1; off >>= 1) {
-        const R oa = __shfl_xor_sync(0xffffffffu, matt, off), os = __shfl_xor_sync(0xffffffffu, msig, off);
-        if (matt < oa) matt = oa;
-        if (msig < os) msig = os;
-    }
-    if (lane == 0) {
-        R *o = out + 10 * (size_t)prob;
-        o[0] = mvx.val; o[1] = max_.val; o[2] = may.val; o[3] = mcur.val; o[4] = matt; o[5] = msig; o[6] = err; o[7] = (R)count; o[8] = Tx; o[9] = Ty;
-    }
-}
-
-// ---------------------------------------------------------------------------------------------
-// The same scan of trajectories the caller holds (ualm_check_trajectories), restricted to the samples t >= t_from of the reference's
-// sequence t = 0, dt, 2dt.. (the sequence is not restarted at t_from, so every kept sample is bit for bit the full scan's), with the
-// time of the first kept sample that breaks each of six limits.  One warp per trajectory, one lane per sample; a first violation is
-// the earliest set lane of its ballot in the first chunk that has one.  Oracle: tests/check_oracle.cpp.
-// out[16 * problem + ...] = the ten values of feasibility_kernel over the kept samples, then the first-violation times of
-// |vx| > max_vel, |ax| > max_acc_lon, |ay| > max_acc_lat, |cur| > max_kap, att > -min_cxi, sig > max_sig (-1: none)
-// ---------------------------------------------------------------------------------------------
-struct CheckLimits { R max_vel, max_acc_lon, max_acc_lat, max_kap, min_cxi, max_sig; };
+// The scan of solved trajectories (ualm_feasibility_batch, t_from null) and of trajectories the caller holds
+// (ualm_check_trajectories), restricted to the samples t >= t_from of the sequence t = 0, dt, 2dt.. (not restarted at t_from, so
+// every kept sample is bit for bit the full scan's), with the time of the first kept sample that breaks each of six limits; a first
+// violation is the earliest set lane of its ballot in the first chunk that has one.  Oracle: tests/check_oracle.cpp.
+// out[16 * problem + ...] = {max_vx, max_ax, max_ay, max_cur, max_att, max_sig, nonhol_error, samples, T_xy piece, T_yaw piece} over
+// the kept samples, then the first-violation times of |vx| > max_vel, |ax| > max_acc_lon, |ay| > max_acc_lat, |cur| > max_kap,
+// att > -min_cxi, sig > max_sig (-1: none).  Not scanned (over the compiled limits, or more than 4e6 samples): zeros, a sample count
+// of -1, no violation, and the piece durations of a trajectory within the limits
 struct CheckPtrs {
-    const ProbDesc *desc;          // N, M, off_cxy, off_cyaw; S == 0 marks a problem over the compiled limits
-    const R *c_xy, *c_yaw, *piece_T, *t_from;
+    const ProbDesc *desc;          // N, M, off_cxy, off_cyaw, the six limits at pp[2..7]; S == 0 marks a problem over the compiled limits
+    const R *c_xy, *c_yaw, *piece_T;
+    const R *t_from;               // null: 0 for every problem
     R *out;
 };
-// idx: the n problems to check, those of one environment, whose grid and gravity this launch carries; lims[problem]: its limits
+// idx: the n problems to scan, those of one environment, whose grid and gravity this launch carries
 __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) check_kernel(const __grid_constant__ CheckPtrs a, const __grid_constant__ DevMap map, R gravity,
-        const CheckLimits *lims, R dt, const int *idx, int n)
+        R dt, const int *idx, int n)
 {
     const int lane = threadIdx.x & 31, w = blockIdx.x * UALM_WPB + (threadIdx.x >> 5);
     if (w >= n) return;         // whole warp exits
     const int prob = idx[w];
-    const CheckLimits lim = lims[prob];
     const ProbDesc *pd = a.desc + prob;
     R *o = a.out + 16 * (size_t)prob;
-    const R Tx = a.piece_T[2 * prob], Ty = a.piece_T[2 * prob + 1];
-    const int N = pd->N, M = pd->M;
-    R tot_xy = 0.0, tot_yaw = 0.0;
-    for (int i = 0; i < N && pd->S; i++) tot_xy += Tx;
-    for (int i = 0; i < M && pd->S; i++) tot_yaw += Ty;
-    const R total = tot_xy < tot_yaw ? tot_xy : tot_yaw;
-    // over the compiled limits: zeros; more than 4e6 samples: zeros and the piece durations, as feasibility_kernel.  Both "not scanned"
-    if (pd->S == 0 || !(total / dt < 4.0e6)) {
-        if (lane < 16) o[lane] = lane == 7 || lane >= 10 ? -1.0 : pd->S && lane == 8 ? Tx : pd->S && lane == 9 ? Ty : 0.0;
+    if (pd->S == 0) {
+        if (lane < 16) o[lane] = lane == 7 || lane >= 10 ? -1.0 : 0.0;
         return;
     }
-    const R *cxy = a.c_xy + pd->off_cxy, *cyaw = a.c_yaw + pd->off_cyaw;
-    const R t0 = a.t_from[prob];
+    const R Tx = a.piece_T[2 * prob], Ty = a.piece_T[2 * prob + 1];
+    const int N = pd->N, M = pd->M;
+    const TrajDur d = traj_duration(N, M, Tx, Ty);
+    if (!d.scannable(dt)) {
+        if (lane < 16) o[lane] = lane == 7 || lane >= 10 ? -1.0 : lane == 8 ? Tx : lane == 9 ? Ty : 0.0;
+        return;
+    }
+    const R *cxy = a.c_xy + pd->off_cxy, *cyaw = a.c_yaw + pd->off_cyaw, *lim = pd->pp + 2;
+    const R max_vel = lim[0], max_acc_lon = lim[1], max_acc_lat = lim[2], max_kap = lim[3], min_cxi = lim[4], max_sig = lim[5];
+    const R t0 = a.t_from ? a.t_from[prob] : 0.0;
     AbsMax mvx, max_, may, mcur;
     mvx.init(); max_.init(); may.init(); mcur.init();
     R matt = -1.0, msig = 0.0, err = 0.0;
@@ -2649,11 +2616,9 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) check_kernel(const __
     unsigned found = 0;
     long long count = 0;
     R tbase = 0.0;
-    int kbase = 0;
-    while (true) {
-        R tm = 0.0, tt = tbase;
-        for (int i = 0; i < 32; i++) { if (i == lane) tm = tt; tt = tt + dt; }   // the reference's t += dt, same additions on every lane
-        const bool valid = tm < total, kept = valid && tm >= t0;
+    for (int kbase = 0;; kbase += 32) {
+        const R tm = chunk_time(tbase, dt, lane);
+        const bool valid = tm < d.total, kept = valid && tm >= t0;
         R term = 0.0;
         unsigned viol = 0;
         if (kept) {
@@ -2663,8 +2628,8 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) check_kernel(const __
             if (matt < s.att) matt = s.att;
             if (msig < s.sig) msig = s.sig;
             term = s.term;
-            viol = (fabs(s.vx) > lim.max_vel ? 1u : 0u) | (fabs(s.ax) > lim.max_acc_lon ? 2u : 0u) | (fabs(s.ay) > lim.max_acc_lat ? 4u : 0u) |
-                   (fabs(s.cur) > lim.max_kap ? 8u : 0u) | (s.att > -lim.min_cxi ? 16u : 0u) | (s.sig > lim.max_sig ? 32u : 0u);
+            viol = (fabs(s.vx) > max_vel ? 1u : 0u) | (fabs(s.ax) > max_acc_lon ? 2u : 0u) | (fabs(s.ay) > max_acc_lat ? 4u : 0u) |
+                   (fabs(s.cur) > max_kap ? 8u : 0u) | (s.att > -min_cxi ? 16u : 0u) | (s.sig > max_sig ? 32u : 0u);
         }
         const unsigned km = __ballot_sync(0xffffffffu, kept);   // the kept lanes are contiguous: t grows with the lane
         for (unsigned m = km; m; m &= m - 1) err += __shfl_sync(0xffffffffu, term, __ffs(m) - 1);
@@ -2676,7 +2641,6 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) check_kernel(const __
             if (vm && !((found >> q) & 1u)) { first[q] = tv; found |= 1u << q; }
         }
         if (__popc(__ballot_sync(0xffffffffu, valid)) < 32) break;
-        tbase = tt; kbase += 32;
     }
     mvx.reduce(); max_.reduce(); may.reduce(); mcur.reduce();
 #pragma unroll
@@ -2692,9 +2656,9 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) check_kernel(const __
 }
 
 // ---------------------------------------------------------------------------------------------
-// Replanned problems of trajectories the caller holds (ualm_submit_replan): the state at tau = t_from (locate_piece + piece_eval),
-// then PlanManager's resampler (resample_stream.h) over the polyline {the point at tau, the samples tau < t < duration of the
-// reference's sequence t = 0, dt, 2dt.. (the same additions as check_kernel), the goal of the original problem}.  One warp per row:
+// Replanned problems of trajectories the caller holds (ualm_submit_replan): the state at tau = t_from, then PlanManager's resampler
+// (resample_stream.h) over the polyline {the point at tau, the samples tau < t < duration of the reference's sequence
+// t = 0, dt, 2dt.., the goal of the original problem}.  One warp per row:
 // each chunk the lanes evaluate 32 sample times, then every lane runs the sequential resampler on the same points broadcast by
 // shuffle, and lane 0 writes.  Waypoints past the compiled limits are counted, not formed; such a row's inner points are zeros.  The
 // stream is bounded (ualm_rs_push), so a row's serial work is bounded whatever its lengths and yaws.
@@ -2721,39 +2685,20 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) replan_kernel(const _
     R *o = a.out + UALM_REPLAN_STRIDE * (size_t)w, *oxy = o + 21, *oyaw = oxy + UALM_REPLAN_INNER_XY;
     for (int q = lane; q < UALM_REPLAN_INNER_XY + UALM_REPLAN_INNER_YAW; q += 32) oxy[q] = 0.0;
     __syncwarp();
-    R tot_xy = 0.0, tot_yaw = 0.0;
-    for (int i = 0; i < N; i++) tot_xy += Tx;
-    for (int i = 0; i < M; i++) tot_yaw += Ty;
-    const R total = tot_xy < tot_yaw ? tot_xy : tot_yaw;
-    // the start state (every lane)
-    R px, py, vx, vy, ax, ay, yaw, dyaw, ddyaw;
-    {
-        R tl = t0;
-        const int ip = locate_piece(N, Tx, tl);
-        piece_eval(cxy + 6 * ip, tl, px, vx, ax);
-        piece_eval(cxy + 6 * N + 6 * ip, tl, py, vy, ay);
-        R ty = t0;
-        const int iy = locate_piece(M, Ty, ty);
-        piece_eval(cyaw + 6 * iy, ty, yaw, dyaw, ddyaw);
-    }
+    const R total = traj_duration(N, M, Tx, Ty).total;
+    const SE2Eval st = se2_eval(cxy, cyaw, N, M, Tx, Ty, t0, t0);     // the start state (every lane)
     R *wxy = lane == 0 ? oxy : nullptr, *wyaw = lane == 0 ? oyaw : nullptr;
     UalmResampleStream s;
     ualm_rs_init(s, rp.piece_len, rp.yaw_piece_times);
-    ualm_rs_push(s, px, py, yaw, wxy, UALM_NMAX - 1, wyaw, UALM_MMAX - 1);
+    ualm_rs_push(s, st.x, st.y, st.yaw, wxy, UALM_NMAX - 1, wyaw, UALM_MMAX - 1);
     R tbase = 0.0;
     while (true) {
-        R tm = 0.0, tt = tbase;
-        for (int i = 0; i < 32; i++) { if (i == lane) tm = tt; tt = tt + rp.dt; }   // check_kernel's additions
+        const R tm = chunk_time(tbase, rp.dt, lane);
         const bool valid = tm < total, kept = valid && tm > t0;
         R x = 0.0, y = 0.0, h = 0.0;
-        if (kept) {     // feas_sample's evaluation
-            R tl = tm, d1, d2;
-            const int ip = locate_piece(N, Tx, tl);
-            piece_eval(cxy + 6 * ip, tl, x, d1, d2);
-            piece_eval(cxy + 6 * N + 6 * ip, tl, y, d1, d2);
-            R ty = tm;
-            const int iy = locate_piece(M, Ty, ty);
-            piece_eval(cyaw + 6 * iy, ty, h, d1, d2);
+        if (kept) {
+            const SE2Eval e = se2_eval(cxy, cyaw, N, M, Tx, Ty, tm, tm);
+            x = e.x; y = e.y; h = e.yaw;
         }
         const unsigned km = __ballot_sync(0xffffffffu, kept);   // the kept lanes are contiguous: t grows with the lane
         for (unsigned m = km; m; m &= m - 1) {
@@ -2762,7 +2707,6 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) replan_kernel(const _
             ualm_rs_push(s, bx, by, bh, wxy, UALM_NMAX - 1, wyaw, UALM_MMAX - 1);
         }
         if (__popc(__ballot_sync(0xffffffffu, valid)) < 32) break;
-        tbase = tt;
     }
     ualm_rs_push(s, bnd[6], bnd[7], bnd[15], wxy, UALM_NMAX - 1, wyaw, UALM_MMAX - 1);   // the goal: end_xy's position, end_yaw's angle
     // cut short (resample_stream.h: a huge or non-finite length or yaw): over the limits, N' = M' = UALM_RS_MAX_WAYPOINTS + 2
@@ -2772,7 +2716,8 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) replan_kernel(const _
         for (int q = lane; q < UALM_REPLAN_INNER_XY + UALM_REPLAN_INNER_YAW; q += 32) oxy[q] = 0.0;
     }
     if (lane == 0) {
-        const R head[18] = {px, py, vx, vy, ax, ay, bnd[6], bnd[7], bnd[8], bnd[9], bnd[10], bnd[11], yaw, dyaw, ddyaw, bnd[15], bnd[16], bnd[17]};
+        const R head[18] = {st.x, st.y, st.vx, st.vy, st.ax, st.ay, bnd[6], bnd[7], bnd[8], bnd[9], bnd[10], bnd[11], st.yaw, st.dyaw, st.ddyaw,
+                            bnd[15], bnd[16], bnd[17]};
         for (int k = 0; k < 18; k++) o[k] = head[k];
         o[18] = ualm_rs_total_time(s, rp.mean_vel, rp.init_time_times);
         o[19] = (R)Nn; o[20] = (R)Mn;
@@ -2869,21 +2814,14 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) mpc_export_kernel(con
     }
     const R *cxy = bp.c_xy + pd->off_cxy, *cyaw = bp.c_yaw + pd->off_cyaw;
     const R Tx = bp.piece_T[2 * prob], Ty = bp.piece_T[2 * prob + 1];
-    R tot_xy = 0.0, tot_yaw = 0.0;
-    for (int i = 0; i < N; i++) tot_xy += Tx;
-    for (int i = 0; i < M; i++) tot_yaw += Ty;
+    const TrajDur d = traj_duration(N, M, Tx, Ty);
     // (1) the message: piece start points are the constant coefficients (getValue(0) only adds exact zeros to them); the end point is
     // PolyTrajectory::getValue at the summed duration
     for (int i = lane; i < N; i += 32) { pp[2 * i] = cxy[6 * i]; pp[2 * i + 1] = cxy[nx + 6 * i]; pt[i] = Tx; }
     for (int i = lane; i < M; i += 32) { ap[i] = cyaw[6 * i]; at[i] = Ty; }
     if (lane == 0) {
-        R t = tot_xy, d1, d2;
-        const int ip = locate_piece(N, Tx, t);
-        piece_eval(cxy + 6 * ip, t, pp[2 * N], d1, d2);
-        piece_eval(cxy + nx + 6 * ip, t, pp[2 * N + 1], d1, d2);
-        t = tot_yaw;
-        const int iy = locate_piece(M, Ty, t);
-        piece_eval(cyaw + 6 * iy, t, ap[M], d1, d2);
+        const SE2Eval e = se2_eval(cxy, cyaw, N, M, Tx, Ty, d.xy, d.yaw);
+        pp[2 * N] = e.x; pp[2 * N + 1] = e.y; ap[M] = e.yaw;
     }
     __syncwarp();
     // (2) the MPC's own MINCO over the message
@@ -2892,31 +2830,25 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) mpc_export_kernel(con
     if (lane == 1) mpc_minco_serial(BandView{band + 13 * nx, 6 * M}, M, 1, Ty, ap, 1, 0, o.init_v + 2, o.init_a + 2, myaw);
     __syncwarp();
     // (3) planned against tracked, over the shorter of the two durations like every scan of the reference (se2traj.hpp:415-418)
-    const R total = tot_xy < tot_yaw ? tot_xy : tot_yaw;
-    if (!(total / dt < 4.0e6)) {
+    if (!d.scannable(dt)) {
         if (lane == 0) { dv[0] = -1.0; dv[1] = 0.0; dv[2] = -1.0; dv[3] = 0.0; }
         return;
     }
     R bp_ = 0.0, bpt = 0.0, by_ = 0.0, byt = 0.0;
     R tbase = 0.0;
     while (true) {
-        R tm = 0.0, tt = tbase;
-        for (int i = 0; i < 32; i++) { if (i == lane) tm = tt; tt = tt + dt; }
-        const bool valid = tm < total;
+        const R tm = chunk_time(tbase, dt, lane);
+        const bool valid = tm < d.total;
         if (valid) {
-            R tl = tm, d1, d2, px, py, qx, qy, ya, yb;
-            const int ip = locate_piece(N, Tx, tl);
-            piece_eval(cxy + 6 * ip, tl, px, d1, d2); piece_eval(cxy + nx + 6 * ip, tl, py, d1, d2);
-            piece_eval(mxy + 6 * ip, tl, qx, d1, d2); piece_eval(mxy + nx + 6 * ip, tl, qy, d1, d2);
-            R ty = tm;
-            const int iy = locate_piece(M, Ty, ty);
-            piece_eval(cyaw + 6 * iy, ty, ya, d1, d2); piece_eval(myaw + 6 * iy, ty, yb, d1, d2);
-            const R ep = sqrt((px - qx) * (px - qx) + (py - qy) * (py - qy)), ey = fabs(ya - yb);
+            const SE2Eval e = se2_eval(cxy, cyaw, N, M, Tx, Ty, tm, tm);
+            R qx, qy, yb, d1, d2;      // the tracked trajectory, whose pieces last as long as the planned one's
+            piece_eval(mxy + 6 * e.ip, e.tl, qx, d1, d2); piece_eval(mxy + nx + 6 * e.ip, e.tl, qy, d1, d2);
+            piece_eval(myaw + 6 * e.iy, e.ty, yb, d1, d2);
+            const R ep = sqrt((e.x - qx) * (e.x - qx) + (e.y - qy) * (e.y - qy)), ey = fabs(e.yaw - yb);
             if (bp_ < ep) { bp_ = ep; bpt = tm; }
             if (by_ < ey) { by_ = ey; byt = tm; }
         }
         if (__popc(__ballot_sync(0xffffffffu, valid)) < 32) break;
-        tbase = tt;
     }
 #pragma unroll
     for (int off = 16; off >= 1; off >>= 1) {      // largest value, earliest time among equals
