@@ -1160,8 +1160,13 @@ struct ALM {
     }
 };
 
-template <class R>
-static int solve_impl(const orc_params_t *p, const orc_map_t *map, const orc_problem_t *prob, orc_result_t *res,
+constexpr int RET_STOPPED = 3;   /* UALM_RET_STOPPED (include/ualm.h) */
+
+/* stop(n_evals, site) is the stop test of the CUDA paths (an evaluation budget, a cancel), called once per test in execution order:
+ * site 0 where earlyExit tests k > 1000 (L-BFGS then returns CANCELED), site 1 after judgeConvergence when the inner solve was not
+ * ended by a stop and the problem has not converged.  orc_solve / orc_solve_f32 pass a stop that never holds. */
+template <class R, class Stop>
+static int solve_impl(const orc_params_t *p, const orc_map_t *map, const orc_problem_t *prob, Stop stop, orc_result_t *res,
                       double *c_xy_out, double *c_yaw_out, double *x_out, double *lambda_out, double *mu_out,
                       double *scale_cx_out)
 {
@@ -1187,9 +1192,13 @@ static int solve_impl(const orc_params_t *p, const orc_map_t *map, const orc_pro
     if (alm.use_scaling) alm.initScaling(x);
 
     auto eval = [&](const std::vector<R> &xx, std::vector<R> &gg) { return alm.evaluate(xx, gg); };
-    auto progress = [&](int k) { return k > 1e3; }; /* earlyExit alm_traj_opt.cpp:1016 */
+    bool fired = false;   /* the stop ended the inner solve that just returned */
+    auto progress = [&](int k) { fired = stop(alm.n_evals, 0); return k > 1e3 || fired; }; /* earlyExit alm_traj_opt.cpp:1016 */
     R rh = 0, rg = 0;
+    /* Exit order: a stop that ended the inner solve just finished -> RET_STOPPED even when judgeConvergence passes; else
+     * converged -> 0; else the stop holds now -> RET_STOPPED; else ++iter > max_iter -> 2 */
     while (true) {
+        fired = false;
         auto a = clk::now();
         int result = lbfgs_optimize(x, inner_cost, eval, progress, lp, st);
         t_lbfgs_all += secs(a, clk::now());
@@ -1199,7 +1208,10 @@ static int solve_impl(const orc_params_t *p, const orc_map_t *map, const orc_pro
         } else if (result == LBFGSERR_MAXIMUMLINESEARCH) {
         } else { ret_code = 1; break; }
         alm.updateDualVars();
-        if (alm.judgeConvergence(rh, rg)) break;
+        const bool converged = alm.judgeConvergence(rh, rg);
+        if (fired) { ret_code = RET_STOPPED; break; }
+        if (converged) break;
+        if (stop(alm.n_evals, 1)) { ret_code = RET_STOPPED; break; }
         if (++iter > alm.max_iter) { ret_code = 2; break; }
     }
     res->ret_code = ret_code; res->outer_iters = iter; res->n_evals = alm.n_evals; res->n_lbfgs_iters = st.iters;
@@ -1221,6 +1233,8 @@ static int solve_impl(const orc_params_t *p, const orc_map_t *map, const orc_pro
     return ret_code;
 }
 
+inline bool never_stop(int, int) { return false; }
+
 } // namespace
 
 extern "C" {
@@ -1229,13 +1243,13 @@ int orc_solve(const orc_params_t *p, const orc_map_t *map, const orc_problem_t *
               double *c_xy_out, double *c_yaw_out, double *x_out, double *lambda_out, double *mu_out,
               double *scale_cx_out)
 {
-    return solve_impl<double>(p, map, prob, res, c_xy_out, c_yaw_out, x_out, lambda_out, mu_out, scale_cx_out);
+    return solve_impl<double>(p, map, prob, never_stop, res, c_xy_out, c_yaw_out, x_out, lambda_out, mu_out, scale_cx_out);
 }
 
 int orc_solve_f32(const orc_params_t *p, const orc_map_t *map, const orc_problem_t *prob, orc_result_t *res,
                   double *c_xy_out, double *c_yaw_out, double *x_out)
 {
-    return solve_impl<float>(p, map, prob, res, c_xy_out, c_yaw_out, x_out, nullptr, nullptr, nullptr);
+    return solve_impl<float>(p, map, prob, never_stop, res, c_xy_out, c_yaw_out, x_out, nullptr, nullptr, nullptr);
 }
 
 int orc_eval(const orc_params_t *p, const orc_map_t *map, const orc_problem_t *prob, const double *x,
@@ -1315,52 +1329,71 @@ inline double piece_ddot(const double *c, double t) /* se2traj.hpp:136-150 */
     for (int k = 2; k <= 5; k++) { v += m * n * tn * c[k]; tn *= t; m++; n++; }
     return v;
 }
+/* PolyTrajectory::getTotalDuration (se2traj.hpp:291-300) of the xy and the yaw part, each summed piece by piece: an SE2 trajectory
+ * lasts the smaller (se2traj.hpp:415-418) */
+inline double traj_duration(int N, int M, double T_xy, double T_yaw)
+{
+    double tot_xy = 0.0, tot_yaw = 0.0;
+    for (int i = 0; i < N; i++) tot_xy += T_xy;
+    for (int i = 0; i < M; i++) tot_yaw += T_yaw;
+    return std::min(tot_xy, tot_yaw);
+}
+/* The pieces at time t and the position, velocity and acceleration of the xy and the yaw part there (PolyTrajectory::getValue /
+ * getVel / getAcc, se2traj.hpp:363-391) */
+struct SE2State { int ip, iy; double x, y, yaw, vx, vy, dyaw, ax, ay, ddyaw; };
+inline SE2State se2_eval(int N, int M, const double *c_xy, const double *c_yaw, double T_xy, double T_yaw, double t)
+{
+    double tl = t, ty = t;
+    const int ip = locate_piece(N, T_xy, tl), iy = locate_piece(M, T_yaw, ty);
+    const double *cx = c_xy + 6 * ip, *cy = c_xy + 6 * N + 6 * ip, *cw = c_yaw + 6 * iy;
+    return {ip, iy, piece_value(cx, tl), piece_value(cy, tl), piece_value(cw, ty), piece_dot(cx, tl), piece_dot(cy, tl),
+            piece_dot(cw, ty), piece_ddot(cx, tl), piece_ddot(cy, tl), piece_ddot(cw, ty)};
+}
+/* One sample of the post-solve scan at time t: vx, ax, ay, cur, att and sig of getMaxVxAxAyCurAttSig and the term getNonHolError
+ * sums */
+struct ScanSample { double vx, ax, ay, cur, att, sig, term; };
+inline ScanSample scan_sample(const MapQ<double> &mq, double gravity, int N, int M, const double *c_xy, const double *c_yaw,
+                              double T_xy, double T_yaw, double t)
+{
+    const SE2State e = se2_eval(N, M, c_xy, c_yaw, T_xy, T_yaw, t);
+    double se2[3] = {e.x, e.y, e.yaw};
+    while (se2[2] < -M_PI) se2[2] += 2 * M_PI; /* getNormSE2Pos, se2traj.hpp:433-443 */
+    while (se2[2] > M_PI) se2[2] -= 2 * M_PI;
+    double tv[7], tg[7][3];
+    mq.getAllWithGrad(se2, tv, tg);
+    const double cy_ = Mth<double>::cos(e.yaw), sy_ = Mth<double>::sin(e.yaw);
+    const double vnorm = std::sqrt(e.vx * e.vx + e.vy * e.vy);   /* getVelNorm */
+    const double lon = e.ax * cy_ + e.ay * sy_;                  /* getLonAcc */
+    const double lat = -e.ax * sy_ + e.ay * cy_;                 /* getLatAcc */
+    ScanSample s;
+    s.vx = vnorm * tv[0];
+    s.ax = lon * tv[0] + gravity * tv[1];
+    s.ay = lat * tv[2] + gravity * tv[3];
+    const double wz = e.dyaw * tv[5];
+    s.cur = wz / std::sqrt(s.vx * s.vx + delta_sigl);
+    s.att = -1.0 / tv[5];
+    s.sig = tv[6];
+    s.term = std::fabs(e.vx * sy_ + e.vy * (-cy_));              /* getNonHolError */
+    return s;
+}
 } // namespace
 
 void orc_feasibility(const orc_map_t *map, double gravity, int N, int M, const double *c_xy, const double *c_yaw, double T_xy,
                      double T_yaw, double dt, double *out)
 {
     MapQ<double> mq(*map);
-    const int nx = 6 * N;
-    double tot_xy = 0.0, tot_yaw = 0.0; /* PolyTrajectory::getTotalDuration, se2traj.hpp:291-300 */
-    for (int i = 0; i < N; i++) tot_xy += T_xy;
-    for (int i = 0; i < M; i++) tot_yaw += T_yaw;
-    const double total = std::min(tot_xy, tot_yaw); /* se2traj.hpp:415-418 */
+    const double total = traj_duration(N, M, T_xy, T_yaw);
     double max_ax = 0.0, max_ay = 0.0, max_vx = 0.0, max_cur = 0.0, max_att = -1.0, max_sig = 0.0, err = 0.0;
     long count = 0;
     for (double t = 0.0; t < total; t += dt) {
-        double tl = t;
-        const int ip = locate_piece(N, T_xy, tl);
-        const double *cx = c_xy + 6 * ip, *cy = c_xy + nx + 6 * ip;
-        const double px = piece_value(cx, tl), py = piece_value(cy, tl);
-        const double vxw = piece_dot(cx, tl), vyw = piece_dot(cy, tl);
-        const double axw = piece_ddot(cx, tl), ayw = piece_ddot(cy, tl);
-        double ty = t;
-        const int iy = locate_piece(M, T_yaw, ty);
-        const double *cw = c_yaw + 6 * iy;
-        const double yaw = piece_value(cw, ty), dyaw = piece_dot(cw, ty);
-        double se2[3] = {px, py, yaw};
-        while (se2[2] < -M_PI) se2[2] += 2 * M_PI; /* getNormSE2Pos, se2traj.hpp:433-443 */
-        while (se2[2] > M_PI) se2[2] -= 2 * M_PI;
-        double tv[7], tg[7][3];
-        mq.getAllWithGrad(se2, tv, tg);
-        const double cy_ = Mth<double>::cos(yaw), sy_ = Mth<double>::sin(yaw);
-        const double vnorm = std::sqrt(vxw * vxw + vyw * vyw);       /* getVelNorm */
-        const double lon = axw * cy_ + ayw * sy_;                    /* getLonAcc */
-        const double lat = -axw * sy_ + ayw * cy_;                   /* getLatAcc */
-        const double vx = vnorm * tv[0];
-        const double ax = lon * tv[0] + gravity * tv[1];
-        const double ay = lat * tv[2] + gravity * tv[3];
-        const double wz = dyaw * tv[5];
-        const double cur = wz / std::sqrt(vx * vx + delta_sigl);
-        const double att = -1.0 / tv[5];
-        if (std::fabs(max_ax) < std::fabs(ax)) max_ax = ax;
-        if (std::fabs(max_ay) < std::fabs(ay)) max_ay = ay;
-        if (std::fabs(max_vx) < std::fabs(vx)) max_vx = vx;
-        if (std::fabs(max_cur) < std::fabs(cur)) max_cur = cur;
-        if (max_att < att) max_att = att;
-        if (max_sig < tv[6]) max_sig = tv[6];
-        err += std::fabs(vxw * sy_ + vyw * (-cy_));                  /* getNonHolError */
+        const ScanSample s = scan_sample(mq, gravity, N, M, c_xy, c_yaw, T_xy, T_yaw, t);
+        if (std::fabs(max_ax) < std::fabs(s.ax)) max_ax = s.ax;
+        if (std::fabs(max_ay) < std::fabs(s.ay)) max_ay = s.ay;
+        if (std::fabs(max_vx) < std::fabs(s.vx)) max_vx = s.vx;
+        if (std::fabs(max_cur) < std::fabs(s.cur)) max_cur = s.cur;
+        if (max_att < s.att) max_att = s.att;
+        if (max_sig < s.sig) max_sig = s.sig;
+        err += s.term;
         count++;
     }
     out[0] = max_vx; out[1] = max_ax; out[2] = max_ay; out[3] = max_cur; out[4] = max_att; out[5] = max_sig; out[6] = err;

@@ -1,6 +1,6 @@
 // replan_oracle.cpp -- the CPU reference of ualm_submit_replan's build (include/ualm.h): the state at t_from and the (x, y, yaw) points of
-// the trajectory by the oracle's own piece lookup and evaluation (oracle/oracle.cpp, included unmodified), and PlanManager's resampler
-// (plan_manager.cpp:62-122) restated here on its own.  TEST INFRASTRUCTURE ONLY, built by tests/replan_oracle.py.
+// the trajectory by the oracle's own durations and evaluation (traj_duration, se2_eval: oracle/oracle.cpp, included unmodified), and
+// PlanManager's resampler (plan_manager.cpp:62-122) restated here on its own.  TEST INFRASTRUCTURE ONLY, built by tests/replan_oracle.py.
 #include "../oracle/oracle.cpp"
 
 #include <vector>
@@ -66,36 +66,23 @@ extern "C" void orc_resample(const double *path_in, int npts, double piece_len, 
 extern "C" long long orc_replan_polyline(int N, int M, const double *c_xy, const double *c_yaw, double T_xy, double T_yaw, const double *bnd,
                                          double t_from, double dt, double *path, double *times, long long cap, double *head9)
 {
-    const int nx = 6 * N;
-    double tot_xy = 0.0, tot_yaw = 0.0;
-    for (int i = 0; i < N; i++) tot_xy += T_xy;
-    for (int i = 0; i < M; i++) tot_yaw += T_yaw;
-    const double total = std::min(tot_xy, tot_yaw);
+    const double total = traj_duration(N, M, T_xy, T_yaw);
     long long n = 0;
     auto put = [&](double x, double y, double yaw, double t) {
         if (path && n < cap) { path[3 * n] = x; path[3 * n + 1] = y; path[3 * n + 2] = yaw; }
         if (times && n < cap) times[n] = t;
         n++;
     };
-    auto at = [&](double t, double *s9) {
-        double tl = t;
-        const int ip = locate_piece(N, T_xy, tl);
-        const double *cx = c_xy + 6 * ip, *cy = c_xy + nx + 6 * ip;
-        double ty = t;
-        const int iy = locate_piece(M, T_yaw, ty);
-        const double *cw = c_yaw + 6 * iy;
-        const double v[9] = {piece_value(cx, tl), piece_value(cy, tl), piece_dot(cx, tl), piece_dot(cy, tl), piece_ddot(cx, tl), piece_ddot(cy, tl),
-                             piece_value(cw, ty), piece_dot(cw, ty), piece_ddot(cw, ty)};
-        for (int q = 0; q < 9; q++) s9[q] = v[q];
-    };
-    double s9[9];
-    at(t_from, s9);
-    if (head9) for (int q = 0; q < 9; q++) head9[q] = s9[q];
-    put(s9[0], s9[1], s9[6], t_from);
+    const SE2State h = se2_eval(N, M, c_xy, c_yaw, T_xy, T_yaw, t_from);
+    if (head9) {
+        const double v[9] = {h.x, h.y, h.vx, h.vy, h.ax, h.ay, h.yaw, h.dyaw, h.ddyaw};
+        for (int q = 0; q < 9; q++) head9[q] = v[q];
+    }
+    put(h.x, h.y, h.yaw, t_from);
     for (double t = 0.0; t < total; t += dt) {
         if (!(t > t_from)) continue;
-        at(t, s9);
-        put(s9[0], s9[1], s9[6], t);
+        const SE2State e = se2_eval(N, M, c_xy, c_yaw, T_xy, T_yaw, t);
+        put(e.x, e.y, e.yaw, t);
     }
     put(bnd[6], bnd[7], bnd[15], -1.0);
     return n;

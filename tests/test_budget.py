@@ -1,4 +1,4 @@
-"""Evaluation budget of a solve (include/ualm.h, UALM_RET_STOPPED) on the CPU: its reference (tests/budget_oracle.cpp, the oracle's
+"""Evaluation budget of a solve (include/ualm.h, UALM_RET_STOPPED) on the CPU: its reference (tests/stop_oracle.cpp, the oracle's
 solve with the stop predicate), and the C ABI entry points that need no device."""
 import os
 import sys
@@ -8,7 +8,7 @@ import pytest
 
 import pyoracle as po
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import budget_oracle as bo  # noqa: E402
+import stop_oracle as so  # noqa: E402
 from uneven_planner_b200 import configs, problems
 
 from harness import solve_diff
@@ -30,7 +30,7 @@ def test_no_budget_and_large_budget_match_golden(terrain, golden, name):
     om = po.OracleMap(m)
     free = po.solve_batch(prm, om, pb, threads=4)
     for max_evals in (0, int(gold["n_evals"].max()) + 1):
-        out = bo.solve_batch(prm, om, pb, max_evals, threads=4)
+        out = so.budget_batch(prm, om, pb, max_evals, threads=4)
         for o, f in zip(out, free):
             assert not solve_diff(o, f), solve_diff(o, f)          # the oracle's orc_solve
         assert np.array_equal(np.array([r[0].ret_code for r in out]), gold["ret_code"]), max_evals
@@ -48,7 +48,7 @@ def test_small_budgets(terrain, golden, name):
     free = po.solve_batch(prm, om, pb, threads=4)
     n_stopped = 0
     for max_evals in (1, 20, 100):
-        out = bo.solve_batch(prm, om, pb, max_evals, threads=4)
+        out = so.budget_batch(prm, om, pb, max_evals, threads=4)
         for i, (o, f) in enumerate(zip(out, free)):
             r = o[0]
             if r.ret_code != STOPPED:

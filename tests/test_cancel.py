@@ -1,5 +1,5 @@
 """Cancelling problems of a batch in flight (include/ualm.h: ualm_cancel_problems) on the CPU: the reference a cancelled parity-path
-solve is checked against (tests/cancel_oracle.cpp: the oracle's solve with a stop predicate that holds from its s-th stop test on),
+solve is checked against (tests/stop_oracle.cpp: the oracle's solve with a stop predicate that holds from its s-th stop test on),
 and the argument checks of the Python wrapper that need no device."""
 import os
 import sys
@@ -9,8 +9,7 @@ import pytest
 
 import pyoracle as po
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import budget_oracle as bo  # noqa: E402
-import cancel_oracle as co  # noqa: E402
+import stop_oracle as so  # noqa: E402
 from uneven_planner_b200 import configs, problems
 
 from harness import solve_diff
@@ -30,8 +29,8 @@ def test_stop_from_the_first_test_is_a_budget_of_one(terrain, golden, name):
     m, _, pb, prm = _golden_problems(terrain, golden, name)
     om = po.OracleMap(m)
     for i in range(pb.B):
-        c = co.solve_one(prm, om, pb, i, 1)
-        d = solve_diff(c, bo.solve_one(prm, om, pb, i, 1))
+        c = so.cancel_one(prm, om, pb, i, 1)
+        d = solve_diff(c, so.budget_one(prm, om, pb, i, 1))
         assert not d, d
         assert c[0].ret_code == STOPPED and c[0].n_lbfgs_iters == 1, i
 
@@ -42,9 +41,9 @@ def test_stop_past_the_last_test_is_the_free_solve(terrain, golden, name):
     om = po.OracleMap(m)
     _, _, ocx, ocy = pb.offsets()
     for i in range(pb.B):
-        ne, site = co.stop_tests(prm, om, pb, i)
+        ne, site = so.stop_tests(prm, om, pb, i)
         assert ne.size > 0 and np.all(np.diff(ne) >= 0) and set(site.tolist()) <= {0, 1}
-        out = co.solve_one(prm, om, pb, i, ne.size + 1)
+        out = so.cancel_one(prm, om, pb, i, ne.size + 1)
         d = solve_diff(out, po.solve_one(prm, om, pb, i))
         assert not d, d
         r = out[0]
@@ -59,15 +58,15 @@ def test_every_stop_is_found_again_from_its_record(terrain, golden):
     om = po.OracleMap(m)
     n = 0
     for i in range(min(pb.B, 6)):
-        ne, _ = co.stop_tests(prm, om, pb, i)
+        ne, _ = so.stop_tests(prm, om, pb, i)
         for s in sorted({1, 2, ne.size // 2, ne.size}):
             if s < 1:
                 continue
-            r, cxy, cyaw, _ = co.solve_one(prm, om, pb, i, s)
+            r, cxy, cyaw, _ = so.cancel_one(prm, om, pb, i, s)
             assert r.ret_code == STOPPED and r.n_evals == ne[s - 1]
-            s2 = co.match_stopped(prm, om, pb, i, r, cxy, cyaw)
+            s2 = so.match_stopped(prm, om, pb, i, r, cxy, cyaw)
             assert s2 is not None
-            d = solve_diff(co.solve_one(prm, om, pb, i, s2), (r, cxy, cyaw, co.solve_one(prm, om, pb, i, s)[3]))
+            d = solve_diff(so.cancel_one(prm, om, pb, i, s2), (r, cxy, cyaw, so.cancel_one(prm, om, pb, i, s)[3]))
             assert not d, d
             n += 1
     assert n > 0

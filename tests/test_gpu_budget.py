@@ -1,5 +1,5 @@
 """Evaluation budgets and deadline-bounded waits (include/ualm.h: ualm_set_budget, ualm_wait_batch_for, UALM_RET_STOPPED) on the
-GPU: the parity path against the budgeted oracle (tests/budget_oracle.cpp) bit for bit, the throughput path against its own unbudgeted solve, and
+GPU: the parity path against the budgeted oracle (tests/stop_oracle.cpp) bit for bit, the throughput path against its own unbudgeted solve, and
 the deadline on both paths.  Workload: the bench's (BASELINE config 2: 1024 problems on the hill terrain or its stand-in)."""
 import os
 import sys
@@ -9,7 +9,7 @@ import numpy as np
 import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import budget_oracle as bo  # noqa: E402
+import stop_oracle as so  # noqa: E402
 from harness import RECORD, ctx, gpu, same_problem  # noqa: F401, E402
 
 
@@ -58,7 +58,7 @@ def test_parity_budget_matches_oracle(gpu, work, max_evals):
     opt = ctx(gpu, 64, work[1], work[0]).set_budget(max_evals)
     res, cxy, cyaw = opt.optimize(pb)
     opt.close()
-    ores = bo.solve_batch(po.params_from(params), po.OracleMap(m), pb, max_evals, threads=min(32, os.cpu_count()))
+    ores = so.budget_batch(po.params_from(params), po.OracleMap(m), pb, max_evals, threads=min(32, os.cpu_count()))
     _, _, ocx, ocy = pb.offsets()
     for i in range(pb.B):
         g, (r, ocxy, ocyaw, _) = res[i], ores[i]

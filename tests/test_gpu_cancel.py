@@ -1,6 +1,6 @@
 """Cancelling problems of a batch in flight (include/ualm.h: ualm_cancel_problems) on both paths.  The parity path is checked bit for
 bit: a problem not cancelled is its uncancelled solve, and a cancelled one is either its uncancelled result (it was final first) or
-the oracle's solve with a stop predicate that holds from its s-th stop test on (tests/cancel_oracle.cpp, tests/cancel_oracle.py).
+the oracle's solve with a stop predicate that holds from its s-th stop test on (tests/stop_oracle.cpp, tests/stop_oracle.py).
 The throughput path keeps every problem not cancelled bit for bit.  Cancels do not reach other tickets or the lane's next batch.
 Workload: 1024 problems on the hill terrain or its stand-in with hill parameters (more than the 528 resident parity slots, so the
 smallest problems start last)."""
@@ -15,7 +15,7 @@ import numpy as np
 import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import cancel_oracle as co  # noqa: E402
+import stop_oracle as so  # noqa: E402
 from harness import build_driver, ctx, gpu, part, same_bytes, same_problem  # noqa: F401, E402
 
 
@@ -112,11 +112,11 @@ def test_parity_cancel_matches_oracle(gpu, work, free):
         if polled[0][i].ret_code != STOPPED:
             assert same_problem(pb, polled, ref, i), i
     prm, om = po.params_from(params), po.OracleMap(m)
-    co.lib()                                      # compiled once, before the threads use it
+    so.lib()                                      # compiled once, before the threads use it
 
     def check(i):
         r, cxy, cyaw = part(pb, polled, i)
-        return i, co.match_stopped(prm, om, pb, i, r, cxy, cyaw)
+        return i, so.match_stopped(prm, om, pb, i, r, cxy, cyaw)
     with ThreadPoolExecutor(min(32, os.cpu_count() or 1)) as ex:
         found = list(ex.map(check, stopped))
     assert all(s is not None for _, s in found), [i for i, s in found if s is None]

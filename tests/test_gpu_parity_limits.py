@@ -7,7 +7,7 @@ and at its largest shared-memory layouts:
     generated problems (N > 32), with sample counts S = N (int_K + 1) that are not multiples of 4 (the packed yaw-index table) or
     of 32 (the cost chain's last 32-sample block);
   * eval_batch at the guesses and at perturbed points with random duals on both branches of every inequality, init_scaling_batch,
-    solves under budgets of 1, 5 and 30 evaluations against budget_oracle, and unbudgeted solves against the oracle's own;
+    solves under budgets of 1, 5 and 30 evaluations against stop_oracle's budget, and unbudgeted solves against the oracle's own;
   * the same solves as four-warp groups, as two-warp groups (UALM_F4=0 UALM_F2=1) and as single warps (UALM_GROUPS=0, which
     refuses a batch holding a problem whose layout does not fit four to a CTA), byte for byte the same;
   * the shared-memory boundary: one N = 64, M = 128 problem at the largest int_K that fits four to a CTA and the next one up (past
@@ -218,7 +218,7 @@ def test_eval_and_scaling_bitwise(gpu, cases, bumps_map, K):
 @pytest.mark.gpu
 @pytest.mark.parametrize("K", INT_K)
 def test_budgeted_solves_bitwise_in_every_group_size(gpu, cases, bumps_map, K):
-    """budgets 1, 5, 30: whole record and coefficients against budget_oracle; the post-solve scan and ualm_check_trajectories of
+    """budgets 1, 5, 30: whole record and coefficients against stop_oracle's budget; the post-solve scan and ualm_check_trajectories of
     the 30-evaluation solves against the oracle's"""
     p = _params(K)
     for k in BUDGETS:

@@ -2,7 +2,7 @@
 (the case table of tests/test_solver_control.py, which also checks that every case still reaches its branch):
 
   * parity path (precision 64): every case on generated bumps and hill problems and the N1_M1 / N64_M128 / off_map shapes, whole
-    record and coefficients bit for bit against the oracle, unbudgeted and under set_budget(k) against budget_oracle;
+    record and coefficients bit for bit against the oracle, unbudgeted and under set_budget(k) against stop_oracle's budget;
   * throughput path: every case at precision 65 (under the case's evaluation budget, CASE_BUDGET) and the structural cases at
     precision 32, and set_budget(k) for k in BUDGETS on 128 problems of the bench's workload, against the same oracle runs.  Every
     decided trajectory (test_solver_control.decided: three runs from inputs perturbed by EPS agree with the unperturbed one) must
@@ -54,7 +54,7 @@ def _check_decided(got, ref, mask, prec, what):
 # ------------------------------------------------------------------ A: the parity path, bit for bit
 @pytest.mark.parametrize("case", list(workloads.SOLVER_CASES))
 def test_parity_case_bitwise(gpu, sets, case):
-    """unbudgeted against the oracle, and under set_budget(k) against budget_oracle"""
+    """unbudgeted against the oracle, and under set_budget(k) against stop_oracle's budget"""
     p = workloads.case_params(case)
     for label, m, pb in sets:
         for k in (0, 1, 5, 30):

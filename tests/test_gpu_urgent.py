@@ -12,7 +12,7 @@ import numpy as np
 import pytest
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import cancel_oracle as co  # noqa: E402
+import stop_oracle as so  # noqa: E402
 from harness import build_driver, ctx, gpu, part, pending, same_bytes, same_problem  # noqa: F401, E402
 
 
@@ -188,12 +188,12 @@ def test_interplay_with_cancel_deadline_and_budget(gpu, work, free):
                 assert same_problem(b, out, r, i), i
     assert any(o is out1 for _, o, _ in stopped)
     prm, om = po.params_from(work["params"]), po.OracleMap(work["m"])
-    co.lib()
+    so.lib()
     rng = np.random.default_rng(3)
     pick = [stopped[k] for k in rng.choice(len(stopped), min(24, len(stopped)), replace=False)]
     for b, out, i in pick:
         r, cxy, cyaw = part(b, out, i)
-        assert co.match_stopped(prm, om, b, i, r, cxy, cyaw) is not None, i
+        assert so.match_stopped(prm, om, b, i, r, cxy, cyaw) is not None, i
     # a budget: the urgent ticket and the held ones, each bit for bit its free solve under the same budget
     budget = 40
     opt = ctx(gpu, 64, work["params"], work["m"])

@@ -10,7 +10,7 @@ import numpy as np
 import pytest
 
 import alm_ref as ar
-import budget_oracle as bo
+import stop_oracle as so
 import map_build_ref as mref
 from harness import bits, cat, ctx
 from uneven_planner_b200 import configs, problems
@@ -965,9 +965,9 @@ def perturb(pb, eps, seed):
 
 
 def oracle(params, mapdata, pb, max_evals=0):
-    """budget_oracle (max_evals 0: the oracle's own solve) of every problem: [(record, c_xy, c_yaw)]"""
+    """stop_oracle's budget (max_evals 0: the oracle's own solve) of every problem: [(record, c_xy, c_yaw)]"""
     import pyoracle as po
-    out = bo.solve_batch(po.params_from(params), po.OracleMap(mapdata), pb, max_evals, threads=THREADS)
+    out = so.budget_batch(po.params_from(params), po.OracleMap(mapdata), pb, max_evals, threads=THREADS)
     return [(r, cxy, cyaw) for r, cxy, cyaw, _ in out]
 
 
