@@ -3,9 +3,10 @@ import collections, os, re, subprocess, sys, tempfile
 so, kname = sys.argv[1:3]
 ops = sys.argv[3:] or ["LDL", "STL", "LDG", "LD", "ST", "STG", "LDS", "STS", "DFMA", "DMUL", "DADD", "CALL"]
 d = tempfile.mkdtemp(); subprocess.run(["cuobjdump", "-xelf", "all", os.path.abspath(so)], cwd=d, capture_output=True)
-cub = [f for f in os.listdir(d) if "host_tools" not in f][0]
-lines = subprocess.run(["nvdisasm", "-c", os.path.join(d, cub)], capture_output=True, text=True).stdout.split("\n")
-start = [i for i, l in enumerate(lines) if l.startswith(".text.") and kname in l][0]
+for cub in sorted(os.listdir(d)):   # the cubin that holds the kernel (the library carries one per translation unit)
+    lines = subprocess.run(["nvdisasm", "-c", os.path.join(d, cub)], capture_output=True, text=True).stdout.split("\n")
+    start = [i for i, l in enumerate(lines) if l.startswith(".text.") and kname in l]
+    if start: start = start[0]; break
 cur, agg = "kernel body", collections.defaultdict(collections.Counter)
 for l in lines[start + 1:]:
     if l.startswith(".text.") or l.lstrip().startswith(".section"): break

@@ -363,6 +363,13 @@ __device__ __forceinline__ R getTtoTauGrad(R tau) // alm_traj_opt.h:244-253
     R denSqrt = (0.5 * tau - 1.0) * tau + 1.0;
     return (1.0 - tau) / (denSqrt * denSqrt);
 }
+// a yaw cell index wrapped into [0, n)
+__device__ __forceinline__ int wrap_index(int c, int n)
+{
+    while (c > n - 1) c -= n;
+    while (c < 0) c += n;
+    return c;
+}
 __device__ __forceinline__ void normSO2(R &yaw) // uneven_map.cpp:64-71
 {
     while (yaw < -M_PI) yaw += 2 * M_PI;
@@ -381,6 +388,18 @@ __device__ UALM_NOINLINE double2 dev_sincos(R x)
     return make_double2(s, c);
 }
 __device__ UALM_NOINLINE R dev_atan2(R y, R x) { return ualm_atan2(y, x); }
+// the same routines inlined (INL: the per-evaluation penalty loop, which has the registers to spare and where four calls per
+// sample and their argument moves were a measurable share of the phase) or through the out-of-line copies above
+template <bool INL>
+__device__ __forceinline__ double2 sincos_sel(R x)
+{
+    if (!INL) return dev_sincos(x);
+    R s, c;
+    ualm_sincos(x, &s, &c);
+    return make_double2(s, c);
+}
+template <bool INL>
+__device__ __forceinline__ R atan2_sel(R y, R x) { return INL ? ualm_atan2(y, x) : dev_atan2(y, x); }
 
 // IEEE a / b for callers whose numerator is often exactly zero.  The inline fast path of the fp64 division hands a zero (or
 // denormal) quotient to an out-of-line slow path, and it does so for the whole warp when a single lane needs it; here a zero
@@ -965,7 +984,9 @@ __device__ __forceinline__ bool map_in(const DevMap &m, const R pos[3]) // uneve
     return true;
 }
 
-__device__ __forceinline__ void map_get_all_with_grad_impl(const DevMap &m, const R pos[3], R values[7], R grads[7][3])
+// sc_yaw: sin and cos of pos[2] when the caller already has them (have_sc), else computed here
+template <bool INL>
+__device__ __forceinline__ void map_get_all_with_grad_impl(const DevMap &m, const R pos[3], R values[7], R grads[7][3], bool have_sc, double2 sc_yaw)
 {
     // the map descriptor is a kernel parameter read through a generic pointer: fetch every field once (a re-read after any
     // store costs a long-scoreboard wait, and the corner loop below used to re-read vn[2] sixteen times)
@@ -974,7 +995,8 @@ __device__ __forceinline__ void map_get_all_with_grad_impl(const DevMap &m, cons
     const double *const cells64 = m.cells64;
     const R xy_res = m.xy_res, yaw_res = m.yaw_res, xy_inv = m.xy_inv, yaw_inv = m.yaw_inv, org0 = m.origin[0], org1 = m.origin[1], org2 = m.origin[2];
     R rs[3], rg[4][3];
-    if (!map_in(m, pos)) {
+    const bool in = map_in(m, pos);
+    if (!in) {
         for (int r = 0; r < 4; r++) for (int k = 0; k < 3; k++) rg[r][k] = 0.0;
         rs[0] = rs[1] = rs[2] = 0.0;
     } else {
@@ -991,25 +1013,30 @@ __device__ __forceinline__ void map_get_all_with_grad_impl(const DevMap &m, cons
         R diff[3];
         diff[0] = (pos[0] - idx_pos[0]) * xy_inv;
         diff[1] = (pos[1] - idx_pos[1]) * xy_inv;
-        // start the eight corner cells now: the angle difference below costs two out-of-line calls the loads cannot cross
+        // the eight corner cells: clamped x / y and wrapped yaw indices once, then start the loads now, ahead of the angle
+        // difference below, which the loads cannot cross
+        int cx[2], cy[2], cw[2];
+#pragma unroll
+        for (int e = 0; e < 2; e++) {
+            cx[e] = max(min(idx[0] + e, vn0 - 1), 0);
+            cy[e] = max(min(idx[1] + e, vn1 - 1), 0);
+            cw[e] = wrap_index(idx[2] + e, vn2);
+        }
+        size_t cadr[2][2][2];
 #pragma unroll
         for (int x = 0; x < 2; x++)
 #pragma unroll
             for (int y = 0; y < 2; y++)
 #pragma unroll
                 for (int w = 0; w < 2; w++) {
-                    int c0 = idx[0] + x, c1 = idx[1] + y, c2 = idx[2] + w;
-                    c0 = max(min(c0, vn0 - 1), 0);
-                    c1 = max(min(c1, vn1 - 1), 0);
-                    while (c2 > vn2 - 1) c2 -= vn2;
-                    while (c2 < 0) c2 += vn2;
-                    const size_t adr = (size_t)c0 * vn1 * vn2 + (size_t)c1 * vn2 + c2;
+                    const size_t adr = (size_t)cx[x] * vn1 * vn2 + (size_t)cy[y] * vn2 + cw[w];
+                    cadr[x][y][w] = adr;
                     prefetch_l1(cells64 ? (const void *)(cells64 + 4 * adr) : (const void *)&cells[adr]);
                 }
         {
             R sd, cd;
-            { const double2 scv = dev_sincos(pos[2] - idx_pos[2]); sd = scv.x; cd = scv.y; }
-            diff[2] = dev_atan2(sd, cd) * yaw_inv;
+            { const double2 scv = sincos_sel<INL>(pos[2] - idx_pos[2]); sd = scv.x; cd = scv.y; }
+            diff[2] = atan2_sel<INL>(sd, cd) * yaw_inv;
         }
         R v[2][2][2][3];
 #pragma unroll
@@ -1018,12 +1045,10 @@ __device__ __forceinline__ void map_get_all_with_grad_impl(const DevMap &m, cons
             for (int y = 0; y < 2; y++)
 #pragma unroll
                 for (int w = 0; w < 2; w++) {
-                    int c0 = idx[0] + x, c1 = idx[1] + y, c2 = idx[2] + w;
-                    c0 = max(min(c0, vn0 - 1), 0);
-                    c1 = max(min(c1, vn1 - 1), 0);
-                    while (c2 > vn2 - 1) c2 -= vn2;
-                    while (c2 < 0) c2 += vn2;
-                    const size_t adr = (size_t)c0 * vn1 * vn2 + (size_t)c1 * vn2 + c2;
+                    // inlined (the penalty loop), the addresses are held across the angle difference; the out-of-line copy forms
+                    // them again after its two calls: holding eight addresses across the calls took check_kernel from 166 to 205
+                    // registers
+                    const size_t adr = INL ? cadr[x][y][w] : (size_t)cx[x] * vn1 * vn2 + (size_t)cy[y] * vn2 + wrap_index(idx[2] + w, vn2);
                     if (cells64) {
                         const double2 lo = __ldg((const double2 *)(cells64 + 4 * adr)), hi = __ldg((const double2 *)(cells64 + 4 * adr) + 1);
                         v[x][y][w][0] = lo.y; v[x][y][w][1] = hi.x; v[x][y][w][2] = hi.y;
@@ -1050,14 +1075,16 @@ __device__ __forceinline__ void map_get_all_with_grad_impl(const DevMap &m, cons
             g0 *= xy_inv;
             rg[k][0] = g0;
         }
-        const R cc = sqrt(1.0 - rs[1] * rs[1] - rs[2] * rs[2]);
-#pragma unroll
-        for (int k = 0; k < 3; k++) rg[3][k] = div_nz(-(rg[1][k] * rs[1] + rg[2][k] * rs[2]), cc);
     }
     const R c = sqrt(1.0 - rs[1] * rs[1] - rs[2] * rs[2]);
+    // inside the map, the reference divides by the same square root of the same expression (its `cc`): c, formed once
+    if (in) {
+#pragma unroll
+        for (int k = 0; k < 3; k++) rg[3][k] = div_nz(-(rg[1][k] * rs[1] + rg[2][k] * rs[2]), c);
+    }
     const R inv_c = 1.0 / c;
     R syaw, cyaw;
-    { const double2 scv = dev_sincos(pos[2]); syaw = scv.x; cyaw = scv.y; }
+    { const double2 scv = have_sc ? sc_yaw : sincos_sel<INL>(pos[2]); syaw = scv.x; cyaw = scv.y; }
     const R xyaw[2] = {cyaw, syaw};
     const R yyaw[2] = {-syaw, cyaw};
     const R tt = xyaw[0] * rs[1] + xyaw[1] * rs[2];
@@ -1094,7 +1121,7 @@ __device__ __forceinline__ void map_get_all_with_grad_impl(const DevMap &m, cons
 
 __device__ UALM_NOINLINE void map_get_all_with_grad(const DevMap &m, const R pos[3], R values[7], R grads[7][3])
 {
-    map_get_all_with_grad_impl(m, pos, values, grads);
+    map_get_all_with_grad_impl<false>(m, pos, values, grads, false, make_double2(0.0, 0.0));
 }
 
 // kinematics of one constraint sample (alm_traj_opt.cpp:733-817)
@@ -1107,8 +1134,10 @@ struct SampleK {
     int yaw_idx;
 };
 
-template <bool INL>
-__device__ __forceinline__ void sample_kin_impl(const Traj &t, const DevMap &map, R gravity, int i, R s1, R base_time, SampleK &S)
+// before_map(S) runs once the kinematics are complete and before the map lookup: the penalty loop stores there what it only
+// writes out, so that those values are not held in registers across the lookup
+template <bool INL, class BeforeMap>
+__device__ __forceinline__ void sample_kin_impl(const Traj &t, const DevMap &map, R gravity, int i, R s1, R base_time, SampleK &S, BeforeMap before_map)
 {
     const int nx = 6 * t.N;
     const R s2 = s1 * s1, s3 = s2 * s1, s4 = s2 * s2, s5 = s4 * s1;
@@ -1145,11 +1174,14 @@ __device__ __forceinline__ void sample_kin_impl(const Traj &t, const DevMap &map
     S.yaw = yaw; S.dyaw = dyaw; S.d2yaw = d2yaw;
     R se2[3] = {S.pos[0], S.pos[1], yaw};
     normSO2(se2[2]);
-    { const double2 scv = dev_sincos(yaw); S.syaw = scv.x; S.cyaw = scv.y; }
+    const double2 scv = sincos_sel<INL>(yaw);
+    S.syaw = scv.x; S.cyaw = scv.y;
     S.v_norm = sqrt(S.vel[0] * S.vel[0] + S.vel[1] * S.vel[1]);
     S.lon_acc = S.acc[0] * S.cyaw + S.acc[1] * S.syaw;
     S.lat_acc = S.acc[0] * (-S.syaw) + S.acc[1] * S.cyaw;
-    if (INL) map_get_all_with_grad_impl(map, se2, S.tv, S.tg);
+    before_map(S);
+    // the map's sin / cos of the wrapped yaw are the ones above whenever the wrap left the yaw's bits unchanged
+    if (INL) map_get_all_with_grad_impl<true>(map, se2, S.tv, S.tg, __double_as_longlong(se2[2]) == __double_as_longlong(yaw), scv);
     else map_get_all_with_grad(map, se2, S.tv, S.tg);
     S.vx = S.v_norm * S.tv[0];
     S.wz = dyaw * S.tv[5];
@@ -1161,7 +1193,7 @@ __device__ __forceinline__ void sample_kin_impl(const Traj &t, const DevMap &map
 // out-of-line copy (initScaling) and inlined copy (the per-evaluation penalty loop: keeps the sample state in registers)
 __device__ UALM_NOINLINE void sample_kin(const Traj &t, const DevMap &map, R gravity, int i, R s1, R base_time, SampleK &S)
 {
-    sample_kin_impl<false>(t, map, gravity, i, s1, base_time, S);
+    sample_kin_impl<false>(t, map, gravity, i, s1, base_time, S, [](const SampleK &) {});
 }
 
 // sample-time tables: s1tab[j] = j-fold accumulated step, base[i] = i-fold accumulated T (alm_traj_opt.cpp:713-714, 987-989)
@@ -1206,19 +1238,25 @@ __device__ UALM_NOINLINE void penalty_samples(Traj &t, const DevMap &map, const 
     // problem's row is read from its slot where it is used (sq_at: the squared limits), which keeps it out of the registers the
     // sample loop holds
     const R gravity = p.gravity;
-    const bool use_scaling = p.use_scaling != 0;
     R *const lambda_p = t.lambda, *const mu_p = t.mu, *const scale_p = t.scale_cx, *const hx_p = t.hx, *const gx_p = t.gx;
+    // piece i and index j of sample s = i (K + 1) + j, carried from one sample of the lane to its next instead of a division per
+    // sample
+    const int K1 = K + 1;
+    int i = gtid / K1, j = gtid - i * K1;
     for (int s = gtid; s < S; s += GT) {
-        const int i = s / (K + 1), j = s - i * (K + 1);
-        // the duals and scales of this sample are needed only after the kinematics: start their cache lines now, and read them
-        // in one batch before the first store below (a load placed after a store to a may-alias pointer cannot be hoisted by
-        // the compiler, which would expose one memory latency per constraint)
+        // the duals and scales of this sample are needed only after the kinematics and the map lookup: start their cache lines
+        // now, so that their loads, in one batch after the lookup, find them in L1
         prefetch_l1(lambda_p + s);
         prefetch_l1(mu_p + 6 * (size_t)s); prefetch_l1(mu_p + 6 * (size_t)s + 5);
         prefetch_l1(scale_p + 7 * (size_t)s); prefetch_l1(scale_p + 7 * (size_t)s + 6);
         SampleK q;
-        sample_kin_impl<true>(t, map, gravity, i, t.s1tab[j], t.base[i], q);
-        t.yawidx[s] = (unsigned short)q.yaw_idx;
+        sample_kin_impl<true>(t, map, gravity, i, t.s1tab[j], t.base[i], q, [&](const SampleK &k) {
+            t.yawidx[s] = (unsigned short)k.yaw_idx;
+            scr[(SF_ACC + 0) * S + s] = k.acc[0]; scr[(SF_ACC + 1) * S + s] = k.acc[1];
+            scr[(SF_JER + 0) * S + s] = k.jer[0]; scr[(SF_JER + 1) * S + s] = k.jer[1];
+            scr[SF_D2YAW * S + s] = k.d2yaw;
+            scr[SF_S1YAW * S + s] = k.y0[1];
+        });
         R grad_p[2] = {0, 0}, grad_v[2] = {0, 0}, grad_a[2] = {0, 0}, grad_se2[3] = {0, 0, 0};
         R grad_yaw = 0, grad_dyaw = 0, grad_vx2 = 0, grad_wz = 0, grad_ax = 0, grad_ay = 0, aug_grad = 0;
         const R inv_cos_vphix = q.tv[0], inv_cos_vphiy = q.tv[2], cos_xi = q.tv[4], inv_cos_xi = q.tv[5], sigma = q.tv[6];
@@ -1226,6 +1264,9 @@ __device__ UALM_NOINLINE void penalty_samples(Traj &t, const DevMap &map, const 
         R sc7[7], mu6[6];
 #pragma unroll
         for (int k = 0; k < 7; k++) sc7[k] = scale_p[7 * (size_t)s + k];
+        // without scaling, the curvature and surface terms are weighted by fixed factors instead of their scales (the flag is
+        // read here, where it is used, rather than held across the loop)
+        if (!p.use_scaling) { sc7[4] = UALM_CUR_SCALE; sc7[6] = UALM_SIG_SCALE; }
 #pragma unroll
         for (int k = 0; k < 6; k++) mu6[k] = mu_p[6 * (size_t)s + k];
         const R lambda_s = lambda_p[s];
@@ -1282,15 +1323,12 @@ __device__ UALM_NOINLINE void penalty_samples(Traj &t, const DevMap &map, const 
         }
         { // curvature
             const R m_ = mu6[3];
-            R gv;
-            if (use_scaling) gv = (curv_snorm - sq_at(t, SC_MAX_KAP)) * sc7[4];
-            else gv = (curv_snorm - sq_at(t, SC_MAX_KAP)) * UALM_CUR_SCALE;
+            const R gv = (curv_snorm - sq_at(t, SC_MAX_KAP)) * sc7[4];
             gx6[3] = gv;
             if (rho * gv + m_ > 0) {
                 const R denominator = 1.0 / (vx * vx + UALM_DELTA_SIGL);
                 scr[(SF_COST0 + 5) * S + s] = gv * (m_ + 0.5 * rho * gv);
-                if (use_scaling) aug_grad = (rho * gv + m_) * sc7[4];
-                else aug_grad = (rho * gv + m_) * UALM_CUR_SCALE;
+                aug_grad = (rho * gv + m_) * sc7[4];
                 grad_wz += aug_grad * denominator * 2.0 * wz;
                 grad_vx2 -= aug_grad * curv_snorm * denominator;
             } else scr[(SF_COST0 + 5) * S + s] = div_by_recip(-0.5 * m_ * m_, rho, rrho);
@@ -1308,20 +1346,13 @@ __device__ UALM_NOINLINE void penalty_samples(Traj &t, const DevMap &map, const 
         }
         { // surface variation
             const R m_ = mu6[5];
-            R gv;
-            if (use_scaling) gv = (sigma - t.sc[SC_MAX_SIG]) * sc7[6];
-            else gv = (sigma - t.sc[SC_MAX_SIG]) * UALM_SIG_SCALE;
+            const R gv = (sigma - t.sc[SC_MAX_SIG]) * sc7[6];
             gx6[5] = gv;
             if (rho * gv + m_ > 0) {
                 scr[(SF_COST0 + 7) * S + s] = gv * (m_ + 0.5 * rho * gv);
                 const R ag = rho * gv + m_;
-                if (use_scaling) {
 #pragma unroll
-                    for (int k = 0; k < 3; k++) grad_se2[k] += ag * q.tg[6][k] * sc7[6];
-                } else {
-#pragma unroll
-                    for (int k = 0; k < 3; k++) grad_se2[k] += ag * q.tg[6][k] * UALM_SIG_SCALE;
-                }
+                for (int k = 0; k < 3; k++) grad_se2[k] += ag * q.tg[6][k] * sc7[6];
             } else scr[(SF_COST0 + 7) * S + s] = div_by_recip(-0.5 * m_ * m_, rho, rrho);
         }
         // process with vx, wz, ax (alm_traj_opt.cpp:948-964)
@@ -1348,10 +1379,8 @@ __device__ UALM_NOINLINE void penalty_samples(Traj &t, const DevMap &map, const 
         scr[(SF_GA + 0) * S + s] = grad_a[0]; scr[(SF_GA + 1) * S + s] = grad_a[1];
         scr[SF_GYAW * S + s] = grad_yaw; scr[SF_GDYAW * S + s] = grad_dyaw;
         scr[(SF_VEL + 0) * S + s] = q.vel[0]; scr[(SF_VEL + 1) * S + s] = q.vel[1];
-        scr[(SF_ACC + 0) * S + s] = q.acc[0]; scr[(SF_ACC + 1) * S + s] = q.acc[1];
-        scr[(SF_JER + 0) * S + s] = q.jer[0]; scr[(SF_JER + 1) * S + s] = q.jer[1];
-        scr[SF_DYAW * S + s] = q.dyaw; scr[SF_D2YAW * S + s] = q.d2yaw;
-        scr[SF_S1YAW * S + s] = q.y0[1];
+        scr[SF_DYAW * S + s] = q.dyaw;
+        for (j += GT; j >= K1; j -= K1) i++;
     }
 }
 
