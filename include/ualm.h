@@ -305,7 +305,7 @@ int ualm_cancel_problems(ualm_ctx_t *ctx, int ticket, int n, const int32_t *idx)
  * negative values are UALM_EINVAL.  Refused (UALM_ESTATE) while a submitted batch is in flight. */
 int ualm_set_budget(ualm_ctx_t *ctx, int32_t max_evals);
 /* Urgent work: urgent = 1 makes the calls after it urgent until urgent = 0: ualm_submit_batch / ualm_submit_batch_env,
- * ualm_submit_replan (its build and the ticket it submits) and ualm_check_trajectories.  No other call changes.  Any other value or
+ * ualm_submit_replan (its build and the ticket it submits), ualm_check_trajectories and ualm_mpc_export_trajectories.  No other call changes.  Any other value or
  * a null ctx is UALM_EINVAL.  Allowed at any time, also while batches are in flight; like ualm_set_budget it acts on the calls made
  * after it.
  * Every record, coefficient, built replan row and check row is bit for bit what the same call gives without urgency, and so is
@@ -316,9 +316,9 @@ int ualm_set_budget(ualm_ctx_t *ctx, int32_t max_evals);
  * join its CTA mate's problem, as at the end of the queue).  The held launches resume on the device, without a host call, when the
  * urgent work no longer needs slots: for an urgent ticket once every one of its problems has been taken (started, not finished),
  * so a ticket larger than the resident slots holds others back only until its last wave has started; for an urgent check or replan
- * build once its kernels have completed.  The urgent ticket's launches run on streams of the greatest priority.
+ * build or held MPC export once its kernels have completed.  The urgent ticket's launches run on streams of the greatest priority.
  * Throughput path (precision 32 / 65): an urgent ticket's admission and round loops run on streams of the greatest priority.  The
- * check and the replan build run on the greatest-priority check stream on both paths anyway, so urgency changes nothing else there.
+ * check, the replan build and the held MPC export run on the greatest-priority check stream on both paths anyway, so urgency changes nothing else there.
  * Bound: the launches of a held solve wait at most 2 s in all (by the device's global timer, summed over every hold it meets); after
  * that the solve resumes and takes no further hold for the rest of its run, so a hold that is never released can only slow work
  * down, never hang the device.  The hold of an urgent ticket is raised after the submit's host-side allocations: a submit whose lane
@@ -437,6 +437,25 @@ int ualm_check_trajectories_pp(ualm_ctx_t *ctx, int B, const int32_t *N, const i
  * ualm_sync / ualm_download / a wait) is UALM_ESTATE; no output is written on either. */
 int ualm_mpc_export_batch(ualm_ctx_t *ctx, double dt, const double *init_v, const double *init_a, double *pos_pts, double *posT_pts,
                           double *angle_pts, double *angleT_pts, double *c_mpc_xy, double *c_mpc_yaw, double *dev4);
+
+/* The same hand-over for B trajectories the caller holds, each from its own start state, e.g. rows of batches ualm_poll_batch /
+ * ualm_wait_batch returned, or of several lanes.  Inputs (host) in the layouts ualm_check_trajectories takes: N[B], M[B], piece_T[2B]
+ * = {piece_T_xy, piece_T_yaw} of each record, packed c_xy (12 N_b each) and c_yaw (6 M_b each); init_v[3B] / init_a[3B] = {x, y, yaw}
+ * per row, the message's boundary velocity / acceleration (NULL = zero, what the reference publishes; a replanned robot's message
+ * carries its state at the replan time, ualm_submit_replan's bnd' entries 2, 3, 13 and 4, 5, 14).  Outputs as ualm_mpc_export_batch's,
+ * packed row after row in call order; any output pointer may be NULL.  Row b is bit for bit what ualm_mpc_export_batch gives for the
+ * same record with init_v + 3b / init_a + 3b, at every precision (the parity translation unit's double arithmetic).  A row over the
+ * compiled limits (N > UALM_NMAX or M > UALM_MMAX) is zeros; a diverged record (infinite durations, or duration / dt >= 4e6) gets its
+ * message and re-solve and dev4 = {-1, 0, -1, 0}.
+ * Read-only: no grid, parameter, lane or record is read or touched (no environment needs to be bound), and it may be called while
+ * batches are in flight.  It runs on the stream of ualm_check_trajectories and synchronises that stream only; under ualm_set_urgent
+ * it goes ahead of the parity path's batches in flight as the check does, without it it waits there for SM slots in their tail.
+ * A null ctx, or a null N, M, piece_T, c_xy or c_yaw with B > 0, B < 0, dt <= 0 or NaN, N or M < 1, a non-finite init_v / init_a
+ * entry, or a row within the limits whose piece_T is NaN or <= 0 (a record ualm_poll_batch has not filled yet; +inf is a diverged
+ * solve and is accepted) is UALM_EINVAL, and no output is written.  B = 0 is UALM_OK and writes nothing. */
+int ualm_mpc_export_trajectories(ualm_ctx_t *ctx, int B, const int32_t *N, const int32_t *M, const double *piece_T, const double *c_xy,
+                                 const double *c_yaw, const double *init_v, const double *init_a, double dt, double *pos_pts,
+                                 double *posT_pts, double *angle_pts, double *angleT_pts, double *c_mpc_xy, double *c_mpc_yaw, double *dev4);
 
 /* UnevenMap construction on the GPU (SURVEY 8f-1: UnevenMap::init preprocessing on the host, then constructMap + filter,
  * uneven_map.cpp:317-398, 5-43, one thread per (x, y, yaw) cell).  Same arguments and the same arithmetic as ualm_map_build

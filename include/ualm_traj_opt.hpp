@@ -81,6 +81,8 @@ inline double getTotalDuration(const std::vector<Piece<Dim>> &pieces)   // PolyT
 
 // What PlanManager publishes to the MPC (mpc_controller/msg/SE2Traj.msg; plan_manager.cpp:151-185): the piece start points,
 // the end point and the piece durations of both splines; the boundary velocity / acceleration fields are zero in the reference.
+// A replanned robot's message carries its own state at the replan time instead ({x, y, yaw}: bnd' entries 2, 3, 13 and 4, 5, 14 of
+// submitReplan), one message per robot (exportToMpc).
 struct SE2TrajMsg {
     std::vector<double> pos_pts;      // (N + 1) x 2, row-major: pos_traj[i].getValue(0), then pos_traj.getValue(total)
     std::vector<double> posT_pts;     // N
@@ -151,7 +153,7 @@ public:
     void init() { check(ualm_set_params(ctx_, &params), "ualm_set_params"); }
     // evaluation budget per problem of the following solves (0 = none); a stopped problem returns UALM_RET_STOPPED (ualm.h)
     void setBudget(int max_evals) { check(ualm_set_budget(ctx_, max_evals), "ualm_set_budget"); }
-    // ualm_set_urgent: the submitBatch / submitReplan / checkTrajectories calls after it go ahead of the batches in flight, with the same
+    // ualm_set_urgent: the submitBatch / submitReplan / checkTrajectories / exportToMpc calls after it go ahead of the batches in flight, with the same
     // results, until setUrgent(false)
     void setUrgent(bool urgent) { check(ualm_set_urgent(ctx_, urgent ? 1 : 0), "ualm_set_urgent"); }
 
@@ -315,6 +317,17 @@ public:
                           double *dev4, const double *init_v = nullptr, const double *init_a = nullptr)
     {
         check(ualm_mpc_export_batch(ctx_, dt, init_v, init_a, pos_pts, posT_pts, angle_pts, angleT_pts, c_mpc_xy, c_mpc_yaw, dev4), "ualm_mpc_export_batch");
+    }
+
+    // The same hand-over for B trajectories the caller holds (e.g. from waitBatch / pollBatch, in checkTrajectories' layouts), each row
+    // from its own start state: init_v / init_a = 3 doubles {x, y, yaw} per row, null = zero (ualm_mpc_export_trajectories).  Outputs
+    // packed row after row; any output may be null.  Reads no grid or lane and may be called while batches are in flight
+    void exportToMpc(int B, const int32_t *N, const int32_t *M, const double *piece_T, const double *c_xy, const double *c_yaw, const double *init_v,
+                     const double *init_a, double dt, double *pos_pts, double *posT_pts, double *angle_pts, double *angleT_pts, double *c_mpc_xy,
+                     double *c_mpc_yaw, double *dev4)
+    {
+        check(ualm_mpc_export_trajectories(ctx_, B, N, M, piece_T, c_xy, c_yaw, init_v, init_a, dt, pos_pts, posT_pts, angle_pts, angleT_pts, c_mpc_xy,
+                                           c_mpc_yaw, dev4), "ualm_mpc_export_trajectories");
     }
 
     // The post-solve scan of B trajectories the caller holds (e.g. from waitBatch: piece_T = {piece_T_xy, piece_T_yaw} per record)

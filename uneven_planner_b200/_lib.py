@@ -128,6 +128,8 @@ def lib():
         L.ualm_feasibility_batch.restype = C.c_int
         L.ualm_mpc_export_batch.argtypes = [vp, C.c_double] + [dp] * 9
         L.ualm_mpc_export_batch.restype = C.c_int
+        L.ualm_mpc_export_trajectories.argtypes = [vp, C.c_int, ip, ip, dp, dp, dp, dp, dp, C.c_double] + [dp] * 7
+        L.ualm_mpc_export_trajectories.restype = C.c_int
         L.ualm_profile.restype = C.c_int
         L.ualm_reset_stream.argtypes = [vp]
         L.ualm_set_map_f64.argtypes = [vp, C.POINTER(MapGeom), dp, C.c_int]

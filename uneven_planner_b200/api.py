@@ -431,10 +431,7 @@ class BatchALMTrajOpt:
     def mpc_export(self, N, M, dt=0.01, init_v=None, init_a=None):
         """SE2Traj message arrays, the MPC side's re-solved coefficients and the planned-vs-tracked deviation of the resident solved
         batch (see ualm_mpc_export_batch).  N, M: the piece counts of the batch."""
-        N = np.asarray(N, dtype=np.int64); M = np.asarray(M, dtype=np.int64)
-        B, sN, sM = len(N), int(N.sum()), int(M.sum())
-        out = dict(pos_pts=np.zeros(2 * (sN + B)), posT_pts=np.zeros(sN), angle_pts=np.zeros(sM + B), angleT_pts=np.zeros(sM),
-                   c_mpc_xy=np.zeros(12 * sN), c_mpc_yaw=np.zeros(6 * sM), dev=np.zeros((B, 4)))
+        out = self._mpc_outputs(N, M)
         dp = C.POINTER(C.c_double)
         P = lambda a: a.ctypes.data_as(dp)
         iv = None if init_v is None else np.ascontiguousarray(init_v, dtype=np.float64)
@@ -442,6 +439,73 @@ class BatchALMTrajOpt:
         _check(self.L.ualm_mpc_export_batch(self.h, float(dt), None if iv is None else P(iv), None if ia is None else P(ia), P(out["pos_pts"]), P(out["posT_pts"]),
                                             P(out["angle_pts"]), P(out["angleT_pts"]), P(out["c_mpc_xy"]), P(out["c_mpc_yaw"]), P(out["dev"])))
         return out
+
+    @staticmethod
+    def _mpc_outputs(N, M):
+        """zeroed output arrays of a hand-over of trajectories with piece counts N, M (mpc_export's dict)"""
+        N = np.asarray(N, dtype=np.int64); M = np.asarray(M, dtype=np.int64)
+        B, sN, sM = len(N), int(N.sum()), int(M.sum())
+        return dict(pos_pts=np.zeros(2 * (sN + B)), posT_pts=np.zeros(sN), angle_pts=np.zeros(sM + B), angleT_pts=np.zeros(sM),
+                    c_mpc_xy=np.zeros(12 * sN), c_mpc_yaw=np.zeros(6 * sM), dev=np.zeros((B, 4)))
+
+    def mpc_export_trajectories(self, N, M, piece_T, c_xy, c_yaw, init_v=None, init_a=None, dt=0.01, urgent=False):
+        """ualm_mpc_export_trajectories: mpc_export's hand-over for trajectories the caller holds, in check_trajectories' layouts (N, M:
+        [B]; piece_T: [B, 2]; c_xy / c_yaw packed as wait() returns them), each row from its own start state: init_v / init_a = {x, y,
+        yaw} as None (zero, what the reference publishes), one triple for every row, or [B, 3].  Reads no grid, lane or record; may be
+        called while batches are in flight.  urgent: the export goes ahead of the batches in flight (ualm_set_urgent).  Returns the
+        dict mpc_export returns, rows packed in call order."""
+        N = np.ascontiguousarray(N, np.int32).reshape(-1)
+        M = np.ascontiguousarray(M, np.int32).reshape(-1)
+        B = N.size
+        pt = np.ascontiguousarray(piece_T, np.float64).reshape(-1)
+        cxy = np.ascontiguousarray(c_xy, np.float64).reshape(-1)
+        cyaw = np.ascontiguousarray(c_yaw, np.float64).reshape(-1)
+        for a, n, name in ((M, B, "M"), (pt, 2 * B, "piece_T"), (cxy, 12 * int(N.astype(np.int64).sum()), "c_xy"),
+                           (cyaw, 6 * int(M.astype(np.int64).sum()), "c_yaw")):
+            if a.size != n:
+                raise ValueError("mpc_export_trajectories: %s has %d entries, the piece counts need %d" % (name, a.size, n))
+        init = []
+        for v, name in ((init_v, "init_v"), (init_a, "init_a")):
+            if v is None:
+                init.append(None)
+                continue
+            v = np.asarray(v, np.float64)
+            if v.shape not in ((3,), (B, 3)):
+                raise ValueError("mpc_export_trajectories: %s must be None, 3 numbers or [B, 3] = [%d, 3], got %r" % (name, B, v.shape))
+            init.append(np.ascontiguousarray(np.broadcast_to(v, (B, 3))))
+        out = self._mpc_outputs(N, M)
+        with self._urgency(urgent):
+            _check(self.L.ualm_mpc_export_trajectories(self.h, B, _p(N, ip), _p(M, ip), _p(pt), _p(cxy), _p(cyaw), _p(init[0]), _p(init[1]), float(dt),
+                                                       *[_p(out[k]) for k in ("pos_pts", "posT_pts", "angle_pts", "angleT_pts", "c_mpc_xy",
+                                                                              "c_mpc_yaw", "dev")]))
+        return out
+
+    def mpc_export_results(self, pb, out, rows=None, start="rest", dt=0.01, urgent=False):
+        """mpc_export_trajectories of rows `rows` (None: all) of batch `pb` as wait() / poll() returned it: out = (results, c_xy,
+        c_yaw); a record poll() has not filled yet is refused.  start: "rest" = zero boundary derivatives, as the reference publishes;
+        "bnd" = each row's own start state from pb.bnd, v = (bnd[2], bnd[3], bnd[13]) and a = (bnd[4], bnd[5], bnd[14]), which is
+        what a replanned batch (submit_replan) carries.  Returns mpc_export's dict, rows packed in the order of `rows`."""
+        rows = np.arange(pb.B) if rows is None else np.asarray(rows)
+        if rows.ndim != 1 or (rows.size and not np.issubdtype(rows.dtype, np.integer)):
+            raise ValueError("mpc_export_results: rows must be a 1-D sequence of problem indices")
+        rows = rows.astype(np.int64)
+        if rows.size and (rows.min() < 0 or rows.max() >= pb.B):
+            raise ValueError("mpc_export_results: row index out of range [0, %d)" % pb.B)
+        if start not in ("rest", "bnd"):
+            raise ValueError("mpc_export_results: start must be 'rest' or 'bnd', got %r" % (start,))
+        res, cxy, cyaw = out
+        if len(res) != pb.B:
+            raise ValueError("mpc_export_results: out holds %d records, the batch has %d" % (len(res), pb.B))
+        _, _, ocx, ocy = pb.offsets()
+        B = rows.size
+        pt = np.array([(res[i].piece_T_xy, res[i].piece_T_yaw) for i in rows], np.float64).reshape(B, 2)
+        c_xy = np.concatenate([cxy[ocx[i]:ocx[i + 1]] for i in rows]) if B else np.zeros(0)
+        c_yaw = np.concatenate([cyaw[ocy[i]:ocy[i + 1]] for i in rows]) if B else np.zeros(0)
+        v = a = None
+        if start == "bnd":
+            bnd = np.asarray(pb.bnd, np.float64).reshape(pb.B, 18)[rows]
+            v, a = bnd[:, [2, 3, 13]], bnd[:, [4, 5, 14]]
+        return self.mpc_export_trajectories(pb.N[rows], pb.M[rows], pt, c_xy, c_yaw, init_v=v, init_a=a, dt=dt, urgent=urgent)
 
     def feasibility(self, dt=0.01):
         """Post-solve scan of the resident batch: array [B, 10] (see ualm_feasibility_batch)."""

@@ -1701,7 +1701,8 @@ static int check_block(ualm_ctx *c, size_t bytes)
     return UALM_OK;
 }
 
-// Trajectories the caller holds (ualm_check_trajectories, ualm_submit_replan), in the layouts ualm_wait_batch returns
+// Trajectories the caller holds (ualm_check_trajectories, ualm_submit_replan, ualm_mpc_export_trajectories), in the layouts
+// ualm_wait_batch returns
 struct Held {
     int B;
     const int32_t *N, *M;
@@ -1717,12 +1718,12 @@ static int held_counts(const char *what, Held &h)
     }
     return UALM_OK;
 }
-// h staged on the check stream in the context's block, grown in stream order: out (nout doubles) | piece_T 2B | t_from B | bnd 18B
-// (when given) | c_xy | c_yaw, then the descriptors, then B ints of idx (when given).  Under urgent work the hold of the check stream
-// (urgent: unarmed, on that stream) is raised before the copies; the caller lowers it behind its kernel (hold_lower), `urgent` on any
-// earlier exit.  a: the block as check_kernel reads it
-struct Staged { CheckPtrs a; double *bnd; int *idx; };
-static int stage_held(ualm_ctx *c, const Held &h, const std::vector<ProbDesc> &desc, size_t nout, const double *bnd, const std::vector<int> *idx,
+// h staged on the check stream in the context's block, grown in stream order: out (nout doubles) | piece_T 2B | t_from B | rows, rw
+// per problem (when given: a replan's bnd, 18; the MPC's boundary derivatives, 6) | c_xy | c_yaw, then the descriptors, then B ints of
+// idx (when given).  Under urgent work the hold of the check stream (urgent: unarmed, on that stream) is raised before the copies; the
+// caller lowers it behind its kernel (hold_lower), `urgent` on any earlier exit.  a: the block as check_kernel reads it
+struct Staged { CheckPtrs a; double *rows; int *idx; };
+static int stage_held(ualm_ctx *c, const Held &h, const std::vector<ProbDesc> &desc, size_t nout, const double *rows, int rw, const std::vector<int> *idx,
                       HoldGuard &urgent, Staged &s)
 {
     const int B = h.B;
@@ -1731,21 +1732,21 @@ static int stage_held(ualm_ctx *c, const Held &h, const std::vector<ProbDesc> &d
         if (int rc = hold_set(c, UALM_MAX_LANES, 1, st)) return rc;
         urgent.armed = true;
     }
-    const size_t nbnd = bnd ? 18 * (size_t)B : 0, nd = nout + 3 * (size_t)B + nbnd + (size_t)h.ncx + (size_t)h.ncy;
+    const size_t nrows = rows ? (size_t)rw * B : 0, nd = nout + 3 * (size_t)B + nrows + (size_t)h.ncx + (size_t)h.ncy;
     if (int rc = check_block(c, sizeof(double) * nd + sizeof(ProbDesc) * B + (idx ? sizeof(int) * B : 0))) return rc;
-    double *d_out = (double *)c->cbuf, *d_pt = d_out + nout, *d_tf = d_pt + 2 * (size_t)B, *d_bnd = d_tf + B, *d_cxy = d_bnd + nbnd,
+    double *d_out = (double *)c->cbuf, *d_pt = d_out + nout, *d_tf = d_pt + 2 * (size_t)B, *d_rows = d_tf + B, *d_cxy = d_rows + nrows,
            *d_cyaw = d_cxy + h.ncx;
     ProbDesc *d_desc = (ProbDesc *)(d_out + nd);
     int *d_idx = (int *)(d_desc + B);
     CK(cudaMemcpyAsync(d_pt, h.piece_T, sizeof(double) * 2 * B, cudaMemcpyHostToDevice, st));
     if (h.t_from) CK(cudaMemcpyAsync(d_tf, h.t_from, sizeof(double) * B, cudaMemcpyHostToDevice, st));
-    if (bnd) CK(cudaMemcpyAsync(d_bnd, bnd, sizeof(double) * nbnd, cudaMemcpyHostToDevice, st));
+    if (rows) CK(cudaMemcpyAsync(d_rows, rows, sizeof(double) * nrows, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_cxy, h.c_xy, sizeof(double) * h.ncx, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_cyaw, h.c_yaw, sizeof(double) * h.ncy, cudaMemcpyHostToDevice, st));
     CK(cudaMemcpyAsync(d_desc, desc.data(), sizeof(ProbDesc) * B, cudaMemcpyHostToDevice, st));
     if (idx) CK(cudaMemcpyAsync(d_idx, idx->data(), sizeof(int) * B, cudaMemcpyHostToDevice, st));
     s.a.desc = d_desc; s.a.c_xy = d_cxy; s.a.c_yaw = d_cyaw; s.a.piece_T = d_pt; s.a.t_from = h.t_from ? d_tf : nullptr; s.a.out = d_out;
-    s.bnd = bnd ? d_bnd : nullptr;
+    s.rows = rows ? d_rows : nullptr;
     s.idx = idx ? d_idx : nullptr;
     return UALM_OK;
 }
@@ -1796,7 +1797,7 @@ extern "C" int ualm_check_trajectories_pp(ualm_ctx_t *c, int B, const int32_t *N
     } done{c};
     HoldGuard urgent{c, UALM_MAX_LANES, c->cstream, false};
     Staged s;
-    if (int rc = stage_held(c, held, desc, 16 * (size_t)B, nullptr, &idx, urgent, s)) return rc;
+    if (int rc = stage_held(c, held, desc, 16 * (size_t)B, nullptr, 0, &idx, urgent, s)) return rc;
     if (int rc = scan_launch(c, s.a, s.idx, off, hold, dt, c->cstream)) return rc;
     if (int rc = hold_lower(urgent)) return rc;
     CK(cudaMemcpyAsync(out16, s.a.out, sizeof(double) * 16 * B, cudaMemcpyDeviceToHost, c->cstream));
@@ -1853,9 +1854,9 @@ extern "C" int ualm_submit_replan_pp(ualm_ctx_t *c, int B, const int32_t *N, con
     // (ualm_submit_batch_env)
     HoldGuard urgent{c, UALM_MAX_LANES, st, false};
     Staged s;
-    if (int rc = stage_held(c, held, desc, nout, bnd, nullptr, urgent, s)) return rc;
+    if (int rc = stage_held(c, held, desc, nout, bnd, 18, nullptr, urgent, s)) return rc;
     ReplanPtrs a;
-    a.desc = s.a.desc; a.c_xy = s.a.c_xy; a.c_yaw = s.a.c_yaw; a.piece_T = s.a.piece_T; a.bnd = s.bnd; a.t_from = s.a.t_from; a.out = s.a.out;
+    a.desc = s.a.desc; a.c_xy = s.a.c_xy; a.c_yaw = s.a.c_yaw; a.piece_T = s.a.piece_T; a.bnd = s.rows; a.t_from = s.a.t_from; a.out = s.a.out;
     const ReplanParams p{dt, r.piece_len, r.yaw_piece_times, r.mean_vel, r.init_time_times};
     replan_kernel<<<(B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(a, p, B);
     CK(cudaGetLastError());
@@ -1898,28 +1899,46 @@ extern "C" int ualm_submit_replan_pp(ualm_ctx_t *c, int B, const int32_t *N, con
 // ---------------------------------------------------------------------------------------------
 // SURVEY 8f-3: SE2Traj message + the MPC side's MINCO re-solve + planned-vs-tracked deviation for a solved batch (mpc_export_kernel)
 // ---------------------------------------------------------------------------------------------
-static int mpc_export_run(ualm_ctx *c, const BatchPtrs &bp, const BatchLayout &L, double dt, const double *init_v, const double *init_a, double *pos_pts,
-                          double *posT_pts, double *angle_pts, double *angleT_pts, double *c_mpc_xy, double *c_mpc_yaw, double *dev4, cudaStream_t st)
+// doubles of mpc_export_run's device block for B problems of sN xy and sM yaw pieces in all: the seven outputs, then the band scratch
+static size_t mpc_export_doubles(int B, long long sN, long long sM)
 {
-    const int B = L.B;
-    long long sN = 0, sM = 0;
-    for (int b = 0; b < B; b++) { sN += L.N[b]; sM += L.M[b]; }
-    struct Tmp { DevBuf<double> buf; ~Tmp() { buf.release(); } } t;
+    return 2 * (size_t)(sN + B) + (size_t)sN + (size_t)(sM + B) + (size_t)sM + 12 * (size_t)sN + 6 * (size_t)sM + 4 * (size_t)B +
+           13 * (6 * (size_t)sN + 6 * (size_t)sM);
+}
+// mpc_export_kernel over bp's B problems on stream st, its outputs and scratch in `block` (mpc_export_doubles), then the outputs to the
+// host.  The boundary derivatives: d_init_rows (device, 6 per problem, MpcOut) when given, else init_v / init_a for every problem
+// (null = zero).  `urgent` is lowered behind the kernel, before the copies
+static int mpc_export_run(const BatchPtrs &bp, long long sN, long long sM, double dt, const double *init_v, const double *init_a,
+                          const double *d_init_rows, double *block, double *pos_pts, double *posT_pts, double *angle_pts, double *angleT_pts,
+                          double *c_mpc_xy, double *c_mpc_yaw, double *dev4, cudaStream_t st, HoldGuard &urgent)
+{
+    const int B = bp.B;
     const size_t n_pp = 2 * (size_t)(sN + B), n_pt = (size_t)sN, n_ap = (size_t)(sM + B), n_at = (size_t)sM, n_cx = 12 * (size_t)sN, n_cy = 6 * (size_t)sM, n_dv = 4 * (size_t)B;
-    const size_t n_band = 13 * (6 * (size_t)sN + 6 * (size_t)sM);
-    CK(t.buf.ensure(n_pp + n_pt + n_ap + n_at + n_cx + n_cy + n_dv + n_band));
     MpcOut o;
-    double *q = t.buf.p;
+    double *q = block;
     o.pos_pts = q; q += n_pp; o.posT_pts = q; q += n_pt; o.angle_pts = q; q += n_ap; o.angleT_pts = q; q += n_at;
     o.c_mpc_xy = q; q += n_cx; o.c_mpc_yaw = q; q += n_cy; o.dev = q; q += n_dv; o.band = q;
-    for (int k = 0; k < 3; k++) { o.init_v[k] = init_v ? init_v[k] : 0.0; o.init_a[k] = init_a ? init_a[k] : 0.0; }
+    o.init_rows = d_init_rows;
+    for (int k = 0; k < 3; k++) { o.init[k] = init_v ? init_v[k] : 0.0; o.init[3 + k] = init_a ? init_a[k] : 0.0; }
     mpc_export_kernel<<<(B + UALM_WPB - 1) / UALM_WPB, UALM_THREADS * UALM_WPB, 0, st>>>(bp, dt, o);
     CK(cudaGetLastError());
+    if (int rc = hold_lower(urgent)) return rc;
     struct { double *h; const double *d; size_t n; } cp[7] = {{pos_pts, o.pos_pts, n_pp}, {posT_pts, o.posT_pts, n_pt}, {angle_pts, o.angle_pts, n_ap},
         {angleT_pts, o.angleT_pts, n_at}, {c_mpc_xy, o.c_mpc_xy, n_cx}, {c_mpc_yaw, o.c_mpc_yaw, n_cy}, {dev4, o.dev, n_dv}};
     for (auto &e : cp) if (e.h && e.n) CK(cudaMemcpyAsync(e.h, e.d, sizeof(double) * e.n, cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
     return UALM_OK;
+}
+// the lane form: its block from cudaMalloc, freed on return
+static int mpc_export_lane(ualm_ctx *c, const BatchPtrs &bp, const BatchLayout &L, double dt, const double *init_v, const double *init_a, double *pos_pts,
+                           double *posT_pts, double *angle_pts, double *angleT_pts, double *c_mpc_xy, double *c_mpc_yaw, double *dev4, cudaStream_t st)
+{
+    long long sN = 0, sM = 0;
+    for (int b = 0; b < L.B; b++) { sN += L.N[b]; sM += L.M[b]; }
+    struct Tmp { DevBuf<double> buf; ~Tmp() { buf.release(); } } t;
+    CK(t.buf.ensure(mpc_export_doubles(L.B, sN, sM)));
+    HoldGuard none{c, UALM_MAX_LANES, st, false};
+    return mpc_export_run(bp, sN, sM, dt, init_v, init_a, nullptr, t.buf.p, pos_pts, posT_pts, angle_pts, angleT_pts, c_mpc_xy, c_mpc_yaw, dev4, st, none);
 }
 
 extern "C" int ualm_mpc_export_batch(ualm_ctx_t *c, double dt, const double *init_v, const double *init_a, double *pos_pts, double *posT_pts, double *angle_pts,
@@ -1931,13 +1950,58 @@ extern "C" int ualm_mpc_export_batch(ualm_ctx_t *c, double dt, const double *ini
         TpScan s;
         if (int rc = tp_scan(c, "ualm_mpc_export_batch", s)) return rc;
         if (L.B == 0) return UALM_OK;
-        return mpc_export_run(c, s.bp, L, dt, init_v, init_a, pos_pts, posT_pts, angle_pts, angleT_pts, c_mpc_xy, c_mpc_yaw, dev4, 0);
+        return mpc_export_lane(c, s.bp, L, dt, init_v, init_a, pos_pts, posT_pts, angle_pts, angleT_pts, c_mpc_xy, c_mpc_yaw, dev4, 0);
     }
     Lane *l = c->b;
     if (!l->have_batch || !l->solved) return fail(UALM_ESTATE, "ualm_mpc_export_batch needs a solved resident batch");
     CK(cudaSetDevice(c->device));
     if (L.B == 0) return UALM_OK;
-    return mpc_export_run(c, batch_ptrs(c), L, dt, init_v, init_a, pos_pts, posT_pts, angle_pts, angleT_pts, c_mpc_xy, c_mpc_yaw, dev4, l->stream);
+    return mpc_export_lane(c, batch_ptrs(c), L, dt, init_v, init_a, pos_pts, posT_pts, angle_pts, angleT_pts, c_mpc_xy, c_mpc_yaw, dev4, l->stream);
+}
+
+// the held form: the records staged on the check stream (stage_held), the kernel's outputs and scratch at the front of the check block,
+// each row's boundary derivatives behind them.  Reads no grid, parameter, lane or record of the context, so nothing waits for a batch
+// in flight: the block grows in stream order and the call synchronises the check stream only
+extern "C" int ualm_mpc_export_trajectories(ualm_ctx_t *c, int B, const int32_t *N, const int32_t *M, const double *piece_T, const double *c_xy,
+                                            const double *c_yaw, const double *init_v, const double *init_a, double dt, double *pos_pts,
+                                            double *posT_pts, double *angle_pts, double *angleT_pts, double *c_mpc_xy, double *c_mpc_yaw, double *dev4)
+{
+    if (!c || B < 0 || (B > 0 && (!N || !M || !piece_T || !c_xy || !c_yaw)))
+        return fail(UALM_EINVAL, "ualm_mpc_export_trajectories: null argument or B < 0");
+    if (!(dt > 0.0)) return fail(UALM_EINVAL, "ualm_mpc_export_trajectories: dt must be > 0");
+    Held held{B, N, M, piece_T, c_xy, c_yaw, nullptr};
+    if (int rc = held_counts("ualm_mpc_export_trajectories", held)) return rc;
+    for (int b = 0; b < B; b++) {
+        for (const double *v : {init_v, init_a})
+            for (int k = 0; v && k < 3; k++)
+                if (!std::isfinite(v[3 * (size_t)b + k])) return fail(UALM_EINVAL, "ualm_mpc_export_trajectories: init_v and init_a must be finite");
+        // a record ualm_poll_batch has not filled yet (zero durations); +inf is a diverged solve, exported as the lane form exports it
+        if (!over_limits(N[b], M[b]) && (!(piece_T[2 * b] > 0.0) || !(piece_T[2 * b + 1] > 0.0)))
+            return fail(UALM_EINVAL, "ualm_mpc_export_trajectories: piece_T must be > 0 (row " + std::to_string(b) + ")");
+    }
+    if (B == 0) return UALM_OK;
+    CK(cudaSetDevice(c->device));
+    if (int rc = check_stream(c)) return rc;
+    std::vector<double> rows;
+    if (init_v || init_a) {
+        rows.assign(6 * (size_t)B, 0.0);
+        for (int b = 0; b < B; b++)
+            for (int k = 0; k < 3; k++) {
+                if (init_v) rows[6 * (size_t)b + k] = init_v[3 * (size_t)b + k];
+                if (init_a) rows[6 * (size_t)b + 3 + k] = init_a[3 * (size_t)b + k];
+            }
+    }
+    const long long sN = held.ncx / 12, sM = held.ncy / 6;
+    const std::vector<ProbDesc> desc = scan_descs(c, B, N, M, nullptr, nullptr, nullptr);    // (the kernel reads N, M, S and the offsets)
+    HoldGuard urgent{c, UALM_MAX_LANES, c->cstream, false};
+    Staged s;
+    if (int rc = stage_held(c, held, desc, mpc_export_doubles(B, sN, sM), rows.empty() ? nullptr : rows.data(), 6, nullptr, urgent, s)) return rc;
+    BatchPtrs bp;
+    memset(&bp, 0, sizeof(bp));
+    bp.B = B; bp.desc = s.a.desc; bp.c_xy = const_cast<double *>(s.a.c_xy); bp.c_yaw = const_cast<double *>(s.a.c_yaw);
+    bp.piece_T = const_cast<double *>(s.a.piece_T);
+    return mpc_export_run(bp, sN, sM, dt, nullptr, nullptr, s.rows, s.a.out, pos_pts, posT_pts, angle_pts, angleT_pts, c_mpc_xy, c_mpc_yaw, dev4,
+                          c->cstream, urgent);
 }
 
 // ---------------------------------------------------------------------------------------------

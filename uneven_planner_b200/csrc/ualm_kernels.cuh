@@ -2764,6 +2764,7 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) replan_kernel(const _
 //       which the message does not carry): the largest position / yaw deviation over t = 0, dt, 2dt, .. and where it occurs.
 // One warp per problem: lane 0 solves the xy system (one factorization, two right-hand sides), lane 1 the yaw system, every lane
 // takes a slice of the samples of (3).  band: scratch, 13 * (6N + 6M) doubles per problem at 13 * (off_cxy / 2 + off_cyaw).
+// The same kernel serves a lane's solved batch (ualm_mpc_export_batch) and trajectories the caller holds (ualm_mpc_export_trajectories).
 // dev[4 * problem + ..] = {max |p_plan - p_mpc|, its time, max |yaw_plan - yaw_mpc|, its time}
 // ---------------------------------------------------------------------------------------------
 struct BandView {      // BandedSystem storage (banded_system.hpp:25-64): entry (i, j) at [(i - j + 6) * n + j]
@@ -2820,7 +2821,9 @@ __device__ void mpc_minco_serial(BandView A, int P, int Dim, R T, const R *pts, 
             if (A(i, j) != 0.0) for (int d = 0; d < Dim; d++) c[i + d * n] -= A(i, j) * c[j + d * n];
     }
 }
-struct MpcOut { R *pos_pts, *posT_pts, *angle_pts, *angleT_pts, *c_mpc_xy, *c_mpc_yaw, *dev, *band; R init_v[3], init_a[3]; };
+// the message's boundary derivatives: row `prob` of init_rows, 6 doubles {v_x, v_y, v_yaw, a_x, a_y, a_yaw} per problem (each robot
+// its own start state), or `init` for every problem when init_rows is null
+struct MpcOut { R *pos_pts, *posT_pts, *angle_pts, *angleT_pts, *c_mpc_xy, *c_mpc_yaw, *dev, *band; const R *init_rows; R init[6]; };
 __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) mpc_export_kernel(const __grid_constant__ BatchPtrs bp, R dt, const __grid_constant__ MpcOut o)
 {
     const int lane = threadIdx.x & 31, prob = blockIdx.x * UALM_WPB + (threadIdx.x >> 5);
@@ -2855,8 +2858,9 @@ __global__ void __launch_bounds__(UALM_THREADS * UALM_WPB) mpc_export_kernel(con
     __syncwarp();
     // (2) the MPC's own MINCO over the message
     R *band = o.band + 13 * (pd->off_cxy / 2 + pd->off_cyaw);
-    if (lane == 0) mpc_minco_serial(BandView{band, nx}, N, 2, Tx, pp, 2, 1, o.init_v, o.init_a, mxy);
-    if (lane == 1) mpc_minco_serial(BandView{band + 13 * nx, 6 * M}, M, 1, Ty, ap, 1, 0, o.init_v + 2, o.init_a + 2, myaw);
+    const R *init = o.init_rows ? o.init_rows + 6 * (size_t)prob : o.init;
+    if (lane == 0) mpc_minco_serial(BandView{band, nx}, N, 2, Tx, pp, 2, 1, init, init + 3, mxy);
+    if (lane == 1) mpc_minco_serial(BandView{band + 13 * nx, 6 * M}, M, 1, Ty, ap, 1, 0, init + 2, init + 5, myaw);
     __syncwarp();
     // (3) planned against tracked, over the shorter of the two durations like every scan of the reference (se2traj.hpp:415-418)
     if (!d.scannable(dt)) {
